@@ -94,8 +94,8 @@ typedef struct mgc_stats {
     double ms_relabel;          /* device ms inside global-relabel kernels (init + relaxation sweeps)    */
     double ms_boundary;         /* device ms of the last boundary (n-link) kernel alone                  */
     double ms_init;             /* device ms of the solver-state initialisation kernel (k_init_tile); 0 after a fused build */
-    int64_t tiles_materialised; /* lazy build: 8^3 tiles whose capacities k_caps_tiles computed (0 after an eager build) */
-    double ms_caps;             /* device ms of those k_caps_tiles launches (not part of ms_push)                        */
+    int64_t tiles_materialised; /* lazy build: 8^3 tiles whose capacities, tr and excess k_caps_tiles computed (0 eager) */
+    double ms_caps;             /* device ms of the materialiser launches (k_caps_claim + k_caps_tiles; not in ms_push)  */
 } mgc_stats;
 
 /* ---- lifetime ------------------------------------------------------------------------------------- */

@@ -158,14 +158,19 @@ struct mgc_graph {
     bool debug_checks = false;         // MEDPY_GC_DEBUG=1: device-side invariant + flow-conservation checks around every solve
     double debug_excess0 = 0.0;        // clamped source excess the solve started from
     bool fuse_build = true;            // mgc_build_voxel_graph uses the single-pass k_build_tile (MEDPY_GC_FUSE=0: four passes)
-    // lazy capacities: the fused 3-D build writes no capacity planes; k_caps_tiles computes them per tile, from a copy of
-    // the image, for the tiles the push path reaches (MEDPY_GC_LAZY_CAPS=0: the build writes them all)
+    // lazy push state: the fused 3-D build writes no capacity planes, no tr and no excess; k_caps_tiles computes them per
+    // tile, from copies of the build's inputs, for the tiles the push path reaches (MEDPY_GC_LAZY_CAPS=0: the build
+    // writes them all)
     bool lazy_caps = true;
     bool caps_lazy = false;            // the last build was lazy and some tiles are not materialised yet
-    int* cmat = nullptr;               // per tile: capacities materialised since the last lazy build
+    int* cmat = nullptr;               // per tile: push state materialised since the last lazy build
+    int* caps_list = nullptr;          // tiles claimed by the current materialiser launch
     Buf img_copy;                      // the image the lazy build saw, in its own dtype
+    Buf prob_copy;                     // ... its probability map, in its own dtype
+    Buf mark_planes[2];                // ... its fg / bg markers as bit planes (LazyTin)
     int caps_dtype = MGC_F32;
     BoundaryParams caps_P{};           // the boundary term of the lazy build
+    LazyTin caps_tin{};                // its t-link terms
     std::vector<cudaEvent_t> caps_ev;  // start / end of every materialiser launch since the last caps_resolve
     size_t caps_ev_used = 0;
     int build_chunks = 8;              // host inputs: z-chunks whose upload overlaps the build of the previous chunk
@@ -581,6 +586,7 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
         if (!rc) { rc = alloc_buf(g, tb, &p); g->pflag = (int*)p; }
         if (!rc) { rc = alloc_buf(g, tb, &p); g->rflag = (int*)p; }
         if (!rc) { rc = alloc_buf(g, tb, &p); g->cmat = (int*)p; }
+        if (!rc) { rc = alloc_buf(g, tb, &p); g->caps_list = (int*)p; }
         for (int i = 0; i < 2 && !rc; ++i) { rc = alloc_buf(g, tb, &p); g->rl_items[i] = (int*)p; }
         for (int i = 0; i < 4 && !rc; ++i) { rc = alloc_buf(g, tb, &p); g->pl_items[i >> 1][i & 1] = (int*)p; }
         if (!rc) { rc = alloc_buf(g, 256, &p); g->d_tcount = (int*)p; }
@@ -796,22 +802,23 @@ int materialise_zeros(mgc_graph* g)
     return MGC_OK;
 }
 
-// ---- lazy capacities: k_caps_tiles over a push worklist or over every tile -----------------------------------------
+// ---- lazy push state: k_caps_tiles over a push worklist or over every tile -----------------------------------------
 template <typename E>
-void caps_launch_t(mgc_graph* g, WorkList wl)
+void caps_launch_t(mgc_graph* g)
 {
     const BoundaryParams& P = g->caps_P;
     const E* img = (const E*)g->img_copy.p;
+    int* count = g->d_flags + 4;              // [4] tiles claimed by this launch, [5] cursor
     int* done = g->d_flags + 3;               // tiles materialised since the build
     const unsigned grid = (unsigned)g->n_ctas;
     if constexpr (!std::is_integral<E>::value) {
         if (P.fn == 1 && P.inv_spacing_on == 0.0) {
-            if (P.use_max) k_caps_tiles<E, 1, 1, 0><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->cmat, wl, done);
-            else           k_caps_tiles<E, 1, 0, 0><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->cmat, wl, done);
+            if (P.use_max) k_caps_tiles<E, 1, 1, 0><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->caps_tin, g->caps_list, count, count + 1, done);
+            else           k_caps_tiles<E, 1, 0, 0><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->caps_tin, g->caps_list, count, count + 1, done);
             return;
         }
     }
-    k_caps_tiles<E, -1, -1, -1><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->cmat, wl, done);
+    k_caps_tiles<E, -1, -1, -1><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->caps_tin, g->caps_list, count, count + 1, done);
 }
 
 // materialise the tiles of a push worklist and their face neighbours (wl.items == nullptr: every tile), between a pair of
@@ -821,22 +828,24 @@ int caps_launch(mgc_graph* g, WorkList wl)
     if (g->caps_ev_used + 2 > g->caps_ev.size()) g->caps_ev.resize(g->caps_ev_used + 2, nullptr);
     for (size_t i = g->caps_ev_used; i < g->caps_ev_used + 2; ++i) if (!g->caps_ev[i]) CK(cudaEventCreate(&g->caps_ev[i]));
     CK(cudaEventRecord(g->caps_ev[g->caps_ev_used], g->stream));
+    CK(cudaMemsetAsync(g->d_flags + 4, 0, 2 * sizeof(int), g->stream));
+    k_caps_claim<<<(unsigned)g->n_ctas * 4u, 256, 0, g->stream>>>(g->TL, g->cmat, wl, g->caps_list, g->d_flags + 4);
     switch (g->caps_dtype) {
-        case MGC_F32: caps_launch_t<float>(g, wl); break;
-        case MGC_F64: caps_launch_t<double>(g, wl); break;
-        case MGC_U8: caps_launch_t<uint8_t>(g, wl); break;
-        case MGC_I16: caps_launch_t<int16_t>(g, wl); break;
-        default: caps_launch_t<int32_t>(g, wl); break;
+        case MGC_F32: caps_launch_t<float>(g); break;
+        case MGC_F64: caps_launch_t<double>(g); break;
+        case MGC_U8: caps_launch_t<uint8_t>(g); break;
+        case MGC_I16: caps_launch_t<int16_t>(g); break;
+        default: caps_launch_t<int32_t>(g); break;
     }
     CK(cudaEventRecord(g->caps_ev[g->caps_ev_used + 1], g->stream));
     g->caps_ev_used += 2;
-    g->st.kernel_launches++;
+    g->st.kernel_launches += 2;
     CK(cudaGetLastError());
     return MGC_OK;
 }
 
-// every capacity is about to be read or written outside the push path: materialise the tiles that are not yet
-int caps_all(mgc_graph* g)
+// capacities, tr or excess are about to be read or written outside the push path: materialise the tiles that are not yet
+int push_state_all(mgc_graph* g)
 {
     if (!g->caps_lazy) return MGC_OK;
     g->caps_lazy = false;
@@ -862,7 +871,7 @@ int ensure_state(mgc_graph* g)
 {
     if (g->state_init) return MGC_OK;
     { int rc0 = materialise_zeros(g); if (rc0) return rc0; }
-    { int rc0 = caps_all(g); if (rc0) return rc0; }
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }
     if (g->nd == 3) k_init_state<3, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
     else            k_init_state<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
     g->st.kernel_launches++;
@@ -967,7 +976,7 @@ int dirty_clear(mgc_graph* g)
 int init_tiles(mgc_graph* g)
 {
     Nvtx range("mgc:init_state");
-    { int rc0 = caps_all(g); if (rc0) return rc0; }       // k_init_tile reads every capacity
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // k_init_tile reads every capacity
     CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
     g->pl_sel[0] = g->pl_sel[1] = 0;
     cudaEventRecord(g->ev[4], g->stream);
@@ -1144,7 +1153,7 @@ int push_color(mgc_graph* g, int color)
     if (g->caps_lazy) {
         // the pushers are the listed tiles, the receivers of cross-face flow their face neighbours: materialise those.  A
         // hard instance (sweeps at every relabel) pushes through most of the lattice: everything at once, then no more
-        const int rc = g->sweep_mode == 1 ? caps_all(g) : caps_launch(g, pl(g, color, a));
+        const int rc = g->sweep_mode == 1 ? push_state_all(g) : caps_launch(g, pl(g, color, a));
         if (rc) return rc;
     }
     CK(cudaMemsetAsync(cursor(g), 0, sizeof(int), g->stream));
@@ -1187,6 +1196,10 @@ int push_tiles(mgc_graph* g, int passes)
 // active voxels, counted exactly over the two pending push lists (a superset of the tiles that can hold one)
 int count_active_tiles_enqueue(mgc_graph* g, unsigned long long* dst)
 {
+    if (g->caps_lazy && !g->flow_started) {
+        // no push since the lazy build: the listed tiles hold no excess yet
+        for (int color = 0; color < 2; ++color) { const int rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
+    }
     CK(cudaMemsetAsync(dst, 0, sizeof(unsigned long long), g->stream));
     if (g->nd == 4) {
         for (int color = 0; color < 2; ++color)
@@ -1217,7 +1230,7 @@ int count_active_tiles(mgc_graph* g, int64_t* out)
 int solve_coop(mgc_graph* g, int flags, int passes, int64_t* active_out)
 {
     if (flags & (SOLVE_F_PUSH | SOLVE_F_LOOP)) g->flow_started = true;
-    { int rc0 = caps_all(g); if (rc0) return rc0; }       // the cooperative solve pushes wherever it likes
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the cooperative solve pushes wherever it likes
     int hdr[4] = {0, g->pl_sel[0], g->pl_sel[1], g->rl_cur};     // cursor, list selectors
     CK(cudaMemcpyAsync(g->d_tcount + CTL_CURSOR, hdr, sizeof(hdr), cudaMemcpyHostToDevice, g->stream));
     SolveLists SL;
@@ -1250,7 +1263,7 @@ int solve_coop(mgc_graph* g, int flags, int passes, int64_t* active_out)
 int debug_invariants(mgc_graph* g, bool after)
 {
     if (!g->debug_checks) return MGC_OK;
-    { int rc0 = caps_all(g); if (rc0) return rc0; }
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }
     double* d = g->d_scalars + 4;        // [4] excess, [5] absorbed, [6] violations
     CK(cudaMemsetAsync(d, 0, 3 * sizeof(double), g->stream));
     const bool tiles3 = g->use_tiles && g->nd == 3;
@@ -1373,7 +1386,12 @@ int solve_tiles(mgc_graph* g)
 int readout(mgc_graph* g, double* energy_part)
 {
     Nvtx range("mgc:readout");
-    if (g->use_tiles && g->nd == 3) k_readout<double, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
+    // clean tiles hold the reset labels while no sweep has lowered labels unmarked (the partial reset relies on the same)
+    const bool clean = g->use_tiles && g->nd == 3 && !g->slab && g->TL.dflag && g->sweep_mode != 1 && !g->use_coop &&
+                       g->L.dim[2] % 4 == 0;
+    if (clean) k_readout<double, true, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials, g->TL.dflag,
+                                                                                g->TL.nt[1], g->TL.nt[2]);
+    else if (g->use_tiles && g->nd == 3) k_readout<double, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
     else                            k_readout<double, false><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
     CK(cudaMemsetAsync(g->d_scalars + 1, 0, sizeof(double), g->stream));
     k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, rblocks(g), g->d_scalars + 1);
@@ -1697,6 +1715,8 @@ void mgc_destroy(mgc_graph* g)
     for (auto& b : g->scratch) if (b.p) pool_free(g->device, b.bytes, b.p);
     if (g->raw.p) pool_free(g->device, g->raw.bytes, g->raw.p);
     if (g->img_copy.p) pool_free(g->device, g->img_copy.bytes, g->img_copy.p);
+    if (g->prob_copy.p) pool_free(g->device, g->prob_copy.bytes, g->prob_copy.p);
+    for (auto& b : g->mark_planes) if (b.p) pool_free(g->device, b.bytes, b.p);
     for (auto& ev : g->ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->caps_ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->ev_slot) if (ev) cudaEventDestroy(ev);
@@ -1869,6 +1889,7 @@ int mgc_add_regional_probability(mgc_graph* g, const mgc_array* prob, double alp
     if (prob->dtype != MGC_F32 && prob->dtype != MGC_F64) FAIL(MGC_E_ARG, "probability map must be float32 or float64");
     if (compute_dtype != MGC_F32 && compute_dtype != MGC_F64) FAIL(MGC_E_ARG, "compute dtype must be float32 or float64");
     CK(cudaSetDevice(g->device));
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the term adds to tr
     TermSpan t(g);
     const void* p = nullptr;
     int rc = stage_input(g, prob, 0, &p);
@@ -1897,6 +1918,7 @@ int mgc_add_tweights_dense(mgc_graph* g, const mgc_array* src, const mgc_array* 
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     if (src->dtype != MGC_F64 || snk->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense t-weights must be float64");
     CK(cudaSetDevice(g->device));
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the term adds to tr
     TermSpan t(g);
     const void *ps = nullptr, *pk = nullptr;
     int rc = stage_input(g, src, 0, &ps);
@@ -1923,6 +1945,7 @@ int mgc_add_markers(mgc_graph* g, const mgc_array* fg, const mgc_array* bg)
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     if ((fg && fg->dtype != MGC_U8) || (bg && bg->dtype != MGC_U8)) FAIL(MGC_E_ARG, "markers must be uint8 / bool");
     CK(cudaSetDevice(g->device));
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the term adds to tr
     TermSpan t(g);
     const void *pf = nullptr, *pb = nullptr;
     int rc = MGC_OK;
@@ -1952,7 +1975,7 @@ int mgc_add_boundary(mgc_graph* g, int32_t kind, const mgc_array* image, double 
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
-    { int rc0 = caps_all(g); if (rc0) return rc0; }       // the term adds to every capacity
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the term adds to every capacity
     TermSpan t(g);
     const void* img = nullptr;
     int rc = stage_input(g, image, 2, &img);
@@ -2096,9 +2119,14 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     }
     if (const char* e = getenv("MEDPY_GC_BUILD_DBG")) A.dbg = atoi(e);
     const bool lazy = can_lazy(g);
+    const int mark_words = (g->L.dim[2] + 31) / 32;
     if (lazy) {
         rc = ensure_scratch(g, g->img_copy, n * es_img); if (rc) return rc;
         A.img_copy = g->img_copy.p;
+        if (t->prob) { rc = ensure_scratch(g, g->prob_copy, n * es_prob); if (rc) return rc; A.prob_copy = g->prob_copy.p; }
+        const size_t plane_bytes = (size_t)g->L.dim[0] * (size_t)g->L.dim[1] * (size_t)mark_words * 4;
+        if (t->fg || t->fg_bits) { rc = ensure_scratch(g, g->mark_planes[0], plane_bytes); if (rc) return rc; A.fg_plane = (unsigned*)g->mark_planes[0].p; }
+        if (t->bg || t->bg_bits) { rc = ensure_scratch(g, g->mark_planes[1], plane_bytes); if (rc) return rc; A.bg_plane = (unsigned*)g->mark_planes[1].p; }
         A.cmat = g->cmat;
         CK(cudaMemsetAsync(g->d_flags + 3, 0, sizeof(int), g->stream));      // tiles materialised
     }
@@ -2166,6 +2194,7 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     g->caps_lazy = lazy;
     g->caps_dtype = t->image->dtype;
     g->caps_P = P;
+    g->caps_tin = LazyTin{A.prob_copy, A.prob_f64, A.compute_f32, A.alpha, A.fg_plane, A.bg_plane, mark_words};
     g->has_nlinks = true;
     g->boundary_timed = true;
     g->state_init = true;
@@ -2198,7 +2227,7 @@ int mgc_add_nweights_dense(mgc_graph* g, int32_t axis, const mgc_array* fwd, con
     if (fwd->dtype != MGC_F64 || bwd->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense n-weights must be float64");
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
-    { int rc0 = caps_all(g); if (rc0) return rc0; }       // the term adds to the capacities of one axis
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the term adds to the capacities of one axis
     TermSpan t(g);
     const void *pf = nullptr, *pb = nullptr;
     int rc = stage_input(g, fwd, 0, &pf);
@@ -2328,7 +2357,7 @@ int mgc_get_edge(mgc_graph* g, int64_t i, int64_t j, double* cap)
     *cap = 0.0;
     if (g->caps_fresh) return MGC_OK;
     CK(cudaSetDevice(g->device));
-    { int rc0 = caps_all(g); if (rc0) return rc0; }
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }
     int c[4] = {0, 0, 0, 0};
     unsigned r = (unsigned)i;
     for (int d = 0; d < g->nd; ++d) { c[d] = (int)(r / g->L.stride[d]); r %= g->L.stride[d]; }
@@ -2352,6 +2381,8 @@ int mgc_get_trcap(mgc_graph* g, int64_t node, double* trcap)
     if (!g || !trcap) return MGC_E_ARG;
     if (node < 0 || node >= (int64_t)g->L.n) FAIL(MGC_E_ARG, "node id out of range");
     if (g->tr_fresh) { *trcap = 0.0; return MGC_OK; }
+    CK(cudaSetDevice(g->device));
+    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // tr before the flow, excess after it
     if (!g->state_init || !g->flow_started) {      // no flow yet: the net terminal capacity exactly as add_tweights left it
         CK(cudaMemcpyAsync(trcap, g->S.tr + node, sizeof(double), cudaMemcpyDeviceToHost, g->stream));
         CK(cudaStreamSynchronize(g->stream));

@@ -8,7 +8,8 @@
 // passes here (with capacity planes written by one kernel and read straight back by the next).  Now every input byte is read once and every state byte written once:
 //     read  image 4 + probability 4 + fg 1 + bg 1                         = 10 B/voxel (float32 inputs)
 //     write six float64 capacities 48 + tr 8 + excess 8 + label 4 + rmask 1 = 69 B/voxel
-// (the lazy variant, LAZY = 1 below, writes an image copy instead of the capacities: 25 B/voxel for float32 images)
+// (the lazy variant, LAZY = 1 below, writes copies of the image and the probability map and two marker bit planes
+// instead of the capacities, tr and excess: 13.25 B/voxel for float32 inputs)
 // (`sink[]`, the absorbed-flow accumulator, is no longer zero-filled: bit RM_SINKV of rmask says whether a voxel's
 // entry has been written, see gc_tiles.cuh.)
 //
@@ -64,7 +65,22 @@ struct BuildArgs {
     int z_tile0;               // first z tile layer of this launch (chunked builds)
     int dbg;                   // diagnostics (MEDPY_GC_BUILD_DBG): 1 = do not load the probability map (constant 0.3)
     void* img_copy;            // lazy build: graph-owned copy of the image (input arrays are only borrowed for the call)
-    int* cmat;                 // lazy build: per tile "capacities materialised" flag, cleared here
+    void* prob_copy;           // lazy build: graph-owned copy of the probability map, in its own dtype
+    unsigned* fg_plane;        // lazy build: marker bit planes (nullptr: no such marker), see MarkerPlanes
+    unsigned* bg_plane;
+    int* cmat;                 // lazy build: per tile "push state materialised" flag, cleared here
+};
+
+// What k_caps_tiles needs to replay the t-links of a lazy build.  The marker planes are row-padded: bit x & 31 of word
+// (z * Y + y) * words + x / 32, so that one warp row of the build (x0 .. x0 + 31 of row (z, y)) is one aligned word.
+struct LazyTin {
+    const void* prob;          // probability map copy or nullptr
+    int prob_f64;
+    int compute_f32;
+    double alpha;
+    const unsigned* fg;        // marker planes or nullptr
+    const unsigned* bg;
+    int words;                 // words per row: ceil(X / 32)
 };
 
 template <typename E>
@@ -108,17 +124,63 @@ __device__ __forceinline__ void exp_caps6(const double t[6], bool ordinary, unsi
     for (int k = 0; k < 6; ++k) if (!((valid >> k) & 1u)) c[k] = 0.0;
 }
 
+// The t-links of the build, replayed in the reference's order (regional term with float32 or float64 products,
+// foreground markers, background markers) onto tr; returns the sum of the add_tweights minima.  The build and the
+// materialiser both form tr here, so the lazy tr is the eager one bit for bit.
+template <typename T>
+__device__ __forceinline__ double tlink_replay(T& tr, bool has_prob, double p, bool f32, double alpha, unsigned fb)
+{
+    double mm = 0.0;
+    if (has_prob) {
+        double s, t;
+        if (f32) {
+            const float pf = (float)p;          // exact: the map is float32 when its products are
+            const float af = (float)alpha;
+            s = (double)__fmul_rn(pf, af);
+            t = (double)__fmul_rn(__fsub_rn(1.0f, pf), af);
+        } else {
+            s = __dmul_rn(p, alpha);
+            t = __dmul_rn(__dsub_rn(1.0, p), alpha);
+        }
+        mm = add_tweights_dev(tr, s, t);
+    }
+    if (fb & 1u) mm = __dadd_rn(mm, add_tweights_dev(tr, 65535.0, 0.0));
+    if (fb & 2u) mm = __dadd_rn(mm, add_tweights_dev(tr, 0.0, 65535.0));
+    return mm;
+}
+
+// residual-mask bits 0..5 of a voxel: its arcs with capacity
+__device__ __forceinline__ unsigned cap_bits(const double c[6])
+{
+    return (c[0] > 0 ? 1u : 0u) | (c[1] > 0 ? 2u : 0u) | (c[2] > 0 ? 4u : 0u) | (c[3] > 0 ? 8u : 0u) |
+           (c[4] > 0 ? 16u : 0u) | (c[5] > 0 ? 32u : 0u);
+}
+
+// source excess of a voxel with net terminal capacity tr > 0: clamped to the sum of its out-capacities rounded up,
+// with SOURCE_CLAMP_SLACK head-room (DESIGN.md §4.2); 0 when tr <= 0
+__device__ __forceinline__ double source_excess(double tr, const double c[6])
+{
+    double out = __dadd_ru(0.0, c[0]);
+    out = __dadd_ru(out, c[1]); out = __dadd_ru(out, c[2]); out = __dadd_ru(out, c[3]);
+    out = __dadd_ru(out, c[4]); out = __dadd_ru(out, c[5]);
+    double e = 0.0;
+    if (tr > 0) { const double lim = out * SOURCE_CLAMP_SLACK; e = tr < lim ? tr : lim; if (!(out == out)) e = tr; }
+    return e;
+}
+
 // TIN = 1: the common configuration fixed at compile time -- float32 probability map with float32 products and both
 // marker volumes as bytes, all three staged by TMA.  The generic form (TIN = 0) decides each of those per voxel with
 // warp-uniform branches, whose bookkeeping costs instructions in this issue-heavy loop.
 //
-// LAZY = 1: the capacity planes are not written (k_caps_tiles computes them for the tiles the push path reaches); the
-// kernel writes a copy of the image instead and clears cmat[] of its tiles.  Everything else -- tr, excess, rmask, height,
-// partials, worklists -- is bit for bit what LAZY = 0 writes.  Under the exponential term without spacing every in-lattice
-// weight is >= DBL_MIN, so for a warp whose arguments are ordinary the n-link bits of rmask are the validity bits and the
-// weights are needed only to clamp the source excess of voxels with tr > 0: a warp without such a voxel evaluates no
-// exponential.  A warp that needs them evaluates all six per voxel (no z carry, no shared planes: a neighbouring warp may
-// have skipped).  Other terms still evaluate every weight (weight check, rmask) but store none.
+// LAZY = 1: neither the capacity planes nor tr nor excess are written (k_caps_tiles computes all three for the tiles the
+// push path reaches); the kernel writes what recomputes them bit for bit instead -- copies of the image and of the
+// probability map, the markers as two bit planes (one ballot per warp row) -- and clears cmat[] of its tiles.  rmask,
+// height, partials and worklists are bit for bit what LAZY = 0 writes.  Under the exponential term without spacing every
+// in-lattice weight is >= DBL_MIN, so for a warp whose arguments are ordinary the n-link bits of rmask are the validity
+// bits, and the clamped excess is > 0 exactly when tr > 0 and the voxel has an in-lattice arc: such a warp evaluates no
+// exponential.  A warp whose arguments are not ordinary evaluates all six per voxel (rmask depends on them; no z carry,
+// no shared planes: a neighbouring warp may have skipped).  Other terms still evaluate every weight (weight check,
+// rmask) but store none.
 template <typename E, typename T, int FN, int USE_MAX, int SPACING, int TIN = 0, int LAZY = 0>
 __global__ void __launch_bounds__(BUILD_THREADS)
 k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps maps, BuildArgs A, BoundaryParams P,
@@ -266,36 +328,15 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         const double a = build_val<E>(at(hz, ly + 1, lx + 1), use_max);
         // ---- t-links: add_tweights replay in the reference's order (regional, fg, bg) ----
         auto tlinks = [&](T& tr) -> double {
-            double mm = 0.0;
-            if (TIN == 1) {
-                const float p = (float)cur.p;
-                const float af = (float)A.alpha;
-                mm = add_tweights_dev(tr, (double)__fmul_rn(p, af), (double)__fmul_rn(__fsub_rn(1.0f, p), af));
-            } else if (A.prob) {
-                double s, t;
-                if (A.compute_f32) {
-                    const float p = (float)cur.p;          // exact: the map is float32 when its products are
-                    const float af = (float)A.alpha;
-                    s = (double)__fmul_rn(p, af);
-                    t = (double)__fmul_rn(__fsub_rn(1.0f, p), af);
-                } else {
-                    s = __dmul_rn(cur.p, A.alpha);
-                    t = __dmul_rn(__dsub_rn(1.0, cur.p), A.alpha);
-                }
-                mm = add_tweights_dev(tr, s, t);
-            }
-            const bool f = (cur.fb & 1u) != 0, b = (cur.fb & 2u) != 0;
-            if (f) mm = __dadd_rn(mm, add_tweights_dev(tr, 65535.0, 0.0));
-            if (b) mm = __dadd_rn(mm, add_tweights_dev(tr, 0.0, 65535.0));
-            return mm;
+            return tlink_replay<T>(tr, TIN == 1 || A.prob != nullptr, cur.p, TIN == 1 || A.compute_f32 != 0, A.alpha, cur.fb);
         };
         T tr = (T)0;
         double mm = 0.0;
         double c0 = 0.0, c1 = 0.0, c2 = 0.0, c3 = 0.0, c4 = 0.0, c5 = 0.0;
         double wz = 0.0, wy = 0.0, wx = 0.0;
         if constexpr (LAZY_EXP) {
-            // t-links first: the six weights are needed only when a lane has tr > 0 (source clamp) or the warp's
-            // arguments are not all ordinary (rmask would then depend on the values)
+            // the six weights are needed only when the warp's arguments are not all ordinary (rmask would then depend
+            // on the values)
             if (pin) mm = tlinks(tr);
             auto arg = [&](E iq) -> double {
                 const double b = build_val<E>(iq, use_max);
@@ -308,11 +349,11 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
             const bool ordinary = __all_sync(0xffffffffu, t[0] <= 700.0 && t[1] <= 700.0 && t[2] <= 700.0 &&
                                                           t[3] <= 700.0 && t[4] <= 700.0 && t[5] <= 700.0);
             double c[6];
-            if (!ordinary || __any_sync(0xffffffffu, (double)tr > 0)) {
+            if (!ordinary) {
                 exp_caps6(t, ordinary, valid, c);
             } else {
 #pragma unroll
-                for (int k = 0; k < 6; ++k) c[k] = ((valid >> k) & 1u) ? 1.0 : 0.0;    // stand-ins: only their signs are read
+                for (int k = 0; k < 6; ++k) c[k] = ((valid >> k) & 1u) ? 1.0 : 0.0;    // stand-ins: only signs are read
             }
             c0 = c[0]; c1 = c[1]; c2 = c[2]; c3 = c[3]; c4 = c[4]; c5 = c[5];
         } else {
@@ -358,27 +399,36 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
                 }
                 mm = tlinks(tr);
             }
-            if (LAZY) reinterpret_cast<E*>(A.img_copy)[v] = at(hz, ly + 1, lx + 1);
+            if (LAZY) {
+                reinterpret_cast<E*>(A.img_copy)[v] = at(hz, ly + 1, lx + 1);
+                if (TIN == 1 || (A.prob && !A.prob_f64)) reinterpret_cast<float*>(A.prob_copy)[v] = (float)cur.p;
+                else if (A.prob) reinterpret_cast<double*>(A.prob_copy)[v] = cur.p;
+            }
             const bool own = gz >= L.own0 && gz < L.own1;
             if (own) msum = __dadd_rn(msum, mm);
-            S.tr[v] = tr;
-            // ---- solver state (same arithmetic as k_init_tile) ----
-            unsigned m = (c0 > 0 ? 1u : 0u) | (c1 > 0 ? 2u : 0u) | (c2 > 0 ? 4u : 0u) | (c3 > 0 ? 8u : 0u) |
-                         (c4 > 0 ? 16u : 0u) | (c5 > 0 ? 32u : 0u);
-            double out = __dadd_ru(0.0, c0);
-            out = __dadd_ru(out, c1); out = __dadd_ru(out, c2); out = __dadd_ru(out, c3);
-            out = __dadd_ru(out, c4); out = __dadd_ru(out, c5);
+            if (!LAZY) S.tr[v] = tr;
+            // ---- solver state (same arithmetic as k_init_tile and k_caps_tiles) ----
+            const double c[6] = {c0, c1, c2, c3, c4, c5};
+            unsigned m = cap_bits(c);
             const double trd = (double)tr;
-            double e = 0.0;
-            if (trd > 0) { const double lim = out * SOURCE_CLAMP_SLACK; e = trd < lim ? trd : lim; if (!(out == out)) e = trd; }
+            // LAZY_EXP with ordinary arguments: from the stand-ins, whose sum has the sign of the true one -- only e > 0 is read
+            double e = source_excess(trd, c);
             if (trd < 0) m |= RM_SINK;
             if (!own) e = 0.0;
-            S.excess[v] = (T)e;
+            if (!LAZY) S.excess[v] = (T)e;
             S.rmask[v] = (uint8_t)m;
             const int h = (own && trd < 0) ? 1 : MGC_HINF;
             S.height[v] = h;
             if (own && (m & 0x3fu) != 0 && h == MGC_HINF) needs_any = 1u;
             if (e > 0) exc_any = 1u;
+        }
+        if (LAZY) {      // marker bit planes: one word per warp row and marker
+            const unsigned bf = __ballot_sync(0xffffffffu, pin && (cur.fb & 1u)), bb = __ballot_sync(0xffffffffu, pin && (cur.fb & 2u));
+            if (lx == 0 && gz < L.dim[0] && gy < L.dim[1]) {
+                const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * gridDim.x + blockIdx.x;
+                if (A.fg_plane) A.fg_plane[w] = bf;
+                if (A.bg_plane) A.bg_plane[w] = bb;
+            }
         }
         wz_back = wz;
         cur = nxt;
@@ -431,100 +481,152 @@ constexpr size_t build_smem_bytes()
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Capacity materialiser of the lazy build: the six capacity planes of the tiles the push path is about to touch, from
-// the graph-owned image copy.  Runs over a push worklist -- every listed tile and its six face neighbours, since a push
-// writes across faces -- or, with wl.items == nullptr, over every tile.  A tile is claimed once per build (cmat[t]: 0 -> 1);
-// the claiming CTA stages the tile's image with its six face halos and writes, voxel by voxel, the doubles the eager
-// build writes (build_weight / exp_caps6 on the same operands).  Candidates are claimed CAPS_CHUNK at a time by as many
-// threads, so a launch over tiles that are all materialised already costs one read of the list.
+// Push-state materialiser of the lazy build: the six capacity planes, tr and excess of the tiles the push path is about
+// to touch, from the graph-owned copies the build wrote.  Runs over a push worklist -- every listed tile and its six face
+// neighbours, since a push writes across faces -- or, with wl.items == nullptr, over every tile.  A tile is materialised
+// once per build.  Two launches:
+//   k_caps_claim : claims each candidate tile (cmat[t]: 0 -> 1) and appends the claimed ones to a compact list;
+//   k_caps_tiles : persistent CTAs take the listed tiles one by one through an atomic cursor (even load, whatever the
+//                  list order), staging the image of the next tile in registers while the current one is computed.
+// The values are the doubles the eager build writes: build_weight / exp_caps6 on the same operands, tlink_replay on the
+// same inputs, source_excess on the capacities just computed.
 // ---------------------------------------------------------------------------------------------------
-#define CAPS_CHUNK 64
-template <typename E, int FN, int USE_MAX, int SPACING>
-__global__ void __launch_bounds__(TILE_VOX, 2)
-k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, BoundaryParams P, int* __restrict__ cmat,
-             WorkList wl, int* __restrict__ n_done)
+__global__ void __launch_bounds__(256) k_caps_claim(Tiles TL, int* __restrict__ cmat, WorkList wl, int* __restrict__ list,
+                                                    int* __restrict__ count)
 {
-    __shared__ E s_img[HALO_VOX];
-    __shared__ int s_claim[CAPS_CHUNK];
-    __shared__ int s_n;
-    const int tid = threadIdx.x;
     const bool all = wl.items == nullptr;
     const int n = all ? TL.ntiles : *wl.count * 7;
-    const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
-    const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
-    int claimed = 0;
-    for (int base = blockIdx.x * CAPS_CHUNK; base < n; base += gridDim.x * CAPS_CHUNK) {
-        if (tid == 0) s_n = 0;
-        __syncthreads();
-        if (tid < CAPS_CHUNK && base + tid < n) {
-            const int i = base + tid;
-            int t = all ? i : wl.items[i / 7];
+    const int lane = threadIdx.x & 31;
+    for (int base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31; base < n; base += gridDim.x * blockDim.x) {
+        const int i = base + lane;
+        int t = -1;
+        if (i < n) {
+            t = all ? i : wl.items[i / 7];
             const int k = all ? -1 : i % 7 - 1;          // -1: the listed tile, 0..5: its neighbour across face k
             if (k >= 0) {
                 const int tx = t % TL.nt[2], r = t / TL.nt[2], ty = r % TL.nt[1], tz = r / TL.nt[1];
                 const int ck = (k >> 1) == 0 ? tz : ((k >> 1) == 1 ? ty : tx);
                 t = ((k & 1) ? ck + 1 < TL.nt[k >> 1] : ck > 0) ? tile_nbr(TL, t, k) : -1;
             }
-            if (t >= 0 && cmat[t] == 0 && atomicExch(&cmat[t], 1) == 0) s_claim[atomicAdd(&s_n, 1)] = t;
         }
-        __syncthreads();
-        const int m = s_n;
-        claimed += m;
-        for (int j = 0; j < m; ++j) {
-            const TileCtx c = tile_ctx(L, TL, s_claim[j]);
-            const int h = hidx(c.lz + 1, c.ly + 1, c.lx + 1);
-            s_img[h] = c.inb ? img[c.v] : (E)0;
-            if (tid < 384) {      // the six face halos (edges and corners are never read); out-of-lattice cells are never used
-                const int face = tid >> 6, fa = (tid >> 3) & 7, fb = tid & 7;
-                int z, y, x;
-                switch (face) {
-                    case 0: z = -1; y = fa; x = fb; break;
-                    case 1: z = TILE; y = fa; x = fb; break;
-                    case 2: z = fa; y = -1; x = fb; break;
-                    case 3: z = fa; y = TILE; x = fb; break;
-                    case 4: z = fa; y = fb; x = -1; break;
-                    default: z = fa; y = fb; x = TILE; break;
-                }
-                const int gz = c.tz * TILE + z, gy = c.ty * TILE + y, gx = c.tx * TILE + x;
-                E val = (E)0;
-                if (gz >= 0 && gy >= 0 && gx >= 0 && gz < L.dim[0] && gy < L.dim[1] && gx < L.dim[2])
-                    val = img[(unsigned)gz * L.stride[0] + (unsigned)gy * L.stride[1] + (unsigned)gx];
-                s_img[hidx(z + 1, y + 1, x + 1)] = val;
-            }
-            __syncthreads();
-            const int gz = c.tz * TILE + c.lz, gy = c.ty * TILE + c.ly, gx = c.tx * TILE + c.lx;
-            const unsigned valid = c.inb ? ((gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) |
-                                            (gy + 1 < L.dim[1] ? 8u : 0u) | (gx > 0 ? 16u : 0u) | (gx + 1 < L.dim[2] ? 32u : 0u)) : 0u;
-            const double a = build_val<E>(s_img[h], use_max);
-            const E q[6] = {s_img[h - HALO_DIM * HALO_DIM], s_img[h + HALO_DIM * HALO_DIM], s_img[h - HALO_DIM],
-                            s_img[h + HALO_DIM], s_img[h - 1], s_img[h + 1]};
-            double cap[6];
-            if (FN == 1 && SPACING == 0) {
-                double t[6];
-#pragma unroll
-                for (int k = 0; k < 6; ++k) {
-                    const double b = build_val<E>(q[k], use_max);
-                    // cells outside the lattice were never staged: their (unused) arguments are pinned to 0 so that they
-                    // cannot push the warp off the ordinary path
-                    t[k] = ((valid >> k) & 1u) ? exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b))) : 0.0;
-                }
-                const bool ordinary = __all_sync(0xffffffffu, t[0] <= 700.0 && t[1] <= 700.0 && t[2] <= 700.0 &&
-                                                              t[3] <= 700.0 && t[4] <= 700.0 && t[5] <= 700.0);
-                exp_caps6(t, ordinary, valid, cap);
-            } else {
-#pragma unroll
-                for (int k = 0; k < 6; ++k)
-                    cap[k] = ((valid >> k) & 1u) ? build_weight<FN, E>(P, a, q[k], use_max, spacing, P.spacing[k >> 1]) : 0.0;
-            }
-            if (c.inb) {
-#pragma unroll
-                for (int k = 0; k < 6; ++k) S.cap[k][c.v] = cap[k];
-            }
-            __syncthreads();      // s_img is restaged for the next claimed tile
-        }
-        __syncthreads();          // every thread has read s_n before the next chunk resets it
+        const bool claim = t >= 0 && cmat[t] == 0 && atomicExch(&cmat[t], 1) == 0;
+        const unsigned b = __ballot_sync(0xffffffffu, claim);
+        int slot = 0;
+        if (lane == 0 && b) slot = atomicAdd(count, __popc(b));
+        slot = __shfl_sync(0xffffffffu, slot, 0);
+        if (claim) list[slot + __popc(b & ((1u << lane) - 1u))] = t;
     }
-    if (tid == 0 && claimed) atomicAdd(n_done, claimed);
+}
+
+template <typename E, int FN, int USE_MAX, int SPACING>
+__global__ void __launch_bounds__(TILE_VOX, 2)
+k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, BoundaryParams P, LazyTin tin,
+             const int* __restrict__ list, const int* __restrict__ count, int* __restrict__ cursor, int* __restrict__ n_done)
+{
+    __shared__ E s_img[HALO_VOX];
+    __shared__ int s_slot[2];
+    const int tid = threadIdx.x;
+    const int n = *count;
+    if (blockIdx.x == 0 && tid == 0 && n) atomicAdd(n_done, n);
+    const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
+    const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
+    // this thread's image cells of tile t: its voxel and (tid < 384) one cell of the six face halos (edges and corners
+    // are never read; out-of-lattice cells are never used)
+    struct Cells { E own, halo; };
+    auto load = [&](int t) -> Cells {
+        Cells r{(E)0, (E)0};
+        const TileCtx c = tile_ctx(L, TL, t);
+        if (c.inb) r.own = img[c.v];
+        if (tid < 384) {
+            const int face = tid >> 6, fa = (tid >> 3) & 7, fb = tid & 7;
+            int z, y, x;
+            switch (face) {
+                case 0: z = -1; y = fa; x = fb; break;
+                case 1: z = TILE; y = fa; x = fb; break;
+                case 2: z = fa; y = -1; x = fb; break;
+                case 3: z = fa; y = TILE; x = fb; break;
+                case 4: z = fa; y = fb; x = -1; break;
+                default: z = fa; y = fb; x = TILE; break;
+            }
+            const int gz = c.tz * TILE + z, gy = c.ty * TILE + y, gx = c.tx * TILE + x;
+            if (gz >= 0 && gy >= 0 && gx >= 0 && gz < L.dim[0] && gy < L.dim[1] && gx < L.dim[2])
+                r.halo = img[(unsigned)gz * L.stride[0] + (unsigned)gy * L.stride[1] + (unsigned)gx];
+        }
+        return r;
+    };
+    auto halo_at = [&]() -> int {
+        const int face = tid >> 6, fa = (tid >> 3) & 7, fb = tid & 7;
+        switch (face) {
+            case 0: return hidx(0, fa + 1, fb + 1);
+            case 1: return hidx(TILE + 1, fa + 1, fb + 1);
+            case 2: return hidx(fa + 1, 0, fb + 1);
+            case 3: return hidx(fa + 1, TILE + 1, fb + 1);
+            case 4: return hidx(fa + 1, fb + 1, 0);
+            default: return hidx(fa + 1, fb + 1, TILE + 1);
+        }
+    };
+    if (tid == 0) s_slot[0] = atomicAdd(cursor, 1);
+    __syncthreads();
+    int i = s_slot[0];
+    Cells cur{(E)0, (E)0};
+    if (i < n) cur = load(list[i]);
+    for (int it = 1; i < n; ++it) {
+        const int t = list[i];
+        const TileCtx c = tile_ctx(L, TL, t);
+        const int h = hidx(c.lz + 1, c.ly + 1, c.lx + 1);
+        s_img[h] = cur.own;
+        if (tid < 384) s_img[halo_at()] = cur.halo;
+        if (tid == 0) s_slot[it & 1] = atomicAdd(cursor, 1);
+        __syncthreads();
+        // t-link inputs of this voxel, and the next tile's image: in flight while this tile is computed
+        const int gz = c.tz * TILE + c.lz, gy = c.ty * TILE + c.ly, gx = c.tx * TILE + c.lx;
+        double p = 0.0;
+        unsigned fb = 0u;
+        if (c.inb) {
+            if (tin.prob) p = tin.prob_f64 ? reinterpret_cast<const double*>(tin.prob)[c.v] : (double)reinterpret_cast<const float*>(tin.prob)[c.v];
+            const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * (unsigned)tin.words + ((unsigned)gx >> 5);
+            if (tin.fg) fb |= (tin.fg[w] >> (gx & 31)) & 1u;
+            if (tin.bg) fb |= ((tin.bg[w] >> (gx & 31)) & 1u) << 1;
+        }
+        const int inext = s_slot[it & 1];
+        Cells nxt{(E)0, (E)0};
+        if (inext < n) nxt = load(list[inext]);
+        const unsigned valid = c.inb ? ((gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) |
+                                        (gy + 1 < L.dim[1] ? 8u : 0u) | (gx > 0 ? 16u : 0u) | (gx + 1 < L.dim[2] ? 32u : 0u)) : 0u;
+        const double a = build_val<E>(s_img[h], use_max);
+        const E q[6] = {s_img[h - HALO_DIM * HALO_DIM], s_img[h + HALO_DIM * HALO_DIM], s_img[h - HALO_DIM],
+                        s_img[h + HALO_DIM], s_img[h - 1], s_img[h + 1]};
+        double cap[6];
+        if (FN == 1 && SPACING == 0) {
+            double t6[6];
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+                const double b = build_val<E>(q[k], use_max);
+                // cells outside the lattice were never staged: their (unused) arguments are pinned to 0 so that they
+                // cannot push the warp off the ordinary path
+                t6[k] = ((valid >> k) & 1u) ? exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b))) : 0.0;
+            }
+            const bool ordinary = __all_sync(0xffffffffu, t6[0] <= 700.0 && t6[1] <= 700.0 && t6[2] <= 700.0 &&
+                                                          t6[3] <= 700.0 && t6[4] <= 700.0 && t6[5] <= 700.0);
+            exp_caps6(t6, ordinary, valid, cap);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 6; ++k)
+                cap[k] = ((valid >> k) & 1u) ? build_weight<FN, E>(P, a, q[k], use_max, spacing, P.spacing[k >> 1]) : 0.0;
+        }
+        if (c.inb) {
+            double tr = 0.0;
+            tlink_replay<double>(tr, tin.prob != nullptr, p, tin.compute_f32 != 0, tin.alpha, fb);
+            const double e = c.own ? source_excess(tr, cap) : 0.0;
+#pragma unroll
+            for (int k = 0; k < 6; ++k) S.cap[k][c.v] = cap[k];
+            S.tr[c.v] = tr;
+            S.excess[c.v] = e;
+        }
+        __syncthreads();          // s_img is restaged for the next tile
+        cur = nxt;
+        i = inext;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -157,8 +157,12 @@ __global__ void __launch_bounds__(256) k_count_active(Lattice L, State<T> S, uns
 // energy reduction: flow absorbed by the sink links of the owned voxels (fixed-order fp64 sums, deterministic)
 // LAZY: sink[v] holds a value only where rmask bit 7 (RM_SINKV, gc_tiles.cuh) is set -- the 3-D tile solver never
 // zero-fills the array, and only the voxels that absorbed flow are read here (4 + 1 B/voxel instead of 4 + 8).
-template <typename T, bool LAZY>
-__global__ void __launch_bounds__(256) k_readout(Lattice L, State<T> S, uint8_t* __restrict__ mask, double* __restrict__ partials)
+// CLEAN (3-D tile solver, X % 4 == 0, dirty-tile tracking over the whole solve): a tile that is not flagged in
+// `dflag` still holds the reset labels (1 where the sink link is residual and the voxel owned, HINF elsewhere), so its
+// mask comes from rmask alone and its labels are not read (1 B read per voxel there instead of 5).
+template <typename T, bool LAZY, bool CLEAN = false>
+__global__ void __launch_bounds__(256) k_readout(Lattice L, State<T> S, uint8_t* __restrict__ mask, double* __restrict__ partials,
+                                                 const int* __restrict__ dflag = nullptr, int nty = 0, int ntx = 0)
 {
     __shared__ double sh[8];
     double a = 0.0;
@@ -166,14 +170,28 @@ __global__ void __launch_bounds__(256) k_readout(Lattice L, State<T> S, uint8_t*
     // four voxels per thread and iteration (16 B label load, 32 B of sink flow, 4 B mask store); tail handled scalar
     const unsigned n4 = L.n >> 2;
     for (unsigned q = blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += step) {
-        const int4 h = reinterpret_cast<const int4*>(S.height)[q];
-        uchar4 m;
-        m.x = h.x >= MGC_HINF ? 1 : 0; m.y = h.y >= MGC_HINF ? 1 : 0;
-        m.z = h.z >= MGC_HINF ? 1 : 0; m.w = h.w >= MGC_HINF ? 1 : 0;
-        reinterpret_cast<uchar4*>(mask)[q] = m;
         const unsigned v = q << 2;
+        uchar4 m;
+        unsigned rm = 0;
+        bool clean = false;
+        if (CLEAN) {      // the four voxels lie in one row of one tile
+            rm = reinterpret_cast<const unsigned*>(S.rmask)[q];
+            const unsigned gz = div_stride(L, v, 0), r = v - gz * L.stride[0];
+            const unsigned gy = div_stride(L, r, 1), gx = r - gy * L.stride[1];
+            clean = dflag[((int)(gz >> 3) * nty + (int)(gy >> 3)) * ntx + (int)(gx >> 3)] == 0;
+        }
+        if (clean) {
+            const bool own = owned(L, v);          // bit 6 of rmask: RM_SINK (gc_tiles.cuh)
+            m.x = (own && (rm & 0x40u)) ? 0 : 1; m.y = (own && ((rm >> 8) & 0x40u)) ? 0 : 1;
+            m.z = (own && ((rm >> 16) & 0x40u)) ? 0 : 1; m.w = (own && ((rm >> 24) & 0x40u)) ? 0 : 1;
+        } else {
+            const int4 h = reinterpret_cast<const int4*>(S.height)[q];
+            m.x = h.x >= MGC_HINF ? 1 : 0; m.y = h.y >= MGC_HINF ? 1 : 0;
+            m.z = h.z >= MGC_HINF ? 1 : 0; m.w = h.w >= MGC_HINF ? 1 : 0;
+        }
+        reinterpret_cast<uchar4*>(mask)[q] = m;
         if (LAZY) {
-            const unsigned r4 = reinterpret_cast<const unsigned*>(S.rmask)[q] & 0x80808080u;
+            const unsigned r4 = (CLEAN ? rm : reinterpret_cast<const unsigned*>(S.rmask)[q]) & 0x80808080u;
             if (r4) {
 #pragma unroll
                 for (int i = 0; i < 4; ++i)

@@ -21,7 +21,9 @@ import numpy
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 NSLAB = 8
-BYTES_PER_VOXEL = 88   # solver state 78 (DESIGN.md §3) + image copy of the lazy build 4 + resident image 4 + fg 1 + bg 1
+# solver state 78 (DESIGN.md §3) + lazy build's image copy 4 and marker bit planes 0.25 + resident image 4 + fg 1 + bg 1.
+# Config 5 has no probability map; a run with a regional term would add the lazy build's 4 B copy of it.
+BYTES_PER_VOXEL = 88.25
 
 
 def main():
