@@ -96,6 +96,9 @@ typedef struct mgc_stats {
     double ms_init;             /* device ms of the solver-state initialisation kernel (k_init_tile); 0 after a fused build */
     int64_t tiles_materialised; /* lazy build: 8^3 tiles whose capacities, tr and excess k_caps_tiles computed (0 eager) */
     double ms_caps;             /* device ms of the materialiser launches (k_caps_claim + k_caps_tiles; not in ms_push)  */
+    int64_t seed_folds;         /* mgc_add_seeds calls folded into this handle since its build (reset by the build)   */
+    double ms_seeds;            /* device ms of those calls: tile claim + materialisation, fold, push-list fix-up     */
+    double ms_seeds_host;       /* host ms of those calls before anything is enqueued: id copy, range check, grouping */
 } mgc_stats;
 
 /* ---- lifetime ------------------------------------------------------------------------------------- */
@@ -208,6 +211,21 @@ int mgc_can_fuse(const mgc_graph* g);
  * preflow and returns the min-cut energy INCLUDING the add_tweights constants, like the reference's `flow`.
  * Idempotent after convergence. */
 int mgc_maxflow(mgc_graph* g, double* energy);
+/* Seeds added to a graph and solved warm (the interactive refinement loop of the reference: maxflow(), then
+ * add_tweights(v, 65535, 0) on new foreground seeds and add_tweights(v, 0, 65535) on new background seeds, then
+ * maxflow() again, which continues from BK's residual graph; graph.py:310-380, graph.h:415-425).  The meaning is exactly
+ * add_tweights(v, 65535, 0) for every id of fg_ids in list order, THEN add_tweights(v, 0, 65535) for every id of bg_ids;
+ * duplicate ids count once per occurrence, an id in both lists cancels like fg and bg markers do.  The seeds are folded
+ * into the handle's current state (solved or not; before the first solve the build's pending source excess is
+ * materialised first) and the next mgc_maxflow / mgc_get_mask / mgc_what_segment returns
+ * the result for the enlarged graph, starting from the flow already routed instead of from zero.
+ *   fg_ids / bg_ids : C-order node ids, int64, in host or device memory (`mem`); either may be NULL when its count is 0.
+ * MGC_E_ARG for an id out of range.  MGC_E_STATE unless the handle's last build was the lazy fused build
+ * (mgc_build_voxel_graph on a 1-D..3-D lattice with a boundary term, tile solver, not a z-slab, lazy capacities on): the
+ * fold recomputes capacities from the copies that build keeps.  Elsewhere reset() and a rebuild with the seeds is the way.
+ * mgc_add_tweights_dense / mgc_add_markers and the other term entry points still refuse a solved graph.  Adding this
+ * entry point left MGC_ABI_VERSION at 3: nothing that existed changed. */
+int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
 /* Bulk form of the what_segment loop (bin/medpy_graphcut_voxel.py:177-181): out[v] = 0 if the voxel is in
  * the SINK set else 1, C-order over the logical shape.  `mem` selects host or device destination. */
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem);

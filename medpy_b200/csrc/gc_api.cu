@@ -11,8 +11,10 @@
 #include "gc_tiles4.cuh"
 #include "gc_sweep.cuh"
 #include "gc_build.cuh"
+#include "gc_seeds.cuh"
 #include "gc_gradient.cuh"
 
+#include <algorithm>
 #include <dlfcn.h>
 #include <nccl.h>
 #include <nvtx3/nvToolsExt.h>
@@ -163,11 +165,19 @@ struct mgc_graph {
     // writes them all)
     bool lazy_caps = true;
     bool caps_lazy = false;            // the last build was lazy and some tiles are not materialised yet
+    // the last build was the lazy fused build and nothing else changed the terms since: mgc_add_seeds may fold seeds
+    // into the residual state.  Unlike caps_lazy this stays true once every tile is materialised (hard instances).
+    bool lazy_built = false;
     int* cmat = nullptr;               // per tile: push state materialised since the last lazy build
     int* caps_list = nullptr;          // tiles claimed by the current materialiser launch
+    // The copies below (with caps_P and caps_tin) live as long as the handle's last lazy build: besides the materialiser,
+    // mgc_add_seeds depends on them -- it recomputes a seeded voxel's capacities before any flow from img_copy to know
+    // the source flow its state already holds (gc_seeds.cuh).  Dropping them breaks the warm re-solve.
     Buf img_copy;                      // the image the lazy build saw, in its own dtype
     Buf prob_copy;                     // ... its probability map, in its own dtype
     Buf mark_planes[2];                // ... its fg / bg markers as bit planes (LazyTin)
+    Buf seed_buf;                      // mgc_add_seeds: list count, seeded tiles, grouped seeds
+    cudaEvent_t ev_seed[2] = {};       // span of claim + fold + list fix-up
     int caps_dtype = MGC_F32;
     BoundaryParams caps_P{};           // the boundary term of the lazy build
     LazyTin caps_tin{};                // its t-link terms
@@ -413,6 +423,7 @@ int finish_flow_const(mgc_graph* g)
 
 void invalidate(mgc_graph* g)
 {
+    g->lazy_built = false;             // terms changed outside the lazy build
     g->state_init = false;
     g->solved = false;
     g->host_mask_valid = false;
@@ -842,6 +853,22 @@ int caps_launch(mgc_graph* g, WorkList wl)
     g->st.kernel_launches += 2;
     CK(cudaGetLastError());
     return MGC_OK;
+}
+
+// k_seed_fold with the boundary term of the lazy build (the instantiations of k_caps_tiles)
+template <typename E>
+void seed_fold_launch_t(mgc_graph* g, unsigned grid, const SeedItem* items, int n)
+{
+    const BoundaryParams& P = g->caps_P;
+    const E* img = (const E*)g->img_copy.p;
+    if constexpr (!std::is_integral<E>::value) {
+        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
+            if (P.use_max) k_seed_fold<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, g->partials);
+            else           k_seed_fold<E, 1, 0, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, g->partials);
+            return;
+        }
+    }
+    k_seed_fold<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, g->partials);
 }
 
 // capacities, tr or excess are about to be read or written outside the push path: materialise the tiles that are not yet
@@ -1717,6 +1744,8 @@ void mgc_destroy(mgc_graph* g)
     if (g->img_copy.p) pool_free(g->device, g->img_copy.bytes, g->img_copy.p);
     if (g->prob_copy.p) pool_free(g->device, g->prob_copy.bytes, g->prob_copy.p);
     for (auto& b : g->mark_planes) if (b.p) pool_free(g->device, b.bytes, b.p);
+    if (g->seed_buf.p) pool_free(g->device, g->seed_buf.bytes, g->seed_buf.p);
+    for (auto& ev : g->ev_seed) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->caps_ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->ev_slot) if (ev) cudaEventDestroy(ev);
@@ -2192,6 +2221,10 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     g->caps_fresh = false;
     g->tr_fresh = false;
     g->caps_lazy = lazy;
+    g->lazy_built = lazy;
+    g->st.seed_folds = 0;
+    g->st.ms_seeds = 0.0;
+    g->st.ms_seeds_host = 0.0;
     g->caps_dtype = t->image->dtype;
     g->caps_P = P;
     g->caps_tin = LazyTin{A.prob_copy, A.prob_f64, A.compute_f32, A.alpha, A.fg_plane, A.bg_plane, mark_words};
@@ -2319,6 +2352,122 @@ int mgc_maxflow(mgc_graph* g, double* energy)
     caps_resolve(g);
     g->solved = true;
     if (energy) *energy = g->energy;
+    return MGC_OK;
+}
+
+int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem)
+{
+    if (!g) return MGC_E_ARG;
+    if (n_fg < 0 || n_bg < 0 || (n_fg && !fg_ids) || (n_bg && !bg_ids)) FAIL(MGC_E_ARG, "bad seed lists");
+    if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
+    if (!g->lazy_built || !g->state_init || g->slab || !g->use_tiles || g->nd != 3)
+        FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
+                          "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
+                          "the seeds instead");
+    CK(cudaSetDevice(g->device));
+    { int rc0 = check_pending(g); if (rc0) return rc0; }
+    if (n_fg + n_bg == 0) return MGC_OK;       // nothing to fold: the solved state, mask and energy stay as they are
+    const auto host_t0 = std::chrono::steady_clock::now();
+    std::vector<int64_t> ids((size_t)(n_fg + n_bg));
+    if (mem == MGC_MEM_DEVICE) {
+        if (n_fg) CK(cudaMemcpyAsync(ids.data(), fg_ids, (size_t)n_fg * 8, cudaMemcpyDeviceToHost, g->stream));
+        if (n_bg) CK(cudaMemcpyAsync(ids.data() + n_fg, bg_ids, (size_t)n_bg * 8, cudaMemcpyDeviceToHost, g->stream));
+        CK(cudaStreamSynchronize(g->stream));
+    } else {
+        if (n_fg) std::memcpy(ids.data(), fg_ids, (size_t)n_fg * 8);
+        if (n_bg) std::memcpy(ids.data() + n_fg, bg_ids, (size_t)n_bg * 8);
+    }
+    // group by voxel: key = v * 2 + (background); per voxel the reference applies all its fg seeds, then all its bg seeds
+    const int64_t n = (int64_t)g->L.n;
+    std::vector<uint64_t> keys(ids.size());
+    for (size_t i = 0; i < ids.size(); ++i) {
+        const int64_t v = ids[i];
+        if (v < 0 || v >= n) FAIL(MGC_E_ARG, "node id out of range");
+        keys[i] = ((uint64_t)v << 1) | (i >= (size_t)n_fg ? 1u : 0u);
+    }
+    // ids from a mask arrive sorted: sort each list only when it is not, then merge the two runs in linear time
+    const auto mid = keys.begin() + n_fg;
+    if (!std::is_sorted(keys.begin(), mid)) std::sort(keys.begin(), mid);
+    if (!std::is_sorted(mid, keys.end())) std::sort(mid, keys.end());
+    std::inplace_merge(keys.begin(), mid, keys.end());
+    std::vector<SeedItem> items;
+    items.reserve(keys.size());
+    std::vector<int> tiles;
+    std::vector<uint8_t> tile_seen((size_t)g->TL.ntiles, 0);
+    for (size_t i = 0; i < keys.size();) {
+        const unsigned v = (unsigned)(keys[i] >> 1);
+        SeedItem it{v, 0, 0, 0};
+        for (; i < keys.size() && (unsigned)(keys[i] >> 1) == v; ++i) (keys[i] & 1u) ? ++it.nb : ++it.nf;
+        items.push_back(it);
+        const int gz = (int)(v / g->L.stride[0]), r = (int)(v % g->L.stride[0]);
+        const int gy = r / (int)g->L.stride[1], gx = r % (int)g->L.stride[1];
+        const int t = ((gz / TILE) * g->TL.nt[1] + gy / TILE) * g->TL.nt[2] + gx / TILE;
+        if (!tile_seen[(size_t)t]) { tile_seen[(size_t)t] = 1; tiles.push_back(t); }
+    }
+    // device layout: [count | pad] [tile ids] [items, 16-byte aligned]
+    const size_t tiles_off = 16, items_off = (tiles_off + tiles.size() * 4 + 15) / 16 * 16;
+    const size_t bytes = items_off + items.size() * sizeof(SeedItem);
+    int rc = ensure_scratch(g, g->seed_buf, bytes);
+    if (rc) return rc;
+    std::vector<char> host(bytes, 0);
+    const int nt = (int)tiles.size();
+    std::memcpy(host.data(), &nt, sizeof(int));
+    std::memcpy(host.data() + tiles_off, tiles.data(), tiles.size() * 4);
+    std::memcpy(host.data() + items_off, items.data(), items.size() * sizeof(SeedItem));
+    char* dbuf = (char*)g->seed_buf.p;
+    for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
+    Nvtx range("mgc:add_seeds");
+    g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
+    CK(cudaEventRecord(g->ev_seed[0], g->stream));
+    CK(cudaMemcpyAsync(dbuf, host.data(), bytes, cudaMemcpyHostToDevice, g->stream));
+    // 1. every seeded voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
+    if (g->caps_lazy) {
+        if (!g->flow_started) {
+            // not solved yet: the build's push lists name the tiles with source excess, which is still implicit there.
+            // Materialise them now (as the stop test of a first round does): step 3 rebuilds the lists from cmat.
+            for (int color = 0; color < 2; ++color) { rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
+        }
+        rc = caps_launch(g, WorkList{(int*)(dbuf + tiles_off), (int*)dbuf});
+        if (rc) return rc;
+    }
+    // 2. the fold, its change of the add_tweights constant summed in a fixed order into flow_const
+    const int ni = (int)items.size();
+    unsigned grid = (unsigned)((ni + 255) / 256);
+    if (grid > REDUCE_BLOCKS) grid = REDUCE_BLOCKS;
+    const SeedItem* d_items = (const SeedItem*)(dbuf + items_off);
+    switch (g->caps_dtype) {
+        case MGC_F32: seed_fold_launch_t<float>(g, grid, d_items, ni); break;
+        case MGC_F64: seed_fold_launch_t<double>(g, grid, d_items, ni); break;
+        case MGC_U8: seed_fold_launch_t<uint8_t>(g, grid, d_items, ni); break;
+        case MGC_I16: seed_fold_launch_t<int16_t>(g, grid, d_items, ni); break;
+        default: seed_fold_launch_t<int32_t>(g, grid, d_items, ni); break;
+    }
+    k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, grid, g->d_scalars);
+    // 3. solver state for the next solve: fresh push lists over every materialised tile with excess; labels from a full
+    // relabel reset (sweep_mode = -1: a fold can remove a sink link, so the last solve's labels bound nothing)
+    CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
+    CK(cudaMemsetAsync(g->pflag, 0, (size_t)g->TL.ntiles * sizeof(int), g->stream));
+    g->pl_sel[0] = g->pl_sel[1] = 0;
+    {
+        unsigned lgrid = (unsigned)g->n_ctas * 4u;
+        if (lgrid > (unsigned)g->TL.ntiles) lgrid = (unsigned)g->TL.ntiles;
+        k_seed_lists<<<lgrid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->cmat, g->pflag, pl(g, 0, 0), pl(g, 1, 0));
+    }
+    g->st.kernel_launches += 3;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(g->ev_seed[1], g->stream));
+    CK(cudaEventSynchronize(g->ev_seed[1]));       // the host staging vector is released on return
+    {
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, g->ev_seed[0], g->ev_seed[1]) == cudaSuccess) g->st.ms_seeds += ms;
+        g->st.ms_caps -= caps_resolve(g);          // the claim is part of ms_seeds, not of the solve's materialisation
+    }
+    g->labels_fresh = false;
+    g->rl_cur = 0;
+    g->sweep_mode = -1;
+    g->solved = false;
+    g->host_mask_valid = false;
+    g->st.seed_folds++;
     return MGC_OK;
 }
 

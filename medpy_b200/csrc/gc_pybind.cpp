@@ -218,6 +218,44 @@ public:
         { py::gil_scoped_release rel; rc = mgc_add_nweights_dense(g_, axis, &a.a, &b.a); }
         check(rc, g_);
     }
+    // seeds folded into the solved graph (mgc_add_seeds): 1-D int64 node-id arrays, both on the host (numpy) or both on
+    // the device (__cuda_array_interface__); None = no seeds of that kind
+    void add_seeds(const py::object& fg, const py::object& bg)
+    {
+        struct Ids { const int64_t* p = nullptr; int64_t n = 0; int mem = -1; py::object keep; };
+        auto ids = [](const py::object& o, const char* what) {
+            Ids r;
+            if (o.is_none()) return r;
+            if (py::hasattr(o, "__cuda_array_interface__")) {
+                py::dict d = o.attr("__cuda_array_interface__");
+                py::tuple shp = d["shape"];
+                const std::string ts = d["typestr"].cast<std::string>();
+                if (shp.size() != 1 || ts.substr(1) != "i8") throw py::value_error(std::string(what) + ": expected a 1-D int64 array");
+                if (d.contains("strides") && !d["strides"].is_none()) {
+                    py::tuple st = d["strides"];
+                    if (st[0].cast<int64_t>() != 8) throw py::value_error(std::string(what) + ": ids must be contiguous");
+                }
+                r.p = reinterpret_cast<const int64_t*>(py::tuple(d["data"])[0].cast<uintptr_t>());
+                r.n = shp[0].cast<int64_t>();
+                r.mem = MGC_MEM_DEVICE;
+                r.keep = o;
+            } else {
+                auto a = py::array_t<int64_t, py::array::c_style | py::array::forcecast>::ensure(o);
+                if (!a || a.ndim() != 1) throw py::value_error(std::string(what) + ": expected a 1-D int64 array");
+                r.p = a.data();
+                r.n = a.shape(0);
+                r.mem = MGC_MEM_HOST;
+                r.keep = a;
+            }
+            return r;
+        };
+        Ids f = ids(fg, "fg_ids"), b = ids(bg, "bg_ids");
+        if (f.n && b.n && f.mem != b.mem) throw py::value_error("fg_ids and bg_ids must both be host or both be device arrays");
+        const int mem = f.n ? f.mem : (b.n ? b.mem : MGC_MEM_HOST);
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_add_seeds(g_, f.n ? f.p : nullptr, f.n, b.n ? b.p : nullptr, b.n, mem); }
+        check(rc, g_);
+    }
     double maxflow()
     {
         double e = 0;
@@ -268,6 +306,7 @@ public:
         d["ms_push"] = s.ms_push; d["ms_relabel"] = s.ms_relabel; d["ms_boundary"] = s.ms_boundary; d["ms_init"] = s.ms_init;
         d["flow_const"] = s.flow_const; d["energy"] = s.energy; d["device_bytes"] = s.device_bytes;
         d["tiles_materialised"] = s.tiles_materialised; d["ms_caps"] = s.ms_caps;
+        d["seed_folds"] = s.seed_folds; d["ms_seeds"] = s.ms_seeds; d["ms_seeds_host"] = s.ms_seeds_host;
         return d;
     }
     // ---- z-slab stepping (device pointers as integers, e.g. torch.Tensor.data_ptr()) ----
@@ -594,6 +633,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("add_markers", &PyGraph::add_markers)
         .def("add_boundary", &PyGraph::add_boundary)
         .def("add_nweights_dense", &PyGraph::add_nweights_dense)
+        .def("add_seeds", &PyGraph::add_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
         .def("build_voxel_graph", &PyGraph::build_voxel_graph)
         .def_static("slab_comm_unique_id", &PyGraph::slab_comm_unique_id)
         .def("slab_comm_init", &PyGraph::slab_comm_init)

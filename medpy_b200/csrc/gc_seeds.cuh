@@ -1,0 +1,148 @@
+// gc_seeds.cuh -- seeds added to a solved lazily built 3-D graph, folded into its residual state (mgc_add_seeds).
+//
+// The reference refines a cut by calling add_tweights(v, 65535, 0) / add_tweights(v, 0, 65535) on the new seed voxels of
+// a solved GraphDouble and calling maxflow() again: BK's add_tweights (graph.h:415-425) works on the RESIDUAL terminal
+// capacity r(v) that the first maxflow() left, and the second maxflow() continues from that residual graph.  Here the
+// same happens to the push-relabel state (DESIGN.md §4.6):
+//   1. the tiles of the seeded voxels are materialised first (k_caps_claim / k_caps_tiles), so every seeded voxel holds
+//      cap[], tr, excess and its sink-link state, and the fold below reads one representation only.  The marker bit planes
+//      are never read again for a claimed tile, so they are not updated;
+//   2. k_seed_fold (one thread per seeded voxel, the seeds of a voxel grouped by the host in the reference's order) reads
+//      r(v) from that state, replays the seeds with add_tweights_dev -- the reference's arithmetic on r -- and writes r'
+//      back in the solver's representation;
+//   3. k_seed_lists puts every materialised tile that holds excess back on the push lists; the next solve starts with a
+//      full relabel reset.
+#pragma once
+#include "gc_build.cuh"
+
+// one seeded voxel: `nf` foreground seeds, then `nb` background seeds (list order of the reference: every fg id first)
+struct SeedItem {
+    unsigned v;
+    int nf;
+    int nb;
+    int pad;
+};
+
+// Residual terminal capacity r(v) in the state of a materialised voxel (BK's tr_cap after the flow so far):
+//   tr > 0 : tr - source_excess(tr, c_orig)   -- the source flow the build (or an earlier fold) pushed is
+//            source_excess(tr, c_orig) exactly, c_orig = the voxel's capacities before any flow, from the image copy;
+//   tr < 0 : tr + sink[v]                      -- sink capacity -tr minus the flow it absorbed (0 unless RM_SINKV);
+//   tr = 0 : 0.
+// The fold moves the absorbed flow into the add_tweights constant (it stays counted once: the energy is constant +
+// absorbed flow), applies the seeds to r with the reference's arithmetic and writes r' back:
+//   r' < 0 : tr = r' (a fresh sink link of capacity -r'), and the voxel's own excess goes through it at once
+//            (sink[v] = min(excess, -r'), saturation exact as in the push kernel);
+//   r' > 0 : a source residual of r'.  At least p = min(r', residual out-capacity (rounded up) x SOURCE_CLAMP_SLACK)
+//            joins the excess -- the clamp of DESIGN.md §4.2 on the residual graph: whatever more the source link could
+//            send has to leave through those arcs.  The rest must survive for a later fold (a background seed would count
+//            it in the constant).  When that bound is within lim(c_orig) (no net inflow), source_excess(r', c_orig) is
+//            pushed and tr = r', the build's own representation, read back exactly.  Otherwise p is pushed and
+//            tr = u + lim(c_orig) for the rest u = r' - p > 0, whose source_excess is lim and whose residual reads back
+//            as u to one rounding; tr = 0 when u = 0;
+//   r' = 0 : tr = 0.
+template <typename E, int FN, int USE_MAX, int SPACING>
+__global__ void __launch_bounds__(256)
+k_seed_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParams P, const SeedItem* __restrict__ items,
+            int n, double* __restrict__ partials)
+{
+    const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
+    const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
+    double m = 0.0;
+    const int step = (int)(gridDim.x * blockDim.x);
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
+        const SeedItem it = items[i];
+        const unsigned v = it.v;
+        int c[3];
+        decode<3>(L, v, c);
+        // capacities before any flow: the doubles k_caps_tiles computed from the same image copy
+        const unsigned valid = (c[0] > 0 ? 1u : 0u) | (c[0] + 1 < L.dim[0] ? 2u : 0u) | (c[1] > 0 ? 4u : 0u) |
+                               (c[1] + 1 < L.dim[1] ? 8u : 0u) | (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
+        const double a = build_val<E>(img[v], use_max);
+        double co[6];
+        if (FN == 1 && SPACING == 0) {
+            double t6[6];
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+                t6[k] = 0.0;
+                if ((valid >> k) & 1u) {
+                    const double b = build_val<E>(img[(unsigned)((int)v + dir_offset(L, k))], use_max);
+                    t6[k] = exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
+                }
+            }
+            exp_caps6(t6, false, valid, co);       // the general branch: the same doubles for ordinary arguments
+        } else {
+#pragma unroll
+            for (int k = 0; k < 6; ++k)
+                co[k] = ((valid >> k) & 1u)
+                            ? build_weight<FN, E>(P, a, img[(unsigned)((int)v + dir_offset(L, k))], use_max, spacing, P.spacing[k >> 1])
+                            : 0.0;
+        }
+        double lim0 = __dadd_ru(0.0, co[0]);
+        lim0 = __dadd_ru(lim0, co[1]); lim0 = __dadd_ru(lim0, co[2]); lim0 = __dadd_ru(lim0, co[3]);
+        lim0 = __dadd_ru(lim0, co[4]); lim0 = __dadd_ru(lim0, co[5]);
+        lim0 = lim0 * SOURCE_CLAMP_SLACK;
+
+        const double tr = S.tr[v];
+        const unsigned rm = S.rmask[v];
+        double e = S.excess[v];
+        double dk = 0.0;
+        double r = 0.0;
+        if (tr > 0) {
+            r = __dsub_rn(tr, source_excess(tr, co));
+        } else if (tr < 0) {
+            const double sf = (rm & RM_SINKV) ? S.sink[v] : 0.0;
+            r = __dadd_rn(tr, sf);
+            dk = sf;
+        }
+        for (int j = 0; j < it.nf; ++j) dk = __dadd_rn(dk, add_tweights_dev(r, 65535.0, 0.0));
+        for (int j = 0; j < it.nb; ++j) dk = __dadd_rn(dk, add_tweights_dev(r, 0.0, 65535.0));
+
+        unsigned nm = rm & 0x3fu;
+        double trn = 0.0;
+        if (r < 0) {
+            trn = r;
+            const double cap = -r;
+            double sf;
+            if (e >= cap) { sf = cap; e = __dsub_rn(e, cap); }
+            else { sf = e; e = 0.0; }
+            if (cap - sf > 0) nm |= RM_SINK;
+            S.sink[v] = sf;
+            nm |= RM_SINKV;
+        } else if (r > 0) {
+            double out = __dadd_ru(0.0, S.cap[0][v]);
+            out = __dadd_ru(out, S.cap[1][v]); out = __dadd_ru(out, S.cap[2][v]); out = __dadd_ru(out, S.cap[3][v]);
+            out = __dadd_ru(out, S.cap[4][v]); out = __dadd_ru(out, S.cap[5][v]);
+            const double lim = out * SOURCE_CLAMP_SLACK;
+            if (!(lim > lim0)) {
+                // the usual case (no net inflow through the n-links): push source_excess(r', c_orig) >= min(r', lim) and
+                // keep tr = r', which reads back as r' - source_excess(r', c_orig) bit for bit
+                e = __dadd_rn(e, source_excess(r, co));
+                trn = r;
+            } else {
+                const double p = r < lim ? r : lim;
+                e = __dadd_rn(e, p);
+                const double u = __dsub_rn(r, p);
+                if (u > 0) trn = __dadd_rn(u, lim0);      // reads back as (u + lim0) - lim0: u to one rounding
+            }
+        }
+        S.tr[v] = trn;
+        S.excess[v] = e;
+        S.rmask[v] = (uint8_t)nm;
+        m = __dadd_rn(m, dk);
+    }
+    block_sum_store(m, partials);
+}
+
+// push lists after a fold: every materialised tile (cmat[t] = 1) holding an owned voxel with excess goes on the list its
+// colour consumes next.  Excess stranded at voxels the last solve labelled HINF may reach a new sink link now; only
+// materialised tiles can hold excess (a solve materialises every tile the build listed before it pushes or stops).
+__global__ void __launch_bounds__(TILE_VOX) k_seed_lists(Lattice L, Tiles TL, State<double> S, const int* __restrict__ cmat,
+                                                         int* __restrict__ pflag, WorkList pl0, WorkList pl1)
+{
+    for (int t = blockIdx.x; t < TL.ntiles; t += gridDim.x) {
+        if (cmat[t] == 0) continue;            // block-uniform
+        const TileCtx c = tile_ctx(L, TL, t);
+        const int act = (c.own && S.excess[c.v] > 0) ? 1 : 0;
+        if (__syncthreads_or(act) && threadIdx.x == 0) list_push(pflag, tile_color(c) ? pl1 : pl0, t);
+    }
+}

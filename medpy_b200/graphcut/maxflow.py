@@ -77,6 +77,7 @@ class GraphDouble:
         # needs the graph.  Only while nothing has reached the device yet (_fresh).
         self._lazy = None
         self._fresh = True
+        self._solved = False     # maxflow() ran since the last reset: add_seeds folds into the residual state
         if sparse:
             if self._journal is None:
                 raise ValueError("a lattice shape and sparse=True exclude each other")
@@ -381,7 +382,68 @@ class GraphDouble:
                 "edge {} does not join lattice neighbours of shape {}: build general graphs with "
                 "GraphDouble(nodes, edges) (no shape), which uses the sparse backend".format(self._offlattice, self._shape))
         self._flush()
-        return self._nat().maxflow()
+        flow = self._nat().maxflow()
+        self._solved = True
+        return flow
+
+    def _seed_ids(self, seeds):
+        """Node ids of one seed argument: a boolean mask of the lattice shape (any strides; ids in the logical C order,
+        like generate.py:169-172), or a 1-D integer id array; numpy or a CUDA tensor.  Range-checked like
+        GCGraph.set_source_nodes (graph.py:334-339)."""
+        if seeds is None:
+            return None
+        if hasattr(seeds, "__cuda_array_interface__"):
+            import torch
+            t = torch.as_tensor(seeds)
+            if t.dtype == torch.bool:
+                if tuple(t.shape) != self._shape:
+                    raise ValueError("seed mask of shape {} does not match the graph's shape {}".format(tuple(t.shape), self._shape))
+                ids = t.reshape(-1).nonzero().reshape(-1)
+            else:
+                if t.dim() != 1 or t.dtype.is_floating_point or t.dtype.is_complex:
+                    raise ValueError("seeds must be a boolean mask of the graph's shape or a 1-D integer id array")
+                ids = t.to(torch.int64).contiguous()
+            if ids.numel():
+                lo, hi = int(ids.min()), int(ids.max())
+                if hi >= self._n or lo < 0:
+                    raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(hi, lo, self._n - 1))
+            return ids
+        a = numpy.asarray(seeds)
+        if a.dtype == numpy.bool_:
+            if a.shape != self._shape:
+                raise ValueError("seed mask of shape {} does not match the graph's shape {}".format(a.shape, self._shape))
+            return a.ravel().nonzero()[0].astype(numpy.int64)
+        if a.ndim != 1 or not (a.size == 0 or numpy.issubdtype(a.dtype, numpy.integer)):
+            raise ValueError("seeds must be a boolean mask of the graph's shape or a 1-D integer id array")
+        ids = a.astype(numpy.int64)
+        if ids.size and (ids.max() >= self._n or ids.min() < 0):
+            raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(ids.max(), ids.min(), self._n - 1))
+        return ids
+
+    def add_seeds(self, fg=None, bg=None):
+        """Add foreground / background seeds and let the next ``maxflow()`` return the cut of the enlarged graph.
+
+        Exactly ``add_tweights(v, 65535, 0)`` for every foreground id in order, then ``add_tweights(v, 0, 65535)`` for
+        every background id (GCGraph.set_source_nodes / set_sink_nodes, graph.py:310-380).  ``fg`` / ``bg``: a boolean
+        mask of the lattice shape, a 1-D integer id array (repeated ids count once per occurrence), or None.
+
+        Before the first ``maxflow()`` the calls are staged like ``add_tweights``.  After it, on a graph that
+        ``graph_from_voxels`` built in one fused pass (1-D..3-D lattice on one GPU), the seeds are folded into the solved
+        state and the next solve continues from the flow already routed (mgc_add_seeds).  Any other solved graph raises
+        ``RuntimeError``: ``reset()`` it and build the graph again with the seeds."""
+        fg_ids, bg_ids = self._seed_ids(fg), self._seed_ids(bg)
+        if not self._solved:
+            for ids, src, snk in ((fg_ids, 65535.0, 0.0), (bg_ids, 0.0, 65535.0)):
+                if ids is not None and len(ids):
+                    if not isinstance(ids, numpy.ndarray):
+                        ids = ids.cpu().numpy()
+                    self.stage_tweights_many(ids, src, snk)
+            return
+        if self._sp is not None:
+            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
+                               "rebuild it with the seeds instead")
+        self._dirty()
+        self._nat().add_seeds(fg_ids, bg_ids)
 
     def get_mask(self):
         """Bulk read-out: uint8 array of the lattice shape, 0 where what_segment == SINK else 1
@@ -415,6 +477,7 @@ class GraphDouble:
         self._pending = []
         self._lazy = None
         self._fresh = True
+        self._solved = False
         if self._native is not None:
             self._native.reset()
 

@@ -1,0 +1,121 @@
+"""Warm re-solve after added seeds (GraphDouble.add_seeds -> mgc_add_seeds) against a cold rebuild of the same graph.
+
+Config 3 at 512^3 (regional + boundary) and config 2 at 256^3 (boundary only), inputs resident in HBM.  For each
+configuration: a cold solve, then three strokes, each applied to a freshly solved graph --
+  carve : a background ball of radius 0.05 n inside blob 1 (inside its foreground markers: fg and bg cancel there),
+  line  : a foreground line through the background between the two blobs,
+  both  : the two together.
+Per stroke and run it prints, for the warm path: the wall time of add_seeds (which returns after its device work) with
+the library's split of it into host work before anything is enqueued (ms_seeds_host: id copy, range check, grouping)
+and device time (ms_seeds: claim + materialisation, fold, push-list fix-up); the CUDA-event span of maxflow + mask into
+device memory, with its solve time and relabel / push / materialisation / read-out device ms from the library's stats;
+the wall time from host id arrays to the mask in device memory and on the host.  For the cold path: the CUDA-event
+span of the fused build with the seeds merged into the markers (the same graph) + solve + mask.  Both spans are host
+driven (the solve synchronises once per round), so they contain host gaps.  Also whether the two masks hash equal
+and the energy difference.  Runs alternate warm / cold.
+
+    python tools/bench_refine.py [--runs 3] [--config3 512] [--config2 256] [--out rows.json]
+"""
+import argparse
+import hashlib
+import json
+import os
+import sys
+import time
+
+import numpy
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def _sha(a):
+    return hashlib.sha256(numpy.ascontiguousarray(a).tobytes()).hexdigest()[:16]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--config3", type=int, default=512)
+    ap.add_argument("--config2", type=int, default=256)
+    ap.add_argument("--out", default=None, help="also write the rows to this JSON file")
+    args = ap.parse_args()
+    import torch
+    from medpy_b200 import synthetic
+    from medpy_b200.graphcut.device import graph_from_device_arrays
+    stream = torch.cuda.current_stream()
+    out = []
+    for name, n, regional in (("config3", args.config3, True), ("config2", args.config2, False)):
+        shape = (n, n, n)
+        vol = synthetic.two_blob_volume(shape, seed=0, with_prob=regional)
+        d_img = torch.from_numpy(vol["image"]).cuda()
+        d_prob = torch.from_numpy(vol["prob"]).cuda() if regional else None
+        carve = synthetic._ball_mask(shape, (0.3,), 0.05)
+        line = numpy.zeros(shape, bool)
+        line[n // 2, n // 2, int(0.4 * n):int(0.6 * n)] = True
+        strokes = {"carve": (None, carve), "line": (line, None), "both": (line, carve)}
+        d_mask = torch.empty(shape, dtype=torch.uint8, device="cuda")
+
+        def dev(m):
+            return torch.from_numpy(m.view(numpy.uint8)).cuda()
+
+        def build(d_fg, d_bg, graph=None):
+            return graph_from_device_arrays(d_fg, d_bg, image=d_img, boundary="difference_exponential", sigma=vol["sigma"],
+                                            prob=d_prob, alpha=vol.get("alpha"), graph=graph, stream=stream.cuda_stream)
+
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for sname, (sfg, sbg) in strokes.items():
+            fg_ids = numpy.flatnonzero(sfg) if sfg is not None else numpy.zeros(0, numpy.int64)
+            bg_ids = numpy.flatnonzero(sbg) if sbg is not None else numpy.zeros(0, numpy.int64)
+            d_fg0, d_bg0 = dev(vol["fg"]), dev(vol["bg"])
+            d_fg2 = dev(vol["fg"] | (sfg if sfg is not None else False))
+            d_bg2 = dev(vol["bg"] | (sbg if sbg is not None else False))
+            for run in range(args.runs):
+                # warm: a freshly solved graph, then the stroke
+                g = build(d_fg0, d_bg0)
+                g.maxflow()
+                torch.cuda.synchronize()
+                s0 = dict(g.stats())
+                t0 = time.perf_counter()
+                g.add_seeds(fg_ids, bg_ids)            # returns after its device work finished
+                t1 = time.perf_counter()
+                ev0.record(stream)
+                e_warm = g.maxflow()
+                g._nat().get_mask_into(d_mask.data_ptr())
+                ev1.record(stream)
+                torch.cuda.synchronize()
+                t2 = time.perf_counter()
+                solve_span = ev0.elapsed_time(ev1)
+                m_host = g.get_mask()
+                wall = (time.perf_counter() - t0) * 1e3
+                s1 = g.stats()
+                warm_hash = _sha(m_host)
+                del g
+                # cold: the same graph built from scratch (seeds merged into the markers), solved, mask into device memory
+                torch.cuda.synchronize()
+                ev0.record(stream)
+                gc_ = build(d_fg2, d_bg2)
+                e_cold = gc_.maxflow()
+                gc_._nat().get_mask_into(d_mask.data_ptr())
+                ev1.record(stream)
+                torch.cuda.synchronize()
+                cold_dev = ev0.elapsed_time(ev1)
+                cold_hash = _sha(d_mask.cpu().numpy())
+                del gc_
+                d = {k: s1[k] - s0.get(k, 0.0) for k in ("ms_seeds", "ms_seeds_host", "ms_solve", "ms_relabel", "ms_push",
+                                                          "ms_caps", "ms_readout", "push_sweeps", "global_relabels")}
+                row = dict(config=name, n=n, stroke=sname, run=run, seeds=int(fg_ids.size + bg_ids.size),
+                           add_seeds_wall_ms=(t1 - t0) * 1e3, solve_span_ms=solve_span,
+                           warm_wall_ms_host_ids_to_device_mask=(t2 - t0) * 1e3,
+                           warm_wall_ms_host_ids_to_host_mask=wall, cold_span_ms=cold_dev,
+                           masks_equal=warm_hash == cold_hash, energy_diff=e_warm - e_cold, energy=e_cold, **d)
+                print(json.dumps(row), flush=True)
+                out.append(row)
+        del d_img, d_prob, d_mask
+        torch.cuda.empty_cache()
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
