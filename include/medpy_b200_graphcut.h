@@ -99,6 +99,8 @@ typedef struct mgc_stats {
     int64_t seed_folds;         /* mgc_add_seeds calls folded into this handle since its build (reset by the build)   */
     double ms_seeds;            /* device ms of those calls: tile claim + materialisation, fold, push-list fix-up     */
     double ms_seeds_host;       /* host ms of those calls before anything is enqueued: id copy, range check, grouping */
+    int64_t tiles_deferred;     /* 3-D tile solver, easy instance: listed tiles the label window held back, summed over the push launches of each solve */
+    int64_t tiles_dropped;      /* ... listed tiles that left the push lists without a visit (no active voxel at a finite label) */
 } mgc_stats;
 
 /* ---- lifetime ------------------------------------------------------------------------------------- */

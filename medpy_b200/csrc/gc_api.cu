@@ -201,6 +201,12 @@ struct mgc_graph {
     int* pl_items[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // push worklists [colour][buffer]
     int* d_tcount = nullptr;           // [0..1] relabel counts, [2..5] push counts [colour*2+buffer], [8] cursor
     int pl_sel[2] = {0, 0};            // buffer each colour consumes next
+    // label window of the push passes on easy instances (k_window_min / k_window_split): per list position the lowest
+    // active label of the tile, the list pushed now, control words (WIN_*), the tiles dropped before they were materialised
+    int* win_tmin = nullptr;
+    int* win_items = nullptr;
+    int* win_ctl = nullptr;
+    int* drop_items = nullptr;
     int rl_cur = 0;                    // relabel list consumed next
     bool labels_fresh = false;         // labels + relabel list 0 come straight from k_init_tile
     int n_ctas = 264;                  // persistent CTAs per tile-kernel launch
@@ -601,6 +607,11 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
         for (int i = 0; i < 2 && !rc; ++i) { rc = alloc_buf(g, tb, &p); g->rl_items[i] = (int*)p; }
         for (int i = 0; i < 4 && !rc; ++i) { rc = alloc_buf(g, tb, &p); g->pl_items[i >> 1][i & 1] = (int*)p; }
         if (!rc) { rc = alloc_buf(g, 256, &p); g->d_tcount = (int*)p; }
+        if (!rc) { rc = alloc_buf(g, tb, &p); g->win_tmin = (int*)p; }
+        if (!rc) { rc = alloc_buf(g, tb, &p); g->win_items = (int*)p; }
+        if (!rc) { rc = alloc_buf(g, tb, &p); g->drop_items = (int*)p; }
+        if (!rc) { rc = alloc_buf(g, 64, &p); g->win_ctl = (int*)p; }
+        if (!rc && cudaMemset(g->win_ctl, 0, 64) != cudaSuccess) { g->err = "cudaMemset of the window control words failed"; rc = MGC_E_CUDA; }
         {   // dirty-tile tracking for the partial relabel reset (MEDPY_GC_PARTIAL_RESET=0: off)
             const char* ed = getenv("MEDPY_GC_PARTIAL_RESET");
             g->TL.dflag = nullptr; g->TL.ditems = nullptr; g->TL.dcount = nullptr;
@@ -1173,27 +1184,52 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true)
 
 // one colour: consume its current list; still-active tiles go to its alternate list, receivers of cross-face flow
 // to the list the other colour consumes next
+// tiles whose push state may still be implicit (nullptr: every tile is materialised)
+const int* lazy_cmat(const mgc_graph* g) { return g->caps_lazy ? g->cmat : nullptr; }
+
+// label window of an easy instance (DESIGN.md §4.3): of the colour's current list, the tiles whose lowest active label is
+// within PUSH_WINDOW of the list's lowest go to win_items; the other tiles with an active voxel move to the colour's next
+// list, the rest leave the lists.  Returns the list to push now.
+int window_filter(mgc_graph* g, int color, int a, WorkList* now)
+{
+    const WorkList cur = pl(g, color, a);
+    *now = WorkList{g->win_items, g->win_ctl + WIN_NOW};
+    CK(cudaMemsetAsync(g->win_ctl + WIN_GMIN, 0x7f, sizeof(int), g->stream));      // above every label
+    CK(cudaMemsetAsync(g->win_ctl + WIN_NOW, 0, sizeof(int), g->stream));
+    k_window_min<double><<<g->n_ctas * 2, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, lazy_cmat(g), g->caps_tin, cur, g->win_tmin, g->win_ctl);
+    k_window_split<<<g->n_ctas, 256, 0, g->stream>>>(cur, g->win_tmin, lazy_cmat(g), g->pflag, *now, pl(g, color, 1 - a),
+                                                     g->drop_items, g->win_ctl);
+    g->st.kernel_launches += 2;
+    CK(cudaGetLastError());
+    return MGC_OK;
+}
+
 int push_color(mgc_graph* g, int color)
 {
     g->flow_started = true;
     const int a = g->pl_sel[color], oa = g->pl_sel[1 - color];
+    WorkList cur = pl(g, color, a);
+    if (g->sweep_mode == 0 && g->nd == 3 && !g->slab) {
+        const int rc = window_filter(g, color, a, &cur);
+        if (rc) return rc;
+    }
     if (g->caps_lazy) {
         // the pushers are the listed tiles, the receivers of cross-face flow their face neighbours: materialise those.  A
         // hard instance (sweeps at every relabel) pushes through most of the lattice: everything at once, then no more
-        const int rc = g->sweep_mode == 1 ? push_state_all(g) : caps_launch(g, pl(g, color, a));
+        const int rc = g->sweep_mode == 1 ? push_state_all(g) : caps_launch(g, cur);
         if (rc) return rc;
     }
     CK(cudaMemsetAsync(cursor(g), 0, sizeof(int), g->stream));
     if (g->nd == 4) {
-        k_push_tile4<double><<<g->n_ctas, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->smask, g->iters_now, g->pflag, pl(g, color, a),
+        k_push_tile4<double><<<g->n_ctas, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->smask, g->iters_now, g->pflag, cur,
                                                                   cursor(g), pl(g, color, 1 - a), pl(g, 1 - color, oa));
     } else if (g->use_tma) {
         const size_t smem = 2 * TMA_STAGE_BYTES + 6 * TILE_VOX * sizeof(double) + 1024 * sizeof(int) + 64;
         k_push_tile_tma<double><<<g->n_ctas, TILE_VOX, smem, g->stream>>>(g->L, g->TL, g->S, g->maps, g->iters_now, g->pflag,
-                                                                          pl(g, color, a), cursor(g), pl(g, color, 1 - a),
+                                                                          cur, cursor(g), pl(g, color, 1 - a),
                                                                           pl(g, 1 - color, oa));
     } else
-    k_push_tile<double><<<g->n_ctas, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->iters_now, g->pflag, pl(g, color, a),
+    k_push_tile<double><<<g->n_ctas, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->iters_now, g->pflag, cur,
                                                                cursor(g), pl(g, color, 1 - a), pl(g, 1 - color, oa));
     CK(cudaMemsetAsync(g->d_tcount + 2 + color * 2 + a, 0, sizeof(int), g->stream));   // consumed list is empty again
     g->pl_sel[color] = 1 - a;
@@ -1223,17 +1259,14 @@ int push_tiles(mgc_graph* g, int passes)
 // active voxels, counted exactly over the two pending push lists (a superset of the tiles that can hold one)
 int count_active_tiles_enqueue(mgc_graph* g, unsigned long long* dst)
 {
-    if (g->caps_lazy && !g->flow_started) {
-        // no push since the lazy build: the listed tiles hold no excess yet
-        for (int color = 0; color < 2; ++color) { const int rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
-    }
     CK(cudaMemsetAsync(dst, 0, sizeof(unsigned long long), g->stream));
     if (g->nd == 4) {
         for (int color = 0; color < 2; ++color)
             k_count_active_tiles4<double><<<g->n_ctas * 2, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, pl(g, color, g->pl_sel[color]), dst);
         g->st.kernel_launches += 2;
     } else {
-        k_count_active_tiles2<double><<<g->n_ctas * 2, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, pl(g, 0, g->pl_sel[0]), pl(g, 1, g->pl_sel[1]), dst);
+        k_count_active_tiles2<double><<<g->n_ctas * 2, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, lazy_cmat(g), g->caps_tin,
+                                                                                 pl(g, 0, g->pl_sel[0]), pl(g, 1, g->pl_sel[1]), dst);
         g->st.kernel_launches++;
     }
     CK(cudaGetLastError());
@@ -1326,6 +1359,7 @@ int solve_tiles(mgc_graph* g)
         rc = init_tiles(g);
         if (rc) return rc;
     }
+    if (g->win_ctl) CK(cudaMemsetAsync(g->win_ctl + WIN_DEFERRED, 0, 2 * sizeof(int), g->stream));    // per-solve window counts
     if (g->use_coop && g->nd == 3) {
         const int flags = SOLVE_F_LOOP | (g->labels_fresh ? 0 : SOLVE_F_RESET);
         g->labels_fresh = false;
@@ -1425,11 +1459,15 @@ int readout(mgc_graph* g, double* energy_part)
     g->st.kernel_launches += 2;
     double sc[2] = {0, 0};
     int n_mat = 0;
+    int win[2] = {0, 0};             // WIN_DEFERRED, WIN_DROPPED of this solve
     CK(cudaMemcpyAsync(sc, g->d_scalars, sizeof(sc), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaMemcpyAsync(&n_mat, g->d_flags + 3, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
+    if (g->win_ctl && g->use_tiles) CK(cudaMemcpyAsync(win, g->win_ctl + WIN_DEFERRED, sizeof(win), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
     g->st.flow_const = sc[0];
     g->st.tiles_materialised = n_mat;
+    g->st.tiles_deferred += win[0];
+    g->st.tiles_dropped += win[1];
     *energy_part = sc[0] + sc[1];
     if (g->init_timed) {
         float ms = 0;
@@ -2158,6 +2196,7 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
         if (t->bg || t->bg_bits) { rc = ensure_scratch(g, g->mark_planes[1], plane_bytes); if (rc) return rc; A.bg_plane = (unsigned*)g->mark_planes[1].p; }
         A.cmat = g->cmat;
         CK(cudaMemsetAsync(g->d_flags + 3, 0, sizeof(int), g->stream));      // tiles materialised
+        CK(cudaMemsetAsync(g->win_ctl + WIN_NDROP, 0, sizeof(int), g->stream));   // tiles dropped unmaterialised
     }
 
     CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
@@ -2422,11 +2461,13 @@ int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64
     CK(cudaMemcpyAsync(dbuf, host.data(), bytes, cudaMemcpyHostToDevice, g->stream));
     // 1. every seeded voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
     if (g->caps_lazy) {
-        if (!g->flow_started) {
-            // not solved yet: the build's push lists name the tiles with source excess, which is still implicit there.
-            // Materialise them now (as the stop test of a first round does): step 3 rebuilds the lists from cmat.
-            for (int color = 0; color < 2; ++color) { rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
-        }
+        // Source excess is still implicit on the tiles that are listed but not materialised (before the first solve, or
+        // deferred by the label window of the last one) and on the tiles the window dropped unmaterialised.  A new sink
+        // link may drain it: materialise them, step 3 rebuilds the lists from cmat.
+        for (int color = 0; color < 2; ++color) { rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
+        rc = caps_launch(g, WorkList{g->drop_items, g->win_ctl + WIN_NDROP});
+        if (rc) return rc;
+        CK(cudaMemsetAsync(g->win_ctl + WIN_NDROP, 0, sizeof(int), g->stream));
         rc = caps_launch(g, WorkList{(int*)(dbuf + tiles_off), (int*)dbuf});
         if (rc) return rc;
     }

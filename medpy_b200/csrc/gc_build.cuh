@@ -168,6 +168,15 @@ __device__ __forceinline__ double source_excess(double tr, const double c[6])
     return e;
 }
 
+// source_excess(tr, c) > 0 without the capacities, for a voxel whose in-lattice pairs are `pairs` (bit k: the pair across
+// face k exists).  Every such pair has a weight > 0 (then the rounded-up sum is > 0 and so is the clamp), +inf or NaN
+// (then the excess is tr itself), unless the build's weight check failed; so the excess is > 0 exactly when tr > 0 and
+// the voxel has a pair.  A failed check can only make this claim excess that is not there, which is safe for its users.
+__device__ __forceinline__ bool source_active(double tr, unsigned pairs)
+{
+    return tr > 0 && pairs != 0u;
+}
+
 // TIN = 1: the common configuration fixed at compile time -- float32 probability map with float32 products and both
 // marker volumes as bytes, all three staged by TMA.  The generic form (TIN = 0) decides each of those per voxel with
 // warp-uniform branches, whose bookkeeping costs instructions in this issue-heavy loop.
@@ -481,6 +490,53 @@ constexpr size_t build_smem_bytes()
 }
 
 // ---------------------------------------------------------------------------------------------------
+// The implicit push state of a lazy build, per voxel of a tile that is not materialised yet
+// ---------------------------------------------------------------------------------------------------
+// the in-lattice pairs of an in-lattice voxel (bit k: the pair across face k exists)
+__device__ __forceinline__ unsigned tile_pairs(const Lattice& L, const TileCtx& c)
+{
+    const int gz = c.tz * TILE + c.lz, gy = c.ty * TILE + c.ly, gx = c.tx * TILE + c.lx;
+    return (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) | (gy + 1 < L.dim[1] ? 8u : 0u) |
+           (gx > 0 ? 16u : 0u) | (gx + 1 < L.dim[2] ? 32u : 0u);
+}
+
+// the t-link inputs of an in-lattice voxel: its probability (0 without a map) and marker bits (bit 0 fg, bit 1 bg)
+__device__ __forceinline__ void lazy_tin_load(const Lattice& L, const LazyTin& tin, const TileCtx& c, double& p, unsigned& fb)
+{
+    const int gz = c.tz * TILE + c.lz, gy = c.ty * TILE + c.ly, gx = c.tx * TILE + c.lx;
+    if (tin.prob) p = tin.prob_f64 ? reinterpret_cast<const double*>(tin.prob)[c.v] : (double)reinterpret_cast<const float*>(tin.prob)[c.v];
+    const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * (unsigned)tin.words + ((unsigned)gx >> 5);
+    if (tin.fg) fb |= (tin.fg[w] >> (gx & 31)) & 1u;
+    if (tin.bg) fb |= ((tin.bg[w] >> (gx & 31)) & 1u) << 1;
+}
+
+// tr of the build, from those inputs
+__device__ __forceinline__ double lazy_tr(const LazyTin& tin, double p, unsigned fb)
+{
+    double tr = 0.0;
+    tlink_replay<double>(tr, tin.prob != nullptr, p, tin.compute_f32 != 0, tin.alpha, fb);
+    return tr;
+}
+
+// whether an owned, in-lattice voxel of a tile that is not materialised holds excess: the build's source excess, since
+// nothing else reaches such a tile (a push materialises its receivers first)
+__device__ __forceinline__ bool lazy_has_excess(const Lattice& L, const LazyTin& tin, const TileCtx& c)
+{
+    double p = 0.0;
+    unsigned fb = 0u;
+    lazy_tin_load(L, tin, c, p, fb);
+    return source_active(lazy_tr(tin, p, fb), tile_pairs(L, c));
+}
+
+// an active voxel: owned, at a finite label, with excess; `mat` = its tile's push state is materialised
+template <typename T>
+__device__ __forceinline__ bool voxel_active(const Lattice& L, const State<T>& S, const LazyTin& tin, const TileCtx& c, int h, bool mat)
+{
+    if (!c.own || h >= MGC_HINF) return false;
+    return mat ? S.excess[c.v] > 0 : lazy_has_excess(L, tin, c);
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Push-state materialiser of the lazy build: the six capacity planes, tr and excess of the tiles the push path is about
 // to touch, from the graph-owned copies the build wrote.  Runs over a push worklist -- every listed tile and its six face
 // neighbours, since a push writes across faces -- or, with wl.items == nullptr, over every tile.  A tile is materialised
@@ -579,20 +635,13 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
         if (tid == 0) s_slot[it & 1] = atomicAdd(cursor, 1);
         __syncthreads();
         // t-link inputs of this voxel, and the next tile's image: in flight while this tile is computed
-        const int gz = c.tz * TILE + c.lz, gy = c.ty * TILE + c.ly, gx = c.tx * TILE + c.lx;
         double p = 0.0;
         unsigned fb = 0u;
-        if (c.inb) {
-            if (tin.prob) p = tin.prob_f64 ? reinterpret_cast<const double*>(tin.prob)[c.v] : (double)reinterpret_cast<const float*>(tin.prob)[c.v];
-            const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * (unsigned)tin.words + ((unsigned)gx >> 5);
-            if (tin.fg) fb |= (tin.fg[w] >> (gx & 31)) & 1u;
-            if (tin.bg) fb |= ((tin.bg[w] >> (gx & 31)) & 1u) << 1;
-        }
+        if (c.inb) lazy_tin_load(L, tin, c, p, fb);
         const int inext = s_slot[it & 1];
         Cells nxt{(E)0, (E)0};
         if (inext < n) nxt = load(list[inext]);
-        const unsigned valid = c.inb ? ((gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) |
-                                        (gy + 1 < L.dim[1] ? 8u : 0u) | (gx > 0 ? 16u : 0u) | (gx + 1 < L.dim[2] ? 32u : 0u)) : 0u;
+        const unsigned valid = c.inb ? tile_pairs(L, c) : 0u;
         const double a = build_val<E>(s_img[h], use_max);
         const E q[6] = {s_img[h - HALO_DIM * HALO_DIM], s_img[h + HALO_DIM * HALO_DIM], s_img[h - HALO_DIM],
                         s_img[h + HALO_DIM], s_img[h - 1], s_img[h + 1]};
@@ -615,8 +664,7 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
                 cap[k] = ((valid >> k) & 1u) ? build_weight<FN, E>(P, a, q[k], use_max, spacing, P.spacing[k >> 1]) : 0.0;
         }
         if (c.inb) {
-            double tr = 0.0;
-            tlink_replay<double>(tr, tin.prob != nullptr, p, tin.compute_f32 != 0, tin.alpha, fb);
+            const double tr = lazy_tr(tin, p, fb);
             const double e = c.own ? source_excess(tr, cap) : 0.0;
 #pragma unroll
             for (int k = 0; k < 6; ++k) S.cap[k][c.v] = cap[k];
@@ -627,6 +675,126 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
         cur = nxt;
         i = inext;
     }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Label window of the push passes on an easy instance (sweep_mode == 0, DESIGN.md §4.3).  Before a colour's push launch,
+//   k_window_min   : the lowest label over the active voxels of every listed tile, and the minimum gmin over the list;
+//   k_window_split : tiles whose lowest active label is <= gmin + PUSH_WINDOW go to the list pushed (and materialised)
+//                    now; the other tiles with an active voxel wait on the colour's next list (pflag stays set); tiles
+//                    without one leave the lists.  Every relabel of such a solve is exact, so a voxel it labelled HINF
+//                    never becomes active again; tiles that leave unmaterialised are kept for mgc_add_seeds.
+// Both read a tile that is not materialised yet through its implicit push state (cmat[t] == 0; cmat == nullptr: every
+// tile is materialised).
+// ---------------------------------------------------------------------------------------------------
+#define PUSH_WINDOW 8
+#define WIN_GMIN 0         // control words: lowest active label of the list
+#define WIN_NOW 1          // ... count of the list pushed now
+#define WIN_DEFERRED 2     // ... tile deferrals since the solve started
+#define WIN_DROPPED 3      // ... tiles that left the lists since the solve started
+#define WIN_NDROP 4        // ... tiles that left unmaterialised since the build (list `drop_items`)
+
+template <typename T>
+__global__ void __launch_bounds__(TILE_VOX) k_window_min(Lattice L, Tiles TL, State<T> S, const int* __restrict__ cmat, LazyTin tin,
+                                                         WorkList cur, int* __restrict__ tmin, int* __restrict__ ctl)
+{
+    __shared__ int s_min[TILE_VOX / 32];
+    const int n = *cur.count;
+    for (int i = blockIdx.x; i < n; i += gridDim.x) {
+        const int t = cur.items[i];
+        const TileCtx c = tile_ctx(L, TL, t);
+        const bool mat = !cmat || cmat[t] != 0;
+        const int h = c.own ? S.height[c.v] : MGC_HINF;
+        int lo = voxel_active<T>(L, S, tin, c, h, mat) ? h : MGC_HINF;
+        lo = __reduce_min_sync(0xffffffffu, lo);
+        if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = lo;
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            int m = threadIdx.x < TILE_VOX / 32 ? s_min[threadIdx.x] : MGC_HINF;
+            m = __reduce_min_sync(0xffffffffu, m);
+            if (threadIdx.x == 0) {
+                tmin[i] = m;
+                if (m < MGC_HINF) atomicMin(ctl + WIN_GMIN, m);
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// append t of every lane with `take` to a list, one atomic per warp; returns the ballot
+__device__ __forceinline__ unsigned warp_append(const WorkList& wl, bool take, int t)
+{
+    const int lane = threadIdx.x & 31;
+    const unsigned b = __ballot_sync(0xffffffffu, take);
+    int slot = 0;
+    if (lane == 0 && b) slot = atomicAdd(wl.count, __popc(b));
+    slot = __shfl_sync(0xffffffffu, slot, 0);
+    if (take) wl.items[slot + __popc(b & ((1u << lane) - 1u))] = t;
+    return b;
+}
+
+__global__ void __launch_bounds__(256) k_window_split(WorkList cur, const int* __restrict__ tmin, const int* __restrict__ cmat,
+                                                      int* __restrict__ pflag, WorkList now, WorkList later,
+                                                      int* __restrict__ drop_items, int* __restrict__ ctl)
+{
+    const int n = *cur.count;
+    const int gmin = ctl[WIN_GMIN];
+    const int lane = threadIdx.x & 31;
+    for (int base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31; base < n; base += gridDim.x * blockDim.x) {
+        const int i = base + lane;
+        const int t = i < n ? cur.items[i] : -1;
+        const int m = i < n ? tmin[i] : MGC_HINF;
+        const bool act = t >= 0 && m < MGC_HINF;
+        const bool drop = t >= 0 && !act;
+        if (drop) pflag[t] = 0;
+        warp_append(now, act && m - gmin <= PUSH_WINDOW, t);
+        const unsigned bl = warp_append(later, act && m - gmin > PUSH_WINDOW, t);
+        warp_append(WorkList{drop_items, ctl + WIN_NDROP}, drop && cmat && cmat[t] == 0, t);
+        const unsigned bd = __ballot_sync(0xffffffffu, drop);
+        if (lane == 0) {
+            if (bl) atomicAdd(ctl + WIN_DEFERRED, __popc(bl));
+            if (bd) atomicAdd(ctl + WIN_DROPPED, __popc(bd));
+        }
+    }
+}
+
+// exact count of active voxels, scanning only the tiles of the worklists (a superset of the tiles that can hold one).
+// Both colours' lists in one launch, four tiles in flight per CTA iteration (the loop is latency-bound with one tile
+// per iteration), one atomic per warp at the end.  A listed tile that is not materialised (a window deferred it)
+// counts its implicit source excess.
+template <typename T>
+__global__ void __launch_bounds__(TILE_VOX) k_count_active_tiles2(Lattice L, Tiles TL, State<T> S, const int* __restrict__ cmat,
+                                                                  LazyTin tin, WorkList wa, WorkList wb,
+                                                                  unsigned long long* __restrict__ count)
+{
+    const int na = *(volatile int*)wa.count, nb = *(volatile int*)wb.count;
+    const int n = na + nb;
+    unsigned mine = 0;
+    for (int i0 = blockIdx.x * 4; i0 < n; i0 += gridDim.x * 4) {
+        T e[4];
+        int h[4], t[4];
+        bool own[4], lazy[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int i = i0 + j;
+            own[j] = false; lazy[j] = false; e[j] = 0; h[j] = MGC_HINF; t[j] = -1;
+            if (i < n) {
+                t[j] = i < na ? wa.items[i] : wb.items[i - na];
+                const TileCtx c = tile_ctx(L, TL, t[j]);
+                own[j] = c.own;
+                lazy[j] = cmat && cmat[t[j]] == 0;
+                if (c.own) { h[j] = S.height[c.v]; if (!lazy[j]) e[j] = S.excess[c.v]; }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (own[j] && lazy[j] && h[j] < MGC_HINF) e[j] = lazy_has_excess(L, tin, tile_ctx(L, TL, t[j])) ? (T)1 : (T)0;
+            mine += (own[j] && e[j] > 0 && h[j] < MGC_HINF) ? 1u : 0u;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_down_sync(0xffffffffu, mine, o);
+    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(count, (unsigned long long)mine);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -307,6 +307,7 @@ public:
         d["flow_const"] = s.flow_const; d["energy"] = s.energy; d["device_bytes"] = s.device_bytes;
         d["tiles_materialised"] = s.tiles_materialised; d["ms_caps"] = s.ms_caps;
         d["seed_folds"] = s.seed_folds; d["ms_seeds"] = s.ms_seeds; d["ms_seeds_host"] = s.ms_seeds_host;
+        d["tiles_deferred"] = s.tiles_deferred; d["tiles_dropped"] = s.tiles_dropped;
         return d;
     }
     // ---- z-slab stepping (device pointers as integers, e.g. torch.Tensor.data_ptr()) ----

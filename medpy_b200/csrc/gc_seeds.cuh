@@ -135,7 +135,7 @@ k_seed_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParam
 
 // push lists after a fold: every materialised tile (cmat[t] = 1) holding an owned voxel with excess goes on the list its
 // colour consumes next.  Excess stranded at voxels the last solve labelled HINF may reach a new sink link now; only
-// materialised tiles can hold excess (a solve materialises every tile the build listed before it pushes or stops).
+// materialised tiles can hold excess (mgc_add_seeds first materialises every tile whose source excess is still implicit).
 __global__ void __launch_bounds__(TILE_VOX) k_seed_lists(Lattice L, Tiles TL, State<double> S, const int* __restrict__ cmat,
                                                          int* __restrict__ pflag, WorkList pl0, WorkList pl1)
 {

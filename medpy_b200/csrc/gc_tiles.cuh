@@ -496,38 +496,6 @@ __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, 
     }
 }
 
-// exact count of active voxels, scanning only the tiles of the worklists (a superset of the tiles that can hold one).
-// Both colours' lists in one launch, four tiles in flight per CTA iteration (the loop is latency-bound with one tile
-// per iteration), one atomic per warp at the end.
-template <typename T>
-__device__ __forceinline__ void count_active_body2(const Lattice& L, const Tiles& TL, const State<T>& S, const WorkList& wa,
-                                                   const WorkList& wb, unsigned long long* __restrict__ count)
-{
-    const int na = *(volatile int*)wa.count, nb = *(volatile int*)wb.count;
-    const int n = na + nb;
-    unsigned mine = 0;
-    for (int i0 = blockIdx.x * 4; i0 < n; i0 += gridDim.x * 4) {
-        T e[4];
-        int h[4];
-        bool own[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int i = i0 + j;
-            own[j] = false; e[j] = 0; h[j] = MGC_HINF;
-            if (i < n) {
-                const TileCtx c = tile_ctx(L, TL, i < na ? wa.items[i] : wb.items[i - na]);
-                own[j] = c.own;
-                if (c.own) { e[j] = S.excess[c.v]; h[j] = S.height[c.v]; }
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) mine += (own[j] && e[j] > 0 && h[j] < MGC_HINF) ? 1u : 0u;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mine += __shfl_down_sync(0xffffffffu, mine, o);
-    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(count, (unsigned long long)mine);
-}
-
 template <typename T>
 __device__ __forceinline__ void count_active_body(const Lattice& L, const Tiles& TL, const State<T>& S, const WorkList& wl,
                                                   unsigned long long* __restrict__ count)
@@ -546,13 +514,6 @@ __global__ void __launch_bounds__(TILE_VOX) k_count_active_tiles(Lattice L, Tile
                                                                  unsigned long long* __restrict__ count)
 {
     count_active_body<T>(L, TL, S, wl, count);
-}
-
-template <typename T>
-__global__ void __launch_bounds__(TILE_VOX) k_count_active_tiles2(Lattice L, Tiles TL, State<T> S, WorkList wa, WorkList wb,
-                                                                  unsigned long long* __restrict__ count)
-{
-    count_active_body2<T>(L, TL, S, wa, wb, count);
 }
 
 // ---------------------------------------------------------------------------------------------------
