@@ -101,6 +101,9 @@ typedef struct mgc_stats {
     double ms_seeds_host;       /* host ms of those calls before anything is enqueued: id copy, range check, grouping */
     int64_t tiles_deferred;     /* 3-D tile solver, easy instance: listed tiles the label window held back, summed over the push launches of each solve */
     int64_t tiles_dropped;      /* ... listed tiles that left the push lists without a visit (no active voxel at a finite label) */
+    int64_t relabel_passes;     /* tile solver: BFS passes (worklist generations) of all global relabels; relabel_sweeps counts launches */
+    double ms_relabel_first;    /* device ms of the first global relabel of each solve (3-D host-driven tile solver), summed */
+    int64_t relabel_passes_first; /* ... its BFS passes, summed */
 } mgc_stats;
 
 /* ---- lifetime ------------------------------------------------------------------------------------- */

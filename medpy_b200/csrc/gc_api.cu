@@ -222,6 +222,12 @@ struct mgc_graph {
     // directional line sweeps in front of the worklist BFS (gc_sweep.cuh): used when more than 1/sweep_frac of the
     // tiles are waiting for labels (hard instances: the sink is far from most of the lattice)
     bool skip_first_test = true;       // MEDPY_GC_FIRST_TEST=1 restores the stop test of the first round
+    // label cap of a relabel that no stop test reads (the first of an easy solve, DESIGN.md §4.3): its labels only feed
+    // the label window of round 1's push passes.  MEDPY_GC_FIRST_CAP=0 keeps it exact, =N caps it at N (N >= 2)
+    int first_cap = FIRST_RELABEL_CAP;
+    bool labels_capped = false;        // the last global relabel stopped at first_cap: HINF means "deeper than the cap"
+    int relp_last = 0;                 // BFS passes of the last relabel_tiles_run ...
+    bool relp_pending = false;         // ... still in the control block (cooperative BFS, not read back yet)
     int sweep_mode = -1;               // decided at the first relabel of a solve: 1 = hard instance (sweep at every relabel), 0 = worklist BFS only
     bool use_sweeps = true;
     int sweep_frac = 8;                // sweep when pending tiles > ntiles / sweep_frac
@@ -718,12 +724,13 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
     for (auto& ev : g->ev_terms) cudaEventCreate(&ev);
     if (const char* f0 = getenv("MEDPY_GC_DEBUG")) g->debug_checks = atoi(f0) != 0;
     if (const char* f3 = getenv("MEDPY_GC_FIRST_TEST")) g->skip_first_test = atoi(f3) == 0;
+    if (const char* f5 = getenv("MEDPY_GC_FIRST_CAP")) g->first_cap = atoi(f5) >= 2 ? atoi(f5) : 0;
     if (const char* f1 = getenv("MEDPY_GC_FUSE")) g->fuse_build = atoi(f1) != 0;
     if (const char* f4 = getenv("MEDPY_GC_LAZY_CAPS")) g->lazy_caps = atoi(f4) != 0;
     if (const char* f2 = getenv("MEDPY_GC_CHUNKS")) if (atoi(f2) > 0) g->build_chunks = atoi(f2);
     cudaEventCreateWithFlags(&g->ev_bad, cudaEventDisableTiming);
     for (auto& ev : g->ev_b) cudaEventCreate(&ev);
-    // [0] weight verdict, [2..3] active count.  From the pinned pool: cudaHostAlloc / cudaFreeHost per handle (one handle per
+    // [0] weight verdict, [2..3] active count, [4] BFS passes of the last cooperative relabel.  From the pinned pool: cudaHostAlloc / cudaFreeHost per handle (one handle per
     // graph_from_voxels call) are heavyweight driver calls that synchronise the device
     { void* hp = nullptr; g->h_bad = (mgc_host_alloc(64, &hp) == MGC_OK) ? (int*)hp : nullptr; }
     if (const char* s1 = getenv("MEDPY_GC_SWEEPS")) g->sweeps_per_round = atoi(s1) > 0 ? atoi(s1) : g->sweeps_per_round;
@@ -1110,9 +1117,13 @@ int relabel_sweep_round(mgc_graph* g, int* pending, bool with_check)
     return read_tcount(g, 0, pending);
 }
 
-int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true)
+// `first`: no stop test reads this relabel's labels (the first relabel of a solve, whose round skips the test).  On an
+// easy instance of the 3-D tile solver such a relabel stops at g->first_cap (DESIGN.md §4.3).
+int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true, bool first = false)
 {
     *any = 0;
+    g->relp_last = 0;
+    g->relp_pending = false;
     if (g->use_sweeps && g->use_tiles && g->TL.ntiles >= 64 && g->sweep_mode != 0) {
         int pending = 0;
         int rc = read_tcount(g, g->rl_cur, &pending);
@@ -1136,6 +1147,10 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true)
             }
         }
     }
+    // the sweep decision is made above; the cap needs an easy instance of the 3-D tile solver, where the label window runs
+    const bool capped = first && g->first_cap >= 2 && g->sweep_mode == 0 && g->nd == 3 && !g->slab && !g->use_coop;
+    int cap = capped ? g->first_cap : MGC_HINF;
+    g->labels_capped = capped;
     if (g->coop_bfs_grid > 0 && g->use_tiles) {
         // all passes in one cooperative launch; the list selector lives in the control block (device side), so the
         // host does not have to synchronise unless the caller wants to know whether anything moved
@@ -1145,7 +1160,7 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true)
             void* args4[] = {&g->L, &g->TL4, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount};
             CK(cudaLaunchCooperativeKernel((void*)k_bfs_coop4, dim3(g->coop_bfs_grid), dim3(T4_VOX), args4, 0, g->stream));
         } else {
-            void* args[] = {&g->L, &g->TL, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount};
+            void* args[] = {&g->L, &g->TL, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount, &cap};
             CK(cudaLaunchCooperativeKernel((void*)k_bfs_coop, dim3(g->coop_bfs_grid), dim3(TILE_VOX), args, 0, g->stream));
         }
         g->st.kernel_launches++;
@@ -1155,6 +1170,10 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true)
             CK(cudaMemcpyAsync(&relp, g->d_tcount + CTL_RELP, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
             CK(cudaStreamSynchronize(g->stream));
             if (relp != 0) *any = 1;
+            g->relp_last = relp;
+            g->st.relabel_passes += relp;
+        } else {
+            g->relp_pending = true;     // read back by relabel_passes_fetch / _collect
         }
         return MGC_OK;
     }
@@ -1173,13 +1192,38 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true)
                                                             cursor(g), rl(g, 1 - cur));
         else
         k_relabel_tile<<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S.rmask, g->S.height, g->rflag, rl(g, cur),
-                                                         cursor(g), rl(g, 1 - cur));
+                                                         cursor(g), rl(g, 1 - cur), cap);
         g->rl_cur = 1 - cur;
         g->st.kernel_launches++;
         g->st.relabel_sweeps++;
+        g->st.relabel_passes++;
+        g->relp_last++;
     }
     CK(cudaGetLastError());
     return MGC_OK;
+}
+
+// BFS passes of the last relabel_tiles_run.  The cooperative BFS leaves them in the control block: _fetch enqueues their copy
+// to pinned memory (after the relabel's timing event, so the adaptive schedule does not see the copy), _collect reads them
+// once the stream has passed it (`*enqueued`: a copy was enqueued and needs a stream synchronisation).
+int relabel_passes_fetch(mgc_graph* g, bool* enqueued)
+{
+    *enqueued = false;
+    if (!g->relp_pending) return MGC_OK;
+    if (!g->h_bad) { g->relp_pending = false; return MGC_OK; }       // no pinned slot: the count is not kept
+    CK(cudaMemcpyAsync(g->h_bad + 4, g->d_tcount + CTL_RELP, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
+    *enqueued = true;
+    return MGC_OK;
+}
+
+int relabel_passes_collect(mgc_graph* g)
+{
+    if (g->relp_pending) {
+        g->relp_last = ((volatile int*)g->h_bad)[4];
+        g->st.relabel_passes += g->relp_last;
+        g->relp_pending = false;
+    }
+    return g->relp_last;
 }
 
 // one colour: consume its current list; still-active tiles go to its alternate list, receivers of cross-face flow
@@ -1189,7 +1233,7 @@ const int* lazy_cmat(const mgc_graph* g) { return g->caps_lazy ? g->cmat : nullp
 
 // label window of an easy instance (DESIGN.md §4.3): of the colour's current list, the tiles whose lowest active label is
 // within PUSH_WINDOW of the list's lowest go to win_items; the other tiles with an active voxel move to the colour's next
-// list, the rest leave the lists.  Returns the list to push now.
+// list, the rest leave the lists -- or wait on the next list too while the labels are capped.  Returns the list to push now.
 int window_filter(mgc_graph* g, int color, int a, WorkList* now)
 {
     const WorkList cur = pl(g, color, a);
@@ -1198,7 +1242,7 @@ int window_filter(mgc_graph* g, int color, int a, WorkList* now)
     CK(cudaMemsetAsync(g->win_ctl + WIN_NOW, 0, sizeof(int), g->stream));
     k_window_min<double><<<g->n_ctas * 2, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, lazy_cmat(g), g->caps_tin, cur, g->win_tmin, g->win_ctl);
     k_window_split<<<g->n_ctas, 256, 0, g->stream>>>(cur, g->win_tmin, lazy_cmat(g), g->pflag, *now, pl(g, color, 1 - a),
-                                                     g->drop_items, g->win_ctl);
+                                                     g->drop_items, g->win_ctl, g->labels_capped ? 1 : 0);
     g->st.kernel_launches += 2;
     CK(cudaGetLastError());
     return MGC_OK;
@@ -1220,6 +1264,7 @@ int push_color(mgc_graph* g, int color)
         if (rc) return rc;
     }
     CK(cudaMemsetAsync(cursor(g), 0, sizeof(int), g->stream));
+    const int capped = g->labels_capped ? 1 : 0;
     if (g->nd == 4) {
         k_push_tile4<double><<<g->n_ctas, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->smask, g->iters_now, g->pflag, cur,
                                                                   cursor(g), pl(g, color, 1 - a), pl(g, 1 - color, oa));
@@ -1227,10 +1272,10 @@ int push_color(mgc_graph* g, int color)
         const size_t smem = 2 * TMA_STAGE_BYTES + 6 * TILE_VOX * sizeof(double) + 1024 * sizeof(int) + 64;
         k_push_tile_tma<double><<<g->n_ctas, TILE_VOX, smem, g->stream>>>(g->L, g->TL, g->S, g->maps, g->iters_now, g->pflag,
                                                                           cur, cursor(g), pl(g, color, 1 - a),
-                                                                          pl(g, 1 - color, oa));
+                                                                          pl(g, 1 - color, oa), capped);
     } else
     k_push_tile<double><<<g->n_ctas, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->iters_now, g->pflag, cur,
-                                                               cursor(g), pl(g, color, 1 - a), pl(g, 1 - color, oa));
+                                                               cursor(g), pl(g, color, 1 - a), pl(g, 1 - color, oa), capped);
     CK(cudaMemsetAsync(g->d_tcount + 2 + color * 2 + a, 0, sizeof(int), g->stream));   // consumed list is empty again
     g->pl_sel[color] = 1 - a;
     g->st.kernel_launches++;
@@ -1290,6 +1335,7 @@ int count_active_tiles(mgc_graph* g, int64_t* out)
 int solve_coop(mgc_graph* g, int flags, int passes, int64_t* active_out)
 {
     if (flags & (SOLVE_F_PUSH | SOLVE_F_LOOP)) g->flow_started = true;
+    g->labels_capped = false;
     { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the cooperative solve pushes wherever it likes
     int hdr[4] = {0, g->pl_sel[0], g->pl_sel[1], g->rl_cur};     // cursor, list selectors
     CK(cudaMemcpyAsync(g->d_tcount + CTL_CURSOR, hdr, sizeof(hdr), cudaMemcpyHostToDevice, g->stream));
@@ -1382,11 +1428,14 @@ int solve_tiles(mgc_graph* g)
             rc = relabel_tiles_begin(g);
             if (rc) return rc;
             int any = 0;
-            rc = relabel_tiles_run(g, &any, false);
+            rc = relabel_tiles_run(g, &any, false, rounds == 0 && g->skip_first_test);
             if (rc) return rc;
         }
         cudaEventRecord(g->ev[3], g->stream);
         g->st.global_relabels++;
+        bool relp_copy = false;
+        rc = relabel_passes_fetch(g, &relp_copy);
+        if (rc) return rc;
         const bool test = rounds > 0 || !g->skip_first_test;
         if (test) {
             rc = count_active_tiles_enqueue(g, g->d_count);
@@ -1394,7 +1443,7 @@ int solve_tiles(mgc_graph* g)
             CK(cudaMemcpyAsync(h_active, g->d_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, g->stream));
         }
         CK(cudaEventSynchronize(g->ev[3]));
-        if (test) CK(cudaStreamSynchronize(g->stream));
+        if (test || relp_copy) CK(cudaStreamSynchronize(g->stream));
         float ms = 0;
         const double caps_ms = caps_resolve(g);      // materialiser launches inside the push span: timed apart
         if (g->init_timed) {          // k_init_tile of the per-term path: its events are reused for the push spans below
@@ -1404,6 +1453,8 @@ int solve_tiles(mgc_graph* g)
         cudaEventElapsedTime(&ms, g->ev[2], g->ev[3]);
         const double t_rel = ms;
         g->st.ms_relabel += ms;
+        const int relp = relabel_passes_collect(g);
+        if (rounds == 0) { g->st.ms_relabel_first += ms; g->st.relabel_passes_first += relp; }
         double t_pass = 0.0;
         if (push_open) {
             cudaEventElapsedTime(&ms, g->ev[4], g->ev[5]);

@@ -682,12 +682,17 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
 //   k_window_min   : the lowest label over the active voxels of every listed tile, and the minimum gmin over the list;
 //   k_window_split : tiles whose lowest active label is <= gmin + PUSH_WINDOW go to the list pushed (and materialised)
 //                    now; the other tiles with an active voxel wait on the colour's next list (pflag stays set); tiles
-//                    without one leave the lists.  Every relabel of such a solve is exact, so a voxel it labelled HINF
-//                    never becomes active again; tiles that leave unmaterialised are kept for mgc_add_seeds.
+//                    without one leave the lists.  After an exact relabel a voxel it labelled HINF never becomes active
+//                    again; tiles that leave unmaterialised are kept for mgc_add_seeds.  After a relabel stopped at a
+//                    label cap (`labels_capped`, the first relabel of a solve) HINF only means "deeper than the cap": such
+//                    tiles wait on the next list too, and the next, exact, relabel labels them.
 // Both read a tile that is not materialised yet through its implicit push state (cmat[t] == 0; cmat == nullptr: every
 // tile is materialised).
 // ---------------------------------------------------------------------------------------------------
 #define PUSH_WINDOW 8
+// label cap of the first global relabel of an easy solve (no stop test reads it; only the window above uses its labels):
+// the BFS labels the voxels within FIRST_RELABEL_CAP of the sink and leaves the rest HINF (relabel_visit)
+#define FIRST_RELABEL_CAP 12
 #define WIN_GMIN 0         // control words: lowest active label of the list
 #define WIN_NOW 1          // ... count of the list pushed now
 #define WIN_DEFERRED 2     // ... tile deferrals since the solve started
@@ -735,7 +740,7 @@ __device__ __forceinline__ unsigned warp_append(const WorkList& wl, bool take, i
 
 __global__ void __launch_bounds__(256) k_window_split(WorkList cur, const int* __restrict__ tmin, const int* __restrict__ cmat,
                                                       int* __restrict__ pflag, WorkList now, WorkList later,
-                                                      int* __restrict__ drop_items, int* __restrict__ ctl)
+                                                      int* __restrict__ drop_items, int* __restrict__ ctl, int labels_capped)
 {
     const int n = *cur.count;
     const int gmin = ctl[WIN_GMIN];
@@ -745,10 +750,10 @@ __global__ void __launch_bounds__(256) k_window_split(WorkList cur, const int* _
         const int t = i < n ? cur.items[i] : -1;
         const int m = i < n ? tmin[i] : MGC_HINF;
         const bool act = t >= 0 && m < MGC_HINF;
-        const bool drop = t >= 0 && !act;
+        const bool drop = t >= 0 && !act && !labels_capped;
         if (drop) pflag[t] = 0;
         warp_append(now, act && m - gmin <= PUSH_WINDOW, t);
-        const unsigned bl = warp_append(later, act && m - gmin > PUSH_WINDOW, t);
+        const unsigned bl = warp_append(later, t >= 0 && !drop && !(act && m - gmin <= PUSH_WINDOW), t);
         warp_append(WorkList{drop_items, ctl + WIN_NDROP}, drop && cmat && cmat[t] == 0, t);
         const unsigned bd = __ballot_sync(0xffffffffu, drop);
         if (lane == 0) {

@@ -83,7 +83,7 @@ k_solve_coop(Lattice L, Tiles TL, State<T> S, SolveLists SL, int* __restrict__ r
                 for (;;) {
                     const int t = fetch_tile(cur, ctl + CTL_CURSOR, &s_slot);
                     if (t < 0) break;
-                    relabel_visit(L, TL, S.rmask, S.height, rflag, nxt, t, s_h);
+                    relabel_visit(L, TL, S.rmask, S.height, rflag, nxt, t, s_h, MGC_HINF);
                 }
                 grid.sync();
                 if (leader) { ctl[rl_cur] = 0; ctl[CTL_CURSOR] = 0; }
@@ -140,7 +140,8 @@ k_solve_coop(Lattice L, Tiles TL, State<T> S, SolveLists SL, int* __restrict__ r
 }
 
 // ---------------------------------------------------------------------------------------------------
-// global relabel alone as one cooperative launch: all passes of the BFS with grid-wide barriers between them.
+// global relabel alone as one cooperative launch: all passes of the BFS with grid-wide barriers between them
+// (`cap`: see relabel_visit; MGC_HINF = exact).
 // The relabel visit needs 28 registers and 4 KB of shared memory, so 4 CTAs per SM are co-resident -- twice the
 // parallelism k_solve_coop can offer (it is bounded by the push visit) -- while the per-pass host round trip
 // (count read-back, two memsets, launch) of the list-driven host loop disappears.
@@ -149,7 +150,7 @@ k_solve_coop(Lattice L, Tiles TL, State<T> S, SolveLists SL, int* __restrict__ r
 // ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(TILE_VOX, 4)
 k_bfs_coop(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask, int* __restrict__ height, int* __restrict__ rflag,
-           int* __restrict__ items0, int* __restrict__ items1, int* __restrict__ ctl)
+           int* __restrict__ items0, int* __restrict__ items1, int* __restrict__ ctl, int cap)
 {
     __shared__ int sh[HALO_VOX];
     __shared__ int s_slot;
@@ -164,7 +165,7 @@ k_bfs_coop(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask, int* __restri
         for (;;) {
             const int t = fetch_tile(cur, ctl + CTL_CURSOR, &s_slot);
             if (t < 0) break;
-            relabel_visit(L, TL, rmask, height, rflag, nxt, t, sh);
+            relabel_visit(L, TL, rmask, height, rflag, nxt, t, sh, cap);
         }
         grid.sync();
         if (leader) { ctl[rl_cur] = 0; ctl[CTL_CURSOR] = 0; }

@@ -308,6 +308,8 @@ public:
         d["tiles_materialised"] = s.tiles_materialised; d["ms_caps"] = s.ms_caps;
         d["seed_folds"] = s.seed_folds; d["ms_seeds"] = s.ms_seeds; d["ms_seeds_host"] = s.ms_seeds_host;
         d["tiles_deferred"] = s.tiles_deferred; d["tiles_dropped"] = s.tiles_dropped;
+        d["relabel_passes"] = s.relabel_passes; d["ms_relabel_first"] = s.ms_relabel_first;
+        d["relabel_passes_first"] = s.relabel_passes_first;
         return d;
     }
     // ---- z-slab stepping (device pointers as integers, e.g. torch.Tensor.data_ptr()) ----

@@ -270,9 +270,12 @@ __global__ void __launch_bounds__(TILE_VOX) k_relabel_reset_list(Lattice L, Tile
 // ---------------------------------------------------------------------------------------------------
 // one tile visit of the global relabel: relax inside the tile until nothing changes, write back, list the face
 // neighbours whose halo changed.  `sh` = HALO_VOX ints of shared memory.
+// `cap`: no voxel is lowered to a label above it (it keeps HINF), and no neighbour is woken by a label that could only
+// lower it above the cap.  Labels strictly decrease along a shortest residual path to the sink, so every voxel whose
+// distance is <= cap still gets its exact distance; cap = MGC_HINF is the exact BFS.
 __device__ __forceinline__ void relabel_visit(const Lattice& L, const Tiles& TL, const uint8_t* __restrict__ rmask,
                                               int* __restrict__ height, int* __restrict__ rflag, const WorkList& next,
-                                              int t, int* sh)
+                                              int t, int* sh, int cap)
 {
     const TileCtx c = tile_ctx(L, TL, t);
     if (threadIdx.x == 0) rflag[t] = 0;        // may be listed again by a neighbour from now on
@@ -291,7 +294,7 @@ __device__ __forceinline__ void relabel_visit(const Lattice& L, const Tiles& TL,
             if (m & 8u)  { const int hw = sh[me + hoff<3>()] + 1; best = hw < best ? hw : best; }
             if (m & 16u) { const int hw = sh[me + hoff<4>()] + 1; best = hw < best ? hw : best; }
             if (m & 32u) { const int hw = sh[me + hoff<5>()] + 1; best = hw < best ? hw : best; }
-            if (best < h) { h = best; sh[me] = h; changed = 1; }
+            if (best < h && best <= cap) { h = best; sh[me] = h; changed = 1; }
         }
         if (!__syncthreads_or(changed)) break;
     }
@@ -300,12 +303,15 @@ __device__ __forceinline__ void relabel_visit(const Lattice& L, const Tiles& TL,
         // wake a face neighbour only if my new label can actually lower the voxel across the face: its label (from the
         // halo, and labels only ever decrease during a BFS) must exceed mine + 1.  Without this test every tile was
         // re-listed by each neighbour that settled after it -- most visits of a hard instance changed nothing.
-        if (c.lz == 0 && c.tz > 0 && sh[me + hoff<0>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 0));
-        if (c.lz == TILE - 1 && c.tz + 1 < TL.nt[0] && sh[me + hoff<1>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 1));
-        if (c.ly == 0 && c.ty > 0 && sh[me + hoff<2>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 2));
-        if (c.ly == TILE - 1 && c.ty + 1 < TL.nt[1] && sh[me + hoff<3>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 3));
-        if (c.lx == 0 && c.tx > 0 && sh[me + hoff<4>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 4));
-        if (c.lx == TILE - 1 && c.tx + 1 < TL.nt[2] && sh[me + hoff<5>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 5));
+        // A label at the cap wakes nobody: it could only lower a neighbour above the cap.
+        if (h < cap) {
+            if (c.lz == 0 && c.tz > 0 && sh[me + hoff<0>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 0));
+            if (c.lz == TILE - 1 && c.tz + 1 < TL.nt[0] && sh[me + hoff<1>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 1));
+            if (c.ly == 0 && c.ty > 0 && sh[me + hoff<2>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 2));
+            if (c.ly == TILE - 1 && c.ty + 1 < TL.nt[1] && sh[me + hoff<3>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 3));
+            if (c.lx == 0 && c.tx > 0 && sh[me + hoff<4>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 4));
+            if (c.lx == TILE - 1 && c.tx + 1 < TL.nt[2] && sh[me + hoff<5>()] > h + 1) list_push(rflag, next, tile_nbr(TL, t, 5));
+        }
     }
     if (TL.dflag) {                          // labels of this tile changed: it has to be reset before the next BFS
         const int chg = __syncthreads_or(h != h0 ? 1 : 0);
@@ -315,14 +321,14 @@ __device__ __forceinline__ void relabel_visit(const Lattice& L, const Tiles& TL,
 
 __global__ void __launch_bounds__(TILE_VOX) k_relabel_tile(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask,
                                                            int* __restrict__ height, int* __restrict__ rflag,
-                                                           WorkList cur, int* __restrict__ cursor, WorkList next)
+                                                           WorkList cur, int* __restrict__ cursor, WorkList next, int cap)
 {
     __shared__ int sh[HALO_VOX];
     __shared__ int s_slot;
     for (;;) {
         const int t = fetch_tile(cur, cursor, &s_slot);
         if (t < 0) break;
-        relabel_visit(L, TL, rmask, height, rflag, next, t, sh);
+        relabel_visit(L, TL, rmask, height, rflag, next, t, sh, cap);
     }
 }
 
@@ -384,10 +390,12 @@ __device__ __forceinline__ void pull_dir(const TileCtx& c, const T* s_out, T& e,
 // one push/relabel discharge visit of tile t.  s_out = 6*TILE_VOX values, s_h = HALO_VOX ints of shared memory.
 // `stg` (optional): the tile's six capacity planes + excess already staged in shared memory by TMA (gc_tma.cuh),
 // plane p at stg + p * TILE_VOX, voxel order == thread order; nullptr = load from global memory here.
+// `labels_capped`: the last global relabel stopped at a label cap, so a voxel at HINF may still reach the sink; a tile
+// that keeps excess at such a voxel stays listed for the next (exact) relabel instead of leaving the lists.
 template <typename T>
 __device__ __forceinline__ void push_visit_staged(const Lattice& L, const Tiles& TL, const State<T>& S, int iters,
                                                   int* __restrict__ pflag, const WorkList& self_next, const WorkList& other_next,
-                                                  int t, T* s_out, int* s_h, const double* stg)
+                                                  int t, T* s_out, int* s_h, const double* stg, bool labels_capped = false)
 {
     const TileCtx c = tile_ctx(L, TL, t);
     const int tid = threadIdx.x;
@@ -465,7 +473,7 @@ __device__ __forceinline__ void push_visit_staged(const Lattice& L, const Tiles&
                      (c4 > 0 ? 16u : 0u) | (c5 > 0 ? 32u : 0u) | ((scap - sf > 0) ? RM_SINK : 0u) | sinkv;
         S.rmask[c.v] = (uint8_t)m;
     }
-    const int still = (c.own && e > 0 && h < MGC_HINF) ? 1 : 0;
+    const int still = (c.own && e > 0 && (h < MGC_HINF || labels_capped)) ? 1 : 0;
     if (__syncthreads_or(still) && tid == 0) list_push(pflag, self_next, t);
     if (TL.dflag) {                          // a label or a sink-link residual bit of this tile changed
         const int chg = __syncthreads_or((c.inb && (h != h0 || (dirty & 128u))) ? 1 : 0);
@@ -484,7 +492,7 @@ __device__ __forceinline__ void push_visit(const Lattice& L, const Tiles& TL, co
 template <typename T>
 __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, State<T> S, int iters,
                                                            int* __restrict__ pflag, WorkList cur, int* __restrict__ cursor,
-                                                           WorkList self_next, WorkList other_next)
+                                                           WorkList self_next, WorkList other_next, int labels_capped)
 {
     __shared__ T s_out[6 * TILE_VOX];
     __shared__ int s_h[HALO_VOX];
@@ -492,7 +500,7 @@ __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, 
     for (;;) {
         const int t = fetch_tile(cur, cursor, &s_slot);
         if (t < 0) break;
-        push_visit<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h);
+        push_visit_staged<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h, nullptr, labels_capped != 0);
     }
 }
 

@@ -64,7 +64,7 @@ __device__ __forceinline__ void tma_issue_tile(const PushMaps& maps, const Tiles
 template <typename T>
 __global__ void __launch_bounds__(TILE_VOX, 2)
 k_push_tile_tma(Lattice L, Tiles TL, State<T> S, const __grid_constant__ PushMaps maps, int iters, int* __restrict__ pflag,
-                WorkList cur, int* __restrict__ cursor, WorkList self_next, WorkList other_next)
+                WorkList cur, int* __restrict__ cursor, WorkList self_next, WorkList other_next, int labels_capped)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     double* stage0 = reinterpret_cast<double*>(smem);
@@ -103,7 +103,7 @@ k_push_tile_tma(Lattice L, Tiles TL, State<T> S, const __grid_constant__ PushMap
         mbar_wait(&bars[buf], phase[buf]);
         phase[buf] ^= 1u;
         const double* stg = buf ? stage1 : stage0;
-        push_visit_staged<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h, stg);
+        push_visit_staged<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h, stg, labels_capped != 0);
         __syncthreads();                 // stage `buf` and s_out/s_h are free again; s_next[1] is visible
         t = s_next[1];
         buf ^= 1;
