@@ -164,7 +164,7 @@ def _polyline(points):
     """Voxel coordinates along the polyline, in order."""
     line = []
     for a, b in zip(points[:-1], points[1:]):
-        axis = next(d for d in range(3) if a[d] != b[d])
+        axis = next(d for d in range(len(a)) if a[d] != b[d])
         step = 1 if b[axis] > a[axis] else -1
         for c in range(a[axis], b[axis], step):
             q = list(a)
@@ -371,9 +371,9 @@ def cut_capacity(prob, mask):
     s = numpy.asarray(mask).reshape(shape).astype(bool)
     tr = numpy.asarray(prob["tr"]).reshape(shape)
     terms = [numpy.array([prob["flow_const"]]), tr[~s & (tr > 0)], -tr[s & (tr < 0)]]
-    for d in range(3):
-        lo = [slice(None)] * 3
-        hi = [slice(None)] * 3
+    for d in range(len(shape)):
+        lo = [slice(None)] * len(shape)
+        hi = [slice(None)] * len(shape)
         lo[d], hi[d] = slice(0, -1), slice(1, None)
         lo, hi = tuple(lo), tuple(hi)
         wf = numpy.asarray(prob["wf"][d]).reshape(shape)[lo]

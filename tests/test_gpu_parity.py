@@ -91,6 +91,63 @@ def _oracle_solve(prob):
     return solvers.solve_port(prob)
 
 
+def test_recorded_fuzz_cases_vs_reference():
+    """The 120 cases tests/golden/fuzz_voxels_v1.json recorded from the unmodified reference (1-D..4-D, the eight
+    boundary terms, five image dtypes, spacing, regional term, overlapping markers), regenerated from the recorded seed
+    and solved through graph_from_voxels: the same cases raise ValueError; t-links equal the restatement's bit for bit
+    (which test_oracle pins to the reference), n-link weights within the golden tolerances; flow and mask equal the
+    reference's, a mask only up to an exact tie.  (The recorded set has no refused and no NaN-weight case; the branches
+    for them keep the test right if it is re-recorded with another seed or size.)"""
+    import json
+    import sys
+    import warnings
+    from oracle import energy_terms as et
+    from test_gpu_fullsize import _cut_difference_exact
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+    import fuzz_voxels_against_reference as fuzz
+    with open(fuzz.GOLDEN) as fh:
+        z = json.load(fh)
+    rng = numpy.random.default_rng(z["seed"])
+    solved = refused = nan_weights = 0
+    for i, rec in enumerate(z["records"]):
+        c = fuzz.random_case(rng)
+        c.setdefault("prob", None)
+        shape = c["fg"].shape
+        with warnings.catch_warnings(), numpy.errstate(all="ignore"):
+            warnings.simplefilter("ignore")
+            if rec.get("error"):
+                with pytest.raises(ValueError):
+                    _build_graph(c).maxflow()
+                refused += 1
+                continue
+            prob = et.build_problem(c["fg"], c["bg"], regional=(c["prob"], c["alpha"]) if c["prob"] is not None else None,
+                                    boundary=(c["boundary"], c["image"], c["sigma"], c["spacing"]))
+            g = _build_graph(c)
+        n = int(numpy.prod(shape))
+        tr = numpy.asarray([g.get_trcap(p) for p in range(n)])
+        assert numpy.array_equal(tr, prob["tr"]), (i, c["boundary"])
+        w, wr = _all_edges(g, shape)
+        want = numpy.stack([numpy.asarray(x, dtype=numpy.float64) for x in prob["wf"]])
+        if c["boundary"].split("_")[1] in ("linear", "division"):
+            assert numpy.array_equal(w, want, equal_nan=True), (i, c["boundary"])
+        else:
+            numpy.testing.assert_allclose(w, want, rtol=2e-13, atol=0, err_msg="case %d %s" % (i, c["boundary"]))
+        assert numpy.array_equal(w, wr, equal_nan=True), i
+        if numpy.isnan(want).any():
+            nan_weights += 1    # as check() does: the reference only has to not raise
+            continue
+        flow = g.maxflow()
+        mask = g.get_mask().ravel()
+        rflow = float.fromhex(rec["flow"])
+        rmask = numpy.frombuffer(rec["mask"].encode(), numpy.uint8) - ord("0")
+        assert abs(flow - rflow) <= 1e-9 * max(1.0, abs(rflow)), (i, c["boundary"], flow, rflow)
+        if not numpy.array_equal(mask, rmask):
+            diff = _cut_difference_exact(prob, mask, rmask)
+            assert abs(diff) <= 0.5 * numpy.spacing(abs(rflow)), (i, c["boundary"], "mask differs by more than a tie", diff)
+        solved += 1
+    assert solved + refused + nan_weights == len(z["records"]) and solved > 100, (solved, refused, nan_weights)
+
+
 @pytest.mark.parametrize("shape,seed", [((32, 32, 32), 0), ((40, 24, 56), 1), ((20, 48, 33), 2)])
 def test_config3_regional_plus_exponential_vs_oracle(shape, seed):
     """BASELINE config 3 at oracle-sized volumes: regional_probability_map + boundary_difference_exponential."""
@@ -410,7 +467,10 @@ def _two_slabs_one_gpu(vol, regional, split):
     return energy, mask
 
 
-@pytest.mark.parametrize("shape,split,regional", [((40, 32, 32), 20, True), ((40, 32, 32), 13, False), ((37, 24, 40), 9, True)])
+@pytest.mark.parametrize("shape,split,regional", [((40, 32, 32), 20, True), ((40, 32, 32), 13, False), ((37, 24, 40), 9, True),
+                                                  # 4-D slabs (per-voxel solver): ragged, one-plane and even splits
+                                                  ((20, 12, 16, 9), 7, True), ((17, 10, 8, 33), 1, False),
+                                                  ((16, 8, 8, 4), 8, True)])
 def test_two_slabs_on_one_gpu_vs_oracle(shape, split, regional):
     from medpy_b200 import synthetic
     from oracle import energy_terms as et

@@ -134,7 +134,11 @@ def test_fused_build_reports_non_positive_weights():
                              boundary_term_args=(img, 0.5, (-1.0, 1.0, 1.0)))
 
 
-@pytest.mark.parametrize("shape,regional", [((64, 64, 64), False), ((40, 72, 56), False), ((48, 48, 48), True)])
+@pytest.mark.parametrize("shape,regional", [((64, 64, 64), False), ((40, 72, 56), False), ((48, 48, 48), True),
+                                            ((48, 40, 20), False),      # rows of <= 32 voxels: one thread per row
+                                            ((40, 40, 33), False),      # one warp per row from 33 voxels
+                                            ((16, 16, 1024), False),    # the longest one-segment row
+                                            ((12, 8, 1100), False)])    # two segments with a carry
 def test_sweep_relabel_equals_worklist_relabel_and_oracle(shape, regional):
     """Directional sweeps in front of the worklist BFS (forced on for every relabel) vs the worklist BFS alone vs BK."""
     from medpy_b200 import synthetic

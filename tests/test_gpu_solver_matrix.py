@@ -52,19 +52,21 @@ def _get(name):
 
 
 def _build(case):
+    """The case's graph through graph_from_voxels (fused; difference_exponential unless the case names another boundary
+    term) or the dense per-term calls, in as many dimensions as the case has."""
     import medpy_b200.graphcut as gc
     if case["kind"] == "fused":
         vol = case["vol"]
-        kw = dict(boundary_term=gc.energy_voxel.boundary_difference_exponential,
+        kw = dict(boundary_term=getattr(gc.energy_voxel, "boundary_" + case.get("boundary", "difference_exponential")),
                   boundary_term_args=(vol["image"], vol["sigma"], False))
         if vol.get("prob") is not None:
             kw.update(regional_term=gc.energy_voxel.regional_probability_map, regional_term_args=(vol["prob"], vol["alpha"]))
         return gc.graph_from_voxels(vol["fg"], vol["bg"], **kw)
     shape = tuple(case["prob"]["shape"])
     n = int(numpy.prod(shape))
-    graph = gc.GCGraph(n, 3 * n, shape=shape)
+    graph = gc.GCGraph(n, len(shape) * n, shape=shape)
     graph.set_tweights_dense(case["src"], case["snk"])
-    for d in range(3):
+    for d in range(len(shape)):
         graph.set_nweights_dense(d, case["there"][d], case["back"][d])
     return graph.get_graph()
 
