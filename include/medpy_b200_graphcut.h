@@ -96,9 +96,11 @@ typedef struct mgc_stats {
     double ms_init;             /* device ms of the solver-state initialisation kernel (k_init_tile); 0 after a fused build */
     int64_t tiles_materialised; /* lazy build: 8^3 tiles whose capacities, tr and excess k_caps_tiles computed (0 eager) */
     double ms_caps;             /* device ms of the materialiser launches (k_caps_claim + k_caps_tiles; not in ms_push)  */
-    int64_t seed_folds;         /* mgc_add_seeds calls folded into this handle since its build (reset by the build)   */
-    double ms_seeds;            /* device ms of those calls: tile claim + materialisation, fold, push-list fix-up     */
-    double ms_seeds_host;       /* host ms of those calls before anything is enqueued: id copy, range check, grouping */
+    int64_t seed_folds;         /* mgc_add_seeds and mgc_remove_seeds calls folded into this handle since its build   */
+                                /* (reset by the build; erase calls count like add calls in all three fields)         */
+    double ms_seeds;            /* device ms of those calls: id upload, grouping (sort, run-length), tile claim +      */
+                                /* materialisation, fold, push-list fix-up; not the one read-back of the item count    */
+    double ms_seeds_host;       /* host ms of those calls before anything is enqueued: scratch growth, launch count   */
     int64_t tiles_deferred;     /* 3-D tile solver, easy instance: listed tiles the label window held back, summed over the push launches of each solve */
     int64_t tiles_dropped;      /* ... listed tiles that left the push lists without a visit (no active voxel at a finite label) */
     int64_t relabel_passes;     /* tile solver: BFS passes (worklist generations) of all global relabels; relabel_sweeps counts launches */
@@ -231,6 +233,15 @@ int mgc_maxflow(mgc_graph* g, double* energy);
  * mgc_add_tweights_dense / mgc_add_markers and the other term entry points still refuse a solved graph.  Adding this
  * entry point left MGC_ABI_VERSION at 3: nothing that existed changed. */
 int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
+/* Seeds erased from a graph and solved warm: the inverse call of mgc_add_seeds, as the reference erases a seed
+ * (add_tweights accepts negative capacities, graph.h:415-425).  The meaning is exactly add_tweights(v, -65535, 0) for
+ * every id of fg_ids in list order, THEN add_tweights(v, 0, -65535) for every id of bg_ids; duplicate ids count once per
+ * occurrence.  The call does not check that a seed was ever added: erasing a seed that is not there applies the call
+ * anyway, as the reference does, and leaves the graph with that t-link lowered by 65535.  The markers of
+ * mgc_build_voxel_graph are the same add_tweights calls, so this also erases them.  Same arguments, preconditions and
+ * errors as mgc_add_seeds (MGC_E_ARG for an id out of range, with the handle unchanged; MGC_E_STATE unless the last build
+ * was the lazy fused build), solved or not.  Adding this entry point left MGC_ABI_VERSION at 3. */
+int mgc_remove_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
 /* Bulk form of the what_segment loop (bin/medpy_graphcut_voxel.py:177-181): out[v] = 0 if the voxel is in
  * the SINK set else 1, C-order over the logical shape.  `mem` selects host or device destination. */
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem);

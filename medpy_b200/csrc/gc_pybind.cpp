@@ -218,9 +218,12 @@ public:
         { py::gil_scoped_release rel; rc = mgc_add_nweights_dense(g_, axis, &a.a, &b.a); }
         check(rc, g_);
     }
-    // seeds folded into the solved graph (mgc_add_seeds): 1-D int64 node-id arrays, both on the host (numpy) or both on
-    // the device (__cuda_array_interface__); None = no seeds of that kind
-    void add_seeds(const py::object& fg, const py::object& bg)
+    // seeds folded into the solved graph (mgc_add_seeds / mgc_remove_seeds): 1-D int64 node-id arrays, both on the host
+    // (numpy) or both on the device (__cuda_array_interface__); None = no seeds of that kind
+    void add_seeds(const py::object& fg, const py::object& bg) { fold_seeds(fg, bg, mgc_add_seeds); }
+    void remove_seeds(const py::object& fg, const py::object& bg) { fold_seeds(fg, bg, mgc_remove_seeds); }
+    void fold_seeds(const py::object& fg, const py::object& bg,
+                    int (*fold)(mgc_graph*, const int64_t*, int64_t, const int64_t*, int64_t, int32_t))
     {
         struct Ids { const int64_t* p = nullptr; int64_t n = 0; int mem = -1; py::object keep; };
         auto ids = [](const py::object& o, const char* what) {
@@ -253,7 +256,7 @@ public:
         if (f.n && b.n && f.mem != b.mem) throw py::value_error("fg_ids and bg_ids must both be host or both be device arrays");
         const int mem = f.n ? f.mem : (b.n ? b.mem : MGC_MEM_HOST);
         int rc;
-        { py::gil_scoped_release rel; rc = mgc_add_seeds(g_, f.n ? f.p : nullptr, f.n, b.n ? b.p : nullptr, b.n, mem); }
+        { py::gil_scoped_release rel; rc = fold(g_, f.n ? f.p : nullptr, f.n, b.n ? b.p : nullptr, b.n, mem); }
         check(rc, g_);
     }
     double maxflow()
@@ -637,6 +640,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("add_boundary", &PyGraph::add_boundary)
         .def("add_nweights_dense", &PyGraph::add_nweights_dense)
         .def("add_seeds", &PyGraph::add_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
+        .def("remove_seeds", &PyGraph::remove_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
         .def("build_voxel_graph", &PyGraph::build_voxel_graph)
         .def_static("slab_comm_unique_id", &PyGraph::slab_comm_unique_id)
         .def("slab_comm_init", &PyGraph::slab_comm_init)

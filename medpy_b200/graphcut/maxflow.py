@@ -431,9 +431,26 @@ class GraphDouble:
         ``graph_from_voxels`` built in one fused pass (1-D..3-D lattice on one GPU), the seeds are folded into the solved
         state and the next solve continues from the flow already routed (mgc_add_seeds).  Any other solved graph raises
         ``RuntimeError``: ``reset()`` it and build the graph again with the seeds."""
+        self._fold_seeds(fg, bg, 65535.0, "add_seeds", "with")
+
+    def remove_seeds(self, fg=None, bg=None):
+        """Erase foreground / background seeds and let the next ``maxflow()`` return the cut of the reduced graph.
+
+        The inverse of ``add_seeds``, as the reference erases a seed: exactly ``add_tweights(v, -65535, 0)`` for every
+        foreground id in order, then ``add_tweights(v, 0, -65535)`` for every background id.  ``fg`` / ``bg`` take the
+        same forms as in ``add_seeds``; repeated ids count once per occurrence.  The markers ``graph_from_voxels`` put
+        into the graph are the same ``add_tweights`` calls, so this erases them as well as seeds added later.  Nothing
+        checks that a seed was there: erasing one that was never added applies the call anyway, as the reference does.
+
+        Before the first ``maxflow()`` the calls are staged like ``add_tweights``.  After it the seeds are folded into
+        the solved state on the same graphs as ``add_seeds`` (mgc_remove_seeds); any other solved graph raises
+        ``RuntimeError``: ``reset()`` it and build the graph again without the seeds."""
+        self._fold_seeds(fg, bg, -65535.0, "remove_seeds", "without")
+
+    def _fold_seeds(self, fg, bg, cap, native, rebuild):
         fg_ids, bg_ids = self._seed_ids(fg), self._seed_ids(bg)
         if not self._solved:
-            for ids, src, snk in ((fg_ids, 65535.0, 0.0), (bg_ids, 0.0, 65535.0)):
+            for ids, src, snk in ((fg_ids, cap, 0.0), (bg_ids, 0.0, cap)):
                 if ids is not None and len(ids):
                     if not isinstance(ids, numpy.ndarray):
                         ids = ids.cpu().numpy()
@@ -441,9 +458,9 @@ class GraphDouble:
             return
         if self._sp is not None:
             raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it with the seeds instead")
+                               "rebuild it {} the seeds instead".format(rebuild))
         self._dirty()
-        self._nat().add_seeds(fg_ids, bg_ids)
+        getattr(self._nat(), native)(fg_ids, bg_ids)
 
     def get_mask(self):
         """Bulk read-out: uint8 array of the lattice shape, 0 where what_segment == SINK else 1
