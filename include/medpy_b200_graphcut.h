@@ -96,10 +96,12 @@ typedef struct mgc_stats {
     double ms_init;             /* device ms of the solver-state initialisation kernel (k_init_tile); 0 after a fused build */
     int64_t tiles_materialised; /* lazy build: 8^3 tiles whose capacities, tr and excess k_caps_tiles computed (0 eager) */
     double ms_caps;             /* device ms of the materialiser launches (k_caps_claim + k_caps_tiles; not in ms_push)  */
-    int64_t seed_folds;         /* mgc_add_seeds and mgc_remove_seeds calls folded into this handle since its build   */
-                                /* (reset by the build; erase calls count like add calls in all three fields)         */
-    double ms_seeds;            /* device ms of those calls: id upload, grouping (sort, run-length), tile claim +      */
-                                /* materialisation, fold, push-list fix-up; not the one read-back of the item count    */
+    int64_t seed_folds;         /* mgc_add_seeds, mgc_remove_seeds and mgc_add_tweights_warm calls folded into this   */
+                                /* handle since its build (reset by the build; erase and t-link calls count like add  */
+                                /* calls in all three fields; a call of only zero weights folds nothing, counts not)  */
+    double ms_seeds;            /* device ms of those calls: id / weight upload, grouping (sort or compaction,        */
+                                /* run-length), tile claim + materialisation, fold, push-list fix-up; not the one     */
+                                /* read-back of the item count                                                         */
     double ms_seeds_host;       /* host ms of those calls before anything is enqueued: scratch growth, launch count   */
     int64_t tiles_deferred;     /* 3-D tile solver, easy instance: listed tiles the label window held back, summed over the push launches of each solve */
     int64_t tiles_dropped;      /* ... listed tiles that left the push lists without a visit (no active voxel at a finite label) */
@@ -242,6 +244,20 @@ int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64
  * errors as mgc_add_seeds (MGC_E_ARG for an id out of range, with the handle unchanged; MGC_E_STATE unless the last build
  * was the lazy fused build), solved or not.  Adding this entry point left MGC_ABI_VERSION at 3. */
 int mgc_remove_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
+/* Any add_tweights calls folded into a graph and solved warm (soft strokes, a GrabCut-style re-estimation of the
+ * regional term, a change of the regional / boundary weight on a solved graph; graph.h:415-425: BK applies the call to
+ * the residual terminal capacity and the next maxflow() continues from the residual graph).
+ *   ids != NULL : the list form, add_tweights(ids[k], src[k], snk[k]) for k = 0 .. count-1 in array order; duplicate ids
+ *                 are applied in order, once per occurrence.
+ *   ids == NULL : the dense form, add_tweights(v, src[v], snk[v]) for every voxel in C order (set_tweights_all on a solved
+ *                 graph); count must be the voxel count.  add_tweights(v, 0, 0) changes nothing, so only the voxels with
+ *                 a nonzero weight are touched.
+ * src / snk are contiguous doubles of any sign, `count` of each; ids are C-order int64 node ids.  All three live in `mem`
+ * (host memory is borrowed for the call, device memory is read in place on the handle's stream).  count == 0 does
+ * nothing.  MGC_E_ARG, with the handle unchanged, for an id out of range, a NaN or infinite weight (the reference would
+ * carry it into BK) or bad counts and pointers.  Same preconditions, MGC_E_STATE message and behaviour on solved and
+ * unsolved handles as mgc_add_seeds.  Adding this entry point left MGC_ABI_VERSION at 3. */
+int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, const double* snk, int64_t count, int32_t mem);
 /* Bulk form of the what_segment loop (bin/medpy_graphcut_voxel.py:177-181): out[v] = 0 if the voxel is in
  * the SINK set else 1, C-order over the logical shape.  `mem` selects host or device destination. */
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem);

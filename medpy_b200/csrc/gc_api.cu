@@ -26,6 +26,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -167,9 +168,9 @@ struct mgc_graph {
     // writes them all)
     bool lazy_caps = true;
     bool caps_lazy = false;            // the last build was lazy and some tiles are not materialised yet
-    // the last build was the lazy fused build and nothing else changed the terms since: mgc_add_seeds / mgc_remove_seeds
-    // may fold seeds into the residual state.  Unlike caps_lazy this stays true once every tile is materialised (hard
-    // instances).
+    // the last build was the lazy fused build and nothing else changed the terms since: mgc_add_seeds / mgc_remove_seeds /
+    // mgc_add_tweights_warm may fold t-link calls into the residual state.  Unlike caps_lazy this stays true once every
+    // tile is materialised (hard instances).
     bool lazy_built = false;
     int* cmat = nullptr;               // per tile: push state materialised since the last lazy build
     int* caps_list = nullptr;          // tiles claimed by the current materialiser launch
@@ -179,7 +180,7 @@ struct mgc_graph {
     Buf img_copy;                      // the image the lazy build saw, in its own dtype
     Buf prob_copy;                     // ... its probability map, in its own dtype
     Buf mark_planes[2];                // ... its fg / bg markers as bit planes (LazyTin)
-    Buf seed_buf;                      // seed folds: item count + error flag, ids, keys, runs, seeded tiles, items, sort scratch
+    Buf seed_buf;                      // folds: item count + error flag, inputs, keys, runs, touched tiles, items, cub scratch
     cudaEvent_t ev_seed[4] = {};       // spans of the grouping and of claim + fold + list fix-up
     int caps_dtype = MGC_F32;
     BoundaryParams caps_P{};           // the boundary term of the lazy build
@@ -891,6 +892,23 @@ void seed_fold_launch_t(mgc_graph* g, unsigned grid, const SeedItem* items, int 
         }
     }
     k_seed_fold<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, cap, g->partials);
+}
+
+// k_tweights_fold with the same instantiations
+template <typename E>
+void tweights_fold_launch_t(mgc_graph* g, unsigned grid, const TweightItem* items, int n, const int* order,
+                            const double* src, const double* snk)
+{
+    const BoundaryParams& P = g->caps_P;
+    const E* img = (const E*)g->img_copy.p;
+    if constexpr (!std::is_integral<E>::value) {
+        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
+            if (P.use_max) k_tweights_fold<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
+            else           k_tweights_fold<E, 1, 0, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
+            return;
+        }
+    }
+    k_tweights_fold<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
 }
 
 // capacities, tr or excess are about to be read or written outside the push path: materialise the tiles that are not yet
@@ -2449,20 +2467,21 @@ int mgc_maxflow(mgc_graph* g, double* energy)
     return MGC_OK;
 }
 
-// mgc_add_seeds (cap = 65535) and mgc_remove_seeds (cap = -65535): add_tweights(v, cap, 0) for every fg id in list order,
-// then add_tweights(v, 0, cap) for every bg id, folded into the handle's current state
-// Number of kernels cub::DeviceRadixSort::SortKeys + cub::DeviceScan::InclusiveSum enqueue for n keys of end_bit bits, so
-// that kernel_launches counts them too.  cub decides it on the host from (n, end_bit) and the device; the calls are
-// captured on a capture-only stream of the device (nothing runs) and the kernel nodes of the captured graph counted.
-// The stream lives for the process and the counts are cached, so a call pays only the capture of a few launches.
-static int seed_cub_launches(mgc_graph* g, int n, int end_bit, void* tmp, size_t tmp_bytes, unsigned* keys, unsigned* skeys,
-                             int* head, int* pos, int* out)
+// Number of kernels the cub calls of a fold's grouping enqueue, so that kernel_launches counts them too: CUB_SEED_KEYS =
+// cub::DeviceRadixSort::SortKeys + cub::DeviceScan::InclusiveSum (seeds), CUB_PAIRS = SortPairs + InclusiveSum (the list
+// form of mgc_add_tweights_warm), CUB_SCAN = InclusiveSum alone (its dense form).  cub decides it on the host from
+// (n, end_bit) and the device; the calls are captured on a capture-only stream of the device (nothing runs) and the kernel
+// nodes of the captured graph counted.  The stream lives for the process and the counts are cached, so a call pays only
+// the capture of a few launches.
+enum { CUB_SEED_KEYS = 0, CUB_PAIRS = 1, CUB_SCAN = 2 };
+static int seed_cub_launches(mgc_graph* g, int kind, int n, int end_bit, void* tmp, size_t tmp_bytes, unsigned* keys,
+                             unsigned* skeys, int* vals, int* svals, int* head, int* pos, int* out)
 {
     static std::mutex mu;
     static std::map<int, cudaStream_t> streams;
-    static std::map<std::tuple<int, int, int>, int> counts;
+    static std::map<std::tuple<int, int, int, int>, int> counts;
     std::lock_guard<std::mutex> lock(mu);
-    const auto key = std::make_tuple(g->device, n, end_bit);
+    const auto key = std::make_tuple(g->device, kind, n, end_bit);
     auto it = counts.find(key);
     if (it != counts.end()) { *out = it->second; return MGC_OK; }
     cudaStream_t& s = streams[g->device];
@@ -2471,7 +2490,9 @@ static int seed_cub_launches(mgc_graph* g, int n, int end_bit, void* tmp, size_t
     cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed);
     if (e == cudaSuccess) {
         size_t tb = tmp_bytes;
-        cudaError_t e1 = cub::DeviceRadixSort::SortKeys(tmp, tb, keys, skeys, n, 0, end_bit, s);
+        cudaError_t e1 = cudaSuccess;
+        if (kind == CUB_SEED_KEYS) e1 = cub::DeviceRadixSort::SortKeys(tmp, tb, keys, skeys, n, 0, end_bit, s);
+        else if (kind == CUB_PAIRS) e1 = cub::DeviceRadixSort::SortPairs(tmp, tb, keys, skeys, vals, svals, n, 0, end_bit, s);
         tb = tmp_bytes;
         cudaError_t e2 = e1 == cudaSuccess ? cub::DeviceScan::InclusiveSum(tmp, tb, head, pos, n, s) : e1;
         e = cudaStreamEndCapture(s, &graph);
@@ -2495,6 +2516,82 @@ static int seed_cub_launches(mgc_graph* g, int n, int end_bit, void* tmp, size_t
     return MGC_OK;
 }
 
+// preconditions of every fold into the residual state (the copies of the lazy fused build are what the fold reads)
+static int warm_check(mgc_graph* g)
+{
+    if (!g->lazy_built || !g->state_init || g->slab || !g->use_tiles || g->nd != 3)
+        FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
+                          "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
+                          "the seeds instead");
+    return MGC_OK;
+}
+
+// The steps of a fold after its grouping, shared by seeds_fold and mgc_add_tweights_warm.  The grouping was enqueued after
+// ev_seed[0] and left d_ctl = [item count | FOLD_ERR_* bits | touched-tile count] and the touched tiles in `tiles`;
+// fold(grid, n_items) enqueues the fold kernel, which stores one partial of the add_tweights constant per block.
+static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<void(unsigned, int)>& fold)
+{
+    CK(cudaEventRecord(g->ev_seed[1], g->stream));
+    // the item count and the error bits in one synchronisation, before the claim and the fold are enqueued
+    int h_ctl[2] = {0, 0};
+    CK(cudaMemcpyAsync(h_ctl, d_ctl, sizeof(h_ctl), cudaMemcpyDeviceToHost, g->stream));
+    CK(cudaStreamSynchronize(g->stream));
+    if (h_ctl[1] & FOLD_ERR_RANGE) FAIL(MGC_E_ARG, "node id out of range");
+    if (h_ctl[1] & FOLD_ERR_NONFINITE) FAIL(MGC_E_ARG, "a t-link weight is NaN or infinite");
+    const int ni = h_ctl[0];
+    if (ni == 0) return MGC_OK;                // only add_tweights(v, 0, 0) calls: the state, mask and energy stay
+    CK(cudaEventRecord(g->ev_seed[2], g->stream));
+    // 1. every touched voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
+    if (g->caps_lazy) {
+        // Source excess is still implicit on the tiles that are listed but not materialised (before the first solve, or
+        // deferred by the label window of the last one) and on the tiles the window dropped unmaterialised.  A new sink
+        // link may drain it: materialise them, step 3 rebuilds the lists from cmat.
+        int rc;
+        for (int color = 0; color < 2; ++color) { rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
+        rc = caps_launch(g, WorkList{g->drop_items, g->win_ctl + WIN_NDROP});
+        if (rc) return rc;
+        CK(cudaMemsetAsync(g->win_ctl + WIN_NDROP, 0, sizeof(int), g->stream));
+        rc = caps_launch(g, WorkList{tiles, d_ctl + 2});
+        if (rc) return rc;
+    }
+    // 2. the fold, its change of the add_tweights constant summed in a fixed order into flow_const
+    unsigned grid = (unsigned)((ni + 255) / 256);
+    if (grid > REDUCE_BLOCKS) grid = REDUCE_BLOCKS;
+    fold(grid, ni);
+    k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, grid, g->d_scalars);
+    // 3. solver state for the next solve: fresh push lists over every materialised tile with excess; labels from a full
+    // relabel reset (sweep_mode = -1: a fold can remove a sink link, so the last solve's labels bound nothing)
+    CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
+    CK(cudaMemsetAsync(g->pflag, 0, (size_t)g->TL.ntiles * sizeof(int), g->stream));
+    g->pl_sel[0] = g->pl_sel[1] = 0;
+    {
+        unsigned lgrid = (unsigned)g->n_ctas * 4u;
+        if (lgrid > (unsigned)g->TL.ntiles) lgrid = (unsigned)g->TL.ntiles;
+        k_seed_lists<<<lgrid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->cmat, g->pflag, pl(g, 0, 0), pl(g, 1, 0));
+    }
+    g->st.kernel_launches += 3;
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(g->ev_seed[3], g->stream));
+    CK(cudaEventSynchronize(g->ev_seed[3]));
+    {
+        // two device spans: the grouping, then claim + fold + list fix-up (the read-back between them is not counted)
+        float ms0 = 0, ms1 = 0;
+        if (cudaEventElapsedTime(&ms0, g->ev_seed[0], g->ev_seed[1]) == cudaSuccess &&
+            cudaEventElapsedTime(&ms1, g->ev_seed[2], g->ev_seed[3]) == cudaSuccess)
+            g->st.ms_seeds += ms0 + ms1;
+        g->st.ms_caps -= caps_resolve(g);          // the claim is part of ms_seeds, not of the solve's materialisation
+    }
+    g->labels_fresh = false;
+    g->rl_cur = 0;
+    g->sweep_mode = -1;
+    g->solved = false;
+    g->host_mask_valid = false;
+    g->st.seed_folds++;
+    return MGC_OK;
+}
+
+// mgc_add_seeds (cap = 65535) and mgc_remove_seeds (cap = -65535): add_tweights(v, cap, 0) for every fg id in list order,
+// then add_tweights(v, 0, cap) for every bg id, folded into the handle's current state
 static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem,
                       double cap)
 {
@@ -2502,10 +2599,7 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
     if (n_fg < 0 || n_bg < 0 || (n_fg && !fg_ids) || (n_bg && !bg_ids)) FAIL(MGC_E_ARG, "bad seed lists");
     if (n_fg + n_bg > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 seeds in one call");
     if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
-    if (!g->lazy_built || !g->state_init || g->slab || !g->use_tiles || g->nd != 3)
-        FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
-                          "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
-                          "the seeds instead");
+    { int rc0 = warm_check(g); if (rc0) return rc0; }
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
     if (n_fg + n_bg == 0) return MGC_OK;       // nothing to fold: the solved state, mask and energy stay as they are
@@ -2546,7 +2640,8 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
     int* tiles = (int*)(dbuf + tiles_off);
     SeedItem* d_items = (SeedItem*)(dbuf + items_off);
     int cub_launches = 0;
-    rc = seed_cub_launches(g, n, end_bit, dbuf + tmp_off, tmp_bytes, keys, skeys, head, pos, &cub_launches);
+    rc = seed_cub_launches(g, CUB_SEED_KEYS, n, end_bit, dbuf + tmp_off, tmp_bytes, keys, skeys, nullptr, nullptr, head,
+                           pos, &cub_launches);
     if (rc) return rc;
     for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
     Nvtx range(cap > 0 ? "mgc:add_seeds" : "mgc:remove_seeds");
@@ -2578,66 +2673,15 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
         g->st.kernel_launches += 3 + cub_launches;
         CK(cudaGetLastError());
     }
-    CK(cudaEventRecord(g->ev_seed[1], g->stream));
-    // the item count and the range flag in one synchronisation, before the claim and the fold are enqueued
-    int h_ctl[2] = {0, 0};
-    CK(cudaMemcpyAsync(h_ctl, d_count, sizeof(h_ctl), cudaMemcpyDeviceToHost, g->stream));
-    CK(cudaStreamSynchronize(g->stream));
-    if (h_ctl[1]) FAIL(MGC_E_ARG, "node id out of range");
-    const int ni = h_ctl[0];
-    CK(cudaEventRecord(g->ev_seed[2], g->stream));
-    // 1. every seeded voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
-    if (g->caps_lazy) {
-        // Source excess is still implicit on the tiles that are listed but not materialised (before the first solve, or
-        // deferred by the label window of the last one) and on the tiles the window dropped unmaterialised.  A new sink
-        // link may drain it: materialise them, step 3 rebuilds the lists from cmat.
-        for (int color = 0; color < 2; ++color) { rc = caps_launch(g, pl(g, color, g->pl_sel[color])); if (rc) return rc; }
-        rc = caps_launch(g, WorkList{g->drop_items, g->win_ctl + WIN_NDROP});
-        if (rc) return rc;
-        CK(cudaMemsetAsync(g->win_ctl + WIN_NDROP, 0, sizeof(int), g->stream));
-        rc = caps_launch(g, WorkList{tiles, d_count + 2});
-        if (rc) return rc;
-    }
-    // 2. the fold, its change of the add_tweights constant summed in a fixed order into flow_const
-    unsigned grid = (unsigned)((ni + 255) / 256);
-    if (grid > REDUCE_BLOCKS) grid = REDUCE_BLOCKS;
-    switch (g->caps_dtype) {
-        case MGC_F32: seed_fold_launch_t<float>(g, grid, d_items, ni, cap); break;
-        case MGC_F64: seed_fold_launch_t<double>(g, grid, d_items, ni, cap); break;
-        case MGC_U8: seed_fold_launch_t<uint8_t>(g, grid, d_items, ni, cap); break;
-        case MGC_I16: seed_fold_launch_t<int16_t>(g, grid, d_items, ni, cap); break;
-        default: seed_fold_launch_t<int32_t>(g, grid, d_items, ni, cap); break;
-    }
-    k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, grid, g->d_scalars);
-    // 3. solver state for the next solve: fresh push lists over every materialised tile with excess; labels from a full
-    // relabel reset (sweep_mode = -1: a fold can remove a sink link, so the last solve's labels bound nothing)
-    CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
-    CK(cudaMemsetAsync(g->pflag, 0, (size_t)g->TL.ntiles * sizeof(int), g->stream));
-    g->pl_sel[0] = g->pl_sel[1] = 0;
-    {
-        unsigned lgrid = (unsigned)g->n_ctas * 4u;
-        if (lgrid > (unsigned)g->TL.ntiles) lgrid = (unsigned)g->TL.ntiles;
-        k_seed_lists<<<lgrid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->cmat, g->pflag, pl(g, 0, 0), pl(g, 1, 0));
-    }
-    g->st.kernel_launches += 3;
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(g->ev_seed[3], g->stream));
-    CK(cudaEventSynchronize(g->ev_seed[3]));
-    {
-        // two device spans: the grouping, then claim + fold + list fix-up (the read-back between them is not counted)
-        float ms0 = 0, ms1 = 0;
-        if (cudaEventElapsedTime(&ms0, g->ev_seed[0], g->ev_seed[1]) == cudaSuccess &&
-            cudaEventElapsedTime(&ms1, g->ev_seed[2], g->ev_seed[3]) == cudaSuccess)
-            g->st.ms_seeds += ms0 + ms1;
-        g->st.ms_caps -= caps_resolve(g);          // the claim is part of ms_seeds, not of the solve's materialisation
-    }
-    g->labels_fresh = false;
-    g->rl_cur = 0;
-    g->sweep_mode = -1;
-    g->solved = false;
-    g->host_mask_valid = false;
-    g->st.seed_folds++;
-    return MGC_OK;
+    return fold_items(g, d_count, tiles, [&](unsigned grid, int ni) {
+        switch (g->caps_dtype) {
+            case MGC_F32: seed_fold_launch_t<float>(g, grid, d_items, ni, cap); break;
+            case MGC_F64: seed_fold_launch_t<double>(g, grid, d_items, ni, cap); break;
+            case MGC_U8: seed_fold_launch_t<uint8_t>(g, grid, d_items, ni, cap); break;
+            case MGC_I16: seed_fold_launch_t<int16_t>(g, grid, d_items, ni, cap); break;
+            default: seed_fold_launch_t<int32_t>(g, grid, d_items, ni, cap); break;
+        }
+    });
 }
 
 int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem)
@@ -2648,6 +2692,118 @@ int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64
 int mgc_remove_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem)
 {
     return seeds_fold(g, fg_ids, n_fg, bg_ids, n_bg, mem, -65535.0);
+}
+
+int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, const double* snk, int64_t count, int32_t mem)
+{
+    if (!g) return MGC_E_ARG;
+    if (count < 0 || (count && (!src || !snk))) FAIL(MGC_E_ARG, "bad t-link arrays");
+    if (count > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 add_tweights calls in one call");
+    if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
+    { int rc0 = warm_check(g); if (rc0) return rc0; }
+    const bool dense = ids == nullptr;
+    if (dense && count && count != (int64_t)g->L.n) FAIL(MGC_E_ARG, "the dense form takes one weight pair per voxel");
+    CK(cudaSetDevice(g->device));
+    { int rc0 = check_pending(g); if (rc0) return rc0; }
+    if (count == 0) return MGC_OK;             // nothing to fold: the solved state, mask and energy stay as they are
+    const auto host_t0 = std::chrono::steady_clock::now();
+    const int n = (int)count;
+    // list form: (voxel id, call index) pairs sorted on the bits a voxel id of this lattice can have, then run-length
+    // encoded; dense form: the voxels with a nonzero weight, compacted by a scan of their flags.  In both, a voxel whose
+    // calls all have zero weights is no item (add_tweights(v, 0, 0) changes nothing)
+    int end_bit = 1;
+    while (end_bit < 32 && ((uint64_t)g->L.n - 1ull) >> end_bit) ++end_bit;
+    size_t sort_bytes = 0, scan_bytes = 0;
+    if (!dense)
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr,
+                                           (const int*)nullptr, (int*)nullptr, n, 0, end_bit, g->stream));
+    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
+    // device layout (16-byte aligned pieces): [item count | error bits | touched-tile count | pad] [host ids] [host src]
+    // [host snk] [keys] [sorted keys] [call indices] [sorted call indices] [heads] [positions] [per-tile flags]
+    // [touched tiles] [items] [cub scratch]; no ids, keys or call indices in the dense form
+    auto al = [](size_t b) { return (b + 15) / 16 * 16; };
+    const size_t ntl = (size_t)g->TL.ntiles;
+    const bool host = mem == MGC_MEM_HOST;
+    const size_t w4 = dense ? 0 : al((size_t)n * 4);
+    const size_t ids_off = 16;
+    const size_t src_off = ids_off + (host && !dense ? al((size_t)n * 8) : 0);
+    const size_t snk_off = src_off + (host ? al((size_t)n * 8) : 0);
+    const size_t keys_off = snk_off + (host ? al((size_t)n * 8) : 0);
+    const size_t skeys_off = keys_off + w4;
+    const size_t vals_off = skeys_off + w4;
+    const size_t svals_off = vals_off + w4;
+    const size_t head_off = svals_off + w4;
+    const size_t pos_off = head_off + al((size_t)n * 4);
+    const size_t tflag_off = pos_off + al((size_t)n * 4);
+    const size_t tiles_off = tflag_off + al(ntl * 4);
+    const size_t items_off = tiles_off + al(std::min((size_t)n, ntl) * 4);
+    const size_t tmp_off = items_off + al((size_t)n * sizeof(TweightItem));
+    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
+    int rc = ensure_scratch(g, g->seed_buf, tmp_off + tmp_bytes);
+    if (rc) return rc;
+    char* dbuf = (char*)g->seed_buf.p;
+    int* d_ctl = (int*)dbuf;
+    unsigned* keys = (unsigned*)(dbuf + keys_off);
+    unsigned* skeys = (unsigned*)(dbuf + skeys_off);
+    int* vals = (int*)(dbuf + vals_off);
+    int* svals = (int*)(dbuf + svals_off);
+    int* head = (int*)(dbuf + head_off);
+    int* pos = (int*)(dbuf + pos_off);
+    int* tflag = (int*)(dbuf + tflag_off);
+    int* tiles = (int*)(dbuf + tiles_off);
+    TweightItem* d_items = (TweightItem*)(dbuf + items_off);
+    int cub_launches = 0;
+    rc = seed_cub_launches(g, dense ? CUB_SCAN : CUB_PAIRS, n, end_bit, dbuf + tmp_off, tmp_bytes, keys, skeys, vals, svals,
+                           head, pos, &cub_launches);
+    if (rc) return rc;
+    for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
+    Nvtx range("mgc:add_tweights_warm");
+    g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
+    // 0. grouping on the device; nothing below touches the solver state until the range and finiteness checks have passed
+    CK(cudaEventRecord(g->ev_seed[0], g->stream));
+    const int64_t* d_ids = ids;
+    const double* d_src = src;
+    const double* d_snk = snk;
+    if (host) {
+        // host arrays go straight from the caller into device slots; device arrays are read in place
+        if (!dense) {
+            CK(cudaMemcpyAsync(dbuf + ids_off, ids, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+            d_ids = (const int64_t*)(dbuf + ids_off);
+        }
+        CK(cudaMemcpyAsync(dbuf + src_off, src, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+        CK(cudaMemcpyAsync(dbuf + snk_off, snk, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+        d_src = (const double*)(dbuf + src_off);
+        d_snk = (const double*)(dbuf + snk_off);
+    }
+    CK(cudaMemsetAsync(d_ctl, 0, 3 * sizeof(int), g->stream));
+    CK(cudaMemsetAsync(tflag, 0, ntl * sizeof(int), g->stream));
+    {
+        const unsigned kgrid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
+        size_t tb = tmp_bytes;
+        if (dense) {
+            k_tweights_dense_heads<<<kgrid, 256, 0, g->stream>>>(d_src, d_snk, n, head, d_ctl + 1);
+        } else {
+            k_tweights_keys<<<kgrid, 256, 0, g->stream>>>(d_ids, d_src, d_snk, n, (int64_t)g->L.n, keys, vals, d_ctl + 1);
+            CK(cub::DeviceRadixSort::SortPairs(dbuf + tmp_off, tb, keys, skeys, vals, svals, n, 0, end_bit, g->stream));
+            k_tweights_heads<<<kgrid, 256, 0, g->stream>>>(skeys, svals, d_src, d_snk, n, head);
+            tb = tmp_bytes;
+        }
+        CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
+        k_tweights_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, dense ? nullptr : skeys, pos, n, d_items, tflag, tiles,
+                                                       d_ctl);
+        g->st.kernel_launches += (dense ? 2 : 3) + cub_launches;
+        CK(cudaGetLastError());
+    }
+    const int* order = dense ? nullptr : svals;
+    return fold_items(g, d_ctl, tiles, [&](unsigned grid, int ni) {
+        switch (g->caps_dtype) {
+            case MGC_F32: tweights_fold_launch_t<float>(g, grid, d_items, ni, order, d_src, d_snk); break;
+            case MGC_F64: tweights_fold_launch_t<double>(g, grid, d_items, ni, order, d_src, d_snk); break;
+            case MGC_U8: tweights_fold_launch_t<uint8_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
+            case MGC_I16: tweights_fold_launch_t<int16_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
+            default: tweights_fold_launch_t<int32_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
+        }
+    });
 }
 
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem)

@@ -218,6 +218,37 @@ public:
         { py::gil_scoped_release rel; rc = mgc_add_nweights_dense(g_, axis, &a.a, &b.a); }
         check(rc, g_);
     }
+    // contiguous 1-D array on the host (numpy, converted to T) or on the device (__cuda_array_interface__ of typestr `ts`,
+    // read in place); None = absent
+    struct Vec { const void* p = nullptr; int64_t n = 0; int mem = -1; py::object keep; };
+    template <typename T>
+    static Vec vec_of(const py::object& o, const char* ts, const char* what)
+    {
+        Vec r;
+        if (o.is_none()) return r;
+        const std::string bad = std::string(what) + ": expected a 1-D " + (ts[0] == 'i' ? "int64" : "float64") + " array";
+        if (py::hasattr(o, "__cuda_array_interface__")) {
+            py::dict d = o.attr("__cuda_array_interface__");
+            py::tuple shp = d["shape"];
+            if (shp.size() != 1 || d["typestr"].cast<std::string>().substr(1) != ts) throw py::value_error(bad);
+            if (d.contains("strides") && !d["strides"].is_none()) {
+                py::tuple st = d["strides"];
+                if (st[0].cast<int64_t>() != 8) throw py::value_error(std::string(what) + ": array must be contiguous");
+            }
+            r.p = reinterpret_cast<const void*>(py::tuple(d["data"])[0].cast<uintptr_t>());
+            r.n = shp[0].cast<int64_t>();
+            r.mem = MGC_MEM_DEVICE;
+            r.keep = o;
+        } else {
+            auto a = py::array_t<T, py::array::c_style | py::array::forcecast>::ensure(o);
+            if (!a || a.ndim() != 1) throw py::value_error(bad);
+            r.p = a.data();
+            r.n = a.shape(0);
+            r.mem = MGC_MEM_HOST;
+            r.keep = a;
+        }
+        return r;
+    }
     // seeds folded into the solved graph (mgc_add_seeds / mgc_remove_seeds): 1-D int64 node-id arrays, both on the host
     // (numpy) or both on the device (__cuda_array_interface__); None = no seeds of that kind
     void add_seeds(const py::object& fg, const py::object& bg) { fold_seeds(fg, bg, mgc_add_seeds); }
@@ -225,38 +256,29 @@ public:
     void fold_seeds(const py::object& fg, const py::object& bg,
                     int (*fold)(mgc_graph*, const int64_t*, int64_t, const int64_t*, int64_t, int32_t))
     {
-        struct Ids { const int64_t* p = nullptr; int64_t n = 0; int mem = -1; py::object keep; };
-        auto ids = [](const py::object& o, const char* what) {
-            Ids r;
-            if (o.is_none()) return r;
-            if (py::hasattr(o, "__cuda_array_interface__")) {
-                py::dict d = o.attr("__cuda_array_interface__");
-                py::tuple shp = d["shape"];
-                const std::string ts = d["typestr"].cast<std::string>();
-                if (shp.size() != 1 || ts.substr(1) != "i8") throw py::value_error(std::string(what) + ": expected a 1-D int64 array");
-                if (d.contains("strides") && !d["strides"].is_none()) {
-                    py::tuple st = d["strides"];
-                    if (st[0].cast<int64_t>() != 8) throw py::value_error(std::string(what) + ": ids must be contiguous");
-                }
-                r.p = reinterpret_cast<const int64_t*>(py::tuple(d["data"])[0].cast<uintptr_t>());
-                r.n = shp[0].cast<int64_t>();
-                r.mem = MGC_MEM_DEVICE;
-                r.keep = o;
-            } else {
-                auto a = py::array_t<int64_t, py::array::c_style | py::array::forcecast>::ensure(o);
-                if (!a || a.ndim() != 1) throw py::value_error(std::string(what) + ": expected a 1-D int64 array");
-                r.p = a.data();
-                r.n = a.shape(0);
-                r.mem = MGC_MEM_HOST;
-                r.keep = a;
-            }
-            return r;
-        };
-        Ids f = ids(fg, "fg_ids"), b = ids(bg, "bg_ids");
+        Vec f = vec_of<int64_t>(fg, "i8", "fg_ids"), b = vec_of<int64_t>(bg, "i8", "bg_ids");
         if (f.n && b.n && f.mem != b.mem) throw py::value_error("fg_ids and bg_ids must both be host or both be device arrays");
         const int mem = f.n ? f.mem : (b.n ? b.mem : MGC_MEM_HOST);
         int rc;
-        { py::gil_scoped_release rel; rc = fold(g_, f.n ? f.p : nullptr, f.n, b.n ? b.p : nullptr, b.n, mem); }
+        { py::gil_scoped_release rel; rc = fold(g_, f.n ? (const int64_t*)f.p : nullptr, f.n, b.n ? (const int64_t*)b.p : nullptr, b.n, mem); }
+        check(rc, g_);
+    }
+    // add_tweights calls folded into the solved graph (mgc_add_tweights_warm): ids = 1-D int64 node ids (None: the dense
+    // form, one call per voxel in C order), src / snk = 1-D float64 of the same length; all three on the host or all on
+    // the device
+    void add_tweights_warm(const py::object& ids, const py::object& src, const py::object& snk)
+    {
+        Vec i = vec_of<int64_t>(ids, "i8", "ids"), s = vec_of<double>(src, "f8", "src"), t = vec_of<double>(snk, "f8", "snk");
+        if (s.mem < 0 || t.mem < 0) throw py::value_error("src and snk are required");
+        if (s.n != t.n || (!ids.is_none() && i.n != s.n)) throw py::value_error("ids, src and snk differ in length");
+        if (s.mem != t.mem || (!ids.is_none() && i.mem != s.mem))
+            throw py::value_error("ids, src and snk must all be host or all be device arrays");
+        int rc;
+        {
+            py::gil_scoped_release rel;
+            rc = mgc_add_tweights_warm(g_, ids.is_none() ? nullptr : (const int64_t*)i.p, (const double*)s.p,
+                                       (const double*)t.p, s.n, s.mem);
+        }
         check(rc, g_);
     }
     double maxflow()
@@ -641,6 +663,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("add_nweights_dense", &PyGraph::add_nweights_dense)
         .def("add_seeds", &PyGraph::add_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
         .def("remove_seeds", &PyGraph::remove_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
+        .def("add_tweights_warm", &PyGraph::add_tweights_warm, py::arg("ids"), py::arg("src"), py::arg("snk"))
         .def("build_voxel_graph", &PyGraph::build_voxel_graph)
         .def_static("slab_comm_unique_id", &PyGraph::slab_comm_unique_id)
         .def("slab_comm_init", &PyGraph::slab_comm_init)

@@ -1,5 +1,5 @@
-// gc_seeds.cuh -- seeds added to or erased from a solved lazily built 3-D graph, folded into its residual state
-// (mgc_add_seeds / mgc_remove_seeds).
+// gc_seeds.cuh -- seeds added to or erased from a solved lazily built 3-D graph, and any add_tweights calls, folded into
+// its residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm).
 //
 // The reference refines a cut by calling add_tweights(v, 65535, 0) / add_tweights(v, 0, 65535) on the new seed voxels of
 // a solved GraphDouble and calling maxflow() again, and erases a seed with the inverse call add_tweights(v, -65535, 0) /
@@ -16,6 +16,9 @@
 //      representation;
 //   3. k_seed_lists puts every materialised tile that holds excess back on the push lists; the next solve starts with a
 //      full relabel reset.
+// mgc_add_tweights_warm runs the same steps with a value per call: its own grouping (k_tweights_keys / _heads / _items for a
+// call list, k_tweights_dense_heads / k_tweights_items for one call per voxel) and k_tweights_fold, which shares the read of
+// r(v) and the write-back of r' with k_seed_fold (residual_read / residual_write).
 #pragma once
 #include "gc_build.cuh"
 
@@ -27,6 +30,10 @@ struct SeedItem {
     int pad;
 };
 
+// error bits of a grouping, read back before anything touches the solver state
+#define FOLD_ERR_RANGE 1
+#define FOLD_ERR_NONFINITE 2
+
 // grouping keys v << 1 | bg (the lattice has < 2^31 voxels, so a key fits 32 bits); fg ids first, then bg ids.  An id out
 // of range sets *err and gets key 0: the caller reads *err back before anything uses the items.
 __global__ void __launch_bounds__(256) k_seed_keys(const int64_t* __restrict__ fg, int n_fg, const int64_t* __restrict__ bg,
@@ -37,7 +44,7 @@ __global__ void __launch_bounds__(256) k_seed_keys(const int64_t* __restrict__ f
         const bool b = i >= n_fg;
         const int64_t v = b ? bg[i - n_fg] : fg[i];
         unsigned k = 0u;
-        if (v < 0 || v >= n_vox) *err = 1;
+        if (v < 0 || v >= n_vox) *err = FOLD_ERR_RANGE;
         else k = ((unsigned)v << 1) | (b ? 1u : 0u);
         keys[i] = k;
     }
@@ -51,6 +58,17 @@ __device__ __forceinline__ int seed_lower_bound(const unsigned* __restrict__ key
         if (keys[mid] < x) lo = mid + 1; else hi = mid;
     }
     return lo;
+}
+
+// lists the tile of voxel v for the claim unless an earlier item did: tflag[t] (zeroed by the caller) flips once, ctl[2]
+// counts the listed tiles
+__device__ __forceinline__ void claim_tile_once(const Lattice& L, const Tiles& TL, unsigned v, int* __restrict__ tflag,
+                                                int* __restrict__ tiles, int* __restrict__ ctl)
+{
+    int c[3];
+    decode<3>(L, v, c);
+    const int t = ((c[0] / TILE) * TL.nt[1] + c[1] / TILE) * TL.nt[2] + c[2] / TILE;
+    if (tflag[t] == 0 && atomicExch(&tflag[t], 1) == 0) tiles[atomicAdd(&ctl[2], 1)] = t;
 }
 
 // Run-length pass over the sorted keys: pos = inclusive sum of the voxel-run heads, so the run starting at head i is item
@@ -73,10 +91,7 @@ __global__ void __launch_bounds__(256) k_seed_items(Lattice L, Tiles TL, const u
         const int s = seed_lower_bound(keys, i, n, 2u * v + 1u);
         const int e = seed_lower_bound(keys, s, n, 2u * v + 2u);
         items[pos[i] - 1] = SeedItem{v, s - i, e - s, 0};
-        int c[3];
-        decode<3>(L, v, c);
-        const int t = ((c[0] / TILE) * TL.nt[1] + c[1] / TILE) * TL.nt[2] + c[2] / TILE;
-        if (tflag[t] == 0 && atomicExch(&tflag[t], 1) == 0) tiles[atomicAdd(&ctl[2], 1)] = t;
+        claim_tile_once(L, TL, v, tflag, tiles, ctl);
     }
 }
 
@@ -116,95 +131,217 @@ __global__ void __launch_bounds__(256) k_seed_heads(const unsigned* __restrict__
 //     the flow already pushed, which a later fold reads back as r' - source_excess(r', c_orig), the residual on top of
 //     all the flow pushed so far;
 //   - r' = 0: no terminal link, as for any seed that cancels.
+// A materialised voxel's state read as BK's residual terminal capacity (residual_read), and r' written back in the
+// solver's representation (residual_write): the two halves of every fold, k_seed_fold and k_tweights_fold.
+struct Residual {
+    double co[6];     // capacities before any flow
+    double lim0;      // their sum rounded up, x SOURCE_CLAMP_SLACK
+    double r;         // r(v); the fold applies its add_tweights calls to it
+    double dk;        // change of the add_tweights constant: the absorbed sink flow, then the minima of the calls
+    double e;         // excess
+    unsigned rm;      // rmask
+};
+
+template <typename E, int FN, int USE_MAX, int SPACING>
+__device__ __forceinline__ Residual residual_read(const Lattice& L, const State<double>& S, const E* __restrict__ img,
+                                                  const BoundaryParams& P, unsigned v)
+{
+    const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
+    const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
+    Residual f;
+    int c[3];
+    decode<3>(L, v, c);
+    // capacities before any flow: the doubles k_caps_tiles computed from the same image copy
+    const unsigned valid = (c[0] > 0 ? 1u : 0u) | (c[0] + 1 < L.dim[0] ? 2u : 0u) | (c[1] > 0 ? 4u : 0u) |
+                           (c[1] + 1 < L.dim[1] ? 8u : 0u) | (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
+    const double a = build_val<E>(img[v], use_max);
+    if (FN == 1 && SPACING == 0) {
+        double t6[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+            t6[k] = 0.0;
+            if ((valid >> k) & 1u) {
+                const double b = build_val<E>(img[(unsigned)((int)v + dir_offset(L, k))], use_max);
+                t6[k] = exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
+            }
+        }
+        exp_caps6(t6, false, valid, f.co);     // the general branch: the same doubles for ordinary arguments
+    } else {
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+            f.co[k] = ((valid >> k) & 1u)
+                          ? build_weight<FN, E>(P, a, img[(unsigned)((int)v + dir_offset(L, k))], use_max, spacing, P.spacing[k >> 1])
+                          : 0.0;
+    }
+    double lim0 = __dadd_ru(0.0, f.co[0]);
+    lim0 = __dadd_ru(lim0, f.co[1]); lim0 = __dadd_ru(lim0, f.co[2]); lim0 = __dadd_ru(lim0, f.co[3]);
+    lim0 = __dadd_ru(lim0, f.co[4]); lim0 = __dadd_ru(lim0, f.co[5]);
+    f.lim0 = lim0 * SOURCE_CLAMP_SLACK;
+
+    const double tr = S.tr[v];
+    f.rm = S.rmask[v];
+    f.e = S.excess[v];
+    f.dk = 0.0;
+    f.r = 0.0;
+    if (tr > 0) {
+        f.r = __dsub_rn(tr, source_excess(tr, f.co));
+    } else if (tr < 0) {
+        const double sf = (f.rm & RM_SINKV) ? S.sink[v] : 0.0;
+        f.r = __dadd_rn(tr, sf);
+        f.dk = sf;
+    }
+    return f;
+}
+
+__device__ __forceinline__ void residual_write(const State<double>& S, unsigned v, const Residual& f)
+{
+    const double r = f.r;
+    double e = f.e;
+    unsigned nm = f.rm & 0x3fu;
+    double trn = 0.0;
+    if (r < 0) {
+        trn = r;
+        const double scap = -r;
+        double sf;
+        if (e >= scap) { sf = scap; e = __dsub_rn(e, scap); }
+        else { sf = e; e = 0.0; }
+        if (scap - sf > 0) nm |= RM_SINK;
+        S.sink[v] = sf;
+        nm |= RM_SINKV;
+    } else if (r > 0) {
+        double out = __dadd_ru(0.0, S.cap[0][v]);
+        out = __dadd_ru(out, S.cap[1][v]); out = __dadd_ru(out, S.cap[2][v]); out = __dadd_ru(out, S.cap[3][v]);
+        out = __dadd_ru(out, S.cap[4][v]); out = __dadd_ru(out, S.cap[5][v]);
+        const double lim = out * SOURCE_CLAMP_SLACK;
+        if (!(lim > f.lim0)) {
+            // the usual case (no net inflow through the n-links): push source_excess(r', c_orig) >= min(r', lim) and
+            // keep tr = r', which reads back as r' - source_excess(r', c_orig) bit for bit
+            e = __dadd_rn(e, source_excess(r, f.co));
+            trn = r;
+        } else {
+            const double p = r < lim ? r : lim;
+            e = __dadd_rn(e, p);
+            const double u = __dsub_rn(r, p);
+            if (u > 0) trn = __dadd_rn(u, f.lim0);    // reads back as (u + lim0) - lim0: u to one rounding
+        }
+    }
+    S.tr[v] = trn;
+    S.excess[v] = e;
+    S.rmask[v] = (uint8_t)nm;
+}
+
 template <typename E, int FN, int USE_MAX, int SPACING>
 __global__ void __launch_bounds__(256)
 k_seed_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParams P, const SeedItem* __restrict__ items,
             int n, double cap, double* __restrict__ partials)
 {
-    const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
-    const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
     double m = 0.0;
     const int step = (int)(gridDim.x * blockDim.x);
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
         const SeedItem it = items[i];
-        const unsigned v = it.v;
-        int c[3];
-        decode<3>(L, v, c);
-        // capacities before any flow: the doubles k_caps_tiles computed from the same image copy
-        const unsigned valid = (c[0] > 0 ? 1u : 0u) | (c[0] + 1 < L.dim[0] ? 2u : 0u) | (c[1] > 0 ? 4u : 0u) |
-                               (c[1] + 1 < L.dim[1] ? 8u : 0u) | (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
-        const double a = build_val<E>(img[v], use_max);
-        double co[6];
-        if (FN == 1 && SPACING == 0) {
-            double t6[6];
-#pragma unroll
-            for (int k = 0; k < 6; ++k) {
-                t6[k] = 0.0;
-                if ((valid >> k) & 1u) {
-                    const double b = build_val<E>(img[(unsigned)((int)v + dir_offset(L, k))], use_max);
-                    t6[k] = exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
-                }
-            }
-            exp_caps6(t6, false, valid, co);       // the general branch: the same doubles for ordinary arguments
-        } else {
-#pragma unroll
-            for (int k = 0; k < 6; ++k)
-                co[k] = ((valid >> k) & 1u)
-                            ? build_weight<FN, E>(P, a, img[(unsigned)((int)v + dir_offset(L, k))], use_max, spacing, P.spacing[k >> 1])
-                            : 0.0;
-        }
-        double lim0 = __dadd_ru(0.0, co[0]);
-        lim0 = __dadd_ru(lim0, co[1]); lim0 = __dadd_ru(lim0, co[2]); lim0 = __dadd_ru(lim0, co[3]);
-        lim0 = __dadd_ru(lim0, co[4]); lim0 = __dadd_ru(lim0, co[5]);
-        lim0 = lim0 * SOURCE_CLAMP_SLACK;
+        Residual f = residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, it.v);
+        for (int j = 0; j < it.nf; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, cap, 0.0));
+        for (int j = 0; j < it.nb; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, 0.0, cap));
+        residual_write(S, it.v, f);
+        m = __dadd_rn(m, f.dk);
+    }
+    block_sum_store(m, partials);
+}
 
-        const double tr = S.tr[v];
-        const unsigned rm = S.rmask[v];
-        double e = S.excess[v];
-        double dk = 0.0;
-        double r = 0.0;
-        if (tr > 0) {
-            r = __dsub_rn(tr, source_excess(tr, co));
-        } else if (tr < 0) {
-            const double sf = (rm & RM_SINKV) ? S.sink[v] : 0.0;
-            r = __dadd_rn(tr, sf);
-            dk = sf;
-        }
-        for (int j = 0; j < it.nf; ++j) dk = __dadd_rn(dk, add_tweights_dev(r, cap, 0.0));
-        for (int j = 0; j < it.nb; ++j) dk = __dadd_rn(dk, add_tweights_dev(r, 0.0, cap));
+// ---- general t-link folds (mgc_add_tweights_warm): add_tweights(v, src[k], snk[k]) with any finite values ----------------
+// One voxel's calls: calls order[first .. first + count) in the caller's order (order == nullptr: the single call `first`).
+struct TweightItem {
+    unsigned v;
+    int first;
+    int count;
+    int pad;
+};
 
-        unsigned nm = rm & 0x3fu;
-        double trn = 0.0;
-        if (r < 0) {
-            trn = r;
-            const double scap = -r;
-            double sf;
-            if (e >= scap) { sf = scap; e = __dsub_rn(e, scap); }
-            else { sf = e; e = 0.0; }
-            if (scap - sf > 0) nm |= RM_SINK;
-            S.sink[v] = sf;
-            nm |= RM_SINKV;
-        } else if (r > 0) {
-            double out = __dadd_ru(0.0, S.cap[0][v]);
-            out = __dadd_ru(out, S.cap[1][v]); out = __dadd_ru(out, S.cap[2][v]); out = __dadd_ru(out, S.cap[3][v]);
-            out = __dadd_ru(out, S.cap[4][v]); out = __dadd_ru(out, S.cap[5][v]);
-            const double lim = out * SOURCE_CLAMP_SLACK;
-            if (!(lim > lim0)) {
-                // the usual case (no net inflow through the n-links): push source_excess(r', c_orig) >= min(r', lim) and
-                // keep tr = r', which reads back as r' - source_excess(r', c_orig) bit for bit
-                e = __dadd_rn(e, source_excess(r, co));
-                trn = r;
-            } else {
-                const double p = r < lim ? r : lim;
-                e = __dadd_rn(e, p);
-                const double u = __dsub_rn(r, p);
-                if (u > 0) trn = __dadd_rn(u, lim0);      // reads back as (u + lim0) - lim0: u to one rounding
-            }
+// list form: key = voxel id, value = call index.  A stable radix sort of the pairs keeps a voxel's calls in call order.  An
+// id out of range or a non-finite weight sets a bit of *err (an out-of-range id gets key 0).
+__global__ void __launch_bounds__(256) k_tweights_keys(const int64_t* __restrict__ ids, const double* __restrict__ src,
+                                                       const double* __restrict__ snk, int n, int64_t n_vox,
+                                                       unsigned* __restrict__ keys, int* __restrict__ vals, int* __restrict__ err)
+{
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
+        const int64_t v = ids[i];
+        unsigned k = 0u;
+        if (v < 0 || v >= n_vox) atomicOr(err, FOLD_ERR_RANGE);
+        else k = (unsigned)v;
+        if (!isfinite(src[i]) || !isfinite(snk[i])) atomicOr(err, FOLD_ERR_NONFINITE);
+        keys[i] = k;
+        vals[i] = i;
+    }
+}
+
+// add_tweights(v, 0, 0) is an exact no-op in BK's arithmetic (the minimum is 0 and s - t gives tr back in both branches), so
+// only voxels with a call of a nonzero weight become items, in both forms.
+// list form: 1 at the first sorted key of each voxel that has such a call (order = the sorted call indices)
+__global__ void __launch_bounds__(256) k_tweights_heads(const unsigned* __restrict__ keys, const int* __restrict__ order,
+                                                       const double* __restrict__ src, const double* __restrict__ snk, int n,
+                                                       int* __restrict__ head)
+{
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
+        int h = 0;
+        if (i == 0 || keys[i] != keys[i - 1]) {
+            const int e = seed_lower_bound(keys, i, n, keys[i] + 1u);
+            for (int j = i; j < e && !h; ++j) h = (src[order[j]] != 0.0 || snk[order[j]] != 0.0) ? 1 : 0;
         }
-        S.tr[v] = trn;
-        S.excess[v] = e;
-        S.rmask[v] = (uint8_t)nm;
-        m = __dadd_rn(m, dk);
+        head[i] = h;
+    }
+}
+
+// dense form: 1 where the call has a nonzero weight
+__global__ void __launch_bounds__(256) k_tweights_dense_heads(const double* __restrict__ src, const double* __restrict__ snk,
+                                                              int n, int* __restrict__ head, int* __restrict__ err)
+{
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
+        const double s = src[i], t = snk[i];
+        if (!isfinite(s) || !isfinite(t)) atomicOr(err, FOLD_ERR_NONFINITE);
+        head[i] = (s != 0.0 || t != 0.0) ? 1 : 0;
+    }
+}
+
+// pos = inclusive sum of the heads: the head at i is item pos[i] - 1, in ascending voxel order, and ctl[0] = pos[n - 1]
+// items.  keys == nullptr: the dense form (voxel i, one call).  Each touched tile is listed once (claim_tile_once), which
+// keeps the claim list within TL.ntiles (see k_seed_items).
+__global__ void __launch_bounds__(256) k_tweights_items(Lattice L, Tiles TL, const unsigned* __restrict__ keys,
+                                                        const int* __restrict__ pos, int n, TweightItem* __restrict__ items,
+                                                        int* __restrict__ tflag, int* __restrict__ tiles, int* __restrict__ ctl)
+{
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
+        if (i == n - 1) ctl[0] = pos[i];
+        if (pos[i] == (i > 0 ? pos[i - 1] : 0)) continue;
+        unsigned v = (unsigned)i;
+        int cnt = 1;
+        if (keys) {
+            v = keys[i];
+            cnt = seed_lower_bound(keys, i, n, v + 1u) - i;
+        }
+        items[pos[i] - 1] = TweightItem{v, i, cnt, 0};
+        claim_tile_once(L, TL, v, tflag, tiles, ctl);
+    }
+}
+
+// One thread per touched voxel: r(v) read as in k_seed_fold, its calls applied in the caller's order with the reference's
+// arithmetic, r' written back.  residual_write holds for any finite r and r' (see k_seed_fold), so any weights may come.
+template <typename E, int FN, int USE_MAX, int SPACING>
+__global__ void __launch_bounds__(256)
+k_tweights_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParams P, const TweightItem* __restrict__ items,
+                int n, const int* __restrict__ order, const double* __restrict__ src, const double* __restrict__ snk,
+                double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = (int)(gridDim.x * blockDim.x);
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
+        const TweightItem it = items[i];
+        Residual f = residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, it.v);
+        for (int j = it.first; j < it.first + it.count; ++j) {
+            const int k = order ? order[j] : j;
+            f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, src[k], snk[k]));
+        }
+        residual_write(S, it.v, f);
+        m = __dadd_rn(m, f.dk);
     }
     block_sum_store(m, partials);
 }

@@ -126,7 +126,8 @@ class GCGraph:
         self.__set_terminal_nodes(sink_nodes, False)
 
     def set_tweight(self, node, weight_source, weight_sink):
-        """graph.py:462-498: add_tweights(node, weight_source, weight_sink); weights may be <= 0."""
+        """graph.py:462-498: add_tweights(node, weight_source, weight_sink); weights may be <= 0.  On a solved graph use
+        ``get_graph().add_tweights_warm``, the warm form of the same calls."""
         if node >= self.__nodes or node < 0:
             raise ValueError("Invalid node id of {}. Valid values are 0 to {}.".format(node, self.__nodes - 1))
         self.__graph.add_tweights(int(node), float(weight_source), float(weight_sink))
@@ -137,7 +138,8 @@ class GCGraph:
             self.set_tweight(node, weight[0], weight[1])
 
     def set_tweights_all(self, tweights):
-        """graph.py:532-552: one (source, sink) pair per node, in node order -- done as ONE dense device pass."""
+        """graph.py:532-552: one (source, sink) pair per node, in node order -- done as ONE dense device pass.  On a
+        solved graph use ``get_graph().add_tweights_warm(None, source, sink)``, the warm form of the same calls."""
         tw = numpy.asarray(tweights if isinstance(tweights, numpy.ndarray) else list(tweights), dtype=numpy.float64)
         if tw.ndim != 2 or tw.shape[1] != 2:
             raise ValueError("tweights must hold one (source, sink) pair per node")

@@ -7,7 +7,15 @@ configuration: a cold solve, then five strokes, each applied to a freshly solved
   line          : a foreground line through the background between the two blobs,
   both          : the two together,
   erase_line    : the line added and solved first (not timed), then erased with remove_seeds,
-  erase_markers : the foreground markers of blob 2 erased with remove_seeds.
+  erase_markers : the foreground markers of blob 2 erased with remove_seeds,
+  soft_line     : the line as a soft stroke, add_tweights_warm(line ids, 50, 0),
+  regional_box  : a GrabCut-style regional update inside a box around blob 1: add_tweights_warm(None, (p' - p) alpha,
+                  ((1 - p') - (1 - p)) alpha) for p = sigmoid((image - 50) / 15), p' = sigmoid((image - 55) / 15),
+                  alpha = 0.1, zero outside the box, as float64 CUDA tensors (config 2 has no regional term: there the
+                  same deltas are simply dense t-link calls),
+  regional_all  : the same update over the whole lattice.
+The add_tweights_warm strokes have no seed call: their cold graph is the fused build with the original markers, then the
+same calls staged before the first solve.
 Per stroke and run it prints, for the warm path: the wall time of the seed call (which returns after its device work)
 with the library's split of it into host work before anything is enqueued (ms_seeds_host) and device time (ms_seeds:
 id upload, grouping, claim + materialisation, fold, push-list fix-up); the CUDA-event span of maxflow + mask into device
@@ -50,7 +58,7 @@ def _card():
     return dict(card=name, power_limit_and_max_sm_clock=power)
 
 
-_STROKES = ("carve", "line", "both", "erase_line", "erase_markers")
+_STROKES = ("carve", "line", "both", "erase_line", "erase_markers", "soft_line", "regional_box", "regional_all")
 
 
 def main():
@@ -87,6 +95,21 @@ def main():
                    "both": ("add", line, carve, None, (vol["fg"] | line, vol["bg"] | carve)),
                    "erase_line": ("remove", line, None, line, (vol["fg"], vol["bg"])),
                    "erase_markers": ("remove", blob2, None, None, (vol["fg"] & ~blob2, vol["bg"]))}
+        # add_tweights_warm strokes: (ids or None, src, snk); the regional deltas are built lazily on the device
+        def regional(box):
+            img = d_img.double()
+            p = torch.sigmoid((img - 50.0) / 15.0)
+            p2 = torch.sigmoid((img - 55.0) / 15.0)
+            src, snk = (p2 - p) * 0.1, ((1.0 - p2) - (1.0 - p)) * 0.1
+            if box:
+                keep = torch.zeros(shape, dtype=torch.bool, device="cuda")
+                keep[tuple(slice(int(0.15 * n), int(0.45 * n)) for _ in shape)] = True
+                src, snk = torch.where(keep, src, 0.0), torch.where(keep, snk, 0.0)
+            return None, src.contiguous(), snk.contiguous()
+        warm_calls = {"soft_line": lambda: (numpy.flatnonzero(line), 50.0, 0.0),
+                      "regional_box": lambda: regional(True), "regional_all": lambda: regional(False)}
+        for k in warm_calls:
+            strokes[k] = ("tweights", None, None, None, (vol["fg"], vol["bg"]))
         strokes = {k: strokes[k] for k in names}
         d_mask = torch.empty(shape, dtype=torch.uint8, device="cuda")
 
@@ -103,6 +126,9 @@ def main():
             bg_ids = numpy.flatnonzero(sbg) if sbg is not None else numpy.zeros(0, numpy.int64)
             d_fg0, d_bg0 = dev(vol["fg"]), dev(vol["bg"])
             d_fg2, d_bg2 = dev(cfg), dev(cbg)
+            tw = warm_calls[sname]() if call == "tweights" else None
+            if tw is not None and tw[0] is not None:
+                fg_ids = tw[0]
             for run in range(args.runs):
                 # warm: a freshly solved graph (with the strokes to be erased added and solved), then the stroke
                 g = build(d_fg0, d_bg0)
@@ -113,7 +139,10 @@ def main():
                 torch.cuda.synchronize()
                 s0 = dict(g.stats())
                 t0 = time.perf_counter()
-                getattr(g, call + "_seeds")(fg_ids, bg_ids)     # returns after its device work finished
+                if tw is not None:
+                    g.add_tweights_warm(*tw)                    # returns after its device work finished
+                else:
+                    getattr(g, call + "_seeds")(fg_ids, bg_ids)
                 t1 = time.perf_counter()
                 ev0.record(stream)
                 e_warm = g.maxflow()
@@ -131,6 +160,8 @@ def main():
                 torch.cuda.synchronize()
                 ev0.record(stream)
                 gc_ = build(d_fg2, d_bg2)
+                if tw is not None:
+                    gc_.add_tweights_warm(*tw)                  # staged before the first solve
                 e_cold = gc_.maxflow()
                 gc_._nat().get_mask_into(d_mask.data_ptr())
                 ev1.record(stream)
@@ -140,7 +171,8 @@ def main():
                 del gc_
                 d = {k: s1[k] - s0.get(k, 0.0) for k in ("ms_seeds", "ms_seeds_host", "ms_solve", "ms_relabel", "ms_push",
                                                           "ms_caps", "ms_readout", "push_sweeps", "global_relabels")}
-                row = dict(config=name, n=n, stroke=sname, call=call, run=run, seeds=int(fg_ids.size + bg_ids.size),
+                row = dict(config=name, n=n, stroke=sname, call=call, run=run,
+                           seeds=int(n ** 3 if tw is not None and tw[0] is None else fg_ids.size + bg_ids.size),
                            seed_call_wall_ms=(t1 - t0) * 1e3, solve_span_ms=solve_span,
                            warm_wall_ms_host_ids_to_device_mask=(t2 - t0) * 1e3,
                            warm_wall_ms_host_ids_to_host_mask=wall, cold_span_ms=cold_dev,
