@@ -136,6 +136,9 @@ int mgc_trim_pools(void);
  * markers, maxflow, mgc_check).  graph_from_voxels switches it on because it always adds the markers right after the
  * boundary term, which lets the marker upload overlap the stencil kernel. */
 #define MGC_OPT_DEFER_WEIGHT_CHECK 1
+/* MGC_OPT_WARM (default 0; 1 switches it on): warm re-solves (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm) on
+ * handles the lazy fused build did not build -- see mgc_add_seeds. */
+#define MGC_OPT_WARM 2
 int mgc_set_option(mgc_graph* g, int32_t option, int64_t value);
 /* Deliver a deferred verdict now (MGC_OK / MGC_E_WEIGHT). */
 int mgc_check(mgc_graph* g);
@@ -233,7 +236,18 @@ int mgc_maxflow(mgc_graph* g, double* energy);
  * (mgc_build_voxel_graph on a 1-D..3-D lattice with a boundary term, tile solver, not a z-slab, lazy capacities on): the
  * fold recomputes capacities from the copies that build keeps.  Elsewhere reset() and a rebuild with the seeds is the way.
  * mgc_add_tweights_dense / mgc_add_markers and the other term entry points still refuse a solved graph.  Adding this
- * entry point left MGC_ABI_VERSION at 3: nothing that existed changed. */
+ * entry point left MGC_ABI_VERSION at 3: nothing that existed changed.
+ * MGC_OPT_WARM = 1 (mgc_set_option) extends these folds to every other tile-solver handle of one GPU: 4-D lattices,
+ * 1-D..3-D graphs built term by term, and the eager fused build (lazy capacities off).  Such a handle keeps no copy of its
+ * inputs, so its first solve records the residual source capacity of every voxel in place of the net t-link, before the
+ * first push (a pass over tr and the capacities after the eager fused build; nothing extra on the per-term path).
+ *   - Set it before the first solve: while no flow has started (a handle fresh from create / mgc_reset / a build).  Later
+ *     it returns MGC_E_STATE, except on a lazily built handle, where it changes nothing.
+ *   - It persists across mgc_reset, like MGC_OPT_DEFER_WEIGHT_CHECK, and changes neither results nor the first solve's
+ *     mask and energy.
+ *   - A fold on such a handle before its first solve initialises the solver state and takes the record first.
+ *   - The per-voxel solver (MEDPY_GC_SOLVER=v0) and z-slab handles still return MGC_E_STATE with the option set.
+ * MGC_ABI_VERSION stays 3 and mgc_stats keeps its layout. */
 int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
 /* Seeds erased from a graph and solved warm: the inverse call of mgc_add_seeds, as the reference erases a seed
  * (add_tweights accepts negative capacities, graph.h:415-425).  The meaning is exactly add_tweights(v, -65535, 0) for

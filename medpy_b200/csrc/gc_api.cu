@@ -172,7 +172,12 @@ struct mgc_graph {
     // mgc_add_tweights_warm may fold t-link calls into the residual state.  Unlike caps_lazy this stays true once every
     // tile is materialised (hard instances).
     bool lazy_built = false;
-    int* cmat = nullptr;               // per tile: push state materialised since the last lazy build
+    // MGC_OPT_WARM: the other tile-solver handles (eager fused build, per-term path, 4-D lattices) record their residual
+    // source capacities in tr at the first solve, which lets the same folds work on them (gc_seeds.cuh).  Kept across
+    // mgc_reset, like defer_check.
+    bool warm_opt = false;
+    bool warm_state = false;           // tr holds BK's residual source capacity: recorded since the last init
+    int* cmat = nullptr;              // per tile: push state materialised since the last lazy build
     int* caps_list = nullptr;          // tiles claimed by the current materialiser launch
     // The copies below (with caps_P and caps_tin) live as long as the handle's last lazy build: besides the materialiser,
     // the seed folds depend on them -- they recompute a seeded voxel's capacities before any flow from img_copy to know
@@ -441,6 +446,7 @@ void invalidate(mgc_graph* g)
 {
     g->lazy_built = false;             // terms changed outside the lazy build
     g->state_init = false;
+    g->warm_state = false;
     g->solved = false;
     g->host_mask_valid = false;
 }
@@ -1039,6 +1045,9 @@ int dirty_clear(mgc_graph* g)
     return MGC_OK;
 }
 
+// MGC_OPT_WARM applies: a tile-solver handle of one GPU whose state does not come from the lazy fused build
+bool warm_wanted(const mgc_graph* g) { return g->warm_opt && g->use_tiles && !g->slab && !g->lazy_built; }
+
 // first call: solver state + first labels + first worklists in one pass (k_init_tile)
 int init_tiles(mgc_graph* g)
 {
@@ -1046,13 +1055,20 @@ int init_tiles(mgc_graph* g)
     { int rc0 = push_state_all(g); if (rc0) return rc0; }       // k_init_tile reads every capacity
     CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
     g->pl_sel[0] = g->pl_sel[1] = 0;
+    const bool warm = warm_wanted(g);      // tr > 0 becomes the residual source capacity (gc_seeds.cuh)
     cudaEventRecord(g->ev[4], g->stream);
-    if (g->nd == 4)
-        k_init_tile4<double><<<g->TL4.ntiles, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->smask, g->rflag, rl(g, 0), g->pflag,
+    if (g->nd == 4) {
+        if (warm) k_init_tile4<double, true><<<g->TL4.ntiles, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->smask, g->rflag, rl(g, 0),
+                                                                                     g->pflag, pl(g, 0, 0), pl(g, 1, 0));
+        else k_init_tile4<double><<<g->TL4.ntiles, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->smask, g->rflag, rl(g, 0), g->pflag,
+                                                                           pl(g, 0, 0), pl(g, 1, 0));
+    } else if (warm) {
+        k_init_tile<double, true><<<g->TL.ntiles, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->rflag, rl(g, 0), g->pflag,
+                                                                            pl(g, 0, 0), pl(g, 1, 0));
+    } else {
+        k_init_tile<double><<<g->TL.ntiles, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->rflag, rl(g, 0), g->pflag,
                                                                       pl(g, 0, 0), pl(g, 1, 0));
-    else
-    k_init_tile<double><<<g->TL.ntiles, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->rflag, rl(g, 0), g->pflag,
-                                                                  pl(g, 0, 0), pl(g, 1, 0));
+    }
     cudaEventRecord(g->ev[5], g->stream);
     g->init_timed = true;
     g->st.kernel_launches++;
@@ -1061,7 +1077,36 @@ int init_tiles(mgc_graph* g)
     g->labels_fresh = true;
     g->rl_cur = 0;
     g->sweep_mode = -1;
+    if (warm) {
+        g->warm_state = true;
+        g->flow_started = true;        // tr no longer holds the terms: no term may be added on top of it
+    }
     return dirty_clear(g);
+}
+
+// MGC_OPT_WARM: put tr into BK's representation before the first push (a no-op where it is already, or where the option
+// does not apply).  The per-term path does it in k_init_tile; after the eager fused build, which wrote the state before
+// the option could be read, k_warm_convert does it in a pass of its own (8 B of tr read per voxel, plus the six capacities
+// and the write of tr where tr > 0).
+int warm_prepare(mgc_graph* g)
+{
+    if (!warm_wanted(g) || g->warm_state) return MGC_OK;
+    if (g->flow_started) FAIL(MGC_E_STATE, "MGC_OPT_WARM was set after the first solve: reset() the graph and rebuild it");
+    // no push has run: a 4-D init (the only other source of 4-D state) is simply run again, recording this time
+    if (!g->state_init || g->nd == 4) {
+        int rc = materialise_zeros(g);
+        if (rc) return rc;
+        return init_tiles(g);
+    }
+    Nvtx range("mgc:warm_convert");
+    unsigned grid = nblocks(g);
+    if (grid > (unsigned)g->n_ctas * 8u) grid = (unsigned)g->n_ctas * 8u;
+    k_warm_convert<<<grid, 256, 0, g->stream>>>(g->L, g->S);
+    g->st.kernel_launches++;
+    CK(cudaGetLastError());
+    g->warm_state = true;
+    g->flow_started = true;
+    return MGC_OK;
 }
 
 // exact global relabel by tile-wise relaxation; work is proportional to the tiles whose labels still move.
@@ -1997,6 +2042,15 @@ int mgc_set_option(mgc_graph* g, int32_t option, int64_t value)
 {
     if (!g) return MGC_E_ARG;
     if (option == MGC_OPT_DEFER_WEIGHT_CHECK) { g->defer_check = value != 0; return MGC_OK; }
+    if (option == MGC_OPT_WARM) {
+        // the record is taken before the first push; a lazily built handle folds without it, so there it changes nothing now
+        const bool on = value != 0;
+        if (on != g->warm_opt && g->flow_started && !g->lazy_built)
+            FAIL(MGC_E_STATE, "MGC_OPT_WARM is set before the first solve (the residual source capacities are recorded at "
+                              "its start): reset() the handle and rebuild the graph to change it");
+        g->warm_opt = on;
+        return MGC_OK;
+    }
     FAIL(MGC_E_ARG, "unknown option");
 }
 
@@ -2334,6 +2388,7 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     g->tr_fresh = false;
     g->caps_lazy = lazy;
     g->lazy_built = lazy;
+    g->warm_state = false;
     g->st.seed_folds = 0;
     g->st.ms_seeds = 0.0;
     g->st.ms_seeds_host = 0.0;
@@ -2412,6 +2467,7 @@ int mgc_maxflow(mgc_graph* g, double* energy)
         Timer t(g, &g->st.ms_solve);
         int rc = MGC_OK;
         if (g->use_tiles) {
+            rc = warm_prepare(g); if (rc) return rc;
             if (g->debug_checks) {
                 rc = materialise_zeros(g); if (rc) return rc;
                 if (!g->state_init) { rc = init_tiles(g); if (rc) return rc; }
@@ -2516,14 +2572,16 @@ static int seed_cub_launches(mgc_graph* g, int kind, int n, int end_bit, void* t
     return MGC_OK;
 }
 
-// preconditions of every fold into the residual state (the copies of the lazy fused build are what the fold reads)
-static int warm_check(mgc_graph* g)
+// preconditions of every fold into the residual state: the copies of the lazy fused build are what the fold reads, or
+// (MGC_OPT_WARM, *eager = true) the residual source capacities the first solve records in tr on any other tile-solver handle
+static int warm_check(mgc_graph* g, bool* eager)
 {
-    if (!g->lazy_built || !g->state_init || g->slab || !g->use_tiles || g->nd != 3)
-        FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
-                          "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
-                          "the seeds instead");
-    return MGC_OK;
+    *eager = false;
+    if (!g->slab && g->use_tiles && g->lazy_built && g->state_init && g->nd == 3) return MGC_OK;
+    if (warm_wanted(g)) { *eager = true; return MGC_OK; }
+    FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
+                      "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
+                      "the seeds instead");
 }
 
 // The steps of a fold after its grouping, shared by seeds_fold and mgc_add_tweights_warm.  The grouping was enqueued after
@@ -2540,6 +2598,13 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     if (h_ctl[1] & FOLD_ERR_NONFINITE) FAIL(MGC_E_ARG, "a t-link weight is NaN or infinite");
     const int ni = h_ctl[0];
     if (ni == 0) return MGC_OK;                // only add_tweights(v, 0, 0) calls: the state, mask and energy stay
+    const bool eager = !g->lazy_built;         // MGC_OPT_WARM handle (warm_check passed)
+    if (eager) {
+        // not solved yet: the init and the record of the residual source capacities come first, so the fold reads the
+        // same representation as after a solve
+        int rc = warm_prepare(g);
+        if (rc) return rc;
+    }
     CK(cudaEventRecord(g->ev_seed[2], g->stream));
     // 1. every touched voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
     if (g->caps_lazy) {
@@ -2559,15 +2624,18 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     if (grid > REDUCE_BLOCKS) grid = REDUCE_BLOCKS;
     fold(grid, ni);
     k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, grid, g->d_scalars);
-    // 3. solver state for the next solve: fresh push lists over every materialised tile with excess; labels from a full
-    // relabel reset (sweep_mode = -1: a fold can remove a sink link, so the last solve's labels bound nothing)
+    // 3. solver state for the next solve: fresh push lists over every materialised tile with excess (every tile of an
+    // eager handle; TL.ntiles is the 4-D tile count on a 4-D handle); labels from a full relabel reset (sweep_mode = -1: a
+    // fold can remove a sink link, so the last solve's labels bound nothing)
     CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
     CK(cudaMemsetAsync(g->pflag, 0, (size_t)g->TL.ntiles * sizeof(int), g->stream));
     g->pl_sel[0] = g->pl_sel[1] = 0;
     {
         unsigned lgrid = (unsigned)g->n_ctas * 4u;
         if (lgrid > (unsigned)g->TL.ntiles) lgrid = (unsigned)g->TL.ntiles;
-        k_seed_lists<<<lgrid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->cmat, g->pflag, pl(g, 0, 0), pl(g, 1, 0));
+        if (g->nd == 4) k_seed_lists4<<<lgrid, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->pflag, pl(g, 0, 0), pl(g, 1, 0));
+        else k_seed_lists<<<lgrid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, eager ? nullptr : g->cmat, g->pflag,
+                                                             pl(g, 0, 0), pl(g, 1, 0));
     }
     g->st.kernel_launches += 3;
     CK(cudaGetLastError());
@@ -2599,7 +2667,8 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
     if (n_fg < 0 || n_bg < 0 || (n_fg && !fg_ids) || (n_bg && !bg_ids)) FAIL(MGC_E_ARG, "bad seed lists");
     if (n_fg + n_bg > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 seeds in one call");
     if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
-    { int rc0 = warm_check(g); if (rc0) return rc0; }
+    bool eager = false;
+    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
     if (n_fg + n_bg == 0) return MGC_OK;       // nothing to fold: the solved state, mask and energy stay as they are
@@ -2614,9 +2683,10 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
                                       g->stream));
     CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
     // device layout (16-byte aligned pieces): [item count | error flag | seeded-tile count | pad] [host ids] [keys]
-    // [sorted keys] [run heads] [run positions] [per-tile flags] [seeded tiles] [items] [cub scratch]
+    // [sorted keys] [run heads] [run positions] [per-tile flags] [seeded tiles] [items] [cub scratch]; no tiles on an eager
+    // handle (nothing to claim)
     auto al = [](size_t b) { return (b + 15) / 16 * 16; };
-    const size_t ntl = (size_t)g->TL.ntiles;
+    const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
     const size_t ids_off = 16;
     const size_t keys_off = ids_off + (mem == MGC_MEM_HOST ? al((size_t)n * 8) : 0);
     const size_t skeys_off = keys_off + al((size_t)n * 4);
@@ -2669,11 +2739,16 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
         k_seed_heads<<<kgrid, 256, 0, g->stream>>>(skeys, n, head);
         tb = tmp_bytes;
         CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
-        k_seed_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, skeys, pos, n, d_items, tflag, tiles, d_count);
+        k_seed_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, skeys, pos, n, d_items, eager ? nullptr : tflag, tiles, d_count);
         g->st.kernel_launches += 3 + cub_launches;
         CK(cudaGetLastError());
     }
     return fold_items(g, d_count, tiles, [&](unsigned grid, int ni) {
+        if (eager) {
+            if (g->nd == 4) k_seed_fold_eager<4><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, cap, g->partials);
+            else            k_seed_fold_eager<3><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, cap, g->partials);
+            return;
+        }
         switch (g->caps_dtype) {
             case MGC_F32: seed_fold_launch_t<float>(g, grid, d_items, ni, cap); break;
             case MGC_F64: seed_fold_launch_t<double>(g, grid, d_items, ni, cap); break;
@@ -2700,7 +2775,8 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
     if (count < 0 || (count && (!src || !snk))) FAIL(MGC_E_ARG, "bad t-link arrays");
     if (count > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 add_tweights calls in one call");
     if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
-    { int rc0 = warm_check(g); if (rc0) return rc0; }
+    bool eager = false;
+    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
     const bool dense = ids == nullptr;
     if (dense && count && count != (int64_t)g->L.n) FAIL(MGC_E_ARG, "the dense form takes one weight pair per voxel");
     CK(cudaSetDevice(g->device));
@@ -2720,9 +2796,9 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
     CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
     // device layout (16-byte aligned pieces): [item count | error bits | touched-tile count | pad] [host ids] [host src]
     // [host snk] [keys] [sorted keys] [call indices] [sorted call indices] [heads] [positions] [per-tile flags]
-    // [touched tiles] [items] [cub scratch]; no ids, keys or call indices in the dense form
+    // [touched tiles] [items] [cub scratch]; no ids, keys or call indices in the dense form, no tiles on an eager handle
     auto al = [](size_t b) { return (b + 15) / 16 * 16; };
-    const size_t ntl = (size_t)g->TL.ntiles;
+    const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
     const bool host = mem == MGC_MEM_HOST;
     const size_t w4 = dense ? 0 : al((size_t)n * 4);
     const size_t ids_off = 16;
@@ -2789,13 +2865,18 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
             tb = tmp_bytes;
         }
         CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
-        k_tweights_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, dense ? nullptr : skeys, pos, n, d_items, tflag, tiles,
-                                                       d_ctl);
+        k_tweights_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, dense ? nullptr : skeys, pos, n, d_items,
+                                                       eager ? nullptr : tflag, tiles, d_ctl);
         g->st.kernel_launches += (dense ? 2 : 3) + cub_launches;
         CK(cudaGetLastError());
     }
     const int* order = dense ? nullptr : svals;
     return fold_items(g, d_ctl, tiles, [&](unsigned grid, int ni) {
+        if (eager) {
+            if (g->nd == 4) k_tweights_fold_eager<4><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, order, d_src, d_snk, g->partials);
+            else            k_tweights_fold_eager<3><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, order, d_src, d_snk, g->partials);
+            return;
+        }
         switch (g->caps_dtype) {
             case MGC_F32: tweights_fold_launch_t<float>(g, grid, d_items, ni, order, d_src, d_snk); break;
             case MGC_F64: tweights_fold_launch_t<double>(g, grid, d_items, ni, order, d_src, d_snk); break;

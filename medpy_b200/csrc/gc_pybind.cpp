@@ -627,6 +627,7 @@ PYBIND11_MODULE(_mgc, m)
     m.attr("SOURCE") = MGC_SOURCE;
     m.attr("SINK") = MGC_SINK;
     m.attr("OPT_DEFER_WEIGHT_CHECK") = MGC_OPT_DEFER_WEIGHT_CHECK;
+    m.attr("OPT_WARM") = MGC_OPT_WARM;
     m.attr("LABELS_ADJACENCY") = MGC_LABELS_ADJACENCY;
     m.attr("LABELS_STAWIASKI") = MGC_LABELS_STAWIASKI;
     m.attr("LABELS_STAWIASKI_DIRECTED") = MGC_LABELS_STAWIASKI_DIRECTED;

@@ -19,8 +19,12 @@
 // mgc_add_tweights_warm runs the same steps with a value per call: its own grouping (k_tweights_keys / _heads / _items for a
 // call list, k_tweights_dense_heads / k_tweights_items for one call per voxel) and k_tweights_fold, which shares the read of
 // r(v) and the write-back of r' with k_seed_fold (residual_read / residual_write).
+// Handles that were not built lazily (the eager fused build, the per-term path, every 4-D lattice) fold with the same
+// grouping, no claim and k_seed_fold_eager / k_tweights_fold_eager, once MGC_OPT_WARM had the first solve record their
+// residual source capacities (the end of this file).
 #pragma once
 #include "gc_build.cuh"
+#include "gc_tiles4.cuh"
 
 // one seeded voxel: `nf` foreground seeds, then `nb` background seeds (list order of the reference: every fg id first)
 struct SeedItem {
@@ -91,7 +95,7 @@ __global__ void __launch_bounds__(256) k_seed_items(Lattice L, Tiles TL, const u
         const int s = seed_lower_bound(keys, i, n, 2u * v + 1u);
         const int e = seed_lower_bound(keys, s, n, 2u * v + 2u);
         items[pos[i] - 1] = SeedItem{v, s - i, e - s, 0};
-        claim_tile_once(L, TL, v, tflag, tiles, ctl);
+        if (tflag) claim_tile_once(L, TL, v, tflag, tiles, ctl);      // tflag == nullptr: eager handle, nothing to claim
     }
 }
 
@@ -304,7 +308,8 @@ __global__ void __launch_bounds__(256) k_tweights_dense_heads(const double* __re
 
 // pos = inclusive sum of the heads: the head at i is item pos[i] - 1, in ascending voxel order, and ctl[0] = pos[n - 1]
 // items.  keys == nullptr: the dense form (voxel i, one call).  Each touched tile is listed once (claim_tile_once), which
-// keeps the claim list within TL.ntiles (see k_seed_items).
+// keeps the claim list within TL.ntiles (see k_seed_items); tflag == nullptr lists no tiles (eager and 4-D handles: every
+// voxel already holds its push state, and TL does not describe a 4-D lattice).
 __global__ void __launch_bounds__(256) k_tweights_items(Lattice L, Tiles TL, const unsigned* __restrict__ keys,
                                                         const int* __restrict__ pos, int n, TweightItem* __restrict__ items,
                                                         int* __restrict__ tflag, int* __restrict__ tiles, int* __restrict__ ctl)
@@ -319,7 +324,7 @@ __global__ void __launch_bounds__(256) k_tweights_items(Lattice L, Tiles TL, con
             cnt = seed_lower_bound(keys, i, n, v + 1u) - i;
         }
         items[pos[i] - 1] = TweightItem{v, i, cnt, 0};
-        claim_tile_once(L, TL, v, tflag, tiles, ctl);
+        if (tflag) claim_tile_once(L, TL, v, tflag, tiles, ctl);
     }
 }
 
@@ -349,13 +354,160 @@ k_tweights_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryP
 // push lists after a fold: every materialised tile (cmat[t] = 1) holding an owned voxel with excess goes on the list its
 // colour consumes next.  Excess stranded at voxels the last solve labelled HINF may reach a new sink link now; only
 // materialised tiles can hold excess (mgc_add_seeds first materialises every tile whose source excess is still implicit).
+// cmat == nullptr: an eager handle, every tile holds explicit state.
 __global__ void __launch_bounds__(TILE_VOX) k_seed_lists(Lattice L, Tiles TL, State<double> S, const int* __restrict__ cmat,
                                                          int* __restrict__ pflag, WorkList pl0, WorkList pl1)
 {
     for (int t = blockIdx.x; t < TL.ntiles; t += gridDim.x) {
-        if (cmat[t] == 0) continue;            // block-uniform
+        if (cmat && cmat[t] == 0) continue;    // block-uniform
         const TileCtx c = tile_ctx(L, TL, t);
         const int act = (c.own && S.excess[c.v] > 0) ? 1 : 0;
         if (__syncthreads_or(act) && threadIdx.x == 0) list_push(pflag, tile_color(c) ? pl1 : pl0, t);
+    }
+}
+
+// ---- eager and 4-D handles (MGC_OPT_WARM) -------------------------------------------------------------------------------
+// A handle that was not built lazily keeps no copy of its inputs, and cap[] holds residuals after the first push, so the
+// source flow its state holds cannot be recomputed as residual_read does.  With MGC_OPT_WARM the first solve records it
+// instead, before any push: tr > 0 becomes tr - e0, e0 = the source excess of the init (k_init_tile<T, true> /
+// k_init_tile4<T, true> on the per-term path, k_warm_convert after the eager fused build).  tr then holds BK's own residual
+// source capacity; once the excess is set nothing but these folds reads tr > 0 (DESIGN.md §4.6).
+//   read : r = tr                  for tr > 0;
+//          r = tr + absorbed       for tr < 0 (absorbed = sink[v] under RM_SINKV in 3-D; k_init_tile4 zeroes sink[], so
+//                                  a 4-D voxel always holds it), moved into the add_tweights constant as in residual_read;
+//          r = 0                   for tr = 0.
+//   write: r' < 0 : as residual_write (a fresh sink link that takes the voxel's own excess at once);
+//          r' > 0 : p = min(r', residual out-capacity rounded up x SOURCE_CLAMP_SLACK) joins the excess (r' itself when that
+//                   sum is NaN, as in source_excess) and tr = r' - p, which the next fold reads back as the residual;
+//          r' = 0 : tr = 0.
+// 3-D state: 6 arcs, the sink-link bits RM_SINK / RM_SINKV in rmask.  4-D state: 8 arcs in rmask, the sink-residual bit in
+// smask, and sink[] summed over every voxel by the read-out (so a voxel without a sink link gets sink[v] = 0).
+struct EagerResidual {
+    double r;         // r(v)
+    double dk;        // change of the add_tweights constant
+    double e;         // excess
+    unsigned rm;      // rmask
+};
+
+template <int ND>
+__device__ __forceinline__ EagerResidual eager_read(const State<double>& S, unsigned v)
+{
+    EagerResidual f;
+    const double tr = S.tr[v];
+    f.rm = S.rmask[v];
+    f.e = S.excess[v];
+    f.dk = 0.0;
+    f.r = 0.0;
+    if (tr > 0) {
+        f.r = tr;
+    } else if (tr < 0) {
+        const double sf = (ND == 4 || (f.rm & RM_SINKV)) ? S.sink[v] : 0.0;
+        f.r = __dadd_rn(tr, sf);
+        f.dk = sf;
+    }
+    return f;
+}
+
+template <int ND>
+__device__ __forceinline__ void eager_write(const State<double>& S, uint8_t* __restrict__ smask, unsigned v,
+                                            const EagerResidual& f)
+{
+    const double r = f.r;
+    double e = f.e;
+    double trn = 0.0, sf = 0.0;
+    bool sres = false;
+    if (r < 0) {
+        trn = r;
+        const double scap = -r;
+        if (e >= scap) { sf = scap; e = __dsub_rn(e, scap); }
+        else { sf = e; e = 0.0; }
+        sres = scap - sf > 0;
+    } else if (r > 0) {
+        double out = 0.0;
+#pragma unroll
+        for (int k = 0; k < 2 * ND; ++k) out = __dadd_ru(out, S.cap[k][v]);
+        const double lim = out * SOURCE_CLAMP_SLACK;
+        double p = r < lim ? r : lim;
+        if (!(out == out)) p = r;
+        e = __dadd_rn(e, p);
+        trn = __dsub_rn(r, p);
+    }
+    S.tr[v] = trn;
+    S.excess[v] = e;
+    if (ND == 3) {
+        unsigned nm = f.rm & 0x3fu;
+        if (r < 0) {
+            S.sink[v] = sf;
+            nm |= RM_SINKV | (sres ? RM_SINK : 0u);
+        }
+        S.rmask[v] = (uint8_t)nm;
+    } else {
+        S.sink[v] = sf;
+        smask[v] = sres ? 1 : 0;
+    }
+}
+
+template <int ND>
+__global__ void __launch_bounds__(256)
+k_seed_fold_eager(State<double> S, uint8_t* __restrict__ smask, const SeedItem* __restrict__ items, int n, double cap,
+                  double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = (int)(gridDim.x * blockDim.x);
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
+        const SeedItem it = items[i];
+        EagerResidual f = eager_read<ND>(S, it.v);
+        for (int j = 0; j < it.nf; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, cap, 0.0));
+        for (int j = 0; j < it.nb; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, 0.0, cap));
+        eager_write<ND>(S, smask, it.v, f);
+        m = __dadd_rn(m, f.dk);
+    }
+    block_sum_store(m, partials);
+}
+
+template <int ND>
+__global__ void __launch_bounds__(256)
+k_tweights_fold_eager(State<double> S, uint8_t* __restrict__ smask, const TweightItem* __restrict__ items, int n,
+                      const int* __restrict__ order, const double* __restrict__ src, const double* __restrict__ snk,
+                      double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = (int)(gridDim.x * blockDim.x);
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
+        const TweightItem it = items[i];
+        EagerResidual f = eager_read<ND>(S, it.v);
+        for (int j = it.first; j < it.first + it.count; ++j) {
+            const int k = order ? order[j] : j;
+            f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, src[k], snk[k]));
+        }
+        eager_write<ND>(S, smask, it.v, f);
+        m = __dadd_rn(m, f.dk);
+    }
+    block_sum_store(m, partials);
+}
+
+// the eager fused build (k_build_tile<..., LAZY = 0>) wrote tr and the excess before MGC_OPT_WARM could be set: the same
+// record as k_init_tile<T, true>, as a pass of its own at the first solve, before any push.  The capacity planes still hold
+// the build's weights, so source_excess gives the build's e0 bit for bit.
+__global__ void __launch_bounds__(256) k_warm_convert(Lattice L, State<double> S)
+{
+    for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < L.n; v += gridDim.x * blockDim.x) {
+        const double tr = S.tr[v];
+        if (tr > 0) {
+            const double c[6] = {S.cap[0][v], S.cap[1][v], S.cap[2][v], S.cap[3][v], S.cap[4][v], S.cap[5][v]};
+            S.tr[v] = __dsub_rn(tr, source_excess(tr, c));
+        }
+    }
+}
+
+// push lists after a fold on a 4-D handle (cf. k_seed_lists): every tile holding an owned voxel with excess goes on the
+// list its colour (4-D checkerboard parity) consumes next
+__global__ void __launch_bounds__(T4_VOX) k_seed_lists4(Lattice L, Tiles4 TL, State<double> S, int* __restrict__ pflag,
+                                                        WorkList pl0, WorkList pl1)
+{
+    for (int t = blockIdx.x; t < TL.ntiles; t += gridDim.x) {
+        const Tile4Ctx c = tile4_ctx(L, TL, t);
+        const int act = (c.own && S.excess[c.v] > 0) ? 1 : 0;
+        if (__syncthreads_or(act) && threadIdx.x == 0) list_push(pflag, tile4_color(c) ? pl1 : pl0, t);
     }
 }

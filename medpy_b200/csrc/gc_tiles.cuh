@@ -152,8 +152,10 @@ __device__ __forceinline__ int fetch_tile(const WorkList& cur, int* __restrict__
 //   rmask, first labels (1 where a sink link exists, else HINF)
 //   relabel worklist <- tiles holding an unlabelled voxel with residual out-arcs
 //   push worklists   <- tiles holding a voxel with excess
+// WARM (MGC_OPT_WARM): tr > 0 becomes tr - excess, BK's residual source capacity, which a later fold reads back as r(v)
+// (gc_seeds.cuh).  Nothing else reads tr > 0 once the excess is set.
 // ---------------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, bool WARM = false>
 __global__ void __launch_bounds__(TILE_VOX) k_init_tile(Lattice L, Tiles TL, State<T> S, int* __restrict__ rflag, WorkList rl,
                                                         int* __restrict__ pflag, WorkList pl0, WorkList pl1)
 {
@@ -173,6 +175,7 @@ __global__ void __launch_bounds__(TILE_VOX) k_init_tile(Lattice L, Tiles TL, Sta
         if (tr > 0) { const double lim = out * SOURCE_CLAMP_SLACK; e = tr < lim ? tr : lim; if (!(out == out)) e = tr; }
         if (tr < 0) m |= RM_SINK;
         if (!c.own) e = 0.0;
+        if (WARM && tr > 0) S.tr[c.v] = (T)(tr - e);
         S.excess[c.v] = (T)e;
         S.rmask[c.v] = (uint8_t)m;          // RM_SINKV clear: sink[v] counts as 0 without being written
         const int h = (c.own && tr < 0) ? 1 : MGC_HINF;

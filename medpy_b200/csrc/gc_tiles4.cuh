@@ -98,9 +98,9 @@ __device__ __forceinline__ int load_heights4(const Lattice& L, const Tile4Ctx& c
 }
 
 // ---------------------------------------------------------------------------------------------------
-// init (cf. k_init_tile)
+// init (cf. k_init_tile; WARM: tr > 0 becomes tr - excess, BK's residual source capacity)
 // ---------------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, bool WARM = false>
 __global__ void __launch_bounds__(T4_VOX) k_init_tile4(Lattice L, Tiles4 TL, State<T> S, uint8_t* __restrict__ smask,
                                                        int* __restrict__ rflag, WorkList rl, int* __restrict__ pflag,
                                                        WorkList pl0, WorkList pl1)
@@ -120,6 +120,7 @@ __global__ void __launch_bounds__(T4_VOX) k_init_tile4(Lattice L, Tiles4 TL, Sta
         double e = 0.0;
         if (tr > 0) { const double lim = out * SOURCE_CLAMP_SLACK; e = tr < lim ? tr : lim; if (!(out == out)) e = tr; }
         if (!c.own) e = 0.0;
+        if (WARM && tr > 0) S.tr[c.v] = (T)(tr - e);
         S.excess[c.v] = (T)e;
         S.sink[c.v] = (T)0;
         S.rmask[c.v] = (uint8_t)m;

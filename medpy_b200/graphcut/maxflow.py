@@ -72,6 +72,7 @@ class GraphDouble:
         self._offlattice = None
         self._pending = []
         self._defer_weight_check = False
+        self._warm = False       # enable_warm(): MGC_OPT_WARM, set on the native handle when it is created
         # whole-lattice terms collected while graph_from_voxels runs (regional, boundary, markers): handed to the device
         # in ONE native call (mgc_build_voxel_graph: single-pass fused build) when the markers arrive or anything else
         # needs the graph.  Only while nothing has reached the device yet (_fresh).
@@ -120,7 +121,32 @@ class GraphDouble:
             self._native = _lib.Graph(list(self._shape), self._device)
             if self._defer_weight_check:
                 self._native.set_option(_lib._mgc.OPT_DEFER_WEIGHT_CHECK, 1)
+            if self._warm:
+                self._native.set_option(_lib._mgc.OPT_WARM, 1)
         return self._native
+
+    def enable_warm(self):
+        """Let ``add_seeds``, ``remove_seeds`` and ``add_tweights_warm`` fold into this graph after ``maxflow()`` although
+        the lazy fused build did not make it: a 4-D graph, a graph built term by term (element-wise calls,
+        ``add_nweights_dense``, ``add_regional_probability`` / ``add_boundary`` / ``add_markers``) or by the eager fused
+        build (``MEDPY_GC_LAZY_CAPS=0``).
+
+        Call it before the first ``maxflow()`` -- the graph ``graph_from_voxels`` returns is built but not solved yet, so
+        ``g = graph_from_voxels(...); g.enable_warm(); g.maxflow()`` is the order.  The first solve then records the residual
+        source capacities the folds read (``mgc_set_option(MGC_OPT_WARM)``); its mask and energy are those without the
+        call.  The setting survives ``reset()``.  On a graph the lazy fused build made it changes nothing.  A solved graph
+        that cannot fold raises ``RuntimeError``, a sparse graph ``TypeError``; the per-voxel solver
+        (``MEDPY_GC_SOLVER=v0``) still refuses the folds."""
+        if self._sp is not None:
+            raise TypeError("enable_warm() needs a lattice graph: a general sparse graph has no warm re-solve")
+        if self._native is not None:
+            from .. import _lib
+            try:
+                self._native.set_option(_lib._mgc.OPT_WARM, 1)
+            except RuntimeError:
+                raise RuntimeError("this graph was solved without a warm path: call enable_warm() before the first "
+                                   "maxflow(); reset() the graph and rebuild it to re-solve it warm") from None
+        self._warm = True
 
     def defer_weight_check(self, on=True):
         """Let a boundary term return before its kernel has reported non-positive weights; the ValueError is then
@@ -430,8 +456,9 @@ class GraphDouble:
 
         Before the first ``maxflow()`` the calls are staged like ``add_tweights``.  After it, on a graph that
         ``graph_from_voxels`` built in one fused pass (1-D..3-D lattice on one GPU), the seeds are folded into the solved
-        state and the next solve continues from the flow already routed (mgc_add_seeds).  Any other solved graph raises
-        ``RuntimeError``: ``reset()`` it and build the graph again with the seeds."""
+        state and the next solve continues from the flow already routed (mgc_add_seeds); so on any lattice graph that called
+        ``enable_warm()`` before its first solve.  Any other solved graph raises ``RuntimeError``: ``reset()`` it and
+        build the graph again with the seeds."""
         self._fold_seeds(fg, bg, 65535.0, "add_seeds", "with")
 
     def remove_seeds(self, fg=None, bg=None):
@@ -444,7 +471,8 @@ class GraphDouble:
         checks that a seed was there: erasing one that was never added applies the call anyway, as the reference does.
 
         Before the first ``maxflow()`` the calls are staged like ``add_tweights``.  After it the seeds are folded into
-        the solved state on the same graphs as ``add_seeds`` (mgc_remove_seeds); any other solved graph raises
+        the solved state on the same graphs as ``add_seeds`` (``enable_warm()`` included, mgc_remove_seeds); any other
+        solved graph raises
         ``RuntimeError``: ``reset()`` it and build the graph again without the seeds."""
         self._fold_seeds(fg, bg, -65535.0, "remove_seeds", "without")
 
@@ -477,8 +505,9 @@ class GraphDouble:
 
         Before the first ``maxflow()`` the calls are staged like ``add_tweights``.  After it, on a graph that
         ``graph_from_voxels`` built in one fused pass (1-D..3-D lattice on one GPU), they are folded into the solved state
-        and the next solve continues from the flow already routed (mgc_add_tweights_warm).  Any other solved graph raises
-        ``RuntimeError``: ``reset()`` it and build the graph again with the calls."""
+        and the next solve continues from the flow already routed (mgc_add_tweights_warm); so on any lattice graph that
+        called ``enable_warm()`` before its first solve.  Any other solved graph raises ``RuntimeError``: ``reset()`` it and
+        build the graph again with the calls."""
         cuda = any(hasattr(x, "__cuda_array_interface__") for x in (nodes, cap_source, cap_sink))
         ids = self._seed_ids(nodes) if nodes is not None else None
         if cuda and ids is not None and not hasattr(ids, "__cuda_array_interface__"):
