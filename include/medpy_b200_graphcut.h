@@ -14,7 +14,8 @@
  *   - node id == C-order flat index over the logical shape (generate.py:170-172, energy_voxel.py:650-677);
  *   - arrays are described by (pointer, dtype, byte strides over the logical shape); host pointers are only
  *     borrowed for the duration of the call (copied to the device inside); MGC_MEM_DEVICE pointers must be
- *     valid on the handle's device and are read on the handle's stream;
+ *     valid on the handle's device and are read on the handle's stream; they too are borrowed for the call only,
+ *     except the image and probability map of mgc_build_voxel_graph under MGC_OPT_KEEP_DEVICE_INPUTS (see there);
  *   - all device memory is owned by the library; a handle is not thread-safe, distinct handles are
  *     independent; the GIL can be released around every call;
  *   - there is NO CPU solver behind this ABI: with no usable CUDA device mgc_create fails with
@@ -139,6 +140,15 @@ int mgc_trim_pools(void);
 /* MGC_OPT_WARM (default 0; 1 switches it on): warm re-solves (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm) on
  * handles the lazy fused build did not build -- see mgc_add_seeds. */
 #define MGC_OPT_WARM 2
+/* MGC_OPT_KEEP_DEVICE_INPUTS (default 0; 1 switches it on): a lifetime promise, not a speed knob.  The lazy fused build
+ * (mgc_build_voxel_graph) keeps reading its image and probability map after the call: the materialiser, the solve and
+ * the warm folds recompute capacities and t-links from them.  By default the build keeps a copy of each, and device inputs
+ * are borrowed for the call only.  With the option set, a contiguous MGC_MEM_DEVICE image or map is not copied: the
+ * handle records the caller's pointer and reads it on its stream until the next build, mgc_reset or mgc_destroy.  The
+ * caller then keeps the array alive and unchanged until then, and until the handle's stream has finished the work queued
+ * before (mgc_synchronize).  mgc_destroy never frees it.  Host and strided inputs are staged into buffers the handle
+ * owns as before.  The option applies to builds that start after it is set.  Adding it left MGC_ABI_VERSION at 3. */
+#define MGC_OPT_KEEP_DEVICE_INPUTS 3
 int mgc_set_option(mgc_graph* g, int32_t option, int64_t value);
 /* Deliver a deferred verdict now (MGC_OK / MGC_E_WEIGHT). */
 int mgc_check(mgc_graph* g);

@@ -179,12 +179,17 @@ struct mgc_graph {
     bool warm_state = false;           // tr holds BK's residual source capacity: recorded since the last init
     int* cmat = nullptr;              // per tile: push state materialised since the last lazy build
     int* caps_list = nullptr;          // tiles claimed by the current materialiser launch
-    // The copies below (with caps_P and caps_tin) live as long as the handle's last lazy build: besides the materialiser,
-    // the seed folds depend on them -- they recompute a seeded voxel's capacities before any flow from img_copy to know
+    // The inputs below (with caps_P and caps_tin) live as long as the handle's last lazy build: besides the materialiser,
+    // the seed folds depend on them -- they recompute a seeded voxel's capacities before any flow from caps_img to know
     // the source flow its state already holds (gc_seeds.cuh).  Dropping them breaks the warm re-solve.
-    Buf img_copy;                      // the image the lazy build saw, in its own dtype
+    Buf img_copy;                      // the image the lazy build saw, in its own dtype (a staging buffer of the build, or
+                                       // a copy its kernel wrote)
     Buf prob_copy;                     // ... its probability map, in its own dtype
     Buf mark_planes[2];                // ... its fg / bg markers as bit planes (LazyTin)
+    // what the materialiser and the folds read: img_copy, or the caller's device image (MGC_OPT_KEEP_DEVICE_INPUTS);
+    // caps_tin.prob likewise.  Forgotten by mgc_reset, the per-term calls and every build that is not lazy.
+    const void* caps_img = nullptr;
+    bool keep_device_inputs = false;   // MGC_OPT_KEEP_DEVICE_INPUTS
     Buf seed_buf;                      // folds: item count + error flag, inputs, keys, runs, touched tiles, items, cub scratch
     cudaEvent_t ev_seed[4] = {};       // spans of the grouping and of claim + fold + list fix-up
     int caps_dtype = MGC_F32;
@@ -445,6 +450,8 @@ int finish_flow_const(mgc_graph* g)
 void invalidate(mgc_graph* g)
 {
     g->lazy_built = false;             // terms changed outside the lazy build
+    g->caps_img = nullptr;             // ... so no later call reads its inputs (work already queued may still read them)
+    g->caps_tin.prob = nullptr;
     g->state_init = false;
     g->warm_state = false;
     g->solved = false;
@@ -847,7 +854,7 @@ template <typename E>
 void caps_launch_t(mgc_graph* g)
 {
     const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->img_copy.p;
+    const E* img = (const E*)g->caps_img;
     int* count = g->d_flags + 4;              // [4] tiles claimed by this launch, [5] cursor
     int* done = g->d_flags + 3;               // tiles materialised since the build
     const unsigned grid = (unsigned)g->n_ctas;
@@ -889,7 +896,7 @@ template <typename E>
 void seed_fold_launch_t(mgc_graph* g, unsigned grid, const SeedItem* items, int n, double cap)
 {
     const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->img_copy.p;
+    const E* img = (const E*)g->caps_img;
     if constexpr (!std::is_integral<E>::value) {
         if (P.fn == 1 && P.inv_spacing_on == 0.0) {
             if (P.use_max) k_seed_fold<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, cap, g->partials);
@@ -906,7 +913,7 @@ void tweights_fold_launch_t(mgc_graph* g, unsigned grid, const TweightItem* item
                             const double* src, const double* snk)
 {
     const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->img_copy.p;
+    const E* img = (const E*)g->caps_img;
     if constexpr (!std::is_integral<E>::value) {
         if (P.fn == 1 && P.inv_spacing_on == 0.0) {
             if (P.use_max) k_tweights_fold<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
@@ -2042,6 +2049,7 @@ int mgc_set_option(mgc_graph* g, int32_t option, int64_t value)
 {
     if (!g) return MGC_E_ARG;
     if (option == MGC_OPT_DEFER_WEIGHT_CHECK) { g->defer_check = value != 0; return MGC_OK; }
+    if (option == MGC_OPT_KEEP_DEVICE_INPUTS) { g->keep_device_inputs = value != 0; return MGC_OK; }
     if (option == MGC_OPT_WARM) {
         // the record is taken before the first push; a lazily built handle folds without it, so there it changes nothing now
         const bool on = value != 0;
@@ -2314,10 +2322,21 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     if (const char* e = getenv("MEDPY_GC_BUILD_DBG")) A.dbg = atoi(e);
     const bool lazy = can_lazy(g);
     const int mark_words = (g->L.dim[2] + 31) / 32;
+    // Where the materialiser and the folds read the image and the map of a lazy build later:
+    //   STAGED   -- the staging buffer of this call (host or gathered input) becomes the copy: swapped after the build;
+    //   BORROWED -- the caller's contiguous device array itself (MGC_OPT_KEEP_DEVICE_INPUTS);
+    //   COPIED   -- a copy the build kernel writes as it goes.
+    enum { COPIED, STAGED, BORROWED };
+    auto source_of = [&](const mgc_array* a, const void* d, int slot) {
+        if (d == g->scratch[slot].p) return STAGED;
+        return (g->keep_device_inputs && a->mem == MGC_MEM_DEVICE && d == a->data) ? BORROWED : COPIED;
+    };
+    const int img_src = lazy ? source_of(t->image, d_img, 2) : COPIED;
+    // (MEDPY_GC_BUILD_DBG=1 builds from a constant map: only a copy holds what the build saw)
+    const int prob_src = (lazy && t->prob && !(A.dbg & 1)) ? source_of(t->prob, d_prob, 0) : COPIED;
     if (lazy) {
-        rc = ensure_scratch(g, g->img_copy, n * es_img); if (rc) return rc;
-        A.img_copy = g->img_copy.p;
-        if (t->prob) { rc = ensure_scratch(g, g->prob_copy, n * es_prob); if (rc) return rc; A.prob_copy = g->prob_copy.p; }
+        if (img_src == COPIED) { rc = ensure_scratch(g, g->img_copy, n * es_img); if (rc) return rc; A.img_copy = g->img_copy.p; }
+        if (t->prob && prob_src == COPIED) { rc = ensure_scratch(g, g->prob_copy, n * es_prob); if (rc) return rc; A.prob_copy = g->prob_copy.p; }
         const size_t plane_bytes = (size_t)g->L.dim[0] * (size_t)g->L.dim[1] * (size_t)mark_words * 4;
         if (t->fg || t->fg_bits) { rc = ensure_scratch(g, g->mark_planes[0], plane_bytes); if (rc) return rc; A.fg_plane = (unsigned*)g->mark_planes[0].p; }
         if (t->bg || t->bg_bits) { rc = ensure_scratch(g, g->mark_planes[1], plane_bytes); if (rc) return rc; A.bg_plane = (unsigned*)g->mark_planes[1].p; }
@@ -2394,7 +2413,13 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     g->st.ms_seeds_host = 0.0;
     g->caps_dtype = t->image->dtype;
     g->caps_P = P;
-    g->caps_tin = LazyTin{A.prob_copy, A.prob_f64, A.compute_f32, A.alpha, A.fg_plane, A.bg_plane, mark_words};
+    // a staged input becomes the copy and the old copy the staging buffer; span.stop below records the slot's event after
+    // the build, so the next upload into that buffer waits for whatever already queued still reads the old copy
+    if (img_src == STAGED) std::swap(g->scratch[2], g->img_copy);
+    if (prob_src == STAGED) std::swap(g->scratch[0], g->prob_copy);
+    g->caps_img = !lazy ? nullptr : (img_src == BORROWED ? d_img : g->img_copy.p);
+    const void* caps_prob = !(lazy && t->prob) ? nullptr : (prob_src == BORROWED ? d_prob : g->prob_copy.p);
+    g->caps_tin = LazyTin{caps_prob, A.prob_f64, A.compute_f32, A.alpha, A.fg_plane, A.bg_plane, mark_words};
     g->has_nlinks = true;
     g->boundary_timed = true;
     g->state_init = true;

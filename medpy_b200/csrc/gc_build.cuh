@@ -8,8 +8,8 @@
 // passes here (with capacity planes written by one kernel and read straight back by the next).  Now every input byte is read once and every state byte written once:
 //     read  image 4 + probability 4 + fg 1 + bg 1                         = 10 B/voxel (float32 inputs)
 //     write six float64 capacities 48 + tr 8 + excess 8 + label 4 + rmask 1 = 69 B/voxel
-// (the lazy variant, LAZY = 1 below, writes copies of the image and the probability map and two marker bit planes
-// instead of the capacities, tr and excess: 13.25 B/voxel for float32 inputs)
+// (the lazy variant, LAZY = 1 below, writes two marker bit planes instead of the capacities, tr and excess: 5.25 B/voxel,
+// plus 8 B/voxel of image and probability copies for float32 inputs when the graph cannot read the inputs later)
 // (`sink[]`, the absorbed-flow accumulator, is no longer zero-filled: bit RM_SINKV of rmask says whether a voxel's
 // entry has been written, see gc_tiles.cuh.)
 //
@@ -64,8 +64,8 @@ struct BuildArgs {
     int tma_mark;              // fg / bg byte blocks staged by TMA (bit 0: fg, bit 1: bg)
     int z_tile0;               // first z tile layer of this launch (chunked builds)
     int dbg;                   // diagnostics (MEDPY_GC_BUILD_DBG): 1 = do not load the probability map (constant 0.3)
-    void* img_copy;            // lazy build: graph-owned copy of the image (input arrays are only borrowed for the call)
-    void* prob_copy;           // lazy build: graph-owned copy of the probability map, in its own dtype
+    void* img_copy;            // lazy build: graph-owned copy of the image, or nullptr when the graph reads the input itself later
+    void* prob_copy;           // lazy build: graph-owned copy of the probability map, in its own dtype, or nullptr (as img_copy)
     unsigned* fg_plane;        // lazy build: marker bit planes (nullptr: no such marker), see MarkerPlanes
     unsigned* bg_plane;
     int* cmat;                 // lazy build: per tile "push state materialised" flag, cleared here
@@ -182,8 +182,9 @@ __device__ __forceinline__ bool source_active(double tr, unsigned pairs)
 // warp-uniform branches, whose bookkeeping costs instructions in this issue-heavy loop.
 //
 // LAZY = 1: neither the capacity planes nor tr nor excess are written (k_caps_tiles computes all three for the tiles the
-// push path reaches); the kernel writes what recomputes them bit for bit instead -- copies of the image and of the
-// probability map, the markers as two bit planes (one ballot per warp row) -- and clears cmat[] of its tiles.  rmask,
+// push path reaches); the kernel writes what recomputes them bit for bit instead -- the markers as two bit planes (one
+// ballot per warp row) and, where the graph has no other copy of them to read later (img_copy / prob_copy not nullptr),
+// copies of the image and of the probability map -- and clears cmat[] of its tiles.  rmask,
 // height, partials and worklists are bit for bit what LAZY = 0 writes.  Under the exponential term without spacing every
 // in-lattice weight is >= DBL_MIN, so for a warp whose arguments are ordinary the n-link bits of rmask are the validity
 // bits, and the clamped excess is > 0 exactly when tr > 0 and the voxel has an in-lattice arc: such a warp evaluates no
@@ -409,9 +410,11 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
                 mm = tlinks(tr);
             }
             if (LAZY) {
-                reinterpret_cast<E*>(A.img_copy)[v] = at(hz, ly + 1, lx + 1);
-                if (TIN == 1 || (A.prob && !A.prob_f64)) reinterpret_cast<float*>(A.prob_copy)[v] = (float)cur.p;
-                else if (A.prob) reinterpret_cast<double*>(A.prob_copy)[v] = cur.p;
+                if (A.img_copy) reinterpret_cast<E*>(A.img_copy)[v] = at(hz, ly + 1, lx + 1);
+                if (A.prob_copy) {
+                    if (TIN == 1 || !A.prob_f64) reinterpret_cast<float*>(A.prob_copy)[v] = (float)cur.p;
+                    else reinterpret_cast<double*>(A.prob_copy)[v] = cur.p;
+                }
             }
             const bool own = gz >= L.own0 && gz < L.own1;
             if (own) msum = __dadd_rn(msum, mm);

@@ -123,17 +123,21 @@ public:
     {
         ArrayRef r = make_ref(prob, -1, "probability_map");
         check_shape(r, "probability_map");
+        check_inputs();
         int rc;
         { py::gil_scoped_release rel; rc = mgc_add_regional_probability(g_, &r.a, alpha, compute_f32 ? MGC_F32 : MGC_F64); }
         check(rc, g_);
+        held_live_ = false;
     }
     void add_tweights_dense(const py::object& src, const py::object& snk)
     {
         ArrayRef a = make_ref(src, MGC_F64, "src"), b = make_ref(snk, MGC_F64, "snk");
         check_shape(a, "src"); check_shape(b, "snk");
+        check_inputs();
         int rc;
         { py::gil_scoped_release rel; rc = mgc_add_tweights_dense(g_, &a.a, &b.a); }
         check(rc, g_);
+        held_live_ = false;
     }
     void add_markers(const py::object& fg, const py::object& bg)
     {
@@ -141,9 +145,11 @@ public:
         bool hf = !fg.is_none(), hb = !bg.is_none();
         if (hf) { a = make_ref(fg, MGC_U8, "fg_markers"); check_shape(a, "fg_markers"); }
         if (hb) { b = make_ref(bg, MGC_U8, "bg_markers"); check_shape(b, "bg_markers"); }
+        check_inputs();
         int rc;
         { py::gil_scoped_release rel; rc = mgc_add_markers(g_, hf ? &a.a : nullptr, hb ? &b.a : nullptr); }
         check(rc, g_);
+        held_live_ = false;
     }
     void add_boundary(int kind, const py::object& image, double sigma, const py::object& spacing, double norm)
     {
@@ -154,9 +160,11 @@ public:
             sp = spacing.cast<std::vector<double>>();
             if (sp.size() < shape_.size()) throw py::value_error("spacing has fewer entries than the image has dimensions");
         }
+        check_inputs();
         int rc;
         { py::gil_scoped_release rel; rc = mgc_add_boundary(g_, kind, &r.a, sigma, sp.empty() ? nullptr : sp.data(), norm); }
         check(rc, g_);
+        held_live_ = false;
     }
     // everything graph_from_voxels adds, in one native call (mgc_build_voxel_graph); None = term absent, kind -1 = no boundary
     void build_voxel_graph(const py::object& prob, double alpha, bool compute_f32, int kind, const py::object& image, double sigma,
@@ -203,20 +211,37 @@ public:
             t.bits_mem = MGC_MEM_HOST;
             t.bits_ready_words = reinterpret_cast<const volatile int64_t*>(&packer->ready);
         }
+        // device image and map: the lazy build reads them in place until the next build or reset (no copy), so they stay
+        // referenced here for as long as the handle may read them
+        std::vector<Held> hold;
+        if (keep_inputs_)
+            for (const ArrayRef* r : {&ri, &rp})
+                if (r->keep && r->a.mem == MGC_MEM_DEVICE) hold.push_back(Held{r->keep, version_of(r->keep)});
+        check(mgc_set_option(g_, MGC_OPT_KEEP_DEVICE_INPUTS, hold.empty() ? 0 : 1), g_);
         int rc;
         { py::gil_scoped_release rel; rc = mgc_build_voxel_graph(g_, &t); packer.reset(); }
         for (int p = 0; p < 2; ++p) if (bits[p]) mgc_host_free(bits[p]);
-        check(rc, g_);
+        if (rc != MGC_OK) {
+            // the handle may still read what it held before this call, and queued work may read the new arrays
+            held_.insert(held_.end(), hold.begin(), hold.end());
+            check(rc, g_);
+        }
+        hold_inputs(std::move(hold));
+        held_live_ = !held_.empty() && kind >= 0 && mgc_can_fuse(g_);
     }
     void set_pack_markers(bool on) { pack_markers_ = on; }
+    // off: device inputs are borrowed for the build call only and the build keeps its own copies (the C default)
+    void set_keep_device_inputs(bool on) { keep_inputs_ = on; }
     bool can_fuse() const { return mgc_can_fuse(g_) != 0; }
     void add_nweights_dense(int axis, const py::object& fwd, const py::object& bwd)
     {
         ArrayRef a = make_ref(fwd, MGC_F64, "fwd"), b = make_ref(bwd, MGC_F64, "bwd");
         check_shape(a, "fwd"); check_shape(b, "bwd");
+        check_inputs();
         int rc;
         { py::gil_scoped_release rel; rc = mgc_add_nweights_dense(g_, axis, &a.a, &b.a); }
         check(rc, g_);
+        held_live_ = false;
     }
     // contiguous 1-D array on the host (numpy, converted to T) or on the device (__cuda_array_interface__ of typestr `ts`,
     // read in place); None = absent
@@ -259,6 +284,7 @@ public:
         Vec f = vec_of<int64_t>(fg, "i8", "fg_ids"), b = vec_of<int64_t>(bg, "i8", "bg_ids");
         if (f.n && b.n && f.mem != b.mem) throw py::value_error("fg_ids and bg_ids must both be host or both be device arrays");
         const int mem = f.n ? f.mem : (b.n ? b.mem : MGC_MEM_HOST);
+        check_inputs();
         int rc;
         { py::gil_scoped_release rel; rc = fold(g_, f.n ? (const int64_t*)f.p : nullptr, f.n, b.n ? (const int64_t*)b.p : nullptr, b.n, mem); }
         check(rc, g_);
@@ -273,6 +299,7 @@ public:
         if (s.n != t.n || (!ids.is_none() && i.n != s.n)) throw py::value_error("ids, src and snk differ in length");
         if (s.mem != t.mem || (!ids.is_none() && i.mem != s.mem))
             throw py::value_error("ids, src and snk must all be host or all be device arrays");
+        check_inputs();
         int rc;
         {
             py::gil_scoped_release rel;
@@ -283,6 +310,7 @@ public:
     }
     double maxflow()
     {
+        check_inputs();
         double e = 0;
         int rc;
         { py::gil_scoped_release rel; rc = mgc_maxflow(g_, &e); }
@@ -311,11 +339,12 @@ public:
         check(rc, g_);
     }
     int what_segment(int64_t i) { int32_t s = 0; check(mgc_what_segment(g_, i, &s), g_); return s; }
-    double get_edge(int64_t i, int64_t j) { double c = 0; check(mgc_get_edge(g_, i, j, &c), g_); return c; }
-    double get_trcap(int64_t i) { double c = 0; check(mgc_get_trcap(g_, i, &c), g_); return c; }
+    double get_edge(int64_t i, int64_t j) { check_inputs(); double c = 0; check(mgc_get_edge(g_, i, j, &c), g_); return c; }
+    double get_trcap(int64_t i) { check_inputs(); double c = 0; check(mgc_get_trcap(g_, i, &c), g_); return c; }
     int64_t get_node_num() { int64_t n = 0; check(mgc_get_node_num(g_, &n), g_); return n; }
     int64_t get_arc_num() { int64_t n = 0; check(mgc_get_arc_num(g_, &n), g_); return n; }
-    void reset() { check(mgc_reset(g_), g_); }
+    // the handle forgets the build's inputs; their references go at the next build, once its stream is done with them
+    void reset() { check(mgc_reset(g_), g_); held_live_ = false; }
     void set_option(int option, long long value) { check(mgc_set_option(g_, option, value), g_); }
     void check_deferred() { int rc; { py::gil_scoped_release rel; rc = mgc_check(g_); } check(rc, g_); }
     void set_stream(uintptr_t s) { check(mgc_set_stream(g_, reinterpret_cast<void*>(s)), g_); }
@@ -413,9 +442,42 @@ public:
     std::vector<int64_t> shape() const { return shape_; }
 
 private:
+    // a device array the last build may still read, and its torch version counter at the build (-1: not a tensor)
+    struct Held { py::object obj; int64_t version; };
+    static int64_t version_of(const py::object& o)
+    {
+        return py::hasattr(o, "_version") ? o.attr("_version").cast<int64_t>() : -1;
+    }
+    // take the arrays of a new build; the ones it replaces are dropped only after the handle's stream is done with them
+    // (the caching allocator may hand their memory out again at once).  The same arrays again (a resident loop) cost
+    // no synchronisation.
+    void hold_inputs(std::vector<Held> hold)
+    {
+        bool same = hold.size() == held_.size();
+        for (size_t i = 0; same && i < hold.size(); ++i) same = hold[i].obj.is(held_[i].obj);
+        if (!same && !held_.empty()) {
+            int rc;
+            { py::gil_scoped_release rel; rc = mgc_synchronize(g_); }
+            check(rc, g_);
+        }
+        held_ = std::move(hold);
+    }
+    // before a call that may read the inputs of the last build: an array changed in place since would give another graph
+    void check_inputs() const
+    {
+        if (!held_live_) return;
+        for (const Held& h : held_)
+            if (h.version >= 0 && version_of(h.obj) != h.version)
+                throw std::runtime_error("an image or probability map passed to the graph build was modified in place after "
+                                         "the build; rebuild the graph");
+    }
+
     mgc_graph* g_ = nullptr;
     std::vector<int64_t> shape_;
     int64_t owned_planes_ = -1;
+    std::vector<Held> held_;
+    bool held_live_ = false;           // the handle may read held_ (until reset or a per-term call)
+    bool keep_inputs_ = true;
     bool pack_markers_ = std::getenv("MEDPY_GC_PACK_MARKERS") ? std::atoi(std::getenv("MEDPY_GC_PACK_MARKERS")) != 0 : true;
 };
 
@@ -628,6 +690,7 @@ PYBIND11_MODULE(_mgc, m)
     m.attr("SINK") = MGC_SINK;
     m.attr("OPT_DEFER_WEIGHT_CHECK") = MGC_OPT_DEFER_WEIGHT_CHECK;
     m.attr("OPT_WARM") = MGC_OPT_WARM;
+    m.attr("OPT_KEEP_DEVICE_INPUTS") = MGC_OPT_KEEP_DEVICE_INPUTS;
     m.attr("LABELS_ADJACENCY") = MGC_LABELS_ADJACENCY;
     m.attr("LABELS_STAWIASKI") = MGC_LABELS_STAWIASKI;
     m.attr("LABELS_STAWIASKI_DIRECTED") = MGC_LABELS_STAWIASKI_DIRECTED;
@@ -672,6 +735,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("slab_solve_stats", &PyGraph::slab_solve_stats)
         .def("can_fuse", &PyGraph::can_fuse)
         .def("set_pack_markers", &PyGraph::set_pack_markers)
+        .def("set_keep_device_inputs", &PyGraph::set_keep_device_inputs)
         .def("maxflow", &PyGraph::maxflow)
         .def("get_mask", &PyGraph::get_mask)
         .def("get_mask_into", &PyGraph::get_mask_into)

@@ -32,6 +32,13 @@ def graph_from_device_arrays(fg_markers, bg_markers, image=None, boundary=None, 
     prob/alpha : ``regional_probability_map`` arguments (float32 map * Python float -> float32 products)
     graph : an earlier result to reuse (its device memory is kept, all weights are reset)
     stream : cudaStream_t as int (e.g. ``torch.cuda.current_stream().cuda_stream``) to run on
+
+    The graph keeps reading ``image`` and ``prob`` after this call instead of copying them: the solve, ``get_edge`` /
+    ``get_trcap`` and the warm re-solves (``add_seeds``, ``remove_seeds``, ``add_tweights_warm``) recompute capacities
+    and t-links from them.  It holds references to both until the next build into it, ``reset()`` or its deletion, so
+    dropping yours is safe; changing them in place is not: any such call on a torch tensor modified in place after the
+    build raises ``RuntimeError``, and a rebuild takes the arrays as they are then.  (A contiguous array is read in place;
+    a strided one is gathered into a buffer the graph owns.)
     """
     shape = tuple(int(s) for s in fg_markers.shape)
     n = 1
