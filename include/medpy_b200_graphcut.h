@@ -97,9 +97,10 @@ typedef struct mgc_stats {
     double ms_init;             /* device ms of the solver-state initialisation kernel (k_init_tile); 0 after a fused build */
     int64_t tiles_materialised; /* lazy build: 8^3 tiles whose capacities, tr and excess k_caps_tiles computed (0 eager) */
     double ms_caps;             /* device ms of the materialiser launches (k_caps_claim + k_caps_tiles; not in ms_push)  */
-    int64_t seed_folds;         /* mgc_add_seeds, mgc_remove_seeds and mgc_add_tweights_warm calls folded into this   */
-                                /* handle since its build (reset by the build; erase and t-link calls count like add  */
-                                /* calls in all three fields; a call of only zero weights folds nothing, counts not)  */
+    int64_t seed_folds;         /* mgc_add_seeds, mgc_remove_seeds, mgc_add_tweights_warm and the two n-link warm     */
+                                /* calls (mgc_add_nweights_warm / _dense_warm) folded into this handle since its      */
+                                /* build (reset by the build; erase, t-link and n-link calls count like add calls in  */
+                                /* all three fields; a call of only zero weights folds nothing, counts not)           */
     double ms_seeds;            /* device ms of those calls: id / weight upload, grouping (sort or compaction,        */
                                 /* run-length), tile claim + materialisation, fold, push-list fix-up; not the one     */
                                 /* read-back of the item count                                                         */
@@ -137,8 +138,8 @@ int mgc_trim_pools(void);
  * markers, maxflow, mgc_check).  graph_from_voxels switches it on because it always adds the markers right after the
  * boundary term, which lets the marker upload overlap the stencil kernel. */
 #define MGC_OPT_DEFER_WEIGHT_CHECK 1
-/* MGC_OPT_WARM (default 0; 1 switches it on): warm re-solves (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm) on
- * handles the lazy fused build did not build -- see mgc_add_seeds. */
+/* MGC_OPT_WARM (default 0; 1 switches it on): warm re-solves (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm /
+ * mgc_add_nweights_warm / mgc_add_nweights_dense_warm) on handles the lazy fused build did not build -- see mgc_add_seeds. */
 #define MGC_OPT_WARM 2
 /* MGC_OPT_KEEP_DEVICE_INPUTS (default 0; 1 switches it on): a lifetime promise, not a speed knob.  The lazy fused build
  * (mgc_build_voxel_graph) keeps reading its image and probability map after the call: the materialiser, the solve and
@@ -282,6 +283,30 @@ int mgc_remove_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const in
  * carry it into BK) or bad counts and pointers.  Same preconditions, MGC_E_STATE message and behaviour on solved and
  * unsolved handles as mgc_add_seeds.  Adding this entry point left MGC_ABI_VERSION at 3. */
 int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, const double* snk, int64_t count, int32_t mem);
+/* sum_edge calls folded into a graph and solved warm (a boundary brush, a larger boundary weight, a second boundary term on
+ * a solved graph; graph.h:456-480: BK adds cap to the residual capacity of i -> j and rev_cap to that of j -> i, and the
+ * next maxflow() continues from the residual graph).  The meaning is exactly sum_edge(i[k], j[k], cap[k], rev_cap[k]) for
+ * k = 0 .. count-1 in array order, applied to the residual capacities: a repeated pair is applied once per occurrence, in
+ * call order.  The add_tweights constant does not change.
+ *   i / j          : C-order int64 ids of lattice neighbours (i != j); cap / rev_cap: contiguous doubles; all four in `mem`
+ *                    (host memory is borrowed for the call, device memory is read in place on the handle's stream).
+ *   increments     : nonnegative and finite, as the reference's sum_edge asserts.  A zero increment changes nothing and is
+ *                    skipped; a call of only zero increments keeps the solved state, mask and energy.  Lowering a
+ *                    capacity below the flow it carries would need a reparametrisation the handle cannot check; it is not
+ *                    offered.
+ * count == 0 does nothing.  MGC_E_ARG, with the handle unchanged, for an id out of range, a pair that is not a lattice
+ * neighbour, a NaN or infinite weight, or bad counts and pointers; MGC_E_WEIGHT, with the handle unchanged, for a negative
+ * weight.  Same preconditions, MGC_E_STATE message and behaviour on solved and unsolved handles as mgc_add_tweights_warm.
+ * mgc_add_nweights_dense, mgc_add_boundary and the other term entry points still refuse a solved graph.  Adding this entry
+ * point left MGC_ABI_VERSION at 3. */
+int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
+                          int64_t count, int32_t mem);
+/* The dense form of mgc_add_nweights_warm, in the layout of mgc_add_nweights_dense: fwd / bwd are float64 arrays over the
+ * logical shape (any positive strides, host or device); entry p holds the increments of cap(p -> p+e_axis) and
+ * cap(p+e_axis -> p), and the last plane of `axis` is ignored.  Only the pairs with a nonzero entry are touched, so an
+ * update of a box only materialises that box's tiles on a lazily built handle.  Same errors, preconditions and behaviour
+ * as mgc_add_nweights_warm.  Adding this entry point left MGC_ABI_VERSION at 3. */
+int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd);
 /* Bulk form of the what_segment loop (bin/medpy_graphcut_voxel.py:177-181): out[v] = 0 if the voxel is in
  * the SINK set else 1, C-order over the logical shape.  `mem` selects host or device destination. */
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem);

@@ -12,6 +12,7 @@
 #include "gc_sweep.cuh"
 #include "gc_build.cuh"
 #include "gc_seeds.cuh"
+#include "gc_nlinks.cuh"
 #include "gc_gradient.cuh"
 
 #include <algorithm>
@@ -922,6 +923,22 @@ void tweights_fold_launch_t(mgc_graph* g, unsigned grid, const TweightItem* item
         }
     }
     k_tweights_fold<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
+}
+
+// k_nlinks_reclamp with the same instantiations
+template <typename E>
+void nlinks_reclamp_launch_t(mgc_graph* g, unsigned grid, const unsigned* tails, const int* ntails)
+{
+    const BoundaryParams& P = g->caps_P;
+    const E* img = (const E*)g->caps_img;
+    if constexpr (!std::is_integral<E>::value) {
+        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
+            if (P.use_max) k_nlinks_reclamp<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, tails, ntails, g->partials);
+            else           k_nlinks_reclamp<E, 1, 0, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, tails, ntails, g->partials);
+            return;
+        }
+    }
+    k_nlinks_reclamp<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, tails, ntails, g->partials);
 }
 
 // capacities, tr or excess are about to be read or written outside the push path: materialise the tiles that are not yet
@@ -2550,11 +2567,12 @@ int mgc_maxflow(mgc_graph* g, double* energy)
 
 // Number of kernels the cub calls of a fold's grouping enqueue, so that kernel_launches counts them too: CUB_SEED_KEYS =
 // cub::DeviceRadixSort::SortKeys + cub::DeviceScan::InclusiveSum (seeds), CUB_PAIRS = SortPairs + InclusiveSum (the list
-// form of mgc_add_tweights_warm), CUB_SCAN = InclusiveSum alone (its dense form).  cub decides it on the host from
-// (n, end_bit) and the device; the calls are captured on a capture-only stream of the device (nothing runs) and the kernel
-// nodes of the captured graph counted.  The stream lives for the process and the counts are cached, so a call pays only
-// the capture of a few launches.
-enum { CUB_SEED_KEYS = 0, CUB_PAIRS = 1, CUB_SCAN = 2 };
+// form of mgc_add_tweights_warm), CUB_SCAN = InclusiveSum alone (its dense form, and the dense n-link form), CUB_PAIRS64 =
+// SortPairs on 64-bit keys (passed through `keys` / `skeys`) + InclusiveSum (the list form of mgc_add_nweights_warm).  cub
+// decides it on the host from (n, end_bit) and the device; the calls are captured on a capture-only stream of the device
+// (nothing runs) and the kernel nodes of the captured graph counted.  The stream lives for the process and the counts are
+// cached, so a call pays only the capture of a few launches.
+enum { CUB_SEED_KEYS = 0, CUB_PAIRS = 1, CUB_SCAN = 2, CUB_PAIRS64 = 3 };
 static int seed_cub_launches(mgc_graph* g, int kind, int n, int end_bit, void* tmp, size_t tmp_bytes, unsigned* keys,
                              unsigned* skeys, int* vals, int* svals, int* head, int* pos, int* out)
 {
@@ -2574,6 +2592,9 @@ static int seed_cub_launches(mgc_graph* g, int kind, int n, int end_bit, void* t
         cudaError_t e1 = cudaSuccess;
         if (kind == CUB_SEED_KEYS) e1 = cub::DeviceRadixSort::SortKeys(tmp, tb, keys, skeys, n, 0, end_bit, s);
         else if (kind == CUB_PAIRS) e1 = cub::DeviceRadixSort::SortPairs(tmp, tb, keys, skeys, vals, svals, n, 0, end_bit, s);
+        else if (kind == CUB_PAIRS64)
+            e1 = cub::DeviceRadixSort::SortPairs(tmp, tb, (unsigned long long*)keys, (unsigned long long*)skeys, vals, svals, n,
+                                                 0, end_bit, s);
         tb = tmp_bytes;
         cudaError_t e2 = e1 == cudaSuccess ? cub::DeviceScan::InclusiveSum(tmp, tb, head, pos, n, s) : e1;
         e = cudaStreamEndCapture(s, &graph);
@@ -2609,10 +2630,11 @@ static int warm_check(mgc_graph* g, bool* eager)
                       "the seeds instead");
 }
 
-// The steps of a fold after its grouping, shared by seeds_fold and mgc_add_tweights_warm.  The grouping was enqueued after
+// The steps of a fold after its grouping, shared by seeds_fold, mgc_add_tweights_warm and nweights_fold.  The grouping was enqueued after
 // ev_seed[0] and left d_ctl = [item count | FOLD_ERR_* bits | touched-tile count] and the touched tiles in `tiles`;
 // fold(grid, n_items) enqueues the fold kernel, which stores one partial of the add_tweights constant per block.
-static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<void(unsigned, int)>& fold)
+static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<void(unsigned, int)>& fold,
+                      bool nlinks = false)
 {
     CK(cudaEventRecord(g->ev_seed[1], g->stream));
     // the item count and the error bits in one synchronisation, before the claim and the fold are enqueued
@@ -2620,7 +2642,11 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     CK(cudaMemcpyAsync(h_ctl, d_ctl, sizeof(h_ctl), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
     if (h_ctl[1] & FOLD_ERR_RANGE) FAIL(MGC_E_ARG, "node id out of range");
-    if (h_ctl[1] & FOLD_ERR_NONFINITE) FAIL(MGC_E_ARG, "a t-link weight is NaN or infinite");
+    if (h_ctl[1] & FOLD_ERR_PAIR) FAIL(MGC_E_ARG, "node ids are not lattice neighbours");
+    if (h_ctl[1] & FOLD_ERR_NONFINITE)
+        FAIL(MGC_E_ARG, nlinks ? "an n-link weight is NaN or infinite" : "a t-link weight is NaN or infinite");
+    if (h_ctl[1] & FOLD_ERR_NEGATIVE)
+        FAIL(MGC_E_WEIGHT, "negative n-link weights are not allowed (a warm fold only raises capacities)");
     const int ni = h_ctl[0];
     if (ni == 0) return MGC_OK;                // only add_tweights(v, 0, 0) calls: the state, mask and energy stay
     const bool eager = !g->lazy_built;         // MGC_OPT_WARM handle (warm_check passed)
@@ -2910,6 +2936,171 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
             default: tweights_fold_launch_t<int32_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
         }
     });
+}
+
+// sum_edge calls folded into the handle's current state (gc_nlinks.cuh).  ii != nullptr: the list form, call k is
+// sum_edge(ii[k], jj[k], cap[k], rev[k]) with every array in `mem`.  ii == nullptr: the dense form along canonical axis
+// `axis`, entry p of cap / rev (device memory, count = the voxel count) holds the increments of p -> p + e_axis and back.
+static int nweights_fold(mgc_graph* g, const int64_t* ii, const int64_t* jj, const double* cap, const double* rev,
+                         int64_t count, int32_t mem, int axis, bool eager)
+{
+    if (count == 0) return MGC_OK;             // nothing to fold: the solved state, mask and energy stay as they are
+    const auto host_t0 = std::chrono::steady_clock::now();
+    const bool dense = ii == nullptr;
+    const int n = (int)count;
+    // list form: (arc key, call index) pairs, key = lo << 2 | axis, sorted on the bits a key of this lattice can have, then
+    // run-length encoded; dense form: the pairs with a nonzero increment, compacted by a scan of their flags
+    int end_bit = 1;
+    while (end_bit < 64 && ((4ull * g->L.n - 1ull) >> end_bit)) ++end_bit;
+    size_t sort_bytes = 0, scan_bytes = 0;
+    if (!dense)
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                           (const int*)nullptr, (int*)nullptr, n, 0, end_bit, g->stream));
+    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
+    // device layout (16-byte aligned pieces): [item count | error bits | touched-tile count | tail count] [host i] [host j]
+    // [host cap] [host rev] [keys] [sorted keys] [call indices] [sorted call indices] [heads] [positions] [per-tile flags]
+    // [touched tiles] [items] [per-voxel tail bits] [tails] [cub scratch]; the dense form has no ids, keys or call indices,
+    // an eager handle no tiles
+    auto al = [](size_t b) { return (b + 15) / 16 * 16; };
+    const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
+    const bool host = mem == MGC_MEM_HOST;
+    const size_t w8 = dense ? 0 : al((size_t)n * 8), w4 = dense ? 0 : al((size_t)n * 4), hw = host ? w8 : 0;
+    const size_t i_off = 16;
+    const size_t j_off = i_off + hw;
+    const size_t cap_off = j_off + hw;
+    const size_t rev_off = cap_off + hw;
+    const size_t keys_off = rev_off + hw;
+    const size_t skeys_off = keys_off + w8;
+    const size_t vals_off = skeys_off + w8;
+    const size_t svals_off = vals_off + w4;
+    const size_t head_off = svals_off + w4;
+    const size_t pos_off = head_off + al((size_t)n * 4);
+    const size_t tflag_off = pos_off + al((size_t)n * 4);
+    const size_t tiles_off = tflag_off + al(ntl * 4);
+    const size_t items_off = tiles_off + al(std::min(2 * (size_t)n, ntl) * 4);
+    const size_t tbits_off = items_off + al((size_t)n * sizeof(NlinkItem));
+    const size_t tbits_bytes = ((size_t)g->L.n + 31) / 32 * 4;
+    const size_t tails_off = tbits_off + al(tbits_bytes);
+    const size_t tmp_off = tails_off + al(std::min(2 * (size_t)n, (size_t)g->L.n) * 4);
+    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
+    int rc = ensure_scratch(g, g->seed_buf, tmp_off + tmp_bytes);
+    if (rc) return rc;
+    char* dbuf = (char*)g->seed_buf.p;
+    int* d_ctl = (int*)dbuf;
+    auto* keys = (unsigned long long*)(dbuf + keys_off);
+    auto* skeys = (unsigned long long*)(dbuf + skeys_off);
+    int* vals = (int*)(dbuf + vals_off);
+    int* svals = (int*)(dbuf + svals_off);
+    int* head = (int*)(dbuf + head_off);
+    int* pos = (int*)(dbuf + pos_off);
+    int* tflag = (int*)(dbuf + tflag_off);
+    int* tiles = (int*)(dbuf + tiles_off);
+    NlinkItem* d_items = (NlinkItem*)(dbuf + items_off);
+    unsigned* tbits = (unsigned*)(dbuf + tbits_off);
+    unsigned* tails = (unsigned*)(dbuf + tails_off);
+    int cub_launches = 0;
+    rc = seed_cub_launches(g, dense ? CUB_SCAN : CUB_PAIRS64, n, end_bit, dbuf + tmp_off, tmp_bytes, (unsigned*)keys,
+                           (unsigned*)skeys, vals, svals, head, pos, &cub_launches);
+    if (rc) return rc;
+    for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
+    Nvtx range(dense ? "mgc:add_nweights_dense_warm" : "mgc:add_nweights_warm");
+    g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
+    // 0. grouping on the device; nothing below touches the solver state until the id, pair and weight checks have passed
+    CK(cudaEventRecord(g->ev_seed[0], g->stream));
+    const int64_t* d_i = ii;
+    const int64_t* d_j = jj;
+    const double* d_cap = cap;
+    const double* d_rev = rev;
+    if (host) {
+        // host arrays go straight from the caller into device slots; device arrays are read in place
+        CK(cudaMemcpyAsync(dbuf + i_off, ii, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+        CK(cudaMemcpyAsync(dbuf + j_off, jj, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+        CK(cudaMemcpyAsync(dbuf + cap_off, cap, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+        CK(cudaMemcpyAsync(dbuf + rev_off, rev, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
+        d_i = (const int64_t*)(dbuf + i_off);
+        d_j = (const int64_t*)(dbuf + j_off);
+        d_cap = (const double*)(dbuf + cap_off);
+        d_rev = (const double*)(dbuf + rev_off);
+    }
+    CK(cudaMemsetAsync(d_ctl, 0, 4 * sizeof(int), g->stream));
+    CK(cudaMemsetAsync(tflag, 0, ntl * sizeof(int), g->stream));
+    CK(cudaMemsetAsync(tbits, 0, tbits_bytes, g->stream));
+    {
+        const unsigned kgrid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
+        size_t tb = tmp_bytes;
+        if (dense) {
+            const unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
+            const unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
+            k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap, d_rev,
+                                                               head, d_ctl + 1);
+        } else {
+            if (g->nd == 4) k_nlinks_keys<4><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, keys, vals, d_ctl + 1);
+            else            k_nlinks_keys<3><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, keys, vals, d_ctl + 1);
+            CK(cub::DeviceRadixSort::SortPairs(dbuf + tmp_off, tb, keys, skeys, vals, svals, n, 0, end_bit, g->stream));
+            k_nlinks_heads<<<kgrid, 256, 0, g->stream>>>(skeys, svals, d_cap, d_rev, n, head);
+            tb = tmp_bytes;
+        }
+        CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
+        k_nlinks_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, dense ? nullptr : skeys, axis, pos, n, d_items,
+                                                     eager ? nullptr : tflag, tiles, d_ctl);
+        g->st.kernel_launches += (dense ? 2 : 3) + cub_launches;
+        CK(cudaGetLastError());
+    }
+    const int* order = dense ? nullptr : svals;
+    const int64_t* ids = dense ? nullptr : d_i;
+    int* ntails = d_ctl + 3;
+    return fold_items(g, d_ctl, tiles, [&](unsigned grid, int ni) {
+        // the arcs first, then each tail once: the re-clamp reads the out-capacity after every increment of the call
+        if (g->nd == 4) k_nlinks_fold<4><<<grid, 256, 0, g->stream>>>(g->L, g->S, d_items, ni, order, ids, d_cap, d_rev, tbits, tails, ntails);
+        else            k_nlinks_fold<3><<<grid, 256, 0, g->stream>>>(g->L, g->S, d_items, ni, order, ids, d_cap, d_rev, tbits, tails, ntails);
+        g->st.kernel_launches++;
+        if (eager) {
+            if (g->nd == 4) k_nlinks_reclamp_eager<4><<<grid, 256, 0, g->stream>>>(g->S, g->smask, tails, ntails, g->partials);
+            else            k_nlinks_reclamp_eager<3><<<grid, 256, 0, g->stream>>>(g->S, g->smask, tails, ntails, g->partials);
+            return;
+        }
+        switch (g->caps_dtype) {
+            case MGC_F32: nlinks_reclamp_launch_t<float>(g, grid, tails, ntails); break;
+            case MGC_F64: nlinks_reclamp_launch_t<double>(g, grid, tails, ntails); break;
+            case MGC_U8: nlinks_reclamp_launch_t<uint8_t>(g, grid, tails, ntails); break;
+            case MGC_I16: nlinks_reclamp_launch_t<int16_t>(g, grid, tails, ntails); break;
+            default: nlinks_reclamp_launch_t<int32_t>(g, grid, tails, ntails); break;
+        }
+    }, true);
+}
+
+int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
+                          int64_t count, int32_t mem)
+{
+    if (!g) return MGC_E_ARG;
+    if (count < 0 || (count && (!i || !j || !cap || !rev_cap))) FAIL(MGC_E_ARG, "bad n-link arrays");
+    if (count > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 sum_edge calls in one call");
+    if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
+    bool eager = false;
+    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
+    CK(cudaSetDevice(g->device));
+    { int rc0 = check_pending(g); if (rc0) return rc0; }
+    return nweights_fold(g, i, j, cap, rev_cap, count, mem, 0, eager);
+}
+
+int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
+{
+    if (!g || !fwd || !bwd) return MGC_E_ARG;
+    if (axis < 0 || axis >= g->user_ndim) FAIL(MGC_E_ARG, "bad axis");
+    if (fwd->dtype != MGC_F64 || bwd->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense n-weights must be float64");
+    bool eager = false;
+    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
+    CK(cudaSetDevice(g->device));
+    { int rc0 = check_pending(g); if (rc0) return rc0; }
+    const void *pf = nullptr, *pb = nullptr;
+    int rc = stage_input(g, fwd, 0, &pf);
+    if (rc) return rc;
+    rc = stage_input(g, bwd, 1, &pb);
+    if (rc) return rc;
+    rc = nweights_fold(g, nullptr, nullptr, (const double*)pf, (const double*)pb, (int64_t)g->L.n, MGC_MEM_DEVICE,
+                       axis + g->shift, eager);
+    slots_release(g, 3u);                      // the grouping and the fold read the staging slots
+    return rc;
 }
 
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem)

@@ -308,6 +308,35 @@ public:
         }
         check(rc, g_);
     }
+    // sum_edge calls folded into the solved graph (mgc_add_nweights_warm): i / j = 1-D int64 node ids, cap / rev = 1-D
+    // float64 of the same length, all four on the host or all on the device
+    void add_nweights_warm(const py::object& i, const py::object& j, const py::object& cap, const py::object& rev)
+    {
+        Vec a = vec_of<int64_t>(i, "i8", "i"), b = vec_of<int64_t>(j, "i8", "j");
+        Vec c = vec_of<double>(cap, "f8", "cap"), r = vec_of<double>(rev, "f8", "rev_cap");
+        if (a.mem < 0 || b.mem < 0 || c.mem < 0 || r.mem < 0) throw py::value_error("i, j, cap and rev_cap are required");
+        if (a.n != b.n || a.n != c.n || a.n != r.n) throw py::value_error("i, j, cap and rev_cap differ in length");
+        if (a.mem != b.mem || a.mem != c.mem || a.mem != r.mem)
+            throw py::value_error("i, j, cap and rev_cap must all be host or all be device arrays");
+        check_inputs();
+        int rc;
+        {
+            py::gil_scoped_release rel;
+            rc = mgc_add_nweights_warm(g_, (const int64_t*)a.p, (const int64_t*)b.p, (const double*)c.p, (const double*)r.p,
+                                       a.n, a.mem);
+        }
+        check(rc, g_);
+    }
+    // the dense form (mgc_add_nweights_dense_warm): fwd / bwd float64 arrays of the lattice shape
+    void add_nweights_dense_warm(int axis, const py::object& fwd, const py::object& bwd)
+    {
+        ArrayRef a = make_ref(fwd, MGC_F64, "fwd"), b = make_ref(bwd, MGC_F64, "bwd");
+        check_shape(a, "fwd"); check_shape(b, "bwd");
+        check_inputs();
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_add_nweights_dense_warm(g_, axis, &a.a, &b.a); }
+        check(rc, g_);
+    }
     double maxflow()
     {
         check_inputs();
@@ -728,6 +757,8 @@ PYBIND11_MODULE(_mgc, m)
         .def("add_seeds", &PyGraph::add_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
         .def("remove_seeds", &PyGraph::remove_seeds, py::arg("fg_ids"), py::arg("bg_ids"))
         .def("add_tweights_warm", &PyGraph::add_tweights_warm, py::arg("ids"), py::arg("src"), py::arg("snk"))
+        .def("add_nweights_warm", &PyGraph::add_nweights_warm, py::arg("i"), py::arg("j"), py::arg("cap"), py::arg("rev_cap"))
+        .def("add_nweights_dense_warm", &PyGraph::add_nweights_dense_warm, py::arg("axis"), py::arg("fwd"), py::arg("bwd"))
         .def("build_voxel_graph", &PyGraph::build_voxel_graph)
         .def_static("slab_comm_unique_id", &PyGraph::slab_comm_unique_id)
         .def("slab_comm_init", &PyGraph::slab_comm_init)

@@ -568,6 +568,159 @@ class GraphDouble:
                 out = numpy.ascontiguousarray(t.reshape(-1), dtype=numpy.float64)
         return out
 
+    def add_nweights_warm(self, i, j, cap, rev_cap):
+        """``sum_edge`` calls on a solved graph, re-solved warm by the next ``maxflow()``: a boundary brush ("do not cut
+        here"), a larger boundary weight, a second boundary term.
+
+        One call ``sum_edge(i[k], j[k], cap[k], rev_cap[k])`` per entry, in order, applied to the residual capacities as
+        the reference applies it to a solved graph (graph.h:456-480); repeated pairs count once per occurrence.  ``i`` /
+        ``j``: 1-D integer arrays of lattice-neighbour node ids in logical C order; ``cap`` / ``rev_cap``: nonnegative
+        finite reals, widened to float64.  Scalars broadcast.  numpy arrays or CUDA tensors, all in one memory space.  Bad
+        ids, pairs that are not lattice neighbours, lengths, negative, NaN or infinite weights raise ``ValueError``.
+
+        Before the first ``maxflow()`` the calls are staged exactly like ``sum_edge``.  After it they are folded into the
+        solved state on the graphs ``add_tweights_warm`` folds into (mgc_add_nweights_warm); any other solved graph raises
+        ``RuntimeError``: ``reset()`` it and build the graph again with the calls."""
+        cuda = any(hasattr(x, "__cuda_array_interface__") for x in (i, j, cap, rev_cap))
+        ii, jj = self._pair_ids(i, cuda, "i"), self._pair_ids(j, cuda, "j")
+        sizes = {int(x.shape[0]) for x in (ii, jj) if x.ndim}
+        if len(sizes) > 1:
+            raise ValueError("i and j differ in length")
+        # a scalar id pair takes the length of the weights, so (5, 6, [1.0, 2.0], 0.0) is two calls on one pair
+        wshapes = [tuple(w.shape) if hasattr(w, "shape") else numpy.shape(w) for w in (cap, rev_cap)]
+        wsizes = {int(sh[0]) for sh in wshapes if len(sh) == 1}
+        m = sizes.pop() if sizes else (wsizes.pop() if len(wsizes) == 1 else 1)
+        ii, jj = (x.expand(m) if cuda else numpy.broadcast_to(x, (m,)) for x in (ii, jj))
+        ii, jj = ((x.contiguous() if cuda else numpy.ascontiguousarray(x)) for x in (ii, jj))
+        c = self._warm_weights(cap, m, False, cuda, "cap")
+        r = self._warm_weights(rev_cap, m, False, cuda, "rev_cap")
+        if not self._solved:
+            if cuda:
+                ii, jj, c, r = (x.cpu().numpy() for x in (ii, jj, c, r))
+            self._stage_nweights_calls(ii, jj, c, r)
+            return
+        if self._sp is not None:
+            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
+                               "rebuild it with the n-link calls instead")
+        self._dirty()
+        self._nat().add_nweights_warm(ii, jj, c, r)
+
+    def add_nweights_dense_warm(self, axis, fwd, bwd):
+        """The dense form of ``add_nweights_warm``, in the layout of ``add_nweights_dense``: ``fwd`` / ``bwd`` have the
+        lattice shape (any strides, read in logical C order) and entry p holds the increments of the arcs p -> p + e_axis
+        and back; the last plane of ``axis`` is ignored.  Entries are nonnegative finite reals, widened to float64; only the
+        pairs with a nonzero entry are touched.  numpy arrays or CUDA tensors, both in one memory space.  A bad axis or
+        shape, negative, NaN or infinite weights raise ``ValueError``.
+
+        Before the first ``maxflow()`` the call is staged exactly like ``add_nweights_dense``.  After it, the same graphs
+        as ``add_nweights_warm`` fold it into the solved state (mgc_add_nweights_dense_warm)."""
+        axis = int(axis)
+        if not 0 <= axis < len(self._shape):
+            raise ValueError("axis {} is out of range for a graph of shape {}".format(axis, self._shape))
+        cuda = any(hasattr(x, "__cuda_array_interface__") for x in (fwd, bwd))
+        arrs = []
+        for w, what in ((fwd, "fwd"), (bwd, "bwd")):
+            if cuda:
+                if not hasattr(w, "__cuda_array_interface__"):
+                    raise ValueError("fwd and bwd must both be host or both be device arrays")
+                import torch
+                t = torch.as_tensor(w)
+                if t.dtype == torch.bool or t.dtype.is_complex:
+                    raise ValueError("{} must hold real numbers".format(what))
+                t = t.to(torch.float64)
+            else:
+                t = numpy.asarray(w)
+                if t.dtype.kind not in "iuf":
+                    raise ValueError("{} must hold real numbers".format(what))
+                t = t.astype(numpy.float64, copy=False)
+            if tuple(t.shape) != self._shape:
+                raise ValueError("{} of shape {} does not match the graph's shape {}".format(what, tuple(t.shape), self._shape))
+            arrs.append(t)
+        fwd, bwd = arrs
+        if not self._solved:
+            if cuda:
+                fwd, bwd = fwd.cpu().numpy(), bwd.cpu().numpy()
+            cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
+            for w, what in ((fwd, "fwd"), (bwd, "bwd")):
+                if not numpy.isfinite(w[cut]).all():
+                    raise ValueError("{} holds NaN or infinite values".format(what))
+                if (w[cut] < 0).any():
+                    raise ValueError("{} holds negative values: a warm n-link edit only raises capacities".format(what))
+            staged = [numpy.zeros(self._shape), numpy.zeros(self._shape)]
+            staged[0][cut], staged[1][cut] = fwd[cut], bwd[cut]        # the last plane of `axis` names no pair
+            self.add_nweights_dense(axis, *staged)
+            return
+        if self._sp is not None:
+            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
+                               "rebuild it with the n-link calls instead")
+        self._dirty()
+        self._nat().add_nweights_dense_warm(axis, fwd, bwd)
+
+    def _pair_ids(self, x, cuda, what):
+        """One id argument of add_nweights_warm: a 1-D int64 array (or a 0-d one for a scalar), numpy or -- when ``cuda``
+        -- a CUDA tensor.  Range-checked in both memory spaces, as ``_seed_ids`` checks seeds: before the first solve the
+        ids go to the staging, where no native check runs."""
+        if cuda:
+            import torch
+            if not hasattr(x, "__cuda_array_interface__") and numpy.ndim(x):
+                raise ValueError("i, j, cap and rev_cap must all be host or all be device arrays")
+            t = torch.as_tensor(x, device="cuda")
+            if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex or t.dim() > 1:
+                raise ValueError("{} must be a 1-D integer node id array or an integer".format(what))
+            t = t.to(torch.int64)
+            if t.numel():
+                self._check_id_range(int(t.min()), int(t.max()))
+            return t
+        a = numpy.asarray(x)
+        if a.ndim > 1 or not (numpy.issubdtype(a.dtype, numpy.integer) or (a.ndim == 1 and a.size == 0)):
+            raise ValueError("{} must be a 1-D integer node id array or an integer".format(what))
+        a = a.astype(numpy.int64)
+        if a.size:
+            self._check_id_range(int(a.min()), int(a.max()))
+        return a
+
+    def _check_id_range(self, lo, hi):
+        if lo < 0 or hi >= self._n:
+            raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(hi, lo, self._n - 1))
+
+    def _stage_nweights_calls(self, i, j, cap, rev):
+        """sum_edge(i[k], j[k], cap[k], rev[k]) in order, staged before the first solve: checked like the warm fold checks
+        them, then added into the dense per-axis batches exactly as ``sum_edge`` adds (repeated pairs in call order)."""
+        for a in (i, j):
+            if a.size:
+                self._check_id_range(int(a.min()), int(a.max()))   # numpy.add.at would wrap a negative id
+        for w, what in ((cap, "cap"), (rev, "rev_cap")):
+            if not numpy.isfinite(w).all():
+                raise ValueError("{} holds NaN or infinite values".format(what))
+            if (w < 0).any():
+                raise ValueError("{} holds negative values: a warm n-link edit only raises capacities".format(what))
+        if self._sp is not None:
+            for a, b, c, r in zip(i.tolist(), j.tolist(), cap.tolist(), rev.tolist()):
+                self._sp.sum_edge(a, b, c, r)
+            return
+        lo, d = numpy.minimum(i, j), numpy.abs(i - j)
+        axes = numpy.full(i.shape, -1, numpy.int64)
+        for axis, st in enumerate(self._strides):
+            n_ax = self._shape[axis]
+            axes[(axes < 0) & (d == st) & ((lo // st) % n_ax < n_ax - 1)] = axis
+        if (axes < 0).any():
+            k = int(numpy.flatnonzero(axes < 0)[0])
+            raise ValueError("node ids ({}, {}) are not lattice neighbours".format(int(i[k]), int(j[k])))
+        if self._journal is not None:
+            for a, b, c, r in zip(i.tolist(), j.tolist(), cap.tolist(), rev.tolist()):
+                self.sum_edge(a, b, c, r)
+            return
+        up = i < j
+        f, b = numpy.where(up, cap, rev), numpy.where(up, rev, cap)
+        for axis in numpy.unique(axes).tolist():
+            sel = axes == axis
+            if axis not in self._st_nw:
+                self._st_nw[axis] = [numpy.zeros(self._n, dtype=numpy.float64), numpy.zeros(self._n, dtype=numpy.float64)]
+            fw, bw = self._st_nw[axis]
+            numpy.add.at(fw, lo[sel], f[sel])        # unbuffered, in index order: a repeated pair adds in call order
+            numpy.add.at(bw, lo[sel], b[sel])
+        self._dirty()
+
     def _stage_tweights_calls(self, ids, src, snk):
         """add_tweights(ids[k], src[k], snk[k]) in order (ids None: one call per node), staged before the first solve.
         The k-th call on a node goes into dense batch k: a node's calls keep their order, and no Python loop runs per
