@@ -191,8 +191,8 @@ struct mgc_graph {
     // caps_tin.prob likewise.  Forgotten by mgc_reset, the per-term calls and every build that is not lazy.
     const void* caps_img = nullptr;
     bool keep_device_inputs = false;   // MGC_OPT_KEEP_DEVICE_INPUTS
-    Buf seed_buf;                      // folds: item count + error flag, inputs, keys, runs, touched tiles, items, cub scratch
-    cudaEvent_t ev_seed[4] = {};       // spans of the grouping and of claim + fold + list fix-up
+    Buf fold_buf;                      // folds: control words, inputs, keys, runs, touched tiles, items, cub scratch
+    cudaEvent_t ev_fold[4] = {};       // spans of the grouping and of claim + fold + list fix-up
     int caps_dtype = MGC_F32;
     BoundaryParams caps_P{};           // the boundary term of the lazy build
     LazyTin caps_tin{};                // its t-link terms
@@ -851,22 +851,55 @@ int materialise_zeros(mgc_graph* g)
 }
 
 // ---- lazy push state: k_caps_tiles over a push worklist or over every tile -----------------------------------------
-template <typename E>
-void caps_launch_t(mgc_graph* g)
+// The instantiation of the lazy build's boundary term, as a tag type: E = the image dtype, FN / USE_MAX / SPACING fixed
+// (>= 0) or read from BoundaryParams at run time (-1).
+template <typename E_, int FN_, int USE_MAX_, int SPACING_>
+struct LazyTerm {
+    using E = E_;
+    static constexpr int FN = FN_, USE_MAX = USE_MAX_, SPACING = SPACING_;
+};
+
+// f(LazyTerm<...>{}) for the handle's caps_dtype / caps_P: <1, 1, 0> and <1, 0, 0> for float images with the exponential
+// term without spacing, <-1, -1, -1> for every other case.  k_caps_tiles and the lazy folds are instantiated here only.
+template <typename F>
+void lazy_dispatch(const mgc_graph* g, F&& f)
 {
-    const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->caps_img;
-    int* count = g->d_flags + 4;              // [4] tiles claimed by this launch, [5] cursor
-    int* done = g->d_flags + 3;               // tiles materialised since the build
-    const unsigned grid = (unsigned)g->n_ctas;
-    if constexpr (!std::is_integral<E>::value) {
-        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
-            if (P.use_max) k_caps_tiles<E, 1, 1, 0><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->caps_tin, g->caps_list, count, count + 1, done);
-            else           k_caps_tiles<E, 1, 0, 0><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->caps_tin, g->caps_list, count, count + 1, done);
-            return;
+    auto by_dtype = [&](auto e) {
+        using E = decltype(e);
+        const BoundaryParams& P = g->caps_P;
+        if constexpr (!std::is_integral<E>::value) {
+            if (P.fn == 1 && P.inv_spacing_on == 0.0) {
+                if (P.use_max) f(LazyTerm<E, 1, 1, 0>{});
+                else           f(LazyTerm<E, 1, 0, 0>{});
+                return;
+            }
         }
+        f(LazyTerm<E, -1, -1, -1>{});
+    };
+    switch (g->caps_dtype) {
+        case MGC_F32: by_dtype(float{}); break;
+        case MGC_F64: by_dtype(double{}); break;
+        case MGC_U8: by_dtype(uint8_t{}); break;
+        case MGC_I16: by_dtype(int16_t{}); break;
+        default: by_dtype(int32_t{}); break;
     }
-    k_caps_tiles<E, -1, -1, -1><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, img, P, g->caps_tin, g->caps_list, count, count + 1, done);
+}
+
+// f(A) with the residual access of a fold on this handle (gc_seeds.cuh): LazyResidual with the lazy build's instantiation,
+// or (eager: an MGC_OPT_WARM handle) EagerResidual<3> / <4>
+template <typename F>
+void residual_dispatch(const mgc_graph* g, bool eager, F&& f)
+{
+    if (eager) {
+        if (g->nd == 4) f(EagerResidual<4>{g->S, g->smask});
+        else            f(EagerResidual<3>{g->S, g->smask});
+        return;
+    }
+    lazy_dispatch(g, [&](auto t) {
+        using T = decltype(t);
+        using E = typename T::E;
+        f(LazyResidual<E, T::FN, T::USE_MAX, T::SPACING>{g->L, g->S, (const E*)g->caps_img, g->caps_P});
+    });
 }
 
 // materialise the tiles of a push worklist and their face neighbours (wl.items == nullptr: every tile), between a pair of
@@ -878,67 +911,18 @@ int caps_launch(mgc_graph* g, WorkList wl)
     CK(cudaEventRecord(g->caps_ev[g->caps_ev_used], g->stream));
     CK(cudaMemsetAsync(g->d_flags + 4, 0, 2 * sizeof(int), g->stream));
     k_caps_claim<<<(unsigned)g->n_ctas * 4u, 256, 0, g->stream>>>(g->TL, g->cmat, wl, g->caps_list, g->d_flags + 4);
-    switch (g->caps_dtype) {
-        case MGC_F32: caps_launch_t<float>(g); break;
-        case MGC_F64: caps_launch_t<double>(g); break;
-        case MGC_U8: caps_launch_t<uint8_t>(g); break;
-        case MGC_I16: caps_launch_t<int16_t>(g); break;
-        default: caps_launch_t<int32_t>(g); break;
-    }
+    int* count = g->d_flags + 4;              // [4] tiles claimed by this launch, [5] cursor
+    int* done = g->d_flags + 3;               // tiles materialised since the build
+    lazy_dispatch(g, [&](auto t) {
+        using T = decltype(t);
+        k_caps_tiles<typename T::E, T::FN, T::USE_MAX, T::SPACING><<<(unsigned)g->n_ctas, TILE_VOX, 0, g->stream>>>(
+            g->L, g->TL, g->S, (const typename T::E*)g->caps_img, g->caps_P, g->caps_tin, g->caps_list, count, count + 1, done);
+    });
     CK(cudaEventRecord(g->caps_ev[g->caps_ev_used + 1], g->stream));
     g->caps_ev_used += 2;
     g->st.kernel_launches += 2;
     CK(cudaGetLastError());
     return MGC_OK;
-}
-
-// k_seed_fold with the boundary term of the lazy build (the instantiations of k_caps_tiles)
-template <typename E>
-void seed_fold_launch_t(mgc_graph* g, unsigned grid, const SeedItem* items, int n, double cap)
-{
-    const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->caps_img;
-    if constexpr (!std::is_integral<E>::value) {
-        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
-            if (P.use_max) k_seed_fold<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, cap, g->partials);
-            else           k_seed_fold<E, 1, 0, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, cap, g->partials);
-            return;
-        }
-    }
-    k_seed_fold<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, cap, g->partials);
-}
-
-// k_tweights_fold with the same instantiations
-template <typename E>
-void tweights_fold_launch_t(mgc_graph* g, unsigned grid, const TweightItem* items, int n, const int* order,
-                            const double* src, const double* snk)
-{
-    const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->caps_img;
-    if constexpr (!std::is_integral<E>::value) {
-        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
-            if (P.use_max) k_tweights_fold<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
-            else           k_tweights_fold<E, 1, 0, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
-            return;
-        }
-    }
-    k_tweights_fold<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, items, n, order, src, snk, g->partials);
-}
-
-// k_nlinks_reclamp with the same instantiations
-template <typename E>
-void nlinks_reclamp_launch_t(mgc_graph* g, unsigned grid, const unsigned* tails, const int* ntails)
-{
-    const BoundaryParams& P = g->caps_P;
-    const E* img = (const E*)g->caps_img;
-    if constexpr (!std::is_integral<E>::value) {
-        if (P.fn == 1 && P.inv_spacing_on == 0.0) {
-            if (P.use_max) k_nlinks_reclamp<E, 1, 1, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, tails, ntails, g->partials);
-            else           k_nlinks_reclamp<E, 1, 0, 0><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, tails, ntails, g->partials);
-            return;
-        }
-    }
-    k_nlinks_reclamp<E, -1, -1, -1><<<grid, 256, 0, g->stream>>>(g->L, g->S, img, P, tails, ntails, g->partials);
 }
 
 // capacities, tr or excess are about to be read or written outside the push path: materialise the tiles that are not yet
@@ -1924,8 +1908,8 @@ void mgc_destroy(mgc_graph* g)
     if (g->img_copy.p) pool_free(g->device, g->img_copy.bytes, g->img_copy.p);
     if (g->prob_copy.p) pool_free(g->device, g->prob_copy.bytes, g->prob_copy.p);
     for (auto& b : g->mark_planes) if (b.p) pool_free(g->device, b.bytes, b.p);
-    if (g->seed_buf.p) pool_free(g->device, g->seed_buf.bytes, g->seed_buf.p);
-    for (auto& ev : g->ev_seed) if (ev) cudaEventDestroy(ev);
+    if (g->fold_buf.p) pool_free(g->device, g->fold_buf.bytes, g->fold_buf.p);
+    for (auto& ev : g->ev_fold) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->caps_ev) if (ev) cudaEventDestroy(ev);
     for (auto& ev : g->ev_slot) if (ev) cudaEventDestroy(ev);
@@ -2565,22 +2549,47 @@ int mgc_maxflow(mgc_graph* g, double* energy)
     return MGC_OK;
 }
 
-// Number of kernels the cub calls of a fold's grouping enqueue, so that kernel_launches counts them too: CUB_SEED_KEYS =
-// cub::DeviceRadixSort::SortKeys + cub::DeviceScan::InclusiveSum (seeds), CUB_PAIRS = SortPairs + InclusiveSum (the list
-// form of mgc_add_tweights_warm), CUB_SCAN = InclusiveSum alone (its dense form, and the dense n-link form), CUB_PAIRS64 =
-// SortPairs on 64-bit keys (passed through `keys` / `skeys`) + InclusiveSum (the list form of mgc_add_nweights_warm).  cub
-// decides it on the host from (n, end_bit) and the device; the calls are captured on a capture-only stream of the device
-// (nothing runs) and the kernel nodes of the captured graph counted.  The stream lives for the process and the counts are
-// cached, so a call pays only the capture of a few launches.
-enum { CUB_SEED_KEYS = 0, CUB_PAIRS = 1, CUB_SCAN = 2, CUB_PAIRS64 = 3 };
-static int seed_cub_launches(mgc_graph* g, int kind, int n, int end_bit, void* tmp, size_t tmp_bytes, unsigned* keys,
-                             unsigned* skeys, int* vals, int* svals, int* head, int* pos, int* out)
+}  // extern "C"
+
+// ---- folds into the residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm / mgc_add_nweights*_warm)
+// The cub calls of a fold's grouping: the radix sort of its keys (FOLD_SORT_KEYS: the keys alone, FOLD_SORT_PAIRS: keys
+// and call indices, stable; FOLD_SCAN: no sort), then the inclusive sum of the heads.  tmp == nullptr only sizes them:
+// *bytes is the larger scratch size of the two.
+enum { FOLD_SORT_KEYS = 0, FOLD_SORT_PAIRS = 1, FOLD_SCAN = 2 };
+template <typename Key>
+static cudaError_t fold_sort(int sort, void* tmp, size_t* bytes, Key* keys, Key* skeys, int* vals, int* svals, int n,
+                             int end_bit, cudaStream_t s)
+{
+    size_t tb = *bytes;
+    cudaError_t e = cudaSuccess;
+    if constexpr (sizeof(Key) == 4)             // seeds sort 32-bit keys only
+        if (sort == FOLD_SORT_KEYS) e = cub::DeviceRadixSort::SortKeys(tmp, tb, keys, skeys, n, 0, end_bit, s);
+    if (sort == FOLD_SORT_PAIRS) e = cub::DeviceRadixSort::SortPairs(tmp, tb, keys, skeys, vals, svals, n, 0, end_bit, s);
+    if (!tmp && sort != FOLD_SCAN) *bytes = tb;
+    return e;
+}
+
+static cudaError_t fold_scan(void* tmp, size_t* bytes, int* head, int* pos, int n, cudaStream_t s)
+{
+    size_t tb = *bytes;
+    const cudaError_t e = cub::DeviceScan::InclusiveSum(tmp, tb, head, pos, n, s);
+    if (!tmp) *bytes = std::max(*bytes, tb);
+    return e;
+}
+
+// Number of kernels the cub calls of a fold's grouping enqueue, so that kernel_launches counts them too.  cub decides it
+// on the host from (n, end_bit) and the device; the calls are captured on a capture-only stream of the device (nothing
+// runs) and the kernel nodes of the captured graph counted.  The stream lives for the process and the counts are cached,
+// so a call pays only the capture of a few launches.
+template <typename Key>
+static int fold_cub_launches(mgc_graph* g, int sort, int n, int end_bit, void* tmp, size_t tmp_bytes, Key* keys, Key* skeys,
+                             int* vals, int* svals, int* head, int* pos, int* out)
 {
     static std::mutex mu;
     static std::map<int, cudaStream_t> streams;
-    static std::map<std::tuple<int, int, int, int>, int> counts;
+    static std::map<std::tuple<int, int, int, int, int>, int> counts;
     std::lock_guard<std::mutex> lock(mu);
-    const auto key = std::make_tuple(g->device, kind, n, end_bit);
+    const auto key = std::make_tuple(g->device, sort, (int)sizeof(Key), n, end_bit);
     auto it = counts.find(key);
     if (it != counts.end()) { *out = it->second; return MGC_OK; }
     cudaStream_t& s = streams[g->device];
@@ -2589,14 +2598,9 @@ static int seed_cub_launches(mgc_graph* g, int kind, int n, int end_bit, void* t
     cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed);
     if (e == cudaSuccess) {
         size_t tb = tmp_bytes;
-        cudaError_t e1 = cudaSuccess;
-        if (kind == CUB_SEED_KEYS) e1 = cub::DeviceRadixSort::SortKeys(tmp, tb, keys, skeys, n, 0, end_bit, s);
-        else if (kind == CUB_PAIRS) e1 = cub::DeviceRadixSort::SortPairs(tmp, tb, keys, skeys, vals, svals, n, 0, end_bit, s);
-        else if (kind == CUB_PAIRS64)
-            e1 = cub::DeviceRadixSort::SortPairs(tmp, tb, (unsigned long long*)keys, (unsigned long long*)skeys, vals, svals, n,
-                                                 0, end_bit, s);
+        cudaError_t e1 = fold_sort(sort, tmp, &tb, keys, skeys, vals, svals, n, end_bit, s);
         tb = tmp_bytes;
-        cudaError_t e2 = e1 == cudaSuccess ? cub::DeviceScan::InclusiveSum(tmp, tb, head, pos, n, s) : e1;
+        cudaError_t e2 = e1 == cudaSuccess ? fold_scan(tmp, &tb, head, pos, n, s) : e1;
         e = cudaStreamEndCapture(s, &graph);
         if (e == cudaSuccess) e = e2;
     }
@@ -2630,21 +2634,21 @@ static int warm_check(mgc_graph* g, bool* eager)
                       "the seeds instead");
 }
 
-// The steps of a fold after its grouping, shared by seeds_fold, mgc_add_tweights_warm and nweights_fold.  The grouping was enqueued after
-// ev_seed[0] and left d_ctl = [item count | FOLD_ERR_* bits | touched-tile count] and the touched tiles in `tiles`;
-// fold(grid, n_items) enqueues the fold kernel, which stores one partial of the add_tweights constant per block.
+// The steps of a fold after its grouping (fold_run).  The grouping was enqueued after ev_fold[0] and left d_ctl = [item
+// count | FOLD_ERR_* bits | touched-tile count] and the touched tiles in `tiles`; fold(grid, n_items) enqueues the fold
+// kernel, which stores one partial of the add_tweights constant per block.  `nonfinite` is the message of
+// FOLD_ERR_NONFINITE, which names the kind of weight.
 static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<void(unsigned, int)>& fold,
-                      bool nlinks = false)
+                      const char* nonfinite)
 {
-    CK(cudaEventRecord(g->ev_seed[1], g->stream));
+    CK(cudaEventRecord(g->ev_fold[1], g->stream));
     // the item count and the error bits in one synchronisation, before the claim and the fold are enqueued
     int h_ctl[2] = {0, 0};
     CK(cudaMemcpyAsync(h_ctl, d_ctl, sizeof(h_ctl), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
     if (h_ctl[1] & FOLD_ERR_RANGE) FAIL(MGC_E_ARG, "node id out of range");
     if (h_ctl[1] & FOLD_ERR_PAIR) FAIL(MGC_E_ARG, "node ids are not lattice neighbours");
-    if (h_ctl[1] & FOLD_ERR_NONFINITE)
-        FAIL(MGC_E_ARG, nlinks ? "an n-link weight is NaN or infinite" : "a t-link weight is NaN or infinite");
+    if (h_ctl[1] & FOLD_ERR_NONFINITE) FAIL(MGC_E_ARG, nonfinite);
     if (h_ctl[1] & FOLD_ERR_NEGATIVE)
         FAIL(MGC_E_WEIGHT, "negative n-link weights are not allowed (a warm fold only raises capacities)");
     const int ni = h_ctl[0];
@@ -2656,7 +2660,7 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
         int rc = warm_prepare(g);
         if (rc) return rc;
     }
-    CK(cudaEventRecord(g->ev_seed[2], g->stream));
+    CK(cudaEventRecord(g->ev_fold[2], g->stream));
     // 1. every touched voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
     if (g->caps_lazy) {
         // Source excess is still implicit on the tiles that are listed but not materialised (before the first solve, or
@@ -2690,13 +2694,13 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     }
     g->st.kernel_launches += 3;
     CK(cudaGetLastError());
-    CK(cudaEventRecord(g->ev_seed[3], g->stream));
-    CK(cudaEventSynchronize(g->ev_seed[3]));
+    CK(cudaEventRecord(g->ev_fold[3], g->stream));
+    CK(cudaEventSynchronize(g->ev_fold[3]));
     {
         // two device spans: the grouping, then claim + fold + list fix-up (the read-back between them is not counted)
         float ms0 = 0, ms1 = 0;
-        if (cudaEventElapsedTime(&ms0, g->ev_seed[0], g->ev_seed[1]) == cudaSuccess &&
-            cudaEventElapsedTime(&ms1, g->ev_seed[2], g->ev_seed[3]) == cudaSuccess)
+        if (cudaEventElapsedTime(&ms0, g->ev_fold[0], g->ev_fold[1]) == cudaSuccess &&
+            cudaEventElapsedTime(&ms1, g->ev_fold[2], g->ev_fold[3]) == cudaSuccess)
             g->st.ms_seeds += ms0 + ms1;
         g->st.ms_caps -= caps_resolve(g);          // the claim is part of ms_seeds, not of the solve's materialisation
     }
@@ -2709,105 +2713,185 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     return MGC_OK;
 }
 
+// One fold call as its entry point describes it to fold_run: the argument checks, the inputs, and how the grouping keys
+// its calls.  The rest of a fold is the same for seeds, t-links and n-links.
+struct FoldCall {
+    const char* range;            // NVTX range
+    const char* bad;              // MGC_E_ARG message of malformed arrays or counts (nullptr: well formed)
+    const char* too_many;         // MGC_E_ARG message of more than 2^31 - 1 calls
+    int64_t count;                // calls: seed ids, add_tweights or sum_edge calls, or dense entries
+    int32_t mem;                  // memory space of in[]
+    bool dense;                   // one entry per voxel (count == the voxel count)
+    const void* in[4];            // input arrays of 8-byte elements, in[k] with in_n[k] of them (nullptr: unused)
+    int64_t in_n[4];
+    const mgc_array* arrays[2];   // dense inputs as caller arrays, staged into in[2] / in[3] through slots 0 / 1
+    int sort;                     // FOLD_SORT_KEYS / FOLD_SORT_PAIRS / FOLD_SCAN
+    int key_shift;                // a key is voxel << key_shift | low bits: it has the bits of n << key_shift - 1
+    int axis;                     // k_nlinks_items: the axis of the dense form
+};
+
+// The device buffers of a fold in fold_buf, 16-byte aligned pieces in this order
+template <typename Key, typename Item>
+struct FoldBufs {
+    int* ctl;                     // [item count | FOLD_ERR_* bits | touched-tile count | tail count]
+    const void* in[4];            // the inputs on the device: host arrays uploaded, device arrays in place
+    Key* keys;                    // list forms: the keys of the calls, and sorted
+    Key* skeys;
+    int* vals;                    // pair sorts: the call indices, and sorted (each key's calls in call order)
+    int* svals;
+    int* head;                    // item heads, and their inclusive sum
+    int* pos;
+    int* tflag;                   // lazy handles: per-tile flags, and the touched tiles for the claim
+    int* tiles;
+    Item* items;
+    unsigned* tbits;              // n-links: per-voxel tail bits, and the tails for the re-clamp
+    unsigned* tails;
+    void* tmp;                    // cub scratch
+};
+
+// A bump allocator of 16-byte aligned pieces over one buffer; base == nullptr only measures the pieces
+struct Bump {
+    char* base;
+    size_t used;
+    template <typename T>
+    T* take(size_t count)
+    {
+        T* p = base ? (T*)(base + used) : nullptr;
+        used += (count * sizeof(T) + 15) / 16 * 16;
+        return p;
+    }
+};
+
+// A fold: the checks, the grouping of the calls into items on the device, then fold_items.  An item of NlinkItem names an
+// arc: both ends are listed for the claim and its tails re-clamped.  group(b, grid) enqueues the keys, the sort
+// (fold_sort) and the heads of the calls; fold(b, grid, n_items) the fold kernel(s).
+template <typename Key, typename Item, typename Group, typename Fold>
+static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold)
+{
+    constexpr bool arcs = std::is_same<Item, NlinkItem>::value;
+    if (!g) return MGC_E_ARG;
+    if (c.bad) FAIL(MGC_E_ARG, c.bad);
+    if (c.count > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, c.too_many);
+    if (c.mem != MGC_MEM_HOST && c.mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
+    bool eager = false;
+    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
+    if (c.dense && c.count && c.count != (int64_t)g->L.n) FAIL(MGC_E_ARG, "the dense form takes one weight pair per voxel");
+    CK(cudaSetDevice(g->device));
+    { int rc0 = check_pending(g); if (rc0) return rc0; }
+    const void* in[4] = {c.in[0], c.in[1], c.in[2], c.in[3]};
+    for (int k = 0; k < 2; ++k)
+        if (c.arrays[k]) { int rc0 = stage_input(g, c.arrays[k], k, &in[2 + k]); if (rc0) return rc0; }
+    int rc = MGC_OK;
+    if (c.count) {                              // else nothing to fold: the solved state, mask and energy stay as they are
+        const auto host_t0 = std::chrono::steady_clock::now();
+        const int n = (int)c.count;
+        // sort only the bits a key of this lattice can have
+        int end_bit = 1;
+        while (end_bit < 8 * (int)sizeof(Key) && (((uint64_t)g->L.n << c.key_shift) - 1ull) >> end_bit) ++end_bit;
+        size_t tmp_bytes = 0;
+        CK(fold_sort(c.sort, nullptr, &tmp_bytes, (Key*)nullptr, (Key*)nullptr, nullptr, nullptr, n, end_bit, g->stream));
+        CK(fold_scan(nullptr, &tmp_bytes, nullptr, nullptr, n, g->stream));
+        // no host slots for device inputs, no keys or call indices in a dense form, no tiles on an eager handle (nothing
+        // to claim), no tails but for n-links
+        const bool host = c.mem == MGC_MEM_HOST;
+        const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
+        const size_t nk = c.sort == FOLD_SCAN ? 0 : (size_t)n;
+        const size_t nv = c.sort == FOLD_SORT_PAIRS ? (size_t)n : 0;
+        const size_t claims = std::min((arcs ? 2 : 1) * (size_t)n, ntl);
+        const size_t ntails = arcs ? std::min(2 * (size_t)n, (size_t)g->L.n) : 0;
+        const size_t nbits = arcs ? ((size_t)g->L.n + 31) / 32 : 0;
+        FoldBufs<Key, Item> b{};
+        auto layout = [&](Bump m) {
+            b.ctl = m.take<int>(4);
+            for (int k = 0; k < 4; ++k)
+                b.in[k] = host && c.in[k] ? m.take<int64_t>((size_t)c.in_n[k]) : in[k];
+            b.keys = m.take<Key>(nk);
+            b.skeys = m.take<Key>(nk);
+            b.vals = m.take<int>(nv);
+            b.svals = m.take<int>(nv);
+            b.head = m.take<int>(n);
+            b.pos = m.take<int>(n);
+            b.tflag = m.take<int>(ntl);
+            b.tiles = m.take<int>(claims);
+            b.items = m.take<Item>(n);
+            b.tbits = m.take<unsigned>(nbits);
+            b.tails = m.take<unsigned>(ntails);
+            b.tmp = m.take<char>(tmp_bytes);
+            return m.used;
+        };
+        rc = ensure_scratch(g, g->fold_buf, layout(Bump{nullptr, 0}));
+        if (rc) return rc;
+        layout(Bump{(char*)g->fold_buf.p, 0});
+        int cub_launches = 0;
+        rc = fold_cub_launches(g, c.sort, n, end_bit, b.tmp, tmp_bytes, b.keys, b.skeys, b.vals, b.svals, b.head, b.pos,
+                               &cub_launches);
+        if (rc) return rc;
+        for (auto& ev : g->ev_fold) if (!ev) CK(cudaEventCreate(&ev));
+        Nvtx range(c.range);
+        g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
+        // 0. grouping on the device; nothing below touches the solver state until the checks of the calls have passed.
+        // Host arrays go straight from the caller into their device slots: no host pass over them.
+        CK(cudaEventRecord(g->ev_fold[0], g->stream));
+        for (int k = 0; k < 4; ++k)
+            if (host && c.in[k] && c.in_n[k])
+                CK(cudaMemcpyAsync((void*)b.in[k], c.in[k], (size_t)c.in_n[k] * 8, cudaMemcpyHostToDevice, g->stream));
+        CK(cudaMemsetAsync(b.ctl, 0, 4 * sizeof(int), g->stream));
+        CK(cudaMemsetAsync(b.tflag, 0, ntl * sizeof(int), g->stream));
+        if (arcs) CK(cudaMemsetAsync(b.tbits, 0, nbits * 4, g->stream));
+        const unsigned kgrid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
+        rc = group(b, kgrid, [&]() { return fold_sort(c.sort, b.tmp, &tmp_bytes, b.keys, b.skeys, b.vals, b.svals, n,
+                                                      end_bit, g->stream); });
+        if (rc) return rc;
+        CK(fold_scan(b.tmp, &tmp_bytes, b.head, b.pos, n, g->stream));
+        int* tflag = eager ? nullptr : b.tflag;
+        const Key* skeys = c.sort == FOLD_SCAN ? nullptr : b.skeys;
+        if constexpr (arcs)
+            k_nlinks_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, skeys, c.axis, b.pos, n, b.items, tflag, b.tiles, b.ctl);
+        else
+            k_tweights_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, skeys, c.key_shift, b.pos, n, b.items, tflag, b.tiles,
+                                                           b.ctl);
+        g->st.kernel_launches += (c.sort == FOLD_SCAN ? 2 : 3) + cub_launches;
+        CK(cudaGetLastError());
+        rc = fold_items(g, b.ctl, b.tiles, [&](unsigned grid, int ni) { fold(b, eager, grid, ni); },
+                        arcs ? "an n-link weight is NaN or infinite" : "a t-link weight is NaN or infinite");
+    }
+    if (c.arrays[0]) slots_release(g, 3u);     // the grouping and the fold read the staging slots
+    return rc;
+}
+
+extern "C" {
+
 // mgc_add_seeds (cap = 65535) and mgc_remove_seeds (cap = -65535): add_tweights(v, cap, 0) for every fg id in list order,
-// then add_tweights(v, 0, cap) for every bg id, folded into the handle's current state
+// then add_tweights(v, 0, cap) for every bg id, folded into the handle's current state.  Key = v << 1 | (background):
+// sorted, a voxel's fg seeds precede its bg seeds, the reference's order for one voxel (a voxel's t-link only depends on
+// its own calls).
 static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem,
                       double cap)
 {
-    if (!g) return MGC_E_ARG;
-    if (n_fg < 0 || n_bg < 0 || (n_fg && !fg_ids) || (n_bg && !bg_ids)) FAIL(MGC_E_ARG, "bad seed lists");
-    if (n_fg + n_bg > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 seeds in one call");
-    if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
-    bool eager = false;
-    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
-    CK(cudaSetDevice(g->device));
-    { int rc0 = check_pending(g); if (rc0) return rc0; }
-    if (n_fg + n_bg == 0) return MGC_OK;       // nothing to fold: the solved state, mask and energy stay as they are
-    const auto host_t0 = std::chrono::steady_clock::now();
-    const int n = (int)(n_fg + n_bg);
-    // key = v << 1 | (background): sorted, a voxel's fg seeds precede its bg seeds, the reference's order for one voxel
-    // (a voxel's t-link only depends on its own calls).  Sort only the bits a key of this lattice can have.
-    int end_bit = 1;
-    while (end_bit < 32 && (2ull * g->L.n - 1ull) >> end_bit) ++end_bit;
-    size_t sort_bytes = 0, scan_bytes = 0;
-    CK(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, n, 0, end_bit,
-                                      g->stream));
-    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
-    // device layout (16-byte aligned pieces): [item count | error flag | seeded-tile count | pad] [host ids] [keys]
-    // [sorted keys] [run heads] [run positions] [per-tile flags] [seeded tiles] [items] [cub scratch]; no tiles on an eager
-    // handle (nothing to claim)
-    auto al = [](size_t b) { return (b + 15) / 16 * 16; };
-    const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
-    const size_t ids_off = 16;
-    const size_t keys_off = ids_off + (mem == MGC_MEM_HOST ? al((size_t)n * 8) : 0);
-    const size_t skeys_off = keys_off + al((size_t)n * 4);
-    const size_t head_off = skeys_off + al((size_t)n * 4);
-    const size_t pos_off = head_off + al((size_t)n * 4);
-    const size_t tflag_off = pos_off + al((size_t)n * 4);
-    const size_t tiles_off = tflag_off + al(ntl * 4);
-    const size_t items_off = tiles_off + al(std::min((size_t)n, ntl) * 4);
-    const size_t tmp_off = items_off + al((size_t)n * sizeof(SeedItem));
-    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
-    const size_t bytes = tmp_off + tmp_bytes;
-    int rc = ensure_scratch(g, g->seed_buf, bytes);
-    if (rc) return rc;
-    char* dbuf = (char*)g->seed_buf.p;
-    int* d_count = (int*)dbuf;
-    unsigned* keys = (unsigned*)(dbuf + keys_off);
-    unsigned* skeys = (unsigned*)(dbuf + skeys_off);
-    int* head = (int*)(dbuf + head_off);
-    int* pos = (int*)(dbuf + pos_off);
-    int* tflag = (int*)(dbuf + tflag_off);
-    int* tiles = (int*)(dbuf + tiles_off);
-    SeedItem* d_items = (SeedItem*)(dbuf + items_off);
-    int cub_launches = 0;
-    rc = seed_cub_launches(g, CUB_SEED_KEYS, n, end_bit, dbuf + tmp_off, tmp_bytes, keys, skeys, nullptr, nullptr, head,
-                           pos, &cub_launches);
-    if (rc) return rc;
-    for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
-    Nvtx range(cap > 0 ? "mgc:add_seeds" : "mgc:remove_seeds");
-    g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
-    // 0. grouping on the device; nothing below touches the solver state until the range check has passed
-    CK(cudaEventRecord(g->ev_seed[0], g->stream));
-    const int64_t* d_fg = fg_ids;
-    const int64_t* d_bg = bg_ids;
-    if (mem == MGC_MEM_HOST) {
-        // host ids go straight from the caller's arrays into adjacent device slots (fg, then bg): no host pass over them;
-        // device ids are read in place
-        int64_t* d_ids = (int64_t*)(dbuf + ids_off);
-        if (n_fg) CK(cudaMemcpyAsync(d_ids, fg_ids, (size_t)n_fg * 8, cudaMemcpyHostToDevice, g->stream));
-        if (n_bg) CK(cudaMemcpyAsync(d_ids + n_fg, bg_ids, (size_t)n_bg * 8, cudaMemcpyHostToDevice, g->stream));
-        d_fg = d_ids;
-        d_bg = d_ids + n_fg;
-    }
-    CK(cudaMemsetAsync(d_count, 0, 3 * sizeof(int), g->stream));
-    CK(cudaMemsetAsync(tflag, 0, ntl * sizeof(int), g->stream));
-    {
-        const unsigned kgrid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
-        k_seed_keys<<<kgrid, 256, 0, g->stream>>>(d_fg, (int)n_fg, d_bg, (int)n_bg, (int64_t)g->L.n, keys, d_count + 1);
-        size_t tb = tmp_bytes;
-        CK(cub::DeviceRadixSort::SortKeys(dbuf + tmp_off, tb, keys, skeys, n, 0, end_bit, g->stream));
-        k_seed_heads<<<kgrid, 256, 0, g->stream>>>(skeys, n, head);
-        tb = tmp_bytes;
-        CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
-        k_seed_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, skeys, pos, n, d_items, eager ? nullptr : tflag, tiles, d_count);
-        g->st.kernel_launches += 3 + cub_launches;
-        CK(cudaGetLastError());
-    }
-    return fold_items(g, d_count, tiles, [&](unsigned grid, int ni) {
-        if (eager) {
-            if (g->nd == 4) k_seed_fold_eager<4><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, cap, g->partials);
-            else            k_seed_fold_eager<3><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, cap, g->partials);
-            return;
-        }
-        switch (g->caps_dtype) {
-            case MGC_F32: seed_fold_launch_t<float>(g, grid, d_items, ni, cap); break;
-            case MGC_F64: seed_fold_launch_t<double>(g, grid, d_items, ni, cap); break;
-            case MGC_U8: seed_fold_launch_t<uint8_t>(g, grid, d_items, ni, cap); break;
-            case MGC_I16: seed_fold_launch_t<int16_t>(g, grid, d_items, ni, cap); break;
-            default: seed_fold_launch_t<int32_t>(g, grid, d_items, ni, cap); break;
-        }
-    });
+    const bool bad = n_fg < 0 || n_bg < 0 || (n_fg && !fg_ids) || (n_bg && !bg_ids);
+    FoldCall c{};
+    c.range = cap > 0 ? "mgc:add_seeds" : "mgc:remove_seeds";
+    c.bad = bad ? "bad seed lists" : nullptr;
+    c.too_many = "more than 2^31 - 1 seeds in one call";
+    c.count = bad ? 0 : n_fg + n_bg;
+    c.mem = mem;
+    c.in[0] = fg_ids; c.in_n[0] = n_fg;
+    c.in[1] = bg_ids; c.in_n[1] = n_bg;
+    c.sort = FOLD_SORT_KEYS;
+    c.key_shift = 1;
+    return fold_run<unsigned, TweightItem>(g, c,
+        [&](const FoldBufs<unsigned, TweightItem>& b, unsigned kgrid, auto sort) {
+            k_seed_keys<<<kgrid, 256, 0, g->stream>>>((const int64_t*)b.in[0], (int)n_fg, (const int64_t*)b.in[1], (int)n_bg,
+                                                      (int64_t)g->L.n, b.keys, b.ctl + 1);
+            CK(sort());
+            k_seed_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, (int)(n_fg + n_bg), b.head);
+            return MGC_OK;
+        },
+        [&](const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni) {
+            residual_dispatch(g, eager, [&](auto A) {
+                k_tlink_fold<<<grid, 256, 0, g->stream>>>(A, b.items, ni, SeedCalls{b.skeys, cap}, g->partials);
+            });
+        });
 }
 
 int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem)
@@ -2820,267 +2904,106 @@ int mgc_remove_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const in
     return seeds_fold(g, fg_ids, n_fg, bg_ids, n_bg, mem, -65535.0);
 }
 
+// list form: (voxel id, call index) pairs, stably sorted so a voxel's calls keep their order, then run-length encoded;
+// dense form (ids == nullptr): the voxels with a nonzero weight, compacted by a scan of their flags.  In both, a voxel
+// whose calls all have zero weights is no item (add_tweights(v, 0, 0) changes nothing).
 int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, const double* snk, int64_t count, int32_t mem)
 {
-    if (!g) return MGC_E_ARG;
-    if (count < 0 || (count && (!src || !snk))) FAIL(MGC_E_ARG, "bad t-link arrays");
-    if (count > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 add_tweights calls in one call");
-    if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
-    bool eager = false;
-    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
     const bool dense = ids == nullptr;
-    if (dense && count && count != (int64_t)g->L.n) FAIL(MGC_E_ARG, "the dense form takes one weight pair per voxel");
-    CK(cudaSetDevice(g->device));
-    { int rc0 = check_pending(g); if (rc0) return rc0; }
-    if (count == 0) return MGC_OK;             // nothing to fold: the solved state, mask and energy stay as they are
-    const auto host_t0 = std::chrono::steady_clock::now();
-    const int n = (int)count;
-    // list form: (voxel id, call index) pairs sorted on the bits a voxel id of this lattice can have, then run-length
-    // encoded; dense form: the voxels with a nonzero weight, compacted by a scan of their flags.  In both, a voxel whose
-    // calls all have zero weights is no item (add_tweights(v, 0, 0) changes nothing)
-    int end_bit = 1;
-    while (end_bit < 32 && ((uint64_t)g->L.n - 1ull) >> end_bit) ++end_bit;
-    size_t sort_bytes = 0, scan_bytes = 0;
-    if (!dense)
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr,
-                                           (const int*)nullptr, (int*)nullptr, n, 0, end_bit, g->stream));
-    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
-    // device layout (16-byte aligned pieces): [item count | error bits | touched-tile count | pad] [host ids] [host src]
-    // [host snk] [keys] [sorted keys] [call indices] [sorted call indices] [heads] [positions] [per-tile flags]
-    // [touched tiles] [items] [cub scratch]; no ids, keys or call indices in the dense form, no tiles on an eager handle
-    auto al = [](size_t b) { return (b + 15) / 16 * 16; };
-    const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
-    const bool host = mem == MGC_MEM_HOST;
-    const size_t w4 = dense ? 0 : al((size_t)n * 4);
-    const size_t ids_off = 16;
-    const size_t src_off = ids_off + (host && !dense ? al((size_t)n * 8) : 0);
-    const size_t snk_off = src_off + (host ? al((size_t)n * 8) : 0);
-    const size_t keys_off = snk_off + (host ? al((size_t)n * 8) : 0);
-    const size_t skeys_off = keys_off + w4;
-    const size_t vals_off = skeys_off + w4;
-    const size_t svals_off = vals_off + w4;
-    const size_t head_off = svals_off + w4;
-    const size_t pos_off = head_off + al((size_t)n * 4);
-    const size_t tflag_off = pos_off + al((size_t)n * 4);
-    const size_t tiles_off = tflag_off + al(ntl * 4);
-    const size_t items_off = tiles_off + al(std::min((size_t)n, ntl) * 4);
-    const size_t tmp_off = items_off + al((size_t)n * sizeof(TweightItem));
-    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
-    int rc = ensure_scratch(g, g->seed_buf, tmp_off + tmp_bytes);
-    if (rc) return rc;
-    char* dbuf = (char*)g->seed_buf.p;
-    int* d_ctl = (int*)dbuf;
-    unsigned* keys = (unsigned*)(dbuf + keys_off);
-    unsigned* skeys = (unsigned*)(dbuf + skeys_off);
-    int* vals = (int*)(dbuf + vals_off);
-    int* svals = (int*)(dbuf + svals_off);
-    int* head = (int*)(dbuf + head_off);
-    int* pos = (int*)(dbuf + pos_off);
-    int* tflag = (int*)(dbuf + tflag_off);
-    int* tiles = (int*)(dbuf + tiles_off);
-    TweightItem* d_items = (TweightItem*)(dbuf + items_off);
-    int cub_launches = 0;
-    rc = seed_cub_launches(g, dense ? CUB_SCAN : CUB_PAIRS, n, end_bit, dbuf + tmp_off, tmp_bytes, keys, skeys, vals, svals,
-                           head, pos, &cub_launches);
-    if (rc) return rc;
-    for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
-    Nvtx range("mgc:add_tweights_warm");
-    g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
-    // 0. grouping on the device; nothing below touches the solver state until the range and finiteness checks have passed
-    CK(cudaEventRecord(g->ev_seed[0], g->stream));
-    const int64_t* d_ids = ids;
-    const double* d_src = src;
-    const double* d_snk = snk;
-    if (host) {
-        // host arrays go straight from the caller into device slots; device arrays are read in place
-        if (!dense) {
-            CK(cudaMemcpyAsync(dbuf + ids_off, ids, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-            d_ids = (const int64_t*)(dbuf + ids_off);
-        }
-        CK(cudaMemcpyAsync(dbuf + src_off, src, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-        CK(cudaMemcpyAsync(dbuf + snk_off, snk, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-        d_src = (const double*)(dbuf + src_off);
-        d_snk = (const double*)(dbuf + snk_off);
-    }
-    CK(cudaMemsetAsync(d_ctl, 0, 3 * sizeof(int), g->stream));
-    CK(cudaMemsetAsync(tflag, 0, ntl * sizeof(int), g->stream));
-    {
-        const unsigned kgrid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
-        size_t tb = tmp_bytes;
-        if (dense) {
-            k_tweights_dense_heads<<<kgrid, 256, 0, g->stream>>>(d_src, d_snk, n, head, d_ctl + 1);
-        } else {
-            k_tweights_keys<<<kgrid, 256, 0, g->stream>>>(d_ids, d_src, d_snk, n, (int64_t)g->L.n, keys, vals, d_ctl + 1);
-            CK(cub::DeviceRadixSort::SortPairs(dbuf + tmp_off, tb, keys, skeys, vals, svals, n, 0, end_bit, g->stream));
-            k_tweights_heads<<<kgrid, 256, 0, g->stream>>>(skeys, svals, d_src, d_snk, n, head);
-            tb = tmp_bytes;
-        }
-        CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
-        k_tweights_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, dense ? nullptr : skeys, pos, n, d_items,
-                                                       eager ? nullptr : tflag, tiles, d_ctl);
-        g->st.kernel_launches += (dense ? 2 : 3) + cub_launches;
-        CK(cudaGetLastError());
-    }
-    const int* order = dense ? nullptr : svals;
-    return fold_items(g, d_ctl, tiles, [&](unsigned grid, int ni) {
-        if (eager) {
-            if (g->nd == 4) k_tweights_fold_eager<4><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, order, d_src, d_snk, g->partials);
-            else            k_tweights_fold_eager<3><<<grid, 256, 0, g->stream>>>(g->S, g->smask, d_items, ni, order, d_src, d_snk, g->partials);
-            return;
-        }
-        switch (g->caps_dtype) {
-            case MGC_F32: tweights_fold_launch_t<float>(g, grid, d_items, ni, order, d_src, d_snk); break;
-            case MGC_F64: tweights_fold_launch_t<double>(g, grid, d_items, ni, order, d_src, d_snk); break;
-            case MGC_U8: tweights_fold_launch_t<uint8_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
-            case MGC_I16: tweights_fold_launch_t<int16_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
-            default: tweights_fold_launch_t<int32_t>(g, grid, d_items, ni, order, d_src, d_snk); break;
-        }
-    });
+    FoldCall c{};
+    c.range = "mgc:add_tweights_warm";
+    c.bad = count < 0 || (count && (!src || !snk)) ? "bad t-link arrays" : nullptr;
+    c.too_many = "more than 2^31 - 1 add_tweights calls in one call";
+    c.count = count;
+    c.mem = mem;
+    c.dense = dense;
+    c.in[0] = ids; c.in_n[0] = count;
+    c.in[1] = src; c.in_n[1] = count;
+    c.in[2] = snk; c.in_n[2] = count;
+    c.sort = dense ? FOLD_SCAN : FOLD_SORT_PAIRS;
+    return fold_run<unsigned, TweightItem>(g, c,
+        [&](const FoldBufs<unsigned, TweightItem>& b, unsigned kgrid, auto sort) {
+            const double* d_src = (const double*)b.in[1];
+            const double* d_snk = (const double*)b.in[2];
+            if (dense) {
+                k_tweights_dense_heads<<<kgrid, 256, 0, g->stream>>>(d_src, d_snk, (int)count, b.head, b.ctl + 1);
+                return MGC_OK;
+            }
+            k_tweights_keys<<<kgrid, 256, 0, g->stream>>>((const int64_t*)b.in[0], d_src, d_snk, (int)count, (int64_t)g->L.n,
+                                                          b.keys, b.vals, b.ctl + 1);
+            CK(sort());
+            k_weighted_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_src, d_snk, (int)count, b.head);
+            return MGC_OK;
+        },
+        [&](const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni) {
+            const ListCalls calls{dense ? nullptr : b.svals, (const double*)b.in[1], (const double*)b.in[2]};
+            residual_dispatch(g, eager, [&](auto A) {
+                k_tlink_fold<<<grid, 256, 0, g->stream>>>(A, b.items, ni, calls, g->partials);
+            });
+        });
 }
 
 // sum_edge calls folded into the handle's current state (gc_nlinks.cuh).  ii != nullptr: the list form, call k is
-// sum_edge(ii[k], jj[k], cap[k], rev[k]) with every array in `mem`.  ii == nullptr: the dense form along canonical axis
-// `axis`, entry p of cap / rev (device memory, count = the voxel count) holds the increments of p -> p + e_axis and back.
-static int nweights_fold(mgc_graph* g, const int64_t* ii, const int64_t* jj, const double* cap, const double* rev,
-                         int64_t count, int32_t mem, int axis, bool eager)
+// sum_edge(ii[k], jj[k], cap[k], rev[k]) with every array in `mem`: (arc key, call index) pairs, key = lo << 2 | axis,
+// stably sorted, then run-length encoded.  ii == nullptr: the dense form along canonical axis `axis`, entry p of the
+// staged cap / rev (count = the voxel count) holds the increments of p -> p + e_axis and back; the pairs with a nonzero
+// increment are compacted by a scan of their flags.
+static int nweights_fold(mgc_graph* g, FoldCall& c, int axis)
 {
-    if (count == 0) return MGC_OK;             // nothing to fold: the solved state, mask and energy stay as they are
-    const auto host_t0 = std::chrono::steady_clock::now();
-    const bool dense = ii == nullptr;
-    const int n = (int)count;
-    // list form: (arc key, call index) pairs, key = lo << 2 | axis, sorted on the bits a key of this lattice can have, then
-    // run-length encoded; dense form: the pairs with a nonzero increment, compacted by a scan of their flags
-    int end_bit = 1;
-    while (end_bit < 64 && ((4ull * g->L.n - 1ull) >> end_bit)) ++end_bit;
-    size_t sort_bytes = 0, scan_bytes = 0;
-    if (!dense)
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                           (const int*)nullptr, (int*)nullptr, n, 0, end_bit, g->stream));
-    CK(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, n, g->stream));
-    // device layout (16-byte aligned pieces): [item count | error bits | touched-tile count | tail count] [host i] [host j]
-    // [host cap] [host rev] [keys] [sorted keys] [call indices] [sorted call indices] [heads] [positions] [per-tile flags]
-    // [touched tiles] [items] [per-voxel tail bits] [tails] [cub scratch]; the dense form has no ids, keys or call indices,
-    // an eager handle no tiles
-    auto al = [](size_t b) { return (b + 15) / 16 * 16; };
-    const size_t ntl = eager ? 0 : (size_t)g->TL.ntiles;
-    const bool host = mem == MGC_MEM_HOST;
-    const size_t w8 = dense ? 0 : al((size_t)n * 8), w4 = dense ? 0 : al((size_t)n * 4), hw = host ? w8 : 0;
-    const size_t i_off = 16;
-    const size_t j_off = i_off + hw;
-    const size_t cap_off = j_off + hw;
-    const size_t rev_off = cap_off + hw;
-    const size_t keys_off = rev_off + hw;
-    const size_t skeys_off = keys_off + w8;
-    const size_t vals_off = skeys_off + w8;
-    const size_t svals_off = vals_off + w4;
-    const size_t head_off = svals_off + w4;
-    const size_t pos_off = head_off + al((size_t)n * 4);
-    const size_t tflag_off = pos_off + al((size_t)n * 4);
-    const size_t tiles_off = tflag_off + al(ntl * 4);
-    const size_t items_off = tiles_off + al(std::min(2 * (size_t)n, ntl) * 4);
-    const size_t tbits_off = items_off + al((size_t)n * sizeof(NlinkItem));
-    const size_t tbits_bytes = ((size_t)g->L.n + 31) / 32 * 4;
-    const size_t tails_off = tbits_off + al(tbits_bytes);
-    const size_t tmp_off = tails_off + al(std::min(2 * (size_t)n, (size_t)g->L.n) * 4);
-    const size_t tmp_bytes = std::max(sort_bytes, scan_bytes);
-    int rc = ensure_scratch(g, g->seed_buf, tmp_off + tmp_bytes);
-    if (rc) return rc;
-    char* dbuf = (char*)g->seed_buf.p;
-    int* d_ctl = (int*)dbuf;
-    auto* keys = (unsigned long long*)(dbuf + keys_off);
-    auto* skeys = (unsigned long long*)(dbuf + skeys_off);
-    int* vals = (int*)(dbuf + vals_off);
-    int* svals = (int*)(dbuf + svals_off);
-    int* head = (int*)(dbuf + head_off);
-    int* pos = (int*)(dbuf + pos_off);
-    int* tflag = (int*)(dbuf + tflag_off);
-    int* tiles = (int*)(dbuf + tiles_off);
-    NlinkItem* d_items = (NlinkItem*)(dbuf + items_off);
-    unsigned* tbits = (unsigned*)(dbuf + tbits_off);
-    unsigned* tails = (unsigned*)(dbuf + tails_off);
-    int cub_launches = 0;
-    rc = seed_cub_launches(g, dense ? CUB_SCAN : CUB_PAIRS64, n, end_bit, dbuf + tmp_off, tmp_bytes, (unsigned*)keys,
-                           (unsigned*)skeys, vals, svals, head, pos, &cub_launches);
-    if (rc) return rc;
-    for (auto& ev : g->ev_seed) if (!ev) CK(cudaEventCreate(&ev));
-    Nvtx range(dense ? "mgc:add_nweights_dense_warm" : "mgc:add_nweights_warm");
-    g->st.ms_seeds_host += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
-    // 0. grouping on the device; nothing below touches the solver state until the id, pair and weight checks have passed
-    CK(cudaEventRecord(g->ev_seed[0], g->stream));
-    const int64_t* d_i = ii;
-    const int64_t* d_j = jj;
-    const double* d_cap = cap;
-    const double* d_rev = rev;
-    if (host) {
-        // host arrays go straight from the caller into device slots; device arrays are read in place
-        CK(cudaMemcpyAsync(dbuf + i_off, ii, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-        CK(cudaMemcpyAsync(dbuf + j_off, jj, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-        CK(cudaMemcpyAsync(dbuf + cap_off, cap, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-        CK(cudaMemcpyAsync(dbuf + rev_off, rev, (size_t)n * 8, cudaMemcpyHostToDevice, g->stream));
-        d_i = (const int64_t*)(dbuf + i_off);
-        d_j = (const int64_t*)(dbuf + j_off);
-        d_cap = (const double*)(dbuf + cap_off);
-        d_rev = (const double*)(dbuf + rev_off);
-    }
-    CK(cudaMemsetAsync(d_ctl, 0, 4 * sizeof(int), g->stream));
-    CK(cudaMemsetAsync(tflag, 0, ntl * sizeof(int), g->stream));
-    CK(cudaMemsetAsync(tbits, 0, tbits_bytes, g->stream));
-    {
-        const unsigned kgrid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
-        size_t tb = tmp_bytes;
-        if (dense) {
-            const unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
-            const unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
-            k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap, d_rev,
-                                                               head, d_ctl + 1);
-        } else {
-            if (g->nd == 4) k_nlinks_keys<4><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, keys, vals, d_ctl + 1);
-            else            k_nlinks_keys<3><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, keys, vals, d_ctl + 1);
-            CK(cub::DeviceRadixSort::SortPairs(dbuf + tmp_off, tb, keys, skeys, vals, svals, n, 0, end_bit, g->stream));
-            k_nlinks_heads<<<kgrid, 256, 0, g->stream>>>(skeys, svals, d_cap, d_rev, n, head);
-            tb = tmp_bytes;
-        }
-        CK(cub::DeviceScan::InclusiveSum(dbuf + tmp_off, tb, head, pos, n, g->stream));
-        k_nlinks_items<<<kgrid, 256, 0, g->stream>>>(g->L, g->TL, dense ? nullptr : skeys, axis, pos, n, d_items,
-                                                     eager ? nullptr : tflag, tiles, d_ctl);
-        g->st.kernel_launches += (dense ? 2 : 3) + cub_launches;
-        CK(cudaGetLastError());
-    }
-    const int* order = dense ? nullptr : svals;
-    const int64_t* ids = dense ? nullptr : d_i;
-    int* ntails = d_ctl + 3;
-    return fold_items(g, d_ctl, tiles, [&](unsigned grid, int ni) {
-        // the arcs first, then each tail once: the re-clamp reads the out-capacity after every increment of the call
-        if (g->nd == 4) k_nlinks_fold<4><<<grid, 256, 0, g->stream>>>(g->L, g->S, d_items, ni, order, ids, d_cap, d_rev, tbits, tails, ntails);
-        else            k_nlinks_fold<3><<<grid, 256, 0, g->stream>>>(g->L, g->S, d_items, ni, order, ids, d_cap, d_rev, tbits, tails, ntails);
-        g->st.kernel_launches++;
-        if (eager) {
-            if (g->nd == 4) k_nlinks_reclamp_eager<4><<<grid, 256, 0, g->stream>>>(g->S, g->smask, tails, ntails, g->partials);
-            else            k_nlinks_reclamp_eager<3><<<grid, 256, 0, g->stream>>>(g->S, g->smask, tails, ntails, g->partials);
-            return;
-        }
-        switch (g->caps_dtype) {
-            case MGC_F32: nlinks_reclamp_launch_t<float>(g, grid, tails, ntails); break;
-            case MGC_F64: nlinks_reclamp_launch_t<double>(g, grid, tails, ntails); break;
-            case MGC_U8: nlinks_reclamp_launch_t<uint8_t>(g, grid, tails, ntails); break;
-            case MGC_I16: nlinks_reclamp_launch_t<int16_t>(g, grid, tails, ntails); break;
-            default: nlinks_reclamp_launch_t<int32_t>(g, grid, tails, ntails); break;
-        }
-    }, true);
+    const bool dense = c.dense;
+    c.sort = dense ? FOLD_SCAN : FOLD_SORT_PAIRS;
+    c.key_shift = 2;
+    c.axis = axis;
+    const int n = (int)c.count;
+    return fold_run<unsigned long long, NlinkItem>(g, c,
+        [&](const FoldBufs<unsigned long long, NlinkItem>& b, unsigned kgrid, auto sort) {
+            const double* d_cap = (const double*)b.in[2];
+            const double* d_rev = (const double*)b.in[3];
+            if (dense) {
+                const unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
+                const unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
+                k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap,
+                                                                   d_rev, b.head, b.ctl + 1);
+                return MGC_OK;
+            }
+            const int64_t* d_i = (const int64_t*)b.in[0];
+            const int64_t* d_j = (const int64_t*)b.in[1];
+            if (g->nd == 4) k_nlinks_keys<4><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
+            else            k_nlinks_keys<3><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
+            CK(sort());
+            k_weighted_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_cap, d_rev, n, b.head);
+            return MGC_OK;
+        },
+        [&](const FoldBufs<unsigned long long, NlinkItem>& b, bool eager, unsigned grid, int ni) {
+            // the arcs first, then each tail once: the re-clamp reads the out-capacity after every increment of the call
+            const int* order = dense ? nullptr : b.svals;
+            const int64_t* ids = dense ? nullptr : (const int64_t*)b.in[0];
+            const double* d_cap = (const double*)b.in[2];
+            const double* d_rev = (const double*)b.in[3];
+            int* ntails = b.ctl + 3;
+            if (g->nd == 4) k_nlinks_fold<4><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.tbits, b.tails, ntails);
+            else            k_nlinks_fold<3><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.tbits, b.tails, ntails);
+            g->st.kernel_launches++;
+            residual_dispatch(g, eager, [&](auto A) {
+                k_nlinks_reclamp<<<grid, 256, 0, g->stream>>>(A, b.tails, ntails, g->partials);
+            });
+        });
 }
 
 int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
                           int64_t count, int32_t mem)
 {
-    if (!g) return MGC_E_ARG;
-    if (count < 0 || (count && (!i || !j || !cap || !rev_cap))) FAIL(MGC_E_ARG, "bad n-link arrays");
-    if (count > (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "more than 2^31 - 1 sum_edge calls in one call");
-    if (mem != MGC_MEM_HOST && mem != MGC_MEM_DEVICE) FAIL(MGC_E_ARG, "bad memory space");
-    bool eager = false;
-    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
-    CK(cudaSetDevice(g->device));
-    { int rc0 = check_pending(g); if (rc0) return rc0; }
-    return nweights_fold(g, i, j, cap, rev_cap, count, mem, 0, eager);
+    FoldCall c{};
+    c.range = "mgc:add_nweights_warm";
+    c.bad = count < 0 || (count && (!i || !j || !cap || !rev_cap)) ? "bad n-link arrays" : nullptr;
+    c.too_many = "more than 2^31 - 1 sum_edge calls in one call";
+    c.count = count;
+    c.mem = mem;
+    c.in[0] = i; c.in_n[0] = count;
+    c.in[1] = j; c.in_n[1] = count;
+    c.in[2] = cap; c.in_n[2] = count;
+    c.in[3] = rev_cap; c.in_n[3] = count;
+    return nweights_fold(g, c, 0);
 }
 
 int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
@@ -3088,19 +3011,14 @@ int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd
     if (!g || !fwd || !bwd) return MGC_E_ARG;
     if (axis < 0 || axis >= g->user_ndim) FAIL(MGC_E_ARG, "bad axis");
     if (fwd->dtype != MGC_F64 || bwd->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense n-weights must be float64");
-    bool eager = false;
-    { int rc0 = warm_check(g, &eager); if (rc0) return rc0; }
-    CK(cudaSetDevice(g->device));
-    { int rc0 = check_pending(g); if (rc0) return rc0; }
-    const void *pf = nullptr, *pb = nullptr;
-    int rc = stage_input(g, fwd, 0, &pf);
-    if (rc) return rc;
-    rc = stage_input(g, bwd, 1, &pb);
-    if (rc) return rc;
-    rc = nweights_fold(g, nullptr, nullptr, (const double*)pf, (const double*)pb, (int64_t)g->L.n, MGC_MEM_DEVICE,
-                       axis + g->shift, eager);
-    slots_release(g, 3u);                      // the grouping and the fold read the staging slots
-    return rc;
+    FoldCall c{};
+    c.range = "mgc:add_nweights_dense_warm";
+    c.count = (int64_t)g->L.n;
+    c.mem = MGC_MEM_DEVICE;
+    c.dense = true;
+    c.arrays[0] = fwd;
+    c.arrays[1] = bwd;
+    return nweights_fold(g, c, axis + g->shift);
 }
 
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem)

@@ -6,24 +6,22 @@
 // happens to the push-relabel state (DESIGN.md §4.6), with the steps of the t-link folds (gc_seeds.cuh):
 //   0. the calls are grouped by arc on the device: key = lower endpoint << 2 | canonical axis, a stable radix sort of
 //      (key, call index) pairs keeps the calls of one arc in call order, and a run-length pass makes one NlinkItem per
-//      arc that has a nonzero increment (k_nlinks_keys / _heads / _items; the dense form flags and compacts the nonzero
-//      entries instead, k_nlinks_dense_heads).  On lazily built handles the tiles of BOTH endpoints are listed once each;
+//      arc that has a nonzero increment (k_nlinks_keys / k_weighted_heads / k_nlinks_items; the dense form flags and
+//      compacts the nonzero entries instead, k_nlinks_dense_heads).  On lazily built handles the tiles of BOTH endpoints
+//      are listed once each;
 //   1. those tiles are materialised before any capacity is written (fold_items), so the materialiser never overwrites an
 //      edited arc;
 //   2. k_nlinks_fold adds the increments of each arc in call order to the residual capacities cap[2a+1][lo] and cap[2a][hi]
 //      and lists every tail whose out-capacity rose once, through a per-voxel bit;
-//   3. after every arc update, k_nlinks_reclamp (lazy) / k_nlinks_reclamp_eager (eager and 4-D) visit each listed tail once:
-//      the residual bits of the arcs that became positive are set, and a tail that still holds an un-pushed source
-//      residual r(v) > 0 is read and written back (residual_read -> residual_write, eager_read -> eager_write), which
-//      pushes what the larger out-capacity can carry -- without it that capacity would never see source flow;
+//   3. after every arc update, k_nlinks_reclamp visits each listed tail once: the residual bits of the arcs that became
+//      positive are set, and a tail that still holds an un-pushed source residual r(v) > 0 is read and written back through
+//      the fold's residual access (LazyResidual / EagerResidual, gc_seeds.cuh), which pushes what the larger out-capacity
+//      can carry -- without it that capacity would never see source flow;
 //   4. fold_items rebuilds the push lists and the next solve starts with a full relabel reset.
 // Only nonnegative, finite increments come here (the grouping checks them before anything is touched); the add_tweights
 // constant does not change.
 #pragma once
 #include "gc_seeds.cuh"
-
-#define FOLD_ERR_PAIR 4         // a pair of ids that are not lattice neighbours (or i == j)
-#define FOLD_ERR_NEGATIVE 8     // a negative n-link increment
 
 // element k of a small array indexed by a runtime value, unrolled into selects so the kernel parameters stay in registers
 // (a dynamic index would copy the whole parameter struct to local memory)
@@ -87,33 +85,6 @@ __global__ void __launch_bounds__(256) k_nlinks_keys(Lattice L, const int64_t* _
     }
 }
 
-// first index in [lo, hi) of the sorted keys whose key is >= x
-__device__ __forceinline__ int nlink_lower_bound(const unsigned long long* __restrict__ keys, int lo, int hi,
-                                                 unsigned long long x)
-{
-    while (lo < hi) {
-        const int mid = lo + ((hi - lo) >> 1);
-        if (keys[mid] < x) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
-
-// sum_edge(i, j, 0, 0) changes nothing, so only arcs with a call of a nonzero increment become items.  List form: 1 at the
-// first sorted key of each such arc (order = the sorted call indices).
-__global__ void __launch_bounds__(256) k_nlinks_heads(const unsigned long long* __restrict__ keys, const int* __restrict__ order,
-                                                      const double* __restrict__ cap, const double* __restrict__ rev, int n,
-                                                      int* __restrict__ head)
-{
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
-        int h = 0;
-        if (i == 0 || keys[i] != keys[i - 1]) {
-            const int e = nlink_lower_bound(keys, i, n, keys[i] + 1ull);
-            for (int j = i; j < e && !h; ++j) h = (cap[order[j]] != 0.0 || rev[order[j]] != 0.0) ? 1 : 0;
-        }
-        head[i] = h;
-    }
-}
-
 // dense form: 1 where the entry has a nonzero increment; entries on the last plane of the axis name no pair and are ignored
 // (as mgc_add_nweights_dense ignores them).  The axis arrives as scalars, so no lattice array is indexed at run time:
 // span = stride[axis] * dim[axis] (the stride of the next slower axis, or n for axis 0), span_magic its ceil(2^64 / span)
@@ -136,9 +107,11 @@ __global__ void __launch_bounds__(256) k_nlinks_dense_heads(unsigned n, unsigned
     }
 }
 
+// sum_edge(i, j, 0, 0) changes nothing, so only arcs with a call of a nonzero increment become items: the list form flags
+// the first sorted key of each such arc with k_weighted_heads (gc_seeds.cuh).
 // pos = inclusive sum of the heads: the head at i is item pos[i] - 1, in ascending key order, and ctl[0] = pos[n - 1]
 // items.  keys == nullptr: the dense form (pair i along `axis`, one call).  The tiles of both endpoints are listed once each
-// (claim_tile_once), which keeps the claim list within TL.ntiles (see k_seed_items); tflag == nullptr lists none (eager
+// (claim_tile_once), which keeps the claim list within TL.ntiles (see k_tweights_items); tflag == nullptr lists none (eager
 // and 4-D handles).
 __global__ void __launch_bounds__(256) k_nlinks_items(Lattice L, Tiles TL, const unsigned long long* __restrict__ keys, int axis,
                                                       const int* __restrict__ pos, int n, NlinkItem* __restrict__ items,
@@ -152,7 +125,7 @@ __global__ void __launch_bounds__(256) k_nlinks_items(Lattice L, Tiles TL, const
         if (keys) {
             lo = (unsigned)(keys[i] >> 2);
             a = (int)(keys[i] & 3ull);
-            cnt = nlink_lower_bound(keys, i, n, keys[i] + 1ull) - i;
+            cnt = lower_bound(keys, i, n, keys[i] + 1ull) - i;
         }
         items[pos[i] - 1] = NlinkItem{lo, a, i, cnt};
         if (tflag) {
@@ -173,7 +146,7 @@ __device__ __forceinline__ void nlink_tail_once(unsigned v, unsigned* __restrict
 // One thread per arc pair: the increments added to the two residual capacities in call order, (r + a) + b, as BK's
 // sum_edge does.  ids != nullptr: the list form, where a call (i, j) with i > j names the pair from its upper end, so its
 // cap is the backward and its rev_cap the forward increment.  A zero increment is skipped (exact: r + 0 == r).  Nothing
-// else is written here: the residual bits and the source re-clamp of the tails wait for k_nlinks_reclamp*, after every
+// else is written here: the residual bits and the source re-clamp of the tails wait for k_nlinks_reclamp, after every
 // arc of the call has its new capacity.
 template <int ND>
 __global__ void __launch_bounds__(256)
@@ -212,52 +185,27 @@ __device__ __forceinline__ unsigned nlink_arc_bits(const State<double>& S, unsig
     return m;
 }
 
-// Lazily built handle, one thread per listed tail.  residual_read's co[] / lim0 are the capacities of the build,
-// recomputed from the image: they describe how tr encodes the pushed source flow, not the current capacities, so they
-// stay right after an n-link edit.  residual_write then sees the new out-capacity: lim > lim0 pushes min(r, lim) more and
-// keeps tr = u + lim0 (read back as u), otherwise source_excess(r, co) >= min(r, lim) as before.  A tail with r(v) <= 0
-// keeps its state (a rewrite would cost a rounding of a voxel with net inflow).  r > 0 needs tr > 0, which holds no sink
-// flow, so the add_tweights constant does not move; each block stores a zero partial for fold_items' sum.
-template <typename E, int FN, int USE_MAX, int SPACING>
+// One thread per listed tail: the new arc bits ORed into rmask first (4-D eager_write never stores rmask, and residual_write /
+// 3-D eager_write keep bits 0..5 of what they read), then a tail with tr > 0 is read and, if r(v) > 0, written back.
+// Lazily built handles: residual_read's co[] / lim0 are the capacities of the build, recomputed from the image: they
+// describe how tr encodes the pushed source flow, not the current capacities, so they stay right after an n-link edit.
+// residual_write then sees the new out-capacity: lim > lim0 pushes min(r, lim) more and keeps tr = u + lim0 (read back as
+// u), otherwise source_excess(r, co) >= min(r, lim) as before.  A tail with r(v) <= 0 keeps its state (a rewrite would
+// cost a rounding of a voxel with net inflow).  Eager and 4-D handles: tr > 0 is r(v) itself (the record of the first
+// solve), and eager_write pushes min(r, lim) of the new out-capacity.  r > 0 needs tr > 0, which holds no sink flow, so
+// the add_tweights constant does not move; each block stores a zero partial for fold_items' sum.
+template <typename Access>
 __global__ void __launch_bounds__(256)
-k_nlinks_reclamp(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParams P, const unsigned* __restrict__ tails,
-                 const int* __restrict__ ntails, double* __restrict__ partials)
+k_nlinks_reclamp(Access A, const unsigned* __restrict__ tails, const int* __restrict__ ntails, double* __restrict__ partials)
 {
+    const State<double>& S = A.S;
     const int n = *ntails;
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
         const unsigned v = tails[i];
-        const unsigned bits = nlink_arc_bits<3>(S, v);
-        bool done = false;
+        S.rmask[v] = (uint8_t)(S.rmask[v] | nlink_arc_bits<Access::ND>(S, v));
         if (S.tr[v] > 0) {
-            Residual f = residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, v);
-            if (f.r > 0) {
-                f.rm |= bits;
-                residual_write(S, v, f);
-                done = true;
-            }
-        }
-        if (!done) S.rmask[v] = (uint8_t)(S.rmask[v] | bits);
-    }
-    block_sum_store(0.0, partials);
-}
-
-// Eager and 4-D handles (MGC_OPT_WARM): tr > 0 is r(v) itself (the record of the first solve), and eager_write pushes
-// min(r, lim) of the new out-capacity.
-template <int ND>
-__global__ void __launch_bounds__(256)
-k_nlinks_reclamp_eager(State<double> S, uint8_t* __restrict__ smask, const unsigned* __restrict__ tails,
-                       const int* __restrict__ ntails, double* __restrict__ partials)
-{
-    const int n = *ntails;
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
-        const unsigned v = tails[i];
-        const unsigned bits = nlink_arc_bits<ND>(S, v);
-        const unsigned rm = S.rmask[v] | bits;
-        S.rmask[v] = (uint8_t)rm;
-        if (S.tr[v] > 0) {
-            EagerResidual f = eager_read<ND>(S, v);
-            f.rm = rm;
-            eager_write<ND>(S, smask, v, f);
+            const auto f = A.read(v);
+            if (f.r > 0) A.write(v, f);
         }
     }
     block_sum_store(0.0, partials);

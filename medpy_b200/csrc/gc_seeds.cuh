@@ -1,42 +1,42 @@
-// gc_seeds.cuh -- seeds added to or erased from a solved lazily built 3-D graph, and any add_tweights calls, folded into
-// its residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm).
+// gc_seeds.cuh -- seeds added to or erased from a solved lattice graph, and any add_tweights calls, folded into its
+// residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm).
 //
 // The reference refines a cut by calling add_tweights(v, 65535, 0) / add_tweights(v, 0, 65535) on the new seed voxels of
 // a solved GraphDouble and calling maxflow() again, and erases a seed with the inverse call add_tweights(v, -65535, 0) /
 // add_tweights(v, 0, -65535): BK's add_tweights (graph.h:415-425) works on the RESIDUAL terminal capacity r(v) that the
 // first maxflow() left, and the second maxflow() continues from that residual graph.  Here the same happens to the
 // push-relabel state (DESIGN.md §4.6):
-//   0. the seed ids are grouped by voxel on the device: keys v << 1 | bg, radix sorted, run-length encoded into SeedItems
-//      (k_seed_keys / k_seed_items) in ascending voxel order, with each seeded tile listed once for the claim;
-//   1. the tiles of the seeded voxels are materialised first (k_caps_claim / k_caps_tiles), so every seeded voxel holds
-//      cap[], tr, excess and its sink-link state, and the fold below reads one representation only.  The marker bit planes
-//      are never read again for a claimed tile, so they are not updated;
-//   2. k_seed_fold (one thread per seeded voxel, its seeds in the reference's order) reads r(v) from that state, replays
-//      the seeds with add_tweights_dev -- the reference's arithmetic on r -- and writes r' back in the solver's
-//      representation;
-//   3. k_seed_lists puts every materialised tile that holds excess back on the push lists; the next solve starts with a
+//   0. the calls are grouped by voxel on the device into TweightItems {v, first, count} in ascending voxel order, with
+//      each touched tile listed once for the claim: seeds as keys v << 1 | bg, radix sorted (k_seed_keys / k_seed_heads);
+//      a call list as (voxel, call index) pairs, stably radix sorted (k_tweights_keys / k_weighted_heads); the dense form
+//      by a flag per voxel (k_tweights_dense_heads); then a scan and k_tweights_items;
+//   1. on lazily built handles the tiles of the touched voxels are materialised first (k_caps_claim / k_caps_tiles), so
+//      every touched voxel holds cap[], tr, excess and its sink-link state, and the fold below reads one representation
+//      only.  The marker bit planes are never read again for a claimed tile, so they are not updated;
+//   2. k_tlink_fold (one thread per item) reads r(v) from that state, replays the voxel's calls with add_tweights_dev --
+//      the reference's arithmetic on r -- and writes r' back in the solver's representation.  The residual access is a
+//      type: LazyResidual (residual_read / residual_write) on lazily built handles, EagerResidual (eager_read /
+//      eager_write) on the others, once MGC_OPT_WARM had the first solve record their residual source capacities (the
+//      end of this file).  The calls are a type as well: SeedCalls (the sorted seed keys) or ListCalls (src / snk);
+//   3. k_seed_lists / k_seed_lists4 put every tile that holds excess back on the push lists; the next solve starts with a
 //      full relabel reset.
-// mgc_add_tweights_warm runs the same steps with a value per call: its own grouping (k_tweights_keys / _heads / _items for a
-// call list, k_tweights_dense_heads / k_tweights_items for one call per voxel) and k_tweights_fold, which shares the read of
-// r(v) and the write-back of r' with k_seed_fold (residual_read / residual_write).
-// Handles that were not built lazily (the eager fused build, the per-term path, every 4-D lattice) fold with the same
-// grouping, no claim and k_seed_fold_eager / k_tweights_fold_eager, once MGC_OPT_WARM had the first solve record their
-// residual source capacities (the end of this file).
 #pragma once
 #include "gc_build.cuh"
 #include "gc_tiles4.cuh"
 
-// one seeded voxel: `nf` foreground seeds, then `nb` background seeds (list order of the reference: every fg id first)
-struct SeedItem {
+// error bits of a grouping, read back before anything touches the solver state
+#define FOLD_ERR_RANGE 1        // a node id out of range
+#define FOLD_ERR_NONFINITE 2    // a NaN or infinite weight
+#define FOLD_ERR_PAIR 4         // a pair of ids that are not lattice neighbours (or i == j)
+#define FOLD_ERR_NEGATIVE 8     // a negative n-link increment
+
+// One voxel's calls: calls first .. first + count - 1 of the sorted grouping (the dense form: the single call `first`)
+struct TweightItem {
     unsigned v;
-    int nf;
-    int nb;
+    int first;
+    int count;
     int pad;
 };
-
-// error bits of a grouping, read back before anything touches the solver state
-#define FOLD_ERR_RANGE 1
-#define FOLD_ERR_NONFINITE 2
 
 // grouping keys v << 1 | bg (the lattice has < 2^31 voxels, so a key fits 32 bits); fg ids first, then bg ids.  An id out
 // of range sets *err and gets key 0: the caller reads *err back before anything uses the items.
@@ -55,7 +55,8 @@ __global__ void __launch_bounds__(256) k_seed_keys(const int64_t* __restrict__ f
 }
 
 // first index in [lo, hi) of the sorted keys whose key is >= x
-__device__ __forceinline__ int seed_lower_bound(const unsigned* __restrict__ keys, int lo, int hi, unsigned x)
+template <typename K>
+__device__ __forceinline__ int lower_bound(const K* __restrict__ keys, int lo, int hi, K x)
 {
     while (lo < hi) {
         const int mid = lo + ((hi - lo) >> 1);
@@ -75,30 +76,7 @@ __device__ __forceinline__ void claim_tile_once(const Lattice& L, const Tiles& T
     if (tflag[t] == 0 && atomicExch(&tflag[t], 1) == 0) tiles[atomicAdd(&ctl[2], 1)] = t;
 }
 
-// Run-length pass over the sorted keys: pos = inclusive sum of the voxel-run heads, so the run starting at head i is item
-// pos[i] - 1 and there are pos[n - 1] items, in ascending voxel order.  Within a run the fg keys (2v) precede the bg keys
-// (2v + 1).  ctl[0] = the number of items.  Each seeded tile is listed once, by the first item that flips tflag[t]
-// (zeroed by the caller), and ctl[2] counts them: the claim list holds at most TL.ntiles entries whatever the number of
-// seeds.  That bound matters -- k_caps_claim enumerates count * 7 candidates in 32-bit arithmetic, and 7 * ntiles < 2^31
-// for every lattice below 2^31 voxels (ntiles = prod ceil(dim/8) <= n/8 + n^(2/3), taking the longest axis, c >= n^(1/3),
-// at ceil(c/8)/c <= 1/8 + 1/c and the others at <= 1; so ntiles < 2^28 + 2^21), while one entry per item could pass
-// 2^31 / 7 on a large erase.  The list order follows the atomics; k_caps_claim appends in atomic order anyway and each
-// tile's materialisation does not depend on it.
-__global__ void __launch_bounds__(256) k_seed_items(Lattice L, Tiles TL, const unsigned* __restrict__ keys,
-                                                    const int* __restrict__ pos, int n, SeedItem* __restrict__ items,
-                                                    int* __restrict__ tflag, int* __restrict__ tiles, int* __restrict__ ctl)
-{
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
-        if (i == n - 1) ctl[0] = pos[i];
-        if (i > 0 && pos[i] == pos[i - 1]) continue;
-        const unsigned v = keys[i] >> 1;
-        const int s = seed_lower_bound(keys, i, n, 2u * v + 1u);
-        const int e = seed_lower_bound(keys, s, n, 2u * v + 2u);
-        items[pos[i] - 1] = SeedItem{v, s - i, e - s, 0};
-        if (tflag) claim_tile_once(L, TL, v, tflag, tiles, ctl);      // tflag == nullptr: eager handle, nothing to claim
-    }
-}
-
+// 1 at the first sorted key of each voxel (a run of keys 2v, then 2v + 1)
 __global__ void __launch_bounds__(256) k_seed_heads(const unsigned* __restrict__ keys, int n, int* __restrict__ head)
 {
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x))
@@ -136,7 +114,7 @@ __global__ void __launch_bounds__(256) k_seed_heads(const unsigned* __restrict__
 //     all the flow pushed so far;
 //   - r' = 0: no terminal link, as for any seed that cancels.
 // A materialised voxel's state read as BK's residual terminal capacity (residual_read), and r' written back in the
-// solver's representation (residual_write): the two halves of every fold, k_seed_fold and k_tweights_fold.
+// solver's representation (residual_write): the two halves of every fold on a lazily built handle (LazyResidual).
 struct Residual {
     double co[6];     // capacities before any flow
     double lim0;      // their sum rounded up, x SOURCE_CLAMP_SLACK
@@ -158,14 +136,14 @@ __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<
     // capacities before any flow: the doubles k_caps_tiles computed from the same image copy
     const unsigned valid = (c[0] > 0 ? 1u : 0u) | (c[0] + 1 < L.dim[0] ? 2u : 0u) | (c[1] > 0 ? 4u : 0u) |
                            (c[1] + 1 < L.dim[1] ? 8u : 0u) | (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
-    const double a = build_val<E>(img[v], use_max);
+    const double a = build_val<E>(__ldg(img + v), use_max);
     if (FN == 1 && SPACING == 0) {
         double t6[6];
 #pragma unroll
         for (int k = 0; k < 6; ++k) {
             t6[k] = 0.0;
             if ((valid >> k) & 1u) {
-                const double b = build_val<E>(img[(unsigned)((int)v + dir_offset(L, k))], use_max);
+                const double b = build_val<E>(__ldg(img + (unsigned)((int)v + dir_offset(L, k))), use_max);
                 t6[k] = exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
             }
         }
@@ -174,7 +152,8 @@ __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<
 #pragma unroll
         for (int k = 0; k < 6; ++k)
             f.co[k] = ((valid >> k) & 1u)
-                          ? build_weight<FN, E>(P, a, img[(unsigned)((int)v + dir_offset(L, k))], use_max, spacing, P.spacing[k >> 1])
+                          ? build_weight<FN, E>(P, a, __ldg(img + (unsigned)((int)v + dir_offset(L, k))), use_max, spacing,
+                                                P.spacing[k >> 1])
                           : 0.0;
     }
     double lim0 = __dadd_ru(0.0, f.co[0]);
@@ -234,33 +213,7 @@ __device__ __forceinline__ void residual_write(const State<double>& S, unsigned 
     S.rmask[v] = (uint8_t)nm;
 }
 
-template <typename E, int FN, int USE_MAX, int SPACING>
-__global__ void __launch_bounds__(256)
-k_seed_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParams P, const SeedItem* __restrict__ items,
-            int n, double cap, double* __restrict__ partials)
-{
-    double m = 0.0;
-    const int step = (int)(gridDim.x * blockDim.x);
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
-        const SeedItem it = items[i];
-        Residual f = residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, it.v);
-        for (int j = 0; j < it.nf; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, cap, 0.0));
-        for (int j = 0; j < it.nb; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, 0.0, cap));
-        residual_write(S, it.v, f);
-        m = __dadd_rn(m, f.dk);
-    }
-    block_sum_store(m, partials);
-}
-
 // ---- general t-link folds (mgc_add_tweights_warm): add_tweights(v, src[k], snk[k]) with any finite values ----------------
-// One voxel's calls: calls order[first .. first + count) in the caller's order (order == nullptr: the single call `first`).
-struct TweightItem {
-    unsigned v;
-    int first;
-    int count;
-    int pad;
-};
-
 // list form: key = voxel id, value = call index.  A stable radix sort of the pairs keeps a voxel's calls in call order.  An
 // id out of range or a non-finite weight sets a bit of *err (an out-of-range id gets key 0).
 __global__ void __launch_bounds__(256) k_tweights_keys(const int64_t* __restrict__ ids, const double* __restrict__ src,
@@ -280,16 +233,18 @@ __global__ void __launch_bounds__(256) k_tweights_keys(const int64_t* __restrict
 
 // add_tweights(v, 0, 0) is an exact no-op in BK's arithmetic (the minimum is 0 and s - t gives tr back in both branches), so
 // only voxels with a call of a nonzero weight become items, in both forms.
-// list form: 1 at the first sorted key of each voxel that has such a call (order = the sorted call indices)
-__global__ void __launch_bounds__(256) k_tweights_heads(const unsigned* __restrict__ keys, const int* __restrict__ order,
-                                                       const double* __restrict__ src, const double* __restrict__ snk, int n,
-                                                       int* __restrict__ head)
+// list form: 1 at the first sorted key of each voxel that has such a call (order = the sorted call indices).  The n-link
+// list form (gc_nlinks.cuh) groups its arcs the same way: a, b = cap, rev_cap there.
+template <typename K>
+__global__ void __launch_bounds__(256) k_weighted_heads(const K* __restrict__ keys, const int* __restrict__ order,
+                                                        const double* __restrict__ a, const double* __restrict__ b, int n,
+                                                        int* __restrict__ head)
 {
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
         int h = 0;
         if (i == 0 || keys[i] != keys[i - 1]) {
-            const int e = seed_lower_bound(keys, i, n, keys[i] + 1u);
-            for (int j = i; j < e && !h; ++j) h = (src[order[j]] != 0.0 || snk[order[j]] != 0.0) ? 1 : 0;
+            const int e = lower_bound(keys, i, n, (K)(keys[i] + 1u));
+            for (int j = i; j < e && !h; ++j) h = (a[order[j]] != 0.0 || b[order[j]] != 0.0) ? 1 : 0;
         }
         head[i] = h;
     }
@@ -307,10 +262,16 @@ __global__ void __launch_bounds__(256) k_tweights_dense_heads(const double* __re
 }
 
 // pos = inclusive sum of the heads: the head at i is item pos[i] - 1, in ascending voxel order, and ctl[0] = pos[n - 1]
-// items.  keys == nullptr: the dense form (voxel i, one call).  Each touched tile is listed once (claim_tile_once), which
-// keeps the claim list within TL.ntiles (see k_seed_items); tflag == nullptr lists no tiles (eager and 4-D handles: every
-// voxel already holds its push state, and TL does not describe a 4-D lattice).
-__global__ void __launch_bounds__(256) k_tweights_items(Lattice L, Tiles TL, const unsigned* __restrict__ keys,
+// items; the voxel of sorted key i is keys[i] >> shift (shift 1: the seed keys v << 1 | bg, whose fg keys precede the bg
+// keys of a voxel).  keys == nullptr: the dense form (voxel i, one call).  Each touched tile is listed once, by the first
+// item that flips tflag[t] (zeroed by the caller), and ctl[2] counts them: the claim list holds at most TL.ntiles entries
+// whatever the number of calls.  That bound matters -- k_caps_claim enumerates count * 7 candidates in 32-bit arithmetic,
+// and 7 * ntiles < 2^31 for every lattice below 2^31 voxels (ntiles = prod ceil(dim/8) <= n/8 + n^(2/3), taking the
+// longest axis, c >= n^(1/3), at ceil(c/8)/c <= 1/8 + 1/c and the others at <= 1; so ntiles < 2^28 + 2^21), while one
+// entry per item could pass 2^31 / 7 on a large erase.  The list order follows the atomics; k_caps_claim appends in atomic
+// order anyway and each tile's materialisation does not depend on it.  tflag == nullptr lists no tiles (eager and 4-D
+// handles: every voxel already holds its push state, and TL does not describe a 4-D lattice).
+__global__ void __launch_bounds__(256) k_tweights_items(Lattice L, Tiles TL, const unsigned* __restrict__ keys, int shift,
                                                         const int* __restrict__ pos, int n, TweightItem* __restrict__ items,
                                                         int* __restrict__ tflag, int* __restrict__ tiles, int* __restrict__ ctl)
 {
@@ -320,35 +281,12 @@ __global__ void __launch_bounds__(256) k_tweights_items(Lattice L, Tiles TL, con
         unsigned v = (unsigned)i;
         int cnt = 1;
         if (keys) {
-            v = keys[i];
-            cnt = seed_lower_bound(keys, i, n, v + 1u) - i;
+            v = keys[i] >> shift;
+            cnt = lower_bound(keys, i, n, (v + 1u) << shift) - i;
         }
         items[pos[i] - 1] = TweightItem{v, i, cnt, 0};
         if (tflag) claim_tile_once(L, TL, v, tflag, tiles, ctl);
     }
-}
-
-// One thread per touched voxel: r(v) read as in k_seed_fold, its calls applied in the caller's order with the reference's
-// arithmetic, r' written back.  residual_write holds for any finite r and r' (see k_seed_fold), so any weights may come.
-template <typename E, int FN, int USE_MAX, int SPACING>
-__global__ void __launch_bounds__(256)
-k_tweights_fold(Lattice L, State<double> S, const E* __restrict__ img, BoundaryParams P, const TweightItem* __restrict__ items,
-                int n, const int* __restrict__ order, const double* __restrict__ src, const double* __restrict__ snk,
-                double* __restrict__ partials)
-{
-    double m = 0.0;
-    const int step = (int)(gridDim.x * blockDim.x);
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
-        const TweightItem it = items[i];
-        Residual f = residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, it.v);
-        for (int j = it.first; j < it.first + it.count; ++j) {
-            const int k = order ? order[j] : j;
-            f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, src[k], snk[k]));
-        }
-        residual_write(S, it.v, f);
-        m = __dadd_rn(m, f.dk);
-    }
-    block_sum_store(m, partials);
 }
 
 // push lists after a fold: every materialised tile (cmat[t] = 1) holding an owned voxel with excess goes on the list its
@@ -382,7 +320,7 @@ __global__ void __launch_bounds__(TILE_VOX) k_seed_lists(Lattice L, Tiles TL, St
 //          r' = 0 : tr = 0.
 // 3-D state: 6 arcs, the sink-link bits RM_SINK / RM_SINKV in rmask.  4-D state: 8 arcs in rmask, the sink-residual bit in
 // smask, and sink[] summed over every voxel by the read-out (so a voxel without a sink link gets sink[v] = 0).
-struct EagerResidual {
+struct EagerRead {
     double r;         // r(v)
     double dk;        // change of the add_tweights constant
     double e;         // excess
@@ -390,9 +328,9 @@ struct EagerResidual {
 };
 
 template <int ND>
-__device__ __forceinline__ EagerResidual eager_read(const State<double>& S, unsigned v)
+__device__ __forceinline__ EagerRead eager_read(const State<double>& S, unsigned v)
 {
-    EagerResidual f;
+    EagerRead f;
     const double tr = S.tr[v];
     f.rm = S.rmask[v];
     f.e = S.excess[v];
@@ -410,7 +348,7 @@ __device__ __forceinline__ EagerResidual eager_read(const State<double>& S, unsi
 
 template <int ND>
 __device__ __forceinline__ void eager_write(const State<double>& S, uint8_t* __restrict__ smask, unsigned v,
-                                            const EagerResidual& f)
+                                            const EagerRead& f)
 {
     const double r = f.r;
     double e = f.e;
@@ -447,40 +385,76 @@ __device__ __forceinline__ void eager_write(const State<double>& S, uint8_t* __r
     }
 }
 
-template <int ND>
-__global__ void __launch_bounds__(256)
-k_seed_fold_eager(State<double> S, uint8_t* __restrict__ smask, const SeedItem* __restrict__ items, int n, double cap,
-                  double* __restrict__ partials)
-{
-    double m = 0.0;
-    const int step = (int)(gridDim.x * blockDim.x);
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
-        const SeedItem it = items[i];
-        EagerResidual f = eager_read<ND>(S, it.v);
-        for (int j = 0; j < it.nf; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, cap, 0.0));
-        for (int j = 0; j < it.nb; ++j) f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, 0.0, cap));
-        eager_write<ND>(S, smask, it.v, f);
-        m = __dadd_rn(m, f.dk);
-    }
-    block_sum_store(m, partials);
-}
+// ---- the fold ----------------------------------------------------------------------------------------------------------
+// Residual access of a fold: read(v) gives r(v) and the voxel's state, write(v, f) stores r' back.  How tr holds the
+// residual source capacity is the access type's business: a lazily built handle recomputes the pushed source flow from
+// its image (residual_read), an eager or 4-D handle recorded r(v) itself at the first solve (eager_read).  The members
+// are the fold kernels' first parameters.
+template <typename E, int FN, int USE_MAX, int SPACING>
+struct LazyResidual {
+    static constexpr int ND = 3;
+    Lattice L;
+    State<double> S;
+    const E* img;
+    BoundaryParams P;
+    __device__ __forceinline__ Residual read(unsigned v) const { return residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, v); }
+    __device__ __forceinline__ void write(unsigned v, const Residual& f) const { residual_write(S, v, f); }
+};
 
-template <int ND>
+template <int ND_>
+struct EagerResidual {
+    static constexpr int ND = ND_;
+    State<double> S;
+    uint8_t* smask;
+    __device__ __forceinline__ EagerRead read(unsigned v) const { return eager_read<ND>(S, v); }
+    __device__ __forceinline__ void write(unsigned v, const EagerRead& f) const { eager_write<ND>(S, smask, v, f); }
+};
+
+// The calls of a fold: get(j, s, t) gives add_tweights call j of the sorted grouping.  Read-only inputs are loaded through
+// __ldg: a pointer inside a parameter struct carries no __restrict__.
+// Seeds: sorted key j = v << 1 | bg is add_tweights(v, cap, 0) (fg) or add_tweights(v, 0, cap) (bg), cap = +-65535.
+struct SeedCalls {
+    const unsigned* keys;
+    double cap;
+    __device__ __forceinline__ void get(int j, double& s, double& t) const
+    {
+        const bool bg = (__ldg(keys + j) & 1u) != 0;
+        s = bg ? 0.0 : cap;
+        t = bg ? cap : 0.0;
+    }
+};
+
+// mgc_add_tweights_warm: add_tweights(v, src[k], snk[k]), k = order[j] (the sorted call indices; nullptr: k = j)
+struct ListCalls {
+    const int* order;
+    const double* src;
+    const double* snk;
+    __device__ __forceinline__ void get(int j, double& s, double& t) const
+    {
+        const int k = order ? __ldg(order + j) : j;
+        s = __ldg(src + k);
+        t = __ldg(snk + k);
+    }
+};
+
+// One thread per touched voxel: r(v) read, its calls applied in order with the reference's arithmetic, r' written back;
+// the change of the add_tweights constant summed into one partial per block.  residual_write and eager_write hold for
+// any finite r and r', so any weights may come.
+template <typename Access, typename Calls>
 __global__ void __launch_bounds__(256)
-k_tweights_fold_eager(State<double> S, uint8_t* __restrict__ smask, const TweightItem* __restrict__ items, int n,
-                      const int* __restrict__ order, const double* __restrict__ src, const double* __restrict__ snk,
-                      double* __restrict__ partials)
+k_tlink_fold(Access A, const TweightItem* __restrict__ items, int n, Calls C, double* __restrict__ partials)
 {
     double m = 0.0;
     const int step = (int)(gridDim.x * blockDim.x);
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
         const TweightItem it = items[i];
-        EagerResidual f = eager_read<ND>(S, it.v);
+        auto f = A.read(it.v);
         for (int j = it.first; j < it.first + it.count; ++j) {
-            const int k = order ? order[j] : j;
-            f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, src[k], snk[k]));
+            double s, t;
+            C.get(j, s, t);
+            f.dk = __dadd_rn(f.dk, add_tweights_dev(f.r, s, t));
         }
-        eager_write<ND>(S, smask, it.v, f);
+        A.write(it.v, f);
         m = __dadd_rn(m, f.dk);
     }
     block_sum_store(m, partials);
