@@ -186,11 +186,13 @@ __device__ __forceinline__ bool source_active(double tr, unsigned pairs)
 // ballot per warp row) and, where the graph has no other copy of them to read later (img_copy / prob_copy not nullptr),
 // copies of the image and of the probability map -- and clears cmat[] of its tiles.  rmask,
 // height, partials and worklists are bit for bit what LAZY = 0 writes.  Under the exponential term without spacing every
-// in-lattice weight is >= DBL_MIN, so for a warp whose arguments are ordinary the n-link bits of rmask are the validity
-// bits, and the clamped excess is > 0 exactly when tr > 0 and the voxel has an in-lattice arc: such a warp evaluates no
-// exponential.  A warp whose arguments are not ordinary evaluates all six per voxel (rmask depends on them; no z carry,
-// no shared planes: a neighbouring warp may have skipped).  Other terms still evaluate every weight (weight check,
-// rmask) but store none.
+// in-lattice weight is >= DBL_MIN, so for a voxel whose arguments are ordinary the n-link bits of rmask are the validity
+// bits, and the clamped excess is > 0 exactly when tr > 0 and the voxel has an in-lattice arc.  One range test over the
+// staged image block (block_exp_ordinary, gc_exprange.cuh) decides that for every pair of the block at once: in a block
+// that passes, no z-step reads a neighbour cell, forms an argument or takes a vote.  A block that does not pass takes
+// the warp vote per z-step, and a warp whose arguments are not ordinary evaluates all six weights per voxel (rmask
+// depends on them; no z carry, no shared planes: a neighbouring warp may have skipped).  Other terms still evaluate
+// every weight (weight check, rmask) but store none.
 template <typename E, typename T, int FN, int USE_MAX, int SPACING, int TIN = 0, int LAZY = 0>
 __global__ void __launch_bounds__(BUILD_THREADS)
 k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps maps, BuildArgs A, BoundaryParams P,
@@ -218,6 +220,7 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
     const int x0 = blockIdx.x * BUILD_TX, y0 = blockIdx.y * BUILD_TY, z0 = (A.z_tile0 + (int)blockIdx.z) * BUILD_TZ;
     const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
     const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
+    constexpr bool LAZY_EXP = LAZY && FN == 1 && SPACING == 0;      // the lazy path that may skip the weights
 
     const int gy = y0 + ly, gx = x0 + lx;
     const bool col_in = gy < L.dim[1] && gx < L.dim[2];
@@ -277,9 +280,11 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         mbar_wait(bar, 0u);
         if (staged_tin) cur = fetch(0);
     } else {
+        // (LAZY_EXP stages whole rows of the box, as TMA does: the block's range test reads every cell)
+        constexpr int SX = LAZY_EXP ? BUILD_BX : 34;
         const E* img = reinterpret_cast<const E*>(A.img);
-        for (int i = tid; i < BUILD_HZ * BUILD_HY * 34; i += BUILD_THREADS) {
-            const int hx = i % 34, r = i / 34, hy = r % BUILD_HY, hz = r / BUILD_HY;
+        for (int i = tid; i < BUILD_HZ * BUILD_HY * SX; i += BUILD_THREADS) {
+            const int hx = i % SX, r = i / SX, hy = r % BUILD_HY, hz = r / BUILD_HY;
             const int gz = z0 - 1 + hz, gy = y0 - 1 + hy, gx = x0 - 1 + hx;
             E val = (E)0;
             if (gz >= 0 && gy >= 0 && gx >= 0 && gz < L.dim[0] && gy < L.dim[1] && gx < L.dim[2])
@@ -287,6 +292,41 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
             s_img[(hz * BUILD_HY + hy) * BUILD_BX + hx] = val;
         }
         __syncthreads();
+    }
+
+    // ---- LAZY_EXP: one range test for the whole staged block instead of a warp vote per voxel and z-step.  Every cell
+    // of the box counts -- halo, pad and zero fill included, which can only make the test stricter -- and
+    // block_exp_ordinary (gc_exprange.cuh) states why a block that passes holds no pair whose own test would fail.  The
+    // result is uniform over the CTA.  Scratch: the weight planes, which LAZY_EXP does not use.
+    bool blk_ordinary = false;
+    if constexpr (LAZY_EXP) {
+        E lo = (E)INFINITY, hi = (E)-INFINITY;
+        bool nan = false;
+        for (int i = tid; i < IMG_BYTES / 16; i += BUILD_THREADS) {
+            const uint4 q = reinterpret_cast<const uint4*>(s_img)[i];
+            E e[16 / sizeof(E)];
+            memcpy(e, &q, 16);
+#pragma unroll
+            for (int k = 0; k < (int)(16 / sizeof(E)); ++k) block_range_add<E>(lo, hi, nan, e[k]);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const E olo = __shfl_xor_sync(0xffffffffu, lo, o), ohi = __shfl_xor_sync(0xffffffffu, hi, o);
+            block_range_add<E>(lo, hi, nan, olo);
+            block_range_add<E>(lo, hi, nan, ohi);
+        }
+        nan = __any_sync(0xffffffffu, nan);
+        E* s_rng = reinterpret_cast<E*>(s_wy);                       // [8] warp minima, [8] warp maxima
+        int* s_rnan = reinterpret_cast<int*>(s_wy + 16);             // [8] warp NaN flags
+        if (lx == 0) { s_rng[ly] = lo; s_rng[8 + ly] = hi; s_rnan[ly] = nan ? 1 : 0; }
+        __syncthreads();
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+            block_range_add<E>(lo, hi, nan, s_rng[w]);
+            block_range_add<E>(lo, hi, nan, s_rng[8 + w]);
+            nan = nan || s_rnan[w] != 0;
+        }
+        blk_ordinary = block_exp_ordinary(Elem<E>::val(lo), Elem<E>::val(hi), nan, use_max, P.inv_sigma2);
     }
 
     const bool has_py = gy + 1 < L.dim[1], has_px = gx + 1 < L.dim[2];
@@ -312,7 +352,6 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
     // weight per thread, the 64 x-face weights on the first two warps) so that no warp carries extra work in the loop ----
     double* s_wyh = s_wx + 2 * 8 * 33;          // [8 z][32 x]: pair (y0 - 1, y0)
     double* s_wxh = s_wyh + 8 * 32;             // [8 z][8 y]:  pair (x0 - 1, x0)
-    constexpr bool LAZY_EXP = LAZY && FN == 1 && SPACING == 0;      // the lazy path that may skip the weights
     double wz_back = 0.0;
     if (!LAZY_EXP) {
         const bool vz = col_in && z0 > 0;
@@ -327,6 +366,12 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         }
     }
 
+    // the in-lattice pairs of this thread's voxel in plane gz (bit k: the pair across face k exists)
+    auto pairs_at = [&](int gz) -> unsigned {
+        return (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) | (has_py ? 8u : 0u) |
+               (gx > 0 ? 16u : 0u) | (has_px ? 32u : 0u);
+    };
+    const bool copies = A.img_copy != nullptr || A.prob_copy != nullptr;
     for (int lz = 0; lz < BUILD_TZ; ++lz) {
         const int gz = z0 + lz;
         const bool pin = col_in && gz < L.dim[0];            // block-uniform in z, per thread in y/x
@@ -335,7 +380,8 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         const int hz = lz + 1;
         TIn nxt{0.0, 0u};
         if (lz + 1 < BUILD_TZ) nxt = fetch(lz + 1);
-        const double a = build_val<E>(at(hz, ly + 1, lx + 1), use_max);
+        // (the voxel's own value: read where a weight or an argument needs it)
+        auto own_val = [&]() -> double { return build_val<E>(at(hz, ly + 1, lx + 1), use_max); };
         // ---- t-links: add_tweights replay in the reference's order (regional, fg, bg) ----
         auto tlinks = [&](T& tr) -> double {
             return tlink_replay<T>(tr, TIN == 1 || A.prob != nullptr, cur.p, TIN == 1 || A.compute_f32 != 0, A.alpha, cur.fb);
@@ -344,30 +390,33 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         double mm = 0.0;
         double c0 = 0.0, c1 = 0.0, c2 = 0.0, c3 = 0.0, c4 = 0.0, c5 = 0.0;
         double wz = 0.0, wy = 0.0, wx = 0.0;
+        // LAZY_EXP: every argument of the warp is ordinary -- rmask then holds the validity bits and the excess follows
+        // from tr (source_active) -- or else c0..c5 are the six weights
+        bool lean = false;
         if constexpr (LAZY_EXP) {
-            // the six weights are needed only when the warp's arguments are not all ordinary (rmask would then depend
-            // on the values)
+            // the six weights are needed only when some argument of the warp is not ordinary (rmask would then depend on
+            // the values): never in a block that passed its range test, else when the warp's vote fails
             if (pin) mm = tlinks(tr);
-            auto arg = [&](E iq) -> double {
-                const double b = build_val<E>(iq, use_max);
-                return exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
-            };
-            const double t[6] = {arg(at(hz - 1, ly + 1, lx + 1)), arg(at(hz + 1, ly + 1, lx + 1)), arg(at(hz, ly, lx + 1)),
-                                 arg(at(hz, ly + 2, lx + 1)), arg(at(hz, ly + 1, lx)), arg(at(hz, ly + 1, lx + 2))};
-            const unsigned valid = pin ? ((gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) |
-                                          (has_py ? 8u : 0u) | (gx > 0 ? 16u : 0u) | (has_px ? 32u : 0u)) : 0u;
-            const bool ordinary = __all_sync(0xffffffffu, t[0] <= 700.0 && t[1] <= 700.0 && t[2] <= 700.0 &&
-                                                          t[3] <= 700.0 && t[4] <= 700.0 && t[5] <= 700.0);
-            double c[6];
-            if (!ordinary) {
-                exp_caps6(t, ordinary, valid, c);
-            } else {
-#pragma unroll
-                for (int k = 0; k < 6; ++k) c[k] = ((valid >> k) & 1u) ? 1.0 : 0.0;    // stand-ins: only signs are read
+            lean = blk_ordinary;
+            if (!lean) {
+                const double a = own_val();
+                auto arg = [&](E iq) -> double {
+                    const double b = build_val<E>(iq, use_max);
+                    return exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
+                };
+                const double t[6] = {arg(at(hz - 1, ly + 1, lx + 1)), arg(at(hz + 1, ly + 1, lx + 1)), arg(at(hz, ly, lx + 1)),
+                                     arg(at(hz, ly + 2, lx + 1)), arg(at(hz, ly + 1, lx)), arg(at(hz, ly + 1, lx + 2))};
+                lean = __all_sync(0xffffffffu, t[0] <= 700.0 && t[1] <= 700.0 && t[2] <= 700.0 &&
+                                               t[3] <= 700.0 && t[4] <= 700.0 && t[5] <= 700.0);
+                if (!lean) {
+                    double c[6];
+                    exp_caps6(t, false, pin ? pairs_at(gz) : 0u, c);
+                    c0 = c[0]; c1 = c[1]; c2 = c[2]; c3 = c[3]; c4 = c[4]; c5 = c[5];
+                }
             }
-            c0 = c[0]; c1 = c[1]; c2 = c[2]; c3 = c[3]; c4 = c[4]; c5 = c[5];
         } else {
             // the three forward pair weights of this voxel: independent, branch-free evaluations
+            const double a = own_val();
             if (FN == 1 && SPACING == 0) {
                 // exponential term: form the three arguments, let the WARP agree that all of them are ordinary (<= 700, not
                 // NaN -- true for every warp of a sane image) and evaluate without any range handling; the rare warp that
@@ -409,7 +458,7 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
                 }
                 mm = tlinks(tr);
             }
-            if (LAZY) {
+            if (LAZY && copies) {
                 if (A.img_copy) reinterpret_cast<E*>(A.img_copy)[v] = at(hz, ly + 1, lx + 1);
                 if (A.prob_copy) {
                     if (TIN == 1 || !A.prob_f64) reinterpret_cast<float*>(A.prob_copy)[v] = (float)cur.p;
@@ -420,19 +469,28 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
             if (own) msum = __dadd_rn(msum, mm);
             if (!LAZY) S.tr[v] = tr;
             // ---- solver state (same arithmetic as k_init_tile and k_caps_tiles) ----
-            const double c[6] = {c0, c1, c2, c3, c4, c5};
-            unsigned m = cap_bits(c);
             const double trd = (double)tr;
-            // LAZY_EXP with ordinary arguments: from the stand-ins, whose sum has the sign of the true one -- only e > 0 is read
-            double e = source_excess(trd, c);
+            unsigned m;
+            bool exc;
+            if (LAZY_EXP && lean) {
+                // every in-lattice weight is >= DBL_MIN: cap_bits gives the validity bits, and the clamped source excess
+                // is > 0 exactly when source_active says so
+                m = pairs_at(gz);
+                exc = own && source_active(trd, m);
+            } else {
+                const double c[6] = {c0, c1, c2, c3, c4, c5};
+                m = cap_bits(c);
+                double e = source_excess(trd, c);
+                if (!own) e = 0.0;
+                if (!LAZY) S.excess[v] = (T)e;
+                exc = e > 0;
+            }
             if (trd < 0) m |= RM_SINK;
-            if (!own) e = 0.0;
-            if (!LAZY) S.excess[v] = (T)e;
             S.rmask[v] = (uint8_t)m;
             const int h = (own && trd < 0) ? 1 : MGC_HINF;
             S.height[v] = h;
             if (own && (m & 0x3fu) != 0 && h == MGC_HINF) needs_any = 1u;
-            if (e > 0) exc_any = 1u;
+            if (exc) exc_any = 1u;
         }
         if (LAZY) {      // marker bit planes: one word per warp row and marker
             const unsigned bf = __ballot_sync(0xffffffffu, pin && (cur.fb & 1u)), bb = __ballot_sync(0xffffffffu, pin && (cur.fb & 2u));

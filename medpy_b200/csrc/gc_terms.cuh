@@ -9,6 +9,7 @@
 // pow are within an ulp or two of numpy's libm.
 #pragma once
 #include "gc_common.cuh"
+#include "gc_exprange.cuh"
 #include <cfloat>
 
 // ---------------------------------------------------------------------------------------------------
@@ -189,11 +190,10 @@ __device__ __forceinline__ double exp_neg_inrange(double t)
     return __hiloint2double(__double2hiint(p) + ((int)n << 20), __double2loint(p));
 }
 
-// argument of the exponential term, exactly as g_weight<1> forms it
+// argument of the exponential term, exactly as g_weight<1> forms it (gc_exprange.cuh)
 __device__ __forceinline__ double exp_term_arg(const BoundaryParams& P, double x)
 {
-    return (P.inv_sigma2 > 0.0 && P.inv_sigma2 < 1e300) ? __dmul_rn(__dmul_rn(x, x), P.inv_sigma2)
-                                                        : __ddiv_rn(__dmul_rn(x, x), P.sigma);
+    return exp_arg(x, P.inv_sigma2, P.sigma);
 }
 
 // FN >= 0 fixes the term at compile time (the specialised kernels of the common cases), FN < 0 reads it from P
