@@ -225,11 +225,9 @@ struct mgc_graph {
     int rl_cur = 0;                    // relabel list consumed next
     bool labels_fresh = false;         // labels + relabel list 0 come straight from k_init_tile
     int n_ctas = 264;                  // persistent CTAs per tile-kernel launch
-    bool use_coop = false;             // whole solve as one cooperative launch (gc_persist.cuh); opt-in, MEDPY_GC_COOP=1
     int coop_bfs_grid = 0;             // co-resident CTAs of k_bfs_coop (0: per-pass host loop)
     bool use_tma = false;              // push kernel stages its tile planes with TMA (gc_tma.cuh)
     PushMaps maps{};                   // tensor maps of cap[0..5] and excess
-    int coop_grid = 0;                 // co-resident CTAs of k_solve_coop
     int tile_iters = 8;                // synchronous push/relabel rounds per tile visit
     int tile_iters_first = 4;          // ... in the first round after init (mostly stranded excess drains locally)
     int iters_now = 8;
@@ -546,6 +544,32 @@ bool make_push_maps(mgc_graph* g)
     return true;
 }
 
+// the environment options of the tile solver, the same for 3-D and 4-D lattices (4-D z-slab handles run the per-voxel
+// solver and read none of them).  `bfs` is the cooperative BFS kernel of the lattice's tile shape, launched with
+// `bfs_threads` threads per CTA: its occupancy sizes the grid (MEDPY_GC_BFS=host: the host-driven BFS instead).
+void tile_solver_options(mgc_graph* g, const void* bfs, int bfs_threads)
+{
+    g->n_ctas = 2 * cached_sm_count(g->device);   // k_push_tile is built for 2 CTAs per SM
+    g->use_tiles = true;
+    if (const char* sv = getenv("MEDPY_GC_SOLVER")) if (!strcmp(sv, "v0")) g->use_tiles = false;
+    if (const char* e1 = getenv("MEDPY_GC_ITERS")) if (atoi(e1) > 0) g->tile_iters = g->tile_iters_first = atoi(e1);
+    if (const char* e2 = getenv("MEDPY_GC_PASSES0")) if (atoi(e2) > 0) g->passes0 = atoi(e2);
+    if (const char* e3 = getenv("MEDPY_GC_PASSES_MAX")) if (atoi(e3) > 0) g->passes_max = atoi(e3);
+    if (const char* e7 = getenv("MEDPY_GC_SWEEP")) g->use_sweeps = atoi(e7) != 0;
+    if (const char* e8 = getenv("MEDPY_GC_SWEEP_FRAC")) if (atoi(e8) > 0) g->sweep_frac = atoi(e8);
+    if (const char* e9 = getenv("MEDPY_GC_SWEEP_ROUNDS")) if (atoi(e9) > 0) g->sweep_rounds_max = atoi(e9);
+    if (const char* e11 = getenv("MEDPY_GC_SWEEP_MIN_ROUNDS")) if (atoi(e11) > 0) g->sweep_rounds_min = atoi(e11);
+    if (const char* e10 = getenv("MEDPY_GC_SWEEP_DONE_FRAC")) if (atoi(e10) > 0) g->sweep_done_frac = atoi(e10);
+    int coop = 0, nb = 0;
+    const char* e5 = getenv("MEDPY_GC_BFS");
+    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, g->device);
+    if ((!e5 || strcmp(e5, "host") != 0) && coop &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, bfs, bfs_threads, 0) == cudaSuccess && nb >= 1)
+        g->coop_bfs_grid = nb * cached_sm_count(g->device);
+    else
+        cudaGetLastError();
+}
+
 int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool slab, int32_t device, mgc_graph** out)
 {
     if (!out) return MGC_E_ARG;
@@ -639,34 +663,13 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
         {   // dirty-tile tracking for the partial relabel reset (MEDPY_GC_PARTIAL_RESET=0: off)
             const char* ed = getenv("MEDPY_GC_PARTIAL_RESET");
             g->TL.dflag = nullptr; g->TL.ditems = nullptr; g->TL.dcount = nullptr;
-            g->TL.schg = nullptr; g->TL.sweep_stamp = 0;
-            {   // MEDPY_GC_SWEEP_CHECK=0: tile marks + k_sweep_list instead of the exhaustive fixed-point check.  Opt-in because
-                // "changed in the last round, or next to it" is a much larger worklist than "still
-                // violating", and the finishing BFS pays per listed tile -- so the check pass stays the default.
-                const char* es = getenv("MEDPY_GC_SWEEP_CHECK");
-                if (!rc && es && atoi(es) == 0) {
-                    rc = alloc_buf(g, tb, &p); g->TL.schg = (int*)p;
-                    if (!rc && cudaMemset(p, 0, tb) != cudaSuccess) { cudaGetLastError(); g->TL.schg = nullptr; }
-                }
-            }
             if (!rc && (!ed || atoi(ed) != 0)) {
                 rc = alloc_buf(g, tb, &p); g->TL.dflag = (int*)p;
                 if (!rc) { rc = alloc_buf(g, tb, &p); g->TL.ditems = (int*)p; }
                 if (!rc) { rc = alloc_buf(g, 64, &p); g->TL.dcount = (int*)p; }
             }
         }
-        g->n_ctas = 2 * cached_sm_count(device);   // k_push_tile is built for 2 CTAs per SM
-        g->use_tiles = true;
-        if (const char* sv = getenv("MEDPY_GC_SOLVER")) if (!strcmp(sv, "v0")) g->use_tiles = false;
-        if (const char* e1 = getenv("MEDPY_GC_ITERS")) if (atoi(e1) > 0) g->tile_iters = g->tile_iters_first = atoi(e1);
-        if (const char* e2 = getenv("MEDPY_GC_PASSES0")) if (atoi(e2) > 0) g->passes0 = atoi(e2);
-        if (const char* e3 = getenv("MEDPY_GC_PASSES_MAX")) if (atoi(e3) > 0) g->passes_max = atoi(e3);
-        if (const char* e4 = getenv("MEDPY_GC_COOP")) g->use_coop = atoi(e4) != 0;
-        if (const char* e7 = getenv("MEDPY_GC_SWEEP")) g->use_sweeps = atoi(e7) != 0;
-        if (const char* e8 = getenv("MEDPY_GC_SWEEP_FRAC")) if (atoi(e8) > 0) g->sweep_frac = atoi(e8);
-        if (const char* e9 = getenv("MEDPY_GC_SWEEP_ROUNDS")) if (atoi(e9) > 0) g->sweep_rounds_max = atoi(e9);
-        if (const char* e11 = getenv("MEDPY_GC_SWEEP_MIN_ROUNDS")) if (atoi(e11) > 0) g->sweep_rounds_min = atoi(e11);
-        if (const char* e10 = getenv("MEDPY_GC_SWEEP_DONE_FRAC")) if (atoi(e10) > 0) g->sweep_done_frac = atoi(e10);
+        tile_solver_options(g, (const void*)k_bfs_coop, TILE_VOX);
         {
             const char* e6 = getenv("MEDPY_GC_TMA");
             const size_t smem = 2 * TMA_STAGE_BYTES + 6 * TILE_VOX * sizeof(double) + 1024 * sizeof(int) + 64;
@@ -675,27 +678,6 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
                 g->use_tma = true;
             else
                 cudaGetLastError();
-        }
-        {
-            int coop = 0, nb = 0;
-            const char* e5 = getenv("MEDPY_GC_BFS");
-            cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device);
-            if ((!e5 || strcmp(e5, "host") != 0) && coop &&
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_bfs_coop, TILE_VOX, 0) == cudaSuccess && nb >= 1)
-                g->coop_bfs_grid = nb * cached_sm_count(device);
-            else
-                cudaGetLastError();
-        }
-        {
-            int coop = 0, nb = 0;
-            cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device);
-            if (!g->use_coop) { /* not requested */ }
-            else if (!coop || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_solve_coop<double>, TILE_VOX, 0) != cudaSuccess || nb < 1) {
-                cudaGetLastError();
-                g->use_coop = false;
-            } else {
-                g->coop_grid = nb * cached_sm_count(device);
-            }
         }
     }
     if (!rc && g->nd == 4 && !slab) {
@@ -710,27 +692,7 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
         for (int i = 0; i < 4 && !rc; ++i) { rc = alloc_buf(g, tb, &p); g->pl_items[i >> 1][i & 1] = (int*)p; }
         if (!rc) { rc = alloc_buf(g, 256, &p); g->d_tcount = (int*)p; }
         if (!rc) { rc = alloc_buf(g, nb, &p); g->smask = (uint8_t*)p; }
-        g->n_ctas = 2 * cached_sm_count(device);
-        g->use_tiles = true;
-        if (const char* sv = getenv("MEDPY_GC_SOLVER")) if (!strcmp(sv, "v0")) g->use_tiles = false;
-        {
-            int coop = 0, nbk = 0;
-            const char* e5 = getenv("MEDPY_GC_BFS");
-            cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device);
-            if ((!e5 || strcmp(e5, "host") != 0) && coop &&
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nbk, k_bfs_coop4, T4_VOX, 0) == cudaSuccess && nbk >= 1)
-                g->coop_bfs_grid = nbk * cached_sm_count(device);
-            else
-                cudaGetLastError();
-        }
-        if (const char* e1 = getenv("MEDPY_GC_ITERS")) if (atoi(e1) > 0) g->tile_iters = g->tile_iters_first = atoi(e1);
-        if (const char* e2 = getenv("MEDPY_GC_PASSES0")) if (atoi(e2) > 0) g->passes0 = atoi(e2);
-        if (const char* e3 = getenv("MEDPY_GC_PASSES_MAX")) if (atoi(e3) > 0) g->passes_max = atoi(e3);
-        if (const char* e7 = getenv("MEDPY_GC_SWEEP")) g->use_sweeps = atoi(e7) != 0;
-        if (const char* e8 = getenv("MEDPY_GC_SWEEP_FRAC")) if (atoi(e8) > 0) g->sweep_frac = atoi(e8);
-        if (const char* e9 = getenv("MEDPY_GC_SWEEP_ROUNDS")) if (atoi(e9) > 0) g->sweep_rounds_max = atoi(e9);
-        if (const char* e11 = getenv("MEDPY_GC_SWEEP_MIN_ROUNDS")) if (atoi(e11) > 0) g->sweep_rounds_min = atoi(e11);
-        if (const char* e10 = getenv("MEDPY_GC_SWEEP_DONE_FRAC")) if (atoi(e10) > 0) g->sweep_done_frac = atoi(e10);
+        tile_solver_options(g, (const void*)k_bfs_coop4, T4_VOX);
     }
     if (rc) { g_create_error = g->err; mgc_destroy(g); return rc; }
     if (cudaStreamCreate(&g->stream) != cudaSuccess) { g_create_error = "cudaStreamCreate failed"; mgc_destroy(g); return MGC_E_CUDA; }
@@ -1158,15 +1120,13 @@ int relabel_tiles_begin(mgc_graph* g)
 int relabel_sweep_round(mgc_graph* g, int* pending, bool with_check)
 {
     const int last = g->nd - 1;
-    if (g->nd == 3 && g->TL.schg) g->TL.sweep_stamp++;        // marks of this round (the array is never cleared)
     for (int a = 0; a < last; ++a) {
         if (g->L.dim[a] < 2) continue;
         const unsigned nlines = g->L.n / (unsigned)g->L.dim[a];
-        k_sweep_axis<<<(nlines + 255u) / 256u, 256, 0, g->stream>>>(g->L, g->TL, g->S.rmask, g->S.height, a);
+        k_sweep_axis<<<(nlines + 255u) / 256u, 256, 0, g->stream>>>(g->L, g->S.rmask, g->S.height, a);
         g->st.kernel_launches++;
     }
-    const bool marks = g->nd == 3 && g->TL.schg;      // the short-row kernel does not mark tiles: 3-D lattices use the general one
-    if (g->L.dim[last] >= 2 && g->L.dim[last] <= SWEEP_SHORT && !marks) {
+    if (g->L.dim[last] >= 2 && g->L.dim[last] <= SWEEP_SHORT) {
         const unsigned nrows = g->L.n / (unsigned)g->L.dim[last];
         k_sweep_rows_short<<<(nrows + 255u) / 256u, 256, 0, g->stream>>>(g->L, g->S.rmask, g->S.height);
         g->st.kernel_launches++;
@@ -1175,7 +1135,7 @@ int relabel_sweep_round(mgc_graph* g, int* pending, bool with_check)
         unsigned grid = (nrows + SWEEP_WARPS - 1) / SWEEP_WARPS;
         const unsigned cap = (unsigned)cached_sm_count(g->device) * 16u;
         if (grid > cap) grid = cap;
-        k_sweep_rows<<<grid, 32 * SWEEP_WARPS, 0, g->stream>>>(g->L, g->TL, g->S.rmask, g->S.height);
+        k_sweep_rows<<<grid, 32 * SWEEP_WARPS, 0, g->stream>>>(g->L, g->S.rmask, g->S.height);
         g->st.kernel_launches++;
     }
     g->st.relabel_sweeps++;
@@ -1183,7 +1143,6 @@ int relabel_sweep_round(mgc_graph* g, int* pending, bool with_check)
     CK(cudaMemsetAsync(g->d_tcount, 0, 2 * sizeof(int), g->stream));
     CK(cudaMemsetAsync(g->rflag, 0, (size_t)g->TL.ntiles * sizeof(int), g->stream));
     if (g->nd == 4) k_relabel_check4<<<nblocks(g), 256, 0, g->stream>>>(g->L, g->TL4, g->S.rmask, g->S.height, g->rflag, rl(g, 0));
-    else if (g->TL.schg) k_sweep_list<<<(g->TL.ntiles + 255) / 256, 256, 0, g->stream>>>(g->TL, g->rflag, rl(g, 0));
     else            k_relabel_check<<<nblocks(g), 256, 0, g->stream>>>(g->L, g->TL, g->S.rmask, g->S.height, g->rflag, rl(g, 0));
     g->st.kernel_launches++;
     g->rl_cur = 0;
@@ -1223,7 +1182,7 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true, bool first =
         }
     }
     // the sweep decision is made above; the cap needs an easy instance of the 3-D tile solver, where the label window runs
-    const bool capped = first && g->first_cap >= 2 && g->sweep_mode == 0 && g->nd == 3 && !g->slab && !g->use_coop;
+    const bool capped = first && g->first_cap >= 2 && g->sweep_mode == 0 && g->nd == 3 && !g->slab;
     int cap = capped ? g->first_cap : MGC_HINF;
     g->labels_capped = capped;
     if (g->coop_bfs_grid > 0 && g->use_tiles) {
@@ -1357,10 +1316,9 @@ int push_color(mgc_graph* g, int color)
     return MGC_OK;
 }
 
-int push_tiles(mgc_graph* g, int passes)
+// `passes` two-colour passes: colour 0's list, then colour 1's
+int push_passes(mgc_graph* g, int passes)
 {
-    Nvtx range("mgc:push_passes");
-    cudaEventRecord(g->ev[2], g->stream);
     for (int p = 0; p < passes; ++p) {
         int rc = push_color(g, 0);
         if (rc) return rc;
@@ -1369,6 +1327,15 @@ int push_tiles(mgc_graph* g, int passes)
     }
     g->st.push_sweeps += passes;
     CK(cudaGetLastError());
+    return MGC_OK;
+}
+
+int push_tiles(mgc_graph* g, int passes)
+{
+    Nvtx range("mgc:push_passes");
+    cudaEventRecord(g->ev[2], g->stream);
+    int rc = push_passes(g, passes);
+    if (rc) return rc;
     if (g->slab) return MGC_OK;      // slabs are stepped asynchronously: no per-call timing synchronisation
     cudaEventRecord(g->ev[3], g->stream);
     CK(cudaEventSynchronize(g->ev[3]));
@@ -1402,41 +1369,6 @@ int count_active_tiles(mgc_graph* g, int64_t* out)
     CK(cudaStreamSynchronize(g->stream));
     *out = (int64_t)c;
     g->st.active_last = (int64_t)c;
-    return MGC_OK;
-}
-
-// One cooperative launch running the phases selected by `flags` (gc_persist.cuh); the host mirrors of the list
-// selectors and the statistics are refreshed from the control block afterwards.
-int solve_coop(mgc_graph* g, int flags, int passes, int64_t* active_out)
-{
-    if (flags & (SOLVE_F_PUSH | SOLVE_F_LOOP)) g->flow_started = true;
-    g->labels_capped = false;
-    { int rc0 = push_state_all(g); if (rc0) return rc0; }       // the cooperative solve pushes wherever it likes
-    int hdr[4] = {0, g->pl_sel[0], g->pl_sel[1], g->rl_cur};     // cursor, list selectors
-    CK(cudaMemcpyAsync(g->d_tcount + CTL_CURSOR, hdr, sizeof(hdr), cudaMemcpyHostToDevice, g->stream));
-    SolveLists SL;
-    SL.rl_items[0] = g->rl_items[0]; SL.rl_items[1] = g->rl_items[1];
-    for (int c = 0; c < 2; ++c) for (int b = 0; b < 2; ++b) SL.pl_items[c][b] = g->pl_items[c][b];
-    unsigned long long* active = g->d_count;
-    unsigned long long* timers = g->d_count + 1;
-    int iters = g->tile_iters, pmax = g->passes_max, mr = (int)(g->max_rounds > 0x7fffffff ? 0x7fffffff : g->max_rounds);
-    void* args[] = {&g->L, &g->TL, &g->S, &SL, &g->rflag, &g->pflag, &g->d_tcount, &active, &timers,
-                    &flags, &iters, &passes, &pmax, &mr};
-    CK(cudaLaunchCooperativeKernel((void*)k_solve_coop<double>, dim3(g->coop_grid), dim3(TILE_VOX), args, 0, g->stream));
-    g->st.kernel_launches++;
-    int ctl[20];
-    unsigned long long cnt[3];
-    CK(cudaMemcpyAsync(ctl, g->d_tcount, sizeof(ctl), cudaMemcpyDeviceToHost, g->stream));
-    CK(cudaMemcpyAsync(cnt, g->d_count, sizeof(cnt), cudaMemcpyDeviceToHost, g->stream));
-    CK(cudaStreamSynchronize(g->stream));
-    g->pl_sel[0] = ctl[CTL_SEL0]; g->pl_sel[1] = ctl[CTL_SEL0 + 1]; g->rl_cur = ctl[CTL_RLCUR];
-    g->st.push_sweeps += ctl[CTL_PUSHP];
-    g->st.relabel_sweeps += ctl[CTL_RELP];
-    g->st.global_relabels += ctl[CTL_GREL];
-    g->st.ms_relabel += 1e-6 * (double)cnt[1];
-    g->st.ms_push += 1e-6 * (double)cnt[2];
-    if (flags & (SOLVE_F_COUNT | SOLVE_F_LOOP)) { g->st.active_last = (int64_t)cnt[0]; if (active_out) *active_out = (int64_t)cnt[0]; }
-    if (ctl[CTL_STATUS] != 0) FAIL(MGC_E_NOCONV, "push-relabel did not converge within the round cap");
     return MGC_OK;
 }
 
@@ -1481,11 +1413,6 @@ int solve_tiles(mgc_graph* g)
         if (rc) return rc;
     }
     if (g->win_ctl) CK(cudaMemsetAsync(g->win_ctl + WIN_DEFERRED, 0, 2 * sizeof(int), g->stream));    // per-solve window counts
-    if (g->use_coop && g->nd == 3) {
-        const int flags = SOLVE_F_LOOP | (g->labels_fresh ? 0 : SOLVE_F_RESET);
-        g->labels_fresh = false;
-        return solve_coop(g, flags, g->passes0, nullptr);
-    }
     // One host synchronisation per round: relabel (reset + BFS), stop test and the previous round's push passes are all
     // enqueued back to back; the host waits once, reads the active count and the CUDA-event times of both phases and
     // decides.  The stop test of the FIRST round is skipped (a graph that was just built almost always has active
@@ -1553,17 +1480,11 @@ int solve_tiles(mgc_graph* g)
         {
             Nvtx range("mgc:push_passes");
             cudaEventRecord(g->ev[4], g->stream);
-            for (int p = 0; p < passes; ++p) {
-                rc = push_color(g, 0);
-                if (rc) return rc;
-                rc = push_color(g, 1);
-                if (rc) return rc;
-            }
+            rc = push_passes(g, passes);
+            if (rc) return rc;
             cudaEventRecord(g->ev[5], g->stream);
-            g->st.push_sweeps += passes;
             passes_done = passes;
             push_open = true;
-            CK(cudaGetLastError());
         }
     }
     g->init_timed = false;       // ev[4..5] were reused for the push spans
@@ -1574,8 +1495,7 @@ int readout(mgc_graph* g, double* energy_part)
 {
     Nvtx range("mgc:readout");
     // clean tiles hold the reset labels while no sweep has lowered labels unmarked (the partial reset relies on the same)
-    const bool clean = g->use_tiles && g->nd == 3 && !g->slab && g->TL.dflag && g->sweep_mode != 1 && !g->use_coop &&
-                       g->L.dim[2] % 4 == 0;
+    const bool clean = g->use_tiles && g->nd == 3 && !g->slab && g->TL.dflag && g->sweep_mode != 1 && g->L.dim[2] % 4 == 0;
     if (clean) k_readout<double, true, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials, g->TL.dflag,
                                                                                 g->TL.nt[1], g->TL.nt[2]);
     else if (g->use_tiles && g->nd == 3) k_readout<double, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
@@ -3156,7 +3076,7 @@ int mgc_slab_push(mgc_graph* g, int32_t n)
     if (!g->state_init) FAIL(MGC_E_STATE, "call mgc_slab_begin first");
     CK(cudaSetDevice(g->device));
     g->iters_now = g->tile_iters;
-    if (g->use_tiles) return g->use_coop ? solve_coop(g, SOLVE_F_PUSH, n, nullptr) : push_tiles(g, n);
+    if (g->use_tiles) return push_tiles(g, n);
     return push_sweeps(g, n, nullptr);
 }
 
@@ -3225,15 +3145,7 @@ int mgc_slab_relabel_relax(mgc_graph* g, int32_t* changed_out)
     if (!g) return MGC_E_ARG;
     CK(cudaSetDevice(g->device));
     int any = 0;
-    int rc = MGC_OK;
-    if (g->use_tiles && g->use_coop) {
-        const int64_t before = g->st.relabel_sweeps;
-        rc = solve_coop(g, SOLVE_F_BFS, 0, nullptr);
-        any = g->st.relabel_sweeps != before;
-        g->st.global_relabels--;      // counted by mgc_slab_relabel_begin already
-    } else {
-        rc = g->use_tiles ? relabel_tiles_run(g, &any, changed_out != nullptr) : relabel_relax(g, &any);
-    }
+    const int rc = g->use_tiles ? relabel_tiles_run(g, &any, changed_out != nullptr) : relabel_relax(g, &any);
     if (rc) return rc;
     if (changed_out) *changed_out = any ? 1 : 0;
     return MGC_OK;

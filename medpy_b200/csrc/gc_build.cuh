@@ -862,15 +862,3 @@ __global__ void __launch_bounds__(TILE_VOX) k_count_active_tiles2(Lattice L, Til
     for (int o = 16; o > 0; o >>= 1) mine += __shfl_down_sync(0xffffffffu, mine, o);
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(count, (unsigned long long)mine);
 }
-
-// ---------------------------------------------------------------------------------------------------
-// marker volumes -> bit planes (device side; the host binding packs on the CPU for the end-to-end path so that the
-// markers cross PCIe as 0.25 B/voxel instead of 2): bit (v & 31) of word (v >> 5) = marker[v] != 0
-// ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_pack_bits(const uint8_t* __restrict__ src, unsigned n, unsigned* __restrict__ dst)
-{
-    const unsigned v = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool on = v < n && src[v] != 0;
-    const unsigned w = __ballot_sync(0xffffffffu, on);
-    if ((threadIdx.x & 31) == 0 && v < n) dst[v >> 5] = w;
-}

@@ -30,28 +30,9 @@ __device__ __forceinline__ int sweep_inc(int h) { return h >= MGC_HINF ? MGC_HIN
 // `line` enumerates the lines: line = hi * stride + lo with lo = position inside one axis-plane (all faster axes)
 // and hi = combined index of the slower axes, so the first voxel of the line is hi * dim * stride + lo.
 // ---------------------------------------------------------------------------------------------------
-// tile marking: a thread that lowers a label stores the round's stamp into schg[] of the voxel's 8^3 tile (once per tile it
-// walks through).  After the round, only tiles that changed -- and their face neighbours -- can hold a voxel that is not
-// at the fixed point: every residual arc (v -> w) is relaxed once per round, at which moment h(v) <= h(w) + 1 holds; it can
-// only break if h(w) is lowered LATER in the same round, i.e. if w's tile is marked.  k_sweep_list turns the marks into the
-// worklist of the finishing BFS, which replaces the 5 B/voxel check pass of the first version.
-struct SweepMark {
-    int* schg;          // nullptr: no marking (4-D lattices use k_relabel_check4)
-    int stamp;
-    int tbase;          // tile index of the line's first voxel
-    int tstride;        // tile-index stride along the line's axis
-    int last;           // last tile marked by this thread
-    __device__ __forceinline__ void hit(int i)
-    {
-        if (!schg) return;
-        const int t = tbase + (i >> 3) * tstride;
-        if (t != last) { schg[t] = stamp; last = t; }
-    }
-};
-
 template <bool FWD>
 __device__ __forceinline__ void sweep_line(const uint8_t* __restrict__ rmask, int* __restrict__ height, unsigned base,
-                                           unsigned stride, int D, int i_own0, int i_own1, unsigned bit, SweepMark& mk)
+                                           unsigned stride, int D, int i_own0, int i_own1, unsigned bit)
 {
     int carry = MGC_HINF;
     for (int i0 = 0; i0 < D; i0 += SWEEP_UNROLL) {
@@ -75,7 +56,7 @@ __device__ __forceinline__ void sweep_line(const uint8_t* __restrict__ rmask, in
                 int h = hb[u];
                 if ((mb[u] & bit) && i >= i_own0 && i < i_own1) {
                     const int cand = sweep_inc(carry);
-                    if (cand < h) { h = cand; height[base + (unsigned)i * stride] = h; mk.hit(i); }
+                    if (cand < h) { h = cand; height[base + (unsigned)i * stride] = h; }
                 }
                 carry = h;
             }
@@ -83,7 +64,7 @@ __device__ __forceinline__ void sweep_line(const uint8_t* __restrict__ rmask, in
     }
 }
 
-__global__ void __launch_bounds__(256) k_sweep_axis(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask, int* __restrict__ height, int axis)
+__global__ void __launch_bounds__(256) k_sweep_axis(Lattice L, const uint8_t* __restrict__ rmask, int* __restrict__ height, int axis)
 {
     const unsigned stride = L.stride[axis];
     const int D = L.dim[axis];
@@ -98,19 +79,10 @@ __global__ void __launch_bounds__(256) k_sweep_axis(Lattice L, Tiles TL, const u
         const int z = (int)(base / L.stride[0]);
         if (z < L.own0 || z >= L.own1) return;          // a line inside a ghost plane: nothing to relabel
     }
-    SweepMark mk{nullptr, 0, 0, 0, -1};
-    if (L.nd == 3 && TL.schg) {
-        int c[3];
-        decode<3>(L, base, c);
-        c[axis] = 0;
-        mk.schg = TL.schg; mk.stamp = TL.sweep_stamp;
-        mk.tbase = ((c[0] >> 3) * TL.nt[1] + (c[1] >> 3)) * TL.nt[2] + (c[2] >> 3);
-        mk.tstride = axis == 0 ? TL.nt[1] * TL.nt[2] : (axis == 1 ? TL.nt[2] : 1);
-    }
     // forward: voxel i receives from i-1 through its own arc towards -axis (bit 2*axis)
-    sweep_line<true>(rmask, height, base, stride, D, i_own0, i_own1, 1u << (2 * axis), mk);
+    sweep_line<true>(rmask, height, base, stride, D, i_own0, i_own1, 1u << (2 * axis));
     // backward: voxel i receives from i+1 through its arc towards +axis
-    sweep_line<false>(rmask, height, base, stride, D, i_own0, i_own1, 1u << (2 * axis + 1), mk);
+    sweep_line<false>(rmask, height, base, stride, D, i_own0, i_own1, 1u << (2 * axis + 1));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -128,8 +100,7 @@ __device__ __forceinline__ int srow_idx(int x) { return x + (x >> 5); }   // one
 // one direction over the staged segment [0, n): FWD = towards +x.  carry_in = label of the voxel in front of the
 // segment (HINF if none); returns the label of the segment's last voxel in sweep direction.  `changed` accumulates.
 template <bool FWD>
-__device__ __forceinline__ int sweep_row_dir(int* sh, const uint8_t* sm, int n, int len, unsigned bit, int carry_in, int& changed,
-                                             SweepMark& mk, int x_off)
+__device__ __forceinline__ int sweep_row_dir(int* sh, const uint8_t* sm, int n, int len, unsigned bit, int carry_in, int& changed)
 {
     const int lane = threadIdx.x & 31;
     const int c0 = lane * len;
@@ -144,7 +115,7 @@ __device__ __forceinline__ int sweep_row_dir(int* sh, const uint8_t* sm, int n, 
         const bool open = (sm[x] & bit) != 0;
         if (open) {
             const int cand = sweep_inc(prev);
-            if (cand < h) { h = cand; sh[srow_idx(x)] = h; changed = 1; mk.hit(x_off + x); }
+            if (cand < h) { h = cand; sh[srow_idx(x)] = h; changed = 1; }
         }
         if (chain) { if (open) ++nopen; else chain = false; }
         prev = h;
@@ -181,7 +152,7 @@ __device__ __forceinline__ int sweep_row_dir(int* sh, const uint8_t* sm, int n, 
         for (int j = 0; j < nopen; ++j) {
             const int x = FWD ? c0 + j : c0 + cnt - 1 - j;
             c = sweep_inc(c);
-            if (c < sh[srow_idx(x)]) { sh[srow_idx(x)] = c; changed = 1; mk.hit(x_off + x); }
+            if (c < sh[srow_idx(x)]) { sh[srow_idx(x)] = c; changed = 1; }
             else break;                 // from here on my own labels are at least as good (they grow by <= 1 per step)
         }
     }
@@ -206,7 +177,7 @@ __device__ __forceinline__ void srow_store(int* __restrict__ height, unsigned g0
     for (int x = lane; x < n; x += 32) height[g0 + x] = sh[srow_idx(x)];
 }
 
-__global__ void __launch_bounds__(32 * SWEEP_WARPS) k_sweep_rows(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask, int* __restrict__ height)
+__global__ void __launch_bounds__(32 * SWEEP_WARPS) k_sweep_rows(Lattice L, const uint8_t* __restrict__ rmask, int* __restrict__ height)
 {
     __shared__ int s_h[SWEEP_WARPS][SWEEP_ROW_PAD];
     __shared__ uint8_t s_m[SWEEP_WARPS][SWEEP_ROW_MAX];
@@ -222,19 +193,13 @@ __global__ void __launch_bounds__(32 * SWEEP_WARPS) k_sweep_rows(Lattice L, Tile
         const unsigned g = row * (unsigned)X;
         const int z = (int)(g / L.stride[0]);
         if (z < L.own0 || z >= L.own1) continue;
-        SweepMark mk{nullptr, 0, 0, 1, -1};
-        if (L.nd == 3 && TL.schg) {
-            const int y = (int)((g - (unsigned)z * L.stride[0]) / L.stride[1]);
-            mk.schg = TL.schg; mk.stamp = TL.sweep_stamp;
-            mk.tbase = ((z >> 3) * TL.nt[1] + (y >> 3)) * TL.nt[2];
-        }
         if (nseg == 1) {
             const int len = (X + 31) >> 5;
             srow_load(rmask, height, g, X, sh, sm);
             int changed = 0;
-            sweep_row_dir<true>(sh, sm, X, len, bit_m, MGC_HINF, changed, mk, 0);
+            sweep_row_dir<true>(sh, sm, X, len, bit_m, MGC_HINF, changed);
             __syncwarp();
-            sweep_row_dir<false>(sh, sm, X, len, bit_p, MGC_HINF, changed, mk, 0);
+            sweep_row_dir<false>(sh, sm, X, len, bit_p, MGC_HINF, changed);
             if (__any_sync(0xffffffffu, changed)) srow_store(height, g, X, sh);
             __syncwarp();
         } else {
@@ -243,7 +208,7 @@ __global__ void __launch_bounds__(32 * SWEEP_WARPS) k_sweep_rows(Lattice L, Tile
                 const int x0 = s * SWEEP_ROW_MAX, n = min(SWEEP_ROW_MAX, X - x0);
                 srow_load(rmask, height, g + x0, n, sh, sm);
                 int changed = 0;
-                carry = sweep_row_dir<true>(sh, sm, n, (n + 31) >> 5, bit_m, carry, changed, mk, x0);
+                carry = sweep_row_dir<true>(sh, sm, n, (n + 31) >> 5, bit_m, carry, changed);
                 if (__any_sync(0xffffffffu, changed)) srow_store(height, g + x0, n, sh);
                 __syncwarp();
             }
@@ -252,7 +217,7 @@ __global__ void __launch_bounds__(32 * SWEEP_WARPS) k_sweep_rows(Lattice L, Tile
                 const int x0 = s * SWEEP_ROW_MAX, n = min(SWEEP_ROW_MAX, X - x0);
                 srow_load(rmask, height, g + x0, n, sh, sm);
                 int changed = 0;
-                carry = sweep_row_dir<false>(sh, sm, n, (n + 31) >> 5, bit_p, carry, changed, mk, x0);
+                carry = sweep_row_dir<false>(sh, sm, n, (n + 31) >> 5, bit_p, carry, changed);
                 if (__any_sync(0xffffffffu, changed)) srow_store(height, g + x0, n, sh);
                 __syncwarp();
             }
@@ -317,26 +282,6 @@ __global__ void __launch_bounds__(256) k_relabel_check(Lattice L, Tiles TL, cons
         const int t = ((c[0] >> 3) * TL.nt[1] + (c[1] >> 3)) * TL.nt[2] + (c[2] >> 3);
         if (*(volatile int*)(rflag + t) == 0) list_push(rflag, rl, t);
     }
-}
-
-// worklist of the finishing BFS from the sweep marks: a tile is listed if it, or one of its six face neighbours, was
-// marked in the round `TL.sweep_stamp` (see SweepMark).  One thread per tile; rflag and the list count are zeroed by the host.
-__global__ void __launch_bounds__(256) k_sweep_list(Tiles TL, int* __restrict__ rflag, WorkList rl)
-{
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= TL.ntiles) return;
-    const int st = TL.sweep_stamp;
-    const int tx = t % TL.nt[2];
-    const int r = t / TL.nt[2];
-    const int ty = r % TL.nt[1], tz = r / TL.nt[1];
-    bool hit = TL.schg[t] == st;
-    if (!hit && tz > 0) hit = TL.schg[t - TL.nt[1] * TL.nt[2]] == st;
-    if (!hit && tz + 1 < TL.nt[0]) hit = TL.schg[t + TL.nt[1] * TL.nt[2]] == st;
-    if (!hit && ty > 0) hit = TL.schg[t - TL.nt[2]] == st;
-    if (!hit && ty + 1 < TL.nt[1]) hit = TL.schg[t + TL.nt[2]] == st;
-    if (!hit && tx > 0) hit = TL.schg[t - 1] == st;
-    if (!hit && tx + 1 < TL.nt[2]) hit = TL.schg[t + 1] == st;
-    if (hit) list_push(rflag, rl, t);
 }
 
 // 4-D lattices (4 x 4 x 8 x 4 tiles of gc_tiles4.cuh; all eight mask bits are arcs, the sink flag lives in smask and is

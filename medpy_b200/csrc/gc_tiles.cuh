@@ -40,9 +40,6 @@ struct Tiles {
     int* dflag;     // per tile: already on the dirty list (nullptr: tracking off)
     int* ditems;    // the dirty list
     int* dcount;
-    // directional sweeps (gc_sweep.cuh): schg[t] = stamp of the last sweep round that lowered a label inside tile t
-    int* schg;
-    int sweep_stamp;
 };
 
 __device__ __forceinline__ void mark_dirty(const Tiles& TL, int t)
@@ -199,8 +196,8 @@ __global__ void __launch_bounds__(TILE_VOX) k_init_tile(Lattice L, Tiles TL, Sta
 // later global relabels: labels from the (incrementally maintained) residual mask; 1 B read + 4 B written per voxel.
 // One thread per 8-voxel x-run of a tile row, consecutive threads on consecutive runs (coalesced); rflag must be
 // zero on entry (the host memsets it): a run that holds an unlabelled voxel with residual out-arcs lists its tile.
-__device__ __forceinline__ void relabel_reset_body(const Lattice& L, const Tiles& TL, const uint8_t* __restrict__ rmask,
-                                                   int* __restrict__ height, int* __restrict__ rflag, const WorkList& rl)
+__global__ void __launch_bounds__(256) k_relabel_reset(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask,
+                                                       int* __restrict__ height, int* __restrict__ rflag, WorkList rl)
 {
     const unsigned ntx = (unsigned)TL.nt[2];
     const unsigned nruns = (unsigned)L.dim[0] * (unsigned)L.dim[1] * ntx;
@@ -234,12 +231,6 @@ __device__ __forceinline__ void relabel_reset_body(const Lattice& L, const Tiles
         }
         if (needs) list_push(rflag, rl, (int)(((gz >> 3) * (unsigned)TL.nt[1] + (gy >> 3)) * ntx + tx));
     }
-}
-
-__global__ void __launch_bounds__(256) k_relabel_reset(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask,
-                                                       int* __restrict__ height, int* __restrict__ rflag, WorkList rl)
-{
-    relabel_reset_body(L, TL, rmask, height, rflag, rl);
 }
 
 // the same reset restricted to the DIRTY tiles (Tiles::ditems): every other tile is still in the reset state, so an easy
@@ -485,14 +476,6 @@ __device__ __forceinline__ void push_visit_staged(const Lattice& L, const Tiles&
 }
 
 template <typename T>
-__device__ __forceinline__ void push_visit(const Lattice& L, const Tiles& TL, const State<T>& S, int iters,
-                                           int* __restrict__ pflag, const WorkList& self_next, const WorkList& other_next,
-                                           int t, T* s_out, int* s_h)
-{
-    push_visit_staged<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h, nullptr);
-}
-
-template <typename T>
 __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, State<T> S, int iters,
                                                            int* __restrict__ pflag, WorkList cur, int* __restrict__ cursor,
                                                            WorkList self_next, WorkList other_next, int labels_capped)
@@ -505,26 +488,6 @@ __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, 
         if (t < 0) break;
         push_visit_staged<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h, nullptr, labels_capped != 0);
     }
-}
-
-template <typename T>
-__device__ __forceinline__ void count_active_body(const Lattice& L, const Tiles& TL, const State<T>& S, const WorkList& wl,
-                                                  unsigned long long* __restrict__ count)
-{
-    const int n = *(volatile int*)wl.count;
-    for (int i = blockIdx.x; i < n; i += gridDim.x) {
-        const TileCtx c = tile_ctx(L, TL, wl.items[i]);
-        const bool act = c.own && (S.excess[c.v] > 0) && (S.height[c.v] < MGC_HINF);
-        const unsigned b = __ballot_sync(0xffffffffu, act);
-        if ((threadIdx.x & 31) == 0 && b) atomicAdd(count, (unsigned long long)__popc(b));
-    }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(TILE_VOX) k_count_active_tiles(Lattice L, Tiles TL, State<T> S, WorkList wl,
-                                                                 unsigned long long* __restrict__ count)
-{
-    count_active_body<T>(L, TL, S, wl, count);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -179,8 +179,7 @@ def test_round_trip_restores_the_pre_stroke_result(shape):
     assert abs(e2 - e0) <= 1e-9 * abs(e0), (e2, e0)
 
 
-@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_COOP=1),
-                                 dict(MEDPY_GC_DEBUG=1)])
+@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_DEBUG=1)])
 def test_warm_erase_solver_options(env):
     """MEDPY_GC_DEBUG=1 runs the conservation and invariant checks of every solve across the erase folds."""
     shape = (32, 32, 32)

@@ -146,7 +146,6 @@ def test_sweep_relabel_equals_worklist_relabel_and_oracle(shape, regional):
     vol = synthetic.two_blob_volume(shape, seed=11)
     out = []
     for env in (dict(MEDPY_GC_SWEEP=1, MEDPY_GC_SWEEP_FRAC=1000000), dict(MEDPY_GC_SWEEP=0), dict(),
-                dict(MEDPY_GC_SWEEP_FRAC=1000000, MEDPY_GC_SWEEP_CHECK=0),              # tile marks instead of the check pass
                 dict(MEDPY_GC_SWEEP_FRAC=1000000, MEDPY_GC_SWEEP_MIN_ROUNDS=1, MEDPY_GC_SWEEP_ROUNDS=4)):
         with _env(**env):
             g = _build(vol, regional=regional)

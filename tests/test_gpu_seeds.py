@@ -187,8 +187,7 @@ def test_warm_refinement_2d_and_1d():
         _check(vol, "difference_exponential", True, False, steps)
 
 
-@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_COOP=1),
-                                 dict(MEDPY_GC_DEBUG=1)])
+@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_DEBUG=1)])
 def test_warm_refinement_solver_options(env):
     shape = (32, 32, 32)
     vol = _volume(shape, seed=5, dtype="float32")

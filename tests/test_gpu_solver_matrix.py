@@ -26,7 +26,6 @@ OPTIONS = {
     "iters1": dict(MEDPY_GC_ITERS=1, MEDPY_GC_PASSES_MAX=1),
     "easy": dict(MEDPY_GC_SWEEP_FRAC=1),
     "hard": dict(MEDPY_GC_SWEEP_FRAC=1000000),
-    "coop": dict(MEDPY_GC_COOP=1),
     "debug": dict(MEDPY_GC_DEBUG=1),
     "easy_cap0": dict(MEDPY_GC_SWEEP_FRAC=1, MEDPY_GC_FIRST_CAP=0),     # only read by the `easy` cells
 }

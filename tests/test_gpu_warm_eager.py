@@ -264,9 +264,9 @@ def test_bad_ids_and_nan_leave_the_4d_result():
     assert abs(e2 - oe) <= 1e-9 * max(abs(oe), scale), (e2, oe)
 
 
-@pytest.mark.parametrize("env", [dict(MEDPY_GC_COOP=1), dict(MEDPY_GC_SWEEP=0), dict(MEDPY_GC_FIRST_CAP=0),
+@pytest.mark.parametrize("env", [dict(MEDPY_GC_SWEEP=0), dict(MEDPY_GC_FIRST_CAP=0),
                                  dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_DEBUG=1)],
-                         ids=["coop", "sweep0", "first_cap0", "partial_reset0", "debug"])
+                         ids=["sweep0", "first_cap0", "partial_reset0", "debug"])
 @pytest.mark.parametrize("handle,shape", [("4d", (12, 12, 16, 6)), ("eager", (32, 32, 32))])
 def test_solver_options(handle, shape, env):
     """MEDPY_GC_DEBUG=1 checks the invariants and flow conservation around every solve after every fold."""

@@ -211,8 +211,7 @@ def test_opted_in_warm_matches_from_scratch(handle, shape, which):
          env=_ENV.get(handle), warm=True)
 
 
-@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_COOP=1),
-                                 dict(MEDPY_GC_DEBUG=1)])
+@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_DEBUG=1)])
 def test_solver_options(env):
     """MEDPY_GC_DEBUG=1 checks the invariants (residual mask included) and flow conservation around every warm solve."""
     shape = (32, 32, 32)

@@ -179,8 +179,7 @@ def test_warm_tweights_2d_1d_and_ragged(shape, which):
     _check(vol, "difference_exponential", True, False, _sequences(shape, vol, which))
 
 
-@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_COOP=1),
-                                 dict(MEDPY_GC_DEBUG=1)])
+@pytest.mark.parametrize("env", [dict(MEDPY_GC_PARTIAL_RESET=0), dict(MEDPY_GC_FIRST_TEST=1), dict(MEDPY_GC_DEBUG=1)])
 def test_warm_tweights_solver_options(env):
     """MEDPY_GC_DEBUG=1 runs the conservation and invariant checks of every solve across the folds."""
     shape = (32, 32, 32)
