@@ -108,7 +108,7 @@ typedef struct mgc_stats {
     int64_t tiles_deferred;     /* 3-D tile solver, easy instance: listed tiles the label window held back, summed over the push launches of each solve */
     int64_t tiles_dropped;      /* ... listed tiles that left the push lists without a visit (no active voxel at a finite label) */
     int64_t relabel_passes;     /* tile solver: BFS passes (worklist generations) of all global relabels; relabel_sweeps counts launches */
-    double ms_relabel_first;    /* device ms of the first global relabel of each solve (3-D host-driven tile solver), summed */
+    double ms_relabel_first;    /* device ms of the first global relabel of each solve (tile solver), summed */
     int64_t relabel_passes_first; /* ... its BFS passes, summed */
 } mgc_stats;
 
@@ -257,7 +257,7 @@ int mgc_maxflow(mgc_graph* g, double* energy);
  *   - It persists across mgc_reset, like MGC_OPT_DEFER_WEIGHT_CHECK, and changes neither results nor the first solve's
  *     mask and energy.
  *   - A fold on such a handle before its first solve initialises the solver state and takes the record first.
- *   - The per-voxel solver (MEDPY_GC_SOLVER=v0) and z-slab handles still return MGC_E_STATE with the option set.
+ *   - z-slab handles still return MGC_E_STATE with the option set.
  * MGC_ABI_VERSION stays 3 and mgc_stats keeps its layout. */
 int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
 /* Seeds erased from a graph and solved warm: the inverse call of mgc_add_seeds, as the reference erases a seed

@@ -209,7 +209,7 @@ struct mgc_graph {
     Tiles TL{};
     Tiles4 TL4{};                      // 4-D lattices: 4x4x8x4 tiles (gc_tiles4.cuh)
     uint8_t* smask = nullptr;          // 4-D: residual sink link flag (the 8 arc bits fill rmask)
-    bool use_tiles = false;
+    bool use_tiles = false;            // false on 4-D z-slabs only: they run the per-voxel solver of gc_solver.cuh
     int* pflag = nullptr;              // push: tile is already on the list its colour consumes next
     int* rflag = nullptr;              // relabel: tile is already on the next relabel list
     int* rl_items[2] = {nullptr, nullptr};     // relabel worklists (double buffered)
@@ -222,10 +222,9 @@ struct mgc_graph {
     int* win_items = nullptr;
     int* win_ctl = nullptr;
     int* drop_items = nullptr;
-    int rl_cur = 0;                    // relabel list consumed next
     bool labels_fresh = false;         // labels + relabel list 0 come straight from k_init_tile
     int n_ctas = 264;                  // persistent CTAs per tile-kernel launch
-    int coop_bfs_grid = 0;             // co-resident CTAs of k_bfs_coop (0: per-pass host loop)
+    int coop_bfs_grid = 0;             // co-resident CTAs of k_bfs_coop / k_bfs_coop4
     bool use_tma = false;              // push kernel stages its tile planes with TMA (gc_tma.cuh)
     PushMaps maps{};                   // tensor maps of cap[0..5] and excess
     int tile_iters = 8;                // synchronous push/relabel rounds per tile visit
@@ -250,7 +249,6 @@ struct mgc_graph {
     int sweep_done_frac = 16;          // hand over to the worklist BFS when violating tiles <= ntiles / sweep_done_frac
 
     // tuning
-    int sweeps_per_round = 32;
     int relax_batch = 4;
     int64_t max_rounds = 100000;
 
@@ -546,12 +544,11 @@ bool make_push_maps(mgc_graph* g)
 
 // the environment options of the tile solver, the same for 3-D and 4-D lattices (4-D z-slab handles run the per-voxel
 // solver and read none of them).  `bfs` is the cooperative BFS kernel of the lattice's tile shape, launched with
-// `bfs_threads` threads per CTA: its occupancy sizes the grid (MEDPY_GC_BFS=host: the host-driven BFS instead).
-void tile_solver_options(mgc_graph* g, const void* bfs, int bfs_threads)
+// `bfs_threads` threads per CTA: its occupancy sizes the grid.
+int tile_solver_options(mgc_graph* g, const void* bfs, int bfs_threads)
 {
     g->n_ctas = 2 * cached_sm_count(g->device);   // k_push_tile is built for 2 CTAs per SM
     g->use_tiles = true;
-    if (const char* sv = getenv("MEDPY_GC_SOLVER")) if (!strcmp(sv, "v0")) g->use_tiles = false;
     if (const char* e1 = getenv("MEDPY_GC_ITERS")) if (atoi(e1) > 0) g->tile_iters = g->tile_iters_first = atoi(e1);
     if (const char* e2 = getenv("MEDPY_GC_PASSES0")) if (atoi(e2) > 0) g->passes0 = atoi(e2);
     if (const char* e3 = getenv("MEDPY_GC_PASSES_MAX")) if (atoi(e3) > 0) g->passes_max = atoi(e3);
@@ -561,13 +558,13 @@ void tile_solver_options(mgc_graph* g, const void* bfs, int bfs_threads)
     if (const char* e11 = getenv("MEDPY_GC_SWEEP_MIN_ROUNDS")) if (atoi(e11) > 0) g->sweep_rounds_min = atoi(e11);
     if (const char* e10 = getenv("MEDPY_GC_SWEEP_DONE_FRAC")) if (atoi(e10) > 0) g->sweep_done_frac = atoi(e10);
     int coop = 0, nb = 0;
-    const char* e5 = getenv("MEDPY_GC_BFS");
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, g->device);
-    if ((!e5 || strcmp(e5, "host") != 0) && coop &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, bfs, bfs_threads, 0) == cudaSuccess && nb >= 1)
-        g->coop_bfs_grid = nb * cached_sm_count(g->device);
-    else
+    if (!coop || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, bfs, bfs_threads, 0) != cudaSuccess || nb < 1) {
         cudaGetLastError();
+        FAIL(MGC_E_CUDA, "the cooperative BFS of the tile solver cannot be launched on this device (no co-resident CTA)");
+    }
+    g->coop_bfs_grid = nb * cached_sm_count(g->device);
+    return MGC_OK;
 }
 
 int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool slab, int32_t device, mgc_graph** out)
@@ -669,7 +666,7 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
                 if (!rc) { rc = alloc_buf(g, 64, &p); g->TL.dcount = (int*)p; }
             }
         }
-        tile_solver_options(g, (const void*)k_bfs_coop, TILE_VOX);
+        if (!rc) rc = tile_solver_options(g, (const void*)k_bfs_coop, TILE_VOX);
         {
             const char* e6 = getenv("MEDPY_GC_TMA");
             const size_t smem = 2 * TMA_STAGE_BYTES + 6 * TILE_VOX * sizeof(double) + 1024 * sizeof(int) + 64;
@@ -692,7 +689,7 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
         for (int i = 0; i < 4 && !rc; ++i) { rc = alloc_buf(g, tb, &p); g->pl_items[i >> 1][i & 1] = (int*)p; }
         if (!rc) { rc = alloc_buf(g, 256, &p); g->d_tcount = (int*)p; }
         if (!rc) { rc = alloc_buf(g, nb, &p); g->smask = (uint8_t*)p; }
-        tile_solver_options(g, (const void*)k_bfs_coop4, T4_VOX);
+        if (!rc) rc = tile_solver_options(g, (const void*)k_bfs_coop4, T4_VOX);
     }
     if (rc) { g_create_error = g->err; mgc_destroy(g); return rc; }
     if (cudaStreamCreate(&g->stream) != cudaSuccess) { g_create_error = "cudaStreamCreate failed"; mgc_destroy(g); return MGC_E_CUDA; }
@@ -714,7 +711,6 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
     // [0] weight verdict, [2..3] active count, [4] BFS passes of the last cooperative relabel.  From the pinned pool: cudaHostAlloc / cudaFreeHost per handle (one handle per
     // graph_from_voxels call) are heavyweight driver calls that synchronise the device
     { void* hp = nullptr; g->h_bad = (mgc_host_alloc(64, &hp) == MGC_OK) ? (int*)hp : nullptr; }
-    if (const char* s1 = getenv("MEDPY_GC_SWEEPS")) g->sweeps_per_round = atoi(s1) > 0 ? atoi(s1) : g->sweeps_per_round;
     if (const char* s2 = getenv("MEDPY_GC_RELAX_BATCH")) g->relax_batch = atoi(s2) > 0 ? atoi(s2) : g->relax_batch;
     g->st.n_voxels = (int64_t)n;
     rc = mgc_reset(g);
@@ -910,13 +906,13 @@ double caps_resolve(mgc_graph* g)
     return total;
 }
 
+// ---- per-voxel solver (gc_solver.cuh): 4-D z-slabs only --------------------------------------------------
 int ensure_state(mgc_graph* g)
 {
     if (g->state_init) return MGC_OK;
     { int rc0 = materialise_zeros(g); if (rc0) return rc0; }
     { int rc0 = push_state_all(g); if (rc0) return rc0; }
-    if (g->nd == 3) k_init_state<3, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
-    else            k_init_state<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
+    k_init_state<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
     g->st.kernel_launches++;
     CK(cudaGetLastError());
     g->state_init = true;
@@ -925,8 +921,7 @@ int ensure_state(mgc_graph* g)
 
 int relabel_init(mgc_graph* g)
 {
-    if (g->nd == 3) k_relabel_init<3, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
-    else            k_relabel_init<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
+    k_relabel_init<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
     g->st.kernel_launches++;
     CK(cudaGetLastError());
     return MGC_OK;
@@ -939,10 +934,8 @@ int relabel_relax(mgc_graph* g, int* any)
     for (;;) {
         CK(cudaMemsetAsync(g->d_flags + 1, 0, sizeof(int), g->stream));
         cudaEventRecord(g->ev[2], g->stream);
-        for (int i = 0; i < g->relax_batch; ++i) {
-            if (g->nd == 3) k_relabel_relax<3><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S.rmask, g->S.height, g->d_flags + 1);
-            else            k_relabel_relax<4><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S.rmask, g->S.height, g->d_flags + 1);
-        }
+        for (int i = 0; i < g->relax_batch; ++i)
+            k_relabel_relax<4><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S.rmask, g->S.height, g->d_flags + 1);
         g->st.kernel_launches += g->relax_batch;
         g->st.relabel_sweeps += g->relax_batch;
         cudaEventRecord(g->ev[3], g->stream);
@@ -969,27 +962,14 @@ int count_active(mgc_graph* g, int64_t* out)
     return MGC_OK;
 }
 
-// n push sweeps; *work_last = whether the last sweep still found an active voxel
-int push_sweeps(mgc_graph* g, int n, int* work_last)
+// n push sweeps (k_push raises the work flag d_flags[2]; nobody reads it here)
+int push_sweeps(mgc_graph* g, int n)
 {
     g->flow_started = true;
-    if (work_last) cudaEventRecord(g->ev[2], g->stream);
-    for (int i = 0; i < n; ++i) {
-        if (i == n - 1) CK(cudaMemsetAsync(g->d_flags + 2, 0, sizeof(int), g->stream));
-        if (g->nd == 3) k_push<3, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->d_flags + 2);
-        else            k_push<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->d_flags + 2);
-    }
+    for (int i = 0; i < n; ++i) k_push<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->d_flags + 2);
     g->st.kernel_launches += n;
     g->st.push_sweeps += n;
     CK(cudaGetLastError());
-    if (work_last) {
-        cudaEventRecord(g->ev[3], g->stream);
-        CK(cudaMemcpyAsync(work_last, g->d_flags + 2, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
-        CK(cudaStreamSynchronize(g->stream));
-        float ms = 0;
-        cudaEventElapsedTime(&ms, g->ev[2], g->ev[3]);
-        g->st.ms_push += ms;
-    }
     return MGC_OK;
 }
 
@@ -1016,7 +996,7 @@ int dirty_clear(mgc_graph* g)
 }
 
 // MGC_OPT_WARM applies: a tile-solver handle of one GPU whose state does not come from the lazy fused build
-bool warm_wanted(const mgc_graph* g) { return g->warm_opt && g->use_tiles && !g->slab && !g->lazy_built; }
+bool warm_wanted(const mgc_graph* g) { return g->warm_opt && !g->slab && !g->lazy_built; }
 
 // first call: solver state + first labels + first worklists in one pass (k_init_tile)
 int init_tiles(mgc_graph* g)
@@ -1045,7 +1025,6 @@ int init_tiles(mgc_graph* g)
     CK(cudaGetLastError());
     g->state_init = true;
     g->labels_fresh = true;
-    g->rl_cur = 0;
     g->sweep_mode = -1;
     if (warm) {
         g->warm_state = true;
@@ -1085,7 +1064,6 @@ int relabel_tiles_begin(mgc_graph* g)
 {
     if (g->labels_fresh) {
         g->labels_fresh = false;
-        g->rl_cur = 0;
         CK(cudaMemsetAsync(g->d_tcount + CTL_RLCUR, 0, sizeof(int), g->stream));
         return MGC_OK;
     }
@@ -1108,7 +1086,6 @@ int relabel_tiles_begin(mgc_graph* g)
         }
     }
     g->st.kernel_launches++;
-    g->rl_cur = 0;
     CK(cudaMemsetAsync(g->d_tcount + CTL_RLCUR, 0, sizeof(int), g->stream));
     CK(cudaGetLastError());
     return MGC_OK;
@@ -1145,7 +1122,6 @@ int relabel_sweep_round(mgc_graph* g, int* pending, bool with_check)
     if (g->nd == 4) k_relabel_check4<<<nblocks(g), 256, 0, g->stream>>>(g->L, g->TL4, g->S.rmask, g->S.height, g->rflag, rl(g, 0));
     else            k_relabel_check<<<nblocks(g), 256, 0, g->stream>>>(g->L, g->TL, g->S.rmask, g->S.height, g->rflag, rl(g, 0));
     g->st.kernel_launches++;
-    g->rl_cur = 0;
     CK(cudaMemsetAsync(g->d_tcount + CTL_RLCUR, 0, sizeof(int), g->stream));
     CK(cudaGetLastError());
     return read_tcount(g, 0, pending);
@@ -1158,9 +1134,9 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true, bool first =
     *any = 0;
     g->relp_last = 0;
     g->relp_pending = false;
-    if (g->use_sweeps && g->use_tiles && g->TL.ntiles >= 64 && g->sweep_mode != 0) {
+    if (g->use_sweeps && g->TL.ntiles >= 64 && g->sweep_mode != 0) {
         int pending = 0;
-        int rc = read_tcount(g, g->rl_cur, &pending);
+        int rc = read_tcount(g, 0, &pending);
         if (rc) return rc;
         // one decision per solve (one host synchronisation): an instance whose first relabel has to label most of the
         // lattice is a hard one at every later relabel too, an easy one (regional term: most voxels own a sink link) never is
@@ -1185,55 +1161,29 @@ int relabel_tiles_run(mgc_graph* g, int* any, bool want_any = true, bool first =
     const bool capped = first && g->first_cap >= 2 && g->sweep_mode == 0 && g->nd == 3 && !g->slab;
     int cap = capped ? g->first_cap : MGC_HINF;
     g->labels_capped = capped;
-    if (g->coop_bfs_grid > 0 && g->use_tiles) {
-        // all passes in one cooperative launch; the list selector lives in the control block (device side), so the
-        // host does not have to synchronise unless the caller wants to know whether anything moved
-        CK(cudaMemsetAsync(g->d_tcount + CTL_CURSOR, 0, sizeof(int), g->stream));
-        int* it0 = g->rl_items[0]; int* it1 = g->rl_items[1];
-        if (g->nd == 4) {
-            void* args4[] = {&g->L, &g->TL4, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount};
-            CK(cudaLaunchCooperativeKernel((void*)k_bfs_coop4, dim3(g->coop_bfs_grid), dim3(T4_VOX), args4, 0, g->stream));
-        } else {
-            void* args[] = {&g->L, &g->TL, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount, &cap};
-            CK(cudaLaunchCooperativeKernel((void*)k_bfs_coop, dim3(g->coop_bfs_grid), dim3(TILE_VOX), args, 0, g->stream));
-        }
-        g->st.kernel_launches++;
-        g->st.relabel_sweeps++;     // passes are counted on the device (ctl[CTL_RELP]); one launch here
-        if (want_any) {
-            int relp = 0;
-            CK(cudaMemcpyAsync(&relp, g->d_tcount + CTL_RELP, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
-            CK(cudaStreamSynchronize(g->stream));
-            if (relp != 0) *any = 1;
-            g->relp_last = relp;
-            g->st.relabel_passes += relp;
-        } else {
-            g->relp_pending = true;     // read back by relabel_passes_fetch / _collect
-        }
-        return MGC_OK;
+    // all passes in one cooperative launch; the list selector lives in the control block (device side), so the
+    // host does not have to synchronise unless the caller wants to know whether anything moved
+    CK(cudaMemsetAsync(g->d_tcount + CTL_CURSOR, 0, sizeof(int), g->stream));
+    int* it0 = g->rl_items[0]; int* it1 = g->rl_items[1];
+    if (g->nd == 4) {
+        void* args4[] = {&g->L, &g->TL4, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount};
+        CK(cudaLaunchCooperativeKernel((void*)k_bfs_coop4, dim3(g->coop_bfs_grid), dim3(T4_VOX), args4, 0, g->stream));
+    } else {
+        void* args[] = {&g->L, &g->TL, &g->S.rmask, &g->S.height, &g->rflag, &it0, &it1, &g->d_tcount, &cap};
+        CK(cudaLaunchCooperativeKernel((void*)k_bfs_coop, dim3(g->coop_bfs_grid), dim3(TILE_VOX), args, 0, g->stream));
     }
-    for (;;) {
-        const int cur = g->rl_cur;
-        int pending = 0;
-        int rc = read_tcount(g, cur, &pending);
-        if (rc) return rc;
-        if (!pending) break;
-        *any = 1;
-        CK(cudaMemsetAsync(g->d_tcount + (1 - cur), 0, sizeof(int), g->stream));
-        CK(cudaMemsetAsync(cursor(g), 0, sizeof(int), g->stream));
-        const int grid = pending < g->n_ctas * 2 ? pending : g->n_ctas * 2;   // 4 KB smem: more CTAs per SM fit
-        if (g->nd == 4)
-            k_relabel_tile4<<<grid, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S.rmask, g->S.height, g->rflag, rl(g, cur),
-                                                            cursor(g), rl(g, 1 - cur));
-        else
-        k_relabel_tile<<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S.rmask, g->S.height, g->rflag, rl(g, cur),
-                                                         cursor(g), rl(g, 1 - cur), cap);
-        g->rl_cur = 1 - cur;
-        g->st.kernel_launches++;
-        g->st.relabel_sweeps++;
-        g->st.relabel_passes++;
-        g->relp_last++;
+    g->st.kernel_launches++;
+    g->st.relabel_sweeps++;     // passes are counted on the device (ctl[CTL_RELP]); one launch here
+    if (want_any) {
+        int relp = 0;
+        CK(cudaMemcpyAsync(&relp, g->d_tcount + CTL_RELP, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
+        CK(cudaStreamSynchronize(g->stream));
+        if (relp != 0) *any = 1;
+        g->relp_last = relp;
+        g->st.relabel_passes += relp;
+    } else {
+        g->relp_pending = true;     // read back by relabel_passes_fetch / _collect
     }
-    CK(cudaGetLastError());
     return MGC_OK;
 }
 
@@ -1379,13 +1329,8 @@ int debug_invariants(mgc_graph* g, bool after)
     { int rc0 = push_state_all(g); if (rc0) return rc0; }
     double* d = g->d_scalars + 4;        // [4] excess, [5] absorbed, [6] violations
     CK(cudaMemsetAsync(d, 0, 3 * sizeof(double), g->stream));
-    const bool tiles3 = g->use_tiles && g->nd == 3;
-    if (g->nd == 3) {
-        if (tiles3) k_debug_invariants<3, double, true><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, d);
-        else        k_debug_invariants<3, double, false><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, d);
-    } else {
-        k_debug_invariants<4, double, false><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, d);
-    }
+    if (g->nd == 3) k_debug_invariants<3, double, true><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, d);
+    else            k_debug_invariants<4, double, false><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, d);
     double h[3] = {0, 0, 0};
     CK(cudaMemcpyAsync(h, d, sizeof(h), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
@@ -1495,11 +1440,11 @@ int readout(mgc_graph* g, double* energy_part)
 {
     Nvtx range("mgc:readout");
     // clean tiles hold the reset labels while no sweep has lowered labels unmarked (the partial reset relies on the same)
-    const bool clean = g->use_tiles && g->nd == 3 && !g->slab && g->TL.dflag && g->sweep_mode != 1 && g->L.dim[2] % 4 == 0;
+    const bool clean = g->nd == 3 && !g->slab && g->TL.dflag && g->sweep_mode != 1 && g->L.dim[2] % 4 == 0;
     if (clean) k_readout<double, true, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials, g->TL.dflag,
                                                                                 g->TL.nt[1], g->TL.nt[2]);
-    else if (g->use_tiles && g->nd == 3) k_readout<double, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
-    else                            k_readout<double, false><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
+    else if (g->nd == 3) k_readout<double, true><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
+    else                 k_readout<double, false><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->mask_dev, g->partials);
     CK(cudaMemsetAsync(g->d_scalars + 1, 0, sizeof(double), g->stream));
     k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, rblocks(g), g->d_scalars + 1);
     g->st.kernel_launches += 2;
@@ -1508,7 +1453,7 @@ int readout(mgc_graph* g, double* energy_part)
     int win[2] = {0, 0};             // WIN_DEFERRED, WIN_DROPPED of this solve
     CK(cudaMemcpyAsync(sc, g->d_scalars, sizeof(sc), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaMemcpyAsync(&n_mat, g->d_flags + 3, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
-    if (g->win_ctl && g->use_tiles) CK(cudaMemcpyAsync(win, g->win_ctl + WIN_DEFERRED, sizeof(win), cudaMemcpyDeviceToHost, g->stream));
+    if (g->win_ctl) CK(cudaMemcpyAsync(win, g->win_ctl + WIN_DEFERRED, sizeof(win), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
     g->st.flow_const = sc[0];
     g->st.tiles_materialised = n_mat;
@@ -1769,7 +1714,7 @@ bool c_contiguous(const mgc_graph* g, const mgc_array* a)
     return true;
 }
 
-bool can_fuse(const mgc_graph* g) { return g->use_tiles && g->nd == 3 && g->fuse_build; }
+bool can_fuse(const mgc_graph* g) { return g->nd == 3 && g->fuse_build; }
 // lazy capacities need the per-tile worklists of one whole lattice: no z-slabs
 bool can_lazy(const mgc_graph* g) { return can_fuse(g) && !g->slab && g->lazy_caps && g->cmat; }
 
@@ -2347,7 +2292,6 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     g->solved = false;
     g->host_mask_valid = false;
     g->labels_fresh = true;
-    g->rl_cur = 0;
     g->sweep_mode = -1;
     g->init_timed = false;
     g->st.ms_init = 0.0;
@@ -2411,47 +2355,16 @@ int mgc_maxflow(mgc_graph* g, double* energy)
     resolve_term_span(g);
     {
         Timer t(g, &g->st.ms_solve);
-        int rc = MGC_OK;
-        if (g->use_tiles) {
-            rc = warm_prepare(g); if (rc) return rc;
-            if (g->debug_checks) {
-                rc = materialise_zeros(g); if (rc) return rc;
-                if (!g->state_init) { rc = init_tiles(g); if (rc) return rc; }
-                rc = debug_invariants(g, false); if (rc) return rc;
-            }
-            rc = solve_tiles(g);
-            if (rc) return rc;
-            rc = debug_invariants(g, true);
-            if (rc) return rc;
-        } else {
-        rc = ensure_state(g);
+        int rc = warm_prepare(g); if (rc) return rc;
+        if (g->debug_checks) {
+            rc = materialise_zeros(g); if (rc) return rc;
+            if (!g->state_init) { rc = init_tiles(g); if (rc) return rc; }
+            rc = debug_invariants(g, false); if (rc) return rc;
+        }
+        rc = solve_tiles(g);
         if (rc) return rc;
-        int64_t rounds = 0;
-        for (;;) {
-            rc = relabel_init(g);
-            if (rc) return rc;
-            int any = 0;
-            rc = relabel_relax(g, &any);
-            if (rc) return rc;
-            g->st.global_relabels++;
-            int64_t active = 0;
-            rc = count_active(g, &active);
-            if (rc) return rc;
-            if (active == 0) break;
-            if (++rounds > g->max_rounds) FAIL(MGC_E_NOCONV, "push-relabel did not converge within the round cap");
-            // push sweeps until quiescent or the round budget is used
-            int done = 0;
-            while (done < g->sweeps_per_round) {
-                int chunk = g->sweeps_per_round - done;
-                if (chunk > 8) chunk = 8;
-                int work = 1;
-                rc = push_sweeps(g, chunk, &work);
-                if (rc) return rc;
-                done += chunk;
-                if (!work) break;
-            }
-        }
-        }
+        rc = debug_invariants(g, true);
+        if (rc) return rc;
         t.stop_sync();
     }
     {
@@ -2547,7 +2460,7 @@ static int fold_cub_launches(mgc_graph* g, int sort, int n, int end_bit, void* t
 static int warm_check(mgc_graph* g, bool* eager)
 {
     *eager = false;
-    if (!g->slab && g->use_tiles && g->lazy_built && g->state_init && g->nd == 3) return MGC_OK;
+    if (!g->slab && g->lazy_built && g->state_init && g->nd == 3) return MGC_OK;
     if (warm_wanted(g)) { *eager = true; return MGC_OK; }
     FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
                       "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
@@ -2625,7 +2538,6 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
         g->st.ms_caps -= caps_resolve(g);          // the claim is part of ms_seeds, not of the solve's materialisation
     }
     g->labels_fresh = false;
-    g->rl_cur = 0;
     g->sweep_mode = -1;
     g->solved = false;
     g->host_mask_valid = false;
@@ -3011,7 +2923,7 @@ int mgc_get_trcap(mgc_graph* g, int64_t node, double* trcap)
     uint8_t rm = 0x80u;
     CK(cudaMemcpyAsync(&e, g->S.excess + node, sizeof(double), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaMemcpyAsync(&s, g->S.sink + node, sizeof(double), cudaMemcpyDeviceToHost, g->stream));
-    if (g->use_tiles && g->nd == 3) CK(cudaMemcpyAsync(&rm, g->S.rmask + node, 1, cudaMemcpyDeviceToHost, g->stream));
+    if (g->nd == 3) CK(cudaMemcpyAsync(&rm, g->S.rmask + node, 1, cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
     if (!(rm & 0x80u)) s = 0;        // RM_SINKV clear: nothing absorbed yet, the entry was never written
     double tr = 0;
@@ -3077,7 +2989,7 @@ int mgc_slab_push(mgc_graph* g, int32_t n)
     CK(cudaSetDevice(g->device));
     g->iters_now = g->tile_iters;
     if (g->use_tiles) return push_tiles(g, n);
-    return push_sweeps(g, n, nullptr);
+    return push_sweeps(g, n);
 }
 
 int mgc_slab_pack(mgc_graph* g, int32_t* h_lo, double* f_lo, int32_t* h_hi, double* f_hi)
@@ -3117,8 +3029,8 @@ int mgc_slab_unpack(mgc_graph* g, const int32_t* h_lo, const double* f_lo, const
         const double* fin = side == 0 ? f_lo : f_hi;
         if (g->use_tiles) {
             k_slab_unpack_tiles<double><<<nb, 256, 0, g->stream>>>(g->L, g->TL, g->S, zg, zb, k, hin, fin, g->rflag, rl(g, 0), rl(g, 1),
-                                                                  g->coop_bfs_grid > 0 ? g->d_tcount + CTL_RLCUR : nullptr, g->rl_cur,
-                                                                  g->pflag, pl(g, 0, g->pl_sel[0]), pl(g, 1, g->pl_sel[1]), changed_dev);
+                                                                  g->d_tcount + CTL_RLCUR, g->pflag, pl(g, 0, g->pl_sel[0]),
+                                                                  pl(g, 1, g->pl_sel[1]), changed_dev);
         } else {
             const size_t border = (size_t)zb * P, ghost = (size_t)zg * P;
             k_slab_unpack<double><<<nb, 256, 0, g->stream>>>(P, g->S.height + ghost, g->S.excess + border, g->S.cap[k] + border,

@@ -1,10 +1,10 @@
 // gc_persist.cuh -- the global relabel (worklist BFS) as ONE cooperative launch.
 //
-// The host-driven BFS of gc_api.cu needs a device->host round trip per pass to learn whether the next worklist is
-// empty; on hard instances (hundreds of short passes) those round trips dominate.  k_bfs_coop (3-D) and k_bfs_coop4
-// (4-D) run all passes inside a single persistent cooperative kernel, separating them with grid-wide barriers; the
-// list counts, the cursor and the list selector live in device memory.  The passes call the very same tile bodies as
-// the stand-alone kernels (gc_tiles.cuh, gc_tiles4.cuh).
+// A BFS driven from the host would need a device->host round trip per pass to learn whether the next worklist is
+// empty; on hard instances (hundreds of short passes) those round trips would dominate.  k_bfs_coop (3-D) and
+// k_bfs_coop4 (4-D) run all passes inside a single persistent cooperative kernel, separating them with grid-wide
+// barriers; the list counts, the cursor and the list selector live in device memory.  A pass visits its tiles with
+// relabel_visit (gc_tiles.cuh) / relabel_visit4 (gc_tiles4.cuh).
 #pragma once
 #include <cooperative_groups.h>
 #include "gc_tiles.cuh"
@@ -25,8 +25,7 @@ __device__ __forceinline__ int ld_ctl(const int* ctl, int i) { return *(const vo
 // global relabel as one cooperative launch: all passes of the BFS with grid-wide barriers between them
 // (`cap`: see relabel_visit; MGC_HINF = exact).
 // The relabel visit needs 28 registers and 4 KB of shared memory, so 4 CTAs per SM are co-resident -- twice the
-// parallelism of the push kernel -- while the per-pass host round trip
-// (count read-back, two memsets, launch) of the list-driven host loop disappears.
+// parallelism of the push kernel -- and no pass costs a host round trip (count read-back, two memsets, launch).
 // (A queue-driven asynchronous variant without barriers was tried and rejected: label-correcting order made tiles
 //  converge to non-final labels over and over -- 50x more visits at 512^3.)
 // ---------------------------------------------------------------------------------------------------
@@ -58,8 +57,8 @@ k_bfs_coop(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask, int* __restri
     if (leader) { ctl[CTL_RLCUR] = rl_cur; ctl[CTL_RELP] = n_rel; }
 }
 
-// the same for 4-D lattices (4 x 4 x 8 x 4 tiles): replaces one launch + one host round trip PER PASS (r02 config 4:
-// ~160 passes per solve) by grid barriers inside one cooperative launch
+// the same for 4-D lattices (4 x 4 x 8 x 4 tiles): grid barriers inside one cooperative launch instead of one launch +
+// one host round trip per pass (r02 config 4: ~160 passes per solve)
 __global__ void __launch_bounds__(T4_VOX, 3)
 k_bfs_coop4(Lattice L, Tiles4 TL, const uint8_t* __restrict__ rmask, int* __restrict__ height, int* __restrict__ rflag,
             int* __restrict__ items0, int* __restrict__ items1, int* __restrict__ ctl)

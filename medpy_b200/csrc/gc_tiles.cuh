@@ -1,5 +1,5 @@
-// gc_tiles.cuh -- tile-resident solver kernels for the 3-D lattice (the production path; gc_solver.cuh keeps
-// the per-voxel kernels used for 4-D lattices, z-slabs and as an A/B reference).
+// gc_tiles.cuh -- tile-resident solver kernels for the 3-D lattice (gc_tiles4.cuh holds the 4-D ones;
+// gc_solver.cuh keeps the per-voxel kernels, which only 4-D z-slabs run).
 //
 // The lattice is cut into 8x8x8 tiles.  A 512-thread CTA owns one tile for the duration of a visit, keeps the
 // tile's state on chip (heights with a 1-voxel halo in shared memory; in the push kernel the six residual
@@ -12,7 +12,8 @@
 //  * k_init_tile          : solver state from the terms (source-excess clamp, residual mask, first labels) and
 //                           the first worklists, fused in one pass over the lattice.
 //  * k_relabel_reset      : start of a later global relabel: labels from the residual mask, new worklist.
-//  * k_relabel_tile       : exact backward BFS from the sink (global relabel).  Labels only decrease during it,
+//  * relabel_visit        : exact backward BFS from the sink (global relabel), one tile visit; k_bfs_coop
+//                           (gc_persist.cuh) runs every pass in one cooperative launch.  Labels only decrease during it,
 //                           so tiles run concurrently with benign races on the halo; a tile whose border labels
 //                           dropped lists its face neighbours for the next pass.
 //  * k_push_tile          : push/relabel discharge of one tile: synchronous rounds, "push then pull" through a
@@ -260,7 +261,7 @@ __global__ void __launch_bounds__(TILE_VOX) k_relabel_reset_list(Lattice L, Tile
 }
 
 // ---------------------------------------------------------------------------------------------------
-// global relabel pass: persistent CTAs over the current worklist
+// global relabel: one tile visit (k_bfs_coop of gc_persist.cuh runs the passes over the worklists)
 // ---------------------------------------------------------------------------------------------------
 // one tile visit of the global relabel: relax inside the tile until nothing changes, write back, list the face
 // neighbours whose halo changed.  `sh` = HALO_VOX ints of shared memory.
@@ -310,19 +311,6 @@ __device__ __forceinline__ void relabel_visit(const Lattice& L, const Tiles& TL,
     if (TL.dflag) {                          // labels of this tile changed: it has to be reset before the next BFS
         const int chg = __syncthreads_or(h != h0 ? 1 : 0);
         if (chg && threadIdx.x == 0) mark_dirty(TL, t);
-    }
-}
-
-__global__ void __launch_bounds__(TILE_VOX) k_relabel_tile(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask,
-                                                           int* __restrict__ height, int* __restrict__ rflag,
-                                                           WorkList cur, int* __restrict__ cursor, WorkList next, int cap)
-{
-    __shared__ int sh[HALO_VOX];
-    __shared__ int s_slot;
-    for (;;) {
-        const int t = fetch_tile(cur, cursor, &s_slot);
-        if (t < 0) break;
-        relabel_visit(L, TL, rmask, height, rflag, next, t, sh, cap);
     }
 }
 
@@ -498,15 +486,13 @@ __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, 
 template <typename T>
 __global__ void k_slab_unpack_tiles(Lattice L, Tiles TL, State<T> S, int z_ghost, int z_border, int k_border_to_ghost,
                                     const int* __restrict__ h_in, const double* __restrict__ f_in,
-                                    int* __restrict__ rflag, WorkList rl0, WorkList rl1, const int* __restrict__ rl_cur_dev,
-                                    int rl_cur_host, int* __restrict__ pflag, WorkList pl0, WorkList pl1,
-                                    int* __restrict__ changed)
+                                    int* __restrict__ rflag, WorkList rl0, WorkList rl1, const int* __restrict__ rl_cur,
+                                    int* __restrict__ pflag, WorkList pl0, WorkList pl1, int* __restrict__ changed)
 {
     const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= L.plane) return;
-    // the relabel list consumed next: device-resident selector when the BFS runs as a cooperative kernel
-    const int rc = rl_cur_dev ? *rl_cur_dev : rl_cur_host;
-    const WorkList rl = rc ? rl1 : rl0;
+    // the relabel list consumed next: the cooperative BFS keeps its selector in the control block
+    const WorkList rl = *rl_cur ? rl1 : rl0;
     const int y = (int)(i / L.stride[1]), x = (int)(i % L.stride[1]);
     const unsigned vg = (unsigned)z_ghost * L.plane + i, vb = (unsigned)z_border * L.plane + i;
     const int tg = ((z_ghost / TILE) * TL.nt[1] + y / TILE) * TL.nt[2] + x / TILE;

@@ -164,7 +164,7 @@ __global__ void __launch_bounds__(T4_VOX) k_relabel_reset4(Lattice L, Tiles4 TL,
 }
 
 // ---------------------------------------------------------------------------------------------------
-// global relabel pass (cf. k_relabel_tile)
+// global relabel: one tile visit (k_bfs_coop4 of gc_persist.cuh runs the passes over the worklists)
 // ---------------------------------------------------------------------------------------------------
 // one tile visit of the 4-D global relabel (cf. relabel_visit): relax inside the tile until nothing changes, write back,
 // list the face neighbours whose halo changed.  `sh` = H4_VOX ints of shared memory.
@@ -202,19 +202,6 @@ __device__ __forceinline__ void relabel_visit4(const Lattice& L, const Tiles4& T
             // only if my new label can lower the voxel across the face (see relabel_visit)
             if (edge && sh[me + ((k & 1) ? t4_hoff(ax) : -t4_hoff(ax))] > h + 1) list_push(rflag, next, tile4_nbr(TL, t, k));
         }
-    }
-}
-
-__global__ void __launch_bounds__(T4_VOX) k_relabel_tile4(Lattice L, Tiles4 TL, const uint8_t* __restrict__ rmask,
-                                                          int* __restrict__ height, int* __restrict__ rflag,
-                                                          WorkList cur, int* __restrict__ cursor, WorkList next)
-{
-    __shared__ int sh[H4_VOX];
-    __shared__ int s_slot;
-    for (;;) {
-        const int t = fetch_tile(cur, cursor, &s_slot);
-        if (t < 0) break;
-        relabel_visit4(L, TL, rmask, height, rflag, next, t, sh);
     }
 }
 

@@ -135,8 +135,7 @@ class GraphDouble:
         ``g = graph_from_voxels(...); g.enable_warm(); g.maxflow()`` is the order.  The first solve then records the residual
         source capacities the folds read (``mgc_set_option(MGC_OPT_WARM)``); its mask and energy are those without the
         call.  The setting survives ``reset()``.  On a graph the lazy fused build made it changes nothing.  A solved graph
-        that cannot fold raises ``RuntimeError``, a sparse graph ``TypeError``; the per-voxel solver
-        (``MEDPY_GC_SOLVER=v0``) still refuses the folds."""
+        that cannot fold raises ``RuntimeError``, a sparse graph ``TypeError``."""
         if self._sp is not None:
             raise TypeError("enable_warm() needs a lattice graph: a general sparse graph has no warm re-solve")
         if self._native is not None:

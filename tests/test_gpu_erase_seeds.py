@@ -257,7 +257,7 @@ def test_out_of_range_ids_leave_the_result():
     assert g.stats()["seed_folds"] == 1
 
 
-@pytest.mark.parametrize("case", ["eager", "4d", "per_term", "v0"])
+@pytest.mark.parametrize("case", ["eager", "4d", "per_term"])
 def test_handles_without_warm_path_refuse(case):
     import medpy_b200.graphcut as gc
     from medpy_b200.graphcut.maxflow import GraphDouble
@@ -265,8 +265,6 @@ def test_handles_without_warm_path_refuse(case):
     shape = (12, 12, 16)
     if case == "eager":
         env = dict(MEDPY_GC_LAZY_CAPS=0)
-    if case == "v0":
-        env = dict(MEDPY_GC_SOLVER="v0")
     with _env(**env):
         if case == "4d":
             vol = _volume((6, 8, 8, 3), seed=1, dtype="float32")

@@ -1,12 +1,12 @@
-"""Differential matrix of the 4-D solvers: every lattice_cases4 instance under every solver option that changes how a 4-D
-instance is relabelled (classification, sweeps, sweep rounds, host-driven or cooperative BFS), how long a tile visit
-runs, or which solver runs (the 4 x 4 x 8 x 4 tile solver of gc_tiles4.cuh or the per-voxel one of gc_solver.cuh).  Each
-cell must give BK's mask (bit for bit on integer instances; a float mismatch only with an exact-tie certificate), BK's
-energy (exactly on integer instances), an energy equal to the exact capacity of its own cut and an ended solve.
+"""Differential matrix of the 4-D tile solver (the 4 x 4 x 8 x 4 tiles of gc_tiles4.cuh): every lattice_cases4 instance
+under every solver option that changes how a 4-D instance is relabelled (classification, sweeps, sweep rounds) or how
+long a tile visit runs.  Each cell must give BK's mask (bit for bit on integer instances; a float mismatch only with an
+exact-tie certificate), BK's energy (exactly on integer instances), an energy equal to the exact capacity of its own cut
+and an ended solve.
 
-Where the tile solver runs its cooperative BFS, the statistics also show which relabel ran: every relabel adds 1 to
-`global_relabels` and 1 to `relabel_sweeps` for its BFS launch, and each directional sweep round adds 1 more to
-`relabel_sweeps`.  Sweeps run on instances of at least 64 tiles that are hard, by default or forced."""
+The statistics also show which relabel ran: every relabel adds 1 to `global_relabels` and 1 to `relabel_sweeps` for its
+cooperative BFS launch, and each directional sweep round adds 1 more to `relabel_sweeps`.  Sweeps run on instances of at
+least 64 tiles that are hard, by default or forced."""
 import pytest
 
 import lattice_cases as lc
@@ -22,9 +22,7 @@ OPTIONS = {
     "hard": dict(MEDPY_GC_SWEEP_FRAC=1000000),
     "sweep_off": dict(MEDPY_GC_SWEEP=0),
     "sweep_rounds": dict(MEDPY_GC_SWEEP_FRAC=1000000, MEDPY_GC_SWEEP_MIN_ROUNDS=3, MEDPY_GC_SWEEP_ROUNDS=4),
-    "bfs_host": dict(MEDPY_GC_BFS="host"),
     "iters1": dict(MEDPY_GC_ITERS=1, MEDPY_GC_PASSES_MAX=1),
-    "v0": dict(MEDPY_GC_SOLVER="v0"),
     "debug": dict(MEDPY_GC_DEBUG=1),
 }
 
@@ -69,19 +67,8 @@ def test_cell_matches_bk(name, opt):
     _assert_energy(case, e, lc.cut_capacity(case["prob"], m))
     assert st["active_last"] == 0, st
 
-    if opt == "v0":
-        # the per-voxel solver relaxes labels in batches of launches and runs no tile BFS pass
-        assert st["relabel_passes"] == 0 and st["relabel_sweeps"] > 0, st
-        return
     if not _sweeps_expected(case, opt):
         assert st["relabel_passes"] > 0, st     # where sweeps run they may leave the BFS nothing to do
-    if opt == "bfs_host":
-        # one launch per BFS pass, plus one per sweep round
-        if _sweeps_expected(case, opt):
-            assert st["relabel_sweeps"] > st["relabel_passes"], st
-        else:
-            assert st["relabel_sweeps"] == st["relabel_passes"], st
-        return
     if _sweeps_expected(case, opt):
         assert st["relabel_sweeps"] > st["global_relabels"], st
     else:

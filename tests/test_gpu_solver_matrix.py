@@ -22,7 +22,6 @@ OPTIONS = {
     "full_reset": dict(MEDPY_GC_PARTIAL_RESET=0),
     "eager": dict(MEDPY_GC_LAZY_CAPS=0),
     "no_tma": dict(MEDPY_GC_TMA=0),
-    "bfs_host": dict(MEDPY_GC_BFS="host"),
     "iters1": dict(MEDPY_GC_ITERS=1, MEDPY_GC_PASSES_MAX=1),
     "easy": dict(MEDPY_GC_SWEEP_FRAC=1),
     "hard": dict(MEDPY_GC_SWEEP_FRAC=1000000),
@@ -150,7 +149,7 @@ def test_cell_matches_bk(name, opt):
 
 # --------------------------------------------------------------------------------------------------------- warm seeds
 WARM_CASES = ["a1-ladder-s0", "a1-ladder-s2", "a2-serp-w3"]
-WARM_OPTIONS = ["default", "first_cap2", "full_reset", "no_tma", "bfs_host", "iters1"]
+WARM_OPTIONS = ["default", "first_cap2", "full_reset", "no_tma", "iters1"]
 
 
 def _steps(case):

@@ -220,16 +220,6 @@ def test_option_survives_reset_and_rebuild():
         assert numpy.array_equal(m, om) and abs(e - oe) <= 1e-9 * max(abs(oe), scale)
 
 
-def test_v0_still_refuses():
-    vol = _volume((12, 12, 16), seed=1, dtype="float32")
-    with _env(MEDPY_GC_SOLVER="v0"):
-        g = _graph(vol, _KIND, True, False)
-        g.enable_warm()
-        g.maxflow()
-        with pytest.raises(RuntimeError, match="reset"):
-            g.add_tweights_warm(numpy.array([3], numpy.int64), 1.0, 0.0)
-
-
 def test_bad_ids_and_nan_leave_the_4d_result():
     shape = (9, 5, 17, 3)
     n = int(numpy.prod(shape))

@@ -366,11 +366,11 @@ def test_bad_calls_leave_the_result():
     assert numpy.array_equal(m2, om) and abs(e2 - oe) <= 1e-9 * max(abs(oe), scale)
 
 
-@pytest.mark.parametrize("case", ["eager", "4d", "per_term", "v0", "sparse"])
+@pytest.mark.parametrize("case", ["eager", "4d", "per_term", "sparse"])
 def test_handles_without_warm_path_refuse(case):
     import medpy_b200.graphcut as gc
     from medpy_b200.graphcut.maxflow import GraphDouble
-    env = dict(eager=dict(MEDPY_GC_LAZY_CAPS=0), v0=dict(MEDPY_GC_SOLVER="v0")).get(case, {})
+    env = dict(eager=dict(MEDPY_GC_LAZY_CAPS=0)).get(case, {})
     shape = (12, 12, 16)
     with _env(**env):
         if case == "sparse":
@@ -393,8 +393,6 @@ def test_handles_without_warm_path_refuse(case):
         else:
             vol = _volume(shape, seed=1, dtype="float32")
             g = _graph(vol, _KIND, True, False)
-            if case == "v0":
-                g.enable_warm()
         g.maxflow()
         with pytest.raises(RuntimeError, match="reset"):
             g.add_nweights_warm([3], [4], 1.0, 0.0)

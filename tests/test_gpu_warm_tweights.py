@@ -293,7 +293,7 @@ def test_bad_ids_and_nan_leave_the_result():
     assert g.stats()["seed_folds"] == 1
 
 
-@pytest.mark.parametrize("case", ["eager", "4d", "per_term", "v0", "sparse"])
+@pytest.mark.parametrize("case", ["eager", "4d", "per_term", "sparse"])
 def test_handles_without_warm_path_refuse(case):
     import medpy_b200.graphcut as gc
     from medpy_b200.graphcut.maxflow import GraphDouble
@@ -301,8 +301,6 @@ def test_handles_without_warm_path_refuse(case):
     shape = (12, 12, 16)
     if case == "eager":
         env = dict(MEDPY_GC_LAZY_CAPS=0)
-    if case == "v0":
-        env = dict(MEDPY_GC_SOLVER="v0")
     with _env(**env):
         if case == "sparse":
             g = GraphDouble(4, 4, sparse=True)

@@ -24,7 +24,7 @@ t2 = time.time()
 diff = (m != omask)
 out = dict(shape=list(shape), gpu_energy=e, bk_energy=oflow, rel_err=abs(e - oflow) / abs(oflow), mask_hamming=int(diff.sum()),
            gpu_fg=int(m.sum()), bk_fg=int(omask.sum()), bk_terms_s=t1 - t0, bk_setup_s=tm["setup_s"], bk_maxflow_s=tm["maxflow_s"],
-           gpu_solve_ms=st["ms_solve"], solver=os.environ.get("MEDPY_GC_SOLVER", "tiles"))
+           gpu_solve_ms=st["ms_solve"])
 if diff.any():
     idx = numpy.argwhere(diff)[:20]
     out["first_diffs"] = idx.tolist()
