@@ -334,7 +334,7 @@ int mgc_gradient_magnitude_prewitt(int32_t ndim, const int64_t* shape, const mgc
 int mgc_slab_plane_elems(const mgc_graph* g, int64_t* n);
 /* Initialise the solver state (source-excess clamp, sink capacities) once all terms are in. */
 int mgc_slab_begin(mgc_graph* g);
-/* `n` local push/relabel passes (tile solver: two-colour passes; per-voxel solver: sweeps). */
+/* `n` local push/relabel passes of the tile solver, each one over both tile colours. */
 int mgc_slab_push(mgc_graph* g, int32_t n);
 /* Pack the messages for the lower / upper neighbour into device buffers of plane_elems elements each:
  * heights (int32) of my border plane and the flow (double) pushed across the border since the last pack.

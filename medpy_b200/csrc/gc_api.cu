@@ -132,7 +132,7 @@ struct mgc_graph {
     unsigned n_partials = 0;
     void* minmax_buf = nullptr;        // 3 x 1024 partial min/max/absmax
     double* d_scalars = nullptr;       // [0] flow_const, [1] absorbed, [2..3] minmax out
-    int* d_flags = nullptr;            // [0] bad weight, [1] changed, [2] work
+    int* d_flags = nullptr;            // [0] bad weight, [3] tiles materialised, [4..5] materialiser claim count / cursor
     unsigned long long* d_count = nullptr;
     int64_t device_bytes = 0;
 
@@ -209,7 +209,6 @@ struct mgc_graph {
     Tiles TL{};
     Tiles4 TL4{};                      // 4-D lattices: 4x4x8x4 tiles (gc_tiles4.cuh)
     uint8_t* smask = nullptr;          // 4-D: residual sink link flag (the 8 arc bits fill rmask)
-    bool use_tiles = false;            // false on 4-D z-slabs only: they run the per-voxel solver of gc_solver.cuh
     int* pflag = nullptr;              // push: tile is already on the list its colour consumes next
     int* rflag = nullptr;              // relabel: tile is already on the next relabel list
     int* rl_items[2] = {nullptr, nullptr};     // relabel worklists (double buffered)
@@ -249,7 +248,6 @@ struct mgc_graph {
     int sweep_done_frac = 16;          // hand over to the worklist BFS when violating tiles <= ntiles / sweep_done_frac
 
     // tuning
-    int relax_batch = 4;
     int64_t max_rounds = 100000;
 
     // z-slab solve inside the library (mgc_slab_comm_init / mgc_slab_solve): NCCL communicator of the slab ranks, border
@@ -542,13 +540,11 @@ bool make_push_maps(mgc_graph* g)
     return true;
 }
 
-// the environment options of the tile solver, the same for 3-D and 4-D lattices (4-D z-slab handles run the per-voxel
-// solver and read none of them).  `bfs` is the cooperative BFS kernel of the lattice's tile shape, launched with
-// `bfs_threads` threads per CTA: its occupancy sizes the grid.
+// the environment options of the tile solver, the same for 3-D and 4-D lattices.  `bfs` is the cooperative BFS kernel
+// of the lattice's tile shape, launched with `bfs_threads` threads per CTA: its occupancy sizes the grid.
 int tile_solver_options(mgc_graph* g, const void* bfs, int bfs_threads)
 {
     g->n_ctas = 2 * cached_sm_count(g->device);   // k_push_tile is built for 2 CTAs per SM
-    g->use_tiles = true;
     if (const char* e1 = getenv("MEDPY_GC_ITERS")) if (atoi(e1) > 0) g->tile_iters = g->tile_iters_first = atoi(e1);
     if (const char* e2 = getenv("MEDPY_GC_PASSES0")) if (atoi(e2) > 0) g->passes0 = atoi(e2);
     if (const char* e3 = getenv("MEDPY_GC_PASSES_MAX")) if (atoi(e3) > 0) g->passes_max = atoi(e3);
@@ -677,7 +673,7 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
                 cudaGetLastError();
         }
     }
-    if (!rc && g->nd == 4 && !slab) {
+    if (!rc && g->nd == 4) {
         const int ext[4] = {4, 4, 8, 4};
         g->TL4.ntiles = 1;
         for (int d = 0; d < 4; ++d) { g->TL4.nt[d] = (g->L.dim[d] + ext[d] - 1) / ext[d]; g->TL4.ntiles *= g->TL4.nt[d]; }
@@ -711,7 +707,6 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
     // [0] weight verdict, [2..3] active count, [4] BFS passes of the last cooperative relabel.  From the pinned pool: cudaHostAlloc / cudaFreeHost per handle (one handle per
     // graph_from_voxels call) are heavyweight driver calls that synchronise the device
     { void* hp = nullptr; g->h_bad = (mgc_host_alloc(64, &hp) == MGC_OK) ? (int*)hp : nullptr; }
-    if (const char* s2 = getenv("MEDPY_GC_RELAX_BATCH")) g->relax_batch = atoi(s2) > 0 ? atoi(s2) : g->relax_batch;
     g->st.n_voxels = (int64_t)n;
     rc = mgc_reset(g);
     if (rc) { g_create_error = g->err; mgc_destroy(g); return rc; }
@@ -904,73 +899,6 @@ double caps_resolve(mgc_graph* g)
     g->caps_ev_used = 0;
     g->st.ms_caps += total;
     return total;
-}
-
-// ---- per-voxel solver (gc_solver.cuh): 4-D z-slabs only --------------------------------------------------
-int ensure_state(mgc_graph* g)
-{
-    if (g->state_init) return MGC_OK;
-    { int rc0 = materialise_zeros(g); if (rc0) return rc0; }
-    { int rc0 = push_state_all(g); if (rc0) return rc0; }
-    k_init_state<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
-    g->st.kernel_launches++;
-    CK(cudaGetLastError());
-    g->state_init = true;
-    return MGC_OK;
-}
-
-int relabel_init(mgc_graph* g)
-{
-    k_relabel_init<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S);
-    g->st.kernel_launches++;
-    CK(cudaGetLastError());
-    return MGC_OK;
-}
-
-// relax until a whole batch changes nothing; *any = 1 if anything changed at all
-int relabel_relax(mgc_graph* g, int* any)
-{
-    *any = 0;
-    for (;;) {
-        CK(cudaMemsetAsync(g->d_flags + 1, 0, sizeof(int), g->stream));
-        cudaEventRecord(g->ev[2], g->stream);
-        for (int i = 0; i < g->relax_batch; ++i)
-            k_relabel_relax<4><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S.rmask, g->S.height, g->d_flags + 1);
-        g->st.kernel_launches += g->relax_batch;
-        g->st.relabel_sweeps += g->relax_batch;
-        cudaEventRecord(g->ev[3], g->stream);
-        int changed = 0;
-        CK(cudaMemcpyAsync(&changed, g->d_flags + 1, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
-        CK(cudaStreamSynchronize(g->stream));
-        { float ms = 0; cudaEventElapsedTime(&ms, g->ev[2], g->ev[3]); g->st.ms_relabel += ms; }
-        if (!changed) break;
-        *any = 1;
-    }
-    return MGC_OK;
-}
-
-int count_active(mgc_graph* g, int64_t* out)
-{
-    CK(cudaMemsetAsync(g->d_count, 0, sizeof(unsigned long long), g->stream));
-    k_count_active<double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->d_count);
-    g->st.kernel_launches++;
-    unsigned long long c = 0;
-    CK(cudaMemcpyAsync(&c, g->d_count, sizeof(c), cudaMemcpyDeviceToHost, g->stream));
-    CK(cudaStreamSynchronize(g->stream));
-    *out = (int64_t)c;
-    g->st.active_last = (int64_t)c;
-    return MGC_OK;
-}
-
-// n push sweeps (k_push raises the work flag d_flags[2]; nobody reads it here)
-int push_sweeps(mgc_graph* g, int n)
-{
-    g->flow_started = true;
-    for (int i = 0; i < n; ++i) k_push<4, double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, g->d_flags + 2);
-    g->st.kernel_launches += n;
-    g->st.push_sweeps += n;
-    CK(cudaGetLastError());
-    return MGC_OK;
 }
 
 // ---- tile solver driver --------------------------------------------------------------------------------
@@ -2974,12 +2902,9 @@ int mgc_slab_begin(mgc_graph* g)
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
     resolve_term_span(g);
-    if (g->use_tiles) {
-        int rc = materialise_zeros(g);
-        if (rc) return rc;
-        return g->state_init ? MGC_OK : init_tiles(g);
-    }
-    return ensure_state(g);
+    int rc = materialise_zeros(g);
+    if (rc) return rc;
+    return g->state_init ? MGC_OK : init_tiles(g);
 }
 
 int mgc_slab_push(mgc_graph* g, int32_t n)
@@ -2988,8 +2913,7 @@ int mgc_slab_push(mgc_graph* g, int32_t n)
     if (!g->state_init) FAIL(MGC_E_STATE, "call mgc_slab_begin first");
     CK(cudaSetDevice(g->device));
     g->iters_now = g->tile_iters;
-    if (g->use_tiles) return push_tiles(g, n);
-    return push_sweeps(g, n);
+    return push_tiles(g, n);
 }
 
 int mgc_slab_pack(mgc_graph* g, int32_t* h_lo, double* f_lo, int32_t* h_hi, double* f_hi)
@@ -3027,15 +2951,14 @@ int mgc_slab_unpack(mgc_graph* g, const int32_t* h_lo, const double* f_lo, const
         const int k = side == 0 ? 0 : 1;     // my arc border -> ghost: axis 0, -1 (lo) or +1 (hi)
         const int32_t* hin = side == 0 ? h_lo : h_hi;
         const double* fin = side == 0 ? f_lo : f_hi;
-        if (g->use_tiles) {
+        if (g->nd == 4)
+            k_slab_unpack_tiles4<double><<<nb, 256, 0, g->stream>>>(g->L, g->TL4, g->S, zg, zb, k, hin, fin, g->rflag, rl(g, 0), rl(g, 1),
+                                                                   g->d_tcount + CTL_RLCUR, g->pflag, pl(g, 0, g->pl_sel[0]),
+                                                                   pl(g, 1, g->pl_sel[1]), changed_dev);
+        else
             k_slab_unpack_tiles<double><<<nb, 256, 0, g->stream>>>(g->L, g->TL, g->S, zg, zb, k, hin, fin, g->rflag, rl(g, 0), rl(g, 1),
                                                                   g->d_tcount + CTL_RLCUR, g->pflag, pl(g, 0, g->pl_sel[0]),
                                                                   pl(g, 1, g->pl_sel[1]), changed_dev);
-        } else {
-            const size_t border = (size_t)zb * P, ghost = (size_t)zg * P;
-            k_slab_unpack<double><<<nb, 256, 0, g->stream>>>(P, g->S.height + ghost, g->S.excess + border, g->S.cap[k] + border,
-                                                            hin, fin, changed_dev);
-        }
         g->st.kernel_launches++;
     }
     CK(cudaGetLastError());
@@ -3048,8 +2971,7 @@ int mgc_slab_relabel_begin(mgc_graph* g)
     if (!g->state_init) FAIL(MGC_E_STATE, "call mgc_slab_begin first");
     CK(cudaSetDevice(g->device));
     g->st.global_relabels++;
-    if (g->use_tiles) return relabel_tiles_begin(g);
-    return relabel_init(g);
+    return relabel_tiles_begin(g);
 }
 
 int mgc_slab_relabel_relax(mgc_graph* g, int32_t* changed_out)
@@ -3057,7 +2979,7 @@ int mgc_slab_relabel_relax(mgc_graph* g, int32_t* changed_out)
     if (!g) return MGC_E_ARG;
     CK(cudaSetDevice(g->device));
     int any = 0;
-    const int rc = g->use_tiles ? relabel_tiles_run(g, &any, changed_out != nullptr) : relabel_relax(g, &any);
+    const int rc = relabel_tiles_run(g, &any, changed_out != nullptr);
     if (rc) return rc;
     if (changed_out) *changed_out = any ? 1 : 0;
     return MGC_OK;
@@ -3067,22 +2989,14 @@ int mgc_slab_count_active(mgc_graph* g, int64_t* active_out)
 {
     if (!g || !active_out) return MGC_E_ARG;
     CK(cudaSetDevice(g->device));
-    return g->use_tiles ? count_active_tiles(g, active_out) : count_active(g, active_out);
+    return count_active_tiles(g, active_out);
 }
 
 int mgc_slab_count_active_dev(mgc_graph* g, unsigned long long* count_dev)
 {
     if (!g || !count_dev) return MGC_E_ARG;
     CK(cudaSetDevice(g->device));
-    CK(cudaMemsetAsync(count_dev, 0, sizeof(unsigned long long), g->stream));
-    if (g->use_tiles) {
-        return count_active_tiles_enqueue(g, count_dev);
-    } else {
-        k_count_active<double><<<nblocks(g), 256, 0, g->stream>>>(g->L, g->S, count_dev);
-        g->st.kernel_launches++;
-    }
-    CK(cudaGetLastError());
-    return MGC_OK;
+    return count_active_tiles_enqueue(g, count_dev);
 }
 
 int mgc_slab_finish(mgc_graph* g, double* energy_part)

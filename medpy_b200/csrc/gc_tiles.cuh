@@ -1,5 +1,5 @@
-// gc_tiles.cuh -- tile-resident solver kernels for the 3-D lattice (gc_tiles4.cuh holds the 4-D ones;
-// gc_solver.cuh keeps the per-voxel kernels, which only 4-D z-slabs run).
+// gc_tiles.cuh -- tile-resident solver kernels for the 3-D lattice (gc_tiles4.cuh holds the 4-D ones).  Every lattice
+// handle, z-slabs included, runs the tile solver.
 //
 // The lattice is cut into 8x8x8 tiles.  A 512-thread CTA owns one tile for the duration of a visit, keeps the
 // tile's state on chip (heights with a 1-voxel halo in shared memory; in the push kernel the six residual
@@ -479,9 +479,11 @@ __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, 
 }
 
 // ---------------------------------------------------------------------------------------------------
-// z-slab border messages, tile-aware: besides applying the neighbour's message (see k_slab_unpack) the
-// receiving tiles are put on the worklists -- the relabel list when a ghost label changed, the push list of
-// the tile's colour when flow arrived -- and the border voxel's residual mask gains the arc towards the ghost.
+// z-slab border messages (written by k_slab_pack of gc_solver.cuh; k_slab_unpack_tiles4 is the 4-D form): ghost
+// labels <- the neighbour's border labels; received flow joins the excess of the border voxel and the residual of its
+// arc towards the ghost (the reverse of the arc the flow arrived on), and the border voxel's residual mask gains that
+// arc.  The receiving tiles are put on the worklists -- the relabel list when a ghost label changed, the push list of
+// the tile's colour when flow arrived.
 // ---------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void k_slab_unpack_tiles(Lattice L, Tiles TL, State<T> S, int z_ghost, int z_border, int k_border_to_ghost,

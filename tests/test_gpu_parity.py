@@ -14,6 +14,7 @@ import numpy
 import pytest
 
 from conftest import golden
+from test_gpu_push_window import _env
 
 pytestmark = pytest.mark.gpu
 
@@ -467,11 +468,19 @@ def _two_slabs_one_gpu(vol, regional, split):
     return energy, mask
 
 
-@pytest.mark.parametrize("shape,split,regional", [((40, 32, 32), 20, True), ((40, 32, 32), 13, False), ((37, 24, 40), 9, True),
-                                                  # 4-D slabs (per-voxel solver): ragged, one-plane and even splits
-                                                  ((20, 12, 16, 9), 7, True), ((17, 10, 8, 33), 1, False),
-                                                  ((16, 8, 8, 4), 8, True)])
-def test_two_slabs_on_one_gpu_vs_oracle(shape, split, regional):
+# 4-D slabs (4 x 4 x 8 x 4 tiles with ghost planes): ragged, one-plane and even splits, and a split that leaves both
+# slabs at least 64 tiles (72 and 96), so that their relabels can run directional sweeps
+SLABS4 = [((20, 12, 16, 9), 7, True), ((17, 10, 8, 33), 1, False), ((16, 8, 8, 4), 8, True), ((24, 16, 16, 12), 11, False)]
+
+# tile-solver options that change how a slab is relabelled or how long a tile visit runs; create_impl reads them
+SLAB4_OPTIONS = {
+    "hard": dict(MEDPY_GC_SWEEP_FRAC=1000000),      # directional sweeps in front of every relabel
+    "sweep_off": dict(MEDPY_GC_SWEEP=0),
+    "iters1": dict(MEDPY_GC_ITERS=1),
+}
+
+
+def _two_slabs_vs_oracle(shape, split, regional):
     from medpy_b200 import synthetic
     from oracle import energy_terms as et
     vol = synthetic.two_blob_volume(shape, seed=4)
@@ -481,6 +490,19 @@ def test_two_slabs_on_one_gpu_vs_oracle(shape, split, regional):
     oflow, omask, _ = _oracle_solve(prob)
     assert numpy.array_equal(mask, omask)
     assert abs(energy - oflow) <= 1e-9 * abs(oflow)
+
+
+@pytest.mark.parametrize("shape,split,regional", [((40, 32, 32), 20, True), ((40, 32, 32), 13, False), ((37, 24, 40), 9, True)]
+                         + SLABS4)
+def test_two_slabs_on_one_gpu_vs_oracle(shape, split, regional):
+    _two_slabs_vs_oracle(shape, split, regional)
+
+
+@pytest.mark.parametrize("opt", list(SLAB4_OPTIONS))
+@pytest.mark.parametrize("shape,split,regional", SLABS4)
+def test_two_4d_slabs_on_one_gpu_under_solver_options(shape, split, regional, opt):
+    with _env(**SLAB4_OPTIONS[opt]):
+        _two_slabs_vs_oracle(shape, split, regional)
 
 
 @pytest.mark.parametrize("case", ["regional", "boundary"])
