@@ -110,6 +110,8 @@ typedef struct mgc_stats {
     int64_t relabel_passes;     /* tile solver: BFS passes (worklist generations) of all global relabels; relabel_sweeps counts launches */
     double ms_relabel_first;    /* device ms of the first global relabel of each solve (tile solver), summed */
     int64_t relabel_passes_first; /* ... its BFS passes, summed */
+    int64_t build_blocks_refused; /* lazy exponential build staged by TMA: 8 x 8 x 32 build blocks whose range test failed */
+                                  /* (built by the per-warp fallback launch instead of the lean one); read at the solve  */
 } mgc_stats;
 
 /* ---- lifetime ------------------------------------------------------------------------------------- */

@@ -132,7 +132,8 @@ struct mgc_graph {
     unsigned n_partials = 0;
     void* minmax_buf = nullptr;        // 3 x 1024 partial min/max/absmax
     double* d_scalars = nullptr;       // [0] flow_const, [1] absorbed, [2..3] minmax out
-    int* d_flags = nullptr;            // [0] bad weight, [3] tiles materialised, [4..5] materialiser claim count / cursor
+    int* d_flags = nullptr;            // [0] bad weight, [3] tiles materialised, [4..5] materialiser claim count / cursor,
+                                       // [6] blocks refused by the last lean build launch, [7] ... by the whole build
     unsigned long long* d_count = nullptr;
     int64_t device_bytes = 0;
 
@@ -164,6 +165,10 @@ struct mgc_graph {
     bool debug_checks = false;         // MEDPY_GC_DEBUG=1: device-side invariant + flow-conservation checks around every solve
     double debug_excess0 = 0.0;        // clamped source excess the solve started from
     bool fuse_build = true;            // mgc_build_voxel_graph uses the single-pass k_build_tile (MEDPY_GC_FUSE=0: four passes)
+    // lazy exponential build staged by TMA: every block goes to k_build_refused, none is streamed by k_build_lean
+    // (MEDPY_GC_BUILD_REFUSE_ALL=1; for tests that compare the two paths on one volume)
+    bool build_refuse_all = false;
+    int* build_refused = nullptr;      // blocks k_build_lean refused (indices into its grid), one entry per build block
     // lazy push state: the fused 3-D build writes no capacity planes, no tr and no excess; k_caps_tiles computes them per
     // tile, from copies of the build's inputs, for the tiles the push path reaches (MEDPY_GC_LAZY_CAPS=0: the build
     // writes them all)
@@ -553,6 +558,7 @@ int tile_solver_options(mgc_graph* g, const void* bfs, int bfs_threads)
     if (const char* e9 = getenv("MEDPY_GC_SWEEP_ROUNDS")) if (atoi(e9) > 0) g->sweep_rounds_max = atoi(e9);
     if (const char* e11 = getenv("MEDPY_GC_SWEEP_MIN_ROUNDS")) if (atoi(e11) > 0) g->sweep_rounds_min = atoi(e11);
     if (const char* e10 = getenv("MEDPY_GC_SWEEP_DONE_FRAC")) if (atoi(e10) > 0) g->sweep_done_frac = atoi(e10);
+    if (const char* e12 = getenv("MEDPY_GC_BUILD_REFUSE_ALL")) g->build_refuse_all = atoi(e12) != 0;
     int coop = 0, nb = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, g->device);
     if (!coop || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, bfs, bfs_threads, 0) != cudaSuccess || nb < 1) {
@@ -631,6 +637,7 @@ int create_impl(int32_t ndim, const int64_t* shape, int64_t z0, int64_t z1, bool
     if (g->nd == 3) {   // k_build_tile writes one partial per 8 x 8 x 32 block
         const unsigned nbuild = (unsigned)((g->L.dim[0] + 7) / 8) * (unsigned)((g->L.dim[1] + 7) / 8) * (unsigned)((g->L.dim[2] + 31) / 32);
         if (nbuild > g->n_partials) g->n_partials = nbuild;
+        if (!rc) { rc = alloc_buf(g, (size_t)nbuild * sizeof(int), &p); g->build_refused = (int*)p; }
     }
     if (!rc) { rc = alloc_buf(g, (size_t)g->n_partials * sizeof(double), &p); g->partials = (double*)p; }
     if (!rc) { rc = alloc_buf(g, 3 * 1024 * sizeof(double), &p); g->minmax_buf = p; }
@@ -1377,14 +1384,15 @@ int readout(mgc_graph* g, double* energy_part)
     k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, rblocks(g), g->d_scalars + 1);
     g->st.kernel_launches += 2;
     double sc[2] = {0, 0};
-    int n_mat = 0;
+    int fl[5] = {0, 0, 0, 0, 0};     // d_flags[3..7]: [0] tiles materialised, [4] build blocks refused
     int win[2] = {0, 0};             // WIN_DEFERRED, WIN_DROPPED of this solve
     CK(cudaMemcpyAsync(sc, g->d_scalars, sizeof(sc), cudaMemcpyDeviceToHost, g->stream));
-    CK(cudaMemcpyAsync(&n_mat, g->d_flags + 3, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
+    CK(cudaMemcpyAsync(fl, g->d_flags + 3, sizeof(fl), cudaMemcpyDeviceToHost, g->stream));
     if (g->win_ctl) CK(cudaMemcpyAsync(win, g->win_ctl + WIN_DEFERRED, sizeof(win), cudaMemcpyDeviceToHost, g->stream));
     CK(cudaStreamSynchronize(g->stream));
     g->st.flow_const = sc[0];
-    g->st.tiles_materialised = n_mat;
+    g->st.tiles_materialised = fl[0];
+    g->st.build_blocks_refused = fl[4];
     g->st.tiles_deferred += win[0];
     g->st.tiles_dropped += win[1];
     *energy_part = sc[0] + sc[1];
@@ -1575,9 +1583,47 @@ bool make_block_map(mgc_graph* g, const void* ptr, int dtype, CUtensorMap* out)
                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// The lazy build under the exponential term without spacing, image staged by TMA: k_build_lean over the whole grid, then
+// k_build_refused on the blocks it refused (gc_build.cuh).  No host synchronisation: the second launch reads the count.
+template <typename E, int USE_MAX, int TIN>
+int build_launch_split(mgc_graph* g, const BuildMaps& imap, const BuildArgs& A, const BoundaryParams& P, int nz_layers)
+{
+    auto lean = k_build_lean<E, TIN>;
+    auto ref = k_build_refused<E, USE_MAX, TIN>;
+    const size_t smem_lean = LeanSmem<E, TIN>::BYTES, smem_ref = build_smem_bytes<E>();
+    static int ref_ctas = 0;             // per instantiation: persistent CTAs of the refused launch
+    if (!ref_ctas) {
+        cudaFuncSetAttribute(lean, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_lean);
+        cudaFuncSetAttribute(ref, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ref);
+        int nb = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, ref, BUILD_THREADS, smem_ref) != cudaSuccess || nb < 1) {
+            cudaGetLastError();
+            nb = 1;
+        }
+        ref_ctas = nb * cached_sm_count(g->device);
+    }
+    const int nbx = (g->L.dim[2] + BUILD_TX - 1) / BUILD_TX, nby = (g->L.dim[1] + BUILD_TY - 1) / BUILD_TY;
+    int* count = g->d_flags + 6;         // blocks refused by this lean launch
+    int* total = g->d_flags + 7;         // ... by every lean launch of the build
+    CK(cudaMemsetAsync(count, 0, sizeof(int), g->stream));
+    lean<<<dim3((unsigned)nbx, (unsigned)nby, (unsigned)nz_layers), BUILD_THREADS, smem_lean, g->stream>>>(
+        g->L, g->TL, g->S, imap, A, P, g->partials, g->rflag, rl(g, 0), g->pflag, pl(g, 0, 0), pl(g, 1, 0), g->build_refused,
+        count, g->build_refuse_all ? 1 : 0);
+    CK(cudaGetLastError());
+    const int nblk = nbx * nby * nz_layers;
+    ref<<<(unsigned)(nblk < ref_ctas ? nblk : ref_ctas), BUILD_THREADS, smem_ref, g->stream>>>(
+        g->L, g->TL, g->S, imap, A, P, g->d_flags, g->partials, g->rflag, rl(g, 0), g->pflag, pl(g, 0, 0), pl(g, 1, 0),
+        g->build_refused, count, total, nbx, nby);
+    g->st.kernel_launches += 2;
+    CK(cudaGetLastError());
+    return MGC_OK;
+}
+
 template <typename E, int FN, int USE_MAX, int SPACING, int TIN, int LAZY>
 int build_launch_inst(mgc_graph* g, const BuildMaps& imap, const BuildArgs& A, const BoundaryParams& P, int nz_layers)
 {
+    if constexpr (LAZY && FN == 1 && SPACING == 0 && USE_MAX >= 0 && (std::is_same<E, float>::value || std::is_same<E, double>::value))
+        if (A.use_tma) return build_launch_split<E, USE_MAX, TIN>(g, imap, A, P, nz_layers);
     auto kern = k_build_tile<E, double, FN, USE_MAX, SPACING, TIN, LAZY>;
     const size_t smem = build_smem_bytes<E>();
     static bool attr_done = false;       // per instantiation
@@ -2141,6 +2187,7 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
 
     CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
     CK(cudaMemsetAsync(g->d_flags, 0, sizeof(int), g->stream));
+    CK(cudaMemsetAsync(g->d_flags + 7, 0, sizeof(int), g->stream));     // blocks refused by the lean build
     { int rcd = dirty_clear(g); if (rcd) return rcd; }
     g->pl_sel[0] = g->pl_sel[1] = 0;
     cudaEventRecord(g->ev_b[0], g->stream);

@@ -23,6 +23,8 @@
 // capacity), and publishes the +y / +x weights in a shared-memory plane from which the neighbours in y and x take
 // their backward capacities.  The only weights evaluated twice are those on the block's low faces (12.5 %).
 #pragma once
+#include <climits>
+#include <type_traits>
 #include "gc_terms.cuh"
 #include "gc_tiles.cuh"
 #include "gc_tma.cuh"
@@ -193,13 +195,17 @@ __device__ __forceinline__ bool source_active(double tr, unsigned pairs)
 // the warp vote per z-step, and a warp whose arguments are not ordinary evaluates all six weights per voxel (rmask
 // depends on them; no z carry, no shared planes: a neighbouring warp may have skipped).  Other terms still evaluate
 // every weight (weight check, rmask) but store none.
-template <typename E, typename T, int FN, int USE_MAX, int SPACING, int TIN = 0, int LAZY = 0>
-__global__ void __launch_bounds__(BUILD_THREADS)
-k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps maps, BuildArgs A, BoundaryParams P,
-             int* __restrict__ bad, double* __restrict__ partials, int* __restrict__ rflag, WorkList rl,
-             int* __restrict__ pflag, WorkList pl0, WorkList pl1)
+//
+// The body builds block (bx, by, bz) of a launch of nbx x nby x (layers) blocks; k_build_tile runs it for its own CTA,
+// k_build_refused for the blocks the lean kernel (below) refused.  `first`: the CTA's first block (the mbarrier is
+// initialised), `parity`: the mbarrier phase of this block's copies.
+template <typename E, typename T, int FN, int USE_MAX, int SPACING, int TIN, int LAZY>
+__device__ __forceinline__ void
+build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parity, unsigned char* smem_raw,
+            const Lattice& L, const Tiles& TL, const State<T>& S, const BuildMaps& maps, const BuildArgs& A,
+            const BoundaryParams& P, int* __restrict__ bad, double* __restrict__ partials, int* __restrict__ rflag,
+            const WorkList& rl, int* __restrict__ pflag, const WorkList& pl0, const WorkList& pl1)
 {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
     constexpr int BUILD_BX = BuildBox<E>::BX, BUILD_PAD = BuildBox<E>::PAD;
     E* s_img = reinterpret_cast<E*>(smem_raw);                                   // [10][10][BUILD_BX]
     constexpr int IMG_BYTES = BUILD_HZ * BUILD_HY * BUILD_BX * (int)sizeof(E);
@@ -217,7 +223,7 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
 
     const int tid = threadIdx.x;
     const int lx = tid & 31, ly = tid >> 5;
-    const int x0 = blockIdx.x * BUILD_TX, y0 = blockIdx.y * BUILD_TY, z0 = (A.z_tile0 + (int)blockIdx.z) * BUILD_TZ;
+    const int x0 = bx * BUILD_TX, y0 = by * BUILD_TY, z0 = (A.z_tile0 + bz) * BUILD_TZ;
     const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
     const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
     constexpr bool LAZY_EXP = LAZY && FN == 1 && SPACING == 0;      // the lazy path that may skip the weights
@@ -266,8 +272,12 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
     if (tid < 8) s_flags[tid] = 0;
     if (A.use_tma) {
         if (tid == 0) {
-            mbar_init(bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+            if (first) {
+                mbar_init(bar, 1);
+                asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+            } else {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the previous block's reads are done
+            }
             const unsigned pbytes = (A.prob && A.tma_prob) ? (unsigned)(BUILD_TZ * BUILD_TY * BUILD_TX * (A.prob_f64 ? 8 : 4)) : 0u;
             const unsigned mbytes = (unsigned)(BUILD_TZ * BUILD_TY * BUILD_TX);
             mbar_expect_tx(bar, (unsigned)IMG_BYTES + pbytes + ((A.tma_mark & 1) ? mbytes : 0u) + ((A.tma_mark & 2) ? mbytes : 0u));
@@ -277,7 +287,7 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
             if (A.tma_mark & 2) tma_load_3d(s_bg, &maps.bg, bar, x0, y0, z0);
         }
         __syncthreads();
-        mbar_wait(bar, 0u);
+        mbar_wait(bar, parity);
         if (staged_tin) cur = fetch(0);
     } else {
         // (LAZY_EXP stages whole rows of the box, as TMA does: the block's range test reads every cell)
@@ -495,7 +505,7 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         if (LAZY) {      // marker bit planes: one word per warp row and marker
             const unsigned bf = __ballot_sync(0xffffffffu, pin && (cur.fb & 1u)), bb = __ballot_sync(0xffffffffu, pin && (cur.fb & 2u));
             if (lx == 0 && gz < L.dim[0] && gy < L.dim[1]) {
-                const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * gridDim.x + blockIdx.x;
+                const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * (unsigned)nbx + (unsigned)bx;
                 if (A.fg_plane) A.fg_plane[w] = bf;
                 if (A.bg_plane) A.bg_plane[w] = bb;
             }
@@ -524,7 +534,7 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
         double t = s_red[0];
 #pragma unroll
         for (int w = 1; w < 8; ++w) t = __dadd_rn(t, s_red[w]);
-        partials[((A.z_tile0 + blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = t;
+        partials[((A.z_tile0 + bz) * nby + by) * nbx + bx] = t;
     }
     if (tid < 4) {
         const int tx = (x0 >> 3) + tid, ty = y0 >> 3, tz = z0 >> 3;
@@ -543,11 +553,342 @@ k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps 
     }
 }
 
+template <typename E, typename T, int FN, int USE_MAX, int SPACING, int TIN = 0, int LAZY = 0>
+__global__ void __launch_bounds__(BUILD_THREADS)
+k_build_tile(Lattice L, Tiles TL, State<T> S, const __grid_constant__ BuildMaps maps, BuildArgs A, BoundaryParams P,
+             int* __restrict__ bad, double* __restrict__ partials, int* __restrict__ rflag, WorkList rl,
+             int* __restrict__ pflag, WorkList pl0, WorkList pl1)
+{
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    build_block<E, T, FN, USE_MAX, SPACING, TIN, LAZY>((int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z, (int)gridDim.x,
+                                                       (int)gridDim.y, true, 0u, smem_raw, L, TL, S, maps, A, P, bad,
+                                                       partials, rflag, rl, pflag, pl0, pl1);
+}
+
 template <typename E>
 constexpr size_t build_smem_bytes()
 {
     return (size_t)BUILD_TIN_OFFSET((BUILD_HZ * BUILD_HY * BuildBox<E>::BX * (int)sizeof(E) + 127) / 128 * 128) +
            (size_t)BUILD_TZ * BUILD_TY * BUILD_TX * (8 + 1 + 1);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// The lazy build under the exponential term without spacing, image block staged by TMA, as two launches (DESIGN.md §4.0):
+//   k_build_lean    : stages every block and runs its range test; a block that passes is streamed by a loop that holds
+//                     nothing but the lean path, a block that fails writes nothing and appends its index to a list;
+//   k_build_refused : persistent CTAs run the k_build_tile body (range test, per-warp vote, six weights) on the listed
+//                     blocks.  The launch follows on the same stream without a host synchronisation; it reads the
+//                     list's length on the device and returns at once when nothing was refused.
+// Both write exactly what k_build_tile<..., LAZY = 1> writes for their blocks.
+// ---------------------------------------------------------------------------------------------------
+template <typename E, int USE_MAX, int TIN>
+__global__ void __launch_bounds__(BUILD_THREADS, 4)
+k_build_refused(Lattice L, Tiles TL, State<double> S, const __grid_constant__ BuildMaps maps, BuildArgs A, BoundaryParams P,
+                int* __restrict__ bad, double* __restrict__ partials, int* __restrict__ rflag, WorkList rl,
+                int* __restrict__ pflag, WorkList pl0, WorkList pl1, const int* __restrict__ list,
+                const int* __restrict__ count, int* __restrict__ total, int nbx, int nby)
+{
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const int n = *count;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && n) atomicAdd(total, n);
+    for (int i = blockIdx.x, it = 0; i < n; i += gridDim.x, ++it) {
+        const int b = list[i];
+        const int bx = b % nbx, r = b / nbx;
+        build_block<E, double, 1, USE_MAX, 0, TIN, 1>(bx, r % nby, r / nby, nbx, nby, it == 0, (unsigned)it & 1u, smem_raw,
+                                                      L, TL, S, maps, A, P, bad, partials, rflag, rl, pflag, pl0, pl1);
+        __syncthreads();          // shared memory is restaged for the next block
+    }
+}
+
+// shared memory of k_build_lean: image block with halo | probability block | fg block | bg block | barrier, tile flags,
+// range and reduction scratch.  The add_tweights minima of the block (2048 doubles) overlay the image block once the
+// range test and the image copy have read it; the image region is at least that large.
+template <typename E, int TIN>
+struct LeanSmem {
+    static constexpr int IMG_BYTES = BUILD_HZ * BUILD_HY * BuildBox<E>::BX * (int)sizeof(E);
+    static constexpr int MM_BYTES = BUILD_TZ * BUILD_TY * BUILD_TX * 8;
+    static constexpr int PROB_OFF = (IMG_BYTES > MM_BYTES ? (IMG_BYTES + 127) / 128 * 128 : MM_BYTES);
+    static constexpr int FG_OFF = PROB_OFF + BUILD_TZ * BUILD_TY * BUILD_TX * (TIN == 1 ? 4 : 8);
+    static constexpr int BG_OFF = FG_OFF + BUILD_TZ * BUILD_TY * BUILD_TX;
+    static constexpr int MISC_OFF = BG_OFF + BUILD_TZ * BUILD_TY * BUILD_TX;
+    static constexpr int BYTES = MISC_OFF + 256;
+};
+
+// The range test of a staged block (block_exp_ordinary over every cell of the box), uniform over the CTA.  float32:
+// integer keys (gc_exprange.cuh); other types: the float fold of k_build_tile.  `scratch`: 192 bytes of shared memory.
+template <typename E>
+__device__ __forceinline__ bool lean_range_test(const E* s_img, unsigned char* scratch, bool use_max, double inv_sigma2)
+{
+    constexpr int NV = LeanSmem<E, 0>::IMG_BYTES / 16;
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    if constexpr (std::is_same<E, float>::value) {
+        int kmin = INT_MAX, kmax = INT_MIN;
+        for (int i = tid; i < NV; i += BUILD_THREADS) {
+            const int4 q = reinterpret_cast<const int4*>(s_img)[i];
+            const int a = er_f32_key(q.x), b = er_f32_key(q.y), c = er_f32_key(q.z), d = er_f32_key(q.w);
+            kmin = min(kmin, min(min(a, b), min(c, d)));
+            kmax = max(kmax, max(max(a, b), max(c, d)));
+        }
+        kmin = __reduce_min_sync(0xffffffffu, kmin);
+        kmax = __reduce_max_sync(0xffffffffu, kmax);
+        int* s_k = reinterpret_cast<int*>(scratch);
+        if (lane == 0) { s_k[w] = kmin; s_k[8 + w] = kmax; }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) { kmin = min(kmin, s_k[k]); kmax = max(kmax, s_k[8 + k]); }
+        return block_exp_ordinary_keys(kmin, kmax, use_max, inv_sigma2);
+    } else {
+        E lo = (E)INFINITY, hi = (E)-INFINITY;
+        bool nan = false;
+        for (int i = tid; i < NV; i += BUILD_THREADS) {
+            const uint4 q = reinterpret_cast<const uint4*>(s_img)[i];
+            E e[16 / sizeof(E)];
+            memcpy(e, &q, 16);
+#pragma unroll
+            for (int k = 0; k < (int)(16 / sizeof(E)); ++k) block_range_add<E>(lo, hi, nan, e[k]);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const E olo = __shfl_xor_sync(0xffffffffu, lo, o), ohi = __shfl_xor_sync(0xffffffffu, hi, o);
+            block_range_add<E>(lo, hi, nan, olo);
+            block_range_add<E>(lo, hi, nan, ohi);
+        }
+        nan = __any_sync(0xffffffffu, nan);
+        E* s_rng = reinterpret_cast<E*>(scratch);                    // [8] warp minima, [8] warp maxima
+        int* s_rnan = reinterpret_cast<int*>(scratch + 16 * sizeof(E));
+        if (lane == 0) { s_rng[w] = lo; s_rng[8 + w] = hi; s_rnan[w] = nan ? 1 : 0; }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            block_range_add<E>(lo, hi, nan, s_rng[k]);
+            block_range_add<E>(lo, hi, nan, s_rng[8 + k]);
+            nan = nan || s_rnan[k] != 0;
+        }
+        return block_exp_ordinary(Elem<E>::val(lo), Elem<E>::val(hi), nan, use_max, inv_sigma2);
+    }
+}
+
+// bits k = 0..3 of the result: byte k of w is not zero
+__device__ __forceinline__ unsigned nonzero_bytes4(unsigned w)
+{
+    return ((__vcmpne4(w, 0u) & 0x08040201u) * 0x01010101u) >> 24;
+}
+
+// The lean build.  Thread (z, y, g) of the block -- tid = (z * 8 + y) * 4 + g -- owns the 8 voxels x0 + 8g .. x0 + 8g + 7
+// of row (z, y), the x-range of one 8^3 solver tile: it reads them with vector loads, replays their t-links, and writes
+// rmask (one 8-byte store), height (two 16-byte stores), its byte of the marker words (a quad of threads covers one
+// word) and, where the handle wants them, the image and map copies.  The block's add_tweights partial is formed in
+// k_build_tile's order: every voxel's minimum goes to shared memory, and thread (y, x) then chains its column over z,
+// followed by the same warp shuffle tree and the same fixed order over the 8 warps.  E: float or double (TMA-staged).
+template <typename E, int TIN>
+__global__ void __launch_bounds__(BUILD_THREADS, 6)
+k_build_lean(Lattice L, Tiles TL, State<double> S, const __grid_constant__ BuildMaps maps, BuildArgs A, BoundaryParams P,
+             double* __restrict__ partials, int* __restrict__ rflag, WorkList rl, int* __restrict__ pflag, WorkList pl0,
+             WorkList pl1, int* __restrict__ refused, int* __restrict__ n_refused, int refuse_all)
+{
+    using LS = LeanSmem<E, TIN>;
+    constexpr int BX = BuildBox<E>::BX, PAD = BuildBox<E>::PAD;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    E* s_img = reinterpret_cast<E*>(smem_raw);
+    unsigned char* s_prob = smem_raw + LS::PROB_OFF;
+    unsigned char* s_fg = smem_raw + LS::FG_OFF;
+    unsigned char* s_bg = smem_raw + LS::BG_OFF;
+    unsigned long long* bar = reinterpret_cast<unsigned long long*>(smem_raw + LS::MISC_OFF);
+    int* s_flags = reinterpret_cast<int*>(smem_raw + LS::MISC_OFF + 8);          // [4] needs, [4] has excess
+    unsigned char* s_scr = smem_raw + LS::MISC_OFF + 64;                          // range test, then block reduction
+    double* s_mm = reinterpret_cast<double*>(smem_raw);                           // [8 z][8 y][32 x], x ^ y swizzled
+
+    const int tid = threadIdx.x;
+    const int x0 = blockIdx.x * BUILD_TX, y0 = blockIdx.y * BUILD_TY, z0 = (A.z_tile0 + (int)blockIdx.z) * BUILD_TZ;
+    const int cx = x0 == 0 ? -1 : PAD - 1, cy = y0 == 0 ? -1 : 0, cz = z0 == 0 ? -1 : 0;
+    const bool has_prob = TIN == 1 || A.prob != nullptr;
+    if (tid < 8) s_flags[tid] = 0;
+    if (tid == 0) {
+        mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        const unsigned pbytes = (has_prob && A.tma_prob) ? (unsigned)(BUILD_TZ * BUILD_TY * BUILD_TX * (A.prob_f64 ? 8 : 4)) : 0u;
+        const unsigned mbytes = (unsigned)(BUILD_TZ * BUILD_TY * BUILD_TX);
+        mbar_expect_tx(bar, (unsigned)LS::IMG_BYTES + pbytes + ((A.tma_mark & 1) ? mbytes : 0u) + ((A.tma_mark & 2) ? mbytes : 0u));
+        tma_load_3d(s_img, &maps.img, bar, x0 - 1 - cx, y0 - 1 - cy, z0 - 1 - cz);
+        if (pbytes) tma_load_3d(s_prob, &maps.prob, bar, x0, y0, z0);
+        if (A.tma_mark & 1) tma_load_3d(s_fg, &maps.fg, bar, x0, y0, z0);
+        if (A.tma_mark & 2) tma_load_3d(s_bg, &maps.bg, bar, x0, y0, z0);
+    }
+    __syncthreads();
+    mbar_wait(bar, 0u);
+
+    if (!lean_range_test<E>(s_img, s_scr, P.use_max != 0, P.inv_sigma2) || refuse_all) {
+        if (tid == 0) refused[atomicAdd(n_refused, 1)] = ((int)blockIdx.z * (int)gridDim.y + (int)blockIdx.y) * (int)gridDim.x + (int)blockIdx.x;
+        return;          // uniform over the CTA
+    }
+
+    const int g = tid & 3, ty = (tid >> 2) & 7, tz = tid >> 5;
+    const int gy = y0 + ty, gz = z0 + tz, xb = x0 + 8 * g;
+    const bool row_in = gz < L.dim[0] && gy < L.dim[1];
+    const int nx = row_in ? min(8, L.dim[2] - xb) : 0;                 // in-lattice voxels of this thread (<= 0: none)
+    const unsigned pin = nx >= 8 ? 0xffu : (nx > 0 ? (1u << nx) - 1u : 0u);
+    const unsigned v = (unsigned)gz * L.stride[0] + (unsigned)gy * L.stride[1] + (unsigned)xb;
+    const int si = (tz * BUILD_TY + ty) * BUILD_TX + 8 * g;             // index inside the staged 8 x 8 x 32 blocks
+
+    // ---- the image copy: the last read of the image block, which the minima overlay (the range test's reads end at its
+    // barrier) ----
+    if (A.img_copy) {
+        if (nx > 0) {
+            const E* src = s_img + ((tz + 1 + cz) * BUILD_HY + (ty + 1 + cy)) * BX + (8 * g + 1 + cx);
+            E* dst = reinterpret_cast<E*>(A.img_copy) + v;
+            if (nx == 8 && (v % (16 / sizeof(E))) == 0) {
+#pragma unroll
+                for (int k = 0; k < (int)(8 * sizeof(E) / 16); ++k) reinterpret_cast<uint4*>(dst)[k] = reinterpret_cast<const uint4*>(src)[k];
+            } else {
+                for (int k = 0; k < nx; ++k) dst[k] = src[k];
+            }
+        }
+        __syncthreads();
+    }
+
+    // ---- t-link inputs ----
+    using PT = typename std::conditional<TIN == 1, float, double>::type;
+    PT p[8];
+    unsigned fgm = 0u, bgm = 0u;                     // bit k: voxel k carries the marker
+    if constexpr (TIN == 1) {
+        const float4 a = reinterpret_cast<const float4*>(s_prob + si * 4)[0], b = reinterpret_cast<const float4*>(s_prob + si * 4)[1];
+        p[0] = a.x; p[1] = a.y; p[2] = a.z; p[3] = a.w; p[4] = b.x; p[5] = b.y; p[6] = b.z; p[7] = b.w;
+        const uint2 f = *reinterpret_cast<const uint2*>(s_fg + si), q = *reinterpret_cast<const uint2*>(s_bg + si);
+        fgm = nonzero_bytes4(f.x) | (nonzero_bytes4(f.y) << 4);
+        bgm = nonzero_bytes4(q.x) | (nonzero_bytes4(q.y) << 4);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            p[k] = 0.0;
+            if (k >= nx) continue;
+            const unsigned vk = v + (unsigned)k;
+            if (A.prob) {
+                if (A.tma_prob) p[k] = A.prob_f64 ? reinterpret_cast<const double*>(s_prob)[si + k] : (double)reinterpret_cast<const float*>(s_prob)[si + k];
+                else p[k] = (A.dbg & 1) ? 0.3 : (A.prob_f64 ? reinterpret_cast<const double*>(A.prob)[vk] : (double)reinterpret_cast<const float*>(A.prob)[vk]);
+            }
+            if (A.fg_bits || A.bg_bits) {
+                if (A.fg_bits) fgm |= ((A.fg_bits[vk >> 5] >> (vk & 31u)) & 1u) << k;
+                if (A.bg_bits) bgm |= ((A.bg_bits[vk >> 5] >> (vk & 31u)) & 1u) << k;
+            } else {
+                if (A.fg && ((A.tma_mark & 1) ? s_fg[si + k] : A.fg[vk])) fgm |= 1u << k;
+                if (A.bg && ((A.tma_mark & 2) ? s_bg[si + k] : A.bg[vk])) bgm |= 1u << k;
+            }
+        }
+    }
+    if (A.prob_copy && nx > 0) {
+        if (TIN == 1 || !A.prob_f64) {
+            float* dst = reinterpret_cast<float*>(A.prob_copy) + v;
+            if (nx == 8 && (v & 3u) == 0) {
+                reinterpret_cast<float4*>(dst)[0] = make_float4((float)p[0], (float)p[1], (float)p[2], (float)p[3]);
+                reinterpret_cast<float4*>(dst)[1] = make_float4((float)p[4], (float)p[5], (float)p[6], (float)p[7]);
+            } else {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) if (k < nx) dst[k] = (float)p[k];
+            }
+        } else {
+            double* dst = reinterpret_cast<double*>(A.prob_copy) + v;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) if (k < nx) dst[k] = (double)p[k];
+        }
+    }
+
+    // ---- t-links and solver state ----
+    const bool own = gz >= L.own0 && gz < L.own1;
+    const unsigned zy = (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) | (gy + 1 < L.dim[1] ? 8u : 0u);
+    const bool f32 = TIN == 1 || A.compute_f32 != 0;
+    unsigned rm_lo = 0u, rm_hi = 0u, sinkm = 0u;
+    bool needs = false, exc = false;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        double tr = 0.0;
+        const unsigned fb = ((fgm >> k) & 1u) | (((bgm >> k) & 1u) << 1);
+        s_mm[(tz * BUILD_TY + ty) * BUILD_TX + ((8 * g + k) ^ ty)] = tlink_replay<double>(tr, has_prob, (double)p[k], f32, A.alpha, fb);
+        const int gx = xb + k;
+        // the in-lattice pairs (every weight of the block is >= DBL_MIN: they are the n-link bits of rmask)
+        const unsigned pr = zy | (gx > 0 ? 16u : 0u) | (gx + 1 < L.dim[2] ? 32u : 0u);
+        const unsigned m = pr | (tr < 0 ? RM_SINK : 0u);
+        if (k < 4) rm_lo |= m << (8 * k); else rm_hi |= m << (8 * (k - 4));
+        if (tr < 0) sinkm |= 1u << k;
+        if ((pin >> k) & 1u) {
+            if (own && pr != 0u && !(tr < 0)) needs = true;        // an arc, and the label is not the sink's 1
+            if (own && source_active(tr, pr)) exc = true;
+        }
+    }
+    if (nx > 0) {
+        const int h_sink = own ? 1 : MGC_HINF;
+        auto h_of = [&](int k) -> int { return ((sinkm >> k) & 1u) ? h_sink : MGC_HINF; };
+        if (nx == 8 && (v & 7u) == 0) {
+            *reinterpret_cast<uint2*>(S.rmask + v) = make_uint2(rm_lo, rm_hi);
+        } else {
+            for (int k = 0; k < nx; ++k) S.rmask[v + k] = (uint8_t)((k < 4 ? rm_lo >> (8 * k) : rm_hi >> (8 * (k - 4))) & 0xffu);
+        }
+        if (nx == 8 && (v & 3u) == 0) {
+            reinterpret_cast<int4*>(S.height + v)[0] = make_int4(h_of(0), h_of(1), h_of(2), h_of(3));
+            reinterpret_cast<int4*>(S.height + v)[1] = make_int4(h_of(4), h_of(5), h_of(6), h_of(7));
+        } else {
+            for (int k = 0; k < nx; ++k) S.height[v + k] = h_of(k);
+        }
+    }
+    // marker bit planes: word (gz, gy) of this block is the bytes of the row's four threads
+    {
+        unsigned wf = (fgm & pin) << (8 * g), wb = (bgm & pin) << (8 * g);
+        wf |= __shfl_xor_sync(0xffffffffu, wf, 1); wb |= __shfl_xor_sync(0xffffffffu, wb, 1);
+        wf |= __shfl_xor_sync(0xffffffffu, wf, 2); wb |= __shfl_xor_sync(0xffffffffu, wb, 2);
+        if (g == 0 && row_in) {
+            const unsigned w = ((unsigned)gz * (unsigned)L.dim[1] + (unsigned)gy) * gridDim.x + blockIdx.x;
+            if (A.fg_plane) A.fg_plane[w] = wf;
+            if (A.bg_plane) A.bg_plane[w] = wb;
+        }
+    }
+    // ---- per solver tile flags: lanes g, g + 4, ... of every warp cover tile g ----
+    const unsigned bn = __ballot_sync(0xffffffffu, needs), be = __ballot_sync(0xffffffffu, exc);
+    if ((tid & 31) == 0) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (bn & (0x11111111u << j)) atomicOr(&s_flags[j], 1);
+            if (be & (0x11111111u << j)) atomicOr(&s_flags[4 + j], 1);
+        }
+    }
+    __syncthreads();
+
+    // ---- the block's add_tweights partial, in k_build_tile's order ----
+    {
+        const int lx = tid & 31, ly = tid >> 5;
+        const bool col_in = y0 + ly < L.dim[1] && x0 + lx < L.dim[2];
+        double msum = 0.0;
+#pragma unroll
+        for (int lz = 0; lz < BUILD_TZ; ++lz) {
+            const int cz2 = z0 + lz;
+            if (col_in && cz2 < L.dim[0] && cz2 >= L.own0 && cz2 < L.own1)
+                msum = __dadd_rn(msum, s_mm[(lz * BUILD_TY + ly) * BUILD_TX + (lx ^ ly)]);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) msum = __dadd_rn(msum, __shfl_down_sync(0xffffffffu, msum, o));
+        double* s_red = reinterpret_cast<double*>(s_scr);
+        if (lx == 0) s_red[ly] = msum;
+        __syncthreads();
+        if (tid == 0) {
+            double t = s_red[0];
+#pragma unroll
+            for (int w = 1; w < 8; ++w) t = __dadd_rn(t, s_red[w]);
+            partials[((A.z_tile0 + (int)blockIdx.z) * (int)gridDim.y + (int)blockIdx.y) * (int)gridDim.x + (int)blockIdx.x] = t;
+        }
+    }
+    if (tid < 4) {
+        const int tx = (x0 >> 3) + tid, tyy = y0 >> 3, tzz = z0 >> 3;
+        if (tx < TL.nt[2] && tyy < TL.nt[1] && tzz < TL.nt[0]) {
+            const int t = (tzz * TL.nt[1] + tyy) * TL.nt[2] + tx;
+            const int any_needs = s_flags[tid], any_exc = s_flags[4 + tid];
+            rflag[t] = any_needs;
+            if (any_needs) rl.items[atomicAdd(rl.count, 1)] = t;
+            pflag[t] = any_exc;
+            A.cmat[t] = 0;
+            if (any_exc) {
+                const WorkList& pl = ((tzz + tyy + tx) & 1) ? pl1 : pl0;
+                pl.items[atomicAdd(pl.count, 1)] = t;
+            }
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -9,6 +9,7 @@
 // on random and adversarial blocks that a block that passes holds no pair whose own test fails.
 #pragma once
 #include <cmath>
+#include <cstring>
 
 #if defined(__CUDACC__)
 #define ER_HD __host__ __device__ __forceinline__
@@ -86,4 +87,30 @@ ER_HD bool block_exp_ordinary(double lo, double hi, bool nan, bool use_max, doub
     if (nan || !(inv_sigma2 > 0.0 && inv_sigma2 < 1e300)) return false;
     const double x = use_max ? fmax(fabs(lo), fabs(hi)) : fabs(er_sub(hi, lo));
     return exp_arg_ordinary(er_mul(er_mul(x, x), inv_sigma2));
+}
+
+// Order-preserving integer key of a float32's bits: key(a) < key(b) as signed ints whenever a < b, -0 just below +0, a
+// positive NaN above +inf and a negative NaN below -inf.  The map is its own inverse.  The float32 block range of the lazy
+// build reduces these keys with integer min / max (one instruction each, and __reduce_min_sync / __reduce_max_sync across
+// a warp) instead of comparing floats and tracking NaN separately.
+ER_HD int er_f32_key(int bits)
+{
+    return bits ^ ((bits >> 31) & 0x7fffffff);
+}
+
+// block_exp_ordinary on the smallest and largest key of a float32 block: the same verdict as the float fold above (lo /
+// hi can differ from it only in the sign of a zero, which neither |hi - lo| nor max(|lo|, |hi|) sees)
+ER_HD bool block_exp_ordinary_keys(int kmin, int kmax, bool use_max, double inv_sigma2)
+{
+    const bool nan = kmax > er_f32_key(0x7f800000) || kmin < er_f32_key((int)0xff800000u);
+    float lo, hi;
+    const int blo = er_f32_key(kmin), bhi = er_f32_key(kmax);
+#if defined(__CUDA_ARCH__)
+    lo = __int_as_float(blo);
+    hi = __int_as_float(bhi);
+#else
+    memcpy(&lo, &blo, 4);
+    memcpy(&hi, &bhi, 4);
+#endif
+    return block_exp_ordinary((double)lo, (double)hi, nan, use_max, inv_sigma2);
 }

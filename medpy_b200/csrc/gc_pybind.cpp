@@ -393,6 +393,7 @@ public:
         d["tiles_deferred"] = s.tiles_deferred; d["tiles_dropped"] = s.tiles_dropped;
         d["relabel_passes"] = s.relabel_passes; d["ms_relabel_first"] = s.ms_relabel_first;
         d["relabel_passes_first"] = s.relabel_passes_first;
+        d["build_blocks_refused"] = s.build_blocks_refused;
         return d;
     }
     // ---- z-slab stepping (device pointers as integers, e.g. torch.Tensor.data_ptr()) ----
