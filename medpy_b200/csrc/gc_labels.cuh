@@ -180,11 +180,17 @@ template <> struct LabIsF32<float> { static const bool v = true; };
 
 __device__ __forceinline__ double lab_floor_min(double w) { return (DBL_MIN > w) ? DBL_MIN : w; }   // max(w, float_info.min); NaN stays
 
-template <typename E>
+// The two maxima differ only on NaN: boundary_stawiaski takes numpy.maximum (NaN if either operand is NaN), the
+// directed term Python's max(a, b) (b only when b > a: a NaN second operand is dropped).
+template <typename E> __device__ __forceinline__ E lab_max_numpy(E a, E b) { return (a != a) ? a : ((b != b || b > a) ? b : a); }
+template <typename E> __device__ __forceinline__ E lab_max_python(E a, E b) { return b > a ? b : a; }
+
+// NUMPY_MAX: the maximum of the two magnitudes as boundary_stawiaski takes it, otherwise as the directed term's probe
+template <typename E, bool NUMPY_MAX>
 __device__ __forceinline__ double lab_weight_native(E a, E b)
 {
     const E va = LabAbs<E>::f(a), vb = LabAbs<E>::f(b);
-    const E val = vb > va ? vb : va;
+    const E val = NUMPY_MAX ? lab_max_numpy<E>(va, vb) : lab_max_python<E>(va, vb);
     if (LabIsF32<E>::v) {
         const float s = __fadd_rn(1.0f, (float)val);
         const float r = __fdiv_rn(1.0f, s);
@@ -198,8 +204,7 @@ __device__ __forceinline__ double lab_weight_native(E a, E b)
 template <typename E>
 __device__ __forceinline__ double lab_weight_pyfloat(E a, E b)
 {
-    const double va = fabs((double)a), vb = fabs((double)b);
-    const double val = vb > va ? vb : va;
+    const double val = lab_max_python<double>(fabs((double)a), fabs((double)b));
     const double r = __ddiv_rn(1.0, __dadd_rn(1.0, val));
     return lab_floor_min(__dmul_rn(r, r));
 }
@@ -226,11 +231,11 @@ __global__ void __launch_bounds__(LAB_BLOCK) k_lab_pair_emit(LabGeom G, const in
     for (unsigned r = 0; r < c; ++r) {
         keys[pos + r] = (lo << 32) | hi;
         if (MODE == 1) {
-            wf[pos + r] = lab_weight_native<E>(grad[p], grad[q]);
+            wf[pos + r] = lab_weight_native<E, true>(grad[p], grad[q]);
         } else if (MODE == 2) {
             const E v1 = grad[p], v2 = grad[q];
             const bool probe = (c == 2u && r == 0u);             // the extra call numpy.vectorize makes on element 0
-            const double w = probe ? lab_weight_native<E>(v1, v2) : lab_weight_pyfloat<E>(v1, v2);
+            const double w = probe ? lab_weight_native<E, false>(v1, v2) : lab_weight_pyfloat<E>(v1, v2);
             const double wb = __dadd_rn(w, beta);
             const double capped = (wb < 1.0) ? wb : 1.0;         // min(1, weight + beta)
             const bool first_gets_beta = dark_to_light ? !(v1 > v2) : (v1 > v2);
