@@ -293,9 +293,8 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
  *   i / j          : C-order int64 ids of lattice neighbours (i != j); cap / rev_cap: contiguous doubles; all four in `mem`
  *                    (host memory is borrowed for the call, device memory is read in place on the handle's stream).
  *   increments     : nonnegative and finite, as the reference's sum_edge asserts.  A zero increment changes nothing and is
- *                    skipped; a call of only zero increments keeps the solved state, mask and energy.  Lowering a
- *                    capacity below the flow it carries would need a reparametrisation the handle cannot check; it is not
- *                    offered.
+ *                    skipped; a call of only zero increments keeps the solved state, mask and energy.  Capacities are
+ *                    lowered by mgc_remove_nweights_warm / mgc_remove_nweights_dense_warm.
  * count == 0 does nothing.  MGC_E_ARG, with the handle unchanged, for an id out of range, a pair that is not a lattice
  * neighbour, a NaN or infinite weight, or bad counts and pointers; MGC_E_WEIGHT, with the handle unchanged, for a negative
  * weight.  Same preconditions, MGC_E_STATE message and behaviour on solved and unsolved handles as mgc_add_tweights_warm.
@@ -309,6 +308,34 @@ int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, cons
  * update of a box only materialises that box's tiles on a lazily built handle.  Same errors, preconditions and behaviour
  * as mgc_add_nweights_warm.  Adding this entry point left MGC_ABI_VERSION at 3. */
 int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd);
+/* The inverse of mgc_add_nweights_warm: n-link capacity taken off a graph and solved warm (a boundary brush undone, a lower
+ * boundary weight, a relaxed boundary along a cut).  The meaning is exactly sum_edge(i[k], j[k], -cap[k], -rev_cap[k]) for
+ * k = 0 .. count-1 in array order: the next maxflow() returns the min cut and the energy of a graph built from scratch
+ * with every call so far replayed and the decrements subtracted from the capacities.  On an unsolved graph that is what
+ * the reference's sum_edge with negated values does.  On a solved one the reference has no defined meaning for a
+ * decrease below the flow an arc carries (BK would run on negative residuals); this definition is an extension of the
+ * library: the excess flow is cancelled and a voxel left short takes the shortfall from its terminal link (Kohli and
+ * Torr's reparametrisation, which lowers the add_tweights constant and keeps the cut of the decreased graph).
+ *   i / j, cap / rev_cap, mem : as in mgc_add_nweights_warm; cap / rev_cap are the DECREMENTS, nonnegative and finite.
+ *   caller's promise          : every arc's capacity stays >= 0.  The handle keeps no per-arc capacity, so it checks the
+ *                               pair: r(i->j) + r(j->i) = c(i->j) + c(j->i) under any flow, and a pair whose total
+ *                               decrement exceeds its residual sum by more than 2^-44 x max(sum, decrement) -- a few
+ *                               hundred roundings of the push updates -- is refused.  Within that tolerance a residual
+ *                               that comes out negative is clamped to 0, so removing exactly the weight that was there is
+ *                               accepted.
+ * count == 0 does nothing.  MGC_E_ARG for an id out of range, a pair that is not a lattice neighbour, a NaN or infinite
+ * decrement, or bad counts and pointers; MGC_E_WEIGHT for a negative decrement or a pair whose decrement exceeds its
+ * residual sum.  Every check finishes before anything is written, and the handle is left unchanged when one fails (an
+ * MGC_OPT_WARM handle that was never solved may have run the init its first solve would run).  Same preconditions,
+ * memory spaces, statistics and MGC_E_STATE message as mgc_add_nweights_warm; z-slab handles and sparse graphs refuse.
+ * Adding this entry point left MGC_ABI_VERSION at 3. */
+int mgc_remove_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
+                             int64_t count, int32_t mem);
+/* The dense form of mgc_remove_nweights_warm, in the layout of mgc_add_nweights_dense_warm: entry p of fwd / bwd holds the
+ * decrements of cap(p -> p+e_axis) and cap(p+e_axis -> p); the last plane of `axis` is ignored and only the pairs with a
+ * nonzero entry are touched.  Same meaning, checks and errors as mgc_remove_nweights_warm.  Adding this entry point left
+ * MGC_ABI_VERSION at 3. */
+int mgc_remove_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd);
 /* Bulk form of the what_segment loop (bin/medpy_graphcut_voxel.py:177-181): out[v] = 0 if the voxel is in
  * the SINK set else 1, C-order over the logical shape.  `mem` selects host or device destination. */
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem);

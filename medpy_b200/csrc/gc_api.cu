@@ -13,6 +13,7 @@
 #include "gc_build.cuh"
 #include "gc_seeds.cuh"
 #include "gc_nlinks.cuh"
+#include "gc_nlinks_remove.cuh"
 #include "gc_gradient.cuh"
 
 #include <algorithm>
@@ -2359,11 +2360,12 @@ int mgc_maxflow(mgc_graph* g, double* energy)
 
 }  // extern "C"
 
-// ---- folds into the residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm / mgc_add_nweights*_warm)
+// ---- folds into the residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm / mgc_add_nweights*_warm /
+// mgc_remove_nweights*_warm)
 // The cub calls of a fold's grouping: the radix sort of its keys (FOLD_SORT_KEYS: the keys alone, FOLD_SORT_PAIRS: keys
 // and call indices, stable; FOLD_SCAN: no sort), then the inclusive sum of the heads.  tmp == nullptr only sizes them:
 // *bytes is the larger scratch size of the two.
-enum { FOLD_SORT_KEYS = 0, FOLD_SORT_PAIRS = 1, FOLD_SCAN = 2 };
+enum { FOLD_SORT_KEYS = 0, FOLD_SORT_PAIRS = 1, FOLD_SCAN = 2, FOLD_SORT_TAILS = 3 };
 template <typename Key>
 static cudaError_t fold_sort(int sort, void* tmp, size_t* bytes, Key* keys, Key* skeys, int* vals, int* svals, int n,
                              int end_bit, cudaStream_t s)
@@ -2389,15 +2391,14 @@ static cudaError_t fold_scan(void* tmp, size_t* bytes, int* head, int* pos, int 
 // on the host from (n, end_bit) and the device; the calls are captured on a capture-only stream of the device (nothing
 // runs) and the kernel nodes of the captured graph counted.  The stream lives for the process and the counts are cached,
 // so a call pays only the capture of a few launches.
-template <typename Key>
-static int fold_cub_launches(mgc_graph* g, int sort, int n, int end_bit, void* tmp, size_t tmp_bytes, Key* keys, Key* skeys,
-                             int* vals, int* svals, int* head, int* pos, int* out)
+// `key` names the calls (device, sort kind, key size, n, end_bit); enqueue(s) issues them on the capture stream s.
+static int cub_launches(mgc_graph* g, const std::tuple<int, int, int, int, int>& key,
+                        const std::function<cudaError_t(cudaStream_t)>& enqueue, int* out)
 {
     static std::mutex mu;
     static std::map<int, cudaStream_t> streams;
     static std::map<std::tuple<int, int, int, int, int>, int> counts;
     std::lock_guard<std::mutex> lock(mu);
-    const auto key = std::make_tuple(g->device, sort, (int)sizeof(Key), n, end_bit);
     auto it = counts.find(key);
     if (it != counts.end()) { *out = it->second; return MGC_OK; }
     cudaStream_t& s = streams[g->device];
@@ -2405,10 +2406,7 @@ static int fold_cub_launches(mgc_graph* g, int sort, int n, int end_bit, void* t
     cudaGraph_t graph = nullptr;
     cudaError_t e = cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed);
     if (e == cudaSuccess) {
-        size_t tb = tmp_bytes;
-        cudaError_t e1 = fold_sort(sort, tmp, &tb, keys, skeys, vals, svals, n, end_bit, s);
-        tb = tmp_bytes;
-        cudaError_t e2 = e1 == cudaSuccess ? fold_scan(tmp, &tb, head, pos, n, s) : e1;
+        const cudaError_t e2 = enqueue(s);
         e = cudaStreamEndCapture(s, &graph);
         if (e == cudaSuccess) e = e2;
     }
@@ -2430,6 +2428,35 @@ static int fold_cub_launches(mgc_graph* g, int sort, int n, int end_bit, void* t
     return MGC_OK;
 }
 
+template <typename Key>
+static int fold_cub_launches(mgc_graph* g, int sort, int n, int end_bit, void* tmp, size_t tmp_bytes, Key* keys, Key* skeys,
+                             int* vals, int* svals, int* head, int* pos, int* out)
+{
+    return cub_launches(g, std::make_tuple(g->device, sort, (int)sizeof(Key), n, end_bit), [&](cudaStream_t s) {
+        size_t tb = tmp_bytes;
+        const cudaError_t e1 = fold_sort(sort, tmp, &tb, keys, skeys, vals, svals, n, end_bit, s);
+        tb = tmp_bytes;
+        return e1 == cudaSuccess ? fold_scan(tmp, &tb, head, pos, n, s) : e1;
+    }, out);
+}
+
+// The tail list of an n-link decrement fold in ascending voxel order: the first *ntails of `count` slots hold the listed
+// tails in the order the atomics gave them, the rest 0xffffffff; sorted on the bits below `end_bit`, which put every voxel
+// id below the fill.  tmp == nullptr only sizes the sort (*bytes).
+static cudaError_t tails_sort(void* tmp, size_t* bytes, const unsigned* tails, unsigned* stails, int count, int end_bit,
+                              cudaStream_t s)
+{
+    return cub::DeviceRadixSort::SortKeys(tmp, *bytes, tails, stails, count, 0, end_bit, s);
+}
+
+// bits of a tails_sort key: the smallest end_bit with n < 2^end_bit, so every voxel id is below 2^end_bit - 1, the fill
+static int tails_end_bit(unsigned n)
+{
+    int b = 1;
+    while (b < 32 && ((unsigned long long)n >> b) != 0ull) ++b;
+    return b;
+}
+
 // preconditions of every fold into the residual state: the copies of the lazy fused build are what the fold reads, or
 // (MGC_OPT_WARM, *eager = true) the residual source capacities the first solve records in tr on any other tile-solver handle
 static int warm_check(mgc_graph* g, bool* eager)
@@ -2444,10 +2471,12 @@ static int warm_check(mgc_graph* g, bool* eager)
 
 // The steps of a fold after its grouping (fold_run).  The grouping was enqueued after ev_fold[0] and left d_ctl = [item
 // count | FOLD_ERR_* bits | touched-tile count] and the touched tiles in `tiles`; fold(grid, n_items) enqueues the fold
-// kernel, which stores one partial of the add_tweights constant per block.  `nonfinite` is the message of
-// FOLD_ERR_NONFINITE, which names the kind of weight.
-static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<void(unsigned, int)>& fold,
-                      const char* nonfinite)
+// kernel, which stores one partial of the add_tweights constant per block.  `nonfinite` and `negative` are the messages of
+// FOLD_ERR_NONFINITE and FOLD_ERR_NEGATIVE, which name the kind of weight.  check (optional) enqueues a check of the calls
+// against the current state that may set FOLD_ERR_PAIRSUM in d_ctl[1]; it runs after the first read-back, before anything
+// is claimed or written, and its bits come back in a second read-back (only the folds that have one pay for it).
+static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<int(unsigned, int)>& fold,
+                      const char* nonfinite, const char* negative, const std::function<int()>* check)
 {
     CK(cudaEventRecord(g->ev_fold[1], g->stream));
     // the item count and the error bits in one synchronisation, before the claim and the fold are enqueued
@@ -2457,8 +2486,7 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     if (h_ctl[1] & FOLD_ERR_RANGE) FAIL(MGC_E_ARG, "node id out of range");
     if (h_ctl[1] & FOLD_ERR_PAIR) FAIL(MGC_E_ARG, "node ids are not lattice neighbours");
     if (h_ctl[1] & FOLD_ERR_NONFINITE) FAIL(MGC_E_ARG, nonfinite);
-    if (h_ctl[1] & FOLD_ERR_NEGATIVE)
-        FAIL(MGC_E_WEIGHT, "negative n-link weights are not allowed (a warm fold only raises capacities)");
+    if (h_ctl[1] & FOLD_ERR_NEGATIVE) FAIL(MGC_E_WEIGHT, negative);
     const int ni = h_ctl[0];
     if (ni == 0) return MGC_OK;                // only add_tweights(v, 0, 0) calls: the state, mask and energy stay
     const bool eager = !g->lazy_built;         // MGC_OPT_WARM handle (warm_check passed)
@@ -2467,6 +2495,17 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
         // same representation as after a solve
         int rc = warm_prepare(g);
         if (rc) return rc;
+    }
+    if (check) {
+        // the check reads the state warm_prepare left (the init a first solve runs anyway) and writes nothing
+        int rc = (*check)();
+        if (rc) return rc;
+        int bits = 0;
+        CK(cudaMemcpyAsync(&bits, d_ctl + 1, sizeof(int), cudaMemcpyDeviceToHost, g->stream));
+        CK(cudaStreamSynchronize(g->stream));
+        if (bits & FOLD_ERR_PAIRSUM)
+            FAIL(MGC_E_WEIGHT, "an n-link decrement exceeds what its arc pair holds: r(i->j) + r(j->i), which equals "
+                               "c(i->j) + c(j->i), is below cap + rev_cap");
     }
     CK(cudaEventRecord(g->ev_fold[2], g->stream));
     // 1. every touched voxel's tile (and its face neighbours) holds cap[], tr, excess and the sink-link state from here on
@@ -2485,7 +2524,7 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     // 2. the fold, its change of the add_tweights constant summed in a fixed order into flow_const
     unsigned grid = (unsigned)((ni + 255) / 256);
     if (grid > REDUCE_BLOCKS) grid = REDUCE_BLOCKS;
-    fold(grid, ni);
+    { int rc = fold(grid, ni); if (rc) return rc; }
     k_sum_partials<<<1, 256, 0, g->stream>>>(g->partials, grid, g->d_scalars);
     // 3. solver state for the next solve: fresh push lists over every materialised tile with excess (every tile of an
     // eager handle; TL.ntiles is the 4-D tile count on a 4-D handle); labels from a full relabel reset (sweep_mode = -1: a
@@ -2526,6 +2565,7 @@ struct FoldCall {
     const char* range;            // NVTX range
     const char* bad;              // MGC_E_ARG message of malformed arrays or counts (nullptr: well formed)
     const char* too_many;         // MGC_E_ARG message of more than 2^31 - 1 calls
+    const char* negative;         // MGC_E_WEIGHT message of a negative n-link weight
     int64_t count;                // calls: seed ids, add_tweights or sum_edge calls, or dense entries
     int32_t mem;                  // memory space of in[]
     bool dense;                   // one entry per voxel (count == the voxel count)
@@ -2535,6 +2575,7 @@ struct FoldCall {
     int sort;                     // FOLD_SORT_KEYS / FOLD_SORT_PAIRS / FOLD_SCAN
     int key_shift;                // a key is voxel << key_shift | low bits: it has the bits of n << key_shift - 1
     int axis;                     // k_nlinks_items: the axis of the dense form
+    bool item_flows;              // one double per item for the fold (n-link decrements: the excess change of an arc)
 };
 
 // The device buffers of a fold in fold_buf, 16-byte aligned pieces in this order
@@ -2553,7 +2594,10 @@ struct FoldBufs {
     Item* items;
     unsigned* tbits;              // n-links: per-voxel tail bits, and the tails for the re-clamp
     unsigned* tails;
+    double* dx;                   // item_flows: one double per item
+    unsigned* stails;             // item_flows: the tails in ascending order (tails_sort)
     void* tmp;                    // cub scratch
+    size_t tmp_bytes;
 };
 
 // A bump allocator of 16-byte aligned pieces over one buffer; base == nullptr only measures the pieces
@@ -2571,9 +2615,10 @@ struct Bump {
 
 // A fold: the checks, the grouping of the calls into items on the device, then fold_items.  An item of NlinkItem names an
 // arc: both ends are listed for the claim and its tails re-clamped.  group(b, grid) enqueues the keys, the sort
-// (fold_sort) and the heads of the calls; fold(b, grid, n_items) the fold kernel(s).
-template <typename Key, typename Item, typename Group, typename Fold>
-static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold)
+// (fold_sort) and the heads of the calls; fold(b, grid, n_items) the fold kernel(s); check(b, eager) (optional) the check
+// fold_items runs before the claim.
+template <typename Key, typename Item, typename Group, typename Fold, typename Check = std::nullptr_t>
+static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold, Check&& check = nullptr)
 {
     constexpr bool arcs = std::is_same<Item, NlinkItem>::value;
     if (!g) return MGC_E_ARG;
@@ -2598,6 +2643,13 @@ static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold)
         size_t tmp_bytes = 0;
         CK(fold_sort(c.sort, nullptr, &tmp_bytes, (Key*)nullptr, (Key*)nullptr, nullptr, nullptr, n, end_bit, g->stream));
         CK(fold_scan(nullptr, &tmp_bytes, nullptr, nullptr, n, g->stream));
+        if (c.item_flows) {
+            // the largest tail sort the fold can need (tails_sort; fold_run's callers size it again before the sort)
+            size_t tb = 0;
+            CK(tails_sort(nullptr, &tb, nullptr, nullptr, (int)std::min(2 * (size_t)n, (size_t)g->L.n),
+                          tails_end_bit(g->L.n), g->stream));
+            tmp_bytes = std::max(tmp_bytes, tb);
+        }
         // no host slots for device inputs, no keys or call indices in a dense form, no tiles on an eager handle (nothing
         // to claim), no tails but for n-links
         const bool host = c.mem == MGC_MEM_HOST;
@@ -2623,7 +2675,10 @@ static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold)
             b.items = m.take<Item>(n);
             b.tbits = m.take<unsigned>(nbits);
             b.tails = m.take<unsigned>(ntails);
+            b.dx = m.take<double>(c.item_flows ? (size_t)n : 0);
+            b.stails = m.take<unsigned>(c.item_flows ? ntails : 0);
             b.tmp = m.take<char>(tmp_bytes);
+            b.tmp_bytes = tmp_bytes;
             return m.used;
         };
         rc = ensure_scratch(g, g->fold_buf, layout(Bump{nullptr, 0}));
@@ -2659,8 +2714,16 @@ static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold)
                                                            b.ctl);
         g->st.kernel_launches += (c.sort == FOLD_SCAN ? 2 : 3) + cub_launches;
         CK(cudaGetLastError());
-        rc = fold_items(g, b.ctl, b.tiles, [&](unsigned grid, int ni) { fold(b, eager, grid, ni); },
-                        arcs ? "an n-link weight is NaN or infinite" : "a t-link weight is NaN or infinite");
+        std::function<int()> chk;
+        if constexpr (!std::is_same<std::decay_t<Check>, std::nullptr_t>::value) chk = [&]() { return check(b, eager); };
+        auto fold_call = [&](unsigned grid, int ni) -> int {
+            if constexpr (std::is_void<decltype(fold(b, eager, grid, ni))>::value) { fold(b, eager, grid, ni); return MGC_OK; }
+            else return fold(b, eager, grid, ni);
+        };
+        rc = fold_items(g, b.ctl, b.tiles, fold_call,
+                        arcs ? "an n-link weight is NaN or infinite" : "a t-link weight is NaN or infinite",
+                        c.negative ? c.negative : "negative n-link weights are not allowed (a warm fold only raises capacities)",
+                        chk ? &chk : nullptr);
     }
     if (c.arrays[0]) slots_release(g, 3u);     // the grouping and the fold read the staging slots
     return rc;
@@ -2754,34 +2817,42 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
 // sum_edge(ii[k], jj[k], cap[k], rev[k]) with every array in `mem`: (arc key, call index) pairs, key = lo << 2 | axis,
 // stably sorted, then run-length encoded.  ii == nullptr: the dense form along canonical axis `axis`, entry p of the
 // staged cap / rev (count = the voxel count) holds the increments of p -> p + e_axis and back; the pairs with a nonzero
-// increment are compacted by a scan of their flags.
+// increment are compacted by a scan of their flags.  The grouping is the same for increments and decrements
+// (nweights_group); only the fold differs.
+using NlinkBufs = FoldBufs<unsigned long long, NlinkItem>;
+
+static int nweights_group(mgc_graph* g, const FoldCall& c, const NlinkBufs& b, unsigned kgrid,
+                          const std::function<cudaError_t()>& sort)
+{
+    const int axis = c.axis;
+    const int n = (int)c.count;
+    const double* d_cap = (const double*)b.in[2];
+    const double* d_rev = (const double*)b.in[3];
+    if (c.dense) {
+        const unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
+        const unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
+        k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap, d_rev,
+                                                           b.head, b.ctl + 1);
+        return MGC_OK;
+    }
+    const int64_t* d_i = (const int64_t*)b.in[0];
+    const int64_t* d_j = (const int64_t*)b.in[1];
+    if (g->nd == 4) k_nlinks_keys<4><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
+    else            k_nlinks_keys<3><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
+    CK(sort());
+    k_weighted_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_cap, d_rev, n, b.head);
+    return MGC_OK;
+}
+
 static int nweights_fold(mgc_graph* g, FoldCall& c, int axis)
 {
     const bool dense = c.dense;
     c.sort = dense ? FOLD_SCAN : FOLD_SORT_PAIRS;
     c.key_shift = 2;
     c.axis = axis;
-    const int n = (int)c.count;
     return fold_run<unsigned long long, NlinkItem>(g, c,
-        [&](const FoldBufs<unsigned long long, NlinkItem>& b, unsigned kgrid, auto sort) {
-            const double* d_cap = (const double*)b.in[2];
-            const double* d_rev = (const double*)b.in[3];
-            if (dense) {
-                const unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
-                const unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
-                k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap,
-                                                                   d_rev, b.head, b.ctl + 1);
-                return MGC_OK;
-            }
-            const int64_t* d_i = (const int64_t*)b.in[0];
-            const int64_t* d_j = (const int64_t*)b.in[1];
-            if (g->nd == 4) k_nlinks_keys<4><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
-            else            k_nlinks_keys<3><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
-            CK(sort());
-            k_weighted_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_cap, d_rev, n, b.head);
-            return MGC_OK;
-        },
-        [&](const FoldBufs<unsigned long long, NlinkItem>& b, bool eager, unsigned grid, int ni) {
+        [&](const NlinkBufs& b, unsigned kgrid, auto sort) { return nweights_group(g, c, b, kgrid, sort); },
+        [&](const NlinkBufs& b, bool eager, unsigned grid, int ni) {
             // the arcs first, then each tail once: the re-clamp reads the out-capacity after every increment of the call
             const int* order = dense ? nullptr : b.svals;
             const int64_t* ids = dense ? nullptr : (const int64_t*)b.in[0];
@@ -2797,11 +2868,77 @@ static int nweights_fold(mgc_graph* g, FoldCall& c, int axis)
         });
 }
 
-int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
-                          int64_t count, int32_t mem)
+// sum_edge calls with negated weights (gc_nlinks_remove.cuh): the grouping of nweights_fold, the pair check before the
+// claim, then the arcs (one excess change per item in dx) and each endpoint once.
+static int nweights_remove_fold(mgc_graph* g, FoldCall& c, int axis)
 {
-    FoldCall c{};
-    c.range = "mgc:add_nweights_warm";
+    const bool dense = c.dense;
+    c.sort = dense ? FOLD_SCAN : FOLD_SORT_PAIRS;
+    c.key_shift = 2;
+    c.axis = axis;
+    c.negative = "negative n-link decrements are not allowed (a removal takes nonnegative amounts off the capacities)";
+    c.item_flows = true;
+    const int n = (int)c.count;
+    auto calls = [&](const NlinkBufs& b, const int*& order, const int64_t*& ids) {
+        order = dense ? nullptr : b.svals;
+        ids = dense ? nullptr : (const int64_t*)b.in[0];
+    };
+    return fold_run<unsigned long long, NlinkItem>(g, c,
+        [&](const NlinkBufs& b, unsigned kgrid, auto sort) { return nweights_group(g, c, b, kgrid, sort); },
+        [&](const NlinkBufs& b, bool eager, unsigned grid, int ni) -> int {
+            const int* order; const int64_t* ids;
+            calls(b, order, ids);
+            const double* d_cap = (const double*)b.in[2];
+            const double* d_rev = (const double*)b.in[3];
+            int* ntails = b.ctl + 3;
+            // the tails are listed in atomic order; they are sorted before the voxel pass, so each one lands in the same
+            // thread and block on every run and the per-block sums of the constant are reproducible
+            const int nt = (int)std::min(2 * (int64_t)ni, (int64_t)g->L.n);
+            const int tbit = tails_end_bit(g->L.n);
+            CK(cudaMemsetAsync(b.tails, 0xff, (size_t)nt * sizeof(unsigned), g->stream));
+            if (g->nd == 4) k_nlinks_remove_arcs<4><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.dx, b.tbits, b.tails, ntails);
+            else            k_nlinks_remove_arcs<3><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.dx, b.tbits, b.tails, ntails);
+            g->st.kernel_launches++;
+            size_t tb = 0;
+            CK(tails_sort(nullptr, &tb, b.tails, b.stails, nt, tbit, g->stream));
+            if (tb > b.tmp_bytes) FAIL(MGC_E_CUDA, "the tail sort needs more scratch than was sized");
+            int sort_launches = 0;
+            int rc = cub_launches(g, std::make_tuple(g->device, (int)FOLD_SORT_TAILS, 4, nt, tbit), [&](cudaStream_t s) {
+                size_t t = b.tmp_bytes;
+                return tails_sort(b.tmp, &t, b.tails, b.stails, nt, tbit, s);
+            }, &sort_launches);
+            if (rc) return rc;
+            tb = b.tmp_bytes;
+            CK(tails_sort(b.tmp, &tb, b.tails, b.stails, nt, tbit, g->stream));
+            g->st.kernel_launches += sort_launches;
+            const unsigned long long* skeys = dense ? nullptr : b.skeys;
+            residual_dispatch(g, eager, [&](auto A) {
+                k_nlinks_remove_voxels<<<grid, 256, 0, g->stream>>>(A, g->L, skeys, b.head, b.pos, n, axis, b.dx, b.stails,
+                                                                    ntails, g->partials);
+            });
+            return MGC_OK;
+        },
+        [&](const NlinkBufs& b, bool eager) {
+            // after the first read-back: the item count is on the device in b.ctl[0]
+            const int* order; const int64_t* ids;
+            calls(b, order, ids);
+            const int* cmat = eager || !g->caps_lazy ? nullptr : g->cmat;
+            unsigned grid = (unsigned)std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)g->n_ctas * 8);
+            residual_dispatch(g, eager, [&](auto A) {
+                k_nlinks_remove_check<<<grid, 256, 0, g->stream>>>(A, g->L, g->TL, cmat, b.items, b.ctl, order, ids,
+                                                                   (const double*)b.in[2], (const double*)b.in[3],
+                                                                   b.ctl + 1);
+            });
+            g->st.kernel_launches++;
+            CK(cudaGetLastError());
+            return MGC_OK;
+        });
+}
+
+static void nweights_list_call(FoldCall& c, const char* range, const int64_t* i, const int64_t* j, const double* cap,
+                               const double* rev_cap, int64_t count, int32_t mem)
+{
+    c.range = range;
     c.bad = count < 0 || (count && (!i || !j || !cap || !rev_cap)) ? "bad n-link arrays" : nullptr;
     c.too_many = "more than 2^31 - 1 sum_edge calls in one call";
     c.count = count;
@@ -2810,22 +2947,53 @@ int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, cons
     c.in[1] = j; c.in_n[1] = count;
     c.in[2] = cap; c.in_n[2] = count;
     c.in[3] = rev_cap; c.in_n[3] = count;
-    return nweights_fold(g, c, 0);
 }
 
-int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
+static int nweights_dense_call(mgc_graph* g, FoldCall& c, const char* range, int32_t axis, const mgc_array* fwd,
+                               const mgc_array* bwd)
 {
     if (!g || !fwd || !bwd) return MGC_E_ARG;
     if (axis < 0 || axis >= g->user_ndim) FAIL(MGC_E_ARG, "bad axis");
     if (fwd->dtype != MGC_F64 || bwd->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense n-weights must be float64");
-    FoldCall c{};
-    c.range = "mgc:add_nweights_dense_warm";
+    c.range = range;
     c.count = (int64_t)g->L.n;
     c.mem = MGC_MEM_DEVICE;
     c.dense = true;
     c.arrays[0] = fwd;
     c.arrays[1] = bwd;
+    return MGC_OK;
+}
+
+int mgc_add_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
+                          int64_t count, int32_t mem)
+{
+    FoldCall c{};
+    nweights_list_call(c, "mgc:add_nweights_warm", i, j, cap, rev_cap, count, mem);
+    return nweights_fold(g, c, 0);
+}
+
+int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
+{
+    FoldCall c{};
+    int rc = nweights_dense_call(g, c, "mgc:add_nweights_dense_warm", axis, fwd, bwd);
+    if (rc) return rc;
     return nweights_fold(g, c, axis + g->shift);
+}
+
+int mgc_remove_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
+                             int64_t count, int32_t mem)
+{
+    FoldCall c{};
+    nweights_list_call(c, "mgc:remove_nweights_warm", i, j, cap, rev_cap, count, mem);
+    return nweights_remove_fold(g, c, 0);
+}
+
+int mgc_remove_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
+{
+    FoldCall c{};
+    int rc = nweights_dense_call(g, c, "mgc:remove_nweights_dense_warm", axis, fwd, bwd);
+    if (rc) return rc;
+    return nweights_remove_fold(g, c, axis + g->shift);
 }
 
 int mgc_get_mask(mgc_graph* g, uint8_t* out, int32_t mem)

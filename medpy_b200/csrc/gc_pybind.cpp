@@ -312,6 +312,16 @@ public:
     // float64 of the same length, all four on the host or all on the device
     void add_nweights_warm(const py::object& i, const py::object& j, const py::object& cap, const py::object& rev)
     {
+        fold_nweights(i, j, cap, rev, mgc_add_nweights_warm);
+    }
+    // the same with the decrements of mgc_remove_nweights_warm
+    void remove_nweights_warm(const py::object& i, const py::object& j, const py::object& cap, const py::object& rev)
+    {
+        fold_nweights(i, j, cap, rev, mgc_remove_nweights_warm);
+    }
+    void fold_nweights(const py::object& i, const py::object& j, const py::object& cap, const py::object& rev,
+                       int (*fold)(mgc_graph*, const int64_t*, const int64_t*, const double*, const double*, int64_t, int32_t))
+    {
         Vec a = vec_of<int64_t>(i, "i8", "i"), b = vec_of<int64_t>(j, "i8", "j");
         Vec c = vec_of<double>(cap, "f8", "cap"), r = vec_of<double>(rev, "f8", "rev_cap");
         if (a.mem < 0 || b.mem < 0 || c.mem < 0 || r.mem < 0) throw py::value_error("i, j, cap and rev_cap are required");
@@ -322,19 +332,28 @@ public:
         int rc;
         {
             py::gil_scoped_release rel;
-            rc = mgc_add_nweights_warm(g_, (const int64_t*)a.p, (const int64_t*)b.p, (const double*)c.p, (const double*)r.p,
-                                       a.n, a.mem);
+            rc = fold(g_, (const int64_t*)a.p, (const int64_t*)b.p, (const double*)c.p, (const double*)r.p, a.n, a.mem);
         }
         check(rc, g_);
     }
-    // the dense form (mgc_add_nweights_dense_warm): fwd / bwd float64 arrays of the lattice shape
+    // the dense forms (mgc_add_nweights_dense_warm / mgc_remove_nweights_dense_warm): fwd / bwd float64 arrays of the
+    // lattice shape
     void add_nweights_dense_warm(int axis, const py::object& fwd, const py::object& bwd)
+    {
+        fold_nweights_dense(axis, fwd, bwd, mgc_add_nweights_dense_warm);
+    }
+    void remove_nweights_dense_warm(int axis, const py::object& fwd, const py::object& bwd)
+    {
+        fold_nweights_dense(axis, fwd, bwd, mgc_remove_nweights_dense_warm);
+    }
+    void fold_nweights_dense(int axis, const py::object& fwd, const py::object& bwd,
+                             int (*fold)(mgc_graph*, int32_t, const mgc_array*, const mgc_array*))
     {
         ArrayRef a = make_ref(fwd, MGC_F64, "fwd"), b = make_ref(bwd, MGC_F64, "bwd");
         check_shape(a, "fwd"); check_shape(b, "bwd");
         check_inputs();
         int rc;
-        { py::gil_scoped_release rel; rc = mgc_add_nweights_dense_warm(g_, axis, &a.a, &b.a); }
+        { py::gil_scoped_release rel; rc = fold(g_, axis, &a.a, &b.a); }
         check(rc, g_);
     }
     double maxflow()
@@ -760,6 +779,8 @@ PYBIND11_MODULE(_mgc, m)
         .def("add_tweights_warm", &PyGraph::add_tweights_warm, py::arg("ids"), py::arg("src"), py::arg("snk"))
         .def("add_nweights_warm", &PyGraph::add_nweights_warm, py::arg("i"), py::arg("j"), py::arg("cap"), py::arg("rev_cap"))
         .def("add_nweights_dense_warm", &PyGraph::add_nweights_dense_warm, py::arg("axis"), py::arg("fwd"), py::arg("bwd"))
+        .def("remove_nweights_warm", &PyGraph::remove_nweights_warm, py::arg("i"), py::arg("j"), py::arg("cap"), py::arg("rev_cap"))
+        .def("remove_nweights_dense_warm", &PyGraph::remove_nweights_dense_warm, py::arg("axis"), py::arg("fwd"), py::arg("bwd"))
         .def("build_voxel_graph", &PyGraph::build_voxel_graph)
         .def_static("slab_comm_unique_id", &PyGraph::slab_comm_unique_id)
         .def("slab_comm_init", &PyGraph::slab_comm_init)

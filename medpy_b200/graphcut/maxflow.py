@@ -79,6 +79,9 @@ class GraphDouble:
         self._lazy = None
         self._fresh = True
         self._solved = False     # maxflow() ran since the last reset: add_seeds folds into the residual state
+        # a removal folded into the handle before the first maxflow(): the terms are fixed from then on, and the warm
+        # calls fold natively as on a solved graph
+        self._folded = False
         if sparse:
             if self._journal is None:
                 raise ValueError("a lattice shape and sparse=True exclude each other")
@@ -209,6 +212,7 @@ class GraphDouble:
 
     def stage_tweights_many(self, ids, cap_source, cap_sink):
         """add_tweights(v, cap_source, cap_sink) for every v in ids, in order (ids already range-checked)."""
+        self._terms_open()
         ids = numpy.asarray(ids, dtype=numpy.int64)
         if self._sp is not None:
             return self._sp.stage_tweights_many(ids, cap_source, cap_sink)
@@ -253,6 +257,7 @@ class GraphDouble:
             self._journal = None
 
     def add_regional_probability(self, prob, alpha, compute_f32):
+        self._terms_open()
         self._lattice_term()
         self._dirty()
         if self._collect("reg", (self._positive_strides(prob), float(alpha), bool(compute_f32))):
@@ -263,6 +268,7 @@ class GraphDouble:
 
     def add_tweights_dense(self, src, snk):
         """add_tweights(v, src[v], snk[v]) for every node (GCGraph.set_tweights_all, graph.py:532-552)."""
+        self._terms_open()
         if self._sp is not None:
             return self._sp.add_tweights_bulk(None, numpy.ravel(src), numpy.ravel(snk))
         src = numpy.ascontiguousarray(src, dtype=numpy.float64).reshape(self._shape)
@@ -291,6 +297,7 @@ class GraphDouble:
         return a
 
     def add_markers(self, fg, bg):
+        self._terms_open()
         self._lattice_term()
         self._dirty()
         if self._lazy and "mark" not in self._lazy and self._collect("mark", (self._positive_strides(fg), self._positive_strides(bg))):
@@ -300,6 +307,7 @@ class GraphDouble:
         self._nat().add_markers(self._positive_strides(fg), self._positive_strides(bg))
 
     def add_boundary(self, kind, image, sigma, spacing, norm):
+        self._terms_open()
         self._lattice_term()
         self._dirty()
         if self._collect("bnd", (int(kind), self._positive_strides(image), float(sigma), spacing, float(norm))):
@@ -309,6 +317,7 @@ class GraphDouble:
         self._nat().add_boundary(int(kind), self._positive_strides(image), float(sigma), spacing, float(norm))
 
     def add_nweights_dense(self, axis, fwd, bwd):
+        self._terms_open()
         self._lattice_term()
         self._flush()
         self._dirty()
@@ -323,6 +332,7 @@ class GraphDouble:
     def add_tweights(self, i, cap_source, cap_sink):
         """graph.h:415-425, staged: calls on distinct nodes are batched into one dense device pass.  A solved graph
         refuses it; ``add_tweights_warm`` is the warm form, which folds the calls into the solved state."""
+        self._terms_open()
         i = int(i)
         if i < 0 or i >= self._n:
             raise ValueError("Invalid node id of {}. Valid values are 0 to {}.".format(i, self._n - 1))
@@ -353,6 +363,7 @@ class GraphDouble:
 
     def sum_edge(self, i, j, cap, rev_cap):
         """graph.h:456-480 for lattice neighbours (accumulating)."""
+        self._terms_open()
         i, j = int(i), int(j)
         if i < 0 or j < 0 or i >= self._n or j >= self._n or i == j:
             raise ValueError("invalid node ids ({}, {})".format(i, j))
@@ -477,7 +488,7 @@ class GraphDouble:
 
     def _fold_seeds(self, fg, bg, cap, native, rebuild):
         fg_ids, bg_ids = self._seed_ids(fg), self._seed_ids(bg)
-        if not self._solved:
+        if not self._solved and not self._folded:
             for ids, src, snk in ((fg_ids, cap, 0.0), (bg_ids, 0.0, cap)):
                 if ids is not None and len(ids):
                     if not isinstance(ids, numpy.ndarray):
@@ -514,7 +525,7 @@ class GraphDouble:
         m = self._n if ids is None else int(ids.shape[0])
         src = self._warm_weights(cap_source, m, ids is None, cuda, "cap_source")
         snk = self._warm_weights(cap_sink, m, ids is None, cuda, "cap_sink")
-        if not self._solved:
+        if not self._solved and not self._folded:
             if cuda:
                 ids = None if ids is None else ids.cpu().numpy()
                 src, snk = src.cpu().numpy(), snk.cpu().numpy()
@@ -580,6 +591,21 @@ class GraphDouble:
         Before the first ``maxflow()`` the calls are staged exactly like ``sum_edge``.  After it they are folded into the
         solved state on the graphs ``add_tweights_warm`` folds into (mgc_add_nweights_warm); any other solved graph raises
         ``RuntimeError``: ``reset()`` it and build the graph again with the calls."""
+        ii, jj, c, r, cuda = self._nweights_call_args(i, j, cap, rev_cap)
+        if not self._solved and not self._folded:
+            if cuda:
+                ii, jj, c, r = (x.cpu().numpy() for x in (ii, jj, c, r))
+            self._stage_nweights_calls(ii, jj, c, r)
+            return
+        if self._sp is not None:
+            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
+                               "rebuild it with the n-link calls instead")
+        self._dirty()
+        self._nat().add_nweights_warm(ii, jj, c, r)
+
+    def _nweights_call_args(self, i, j, cap, rev_cap):
+        """The arguments of add_nweights_warm / remove_nweights_warm as four contiguous 1-D arrays of one length (int64
+        ids, float64 weights; numpy, or CUDA tensors when any argument is one), and whether they are on the device."""
         cuda = any(hasattr(x, "__cuda_array_interface__") for x in (i, j, cap, rev_cap))
         ii, jj = self._pair_ids(i, cuda, "i"), self._pair_ids(j, cuda, "j")
         sizes = {int(x.shape[0]) for x in (ii, jj) if x.ndim}
@@ -593,16 +619,7 @@ class GraphDouble:
         ii, jj = ((x.contiguous() if cuda else numpy.ascontiguousarray(x)) for x in (ii, jj))
         c = self._warm_weights(cap, m, False, cuda, "cap")
         r = self._warm_weights(rev_cap, m, False, cuda, "rev_cap")
-        if not self._solved:
-            if cuda:
-                ii, jj, c, r = (x.cpu().numpy() for x in (ii, jj, c, r))
-            self._stage_nweights_calls(ii, jj, c, r)
-            return
-        if self._sp is not None:
-            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it with the n-link calls instead")
-        self._dirty()
-        self._nat().add_nweights_warm(ii, jj, c, r)
+        return ii, jj, c, r, cuda
 
     def add_nweights_dense_warm(self, axis, fwd, bwd):
         """The dense form of ``add_nweights_warm``, in the layout of ``add_nweights_dense``: ``fwd`` / ``bwd`` have the
@@ -613,6 +630,29 @@ class GraphDouble:
 
         Before the first ``maxflow()`` the call is staged exactly like ``add_nweights_dense``.  After it, the same graphs
         as ``add_nweights_warm`` fold it into the solved state (mgc_add_nweights_dense_warm)."""
+        axis, fwd, bwd, cuda = self._dense_nweights_args(axis, fwd, bwd)
+        if not self._solved and not self._folded:
+            if cuda:
+                fwd, bwd = fwd.cpu().numpy(), bwd.cpu().numpy()
+            cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
+            for w, what in ((fwd, "fwd"), (bwd, "bwd")):
+                if not numpy.isfinite(w[cut]).all():
+                    raise ValueError("{} holds NaN or infinite values".format(what))
+                if (w[cut] < 0).any():
+                    raise ValueError("{} holds negative values: a warm n-link edit only raises capacities".format(what))
+            staged = [numpy.zeros(self._shape), numpy.zeros(self._shape)]
+            staged[0][cut], staged[1][cut] = fwd[cut], bwd[cut]        # the last plane of `axis` names no pair
+            self.add_nweights_dense(axis, *staged)
+            return
+        if self._sp is not None:
+            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
+                               "rebuild it with the n-link calls instead")
+        self._dirty()
+        self._nat().add_nweights_dense_warm(axis, fwd, bwd)
+
+    def _dense_nweights_args(self, axis, fwd, bwd):
+        """The arguments of the dense n-link folds: the axis, checked, and fwd / bwd as float64 arrays of the lattice shape
+        (numpy, or CUDA tensors when either is one), and whether they are on the device."""
         axis = int(axis)
         if not 0 <= axis < len(self._shape):
             raise ValueError("axis {} is out of range for a graph of shape {}".format(axis, self._shape))
@@ -635,25 +675,79 @@ class GraphDouble:
             if tuple(t.shape) != self._shape:
                 raise ValueError("{} of shape {} does not match the graph's shape {}".format(what, tuple(t.shape), self._shape))
             arrs.append(t)
-        fwd, bwd = arrs
-        if not self._solved:
-            if cuda:
-                fwd, bwd = fwd.cpu().numpy(), bwd.cpu().numpy()
+        return (axis,) + tuple(arrs) + (cuda,)
+
+    def remove_nweights_warm(self, i, j, cap, rev_cap):
+        """The inverse of ``add_nweights_warm``: n-link capacity taken off the graph, re-solved warm by the next
+        ``maxflow()`` -- a boundary brush undone, a lower boundary weight, a boundary relaxed along a cut.
+
+        Exactly ``sum_edge(i[k], j[k], -cap[k], -rev_cap[k])`` per entry, in order: the next ``maxflow()`` returns the cut
+        and the energy of the graph built from scratch with every call so far and these decrements subtracted.  ``cap`` /
+        ``rev_cap`` are the decrements, nonnegative finite reals; the arguments take the forms of ``add_nweights_warm``.
+        The caller promises that every capacity stays >= 0; a pair whose residual capacities r(i->j) + r(j->i) (which
+        equal c(i->j) + c(j->i)) fall short of its total decrement beyond a few hundred roundings raises ``ValueError``,
+        and the graph is left as it was.  On a solved graph an arc may carry more flow than its lowered capacity: that
+        flow is cancelled and the terminal links make up the difference (a documented extension of the reference, whose
+        BK has no meaning for it; see mgc_remove_nweights_warm).
+
+        Before the first ``maxflow()`` the pending build is flushed and the calls are folded into it natively (staging
+        cannot lower a capacity).  The graph's terms are fixed from then on: a later term call (``add_tweights``,
+        ``sum_edge``, the whole-lattice terms) raises ``RuntimeError``, and the warm calls fold natively as on a solved
+        graph.  So make every term call before the first removal.  The graphs ``add_nweights_warm`` folds into take the calls; any other graph raises
+        ``RuntimeError``: ``reset()`` it and build the graph again without the weight."""
+        ii, jj, c, r, cuda = self._nweights_call_args(i, j, cap, rev_cap)
+        if not cuda:
+            self._check_decrements(((c, "cap"), (r, "rev_cap")))
+        self._fold_decrements("remove_nweights_warm", ii, jj, c, r)
+
+    def remove_nweights_dense_warm(self, axis, fwd, bwd):
+        """The dense form of ``remove_nweights_warm``, in the layout of ``add_nweights_dense_warm``: entry p of ``fwd`` /
+        ``bwd`` holds the decrements of the arcs p -> p + e_axis and back; the last plane of ``axis`` is ignored and only
+        the pairs with a nonzero entry are touched.  Same meaning, checks and errors as ``remove_nweights_warm``."""
+        axis, fwd, bwd, cuda = self._dense_nweights_args(axis, fwd, bwd)
+        if not cuda:
             cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
-            for w, what in ((fwd, "fwd"), (bwd, "bwd")):
-                if not numpy.isfinite(w[cut]).all():
-                    raise ValueError("{} holds NaN or infinite values".format(what))
-                if (w[cut] < 0).any():
-                    raise ValueError("{} holds negative values: a warm n-link edit only raises capacities".format(what))
-            staged = [numpy.zeros(self._shape), numpy.zeros(self._shape)]
-            staged[0][cut], staged[1][cut] = fwd[cut], bwd[cut]        # the last plane of `axis` names no pair
-            self.add_nweights_dense(axis, *staged)
-            return
+            self._check_decrements(((fwd[cut], "fwd"), (bwd[cut], "bwd")))
+        self._fold_decrements("remove_nweights_dense_warm", axis, fwd, bwd)
+
+    @staticmethod
+    def _check_decrements(weights):
+        """Host decrements: finite and nonnegative (the native grouping checks device arrays in the same pass)."""
+        for w, what in weights:
+            if not numpy.isfinite(w).all():
+                raise ValueError("{} holds NaN or infinite values".format(what))
+            if (w < 0).any():
+                raise ValueError("{} holds negative values: n-link decrements are nonnegative amounts".format(what))
+
+    def _terms_open(self):
+        """Term calls are refused once a removal has folded into the graph before its first solve: the handle then holds
+        a residual state, which staged terms cannot be added to."""
+        if self._folded:
+            raise RuntimeError("an n-link removal was folded into this graph before its first maxflow(), so its terms are "
+                               "fixed: make the term calls before remove_nweights_warm / remove_nweights_dense_warm, or "
+                               "reset() the graph and rebuild it")
+
+    def _fold_decrements(self, native, *args):
+        """A removal folds natively on solved and unsolved graphs alike: the pending build is flushed first.  Folded into
+        an unsolved graph, it fixes the terms (``_terms_open``); so does a refused pair check there, which runs after the
+        init that the first solve would run on an ``enable_warm()`` graph."""
+        self._lattice_term()
         if self._sp is not None:
             raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it with the n-link calls instead")
+                               "rebuild it without the n-link weight instead")
+        if self._offlattice is not None:
+            raise RuntimeError("edge {} does not join lattice neighbours: reset() the graph and rebuild it without the "
+                               "n-link weight instead".format(self._offlattice))
+        unsolved = not self._solved
+        if unsolved:
+            self._flush()
         self._dirty()
-        self._nat().add_nweights_dense_warm(axis, fwd, bwd)
+        try:
+            getattr(self._nat(), native)(*args)
+        except ValueError:
+            self._folded = self._folded or unsolved
+            raise
+        self._folded = self._folded or unsolved
 
     def _pair_ids(self, x, cuda, what):
         """One id argument of add_nweights_warm: a 1-D int64 array (or a 0-d one for a scalar), numpy or -- when ``cuda``
@@ -784,6 +878,7 @@ class GraphDouble:
         self._lazy = None
         self._fresh = True
         self._solved = False
+        self._folded = False
         if self._native is not None:
             self._native.reset()
 
