@@ -439,6 +439,25 @@ int mgc_sparse_get_trcap(const mgc_sparse* g, int64_t node, double* trcap);
 int mgc_sparse_get_node_num(const mgc_sparse* g, int64_t* n);
 int mgc_sparse_get_arc_num(const mgc_sparse* g, int64_t* n);    /* 2 per connected node pair */
 int mgc_sparse_get_stats(const mgc_sparse* g, mgc_stats* out);
+/* Warm re-solves of a general sparse graph (DESIGN.md §8, "Warm re-solve of sparse graphs").
+ * mgc_sparse_set_option(g, MGC_OPT_WARM, 1): only on a handle that was not solved since create or mgc_sparse_reset
+ * (MGC_E_STATE otherwise); the option survives mgc_sparse_reset.  The first solve of a warm handle keeps its device
+ * state (about 16 B per arc and 41 B per node) until reset or destroy.  From then on mgc_sparse_sum_edges and
+ * mgc_sparse_add_tweights fold into that residual state as the reference's calls act on its residual graph
+ * (graph.h:415-480), and the next maxflow continues from it; MGC_E_ARG, with the handle unchanged, for bad ids, NaN or
+ * infinite values, or a negative edge capacity.  The getters keep returning the values accumulated from scratch.  If
+ * the first solve's graph held a NaN or infinite capacity or t-link, every fold returns MGC_E_STATE.
+ * Without the option nothing changes: a call after a solve invalidates it and the next maxflow solves from scratch.
+ * Adding these entry points left MGC_ABI_VERSION at 3 and mgc_stats unchanged (seed_folds / ms_seeds count the folds). */
+int mgc_sparse_set_option(mgc_sparse* g, int32_t option, int64_t value);
+/* count x sum_edge(i[k], j[k], -cap[k], -rev_cap[k]) on existing pairs, with nonnegative finite decrements, on a warm
+ * handle (MGC_E_STATE without the option).  Per pair the decrements are summed in call order; the pair is refused with
+ * MGC_E_WEIGHT, the handle unchanged, when δ + δ' − (r_ij + r_ji) > 2^-44 · max(r_ij + r_ji, δ + δ') (residual
+ * capacities after a solve, accumulated ones before).  After a solve, flow beyond a lowered capacity is cancelled and a
+ * node left short is covered by its terminal links (Kohli-Torr).  MGC_E_ARG for bad ids, a pair without an edge or NaN
+ * / infinite values. */
+int mgc_sparse_remove_edges_warm(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t* j, const double* cap,
+                                 const double* rev_cap);
 
 /* ---- label images: the region adjacency graph built on the device (row f3) ------------------------------------ */
 

@@ -562,6 +562,18 @@ public:
         { py::gil_scoped_release rel; rc = mgc_sparse_sum_edges(g_, (int64_t)m, i.data(), j.data(), cap.data(), rev.data()); }
         check_sparse(rc, g_);
     }
+    void remove_edges_warm(py::array_t<int32_t, py::array::c_style | py::array::forcecast> i,
+                           py::array_t<int32_t, py::array::c_style | py::array::forcecast> j,
+                           py::array_t<double, py::array::c_style | py::array::forcecast> cap,
+                           py::array_t<double, py::array::c_style | py::array::forcecast> rev)
+    {
+        const py::ssize_t m = i.size();
+        if (j.size() != m || cap.size() != m || rev.size() != m) throw py::value_error("edge arrays differ in length");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_sparse_remove_edges_warm(g_, (int64_t)m, i.data(), j.data(), cap.data(), rev.data()); }
+        check_sparse(rc, g_);
+    }
+    void set_option(int32_t option, int64_t value) { check_sparse(mgc_sparse_set_option(g_, option, value), g_); }
     void add_tweights(const py::object& nodes, py::array_t<double, py::array::c_style | py::array::forcecast> src,
                       py::array_t<double, py::array::c_style | py::array::forcecast> snk)
     {
@@ -748,6 +760,8 @@ PYBIND11_MODULE(_mgc, m)
     py::class_<PySparse>(m, "SparseGraph")
         .def(py::init<int64_t, int>(), py::arg("n_nodes"), py::arg("device") = -1)
         .def("sum_edges", &PySparse::sum_edges)
+        .def("remove_edges_warm", &PySparse::remove_edges_warm)
+        .def("set_option", &PySparse::set_option)
         .def("add_tweights", &PySparse::add_tweights)
         .def("maxflow", &PySparse::maxflow)
         .def("get_mask", &PySparse::get_mask)

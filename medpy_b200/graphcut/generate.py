@@ -95,7 +95,7 @@ def _takes_three_parameters(fn):
 
 
 def graph_from_labels(label_image, fg_markers, bg_markers, regional_term=False, boundary_term=False,
-                      regional_term_args=False, boundary_term_args=False):
+                      regional_term_args=False, boundary_term_args=False, *, warm=False):
     """Create a graph-cut ready graph from a label (region) image -- generate.py:177-338.
 
     Every region of ``label_image`` (ids exactly 1..K, ``AttributeError`` otherwise) is a node (id = label - 1);
@@ -108,6 +108,10 @@ def graph_from_labels(label_image, fg_markers, bg_markers, regional_term=False, 
     The label image is staged on the device once and shared by the terms and the marker step; the resulting region
     graph is solved by the sparse push-relabel (csrc/gc_sparse.cuh).  (The reference itself cannot run this function on
     Python >= 3.11: it calls ``inspect.getargspec``, generate.py:280.)
+
+    ``warm=True`` (an addition to the reference's parameters) keeps the solved state: seeds added or erased on regions
+    (``add_seeds`` / ``remove_seeds`` with region ids or a boolean mask over the regions), t-link and edge calls made
+    after ``maxflow()`` fold into it, and the next ``maxflow()`` continues from the flow already routed.
     """
     from .energy_label import LabelContext
     label_image = numpy.asarray(label_image)
@@ -127,7 +131,7 @@ def graph_from_labels(label_image, fg_markers, bg_markers, regional_term=False, 
     nodes = context.regions
     edges = 10 * nodes                                       # the reference's guess (generate.py:296)
     _logger.debug("guessed: #nodes=%d nodes / #edges=%d", nodes, edges)
-    graph = GCGraph(nodes, edges, sparse=True)
+    graph = GCGraph(nodes, edges, sparse=True, warm=warm)
     graph._label_context = context
 
     _logger.info("Computing and adding terminal edge weights...")

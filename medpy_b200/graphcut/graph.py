@@ -92,12 +92,13 @@ class GCGraph:
     MAX = __UINT_16_BIT
     """The maximum value a terminal weight can take."""
 
-    def __init__(self, nodes, edges, shape=None, device=-1, sparse=None):
+    def __init__(self, nodes, edges, shape=None, device=-1, sparse=None, warm=False):
         """``GCGraph(nodes, edges)`` as in the reference (graph.py:294-308); ``shape`` (given by
         ``graph_from_voxels``) is the logical lattice shape whose C-order flat index is the node id.  Without a shape
         the graph is general: it moves to the sparse backend with the first edge between arbitrary nodes, or at once
-        with ``sparse=True`` (``graph_from_labels``)."""
-        self.__graph = GraphDouble(int(nodes), int(edges), shape=shape, device=device, sparse=sparse)
+        with ``sparse=True`` (``graph_from_labels``).  ``warm=True`` (with ``sparse=True``): calls made after a solve
+        fold into its residual state and the next solve continues from there."""
+        self.__graph = GraphDouble(int(nodes), int(edges), shape=shape, device=device, sparse=sparse, warm=warm)
         self.__graph.add_node(int(nodes))
         self.__nodes = int(nodes)
         self.__edges = int(edges)

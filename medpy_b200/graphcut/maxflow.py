@@ -41,11 +41,15 @@ class GraphDouble:
 
     termtype = _termtype
 
-    def __init__(self, node_num_max, edge_num_max=0, shape=None, device=-1, sparse=None):
+    def __init__(self, node_num_max, edge_num_max=0, shape=None, device=-1, sparse=None, warm=False):
         # Without a lattice shape the graph starts as a 1-D chain (what element-wise users of the voxel path build) and
         # keeps a journal of its calls; the first edge that does not join chain neighbours -- or sparse=True -- moves
-        # it, journal and all, onto the general sparse backend (sparse.py, SURVEY.md §8 row f4).
+        # it, journal and all, onto the general sparse backend (sparse.py, SURVEY.md §8 row f4).  warm=True (with
+        # sparse=True only) makes the sparse graph fold calls made after a solve into its residual state.
+        if warm and not sparse:
+            raise ValueError("warm=True needs sparse=True; lattice graphs call enable_warm() instead")
         self._sp = None
+        self._sp_warm = bool(warm)
         self._journal = [] if shape is None else None
         if shape is None:
             shape = (int(node_num_max),)
@@ -89,7 +93,7 @@ class GraphDouble:
 
     def _to_sparse(self):
         from .sparse import SparseGraphDouble
-        sp = SparseGraphDouble(self._n, self._edges, device=self._device)
+        sp = SparseGraphDouble(self._n, self._edges, device=self._device, warm=getattr(self, "_sp_warm", False))
         for op in self._journal or []:
             if op[0] == "e":
                 sp.sum_edge(op[1], op[2], op[3], op[4])
@@ -109,6 +113,10 @@ class GraphDouble:
     @property
     def is_sparse(self):
         return self._sp is not None
+
+    def _warm_sparse(self):
+        """A sparse graph created with warm=True: its warm calls are the sparse backend's (sparse.py)."""
+        return self._sp is not None and self._sp.warm
 
     # ------------------------------------------------------------------ native handle
     @property
@@ -140,7 +148,10 @@ class GraphDouble:
         call.  The setting survives ``reset()``.  On a graph the lazy fused build made it changes nothing.  A solved graph
         that cannot fold raises ``RuntimeError``, a sparse graph ``TypeError``."""
         if self._sp is not None:
-            raise TypeError("enable_warm() needs a lattice graph: a general sparse graph has no warm re-solve")
+            if self._sp.warm:
+                return                      # created with warm=True: already warm
+            raise TypeError("enable_warm() needs a lattice graph: a general sparse graph has no warm re-solve unless it "
+                            "is created with warm=True")
         if self._native is not None:
             from .. import _lib
             try:
@@ -469,6 +480,8 @@ class GraphDouble:
         state and the next solve continues from the flow already routed (mgc_add_seeds); so on any lattice graph that called
         ``enable_warm()`` before its first solve.  Any other solved graph raises ``RuntimeError``: ``reset()`` it and
         build the graph again with the seeds."""
+        if self._warm_sparse():
+            return self._sp.add_seeds(fg, bg)
         self._fold_seeds(fg, bg, 65535.0, "add_seeds", "with")
 
     def remove_seeds(self, fg=None, bg=None):
@@ -484,6 +497,8 @@ class GraphDouble:
         the solved state on the same graphs as ``add_seeds`` (``enable_warm()`` included, mgc_remove_seeds); any other
         solved graph raises
         ``RuntimeError``: ``reset()`` it and build the graph again without the seeds."""
+        if self._warm_sparse():
+            return self._sp.remove_seeds(fg, bg)
         self._fold_seeds(fg, bg, -65535.0, "remove_seeds", "without")
 
     def _fold_seeds(self, fg, bg, cap, native, rebuild):
@@ -518,6 +533,8 @@ class GraphDouble:
         and the next solve continues from the flow already routed (mgc_add_tweights_warm); so on any lattice graph that
         called ``enable_warm()`` before its first solve.  Any other solved graph raises ``RuntimeError``: ``reset()`` it and
         build the graph again with the calls."""
+        if self._warm_sparse():
+            return self._sp.add_tweights_warm(nodes, cap_source, cap_sink)
         cuda = any(hasattr(x, "__cuda_array_interface__") for x in (nodes, cap_source, cap_sink))
         ids = self._seed_ids(nodes) if nodes is not None else None
         if cuda and ids is not None and not hasattr(ids, "__cuda_array_interface__"):
@@ -591,6 +608,8 @@ class GraphDouble:
         Before the first ``maxflow()`` the calls are staged exactly like ``sum_edge``.  After it they are folded into the
         solved state on the graphs ``add_tweights_warm`` folds into (mgc_add_nweights_warm); any other solved graph raises
         ``RuntimeError``: ``reset()`` it and build the graph again with the calls."""
+        if self._warm_sparse():
+            return self._sp.add_nweights_warm(i, j, cap, rev_cap)
         ii, jj, c, r, cuda = self._nweights_call_args(i, j, cap, rev_cap)
         if not self._solved and not self._folded:
             if cuda:
@@ -630,6 +649,8 @@ class GraphDouble:
 
         Before the first ``maxflow()`` the call is staged exactly like ``add_nweights_dense``.  After it, the same graphs
         as ``add_nweights_warm`` fold it into the solved state (mgc_add_nweights_dense_warm)."""
+        if self._warm_sparse():
+            return self._sp.add_nweights_dense_warm(axis, fwd, bwd)
         axis, fwd, bwd, cuda = self._dense_nweights_args(axis, fwd, bwd)
         if not self._solved and not self._folded:
             if cuda:
@@ -695,6 +716,8 @@ class GraphDouble:
         ``sum_edge``, the whole-lattice terms) raises ``RuntimeError``, and the warm calls fold natively as on a solved
         graph.  So make every term call before the first removal.  The graphs ``add_nweights_warm`` folds into take the calls; any other graph raises
         ``RuntimeError``: ``reset()`` it and build the graph again without the weight."""
+        if self._warm_sparse():
+            return self._sp.remove_nweights_warm(i, j, cap, rev_cap)
         ii, jj, c, r, cuda = self._nweights_call_args(i, j, cap, rev_cap)
         if not cuda:
             self._check_decrements(((c, "cap"), (r, "rev_cap")))
@@ -704,6 +727,8 @@ class GraphDouble:
         """The dense form of ``remove_nweights_warm``, in the layout of ``add_nweights_dense_warm``: entry p of ``fwd`` /
         ``bwd`` holds the decrements of the arcs p -> p + e_axis and back; the last plane of ``axis`` is ignored and only
         the pairs with a nonzero entry are touched.  Same meaning, checks and errors as ``remove_nweights_warm``."""
+        if self._warm_sparse():
+            return self._sp.remove_nweights_dense_warm(axis, fwd, bwd)
         axis, fwd, bwd, cuda = self._dense_nweights_args(axis, fwd, bwd)
         if not cuda:
             cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))

@@ -7,6 +7,11 @@ edge by edge (tests/graphcut_/graph.py:47) -- are held by ``SparseGraphDouble``:
 cross the C ABI in bulk (``mgc_sparse_sum_edges`` / ``mgc_sparse_add_tweights``, which apply them in order with the
 reference's accumulation semantics); ``maxflow()`` runs a CSR push-relabel on the device (csrc/gc_sparse.cuh).
 
+A graph created with ``warm=True`` keeps the device state of its first solve.  Calls made after a solve are staged the
+same way and fold into that residual state at the next ``maxflow()`` (or getter), as the reference's ``add_tweights`` /
+``sum_edge`` act on its residual graph (graph.h:415-480); ``remove_nweights_warm`` lowers capacities
+(csrc/gc_sparse_warm.cuh).
+
 No CPU solver: the first call that needs a result creates the native graph and raises ``RuntimeError`` without a CUDA
 device or built extension.
 """
@@ -22,7 +27,7 @@ class SparseGraphDouble:
 
     termtype = _termtype
 
-    def __init__(self, node_num_max, edge_num_max=0, device=-1):
+    def __init__(self, node_num_max, edge_num_max=0, device=-1, warm=False):
         self._n = int(node_num_max)
         if self._n < 1:
             raise ValueError("a graph needs at least one node")
@@ -33,13 +38,36 @@ class SparseGraphDouble:
         self._e = ([], [], [], [])
         self._t = ([], [], [])
         self._mask = None
+        self._warm = bool(warm)   # MGC_OPT_WARM on the handle: calls after a solve fold into its residual state
+        self._solved = False      # a warm graph was solved since the last reset
+
+    @property
+    def warm(self):
+        return self._warm
 
     # ------------------------------------------------------------------ staging
     def _nat(self):
         if self._native is None:
             from .. import _lib  # raises ImportError loudly when the extension is not built
             self._native = _lib._mgc.SparseGraph(self._n, self._device)
+            if self._warm:
+                self._native.set_option(_lib._mgc.OPT_WARM, 1)
         return self._native
+
+    def _check_warm_tweights(self, src, snk):
+        if self._warm and self._solved and not (numpy.isfinite(src).all() and numpy.isfinite(snk).all()):
+            raise ValueError("t-weights hold NaN or infinite values")
+
+    def _check_warm_edges(self, cap, rev_cap):
+        """Plain sum_edge calls on a solved warm graph fold as increments: capacities only go down through
+        remove_nweights_warm."""
+        if self._warm and self._solved:
+            for w in (cap, rev_cap):
+                if not numpy.isfinite(w).all():
+                    raise ValueError("edge capacities hold NaN or infinite values")
+                if (numpy.asarray(w) < 0).any():
+                    raise ValueError("a negative sum_edge capacity cannot fold into a solved graph: lower capacities "
+                                     "with remove_nweights_warm")
 
     def _close_edges(self):
         if self._e[0]:
@@ -78,6 +106,7 @@ class SparseGraphDouble:
         """graph.h:415-425."""
         i = int(i)
         self._check_node(i)
+        self._check_warm_tweights(numpy.float64(cap_source), numpy.float64(cap_sink))
         self._t[0].append(i)
         self._t[1].append(float(cap_source))
         self._t[2].append(float(cap_sink))
@@ -98,6 +127,7 @@ class SparseGraphDouble:
                 raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(nodes.max(), nodes.min(), self._n - 1))
         elif src.size > self._n:
             raise ValueError("Invalid node id of {}. Valid values are 0 to {}.".format(src.size - 1, self._n - 1))
+        self._check_warm_tweights(src, snk)
         self._close_tweights()
         self._ops.append(("t", nodes, src, snk))
         self._mask = None
@@ -107,6 +137,7 @@ class SparseGraphDouble:
         i, j = int(i), int(j)
         if i < 0 or j < 0 or i >= self._n or j >= self._n or i == j:
             raise ValueError("invalid node ids ({}, {})".format(i, j))
+        self._check_warm_edges(numpy.float64(cap), numpy.float64(rev_cap))
         self._e[0].append(i)
         self._e[1].append(j)
         self._e[2].append(float(cap))
@@ -125,6 +156,7 @@ class SparseGraphDouble:
             raise ValueError("edge arrays differ in length")
         if i.size and (min(i.min(), j.min()) < 0 or max(i.max(), j.max()) >= self._n or (i == j).any()):
             raise ValueError("invalid node ids in the edge arrays")
+        self._check_warm_edges(cap, rev_cap)
         self._close_edges()
         self._ops.append(("e", i, j, cap, rev_cap))
         self._mask = None
@@ -132,7 +164,9 @@ class SparseGraphDouble:
     def maxflow(self):
         """Graph::maxflow (maxflow.cpp:471-604): min-cut energy including the add_tweights constants."""
         self._flush()
-        return self._nat().maxflow()
+        flow = self._nat().maxflow()
+        self._solved = self._warm
+        return flow
 
     def get_mask(self):
         """uint8[n]: 0 where what_segment == SINK else 1 (the loop of bin/medpy_graphcut_label.py:139-145 in bulk)."""
@@ -152,8 +186,9 @@ class SparseGraphDouble:
         self._e = ([], [], [], [])
         self._t = ([], [], [])
         self._mask = None
+        self._solved = False
         if self._native is not None:
-            self._native.reset()
+            self._native.reset()            # the warm option stays set on the handle
 
     def get_edge(self, i, j):
         self._flush()
@@ -172,3 +207,104 @@ class SparseGraphDouble:
 
     def stats(self):
         return self._nat().stats()
+
+    # ------------------------------------------------------------------ warm calls (graphs created with warm=True)
+    def _require_warm(self, what):
+        if not self._warm:
+            raise RuntimeError("{} needs a sparse graph created with warm=True; reset() the graph and rebuild it "
+                               "instead".format(what))
+
+    def _ids(self, x, what):
+        """Node ids of one warm-call argument: a 1-D integer array or a boolean mask of shape (n,); numpy or a tensor
+        (copied to the host: sparse handles take host arrays)."""
+        if hasattr(x, "__cuda_array_interface__") or type(x).__module__.startswith("torch"):
+            x = x.detach().cpu().numpy()
+        a = numpy.asarray(x)
+        if a.dtype == numpy.bool_:
+            if a.shape != (self._n,):
+                raise ValueError("{} mask of shape {} does not match the graph's {} nodes".format(what, a.shape, self._n))
+            return a.nonzero()[0].astype(numpy.int32)
+        if a.ndim > 1 or not (a.size == 0 or numpy.issubdtype(a.dtype, numpy.integer)):
+            raise ValueError("{} must be a boolean mask of shape (n,) or a 1-D integer id array".format(what))
+        a = a.reshape(-1).astype(numpy.int64)
+        if a.size and (a.min() < 0 or a.max() >= self._n):
+            raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(a.max(), a.min(), self._n - 1))
+        return a.astype(numpy.int32)
+
+    def _weights(self, w, m, what):
+        if hasattr(w, "__cuda_array_interface__") or type(w).__module__.startswith("torch"):
+            w = w.detach().cpu().numpy()
+        a = numpy.asarray(w)
+        if a.dtype.kind not in "iuf":
+            raise ValueError("{} must hold real numbers".format(what))
+        if a.ndim == 0:
+            a = numpy.full(m, float(a), dtype=numpy.float64)
+        if a.shape != (m,):
+            raise ValueError("{} has shape {}, expected ({},)".format(what, a.shape, m))
+        a = numpy.ascontiguousarray(a, dtype=numpy.float64)
+        if not numpy.isfinite(a).all():
+            raise ValueError("{} holds NaN or infinite values".format(what))
+        return a
+
+    def add_seeds(self, fg=None, bg=None):
+        """add_tweights(v, 65535, 0) per foreground id in order, then add_tweights(v, 0, 65535) per background id."""
+        self._require_warm("add_seeds")
+        self._seed_calls(fg, bg, 65535.0)
+
+    def remove_seeds(self, fg=None, bg=None):
+        """The inverse of add_seeds: add_tweights(v, -65535, 0) / add_tweights(v, 0, -65535)."""
+        self._require_warm("remove_seeds")
+        self._seed_calls(fg, bg, -65535.0)
+
+    def _seed_calls(self, fg, bg, cap):
+        ids = [None if x is None else self._ids(x, what) for x, what in ((fg, "fg"), (bg, "bg"))]
+        for v, src, snk in ((ids[0], cap, 0.0), (ids[1], 0.0, cap)):
+            if v is not None and v.size:
+                self.add_tweights_bulk(v, numpy.full(v.size, src), numpy.full(v.size, snk))
+
+    def add_tweights_warm(self, nodes, cap_source, cap_sink):
+        """add_tweights(nodes[k], cap_source[k], cap_sink[k]) per entry in order; nodes None: one call per node."""
+        self._require_warm("add_tweights_warm")
+        ids = None if nodes is None else self._ids(nodes, "nodes")
+        m = self._n if ids is None else ids.size
+        self.add_tweights_bulk(ids, self._weights(cap_source, m, "cap_source"), self._weights(cap_sink, m, "cap_sink"))
+
+    def _pairs(self, i, j, cap, rev_cap, what):
+        ii, jj = self._ids(numpy.atleast_1d(i) if numpy.ndim(i) == 0 else i, "i"), self._ids(numpy.atleast_1d(j) if numpy.ndim(j) == 0 else j, "j")
+        m = max(ii.size, jj.size, *(numpy.size(w) for w in (cap, rev_cap) if numpy.ndim(w)))
+        if ii.size == 1 and m > 1:
+            ii = numpy.full(m, ii[0], numpy.int32)
+        if jj.size == 1 and m > 1:
+            jj = numpy.full(m, jj[0], numpy.int32)
+        if ii.size != jj.size:
+            raise ValueError("i and j differ in length")
+        c, r = self._weights(cap, ii.size, "cap"), self._weights(rev_cap, ii.size, "rev_cap")
+        if (c < 0).any() or (r < 0).any():
+            raise ValueError("{} takes nonnegative amounts".format(what))
+        if (ii == jj).any():
+            raise ValueError("invalid node ids in the edge arrays")
+        return ii, jj, c, r
+
+    def add_nweights_warm(self, i, j, cap, rev_cap):
+        """sum_edge(i[k], j[k], cap[k], rev_cap[k]) per entry in order, on any node pairs (new ones included)."""
+        self._require_warm("add_nweights_warm")
+        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, "add_nweights_warm")
+        if ii.size:
+            self.sum_edges_bulk(ii, jj, c, r)
+
+    def remove_nweights_warm(self, i, j, cap, rev_cap):
+        """sum_edge(i[k], j[k], -cap[k], -rev_cap[k]) per entry in order on existing pairs: the only way to lower a
+        capacity.  What is staged is folded first, so the call order is kept.  A pair whose decrements exceed what it
+        holds (beyond a few hundred roundings) raises ValueError with the graph unchanged."""
+        self._require_warm("remove_nweights_warm")
+        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, "remove_nweights_warm")
+        self._flush()
+        self._mask = None
+        if ii.size:
+            self._nat().remove_edges_warm(ii, jj, c, r)
+
+    def add_nweights_dense_warm(self, *args, **kwargs):
+        raise ValueError("a general sparse graph has no lattice axes: use add_nweights_warm")
+
+    def remove_nweights_dense_warm(self, *args, **kwargs):
+        raise ValueError("a general sparse graph has no lattice axes: use remove_nweights_warm")
