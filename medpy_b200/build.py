@@ -5,6 +5,7 @@
 
 ``python -m medpy_b200.build`` or ``medpy_b200.build.build_all()``; __graft_entry__.build() calls the latter.
 """
+import concurrent.futures
 import os
 import subprocess
 import sys
@@ -54,23 +55,25 @@ def _includes(path, seen=None):
 
 def build_lib(force=False, verbose=False):
     """One object per translation unit (rebuilt only when the unit or a header it includes changed), linked into one
-    shared library: gc_api.cu (lattice path), gc_sparse_api.cu (sparse graphs + label images)."""
+    shared library: the lattice C ABI (gc_api.cu, gc_build_api.cu, gc_solve.cu, gc_fold.cu, gc_slab.cu; gc_handle.cuh)
+    and gc_sparse_api.cu (sparse graphs + label images).  The units compile concurrently, one nvcc process each."""
     units = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith(".cu")]
     objdir = os.path.join(LIBDIR, "obj")
     os.makedirs(objdir, exist_ok=True)
     header = os.path.join(INCLUDE, "medpy_b200_graphcut.h")
     compile_flags = [f for f in NVCC_FLAGS if f != "-shared"]
     objs = []
-    relink = force or not os.path.exists(LIB)
+    stale = []
     for unit in units:
         obj = os.path.join(objdir, os.path.basename(unit)[:-3] + ".o")
         objs.append(obj)
         deps = sorted(_includes(unit)) + [header, os.path.abspath(__file__)]
         if force or _newer(obj, deps):
-            cmd = [NVCC] + compile_flags + (["-Xptxas", "-v"] if verbose else []) + ["-I", INCLUDE, "-c", unit, "-o", obj]
-            subprocess.check_call(cmd)
-            relink = True
-    if relink or _newer(LIB, objs):
+            stale.append([NVCC] + compile_flags + (["-Xptxas", "-v"] if verbose else []) + ["-I", INCLUDE, "-c", unit, "-o", obj])
+    if stale:
+        with concurrent.futures.ThreadPoolExecutor(max_workers=min(len(stale), os.cpu_count() or 1)) as pool:
+            list(pool.map(subprocess.check_call, stale))
+    if force or stale or not os.path.exists(LIB) or _newer(LIB, objs):
         subprocess.check_call([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC",
                                "-o", LIB] + objs)
     return LIB

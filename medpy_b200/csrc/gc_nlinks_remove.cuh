@@ -13,7 +13,7 @@
 //   2. after the claim, k_nlinks_remove_arcs lowers the two residuals of each pair.  Where a residual would go negative the
 //      arc carries d more flow than its new capacity: that flow is cancelled (the residual becomes 0, the reverse one
 //      loses d) and the item records the excess change d of its lower end (-d of its upper end);
-//   3. the endpoint list, filled in atomic order, is sorted (tails_sort in gc_api.cu); k_nlinks_remove_voxels visits each
+//   3. the endpoint list, filled in atomic order, is sorted (tails_sort in gc_fold.cu); k_nlinks_remove_voxels visits each
 //      endpoint once in ascending order and gathers the excess changes of its at most 2 * ND arcs in a fixed order (no
 //      floating-point atomics and no order set by scheduling: the energy is reproducible bit for bit).  It recomputes the
 //      arc bits and stores the new excess.  A voxel left with negative excess takes the shortfall from its terminal link:

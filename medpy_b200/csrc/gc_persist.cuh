@@ -12,13 +12,7 @@
 
 namespace cg = cooperative_groups;
 
-// control block in device memory (ints): see gc_api.cu
-//   [0],[1]   relabel list counts          [2..5] push list counts [colour*2 + buffer]
-//   [8]       work cursor                  [11] relabel list consumed next                [15] relabel passes
-#define CTL_CURSOR 8
-#define CTL_RLCUR 11
-#define CTL_RELP 15
-
+// control block: CTL_* (gc_tiles.cuh)
 __device__ __forceinline__ int ld_ctl(const int* ctl, int i) { return *(const volatile int*)(ctl + i); }
 
 // ---------------------------------------------------------------------------------------------------

@@ -87,23 +87,6 @@ __global__ void __launch_bounds__(256) k_readout(Lattice L, State<T> S, uint8_t*
 }
 
 // ---------------------------------------------------------------------------------------------------
-// z-slab border messages (the tile-aware unpack is k_slab_unpack_tiles / k_slab_unpack_tiles4)
-// ---------------------------------------------------------------------------------------------------
-// pack: heights of my border plane + the flow parked in the ghost plane's excess (my outbox), which is cleared
-template <typename T>
-__global__ void k_slab_pack(unsigned plane, const int* __restrict__ height_border, T* __restrict__ excess_ghost,
-                            int* __restrict__ h_out, double* __restrict__ f_out)
-{
-    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= plane) return;
-    h_out[i] = height_border[i];
-    if (f_out) {                    // labels-only messages (relabel rounds: nothing was pushed since the last exchange) leave the outbox alone
-        f_out[i] = (double)excess_ghost[i];
-        excess_ghost[i] = 0;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
 // debug-mode invariants (MEDPY_GC_DEBUG=1; SURVEY.md §5.2): out[0] += excess, out[1] += flow absorbed by the sink links,
 // out[2] += violations of: excess >= 0, every residual capacity >= 0, absorbed flow within [0, sink capacity], and (tile
 // solver, CHECK_RMASK) every residual-mask bit equal to "capacity > 0".  Flow conservation is checked by the host:

@@ -22,6 +22,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/medpy_b200_graphcut.h"
+#include "gc_host.hpp"
 #include "gc_labels.cuh"
 #include "gc_sparse.cuh"
 #include "gc_sparse_warm.cuh"
@@ -46,25 +47,12 @@ struct DevScope {
     }
 };
 
-int bits_for(unsigned long long v)   // number of bits needed to represent values in [0, v]
-{
-    int b = 0;
-    while (v) { ++b; v >>= 1; }
-    return b ? b : 1;
-}
-
 // grid of the grid-stride kernels: one block per LAB_BLOCK items, at most 32 blocks per SM of the current device
 unsigned grid_for(long long n)
 {
-    static thread_local int dev_cached = -1, cap = 0;
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); dev = 0; }
-    if (dev != dev_cached) {
-        int sms = 0;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) { cudaGetLastError(); sms = 132; }
-        cap = 32 * sms;
-        dev_cached = dev;
-    }
+    const long long cap = 32LL * cached_sm_count(dev);
     long long b = (n + LAB_BLOCK - 1) / LAB_BLOCK;
     if (b < 1) b = 1;
     return (unsigned)(b < cap ? b : cap);
@@ -122,22 +110,6 @@ struct mgc_sparse {
     ~mgc_sparse() { release(); }
 };
 
-#define SPCK(call)                                                                                 \
-    do {                                                                                           \
-        cudaError_t _e = (call);                                                                   \
-        if (_e != cudaSuccess) {                                                                   \
-            g->err = std::string(#call) + ": " + cudaGetErrorString(_e);                           \
-            cudaGetLastError();                                                                    \
-            return MGC_E_CUDA;                                                                     \
-        }                                                                                          \
-    } while (0)
-
-#define SPFAIL(code, msg)                                                                          \
-    do {                                                                                           \
-        g->err = (msg);                                                                            \
-        return (code);                                                                             \
-    } while (0)
-
 namespace {
 
 void sparse_ensure_index(mgc_sparse* g)
@@ -166,26 +138,26 @@ int sparse_loop(mgc_sparse* g, const SparseState& S, int* d_flags, unsigned long
         g->st.kernel_launches++;
         g->st.global_relabels++;
         for (;;) {
-            SPCK(cudaMemsetAsync(d_flags, 0, sizeof(int), 0));
+            CK(cudaMemsetAsync(d_flags, 0, sizeof(int), 0));
             for (int r = 0; r < g->relax_batch; ++r) k_sp_relax<<<blocks, 256>>>(S, d_flags);
             g->st.kernel_launches += g->relax_batch;
             g->st.relabel_sweeps += g->relax_batch;
             int changed = 0;
-            SPCK(cudaMemcpy(&changed, d_flags, sizeof(int), cudaMemcpyDeviceToHost));
+            CK(cudaMemcpy(&changed, d_flags, sizeof(int), cudaMemcpyDeviceToHost));
             if (!changed) break;
         }
         // stop test, only ever right after an exact relabel
-        SPCK(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), 0));
+        CK(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), 0));
         k_sp_count_active<<<blocks, 256>>>(S, d_count);
         g->st.kernel_launches++;
         unsigned long long c = 0;
-        SPCK(cudaMemcpy(&c, d_count, sizeof(c), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(&c, d_count, sizeof(c), cudaMemcpyDeviceToHost));
         active = (long long)c;
         if (!active) break;
         const double elapsed = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count();
         if (++rounds > g->max_rounds || elapsed > g->max_seconds) {
             cudaEventDestroy(ev0); cudaEventDestroy(ev1);
-            SPFAIL(MGC_E_NOCONV, "sparse push-relabel did not converge within " + std::to_string(rounds) + " rounds / " +
+            FAIL(MGC_E_NOCONV, "sparse push-relabel did not converge within " + std::to_string(rounds) + " rounds / " +
                                      std::to_string(elapsed) + " s (" + std::to_string(active) + " active nodes left)");
         }
         for (int s = 0; s < g->sweeps_per_round; ++s) k_sp_push<<<blocks, 256>>>(S, g->push_steps, d_flags + 1);
@@ -194,14 +166,14 @@ int sparse_loop(mgc_sparse* g, const SparseState& S, int* d_flags, unsigned long
     }
     k_sp_readout<<<1, 256>>>(S, d_mask, d_abs);
     g->st.kernel_launches++;
-    SPCK(cudaEventRecord(ev1, 0));
-    SPCK(cudaGetLastError());
+    CK(cudaEventRecord(ev1, 0));
+    CK(cudaGetLastError());
     g->mask.assign((size_t)n, 0);
     double absorbed = 0.0;
-    SPCK(cudaMemcpy(g->mask.data(), d_mask, (size_t)n, cudaMemcpyDeviceToHost));
-    SPCK(cudaMemcpy(&absorbed, d_abs, sizeof(double), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(g->mask.data(), d_mask, (size_t)n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&absorbed, d_abs, sizeof(double), cudaMemcpyDeviceToHost));
     float ms = 0.f;
-    SPCK(cudaEventElapsedTime(&ms, ev0, ev1));
+    CK(cudaEventElapsedTime(&ms, ev0, ev1));
     cudaEventDestroy(ev0);
     cudaEventDestroy(ev1);
     g->energy = base + absorbed;
@@ -235,21 +207,21 @@ SparseWarm warm_view(const mgc_sparse* g)
 // a warm handle with a resident state: the loop only
 int sparse_resolve(mgc_sparse* g)
 {
-    SPCK(cudaSetDevice(g->device));
+    CK(cudaSetDevice(g->device));
     cudaEvent_t ev0, ev1;
-    SPCK(cudaEventCreate(&ev0));
-    SPCK(cudaEventCreate(&ev1));
-    SPCK(cudaEventRecord(ev0, 0));
+    CK(cudaEventCreate(&ev0));
+    CK(cudaEventCreate(&ev1));
+    CK(cudaEventRecord(ev0, 0));
     return sparse_loop(g, warm_state(g), g->dev.flags, g->dev.count, g->dev.mask, g->dev.abs, ev0, ev1, g->wconst);
 }
 
 int sparse_solve(mgc_sparse* g)
 {
     if (g->resident) return sparse_resolve(g);
-    SPCK(cudaSetDevice(g->device));
+    CK(cudaSetDevice(g->device));
     const int n = (int)g->n;
     const int64_t np = (int64_t)g->plo.size();
-    if (2 * np >= (int64_t)INT32_MAX) SPFAIL(MGC_E_ARG, "too many arcs for 32-bit arc ids");
+    if (2 * np >= (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "too many arcs for 32-bit arc ids");
     const int m2 = (int)(2 * np);
     // CSR in insertion order of the pairs (the order add_edge appends arcs to a node's list, graph.h:443-452)
     std::vector<int> row((size_t)n + 1, 0), head((size_t)m2), sis((size_t)m2);
@@ -271,39 +243,39 @@ int sparse_solve(mgc_sparse* g)
     double *d_cap, *d_tr, *d_excess, *d_sunk, *d_abs;
     uint8_t* d_mask;
     unsigned long long* d_count;
-    SPCK(dev.alloc(&d_row, (size_t)n + 1));
-    SPCK(dev.alloc(&d_head, (size_t)m2));
-    SPCK(dev.alloc(&d_sis, (size_t)m2));
-    SPCK(dev.alloc(&d_cap, (size_t)m2));
-    SPCK(dev.alloc(&d_tr, (size_t)n));
-    SPCK(dev.alloc(&d_excess, (size_t)n));
-    SPCK(dev.alloc(&d_sunk, (size_t)n));
-    SPCK(dev.alloc(&d_height, (size_t)n));
-    SPCK(dev.alloc(&d_mask, (size_t)n));
-    SPCK(dev.alloc(&d_flags, 2));
-    SPCK(dev.alloc(&d_abs, 1));
-    SPCK(dev.alloc(&d_count, 1));
-    SPCK(cudaMemcpy(d_row, row.data(), ((size_t)n + 1) * sizeof(int), cudaMemcpyHostToDevice));
+    CK(dev.alloc(&d_row, (size_t)n + 1));
+    CK(dev.alloc(&d_head, (size_t)m2));
+    CK(dev.alloc(&d_sis, (size_t)m2));
+    CK(dev.alloc(&d_cap, (size_t)m2));
+    CK(dev.alloc(&d_tr, (size_t)n));
+    CK(dev.alloc(&d_excess, (size_t)n));
+    CK(dev.alloc(&d_sunk, (size_t)n));
+    CK(dev.alloc(&d_height, (size_t)n));
+    CK(dev.alloc(&d_mask, (size_t)n));
+    CK(dev.alloc(&d_flags, 2));
+    CK(dev.alloc(&d_abs, 1));
+    CK(dev.alloc(&d_count, 1));
+    CK(cudaMemcpy(d_row, row.data(), ((size_t)n + 1) * sizeof(int), cudaMemcpyHostToDevice));
     if (m2) {
-        SPCK(cudaMemcpy(d_head, head.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
-        SPCK(cudaMemcpy(d_sis, sis.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
-        SPCK(cudaMemcpy(d_cap, cap.data(), (size_t)m2 * sizeof(double), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(d_head, head.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(d_sis, sis.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(d_cap, cap.data(), (size_t)m2 * sizeof(double), cudaMemcpyHostToDevice));
     }
-    SPCK(cudaMemcpy(d_tr, g->tr.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_tr, g->tr.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
     S.n = n; S.m2 = m2; S.row = d_row; S.head = d_head; S.sis = d_sis; S.cap = d_cap; S.tr = d_tr;
     S.excess = d_excess; S.sunk = d_sunk; S.height = d_height;
 
     double* d_sent = nullptr;
     uint8_t* d_tail = nullptr;
     if (g->warm) {
-        SPCK(dev.alloc(&d_sent, (size_t)n));
-        SPCK(dev.alloc(&d_tail, (size_t)n));
-        SPCK(cudaMemset(d_tail, 0, (size_t)n));
+        CK(dev.alloc(&d_sent, (size_t)n));
+        CK(dev.alloc(&d_tail, (size_t)n));
+        CK(cudaMemset(d_tail, 0, (size_t)n));
     }
     cudaEvent_t ev0, ev1;
-    SPCK(cudaEventCreate(&ev0));
-    SPCK(cudaEventCreate(&ev1));
-    SPCK(cudaEventRecord(ev0, 0));
+    CK(cudaEventCreate(&ev0));
+    CK(cudaEventCreate(&ev1));
+    CK(cudaEventRecord(ev0, 0));
     const unsigned blocks = grid_for(n);
     if (g->warm) {
         SparseWarm W{};
@@ -346,11 +318,11 @@ int warm_group(mgc_sparse* g, DevScope& dev, const unsigned* h_keys, long long m
                unsigned** keys_sorted, unsigned** order)
 {
     unsigned *keys, *idx;
-    SPCK(dev.alloc(&keys, (size_t)m));
-    SPCK(dev.alloc(&idx, (size_t)m));
-    SPCK(dev.alloc(keys_sorted, (size_t)m));
-    SPCK(dev.alloc(order, (size_t)m));
-    if (h_keys) SPCK(cudaMemcpy(keys, h_keys, (size_t)m * sizeof(unsigned), cudaMemcpyHostToDevice));
+    CK(dev.alloc(&keys, (size_t)m));
+    CK(dev.alloc(&idx, (size_t)m));
+    CK(dev.alloc(keys_sorted, (size_t)m));
+    CK(dev.alloc(order, (size_t)m));
+    if (h_keys) CK(cudaMemcpy(keys, h_keys, (size_t)m * sizeof(unsigned), cudaMemcpyHostToDevice));
     return warm_sort(g, dev, keys, idx, m, key_max, *keys_sorted, *order, true);
 }
 
@@ -361,10 +333,10 @@ int warm_sort(mgc_sparse* g, DevScope& dev, unsigned* keys, unsigned* idx, long 
     if (iota) { k_spw_iota<<<mb, 256>>>(idx, m); g->st.kernel_launches++; }
     const int end_bit = bits_for(key_max);
     size_t tb = 0;
-    SPCK(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys_sorted, idx, order, (int)m, 0, end_bit, 0));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys_sorted, idx, order, (int)m, 0, end_bit, 0));
     char* tmp;
-    SPCK(dev.alloc(&tmp, tb));
-    SPCK(cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_sorted, idx, order, (int)m, 0, end_bit, 0));
+    CK(dev.alloc(&tmp, tb));
+    CK(cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys_sorted, idx, order, (int)m, 0, end_bit, 0));
     g->st.kernel_launches += 4;
     return MGC_OK;
 }
@@ -373,54 +345,48 @@ int warm_sort(mgc_sparse* g, DevScope& dev, unsigned* keys, unsigned* idx, long 
 int warm_constant(mgc_sparse* g, DevScope& dev, const double* partials, long long nb, double* out)
 {
     double* d_out;
-    SPCK(dev.alloc(&d_out, 1));
+    CK(dev.alloc(&d_out, 1));
     k_spw_sum_partials<<<1, 256>>>(partials, nb, d_out);
     g->st.kernel_launches++;
-    SPCK(cudaGetLastError());
-    SPCK(cudaMemcpy(out, d_out, sizeof(double), cudaMemcpyDeviceToHost));
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(out, d_out, sizeof(double), cudaMemcpyDeviceToHost));
     return MGC_OK;
 }
 
 template <typename T>
 int warm_upload(mgc_sparse* g, DevScope& dev, const std::vector<T>& h, T** d)
 {
-    SPCK(dev.alloc(d, h.size()));
-    if (!h.empty()) SPCK(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+    CK(dev.alloc(d, h.size()));
+    if (!h.empty()) CK(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
     return MGC_OK;
 }
 
-#define SPRC(call)                       \
-    do {                                 \
-        int _rc = (call);                \
-        if (_rc) return _rc;             \
-    } while (0)
-
 int warm_fold_tweights(mgc_sparse* g, int64_t count, const int32_t* nodes, const double* src, const double* snk)
 {
-    SPCK(cudaSetDevice(g->device));
+    CK(cudaSetDevice(g->device));
     cudaEvent_t e0, e1;
-    SPCK(cudaEventCreate(&e0));
-    SPCK(cudaEventCreate(&e1));
-    SPCK(cudaEventRecord(e0, 0));
+    CK(cudaEventCreate(&e0));
+    CK(cudaEventCreate(&e1));
+    CK(cudaEventRecord(e0, 0));
     DevScope dev;
     std::vector<unsigned> keys((size_t)count);
     for (int64_t k = 0; k < count; ++k) keys[(size_t)k] = (unsigned)(nodes ? nodes[k] : k);
     unsigned *ks, *order;
-    SPRC(warm_group(g, dev, keys.data(), count, (unsigned)(g->n - 1), &ks, &order));
+    RC(warm_group(g, dev, keys.data(), count, (unsigned)(g->n - 1), &ks, &order));
     double *d_src, *d_snk, *partials;
     const long long nb = (count + 255) / 256;
-    SPCK(dev.alloc(&d_src, (size_t)count));
-    SPCK(dev.alloc(&d_snk, (size_t)count));
-    SPCK(dev.alloc(&partials, (size_t)nb));
-    SPCK(cudaMemcpy(d_src, src, (size_t)count * sizeof(double), cudaMemcpyHostToDevice));
-    SPCK(cudaMemcpy(d_snk, snk, (size_t)count * sizeof(double), cudaMemcpyHostToDevice));
+    CK(dev.alloc(&d_src, (size_t)count));
+    CK(dev.alloc(&d_snk, (size_t)count));
+    CK(dev.alloc(&partials, (size_t)nb));
+    CK(cudaMemcpy(d_src, src, (size_t)count * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_snk, snk, (size_t)count * sizeof(double), cudaMemcpyHostToDevice));
     k_spw_tlink_fold<<<(unsigned)nb, 256>>>(warm_view(g), ks, order, count, d_src, d_snk, partials);
     g->st.kernel_launches++;
     double dk = 0.0;
-    SPRC(warm_constant(g, dev, partials, nb, &dk));
+    RC(warm_constant(g, dev, partials, nb, &dk));
     g->wconst += dk;
-    SPCK(cudaEventRecord(e1, 0));
-    SPCK(cudaEventSynchronize(e1));
+    CK(cudaEventRecord(e1, 0));
+    CK(cudaEventSynchronize(e1));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, e0, e1);
     cudaEventDestroy(e0); cudaEventDestroy(e1);
@@ -435,11 +401,11 @@ int warm_fold_edges(mgc_sparse* g, const std::vector<unsigned>& pk, const std::v
                     const std::vector<int32_t>& olo, const std::vector<int32_t>& ohi, const std::vector<double>& c_lh,
                     const std::vector<double>& c_hl, int64_t first_fresh)
 {
-    SPCK(cudaSetDevice(g->device));
+    CK(cudaSetDevice(g->device));
     cudaEvent_t e0, e1;
-    SPCK(cudaEventCreate(&e0));
-    SPCK(cudaEventCreate(&e1));
-    SPCK(cudaEventRecord(e0, 0));
+    CK(cudaEventCreate(&e0));
+    CK(cudaEventCreate(&e1));
+    CK(cudaEventRecord(e0, 0));
     DevScope dev;
     const int n = (int)g->n;
     const unsigned blocks = grid_for(n);
@@ -452,15 +418,15 @@ int warm_fold_edges(mgc_sparse* g, const std::vector<unsigned>& pk, const std::v
         std::vector<int32_t> qlo(g->plo.begin() + first_fresh, g->plo.end()), qhi(g->phi.begin() + first_fresh, g->phi.end());
         std::vector<int32_t> qol(g->olo.begin() + first_fresh, g->olo.end()), qoh(g->ohi.begin() + first_fresh, g->ohi.end());
         int *d_qlo, *d_qhi, *d_qol, *d_qoh;
-        SPRC(warm_upload(g, dev, qlo, &d_qlo));
-        SPRC(warm_upload(g, dev, qhi, &d_qhi));
-        SPRC(warm_upload(g, dev, qol, &d_qol));
-        SPRC(warm_upload(g, dev, qoh, &d_qoh));
+        RC(warm_upload(g, dev, qlo, &d_qlo));
+        RC(warm_upload(g, dev, qhi, &d_qhi));
+        RC(warm_upload(g, dev, qol, &d_qol));
+        RC(warm_upload(g, dev, qoh, &d_qoh));
         unsigned* cnt;
         unsigned long long* off;
-        SPCK(dev.alloc(&cnt, (size_t)n));
-        SPCK(dev.alloc(&off, (size_t)n + 1));
-        SPCK(cudaMemset(cnt, 0, (size_t)n * sizeof(unsigned)));
+        CK(dev.alloc(&cnt, (size_t)n));
+        CK(dev.alloc(&off, (size_t)n + 1));
+        CK(cudaMemset(cnt, 0, (size_t)n * sizeof(unsigned)));
         const unsigned qb = (unsigned)((q + 255) / 256);
         k_spw_count_new<<<qb, 256>>>(d_qlo, d_qhi, q, cnt);
         k_spw_degree<<<blocks, 256>>>(g->dev.row, n, cnt);
@@ -470,16 +436,16 @@ int warm_fold_edges(mgc_sparse* g, const std::vector<unsigned>& pk, const std::v
         double* cap;
         {
             DevScope keep;
-            SPCK(keep.alloc(&row, (size_t)n + 1));
-            SPCK(keep.alloc(&head, (size_t)m2n));
-            SPCK(keep.alloc(&sis, (size_t)m2n));
-            SPCK(keep.alloc(&cap, (size_t)m2n));
+            CK(keep.alloc(&row, (size_t)n + 1));
+            CK(keep.alloc(&head, (size_t)m2n));
+            CK(keep.alloc(&sis, (size_t)m2n));
+            CK(keep.alloc(&cap, (size_t)m2n));
             k_spw_row<<<blocks, 256>>>(off, n, row);
             k_spw_move<<<blocks, 256>>>(n, g->dev.row, g->dev.head, g->dev.sis, g->dev.cap, row, head, sis, cap);
             k_spw_new_pairs<<<qb, 256>>>(d_qlo, d_qhi, d_qol, d_qoh, q, row, head, sis, cap);
             g->st.kernel_launches += 3;
-            SPCK(cudaGetLastError());
-            SPCK(cudaDeviceSynchronize());
+            CK(cudaGetLastError());
+            CK(cudaDeviceSynchronize());
             keep.ptrs.clear();
         }
         cudaFree(g->dev.row); cudaFree(g->dev.head); cudaFree(g->dev.sis); cudaFree(g->dev.cap);
@@ -488,22 +454,22 @@ int warm_fold_edges(mgc_sparse* g, const std::vector<unsigned>& pk, const std::v
     }
     const long long m = (long long)pk.size();
     unsigned *ks, *order;
-    SPRC(warm_group(g, dev, pk.data(), m, (unsigned)(np > 0 ? np - 1 : 0), &ks, &order));
+    RC(warm_group(g, dev, pk.data(), m, (unsigned)(np > 0 ? np - 1 : 0), &ks, &order));
     int *d_lo, *d_hi, *d_ol, *d_oh;
     double *d_cl, *d_ch;
-    SPRC(warm_upload(g, dev, lo, &d_lo));
-    SPRC(warm_upload(g, dev, hi, &d_hi));
-    SPRC(warm_upload(g, dev, olo, &d_ol));
-    SPRC(warm_upload(g, dev, ohi, &d_oh));
-    SPRC(warm_upload(g, dev, c_lh, &d_cl));
-    SPRC(warm_upload(g, dev, c_hl, &d_ch));
+    RC(warm_upload(g, dev, lo, &d_lo));
+    RC(warm_upload(g, dev, hi, &d_hi));
+    RC(warm_upload(g, dev, olo, &d_ol));
+    RC(warm_upload(g, dev, ohi, &d_oh));
+    RC(warm_upload(g, dev, c_lh, &d_cl));
+    RC(warm_upload(g, dev, c_hl, &d_ch));
     const SparseWarm W = warm_view(g);
     k_spw_pair_inc<<<(unsigned)((m + 255) / 256), 256>>>(W, ks, order, m, d_lo, d_hi, d_ol, d_oh, d_cl, d_ch, g->dev.tail);
     k_spw_reclamp<<<blocks, 256>>>(W, g->dev.tail);
     g->st.kernel_launches += 2;
-    SPCK(cudaGetLastError());
-    SPCK(cudaEventRecord(e1, 0));
-    SPCK(cudaEventSynchronize(e1));
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(e1, 0));
+    CK(cudaEventSynchronize(e1));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, e0, e1);
     cudaEventDestroy(e0); cudaEventDestroy(e1);
@@ -516,48 +482,48 @@ int warm_fold_decrements(mgc_sparse* g, const std::vector<unsigned>& pk, const s
                          const std::vector<int32_t>& olo, const std::vector<int32_t>& ohi, const std::vector<double>& d_lh,
                          const std::vector<double>& d_hl)
 {
-    SPCK(cudaSetDevice(g->device));
+    CK(cudaSetDevice(g->device));
     DevScope dev;
     const long long m = (long long)pk.size();
     const int64_t np = (int64_t)g->plo.size();
     unsigned *ks, *order;
-    SPRC(warm_group(g, dev, pk.data(), m, (unsigned)(np > 0 ? np - 1 : 0), &ks, &order));
+    RC(warm_group(g, dev, pk.data(), m, (unsigned)(np > 0 ? np - 1 : 0), &ks, &order));
     int *d_lo, *d_hi, *d_ol, *d_oh, *refused;
     double *d_l, *d_h;
-    SPRC(warm_upload(g, dev, lo, &d_lo));
-    SPRC(warm_upload(g, dev, hi, &d_hi));
-    SPRC(warm_upload(g, dev, olo, &d_ol));
-    SPRC(warm_upload(g, dev, ohi, &d_oh));
-    SPRC(warm_upload(g, dev, d_lh, &d_l));
-    SPRC(warm_upload(g, dev, d_hl, &d_h));
-    SPCK(dev.alloc(&refused, 1));
-    SPCK(cudaMemset(refused, 0, sizeof(int)));
+    RC(warm_upload(g, dev, lo, &d_lo));
+    RC(warm_upload(g, dev, hi, &d_hi));
+    RC(warm_upload(g, dev, olo, &d_ol));
+    RC(warm_upload(g, dev, ohi, &d_oh));
+    RC(warm_upload(g, dev, d_lh, &d_l));
+    RC(warm_upload(g, dev, d_hl, &d_h));
+    CK(dev.alloc(&refused, 1));
+    CK(cudaMemset(refused, 0, sizeof(int)));
     const SparseWarm W = warm_view(g);
     const unsigned mb = (unsigned)((m + 255) / 256);
     k_spw_pair_check<<<mb, 256>>>(W, ks, order, m, d_lo, d_hi, d_ol, d_oh, d_l, d_h, refused);
     g->st.kernel_launches++;
     int bad = 0;
-    SPCK(cudaMemcpy(&bad, refused, sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(&bad, refused, sizeof(int), cudaMemcpyDeviceToHost));
     if (bad)
-        SPFAIL(MGC_E_WEIGHT, "remove_edges_warm: a pair's decrements exceed its capacities r(i->j) + r(j->i) (the graph is "
+        FAIL(MGC_E_WEIGHT, "remove_edges_warm: a pair's decrements exceed its capacities r(i->j) + r(j->i) (the graph is "
                              "unchanged)");
     // arcs, then every end once in ascending node order with its changes in a fixed order
     unsigned *end_key, *end_idx, *end_ks, *end_order;
     double *end_dx, *partials;
-    SPCK(dev.alloc(&end_key, (size_t)(2 * m)));
-    SPCK(dev.alloc(&end_idx, (size_t)(2 * m)));
-    SPCK(dev.alloc(&end_ks, (size_t)(2 * m)));
-    SPCK(dev.alloc(&end_order, (size_t)(2 * m)));
-    SPCK(dev.alloc(&end_dx, (size_t)(2 * m)));
+    CK(dev.alloc(&end_key, (size_t)(2 * m)));
+    CK(dev.alloc(&end_idx, (size_t)(2 * m)));
+    CK(dev.alloc(&end_ks, (size_t)(2 * m)));
+    CK(dev.alloc(&end_order, (size_t)(2 * m)));
+    CK(dev.alloc(&end_dx, (size_t)(2 * m)));
     k_spw_pair_dec<<<mb, 256>>>(W, ks, order, m, d_lo, d_hi, d_ol, d_oh, d_l, d_h, end_key, end_dx);
     g->st.kernel_launches++;
-    SPRC(warm_sort(g, dev, end_key, end_idx, 2 * m, 0xffffffffu, end_ks, end_order, true));
+    RC(warm_sort(g, dev, end_key, end_idx, 2 * m, 0xffffffffu, end_ks, end_order, true));
     const long long nb = (2 * m + 255) / 256;
-    SPCK(dev.alloc(&partials, (size_t)nb));
+    CK(dev.alloc(&partials, (size_t)nb));
     k_spw_ends<<<(unsigned)nb, 256>>>(W, end_ks, end_order, 2 * m, end_dx, partials);
     g->st.kernel_launches++;
     double dk = 0.0;
-    SPRC(warm_constant(g, dev, partials, nb, &dk));
+    RC(warm_constant(g, dev, partials, nb, &dk));
     g->wconst += dk;
     g->st.seed_folds++;
     return MGC_OK;
@@ -590,7 +556,7 @@ int warm_resolve(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t* 
             g->cap_lh.push_back(0.0); g->cap_hl.push_back(0.0);
             if (g->resident) { g->olo.push_back(g->deg[(size_t)a]++); g->ohi.push_back(g->deg[(size_t)b]++); }
         } else {
-            SPFAIL(MGC_E_ARG, "no edge between nodes " + std::to_string(i[k]) + " and " + std::to_string(j[k]) +
+            FAIL(MGC_E_ARG, "no edge between nodes " + std::to_string(i[k]) + " and " + std::to_string(j[k]) +
                                   ": remove_edges_warm lowers existing capacities");
         }
         pk[(size_t)k] = (unsigned)p;
@@ -604,19 +570,19 @@ int warm_resolve(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t* 
 // sum_edge calls on a solved warm handle: the host mirror accumulates as on a cold graph, the resident state folds
 int warm_sum_edges(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t* j, const double* cap, const double* rev_cap)
 {
-    if (g->warm_bad) SPFAIL(MGC_E_STATE, warm_bad_msg);
+    if (g->warm_bad) FAIL(MGC_E_STATE, warm_bad_msg);
     for (int64_t k = 0; k < count; ++k) {
-        if (!std::isfinite(cap[k]) || !std::isfinite(rev_cap[k])) SPFAIL(MGC_E_ARG, "edge capacities hold NaN or infinite values");
+        if (!std::isfinite(cap[k]) || !std::isfinite(rev_cap[k])) FAIL(MGC_E_ARG, "edge capacities hold NaN or infinite values");
         if (cap[k] < 0 || rev_cap[k] < 0)
-            SPFAIL(MGC_E_ARG, "a negative capacity cannot fold into a solved graph: lower capacities with remove_edges_warm");
+            FAIL(MGC_E_ARG, "a negative capacity cannot fold into a solved graph: lower capacities with remove_edges_warm");
     }
     if (count == 0) return MGC_OK;
-    if (2 * ((int64_t)g->plo.size() + count) >= (int64_t)INT32_MAX) SPFAIL(MGC_E_ARG, "too many arcs for 32-bit arc ids");
+    if (2 * ((int64_t)g->plo.size() + count) >= (int64_t)INT32_MAX) FAIL(MGC_E_ARG, "too many arcs for 32-bit arc ids");
     const int64_t first_fresh = (int64_t)g->plo.size();
     std::vector<unsigned> pk;
     std::vector<int32_t> lo, hi;
     std::vector<double> c_lh, c_hl;
-    SPRC(warm_resolve(g, count, i, j, cap, rev_cap, true, pk, lo, hi, c_lh, c_hl));
+    RC(warm_resolve(g, count, i, j, cap, rev_cap, true, pk, lo, hi, c_lh, c_hl));
     std::vector<int32_t> ol((size_t)count), oh((size_t)count);
     for (int64_t k = 0; k < count; ++k) {
         const size_t p = pk[(size_t)k];
@@ -681,9 +647,9 @@ int mgc_sparse_reset(mgc_sparse* g)
 int mgc_sparse_set_option(mgc_sparse* g, int32_t option, int64_t value)
 {
     if (!g) return MGC_E_ARG;
-    if (option != MGC_OPT_WARM) SPFAIL(MGC_E_ARG, "unknown option for a sparse graph");
+    if (option != MGC_OPT_WARM) FAIL(MGC_E_ARG, "unknown option for a sparse graph");
     if (g->solved_once || g->resident)
-        SPFAIL(MGC_E_STATE, "MGC_OPT_WARM must be set before the first maxflow(): reset() the graph and rebuild it");
+        FAIL(MGC_E_STATE, "MGC_OPT_WARM must be set before the first maxflow(): reset() the graph and rebuild it");
     g->warm = value != 0;
     return MGC_OK;
 }
@@ -693,13 +659,13 @@ const char* mgc_sparse_last_error(const mgc_sparse* g) { return g ? g->err.c_str
 int mgc_sparse_sum_edges(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t* j, const double* cap, const double* rev_cap)
 {
     if (!g) return MGC_E_ARG;
-    if (count < 0 || (count > 0 && (!i || !j || !cap || !rev_cap))) SPFAIL(MGC_E_ARG, "null edge arrays");
+    if (count < 0 || (count > 0 && (!i || !j || !cap || !rev_cap))) FAIL(MGC_E_ARG, "null edge arrays");
     for (int64_t k = 0; k < count; ++k) {
         const int64_t a = i[k], b = j[k];
         if (a < 0 || b < 0 || a >= g->n || b >= g->n)
-            SPFAIL(MGC_E_ARG, "Invalid node id in edge (" + std::to_string(a) + ", " + std::to_string(b) + "). Valid values are 0 to " +
+            FAIL(MGC_E_ARG, "Invalid node id in edge (" + std::to_string(a) + ", " + std::to_string(b) + "). Valid values are 0 to " +
                                   std::to_string(g->n - 1) + ".");
-        if (a == b) SPFAIL(MGC_E_ARG, "The node_from (" + std::to_string(a) + ") can not be equal to the node_to (" + std::to_string(b) + ") (self-connections are forbidden in graph-cuts).");
+        if (a == b) FAIL(MGC_E_ARG, "The node_from (" + std::to_string(a) + ") can not be equal to the node_to (" + std::to_string(b) + ") (self-connections are forbidden in graph-cuts).");
     }
     if (g->resident) return warm_sum_edges(g, count, i, j, cap, rev_cap);
     // A batch of distinct pairs in strictly increasing (i, j) order with i < j -- what the region adjacency reduction
@@ -746,16 +712,16 @@ int mgc_sparse_sum_edges(mgc_sparse* g, int64_t count, const int32_t* i, const i
 int mgc_sparse_add_tweights(mgc_sparse* g, int64_t count, const int32_t* nodes, const double* src, const double* snk)
 {
     if (!g) return MGC_E_ARG;
-    if (count < 0 || (count > 0 && (!src || !snk))) SPFAIL(MGC_E_ARG, "null t-weight arrays");
-    if (!nodes && count > g->n) SPFAIL(MGC_E_ARG, "more t-weights than nodes");
+    if (count < 0 || (count > 0 && (!src || !snk))) FAIL(MGC_E_ARG, "null t-weight arrays");
+    if (!nodes && count > g->n) FAIL(MGC_E_ARG, "more t-weights than nodes");
     if (nodes)
         for (int64_t k = 0; k < count; ++k)
             if (nodes[k] < 0 || nodes[k] >= g->n)
-                SPFAIL(MGC_E_ARG, "Invalid node id of " + std::to_string(nodes[k]) + ". Valid values are 0 to " + std::to_string(g->n - 1) + ".");
+                FAIL(MGC_E_ARG, "Invalid node id of " + std::to_string(nodes[k]) + ". Valid values are 0 to " + std::to_string(g->n - 1) + ".");
     if (g->resident) {
-        if (g->warm_bad) SPFAIL(MGC_E_STATE, warm_bad_msg);
+        if (g->warm_bad) FAIL(MGC_E_STATE, warm_bad_msg);
         for (int64_t k = 0; k < count; ++k)
-            if (!std::isfinite(src[k]) || !std::isfinite(snk[k])) SPFAIL(MGC_E_ARG, "t-weights hold NaN or infinite values");
+            if (!std::isfinite(src[k]) || !std::isfinite(snk[k])) FAIL(MGC_E_ARG, "t-weights hold NaN or infinite values");
         if (count == 0) return MGC_OK;
         int rc = warm_fold_tweights(g, count, nodes, src, snk);
         if (rc) return rc;
@@ -777,21 +743,21 @@ int mgc_sparse_remove_edges_warm(mgc_sparse* g, int64_t count, const int32_t* i,
 {
     if (!g) return MGC_E_ARG;
     if (!g->warm)
-        SPFAIL(MGC_E_STATE, "remove_edges_warm needs a graph created with the warm option (MGC_OPT_WARM): reset() the graph "
+        FAIL(MGC_E_STATE, "remove_edges_warm needs a graph created with the warm option (MGC_OPT_WARM): reset() the graph "
                             "and rebuild it without the weight instead");
-    if (count < 0 || (count > 0 && (!i || !j || !cap || !rev_cap))) SPFAIL(MGC_E_ARG, "null edge arrays");
+    if (count < 0 || (count > 0 && (!i || !j || !cap || !rev_cap))) FAIL(MGC_E_ARG, "null edge arrays");
     for (int64_t k = 0; k < count; ++k) {
         if (i[k] < 0 || j[k] < 0 || i[k] >= g->n || j[k] >= g->n || i[k] == j[k])
-            SPFAIL(MGC_E_ARG, "invalid node ids (" + std::to_string(i[k]) + ", " + std::to_string(j[k]) + ")");
-        if (!std::isfinite(cap[k]) || !std::isfinite(rev_cap[k])) SPFAIL(MGC_E_ARG, "decrements hold NaN or infinite values");
-        if (cap[k] < 0 || rev_cap[k] < 0) SPFAIL(MGC_E_WEIGHT, "decrements are nonnegative amounts");
+            FAIL(MGC_E_ARG, "invalid node ids (" + std::to_string(i[k]) + ", " + std::to_string(j[k]) + ")");
+        if (!std::isfinite(cap[k]) || !std::isfinite(rev_cap[k])) FAIL(MGC_E_ARG, "decrements hold NaN or infinite values");
+        if (cap[k] < 0 || rev_cap[k] < 0) FAIL(MGC_E_WEIGHT, "decrements are nonnegative amounts");
     }
-    if (g->resident && g->warm_bad) SPFAIL(MGC_E_STATE, warm_bad_msg);
+    if (g->resident && g->warm_bad) FAIL(MGC_E_STATE, warm_bad_msg);
     if (count == 0) return MGC_OK;
     std::vector<unsigned> pk;
     std::vector<int32_t> lo, hi;
     std::vector<double> d_lh, d_hl;
-    SPRC(warm_resolve(g, count, i, j, cap, rev_cap, false, pk, lo, hi, d_lh, d_hl));
+    RC(warm_resolve(g, count, i, j, cap, rev_cap, false, pk, lo, hi, d_lh, d_hl));
     // per pair: the decrements summed in call order, pairs in order of their first call
     std::unordered_map<unsigned, size_t> slot;
     std::vector<unsigned> pairs;
@@ -805,12 +771,12 @@ int mgc_sparse_remove_edges_warm(mgc_sparse* g, int64_t count, const int32_t* i,
     if (g->resident) {
         std::vector<int32_t> ol((size_t)count), oh((size_t)count);
         for (int64_t k = 0; k < count; ++k) { ol[(size_t)k] = g->olo[pk[(size_t)k]]; oh[(size_t)k] = g->ohi[pk[(size_t)k]]; }
-        SPRC(warm_fold_decrements(g, pk, lo, hi, ol, oh, d_lh, d_hl));
+        RC(warm_fold_decrements(g, pk, lo, hi, ol, oh, d_lh, d_hl));
     } else {
         // before the first solve: the same pair rule on the accumulated capacities
         for (size_t q = 0; q < pairs.size(); ++q)
             if (spw_pair_refused(g->cap_lh[pairs[q]], g->cap_hl[pairs[q]], sl[q], sh[q]))
-                SPFAIL(MGC_E_WEIGHT, "remove_edges_warm: a pair's decrements exceed its capacities c(i->j) + c(j->i) (the graph "
+                FAIL(MGC_E_WEIGHT, "remove_edges_warm: a pair's decrements exceed its capacities c(i->j) + c(j->i) (the graph "
                                      "is unchanged)");
     }
     for (size_t q = 0; q < pairs.size(); ++q) {
@@ -845,7 +811,7 @@ int mgc_sparse_get_mask(mgc_sparse* g, uint8_t* out)
 int mgc_sparse_what_segment(mgc_sparse* g, int64_t node, int32_t* segment)
 {
     if (!g || !segment) return MGC_E_ARG;
-    if (node < 0 || node >= g->n) SPFAIL(MGC_E_ARG, "node id out of range");
+    if (node < 0 || node >= g->n) FAIL(MGC_E_ARG, "node id out of range");
     if (!g->solved) { int rc = sparse_solve(g); if (rc) return rc; }
     *segment = g->mask[(size_t)node] ? MGC_SOURCE : MGC_SINK;
     return MGC_OK;
@@ -893,8 +859,8 @@ struct mgc_labels {
     std::string err;
 };
 
-#undef SPCK
-#undef SPFAIL
+#undef CK
+#undef FAIL
 #define LBCK(call)                                                                                 \
     do {                                                                                           \
         cudaError_t _e = (call);                                                                   \

@@ -11,7 +11,8 @@
 //
 //  * k_init_tile          : solver state from the terms (source-excess clamp, residual mask, first labels) and
 //                           the first worklists, fused in one pass over the lattice.
-//  * k_relabel_reset      : start of a later global relabel: labels from the residual mask, new worklist.
+//  * k_relabel_reset      : start of a later global relabel: labels from the residual mask, new worklist
+//                           (gc_solve_kernels.cuh, with the z-slab kernels in gc_slab_kernels.cuh).
 //  * relabel_visit        : exact backward BFS from the sink (global relabel), one tile visit; k_bfs_coop
 //                           (gc_persist.cuh) runs every pass in one cooperative launch.  Labels only decrease during it,
 //                           so tiles run concurrently with benign races on the halo; a tile whose border labels
@@ -53,6 +54,13 @@ struct WorkList {
     int* items;
     int* count;
 };
+
+// control block in device memory (ints): mgc_graph::d_tcount (gc_handle.cuh)
+//   [0],[1]   relabel list counts          [2..5] push list counts [colour*2 + buffer]
+//   [8]       work cursor                  [11] relabel list consumed next                [15] relabel passes
+#define CTL_CURSOR 8
+#define CTL_RLCUR 11
+#define CTL_RELP 15
 
 __device__ __forceinline__ int hidx(int z, int y, int x) { return (z * HALO_DIM + y) * HALO_DIM + x; }
 
@@ -190,72 +198,6 @@ __global__ void __launch_bounds__(TILE_VOX) k_init_tile(Lattice L, Tiles TL, Sta
         if (any_exc) {
             const WorkList& pl = tile_color(c) ? pl1 : pl0;
             pl.items[atomicAdd(pl.count, 1)] = c.t;
-        }
-    }
-}
-
-// later global relabels: labels from the (incrementally maintained) residual mask; 1 B read + 4 B written per voxel.
-// One thread per 8-voxel x-run of a tile row, consecutive threads on consecutive runs (coalesced); rflag must be
-// zero on entry (the host memsets it): a run that holds an unlabelled voxel with residual out-arcs lists its tile.
-__global__ void __launch_bounds__(256) k_relabel_reset(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask,
-                                                       int* __restrict__ height, int* __restrict__ rflag, WorkList rl)
-{
-    const unsigned ntx = (unsigned)TL.nt[2];
-    const unsigned nruns = (unsigned)L.dim[0] * (unsigned)L.dim[1] * ntx;
-    for (unsigned r = blockIdx.x * blockDim.x + threadIdx.x; r < nruns; r += gridDim.x * blockDim.x) {
-        const unsigned tx = r % ntx, zy = r / ntx;
-        const unsigned gy = zy % (unsigned)L.dim[1], gz = zy / (unsigned)L.dim[1];
-        const unsigned x0 = tx * TILE;
-        const int nx = (int)min((unsigned)TILE, (unsigned)L.dim[2] - x0);
-        const unsigned base = gz * L.stride[0] + gy * L.stride[1] + x0;
-        const bool own = (int)gz >= L.own0 && (int)gz < L.own1;
-        int needs = 0;
-        if (nx == TILE && (base & 7u) == 0u) {
-            const uint2 m8 = *reinterpret_cast<const uint2*>(rmask + base);
-            int h[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const unsigned m = ((i < 4 ? m8.x : m8.y) >> (8 * (i & 3))) & 0xffu;
-                h[i] = (own && (m & RM_SINK)) ? 1 : MGC_HINF;
-                needs |= (own && (m & 0x3fu) != 0 && h[i] == MGC_HINF) ? 1 : 0;
-            }
-            int4* dst = reinterpret_cast<int4*>(height + base);
-            dst[0] = make_int4(h[0], h[1], h[2], h[3]);
-            dst[1] = make_int4(h[4], h[5], h[6], h[7]);
-        } else {
-            for (int i = 0; i < nx; ++i) {
-                const unsigned m = rmask[base + i];
-                const int h = (own && (m & RM_SINK)) ? 1 : MGC_HINF;
-                height[base + i] = h;
-                needs |= (own && (m & 0x3fu) != 0 && h == MGC_HINF) ? 1 : 0;
-            }
-        }
-        if (needs) list_push(rflag, rl, (int)(((gz >> 3) * (unsigned)TL.nt[1] + (gy >> 3)) * ntx + tx));
-    }
-}
-
-// the same reset restricted to the DIRTY tiles (Tiles::ditems): every other tile is still in the reset state, so an easy
-// instance (regional term: the BFS only ever labels the few tiles around the objects) pays for those tiles instead of a
-// 5 B/voxel pass over the lattice.  Persistent CTAs of one
-// tile each; clears the dirty flags it consumes (the host zeroes the count afterwards).
-__global__ void __launch_bounds__(TILE_VOX) k_relabel_reset_list(Lattice L, Tiles TL, const uint8_t* __restrict__ rmask,
-                                                                 int* __restrict__ height, int* __restrict__ rflag, WorkList rl)
-{
-    const int n = *(volatile int*)TL.dcount;
-    for (int i = blockIdx.x; i < n; i += gridDim.x) {
-        const int t = TL.ditems[i];
-        const TileCtx c = tile_ctx(L, TL, t);
-        int needs = 0;
-        if (c.inb) {
-            const unsigned m = rmask[c.v];
-            const int h = (c.own && (m & RM_SINK)) ? 1 : MGC_HINF;
-            height[c.v] = h;
-            needs = (c.own && (m & 0x3fu) != 0 && h == MGC_HINF) ? 1 : 0;
-        }
-        const int any = __syncthreads_or(needs);
-        if (threadIdx.x == 0) {
-            TL.dflag[t] = 0;
-            if (any) list_push(rflag, rl, t);
         }
     }
 }
@@ -475,44 +417,5 @@ __global__ void __launch_bounds__(TILE_VOX, 2) k_push_tile(Lattice L, Tiles TL, 
         const int t = fetch_tile(cur, cursor, &s_slot);
         if (t < 0) break;
         push_visit_staged<T>(L, TL, S, iters, pflag, self_next, other_next, t, s_out, s_h, nullptr, labels_capped != 0);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// z-slab border messages (written by k_slab_pack of gc_solver.cuh; k_slab_unpack_tiles4 is the 4-D form): ghost
-// labels <- the neighbour's border labels; received flow joins the excess of the border voxel and the residual of its
-// arc towards the ghost (the reverse of the arc the flow arrived on), and the border voxel's residual mask gains that
-// arc.  The receiving tiles are put on the worklists -- the relabel list when a ghost label changed, the push list of
-// the tile's colour when flow arrived.
-// ---------------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void k_slab_unpack_tiles(Lattice L, Tiles TL, State<T> S, int z_ghost, int z_border, int k_border_to_ghost,
-                                    const int* __restrict__ h_in, const double* __restrict__ f_in,
-                                    int* __restrict__ rflag, WorkList rl0, WorkList rl1, const int* __restrict__ rl_cur,
-                                    int* __restrict__ pflag, WorkList pl0, WorkList pl1, int* __restrict__ changed)
-{
-    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= L.plane) return;
-    // the relabel list consumed next: the cooperative BFS keeps its selector in the control block
-    const WorkList rl = *rl_cur ? rl1 : rl0;
-    const int y = (int)(i / L.stride[1]), x = (int)(i % L.stride[1]);
-    const unsigned vg = (unsigned)z_ghost * L.plane + i, vb = (unsigned)z_border * L.plane + i;
-    const int tg = ((z_ghost / TILE) * TL.nt[1] + y / TILE) * TL.nt[2] + x / TILE;
-    const int tb = ((z_border / TILE) * TL.nt[1] + y / TILE) * TL.nt[2] + x / TILE;
-    const int hn = h_in[i];
-    if (S.height[vg] != hn) {
-        S.height[vg] = hn;
-        mark_dirty(TL, tg);
-        if (changed) *changed = 1;
-        list_push(rflag, rl, tb);
-        if (tg != tb) list_push(rflag, rl, tg);
-    }
-    const double f = f_in ? f_in[i] : 0.0;
-    if (f > 0) {
-        S.excess[vb] += (T)f;
-        S.cap[k_border_to_ghost][vb] += (T)f;
-        S.rmask[vb] |= (uint8_t)(1u << k_border_to_ghost);
-        const int color = ((z_border / TILE) + y / TILE + x / TILE) & 1;
-        list_push(pflag, color ? pl1 : pl0, tb);
     }
 }

@@ -143,26 +143,6 @@ __global__ void __launch_bounds__(T4_VOX) k_init_tile4(Lattice L, Tiles4 TL, Sta
     }
 }
 
-// labels from the residual masks; one CTA per tile
-__global__ void __launch_bounds__(T4_VOX) k_relabel_reset4(Lattice L, Tiles4 TL, const uint8_t* __restrict__ rmask,
-                                                           const uint8_t* __restrict__ smask, int* __restrict__ height,
-                                                           int* __restrict__ rflag, WorkList rl)
-{
-    const Tile4Ctx c = tile4_ctx(L, TL, blockIdx.x);
-    int needs = 0;
-    if (c.inb) {
-        const unsigned m = rmask[c.v];
-        const int h = (c.own && smask[c.v]) ? 1 : MGC_HINF;
-        height[c.v] = h;
-        needs = (c.own && m != 0 && h == MGC_HINF) ? 1 : 0;
-    }
-    const int any_needs = __syncthreads_or(needs);
-    if (threadIdx.x == 0) {
-        rflag[c.t] = any_needs;
-        if (any_needs) rl.items[atomicAdd(rl.count, 1)] = c.t;
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------
 // global relabel: one tile visit (k_bfs_coop4 of gc_persist.cuh runs the passes over the worklists)
 // ---------------------------------------------------------------------------------------------------
@@ -321,41 +301,5 @@ __global__ void __launch_bounds__(T4_VOX) k_count_active_tiles4(Lattice L, Tiles
         const bool act = c.own && (S.excess[c.v] > 0) && (S.height[c.v] < MGC_HINF);
         const unsigned b = __ballot_sync(0xffffffffu, act);
         if ((threadIdx.x & 31) == 0 && b) atomicAdd(count, (unsigned long long)__popc(b));
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// z-slab border messages (cf. k_slab_unpack_tiles): ghost labels <- the neighbour's border labels, received flow joins
-// the border voxel's excess and its arc towards the ghost; the receiving tiles go on the relabel list consumed next
-// (ghost label changed) or on the push list of their colour (flow arrived).  4-D lattices keep no dirty tiles to mark.
-// ---------------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void k_slab_unpack_tiles4(Lattice L, Tiles4 TL, State<T> S, int z_ghost, int z_border, int k_border_to_ghost,
-                                     const int* __restrict__ h_in, const double* __restrict__ f_in,
-                                     int* __restrict__ rflag, WorkList rl0, WorkList rl1, const int* __restrict__ rl_cur,
-                                     int* __restrict__ pflag, WorkList pl0, WorkList pl1, int* __restrict__ changed)
-{
-    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= L.plane) return;
-    const WorkList rl = *rl_cur ? rl1 : rl0;
-    const unsigned r = i % L.stride[1];
-    const int c1 = (int)(i / L.stride[1]), c2 = (int)(r / L.stride[2]), c3 = (int)(r % L.stride[2]);
-    const unsigned vg = (unsigned)z_ghost * L.plane + i, vb = (unsigned)z_border * L.plane + i;
-    const int tg = (((z_ghost >> 2) * TL.nt[1] + (c1 >> 2)) * TL.nt[2] + (c2 >> 3)) * TL.nt[3] + (c3 >> 2);
-    const int tb = (((z_border >> 2) * TL.nt[1] + (c1 >> 2)) * TL.nt[2] + (c2 >> 3)) * TL.nt[3] + (c3 >> 2);
-    const int hn = h_in[i];
-    if (S.height[vg] != hn) {
-        S.height[vg] = hn;
-        if (changed) *changed = 1;
-        list_push(rflag, rl, tb);
-        if (tg != tb) list_push(rflag, rl, tg);
-    }
-    const double f = f_in ? f_in[i] : 0.0;
-    if (f > 0) {
-        S.excess[vb] += (T)f;
-        S.cap[k_border_to_ghost][vb] += (T)f;
-        S.rmask[vb] |= (uint8_t)(1u << k_border_to_ghost);
-        const int color = ((z_border >> 2) + (c1 >> 2) + (c2 >> 3) + (c3 >> 2)) & 1;
-        list_push(pflag, color ? pl1 : pl0, tb);
     }
 }
