@@ -14,6 +14,8 @@ import enum
 
 import numpy
 
+from . import _warm_args
+
 __all__ = ["GraphDouble", "GraphFloat", "GraphInt"]
 
 
@@ -30,6 +32,12 @@ def _strides_of(shape):
         st.append(acc)
         acc *= int(s)
     return tuple(reversed(st))
+
+
+def _cannot_fold(rebuild):
+    """The refusal of a warm call that a solved general sparse graph, created without warm=True, cannot fold."""
+    return RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and rebuild "
+                        "it {} instead".format(rebuild))
 
 
 class GraphDouble:
@@ -434,40 +442,6 @@ class GraphDouble:
         self._solved = True
         return flow
 
-    def _seed_ids(self, seeds):
-        """Node ids of one seed argument: a boolean mask of the lattice shape (any strides; ids in the logical C order,
-        like generate.py:169-172), or a 1-D integer id array; numpy or a CUDA tensor.  Range-checked like
-        GCGraph.set_source_nodes (graph.py:334-339)."""
-        if seeds is None:
-            return None
-        if hasattr(seeds, "__cuda_array_interface__"):
-            import torch
-            t = torch.as_tensor(seeds)
-            if t.dtype == torch.bool:
-                if tuple(t.shape) != self._shape:
-                    raise ValueError("seed mask of shape {} does not match the graph's shape {}".format(tuple(t.shape), self._shape))
-                ids = t.reshape(-1).nonzero().reshape(-1)
-            else:
-                if t.dim() != 1 or t.dtype.is_floating_point or t.dtype.is_complex:
-                    raise ValueError("seeds must be a boolean mask of the graph's shape or a 1-D integer id array")
-                ids = t.to(torch.int64).contiguous()
-            if ids.numel():
-                lo, hi = int(ids.min()), int(ids.max())
-                if hi >= self._n or lo < 0:
-                    raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(hi, lo, self._n - 1))
-            return ids
-        a = numpy.asarray(seeds)
-        if a.dtype == numpy.bool_:
-            if a.shape != self._shape:
-                raise ValueError("seed mask of shape {} does not match the graph's shape {}".format(a.shape, self._shape))
-            return a.ravel().nonzero()[0].astype(numpy.int64)
-        if a.ndim != 1 or not (a.size == 0 or numpy.issubdtype(a.dtype, numpy.integer)):
-            raise ValueError("seeds must be a boolean mask of the graph's shape or a 1-D integer id array")
-        ids = a.astype(numpy.int64)
-        if ids.size and (ids.max() >= self._n or ids.min() < 0):
-            raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(ids.max(), ids.min(), self._n - 1))
-        return ids
-
     def add_seeds(self, fg=None, bg=None):
         """Add foreground / background seeds and let the next ``maxflow()`` return the cut of the enlarged graph.
 
@@ -482,7 +456,7 @@ class GraphDouble:
         build the graph again with the seeds."""
         if self._warm_sparse():
             return self._sp.add_seeds(fg, bg)
-        self._fold_seeds(fg, bg, 65535.0, "add_seeds", "with")
+        self._fold_seeds(fg, bg, 65535.0, "add_seeds", "with the seeds")
 
     def remove_seeds(self, fg=None, bg=None):
         """Erase foreground / background seeds and let the next ``maxflow()`` return the cut of the reduced graph.
@@ -499,22 +473,37 @@ class GraphDouble:
         ``RuntimeError``: ``reset()`` it and build the graph again without the seeds."""
         if self._warm_sparse():
             return self._sp.remove_seeds(fg, bg)
-        self._fold_seeds(fg, bg, -65535.0, "remove_seeds", "without")
+        self._fold_seeds(fg, bg, -65535.0, "remove_seeds", "without the seeds")
 
     def _fold_seeds(self, fg, bg, cap, native, rebuild):
-        fg_ids, bg_ids = self._seed_ids(fg), self._seed_ids(bg)
+        ids = [None if x is None else _warm_args.node_ids(x, self._shape, self._n, what)
+               for x, what in ((fg, "fg"), (bg, "bg"))]
+        self._warm_call(native, ids, lambda f, b: self._stage_seeds(f, b, cap), rebuild)
+
+    def _stage_seeds(self, fg, bg, cap):
+        for ids, src, snk in ((fg, cap, 0.0), (bg, 0.0, cap)):
+            if ids is not None and len(ids):
+                self.stage_tweights_many(ids, src, snk)
+
+    def _warm_call(self, native, args, stage, rebuild):
+        """One warm call on parsed arguments: before the first solve (and before a removal folded) ``stage`` takes host
+        copies of them; after it the native fold ``native`` reads them where they are.  ``rebuild`` completes the refusal
+        of a graph that cannot fold."""
         if not self._solved and not self._folded:
-            for ids, src, snk in ((fg_ids, cap, 0.0), (bg_ids, 0.0, cap)):
-                if ids is not None and len(ids):
-                    if not isinstance(ids, numpy.ndarray):
-                        ids = ids.cpu().numpy()
-                    self.stage_tweights_many(ids, src, snk)
-            return
+            return stage(*(a.cpu().numpy() if _warm_args.on_device(a) else a for a in args))
         if self._sp is not None:
-            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it {} the seeds instead".format(rebuild))
+            raise _cannot_fold(rebuild)
         self._dirty()
-        getattr(self._nat(), native)(fg_ids, bg_ids)
+        getattr(self._nat(), native)(*args)
+
+    @staticmethod
+    def _one_space(message, *args):
+        """Whether the arguments of one warm call are on the device.  The native folds take their arrays all on the host or
+        all on the device: a mix raises ``ValueError(message)``; host scalars go with either."""
+        cuda = any(_warm_args.on_device(x) for x in args)
+        if cuda and any(not _warm_args.on_device(x) and numpy.ndim(x) for x in args):
+            raise ValueError(message)
+        return cuda
 
     def add_tweights_warm(self, nodes, cap_source, cap_sink):
         """``add_tweights`` calls on a solved graph, re-solved warm by the next ``maxflow()``: soft strokes, a GrabCut-style
@@ -535,65 +524,13 @@ class GraphDouble:
         build the graph again with the calls."""
         if self._warm_sparse():
             return self._sp.add_tweights_warm(nodes, cap_source, cap_sink)
-        cuda = any(hasattr(x, "__cuda_array_interface__") for x in (nodes, cap_source, cap_sink))
-        ids = self._seed_ids(nodes) if nodes is not None else None
-        if cuda and ids is not None and not hasattr(ids, "__cuda_array_interface__"):
-            raise ValueError("nodes, cap_source and cap_sink must all be host or all be device arrays")
-        m = self._n if ids is None else int(ids.shape[0])
-        src = self._warm_weights(cap_source, m, ids is None, cuda, "cap_source")
-        snk = self._warm_weights(cap_sink, m, ids is None, cuda, "cap_sink")
-        if not self._solved and not self._folded:
-            if cuda:
-                ids = None if ids is None else ids.cpu().numpy()
-                src, snk = src.cpu().numpy(), snk.cpu().numpy()
-            for w, what in ((src, "cap_source"), (snk, "cap_sink")):
-                if not numpy.isfinite(w).all():
-                    raise ValueError("{} holds NaN or infinite values".format(what))
-            self._stage_tweights_calls(ids, src, snk)
-            return
-        if self._sp is not None:
-            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it with the t-link calls instead")
-        self._dirty()
-        self._nat().add_tweights_warm(ids, src, snk)
-
-    def _warm_weights(self, w, m, dense, cuda, what):
-        """One weight argument of add_tweights_warm as m contiguous float64 values (a numpy array, or a CUDA tensor when
-        ``cuda``), checked for shape.  Finiteness is checked where the calls land: by the staging, or by the native fold in
-        the same pass that groups them."""
-        on_device = hasattr(w, "__cuda_array_interface__")
-        if cuda and on_device:
-            import torch
-            t = torch.as_tensor(w)
-            if t.dtype == torch.bool or t.dtype.is_complex:
-                raise ValueError("{} must hold real numbers".format(what))
-        else:
-            a = numpy.asarray(w)
-            if a.dtype.kind not in "iuf":
-                raise ValueError("{} must hold real numbers".format(what))
-            if cuda and a.ndim:
-                raise ValueError("nodes, cap_source and cap_sink must all be host or all be device arrays")
-            if cuda:
-                import torch
-                t = torch.as_tensor(a)
-            else:
-                t = a
-        if t.ndim == 0:
-            full = (lambda v: torch.full((m,), v, dtype=torch.float64, device="cuda")) if cuda else \
-                (lambda v: numpy.full(m, v, dtype=numpy.float64))
-            out = full(float(t))
-        else:
-            shape = tuple(t.shape)
-            if dense and shape != self._shape and shape != (self._n,):
-                raise ValueError("{} of shape {} does not match the graph's shape {} or its {} nodes".format(
-                    what, shape, self._shape, self._n))
-            if not dense and (len(shape) != 1 or shape[0] != m):
-                raise ValueError("{} has shape {}, expected {} entries like the node ids".format(what, shape, m))
-            if cuda:
-                out = t.reshape(-1).to(torch.float64).contiguous()
-            else:
-                out = numpy.ascontiguousarray(t.reshape(-1), dtype=numpy.float64)
-        return out
+        cuda = self._one_space("nodes, cap_source and cap_sink must all be host or all be device arrays",
+                               nodes, cap_source, cap_sink)
+        ids = None if nodes is None else _warm_args.node_ids(nodes, self._shape, self._n, "nodes")
+        m, dense = (self._n, self._shape) if ids is None else (ids.shape[0], None)
+        src = _warm_args.weights(cap_source, m, "cap_source", dense, cuda)
+        snk = _warm_args.weights(cap_sink, m, "cap_sink", dense, cuda)
+        self._warm_call("add_tweights_warm", (ids, src, snk), self._stage_tweights_calls, "with the t-link calls")
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
         """``sum_edge`` calls on a solved graph, re-solved warm by the next ``maxflow()``: a boundary brush ("do not cut
@@ -610,35 +547,15 @@ class GraphDouble:
         ``RuntimeError``: ``reset()`` it and build the graph again with the calls."""
         if self._warm_sparse():
             return self._sp.add_nweights_warm(i, j, cap, rev_cap)
-        ii, jj, c, r, cuda = self._nweights_call_args(i, j, cap, rev_cap)
-        if not self._solved and not self._folded:
-            if cuda:
-                ii, jj, c, r = (x.cpu().numpy() for x in (ii, jj, c, r))
-            self._stage_nweights_calls(ii, jj, c, r)
-            return
-        if self._sp is not None:
-            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it with the n-link calls instead")
-        self._dirty()
-        self._nat().add_nweights_warm(ii, jj, c, r)
+        ii, jj, c, r, _ = self._nlink_args(i, j, cap, rev_cap)
+        self._warm_call("add_nweights_warm", (ii, jj, c, r), self._stage_nweights_calls, "with the n-link calls")
 
-    def _nweights_call_args(self, i, j, cap, rev_cap):
-        """The arguments of add_nweights_warm / remove_nweights_warm as four contiguous 1-D arrays of one length (int64
-        ids, float64 weights; numpy, or CUDA tensors when any argument is one), and whether they are on the device."""
-        cuda = any(hasattr(x, "__cuda_array_interface__") for x in (i, j, cap, rev_cap))
-        ii, jj = self._pair_ids(i, cuda, "i"), self._pair_ids(j, cuda, "j")
-        sizes = {int(x.shape[0]) for x in (ii, jj) if x.ndim}
-        if len(sizes) > 1:
-            raise ValueError("i and j differ in length")
-        # a scalar id pair takes the length of the weights, so (5, 6, [1.0, 2.0], 0.0) is two calls on one pair
-        wshapes = [tuple(w.shape) if hasattr(w, "shape") else numpy.shape(w) for w in (cap, rev_cap)]
-        wsizes = {int(sh[0]) for sh in wshapes if len(sh) == 1}
-        m = sizes.pop() if sizes else (wsizes.pop() if len(wsizes) == 1 else 1)
-        ii, jj = (x.expand(m) if cuda else numpy.broadcast_to(x, (m,)) for x in (ii, jj))
-        ii, jj = ((x.contiguous() if cuda else numpy.ascontiguousarray(x)) for x in (ii, jj))
-        c = self._warm_weights(cap, m, False, cuda, "cap")
-        r = self._warm_weights(rev_cap, m, False, cuda, "rev_cap")
-        return ii, jj, c, r, cuda
+    def _nlink_args(self, i, j, cap, rev_cap):
+        """The arguments of add_nweights_warm / remove_nweights_warm as four contiguous 1-D arrays of one length (int64 ids,
+        float64 weights), and whether they are on the device."""
+        cuda = self._one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
+        ii, jj = _warm_args.pair_ids(i, self._n, "i"), _warm_args.pair_ids(j, self._n, "j")
+        return _warm_args.nlink_calls(ii, jj, cap, rev_cap, cuda) + (cuda,)
 
     def add_nweights_dense_warm(self, axis, fwd, bwd):
         """The dense form of ``add_nweights_warm``, in the layout of ``add_nweights_dense``: ``fwd`` / ``bwd`` have the
@@ -651,52 +568,34 @@ class GraphDouble:
         as ``add_nweights_warm`` fold it into the solved state (mgc_add_nweights_dense_warm)."""
         if self._warm_sparse():
             return self._sp.add_nweights_dense_warm(axis, fwd, bwd)
-        axis, fwd, bwd, cuda = self._dense_nweights_args(axis, fwd, bwd)
-        if not self._solved and not self._folded:
-            if cuda:
-                fwd, bwd = fwd.cpu().numpy(), bwd.cpu().numpy()
-            cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
-            for w, what in ((fwd, "fwd"), (bwd, "bwd")):
-                if not numpy.isfinite(w[cut]).all():
-                    raise ValueError("{} holds NaN or infinite values".format(what))
-                if (w[cut] < 0).any():
-                    raise ValueError("{} holds negative values: a warm n-link edit only raises capacities".format(what))
-            staged = [numpy.zeros(self._shape), numpy.zeros(self._shape)]
-            staged[0][cut], staged[1][cut] = fwd[cut], bwd[cut]        # the last plane of `axis` names no pair
-            self.add_nweights_dense(axis, *staged)
-            return
-        if self._sp is not None:
-            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it with the n-link calls instead")
-        self._dirty()
-        self._nat().add_nweights_dense_warm(axis, fwd, bwd)
+        axis, fwd, bwd, _ = self._dense_args(axis, fwd, bwd)
+        self._warm_call("add_nweights_dense_warm", (axis, fwd, bwd), self._stage_nweights_dense, "with the n-link calls")
 
-    def _dense_nweights_args(self, axis, fwd, bwd):
-        """The arguments of the dense n-link folds: the axis, checked, and fwd / bwd as float64 arrays of the lattice shape
-        (numpy, or CUDA tensors when either is one), and whether they are on the device."""
+    def _dense_args(self, axis, fwd, bwd):
+        """The arguments of the dense n-link folds: the axis, checked, and fwd / bwd as float64 arrays of the lattice shape;
+        and whether they are on the device."""
         axis = int(axis)
         if not 0 <= axis < len(self._shape):
             raise ValueError("axis {} is out of range for a graph of shape {}".format(axis, self._shape))
-        cuda = any(hasattr(x, "__cuda_array_interface__") for x in (fwd, bwd))
-        arrs = []
-        for w, what in ((fwd, "fwd"), (bwd, "bwd")):
-            if cuda:
-                if not hasattr(w, "__cuda_array_interface__"):
-                    raise ValueError("fwd and bwd must both be host or both be device arrays")
-                import torch
-                t = torch.as_tensor(w)
-                if t.dtype == torch.bool or t.dtype.is_complex:
-                    raise ValueError("{} must hold real numbers".format(what))
-                t = t.to(torch.float64)
-            else:
-                t = numpy.asarray(w)
-                if t.dtype.kind not in "iuf":
-                    raise ValueError("{} must hold real numbers".format(what))
-                t = t.astype(numpy.float64, copy=False)
-            if tuple(t.shape) != self._shape:
-                raise ValueError("{} of shape {} does not match the graph's shape {}".format(what, tuple(t.shape), self._shape))
-            arrs.append(t)
-        return (axis,) + tuple(arrs) + (cuda,)
+        cuda = self._one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
+        fwd, bwd = _warm_args.real(fwd, "fwd"), _warm_args.real(bwd, "bwd")
+        for a, what in ((fwd, "fwd"), (bwd, "bwd")):
+            if tuple(a.shape) != self._shape:
+                raise ValueError("{} of shape {} does not match the graph's shape {}".format(what, tuple(a.shape), self._shape))
+        return axis, fwd, bwd, cuda
+
+    def _pairs_of_axis(self, axis):
+        """The entries of a dense n-link array that name a pair: the last plane of ``axis`` names none."""
+        return tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
+
+    def _stage_nweights_dense(self, axis, fwd, bwd):
+        """add_nweights_dense_warm before the first solve: checked like the warm fold checks it, then staged exactly like
+        ``add_nweights_dense``."""
+        cut = self._pairs_of_axis(axis)
+        _warm_args.check_amounts(((fwd[cut], "fwd"), (bwd[cut], "bwd")), _warm_args.ONLY_RAISES)
+        staged = [numpy.zeros(self._shape), numpy.zeros(self._shape)]
+        staged[0][cut], staged[1][cut] = fwd[cut], bwd[cut]
+        self.add_nweights_dense(axis, *staged)
 
     def remove_nweights_warm(self, i, j, cap, rev_cap):
         """The inverse of ``add_nweights_warm``: n-link capacity taken off the graph, re-solved warm by the next
@@ -718,9 +617,9 @@ class GraphDouble:
         ``RuntimeError``: ``reset()`` it and build the graph again without the weight."""
         if self._warm_sparse():
             return self._sp.remove_nweights_warm(i, j, cap, rev_cap)
-        ii, jj, c, r, cuda = self._nweights_call_args(i, j, cap, rev_cap)
-        if not cuda:
-            self._check_decrements(((c, "cap"), (r, "rev_cap")))
+        ii, jj, c, r, cuda = self._nlink_args(i, j, cap, rev_cap)
+        if not cuda:        # the native grouping checks device decrements in the same pass
+            _warm_args.check_amounts(((c, "cap"), (r, "rev_cap")), _warm_args.DECREMENTS)
         self._fold_decrements("remove_nweights_warm", ii, jj, c, r)
 
     def remove_nweights_dense_warm(self, axis, fwd, bwd):
@@ -729,20 +628,11 @@ class GraphDouble:
         the pairs with a nonzero entry are touched.  Same meaning, checks and errors as ``remove_nweights_warm``."""
         if self._warm_sparse():
             return self._sp.remove_nweights_dense_warm(axis, fwd, bwd)
-        axis, fwd, bwd, cuda = self._dense_nweights_args(axis, fwd, bwd)
+        axis, fwd, bwd, cuda = self._dense_args(axis, fwd, bwd)
         if not cuda:
-            cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
-            self._check_decrements(((fwd[cut], "fwd"), (bwd[cut], "bwd")))
+            cut = self._pairs_of_axis(axis)
+            _warm_args.check_amounts(((fwd[cut], "fwd"), (bwd[cut], "bwd")), _warm_args.DECREMENTS)
         self._fold_decrements("remove_nweights_dense_warm", axis, fwd, bwd)
-
-    @staticmethod
-    def _check_decrements(weights):
-        """Host decrements: finite and nonnegative (the native grouping checks device arrays in the same pass)."""
-        for w, what in weights:
-            if not numpy.isfinite(w).all():
-                raise ValueError("{} holds NaN or infinite values".format(what))
-            if (w < 0).any():
-                raise ValueError("{} holds negative values: n-link decrements are nonnegative amounts".format(what))
 
     def _terms_open(self):
         """Term calls are refused once a removal has folded into the graph before its first solve: the handle then holds
@@ -758,8 +648,7 @@ class GraphDouble:
         init that the first solve would run on an ``enable_warm()`` graph."""
         self._lattice_term()
         if self._sp is not None:
-            raise RuntimeError("a warm re-solve needs a lattice graph built by graph_from_voxels; reset() the graph and "
-                               "rebuild it without the n-link weight instead")
+            raise _cannot_fold("without the n-link weight")
         if self._offlattice is not None:
             raise RuntimeError("edge {} does not join lattice neighbours: reset() the graph and rebuild it without the "
                                "n-link weight instead".format(self._offlattice))
@@ -774,44 +663,12 @@ class GraphDouble:
             raise
         self._folded = self._folded or unsolved
 
-    def _pair_ids(self, x, cuda, what):
-        """One id argument of add_nweights_warm: a 1-D int64 array (or a 0-d one for a scalar), numpy or -- when ``cuda``
-        -- a CUDA tensor.  Range-checked in both memory spaces, as ``_seed_ids`` checks seeds: before the first solve the
-        ids go to the staging, where no native check runs."""
-        if cuda:
-            import torch
-            if not hasattr(x, "__cuda_array_interface__") and numpy.ndim(x):
-                raise ValueError("i, j, cap and rev_cap must all be host or all be device arrays")
-            t = torch.as_tensor(x, device="cuda")
-            if t.dtype == torch.bool or t.dtype.is_floating_point or t.dtype.is_complex or t.dim() > 1:
-                raise ValueError("{} must be a 1-D integer node id array or an integer".format(what))
-            t = t.to(torch.int64)
-            if t.numel():
-                self._check_id_range(int(t.min()), int(t.max()))
-            return t
-        a = numpy.asarray(x)
-        if a.ndim > 1 or not (numpy.issubdtype(a.dtype, numpy.integer) or (a.ndim == 1 and a.size == 0)):
-            raise ValueError("{} must be a 1-D integer node id array or an integer".format(what))
-        a = a.astype(numpy.int64)
-        if a.size:
-            self._check_id_range(int(a.min()), int(a.max()))
-        return a
-
-    def _check_id_range(self, lo, hi):
-        if lo < 0 or hi >= self._n:
-            raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(hi, lo, self._n - 1))
-
     def _stage_nweights_calls(self, i, j, cap, rev):
         """sum_edge(i[k], j[k], cap[k], rev[k]) in order, staged before the first solve: checked like the warm fold checks
         them, then added into the dense per-axis batches exactly as ``sum_edge`` adds (repeated pairs in call order)."""
         for a in (i, j):
-            if a.size:
-                self._check_id_range(int(a.min()), int(a.max()))   # numpy.add.at would wrap a negative id
-        for w, what in ((cap, "cap"), (rev, "rev_cap")):
-            if not numpy.isfinite(w).all():
-                raise ValueError("{} holds NaN or infinite values".format(what))
-            if (w < 0).any():
-                raise ValueError("{} holds negative values: a warm n-link edit only raises capacities".format(what))
+            _warm_args.check_ids(a, self._n)          # numpy.add.at would wrap a negative id
+        _warm_args.check_amounts(((cap, "cap"), (rev, "rev_cap")), _warm_args.ONLY_RAISES)
         if self._sp is not None:
             for a, b, c, r in zip(i.tolist(), j.tolist(), cap.tolist(), rev.tolist()):
                 self._sp.sum_edge(a, b, c, r)
@@ -843,6 +700,8 @@ class GraphDouble:
         """add_tweights(ids[k], src[k], snk[k]) in order (ids None: one call per node), staged before the first solve.
         The k-th call on a node goes into dense batch k: a node's calls keep their order, and no Python loop runs per
         call."""
+        _warm_args.check_finite(src, "cap_source")
+        _warm_args.check_finite(snk, "cap_sink")
         if self._sp is not None:
             return self._sp.add_tweights_bulk(ids, src, snk)
         if self._journal is not None:

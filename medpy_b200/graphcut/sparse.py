@@ -17,9 +17,21 @@ device or built extension.
 """
 import numpy
 
+from . import _warm_args
 from .maxflow import _termtype
 
 __all__ = ["SparseGraphDouble"]
+
+
+def _host(x):
+    """Sparse handles take host arrays: a tensor argument (CUDA or CPU) is copied to numpy before it is parsed."""
+    if hasattr(x, "__cuda_array_interface__") or type(x).__module__.startswith("torch"):
+        return x.detach().cpu().numpy()
+    return x
+
+
+# why a sum_edge call on a solved warm graph may not be negative
+_LOWER = "a solved graph lowers capacities only through remove_nweights_warm"
 
 
 class SparseGraphDouble:
@@ -53,21 +65,6 @@ class SparseGraphDouble:
             if self._warm:
                 self._native.set_option(_lib._mgc.OPT_WARM, 1)
         return self._native
-
-    def _check_warm_tweights(self, src, snk):
-        if self._warm and self._solved and not (numpy.isfinite(src).all() and numpy.isfinite(snk).all()):
-            raise ValueError("t-weights hold NaN or infinite values")
-
-    def _check_warm_edges(self, cap, rev_cap):
-        """Plain sum_edge calls on a solved warm graph fold as increments: capacities only go down through
-        remove_nweights_warm."""
-        if self._warm and self._solved:
-            for w in (cap, rev_cap):
-                if not numpy.isfinite(w).all():
-                    raise ValueError("edge capacities hold NaN or infinite values")
-                if (numpy.asarray(w) < 0).any():
-                    raise ValueError("a negative sum_edge capacity cannot fold into a solved graph: lower capacities "
-                                     "with remove_nweights_warm")
 
     def _close_edges(self):
         if self._e[0]:
@@ -106,7 +103,9 @@ class SparseGraphDouble:
         """graph.h:415-425."""
         i = int(i)
         self._check_node(i)
-        self._check_warm_tweights(numpy.float64(cap_source), numpy.float64(cap_sink))
+        if self._solved:                    # the call folds into the residual state: finite weights only
+            _warm_args.check_finite(cap_source, "cap_source")
+            _warm_args.check_finite(cap_sink, "cap_sink")
         self._t[0].append(i)
         self._t[1].append(float(cap_source))
         self._t[2].append(float(cap_sink))
@@ -122,12 +121,12 @@ class SparseGraphDouble:
         src = numpy.ascontiguousarray(src, dtype=numpy.float64).ravel()
         snk = numpy.ascontiguousarray(snk, dtype=numpy.float64).ravel()
         if nodes is not None:
-            nodes = numpy.ascontiguousarray(nodes, dtype=numpy.int32).ravel()
-            if nodes.size and (nodes.min() < 0 or nodes.max() >= self._n):
-                raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(nodes.max(), nodes.min(), self._n - 1))
+            nodes = _warm_args.check_ids(numpy.ascontiguousarray(nodes, dtype=numpy.int32).ravel(), self._n)
         elif src.size > self._n:
             raise ValueError("Invalid node id of {}. Valid values are 0 to {}.".format(src.size - 1, self._n - 1))
-        self._check_warm_tweights(src, snk)
+        if self._solved:
+            _warm_args.check_finite(src, "cap_source")
+            _warm_args.check_finite(snk, "cap_sink")
         self._close_tweights()
         self._ops.append(("t", nodes, src, snk))
         self._mask = None
@@ -137,7 +136,8 @@ class SparseGraphDouble:
         i, j = int(i), int(j)
         if i < 0 or j < 0 or i >= self._n or j >= self._n or i == j:
             raise ValueError("invalid node ids ({}, {})".format(i, j))
-        self._check_warm_edges(numpy.float64(cap), numpy.float64(rev_cap))
+        if self._solved:                    # the call folds as an increment
+            _warm_args.check_amounts(((cap, "cap"), (rev_cap, "rev_cap")), _LOWER)
         self._e[0].append(i)
         self._e[1].append(j)
         self._e[2].append(float(cap))
@@ -156,7 +156,8 @@ class SparseGraphDouble:
             raise ValueError("edge arrays differ in length")
         if i.size and (min(i.min(), j.min()) < 0 or max(i.max(), j.max()) >= self._n or (i == j).any()):
             raise ValueError("invalid node ids in the edge arrays")
-        self._check_warm_edges(cap, rev_cap)
+        if self._solved:
+            _warm_args.check_amounts(((cap, "cap"), (rev_cap, "rev_cap")), _LOWER)
         self._close_edges()
         self._ops.append(("e", i, j, cap, rev_cap))
         self._mask = None
@@ -215,36 +216,17 @@ class SparseGraphDouble:
                                "instead".format(what))
 
     def _ids(self, x, what):
-        """Node ids of one warm-call argument: a 1-D integer array or a boolean mask of shape (n,); numpy or a tensor
-        (copied to the host: sparse handles take host arrays)."""
-        if hasattr(x, "__cuda_array_interface__") or type(x).__module__.startswith("torch"):
-            x = x.detach().cpu().numpy()
-        a = numpy.asarray(x)
-        if a.dtype == numpy.bool_:
-            if a.shape != (self._n,):
-                raise ValueError("{} mask of shape {} does not match the graph's {} nodes".format(what, a.shape, self._n))
-            return a.nonzero()[0].astype(numpy.int32)
-        if a.ndim > 1 or not (a.size == 0 or numpy.issubdtype(a.dtype, numpy.integer)):
-            raise ValueError("{} must be a boolean mask of shape (n,) or a 1-D integer id array".format(what))
-        a = a.reshape(-1).astype(numpy.int64)
-        if a.size and (a.min() < 0 or a.max() >= self._n):
-            raise ValueError("Invalid node id of {} or {}. Valid values are 0 to {}.".format(a.max(), a.min(), self._n - 1))
-        return a.astype(numpy.int32)
+        """Node ids of one warm-call argument as host int32: a boolean mask of shape (n,), a 1-D integer id array or a
+        single id."""
+        a = numpy.asarray(_host(x))
+        if a.ndim == 0 and a.dtype != numpy.bool_:
+            a = a.reshape(1)
+        return _warm_args.node_ids(a, (self._n,), self._n, what).astype(numpy.int32)
 
     def _weights(self, w, m, what):
-        if hasattr(w, "__cuda_array_interface__") or type(w).__module__.startswith("torch"):
-            w = w.detach().cpu().numpy()
-        a = numpy.asarray(w)
-        if a.dtype.kind not in "iuf":
-            raise ValueError("{} must hold real numbers".format(what))
-        if a.ndim == 0:
-            a = numpy.full(m, float(a), dtype=numpy.float64)
-        if a.shape != (m,):
-            raise ValueError("{} has shape {}, expected ({},)".format(what, a.shape, m))
-        a = numpy.ascontiguousarray(a, dtype=numpy.float64)
-        if not numpy.isfinite(a).all():
-            raise ValueError("{} holds NaN or infinite values".format(what))
-        return a
+        w = _warm_args.weights(_host(w), m, what)
+        _warm_args.check_finite(w, what)
+        return w
 
     def add_seeds(self, fg=None, bg=None):
         """add_tweights(v, 65535, 0) per foreground id in order, then add_tweights(v, 0, 65535) per background id."""
@@ -269,18 +251,15 @@ class SparseGraphDouble:
         m = self._n if ids is None else ids.size
         self.add_tweights_bulk(ids, self._weights(cap_source, m, "cap_source"), self._weights(cap_sink, m, "cap_sink"))
 
-    def _pairs(self, i, j, cap, rev_cap, what):
-        ii, jj = self._ids(numpy.atleast_1d(i) if numpy.ndim(i) == 0 else i, "i"), self._ids(numpy.atleast_1d(j) if numpy.ndim(j) == 0 else j, "j")
+    def _pairs(self, i, j, cap, rev_cap, why):
+        """The sum_edge calls of an n-link edit as host arrays.  Unlike on the lattice, a one-element id array broadcasts
+        to the length of the longest argument."""
+        ii, jj = self._ids(i, "i"), self._ids(j, "j")
+        cap, rev_cap = _host(cap), _host(rev_cap)
         m = max(ii.size, jj.size, *(numpy.size(w) for w in (cap, rev_cap) if numpy.ndim(w)))
-        if ii.size == 1 and m > 1:
-            ii = numpy.full(m, ii[0], numpy.int32)
-        if jj.size == 1 and m > 1:
-            jj = numpy.full(m, jj[0], numpy.int32)
-        if ii.size != jj.size:
-            raise ValueError("i and j differ in length")
-        c, r = self._weights(cap, ii.size, "cap"), self._weights(rev_cap, ii.size, "rev_cap")
-        if (c < 0).any() or (r < 0).any():
-            raise ValueError("{} takes nonnegative amounts".format(what))
+        ii, jj = (numpy.repeat(x, m) if x.size == 1 else x for x in (ii, jj))
+        ii, jj, c, r = _warm_args.nlink_calls(ii, jj, cap, rev_cap)
+        _warm_args.check_amounts(((c, "cap"), (r, "rev_cap")), why)
         if (ii == jj).any():
             raise ValueError("invalid node ids in the edge arrays")
         return ii, jj, c, r
@@ -288,7 +267,7 @@ class SparseGraphDouble:
     def add_nweights_warm(self, i, j, cap, rev_cap):
         """sum_edge(i[k], j[k], cap[k], rev_cap[k]) per entry in order, on any node pairs (new ones included)."""
         self._require_warm("add_nweights_warm")
-        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, "add_nweights_warm")
+        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, _warm_args.ONLY_RAISES)
         if ii.size:
             self.sum_edges_bulk(ii, jj, c, r)
 
@@ -297,7 +276,7 @@ class SparseGraphDouble:
         capacity.  What is staged is folded first, so the call order is kept.  A pair whose decrements exceed what it
         holds (beyond a few hundred roundings) raises ValueError with the graph unchanged."""
         self._require_warm("remove_nweights_warm")
-        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, "remove_nweights_warm")
+        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, _warm_args.DECREMENTS)
         self._flush()
         self._mask = None
         if ii.size:

@@ -200,6 +200,12 @@ def test_hand_check_and_refusals_and_reset():
     assert g.maxflow() == 3.0 and g.get_trcap(0) == 3.0 and g.get_arc_num() == 2
     with pytest.raises(ValueError):
         g.add_nweights_dense_warm(0, numpy.zeros(2), numpy.zeros(2))
+    # host and device arguments mix in one call: a sparse graph copies every argument to the host
+    import torch
+    g.add_tweights_warm(torch.tensor([0, 1], device="cuda"), numpy.array([1.0, 0.0]), torch.tensor([0.0, 1.0], device="cuda"))
+    assert g.maxflow() == 3.0
+    g.add_nweights_warm(torch.tensor([0], device="cuda"), [1], numpy.array([1.0]), 0.0)
+    assert g.maxflow() == 4.0
 
 
 def test_nonfinite_first_solve_refuses_folds():

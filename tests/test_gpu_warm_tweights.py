@@ -277,6 +277,9 @@ def test_bad_ids_and_nan_leave_the_result():
         g.add_tweights_warm(numpy.array([0, n]), 1.0, 0.0)
     with pytest.raises(ValueError, match="NaN"):
         g.add_tweights_warm(numpy.array([0, 1]), numpy.array([1.0, numpy.nan]), 0.0)
+    import torch
+    with pytest.raises(ValueError, match="must all be host or all be device arrays"):
+        g.add_tweights_warm(numpy.array([0, 1]), torch.ones(2, dtype=torch.float64, device="cuda"), 0.0)
     nat = g._nat()
     with pytest.raises(ValueError, match="out of range"):
         nat.add_tweights_warm(numpy.array([5, -1], numpy.int64), numpy.ones(2), numpy.zeros(2))

@@ -6,6 +6,7 @@ import sys
 
 import numpy
 import pytest
+import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fake_native  # noqa: E402
@@ -80,6 +81,9 @@ def test_ids_keep_order_and_duplicates(made):
     g.remove_seeds(fg=[5, 3, 5], bg=numpy.array([7, 7], numpy.int32))
     kind, fg, bg = made[0].seed_calls[-1]
     assert kind == "remove" and fg.tolist() == [5, 3, 5] and bg.tolist() == [7, 7]
+    g.remove_seeds(fg=torch.tensor([9, 9]), bg=torch.zeros((6, 7, 8), dtype=torch.bool))
+    kind, fg, bg = made[0].seed_calls[-1]
+    assert kind == "remove" and fg.tolist() == [9, 9] and bg.tolist() == []
 
 
 def test_bad_arguments(made):

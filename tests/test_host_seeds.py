@@ -6,6 +6,7 @@ import sys
 
 import numpy
 import pytest
+import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fake_native  # noqa: E402
@@ -64,6 +65,9 @@ def test_fortran_mask_gives_c_order_ids(made):
     fg, bg = made[0].seed_calls[-1]
     assert fg.tolist() == [0 * 56 + 6 * 8 + 0, 1 * 56 + 2 * 8 + 3, 4 * 56 + 0 * 8 + 7]
     assert bg.tolist() == fg.tolist()
+    g.add_seeds(fg=torch.from_numpy(m), bg=torch.tensor([7, 5], dtype=torch.int32))
+    fg, bg = made[0].seed_calls[-1]
+    assert fg.tolist() == [0 * 56 + 6 * 8 + 0, 1 * 56 + 2 * 8 + 3, 4 * 56 + 0 * 8 + 7] and bg.tolist() == [7, 5]
 
 
 def test_ids_keep_order_and_duplicates(made):
@@ -88,6 +92,8 @@ def test_bad_arguments(made):
         g.add_seeds(fg=numpy.zeros((2, 2), numpy.int64))
     with pytest.raises(ValueError):
         g.add_seeds(fg=[1.5])
+    with pytest.raises(ValueError):
+        g.add_seeds(fg=5)                       # a single id is not an id array on the lattice
     assert made[0].seed_calls == []
     g.add_seeds()
     assert made[0].seed_calls[-1] == (None, None)
@@ -115,9 +121,11 @@ def test_unsolved_graph_stages_add_tweights(made):
     g, _ = _graph()
     ref, _ = _graph()
     g.add_seeds(fg=[3, 3], bg=[4])
+    g.add_seeds(bg=torch.tensor([6, 4]))
     for v in (3, 3):
         ref.add_tweights(v, 65535.0, 0.0)
-    ref.add_tweights(4, 0.0, 65535.0)
+    for v in (4, 6, 4):
+        ref.add_tweights(v, 0.0, 65535.0)
     assert made[0].seed_calls == [] and g.maxflow() == ref.maxflow()
     assert numpy.array_equal(g.get_mask(), ref.get_mask())
     assert numpy.array_equal(made[0].tr, made[1].tr)

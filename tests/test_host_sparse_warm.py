@@ -9,6 +9,7 @@ import sys
 
 import numpy
 import pytest
+import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
@@ -394,12 +395,18 @@ def test_warm_calls_route_to_the_sparse_backend(fake):
     g.add_tweights_warm(None, numpy.zeros(6), numpy.full(6, 0.5))
     g.add_tweights_warm([1, 1], 1.0, [0.0, 2.0])
     g.add_nweights_warm([0, 3], [5, 2], 1.0, [0.0, 4.0])
+    # CPU tensors, a single id, and one-element id arrays that broadcast to the other arguments' length
+    g.add_seeds(fg=torch.tensor([3]), bg=5)
+    g.add_tweights_warm(torch.tensor([2, 0], dtype=torch.int32), torch.tensor([1.5, -1.0]), torch.tensor(0.25))
+    g.add_nweights_warm([1], torch.tensor([4, 2]), 0.5, [1.0, 0.0])
     g.maxflow()
     nat = fake[0]
     tw_nodes = [None if t[0] is None else numpy.asarray(t[0]).tolist() for t in nat.tw[1:]]
-    assert tw_nodes == [[2], [4], [4], list(range(6)), [1, 1]]
+    assert tw_nodes == [[2], [4], [4], list(range(6)), [1, 1], [3], [5], [2, 0]]
     assert nat.tw[3][1].tolist() == [0.0] and nat.tw[3][2].tolist() == [-65535.0]
-    assert nat.e[0][-2:].tolist() == [0, 3] and nat.e[1][-2:].tolist() == [5, 2]
+    assert nat.tw[-1][1].tolist() == [1.5, -1.0] and nat.tw[-1][2].tolist() == [0.25, 0.25]
+    assert nat.e[0][-4:].tolist() == [0, 3, 1, 1] and nat.e[1][-4:].tolist() == [5, 2, 4, 2]
+    assert nat.e[2][-2:].tolist() == [0.5, 0.5] and nat.e[3][-2:].tolist() == [1.0, 0.0]
 
 
 def test_remove_flushes_staged_calls_first(fake):
@@ -425,6 +432,10 @@ def test_bad_arguments_are_refused(fake):
         g.add_seeds(fg=numpy.zeros(5, bool))
     with pytest.raises(ValueError):
         g.add_seeds(fg=[6])
+    with pytest.raises(ValueError):
+        g.add_seeds(fg=numpy.zeros((2, 3), bool))      # a sparse mask has shape (n,)
+    with pytest.raises(ValueError, match="differ in length"):
+        g.add_nweights_warm([], [1], 1.0, 0.0)
     with pytest.raises(ValueError):
         g.remove_nweights_warm([0], [1], -1.0, 0.0)
     with pytest.raises(ValueError):

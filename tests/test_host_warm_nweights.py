@@ -6,12 +6,14 @@ import sys
 
 import numpy
 import pytest
+import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fake_native  # noqa: E402
 from test_host_erase_seeds import _fresh, _lattice, _mask  # noqa: E402
 from test_host_seeds import _reference_bk  # noqa: E402
 from test_host_warm_eager import _lattice4  # noqa: E402
+from test_host_warm_tweights import _DeviceArray  # noqa: E402
 
 _SHAPE = (6, 7, 8)
 _N = 6 * 7 * 8
@@ -76,6 +78,12 @@ def test_list_form_keeps_order_broadcasts_and_widens(made):
     g.add_nweights_warm(7, [15, 6, 63], 2.0, [1.0, 0.0, 4.0])
     op = made[0].warm_calls[-1]
     assert op[1].tolist() == [7] * 3 and op[2].tolist() == [15, 6, 63] and op[3].tolist() == [2.0] * 3
+    g.add_nweights_warm(torch.tensor([5, 21], dtype=torch.int32), torch.tensor(13), torch.tensor([1.5, 2.0], dtype=torch.float32),
+                        torch.tensor(0.5))
+    op = made[0].warm_calls[-1]
+    assert op[1].tolist() == [5, 21] and op[2].tolist() == [13, 13] and op[3].tolist() == [1.5, 2.0] and op[4].tolist() == [0.5] * 2
+    g.add_nweights_warm([3], [4], numpy.nan, 0.0)   # folded calls leave the finite check to the native fold
+    assert numpy.isnan(made[0].warm_calls[-1][3]).all()
 
 
 def test_dense_form_takes_any_strides(made):
@@ -87,6 +95,9 @@ def test_dense_form_takes_any_strides(made):
     g.add_nweights_dense_warm(1, numpy.asfortranarray(a), b[::-1][::-1])
     op = made[0].warm_calls[-1]
     assert op[1] == 1 and numpy.array_equal(op[2], a) and numpy.array_equal(op[3], b.astype(numpy.float64))
+    g.add_nweights_dense_warm(0, torch.from_numpy(a), torch.from_numpy(b))
+    op = made[0].warm_calls[-1]
+    assert op[1] == 0 and numpy.array_equal(op[2], a) and numpy.array_equal(op[3], b.astype(numpy.float64))
 
 
 def test_bad_arguments(made):
@@ -98,6 +109,12 @@ def test_bad_arguments(made):
         g.add_nweights_warm([-1], [0], 1.0, 0.0)
     with pytest.raises(ValueError, match="differ in length"):
         g.add_nweights_warm([1, 2], [2, 3, 4], 1.0, 0.0)
+    with pytest.raises(ValueError, match="differ in length"):
+        g.add_nweights_warm([5], [6, 7], 1.0, 0.0)      # a one-element id array does not broadcast on the lattice
+    with pytest.raises(ValueError, match="must all be host or all be device arrays"):
+        g.add_nweights_warm([1], [2], _DeviceArray(), 0.0)
+    with pytest.raises(ValueError, match="must both be host or both be device arrays"):
+        g.add_nweights_dense_warm(0, numpy.zeros(_SHAPE), _DeviceArray())
     with pytest.raises(ValueError, match="integer"):
         g.add_nweights_warm([1.5], [2], 1.0, 0.0)
     with pytest.raises(ValueError, match="integer"):

@@ -8,10 +8,12 @@ import sys
 
 import numpy
 import pytest
+import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fake_native  # noqa: E402
 from test_host_seeds import _reference_bk  # noqa: E402
+from test_host_warm_tweights import _DeviceArray  # noqa: E402
 
 _SHAPE = (6, 7, 8)
 _N = 6 * 7 * 8
@@ -87,6 +89,9 @@ def test_list_form_broadcasts_and_widens(made):
     op = made[0].calls[-1]
     assert op[1].tolist() == [7] * 3 and op[2].tolist() == [15, 6, 63] and op[3].tolist() == [1.0] * 3
     assert op[4].tolist() == [1.0, 0.0, 2.0]
+    g.remove_nweights_warm(torch.tensor([5, 21]), torch.tensor(13, dtype=torch.int16), torch.tensor([0.5, 1.0]), torch.tensor(0))
+    op = made[0].calls[-1]
+    assert op[1].tolist() == [5, 21] and op[2].tolist() == [13, 13] and op[3].tolist() == [0.5, 1.0] and op[4].tolist() == [0.0] * 2
 
 
 def test_dense_form_takes_any_strides(made):
@@ -107,6 +112,8 @@ def test_bad_arguments_touch_nothing(made):
     n_calls = len(made[0].calls)
     for args, what in ((([0, _N - 1], [1, _N], 1.0, 0.0), "Invalid node id"), (([-1], [0], 1.0, 0.0), "Invalid node id"),
                        (([1, 2], [2, 3, 4], 1.0, 0.0), "differ in length"), (([1.5], [2], 1.0, 0.0), "integer"),
+                       (([5], [6, 7], 1.0, 0.0), "differ in length"),
+                       (([1], [2], _DeviceArray(), 0.0), "must all be host or all be device arrays"),
                        (([1, 2], [2, 3], [1.0, 2.0, 3.0], 0.0), "entries"), (([1], [2], numpy.array([True]), 0.0), "real"),
                        (([1], [2], -1.0, 0.0), "negative"), (([1], [2], 0.0, -1e-300), "negative"),
                        (([1], [2], numpy.nan, 0.0), "NaN"), (([1], [2], 0.0, numpy.inf), "NaN")):

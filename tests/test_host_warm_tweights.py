@@ -6,6 +6,7 @@ import sys
 
 import numpy
 import pytest
+import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fake_native  # noqa: E402
@@ -14,6 +15,11 @@ from test_host_seeds import _reference_bk  # noqa: E402
 
 _SHAPE = (6, 7, 8)
 _N = 6 * 7 * 8
+
+
+class _DeviceArray:
+    """Stands for an array in device memory: a lattice warm call refuses it next to a host array before reading it."""
+    __cuda_array_interface__ = {}
 
 
 class _WarmGraph(fake_native.FakeGraph):
@@ -70,6 +76,9 @@ def test_list_form_keeps_order_duplicates_and_widens(made):
     g.add_tweights_warm(numpy.array([5, 3, 5], numpy.int32), numpy.array([1.5, -2.0, 3.25], numpy.float32), [0.0, 4.0, -1.0])
     ids, src, snk = made[0].warm_calls[-1]
     assert ids.tolist() == [5, 3, 5] and src.tolist() == [1.5, -2.0, 3.25] and snk.tolist() == [0.0, 4.0, -1.0]
+    g.add_tweights_warm(torch.tensor([4, 2], dtype=torch.int32), torch.tensor([0.5, -1.0], dtype=torch.float32), torch.tensor(2))
+    ids, src, snk = made[0].warm_calls[-1]
+    assert ids.tolist() == [4, 2] and src.tolist() == [0.5, -1.0] and snk.tolist() == [2.0, 2.0]
 
 
 def test_scalars_broadcast_and_masks_give_c_order_ids(made):
@@ -96,6 +105,9 @@ def test_dense_form_reads_logical_c_order(made):
     g.add_tweights_warm(None, a.ravel(), 0.0)
     ids, src, snk = made[0].warm_calls[-1]
     assert ids is None and numpy.array_equal(src, a.ravel()) and not snk.any() and snk.size == _N
+    g.add_tweights_warm(None, torch.from_numpy(a), torch.from_numpy(b.ravel()))
+    ids, src, snk = made[0].warm_calls[-1]
+    assert ids is None and numpy.array_equal(src, a.ravel()) and numpy.array_equal(snk, b.astype(numpy.float64).ravel())
 
 
 def test_bad_arguments(made):
@@ -123,6 +135,12 @@ def test_bad_arguments(made):
         g.add_tweights_warm(None, numpy.full(_SHAPE, -numpy.inf), 0.0)
     with pytest.raises(ValueError, match="real"):
         g.add_tweights_warm([1], numpy.array([True]), 0.0)
+    with pytest.raises(ValueError):
+        g.add_tweights_warm(3, 1.0, 0.0)                # a single id is not an id array on the lattice
+    with pytest.raises(ValueError, match="must all be host or all be device arrays"):
+        g.add_tweights_warm([1, 2], _DeviceArray(), 0.0)
+    with pytest.raises(ValueError, match="a t-link weight is NaN"):
+        g.add_tweights_warm([1], numpy.nan, 0.0)        # folded calls are checked by the native fold, not twice
     assert made[0].warm_calls == []
 
 
