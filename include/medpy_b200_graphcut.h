@@ -230,6 +230,28 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* terms);
 /* 1 if mgc_build_voxel_graph would take the single-pass path on a fresh state of this handle. */
 int mgc_can_fuse(const mgc_graph* g);
 
+/* ---- batches of independent images ------------------------------------------------------------------- */
+
+/* A handle for `batch` independent images of shape image_shape[0..ndim) (1 <= ndim <= 3), cut in one build and one
+ * solve.  The images are stacked along axis 0 of one (batch * Z, Y, X) lattice (canonical image shape (Z, Y, X) with
+ * leading 1s) whose pairs across the seams between images do not exist, so each image is cut as if it were alone.
+ * MGC_E_ARG when batch * (voxels per image) would reach 2^31, checked before anything is allocated.
+ * On a batch handle the per-term calls, mgc_build_voxel_graph, every warm call (mgc_add_seeds ...
+ * mgc_remove_nweights_dense_warm), MGC_OPT_WARM and the z-slab calls return MGC_E_STATE with one message.
+ * Adding these three entry points left MGC_ABI_VERSION at 3 and mgc_stats unchanged. */
+int mgc_create_batch(int32_t ndim, const int64_t* image_shape, int64_t batch, int32_t device, mgc_graph** out);
+/* The terms of every image in one fused build.  The arrays of `terms` are over the logical (batch, ...image) shape
+ * (strided arrays are gathered); alpha, compute_dtype, the probability-map dtype and the spacing are shared by the batch.
+ * A boundary term is required (MGC_E_ARG), markers are uint8 arrays (no bit planes).  sigmas / norms: host arrays of
+ * `batch` entries, or NULL for terms->sigma / terms->norm on every image; a NaN norm of a linear term means the image's
+ * normaliser is reduced on the device over that image alone.  MGC_E_STATE on a handle that is not fresh (reset() it),
+ * or when the fused build is switched off (MEDPY_GC_FUSE=0).  mgc_maxflow then returns the energy of the whole lattice
+ * (the sum over the images) and mgc_get_mask the whole (batch, ...image) mask. */
+int mgc_build_voxel_batch(mgc_graph* g, const mgc_voxel_terms* terms, const double* sigmas, const double* norms);
+/* After mgc_maxflow: out[b] (batch host doubles) = the energy of image b, its add_tweights constant plus the flow its
+ * sink links absorbed -- what graph_from_voxels + maxflow return for that image alone, up to the order of the sums. */
+int mgc_get_batch_energies(mgc_graph* g, double* out);
+
 /* ---- solve / read-out ----------------------------------------------------------------------------- */
 
 /* Graph::maxflow() (maxflow.cpp:471-604; wrapper.cpp:68): runs the lattice push-relabel to a maximum

@@ -430,19 +430,33 @@ int boundary_launch(mgc_graph* g, const E* img, const BoundaryParams& P)
     return MGC_OK;
 }
 
+// out[0] = |max - min|, out[1] = max |x| over img[0..n), in the input dtype (device)
 template <typename E>
-int minmax_launch(mgc_graph* g, const E* img)
+int minmax_launch(mgc_graph* g, const E* img, unsigned n, double* out)
 {
     unsigned nb = g->n_partials < 1024u ? g->n_partials : 1024u;
+    if (nb > (n + 255u) / 256u) nb = (n + 255u) / 256u;
     E* pm = (E*)g->minmax_buf;
     E* px = pm + 1024;
     E* pa = px + 1024;
-    k_minmax_partial<E><<<nb, 256, 0, g->stream>>>(img, g->L.n, pm, px, pa);
-    k_minmax_final<E><<<1, 32, 0, g->stream>>>(pm, px, pa, nb, g->d_scalars + 2);
+    k_minmax_partial<E><<<nb, 256, 0, g->stream>>>(img, n, pm, px, pa);
+    k_minmax_final<E><<<1, 32, 0, g->stream>>>(pm, px, pa, nb, out);
     g->st.kernel_launches += 2;
     return MGC_OK;
 }
 }  // namespace
+
+int minmax_dtype(mgc_graph* g, int dtype, const void* img, unsigned n, double* out)
+{
+    switch (dtype) {
+        case MGC_F32: return minmax_launch<float>(g, (const float*)img, n, out);
+        case MGC_F64: return minmax_launch<double>(g, (const double*)img, n, out);
+        case MGC_U8: return minmax_launch<uint8_t>(g, (const uint8_t*)img, n, out);
+        case MGC_I16: return minmax_launch<int16_t>(g, (const int16_t*)img, n, out);
+        case MGC_I32: return minmax_launch<int32_t>(g, (const int32_t*)img, n, out);
+    }
+    return MGC_OK;
+}
 
 // parameters of one of the eight boundary terms; the linear normaliser is computed on the device (K0) when `norm` is NaN
 int boundary_params(mgc_graph* g, int kind, int dtype, const void* img, double sigma, const double* spacing, double norm, BoundaryParams* out)
@@ -459,14 +473,7 @@ int boundary_params(mgc_graph* g, int kind, int dtype, const void* img, double s
     P.norm = norm;
     if (P.fn == 0 && std::isnan(norm)) {
         if (g->slab) FAIL(MGC_E_ARG, "z-slab handles need the global normaliser of the linear terms");
-        int rc = MGC_OK;
-        switch (dtype) {
-            case MGC_F32: rc = minmax_launch<float>(g, (const float*)img); break;
-            case MGC_F64: rc = minmax_launch<double>(g, (const double*)img); break;
-            case MGC_U8: rc = minmax_launch<uint8_t>(g, (const uint8_t*)img); break;
-            case MGC_I16: rc = minmax_launch<int16_t>(g, (const int16_t*)img); break;
-            case MGC_I32: rc = minmax_launch<int32_t>(g, (const int32_t*)img); break;
-        }
+        int rc = minmax_dtype(g, dtype, img, g->L.n, g->d_scalars + 2);
         if (rc) return rc;
         double mm[2];
         CK(cudaMemcpyAsync(mm, g->d_scalars + 2, sizeof(mm), cudaMemcpyDeviceToHost, g->stream));
@@ -561,6 +568,7 @@ int mgc_reset(mgc_graph* g)
     invalidate(g);
     g->flow_started = false;
     g->has_nlinks = false;
+    g->batch_built = false;
     g->energy = 0.0;
     int64_t n = g->st.n_voxels;
     g->st = mgc_stats{};
@@ -673,6 +681,7 @@ int mgc_set_option(mgc_graph* g, int32_t option, int64_t value)
     if (option == MGC_OPT_DEFER_WEIGHT_CHECK) { g->defer_check = value != 0; return MGC_OK; }
     if (option == MGC_OPT_KEEP_DEVICE_INPUTS) { g->keep_device_inputs = value != 0; return MGC_OK; }
     if (option == MGC_OPT_WARM) {
+        if (batch_refused(g)) return MGC_E_STATE;
         // the record is taken before the first push; a lazily built handle folds without it, so there it changes nothing now
         const bool on = value != 0;
         if (on != g->warm_opt && g->flow_started && !g->lazy_built)
@@ -709,6 +718,7 @@ int mgc_synchronize(mgc_graph* g)
 int mgc_add_regional_probability(mgc_graph* g, const mgc_array* prob, double alpha, int32_t compute_dtype)
 {
     if (!g || !prob) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     if (prob->dtype != MGC_F32 && prob->dtype != MGC_F64) FAIL(MGC_E_ARG, "probability map must be float32 or float64");
     if (compute_dtype != MGC_F32 && compute_dtype != MGC_F64) FAIL(MGC_E_ARG, "compute dtype must be float32 or float64");
@@ -739,6 +749,7 @@ int mgc_add_regional_probability(mgc_graph* g, const mgc_array* prob, double alp
 int mgc_add_tweights_dense(mgc_graph* g, const mgc_array* src, const mgc_array* snk)
 {
     if (!g || !src || !snk) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     if (src->dtype != MGC_F64 || snk->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense t-weights must be float64");
     CK(cudaSetDevice(g->device));
@@ -765,6 +776,7 @@ int mgc_add_tweights_dense(mgc_graph* g, const mgc_array* src, const mgc_array* 
 int mgc_add_markers(mgc_graph* g, const mgc_array* fg, const mgc_array* bg)
 {
     if (!g) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (!fg && !bg) return MGC_OK;
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     if ((fg && fg->dtype != MGC_U8) || (bg && bg->dtype != MGC_U8)) FAIL(MGC_E_ARG, "markers must be uint8 / bool");
@@ -795,6 +807,7 @@ int mgc_add_markers(mgc_graph* g, const mgc_array* fg, const mgc_array* bg)
 int mgc_add_boundary(mgc_graph* g, int32_t kind, const mgc_array* image, double sigma, const double* spacing, double norm)
 {
     if (!g || !image) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (kind < 0 || kind > 7) FAIL(MGC_E_ARG, "unknown boundary term");
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     CK(cudaSetDevice(g->device));
@@ -840,6 +853,7 @@ int mgc_add_boundary(mgc_graph* g, int32_t kind, const mgc_array* image, double 
 int mgc_add_nweights_dense(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
 {
     if (!g || !fwd || !bwd) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     if (axis < 0 || axis >= g->user_ndim) FAIL(MGC_E_ARG, "bad axis");
     if (fwd->dtype != MGC_F64 || bwd->dtype != MGC_F64) FAIL(MGC_E_ARG, "dense n-weights must be float64");

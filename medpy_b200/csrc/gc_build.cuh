@@ -336,7 +336,8 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
             block_range_add<E>(lo, hi, nan, s_rng[8 + w]);
             nan = nan || s_rnan[w] != 0;
         }
-        blk_ordinary = block_exp_ordinary(Elem<E>::val(lo), Elem<E>::val(hi), nan, use_max, P.inv_sigma2);
+        blk_ordinary = block_exp_ordinary(Elem<E>::val(lo), Elem<E>::val(hi), nan, use_max,
+                                          range_inv_sigma2(P, L, z0 - 1, z0 + BUILD_TZ));
     }
 
     const bool has_py = gy + 1 < L.dim[1], has_px = gx + 1 < L.dim[2];
@@ -351,9 +352,9 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
     int isbad = 0;
     unsigned needs_any = 0, exc_any = 0;
     double msum = 0.0;
-    // one pair weight: value of the neighbour cell, validity, axis spacing
-    auto pair_w = [&](double a, E iq, bool valid, double sp) -> double {
-        const double w = build_weight<FN, E>(P, a, iq, use_max, spacing, sp);
+    // one pair weight: the term's constants of the pair's plane, value of the neighbour cell, validity, axis spacing
+    auto pair_w = [&](const BoundaryParams& Q, double a, E iq, bool valid, double sp) -> double {
+        const double w = build_weight<FN, E>(Q, a, iq, use_max, spacing, sp);
         // the exponential term without spacing is clamped to DBL_MIN and can never be <= 0 (NaN compares false)
         if (!(FN == 1 && SPACING == 0)) { if (valid && w <= 0.0) isbad = 1; }
         return valid ? w : 0.0;
@@ -364,22 +365,21 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
     double* s_wxh = s_wyh + 8 * 32;             // [8 z][8 y]:  pair (x0 - 1, x0)
     double wz_back = 0.0;
     if (!LAZY_EXP) {
-        const bool vz = col_in && z0 > 0;
-        wz_back = pair_w(build_val<E>(at(0, ly + 1, lx + 1), use_max), at(1, ly + 1, lx + 1), vz, sp_z);
+        const bool vz = col_in && (z_pairs(L, z0) & 1u);
+        wz_back = pair_w(params_at(P, L, z0), build_val<E>(at(0, ly + 1, lx + 1), use_max), at(1, ly + 1, lx + 1), vz, sp_z);
         // thread (ly, lx) -> y-face weight of plane z0 + ly at column x0 + lx
         const bool vy = y0 > 0 && gx < L.dim[2] && z0 + ly < L.dim[0];
-        s_wyh[ly * 32 + lx] = pair_w(build_val<E>(at(ly + 1, 0, lx + 1), use_max), at(ly + 1, 1, lx + 1), vy, sp_y);
+        s_wyh[ly * 32 + lx] = pair_w(params_at(P, L, z0 + ly), build_val<E>(at(ly + 1, 0, lx + 1), use_max), at(ly + 1, 1, lx + 1), vy, sp_y);
         if (tid < 64) {
             const int fz = tid >> 3, fy = tid & 7;
             const bool vx = x0 > 0 && y0 + fy < L.dim[1] && z0 + fz < L.dim[0];
-            s_wxh[fz * 8 + fy] = pair_w(build_val<E>(at(fz + 1, fy + 1, 0), use_max), at(fz + 1, fy + 1, 1), vx, sp_x);
+            s_wxh[fz * 8 + fy] = pair_w(params_at(P, L, z0 + fz), build_val<E>(at(fz + 1, fy + 1, 0), use_max), at(fz + 1, fy + 1, 1), vx, sp_x);
         }
     }
 
     // the in-lattice pairs of this thread's voxel in plane gz (bit k: the pair across face k exists)
     auto pairs_at = [&](int gz) -> unsigned {
-        return (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) | (has_py ? 8u : 0u) |
-               (gx > 0 ? 16u : 0u) | (has_px ? 32u : 0u);
+        return z_pairs(L, gz) | (gy > 0 ? 4u : 0u) | (has_py ? 8u : 0u) | (gx > 0 ? 16u : 0u) | (has_px ? 32u : 0u);
     };
     const bool copies = A.img_copy != nullptr || A.prob_copy != nullptr;
     for (int lz = 0; lz < BUILD_TZ; ++lz) {
@@ -388,6 +388,7 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
         double* wyb = s_wy + (lz & 1) * 9 * 32;
         double* wxb = s_wx + (lz & 1) * 8 * 33;
         const int hz = lz + 1;
+        const BoundaryParams Pz = params_at(P, L, gz);       // this plane's term constants (a batch: its image's)
         TIn nxt{0.0, 0u};
         if (lz + 1 < BUILD_TZ) nxt = fetch(lz + 1);
         // (the voxel's own value: read where a weight or an argument needs it)
@@ -412,7 +413,7 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
                 const double a = own_val();
                 auto arg = [&](E iq) -> double {
                     const double b = build_val<E>(iq, use_max);
-                    return exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
+                    return exp_term_arg(Pz, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
                 };
                 const double t[6] = {arg(at(hz - 1, ly + 1, lx + 1)), arg(at(hz + 1, ly + 1, lx + 1)), arg(at(hz, ly, lx + 1)),
                                      arg(at(hz, ly + 2, lx + 1)), arg(at(hz, ly + 1, lx)), arg(at(hz, ly + 1, lx + 2))};
@@ -433,7 +434,7 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
                 // disagrees takes the general path.  Both paths give bit-identical weights for ordinary arguments.
                 auto arg = [&](E iq) -> double {
                     const double b = build_val<E>(iq, use_max);
-                    return exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
+                    return exp_term_arg(Pz, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
                 };
                 const double tz = arg(at(hz + 1, ly + 1, lx + 1)), ty = arg(at(hz, ly + 2, lx + 1)), tx = arg(at(hz, ly + 1, lx + 2));
                 if (__all_sync(0xffffffffu, tz <= 700.0 && ty <= 700.0 && tx <= 700.0)) {
@@ -444,13 +445,13 @@ build_block(int bx, int by, int bz, int nbx, int nby, bool first, unsigned parit
                     if (wy <= 0.0) wy = DBL_MIN;
                     if (wx <= 0.0) wx = DBL_MIN;
                 }
-                if (!(pin && gz + 1 < L.dim[0])) wz = 0.0;
+                if (!(pin && (z_pairs(L, gz) & 2u))) wz = 0.0;
                 if (!(pin && has_py)) wy = 0.0;
                 if (!(pin && has_px)) wx = 0.0;
             } else {
-                wz = pair_w(a, at(hz + 1, ly + 1, lx + 1), pin && gz + 1 < L.dim[0], sp_z);
-                wy = pair_w(a, at(hz, ly + 2, lx + 1), pin && has_py, sp_y);
-                wx = pair_w(a, at(hz, ly + 1, lx + 2), pin && has_px, sp_x);
+                wz = pair_w(Pz, a, at(hz + 1, ly + 1, lx + 1), pin && (z_pairs(L, gz) & 2u), sp_z);
+                wy = pair_w(Pz, a, at(hz, ly + 2, lx + 1), pin && has_py, sp_y);
+                wx = pair_w(Pz, a, at(hz, ly + 1, lx + 2), pin && has_px, sp_x);
             }
             wyb[(ly + 1) * 32 + lx] = wy;
             wxb[ly * 33 + lx + 1] = wx;
@@ -695,6 +696,7 @@ k_build_lean(Lattice L, Tiles TL, State<double> S, const __grid_constant__ Build
     unsigned char* s_bg = smem_raw + LS::BG_OFF;
     unsigned long long* bar = reinterpret_cast<unsigned long long*>(smem_raw + LS::MISC_OFF);
     int* s_flags = reinterpret_cast<int*>(smem_raw + LS::MISC_OFF + 8);          // [4] needs, [4] has excess
+    unsigned char* s_zp = smem_raw + LS::MISC_OFF + 40;                           // [8] z_pairs of the block's planes
     unsigned char* s_scr = smem_raw + LS::MISC_OFF + 64;                          // range test, then block reduction
     double* s_mm = reinterpret_cast<double*>(smem_raw);                           // [8 z][8 y][32 x], x ^ y swizzled
 
@@ -703,6 +705,9 @@ k_build_lean(Lattice L, Tiles TL, State<double> S, const __grid_constant__ Build
     const int cx = x0 == 0 ? -1 : PAD - 1, cy = y0 == 0 ? -1 : 0, cz = z0 == 0 ? -1 : 0;
     const bool has_prob = TIN == 1 || A.prob != nullptr;
     if (tid < 8) s_flags[tid] = 0;
+    // the axis-0 pair bits of the block's planes, formed once per plane here rather than per thread in the register-bound
+    // state section below
+    if (tid < BUILD_TZ) s_zp[tid] = (unsigned char)z_pairs(L, z0 + tid);
     if (tid == 0) {
         mbar_init(bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -717,7 +722,7 @@ k_build_lean(Lattice L, Tiles TL, State<double> S, const __grid_constant__ Build
     __syncthreads();
     mbar_wait(bar, 0u);
 
-    if (!lean_range_test<E>(s_img, s_scr, P.use_max != 0, P.inv_sigma2) || refuse_all) {
+    if (!lean_range_test<E>(s_img, s_scr, P.use_max != 0, range_inv_sigma2(P, L, z0 - 1, z0 + BUILD_TZ)) || refuse_all) {
         if (tid == 0) refused[atomicAdd(n_refused, 1)] = ((int)blockIdx.z * (int)gridDim.y + (int)blockIdx.y) * (int)gridDim.x + (int)blockIdx.x;
         return;          // uniform over the CTA
     }
@@ -794,7 +799,7 @@ k_build_lean(Lattice L, Tiles TL, State<double> S, const __grid_constant__ Build
 
     // ---- t-links and solver state ----
     const bool own = gz >= L.own0 && gz < L.own1;
-    const unsigned zy = (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) | (gy + 1 < L.dim[1] ? 8u : 0u);
+    const unsigned zy = s_zp[tz] | (gy > 0 ? 4u : 0u) | (gy + 1 < L.dim[1] ? 8u : 0u);
     const bool f32 = TIN == 1 || A.compute_f32 != 0;
     unsigned rm_lo = 0u, rm_hi = 0u, sinkm = 0u;
     bool needs = false, exc = false;
@@ -898,8 +903,8 @@ k_build_lean(Lattice L, Tiles TL, State<double> S, const __grid_constant__ Build
 __device__ __forceinline__ unsigned tile_pairs(const Lattice& L, const TileCtx& c)
 {
     const int gz = c.tz * TILE + c.lz, gy = c.ty * TILE + c.ly, gx = c.tx * TILE + c.lx;
-    return (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u) | (gy > 0 ? 4u : 0u) | (gy + 1 < L.dim[1] ? 8u : 0u) |
-           (gx > 0 ? 16u : 0u) | (gx + 1 < L.dim[2] ? 32u : 0u);
+    return z_pairs(L, gz) | (gy > 0 ? 4u : 0u) | (gy + 1 < L.dim[1] ? 8u : 0u) | (gx > 0 ? 16u : 0u) |
+           (gx + 1 < L.dim[2] ? 32u : 0u);
 }
 
 // the t-link inputs of an in-lattice voxel: its probability (0 without a map) and marker bits (bit 0 fg, bit 1 bg)

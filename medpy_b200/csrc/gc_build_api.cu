@@ -146,9 +146,19 @@ int build_launch_dtype(mgc_graph* g, int dtype, const BuildMaps& imap, const Bui
     }
 }
 
+// gridDim.z is at most 65535 layers of 8 planes: a longer lattice (a batch of many 2-D images) takes several launches,
+// each starting at its own z_tile0 (the kernels index partials, flags and marker planes by the global layer)
 int build_launch_any(mgc_graph* g, bool lazy, int dtype, const BuildMaps& imap, const BuildArgs& A, const BoundaryParams& P, int nz_layers)
 {
-    return lazy ? build_launch_dtype<1>(g, dtype, imap, A, P, nz_layers) : build_launch_dtype<0>(g, dtype, imap, A, P, nz_layers);
+    constexpr int MAX_LAYERS = 65535;
+    BuildArgs Al = A;
+    for (int l = 0; l < nz_layers; l += MAX_LAYERS) {
+        Al.z_tile0 = A.z_tile0 + l;
+        const int nl = nz_layers - l < MAX_LAYERS ? nz_layers - l : MAX_LAYERS;
+        const int rc = lazy ? build_launch_dtype<1>(g, dtype, imap, Al, P, nl) : build_launch_dtype<0>(g, dtype, imap, Al, P, nl);
+        if (rc) return rc;
+    }
+    return MGC_OK;
 }
 
 // C-contiguous over the local lattice?
@@ -170,16 +180,10 @@ bool can_fuse(const mgc_graph* g) { return g->nd == 3 && g->fuse_build; }
 bool can_lazy(const mgc_graph* g) { return can_fuse(g) && !g->slab && g->lazy_caps && g->cmat; }
 }  // namespace
 
-// =====================================================================================================
-// C ABI
-// =====================================================================================================
-extern "C" {
-
-int mgc_can_fuse(const mgc_graph* g) { return g && can_fuse(g) ? 1 : 0; }
-
-int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
+// mgc_build_voxel_graph, and mgc_build_voxel_batch with its arrays over the batch lattice (a batch handle reads its term
+// constants from the table batch_constants fills, and its per-image add_tweights constants are summed after the build)
+int voxel_build(mgc_graph* g, const mgc_voxel_terms* t)
 {
-    if (!g || !t) return MGC_E_ARG;
     if (g->flow_started) FAIL(MGC_E_STATE, "the graph has been solved (its capacities hold residuals): reset() it before adding terms");
     const bool has_bits = t->fg_bits || t->bg_bits;
     if (has_bits && (t->fg || t->bg)) FAIL(MGC_E_ARG, "pass the markers either as byte arrays or bit-packed, not both");
@@ -256,8 +260,9 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     }
 
     BoundaryParams P{};
-    rc = boundary_params(g, t->boundary_kind, t->image->dtype, d_img, t->sigma, t->spacing, t->norm, &P);
+    rc = boundary_params(g, t->boundary_kind, t->image->dtype, d_img, t->sigma, t->spacing, g->batch ? 0.0 : t->norm, &P);
     if (rc) return rc;
+    if (g->batch) { rc = batch_constants(g, t->image->dtype, d_img, &P); if (rc) return rc; }
 
     BuildArgs A{};
     A.img = d_img;
@@ -364,6 +369,7 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
         g->st.kernel_launches++;
         CK(cudaGetLastError());
     }
+    if (g->batch) { rc = batch_tconst(g, A); if (rc) return rc; }
     g->caps_fresh = false;
     g->tr_fresh = false;
     g->caps_lazy = lazy;
@@ -402,6 +408,20 @@ int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
     CK(cudaStreamSynchronize(g->stream));
     if (bad) FAIL(MGC_E_WEIGHT, "Negative or zero weights are not allowed.");
     return MGC_OK;
+}
+
+// =====================================================================================================
+// C ABI
+// =====================================================================================================
+extern "C" {
+
+int mgc_can_fuse(const mgc_graph* g) { return g && can_fuse(g) ? 1 : 0; }
+
+int mgc_build_voxel_graph(mgc_graph* g, const mgc_voxel_terms* t)
+{
+    if (!g || !t) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
+    return voxel_build(g, t);
 }
 
 }  // extern "C"

@@ -29,6 +29,8 @@ struct Lattice {
     unsigned n;             // voxels in the local lattice (< 2^31)
     unsigned plane;         // voxels per axis-0 plane
     int own0, own1;         // owned axis-0 planes [own0, own1): all of them unless this is a z-slab
+    int zper;               // batch of images stacked along axis 0: planes per image (0: one image, DESIGN.md §3.1)
+    unsigned long long zmagic;    // ceil(2^64 / zper) (0 when zper <= 1), as magic[]
 };
 
 template <typename T>
@@ -66,6 +68,27 @@ __device__ __forceinline__ int dir_offset(const Lattice& L, int k)
 {
     int s = (int)L.stride[k >> 1];
     return (k & 1) ? s : -s;
+}
+
+// the image of plane gz >= 0 of a batch lattice (0 on a lattice of one image)
+__device__ __forceinline__ int image_of(const Lattice& L, int gz)
+{
+    if (!L.zper) return 0;
+    return L.zmagic ? (int)__umul64hi((unsigned long long)(unsigned)gz, L.zmagic) : gz;
+}
+
+// The axis-0 pairs of a voxel in plane gz >= 0 (bit 0: the pair with plane gz - 1, bit 1: with plane gz + 1): inside the
+// lattice and, in a batch, not across the seam between two images.  Every place that forms axis-0 validity calls this;
+// on a lattice of one image it is the extent test alone.
+__device__ __forceinline__ unsigned z_pairs(const Lattice& L, int gz)
+{
+    unsigned b = (gz > 0 ? 1u : 0u) | (gz + 1 < L.dim[0] ? 2u : 0u);
+    if (L.zper) {
+        const int r = gz - image_of(L, gz) * L.zper;
+        if (r == 0) b &= ~1u;
+        if (r == L.zper - 1) b &= ~2u;
+    }
+    return b;
 }
 
 __device__ __forceinline__ bool owned(const Lattice& L, unsigned v)

@@ -89,6 +89,22 @@ ER_HD bool block_exp_ordinary(double lo, double hi, bool nan, bool use_max, doub
     return exp_arg_ordinary(er_mul(er_mul(x, x), inv_sigma2));
 }
 
+// The constant of the range test of a block whose staged box touches the images b0 .. b1 of a batch, whose exponential
+// terms use sigma2[b] = pow(sigma_b, 2): the largest of their reciprocals 1 / sigma2[b] (formed as the host forms
+// inv_sigma2), or 0 -- no block passes -- when one of them does not take the product form.  block_exp_ordinary is
+// monotone in that constant (x -> RN(RN(x * x) * c) is monotone in c >= 0), so a block that passes under the largest
+// constant passes under each image's own, and every pair lies inside one image: no pair of the block fails.
+ER_HD double exp_table_inv_max(const double* sigma2, int b0, int b1)
+{
+    double m = 0.0;
+    for (int b = b0; b <= b1; ++b) {
+        const double inv = sigma2[b] != 0.0 ? er_div(1.0, sigma2[b]) : 0.0;
+        if (!(inv > 0.0 && inv < 1e300)) return 0.0;
+        m = inv > m ? inv : m;
+    }
+    return m;
+}
+
 // Order-preserving integer key of a float32's bits: key(a) < key(b) as signed ints whenever a < b, -0 just below +0, a
 // positive NaN above +inf and a negative NaN below -inf.  The map is its own inverse.  The float32 block range of the lazy
 // build reduces these keys with integer min / max (one instruction each, and __reduce_min_sync / __reduce_max_sync across

@@ -156,6 +156,7 @@ static cudaError_t tails_sort(void* tmp, size_t* bytes, const unsigned* tails, u
 static int warm_check(mgc_graph* g, bool* eager)
 {
     *eager = false;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (!g->slab && g->lazy_built && g->state_init && g->nd == 3) return MGC_OK;
     if (warm_wanted(g)) { *eager = true; return MGC_OK; }
     FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "

@@ -6,6 +6,7 @@
 //   gc_solve.cu      the lazy push state, the tile-solver driver, mgc_maxflow
 //   gc_fold.cu       the folds into the residual state (seeds, t-links, n-links)
 //   gc_slab.cu       z-slab stepping and the NCCL slab solve
+//   gc_batch.cu      batches of independent images: create, build, per-image constants and energies
 // Each kernel is compiled into exactly one of them: a unit includes the kernel-only header of the kernels it launches
 // (gc_<unit>_kernels.cuh, gc_persist.cuh, gc_sweep.cuh, ...), and k_sum_partials, which several launch, is behind
 // sum_partials().  Process-wide state (pools, the cub launch counts, the NCCL binding) is defined in one unit each.
@@ -192,6 +193,15 @@ struct mgc_graph {
     size_t ph_used = 0;
     double slab_phase_ms[6] = {0, 0, 0, 0, 0, 0};
 
+    // batch of independent images stacked along axis 0 (mgc_create_batch, DESIGN.md §3.1; L.zper planes per image)
+    int64_t batch = 0;                 // images (0: not a batch handle)
+    int batch_ndim = 0;                // dimensions of one image (1..3)
+    int batch_chunks = 1;              // blocks per image of the per-image reductions
+    bool batch_built = false;          // the state comes from mgc_build_voxel_batch (cleared by mgc_reset)
+    double* batch_buf = nullptr;       // [B] term constants (BoundaryParams::ktab) | [B] add_tweights constants |
+                                       // [B] energies | [2B] min / max read-outs | [B * batch_chunks] partials
+    std::vector<double> batch_k_host;  // the term constants of the next build (NaN: M computed on the device)
+
     mgc_stats st{};
     std::string err;
 };
@@ -208,6 +218,7 @@ void sum_partials(mgc_graph* g, const double* partials, unsigned n, double* out)
 void resolve_term_span(mgc_graph* g);
 int check_pending(mgc_graph* g);
 int boundary_params(mgc_graph* g, int kind, int dtype, const void* img, double sigma, const double* spacing, double norm, BoundaryParams* out);
+int minmax_dtype(mgc_graph* g, int dtype, const void* img, unsigned n, double* out);
 
 // ---- gc_solve.cu ----------------------------------------------------------------------------------------
 typedef CUresult (*tmap_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -229,6 +240,13 @@ int count_active_tiles_enqueue(mgc_graph* g, unsigned long long* dst);
 int count_active_tiles(mgc_graph* g, int64_t* out);
 int readout(mgc_graph* g, double* energy_part);
 
+// ---- gc_build_api.cu ------------------------------------------------------------------------------------
+int voxel_build(mgc_graph* g, const mgc_voxel_terms* t);
+
+// ---- gc_batch.cu ----------------------------------------------------------------------------------------
+int batch_constants(mgc_graph* g, int dtype, const void* d_img, BoundaryParams* P);
+int batch_tconst(mgc_graph* g, const BuildArgs& A);
+
 // ---- gc_fold.cu -----------------------------------------------------------------------------------------
 int warm_prepare(mgc_graph* g);
 
@@ -236,6 +254,15 @@ int warm_prepare(mgc_graph* g);
 void slab_comm_release(mgc_graph* g);
 
 // ---- inline helpers ---------------------------------------------------------------------------------------
+// The one refusal of every call a batch handle does not take: MGC_E_STATE with this message (else MGC_OK)
+inline int batch_refused(const mgc_graph* g)
+{
+    if (!g->batch) return MGC_OK;
+    const_cast<mgc_graph*>(g)->err = "batch handles take their terms from mgc_build_voxel_batch only: the per-term calls, "
+                                     "warm edits, MGC_OPT_WARM and the z-slab calls are not available on them";
+    return MGC_E_STATE;
+}
+
 // NVTX range per phase (build / relabel / push / readout / exchange): visible in nsys / ncu timelines, a no-op without a
 // profiler attached (SURVEY.md §5.1)
 struct Nvtx {

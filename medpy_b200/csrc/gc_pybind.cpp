@@ -110,6 +110,18 @@ public:
         shape_[0] = (z1 - z0) + (z0 > 0 ? 1 : 0) + (z1 < shape[0] ? 1 : 0);  // local extent incl. ghost planes
         owned_planes_ = z1 - z0;
     }
+    // a batch of `batch` images of shape image_shape (mgc_create_batch): the graph's arrays are (batch, ...image)
+    struct BatchTag {};
+    PyGraph(BatchTag, const std::vector<int64_t>& image_shape, int64_t batch, int device) : shape_(image_shape)
+    {
+        int rc = mgc_create_batch((int32_t)image_shape.size(), image_shape.data(), batch, device, &g_);
+        if (rc != MGC_OK) { std::string m = mgc_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
+        shape_.insert(shape_.begin(), batch);
+    }
+    static std::unique_ptr<PyGraph> batch(const std::vector<int64_t>& image_shape, int64_t batch, int device)
+    {
+        return std::unique_ptr<PyGraph>(new PyGraph(BatchTag{}, image_shape, batch, device));
+    }
     ~PyGraph() { if (g_) mgc_destroy(g_); }
     PyGraph(const PyGraph&) = delete;
     PyGraph& operator=(const PyGraph&) = delete;
@@ -228,6 +240,40 @@ public:
         }
         hold_inputs(std::move(hold));
         held_live_ = !held_.empty() && kind >= 0 && mgc_can_fuse(g_);
+    }
+    // mgc_build_voxel_batch: arrays over (batch, ...image); sigmas / norms one per image (norm NaN: reduced on the device)
+    void build_voxel_batch(const py::object& prob, double alpha, bool compute_f32, int kind, const py::object& image,
+                           const std::vector<double>& sigmas, const py::object& spacing, const std::vector<double>& norms,
+                           const py::object& fg, const py::object& bg)
+    {
+        if ((int64_t)sigmas.size() != shape_[0] || (int64_t)norms.size() != shape_[0])
+            throw py::value_error("sigmas and norms need one entry per image");
+        ArrayRef rp, ri, rf, rb;
+        mgc_voxel_terms t{};
+        t.alpha = alpha;
+        t.compute_dtype = compute_f32 ? MGC_F32 : MGC_F64;
+        t.boundary_kind = kind;
+        ri = make_ref(image, -1, "image"); check_shape(ri, "image"); t.image = &ri.a;
+        if (!prob.is_none()) { rp = make_ref(prob, -1, "probability_map"); check_shape(rp, "probability_map"); t.prob = &rp.a; }
+        if (!fg.is_none()) { rf = make_ref(fg, MGC_U8, "fg_markers"); check_shape(rf, "fg_markers"); t.fg = &rf.a; }
+        if (!bg.is_none()) { rb = make_ref(bg, MGC_U8, "bg_markers"); check_shape(rb, "bg_markers"); t.bg = &rb.a; }
+        std::vector<double> sp;
+        if (!spacing.is_none()) {
+            sp = spacing.cast<std::vector<double>>();
+            if (sp.size() + 1 < shape_.size()) throw py::value_error("spacing has fewer entries than the images have dimensions");
+            t.spacing = sp.data();
+        }
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_build_voxel_batch(g_, &t, sigmas.data(), norms.data()); }
+        check(rc, g_);
+    }
+    py::array_t<double> get_batch_energies()
+    {
+        py::array_t<double> out((py::ssize_t)shape_[0]);
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_get_batch_energies(g_, out.mutable_data()); }
+        check(rc, g_);
+        return out;
     }
     void set_pack_markers(bool on) { pack_markers_ = on; }
     // off: device inputs are borrowed for the build call only and the build keeps its own copies (the C default)
@@ -796,6 +842,9 @@ PYBIND11_MODULE(_mgc, m)
         .def("remove_nweights_warm", &PyGraph::remove_nweights_warm, py::arg("i"), py::arg("j"), py::arg("cap"), py::arg("rev_cap"))
         .def("remove_nweights_dense_warm", &PyGraph::remove_nweights_dense_warm, py::arg("axis"), py::arg("fwd"), py::arg("bwd"))
         .def("build_voxel_graph", &PyGraph::build_voxel_graph)
+        .def_static("batch", &PyGraph::batch, py::arg("image_shape"), py::arg("batch"), py::arg("device") = -1)
+        .def("build_voxel_batch", &PyGraph::build_voxel_batch)
+        .def("get_batch_energies", &PyGraph::get_batch_energies)
         .def_static("slab_comm_unique_id", &PyGraph::slab_comm_unique_id)
         .def("slab_comm_init", &PyGraph::slab_comm_init)
         .def("slab_solve", &PyGraph::slab_solve)

@@ -134,8 +134,8 @@ __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<
     int c[3];
     decode<3>(L, v, c);
     // capacities before any flow: the doubles k_caps_tiles computed from the same image copy
-    const unsigned valid = (c[0] > 0 ? 1u : 0u) | (c[0] + 1 < L.dim[0] ? 2u : 0u) | (c[1] > 0 ? 4u : 0u) |
-                           (c[1] + 1 < L.dim[1] ? 8u : 0u) | (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
+    const unsigned valid = z_pairs(L, c[0]) | (c[1] > 0 ? 4u : 0u) | (c[1] + 1 < L.dim[1] ? 8u : 0u) |
+                           (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
     const double a = build_val<E>(__ldg(img + v), use_max);
     if (FN == 1 && SPACING == 0) {
         double t6[6];

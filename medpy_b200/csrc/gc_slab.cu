@@ -154,6 +154,7 @@ extern "C" {
 int mgc_slab_plane_elems(const mgc_graph* g, int64_t* n)
 {
     if (!g || !n) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     *n = (int64_t)g->L.plane;
     return MGC_OK;
 }
@@ -161,6 +162,7 @@ int mgc_slab_plane_elems(const mgc_graph* g, int64_t* n)
 int mgc_slab_begin(mgc_graph* g)
 {
     if (!g) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
     resolve_term_span(g);
@@ -172,6 +174,7 @@ int mgc_slab_begin(mgc_graph* g)
 int mgc_slab_push(mgc_graph* g, int32_t n)
 {
     if (!g || n < 0) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (!g->state_init) FAIL(MGC_E_STATE, "call mgc_slab_begin first");
     CK(cudaSetDevice(g->device));
     g->iters_now = g->tile_iters;
@@ -181,6 +184,7 @@ int mgc_slab_push(mgc_graph* g, int32_t n)
 int mgc_slab_pack(mgc_graph* g, int32_t* h_lo, double* f_lo, int32_t* h_hi, double* f_hi)
 {
     if (!g) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     const unsigned P = g->L.plane;
     const unsigned nb = (P + 255u) / 256u;
@@ -202,6 +206,7 @@ int mgc_slab_unpack(mgc_graph* g, const int32_t* h_lo, const double* f_lo, const
                     int32_t* changed_dev)
 {
     if (!g) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     const unsigned P = g->L.plane;
     const unsigned nb = (P + 255u) / 256u;
@@ -230,6 +235,7 @@ int mgc_slab_unpack(mgc_graph* g, const int32_t* h_lo, const double* f_lo, const
 int mgc_slab_relabel_begin(mgc_graph* g)
 {
     if (!g) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (!g->state_init) FAIL(MGC_E_STATE, "call mgc_slab_begin first");
     CK(cudaSetDevice(g->device));
     g->st.global_relabels++;
@@ -239,6 +245,7 @@ int mgc_slab_relabel_begin(mgc_graph* g)
 int mgc_slab_relabel_relax(mgc_graph* g, int32_t* changed_out)
 {
     if (!g) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     int any = 0;
     const int rc = relabel_tiles_run(g, &any, changed_out != nullptr);
@@ -250,6 +257,7 @@ int mgc_slab_relabel_relax(mgc_graph* g, int32_t* changed_out)
 int mgc_slab_count_active(mgc_graph* g, int64_t* active_out)
 {
     if (!g || !active_out) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     return count_active_tiles(g, active_out);
 }
@@ -257,6 +265,7 @@ int mgc_slab_count_active(mgc_graph* g, int64_t* active_out)
 int mgc_slab_count_active_dev(mgc_graph* g, unsigned long long* count_dev)
 {
     if (!g || !count_dev) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     return count_active_tiles_enqueue(g, count_dev);
 }
@@ -264,6 +273,7 @@ int mgc_slab_count_active_dev(mgc_graph* g, unsigned long long* count_dev)
 int mgc_slab_finish(mgc_graph* g, double* energy_part)
 {
     if (!g || !energy_part) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     CK(cudaSetDevice(g->device));
     int rc = readout(g, energy_part);
     if (rc) return rc;
@@ -290,6 +300,7 @@ int mgc_slab_comm_unique_id(void* out128)
 int mgc_slab_comm_init(mgc_graph* g, int32_t rank, int32_t world, const void* unique_id128)
 {
     if (!g || !unique_id128 || world < 1 || rank < 0 || rank >= world) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (!g->slab) FAIL(MGC_E_STATE, "not a z-slab handle");
     NcclApi& N = nccl_api();
     if (!N.ok) FAIL(MGC_E_CUDA, "libnccl.so.2 could not be loaded");
@@ -318,6 +329,7 @@ int mgc_slab_comm_init(mgc_graph* g, int32_t rank, int32_t world, const void* un
 int mgc_slab_solve(mgc_graph* g, double* energy_total)
 {
     if (!g || !energy_total) return MGC_E_ARG;
+    if (batch_refused(g)) return MGC_E_STATE;
     if (!g->slab || !g->comm) FAIL(MGC_E_STATE, "call mgc_slab_comm_init first");
     NcclApi& N = nccl_api();
     CK(cudaSetDevice(g->device));

@@ -198,6 +198,7 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
         Cells nxt{(E)0, (E)0};
         if (inext < n) nxt = load(list[inext]);
         const unsigned valid = c.inb ? tile_pairs(L, c) : 0u;
+        const BoundaryParams Pv = params_at(P, L, c.tz * TILE + c.lz);     // this voxel's term constants
         const double a = build_val<E>(s_img[h], use_max);
         const E q[6] = {s_img[h - HALO_DIM * HALO_DIM], s_img[h + HALO_DIM * HALO_DIM], s_img[h - HALO_DIM],
                         s_img[h + HALO_DIM], s_img[h - 1], s_img[h + 1]};
@@ -209,7 +210,7 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
                 const double b = build_val<E>(q[k], use_max);
                 // cells outside the lattice were never staged: their (unused) arguments are pinned to 0 so that they
                 // cannot push the warp off the ordinary path
-                t6[k] = ((valid >> k) & 1u) ? exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b))) : 0.0;
+                t6[k] = ((valid >> k) & 1u) ? exp_term_arg(Pv, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b))) : 0.0;
             }
             const bool ordinary = __all_sync(0xffffffffu, t6[0] <= 700.0 && t6[1] <= 700.0 && t6[2] <= 700.0 &&
                                                           t6[3] <= 700.0 && t6[4] <= 700.0 && t6[5] <= 700.0);
@@ -217,7 +218,7 @@ k_caps_tiles(Lattice L, Tiles TL, State<double> S, const E* __restrict__ img, Bo
         } else {
 #pragma unroll
             for (int k = 0; k < 6; ++k)
-                cap[k] = ((valid >> k) & 1u) ? build_weight<FN, E>(P, a, q[k], use_max, spacing, P.spacing[k >> 1]) : 0.0;
+                cap[k] = ((valid >> k) & 1u) ? build_weight<FN, E>(Pv, a, q[k], use_max, spacing, P.spacing[k >> 1]) : 0.0;
         }
         if (c.inb) {
             const double tr = lazy_tr(tin, p, fb);

@@ -142,7 +142,35 @@ struct BoundaryParams {
     double inv_sigma2; // exponential: 1 / pow(sigma, 2) (see g_weight)
     double inv_spacing_on; // 0: no spacing
     double spacing[4]; // canonical axes
+    // batch lattice (Lattice::zper > 0): per image the one constant its term reads -- M (linear), sigma (division, power)
+    // or pow(sigma, 2) (exponential) -- replacing norm / sigma above (device array, one entry per image); else nullptr
+    const double* ktab;
 };
+
+// The term's constants for a voxel in plane gz: P itself on a lattice of one image, else P with the constant of the
+// plane's image (inv_sigma2 formed from it exactly as the host forms it from pow(sigma, 2)).  A pair never spans two images
+// (z_pairs), so either end of a pair gives the same constants.
+__device__ __forceinline__ BoundaryParams params_at(const BoundaryParams& P, const Lattice& L, int gz)
+{
+    BoundaryParams Q = P;
+    if (L.zper) {
+        const double k = P.ktab[image_of(L, gz < L.dim[0] ? gz : L.dim[0] - 1)];
+        Q.norm = k;
+        Q.sigma = k;
+        Q.inv_sigma2 = (P.fn == 1 && k != 0.0) ? __ddiv_rn(1.0, k) : 0.0;
+    }
+    return Q;
+}
+
+// The exponential constant of the range test of a block whose staged box covers planes z_lo .. z_hi (clamped to the
+// lattice): on a batch lattice the largest of the images' constants (exp_table_inv_max, gc_exprange.cuh)
+__device__ __forceinline__ double range_inv_sigma2(const BoundaryParams& P, const Lattice& L, int z_lo, int z_hi)
+{
+    if (!L.zper) return P.inv_sigma2;
+    z_lo = z_lo < 0 ? 0 : z_lo;
+    z_hi = z_hi < L.dim[0] ? z_hi : L.dim[0] - 1;
+    return exp_table_inv_max(P.ktab, image_of(L, z_lo), image_of(L, z_hi));
+}
 
 // exp(-t) for t >= 0 in ~25 instructions (CUDA's general exp() costs ~80 here, and K1 is bound by instruction issue):
 // n = rint(-t*log2 e), r = -t - n*ln2 (two-step, exact product with the hi part), e^r by a degree-13 Taylor polynomial in

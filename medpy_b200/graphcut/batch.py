@@ -1,0 +1,173 @@
+"""Many small, independent cuts in one build and one solve: the slices of a stack segmented slice by slice, a cohort of
+volumes, the patches of a tiled image (DESIGN.md §3.1).
+
+``graph_from_voxels_batch`` takes B images of the same shape (1-D to 3-D) stacked along a leading batch axis, with one
+set of markers and (optionally) one probability map per image, and returns a ``BatchGraph`` whose ``maxflow()`` gives
+the B energies and whose ``get_mask()`` gives the B masks.  Each image is cut as if it were alone: its mask and energy
+are those of ``graph_from_voxels`` on that image (the energy up to the order of the sums).  The images share one
+lattice on the device, so a batch of small images fills the GPU where one of them would not.
+"""
+import math
+import numbers
+
+import numpy
+
+from .device import _KINDS, _as_u8
+from .energy_voxel import _device_image, _native_order
+
+# the lattice index of one handle is 32-bit: batch x voxels per image must stay below this
+INDEX_LIMIT = 1 << 31
+
+_LINEAR = {"difference_linear": False, "maximum_linear": True}     # name -> the normaliser is max |x|
+_MAX_TERMS = ("maximum_linear", "maximum_exponential", "maximum_power")
+
+
+def _is_cuda(a):
+    return hasattr(a, "__cuda_array_interface__")
+
+
+def _shape(a):
+    return tuple(int(s) for s in a.shape)
+
+
+def _markers(m):
+    if m is None or _is_cuda(m):
+        return _as_u8(m)
+    m = numpy.asarray(m)
+    return m.view(numpy.uint8) if m.dtype in (numpy.bool_, numpy.uint8) else (m != 0).view(numpy.uint8)
+
+
+def _sigmas(sigma, batch):
+    if sigma is None:
+        return [0.0] * batch
+    if isinstance(sigma, numbers.Real):
+        return [float(sigma)] * batch
+    s = [float(x) for x in sigma]
+    if len(s) != batch:
+        raise ValueError(f"sigma has {len(s)} entries for a batch of {batch} images")
+    return s
+
+
+def _host_image(image, boundary):
+    """A host image as the native build reads it, and the linear normaliser of every image (NaN: reduced on the device).
+    Integer images are normalised with numpy per image, in their own dtype, as ``energy_voxel`` does for one image."""
+    image = _native_order(numpy.asarray(image))
+    batch = image.shape[0]
+    norms = [math.nan] * batch
+    if boundary in _LINEAR and image.dtype.type not in (numpy.float32, numpy.float64):
+        for b in range(batch):
+            if _LINEAR[boundary]:
+                norms[b] = float(numpy.abs(image[b]).max())
+            else:
+                norms[b] = float(abs(image[b].max() - image[b].min()))
+    dev = _device_image(image)
+    if boundary in _MAX_TERMS and dev.dtype != image.dtype:
+        dev = numpy.abs(image).astype(numpy.float64)     # numpy.abs in the input dtype first (energy_voxel.py:558)
+    return dev, norms
+
+
+def _prob_arg(prob, alpha):
+    """The probability map as the fused build reads it, and whether its products are float32, decided as
+    ``energy_voxel.regional_probability_map`` decides them for one image: the map in native byte order, float32 products
+    where numpy forms them in float32 (a float32 map times a Python float).  Integer maps give float64 products, which a
+    float64 copy gives exactly; other dtypes (float16) have products the build cannot form."""
+    if _is_cuda(prob):
+        kind = str(prob.dtype)
+        if "float32" not in kind and "float64" not in kind:
+            raise ValueError(f"a batch's probability map must be float32 or float64, got {prob.dtype}")
+        return prob, "float32" in kind
+    prob = _native_order(numpy.asarray(prob))
+    src_dtype = (prob[:0] * alpha).dtype
+    snk_dtype = ((1 - prob[:0]) * alpha).dtype
+    if prob.dtype == numpy.float32 or prob.dtype == numpy.float64:
+        return prob, bool(prob.dtype == numpy.float32 and src_dtype == numpy.float32 and snk_dtype == numpy.float32)
+    if src_dtype == numpy.float64 and snk_dtype == numpy.float64:
+        return prob.astype(numpy.float64), False
+    raise ValueError(f"a batch's probability map must give float32 or float64 products, got {prob.dtype}")
+
+
+class BatchGraph:
+    """The graph of a batch of images (``graph_from_voxels_batch``)."""
+
+    def __init__(self, native, batch):
+        self._native = native
+        self.batch = batch
+
+    def maxflow(self):
+        """Solve every image; returns a float64 array of the B energies."""
+        self._native.maxflow()
+        return self._native.get_batch_energies()
+
+    def get_mask(self):
+        """uint8 array of shape (B, ...image): 1 where the voxel is not on the SINK side, as ``GraphDouble.get_mask``."""
+        return self._native.get_mask()
+
+    def stats(self):
+        return self._native.stats()
+
+    # Warm edits are not available on a batch: each of these raises (the native handle refuses them).
+    def add_seeds(self, fg_ids=None, bg_ids=None):
+        self._native.add_seeds(fg_ids, bg_ids)
+
+    def remove_seeds(self, fg_ids=None, bg_ids=None):
+        self._native.remove_seeds(fg_ids, bg_ids)
+
+    def add_tweights_warm(self, ids, src, snk):
+        self._native.add_tweights_warm(ids, src, snk)
+
+    def add_nweights_warm(self, i, j, cap, rev_cap):
+        self._native.add_nweights_warm(i, j, cap, rev_cap)
+
+    def remove_nweights_warm(self, i, j, cap, rev_cap):
+        self._native.remove_nweights_warm(i, j, cap, rev_cap)
+
+    def add_nweights_dense_warm(self, axis, fwd, bwd):
+        self._native.add_nweights_dense_warm(axis, fwd, bwd)
+
+    def remove_nweights_dense_warm(self, axis, fwd, bwd):
+        self._native.remove_nweights_dense_warm(axis, fwd, bwd)
+
+
+def graph_from_voxels_batch(fg_markers, bg_markers, image, boundary, sigma=None, spacing=False, prob=None, alpha=None):
+    """Build the graphs of B independent images in one fused build.
+
+    The leading axis of every array is the batch; numpy arrays and CUDA arrays (``__cuda_array_interface__``, e.g. torch
+    tensors) are both accepted, as in ``graph_from_device_arrays``.
+    boundary : one of the eight ``energy_voxel.boundary_*`` names without the prefix (required)
+    sigma : a float for every image, or one per image
+    spacing, prob, alpha : as in ``graph_from_device_arrays``; shared by the whole batch
+    """
+    if boundary not in _KINDS:
+        raise ValueError(f"a batch needs one of the boundary terms {sorted(_KINDS)}, got {boundary!r}")
+    shape = _shape(image)
+    if len(shape) < 2:
+        raise ValueError("the leading axis of the arrays is the batch: image needs at least two axes")
+    batch, image_shape = shape[0], shape[1:]
+    if len(image_shape) > 3:
+        raise ValueError("batch images are 1-D to 3-D")
+    for name, a in (("fg_markers", fg_markers), ("bg_markers", bg_markers), ("prob", prob)):
+        if a is not None and _shape(a) != shape:
+            raise ValueError(f"{name} has shape {_shape(a)}, image has {shape}")
+    if batch * math.prod(image_shape) >= INDEX_LIMIT:
+        raise ValueError(f"{batch} images of {math.prod(image_shape)} voxels reach the 2^31 voxel index limit of one batch")
+    sigmas = _sigmas(sigma, batch)
+    sp = None
+    if spacing:
+        sp = [float(s) for s in spacing]
+        if len(sp) < len(image_shape):
+            raise ValueError("spacing has fewer entries than the images have dimensions")
+    if _is_cuda(image):
+        norms = [math.nan] * batch
+    else:
+        image, norms = _host_image(image, boundary)
+
+    alpha = 0.0 if alpha is None else float(alpha)
+    compute_f32 = False
+    if prob is not None:
+        prob, compute_f32 = _prob_arg(prob, alpha)
+
+    from .. import _lib   # raises ImportError loudly when the extension is not built
+    native = _lib.Graph.batch(list(image_shape), batch, -1)
+    native.build_voxel_batch(prob, alpha, compute_f32, _KINDS[boundary], image, sigmas, sp, norms, _markers(fg_markers),
+                             _markers(bg_markers))
+    return BatchGraph(native, batch)
