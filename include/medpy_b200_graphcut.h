@@ -236,8 +236,17 @@ int mgc_can_fuse(const mgc_graph* g);
  * solve.  The images are stacked along axis 0 of one (batch * Z, Y, X) lattice (canonical image shape (Z, Y, X) with
  * leading 1s) whose pairs across the seams between images do not exist, so each image is cut as if it were alone.
  * MGC_E_ARG when batch * (voxels per image) would reach 2^31, checked before anything is allocated.
- * On a batch handle the per-term calls, mgc_build_voxel_graph, every warm call (mgc_add_seeds ...
- * mgc_remove_nweights_dense_warm), MGC_OPT_WARM and the z-slab calls return MGC_E_STATE with one message.
+ * On a batch handle the per-term calls, mgc_build_voxel_graph and the z-slab calls return MGC_E_STATE with one message.
+ * The warm calls (mgc_add_seeds ... mgc_remove_nweights_dense_warm) return it too unless MGC_OPT_WARM is set and the
+ * state comes from mgc_build_voxel_batch (not after mgc_reset).  The option follows the rule of a single handle: on an
+ * eagerly built batch (MEDPY_GC_LAZY_CAPS=0) it must be set before the first solve, whose start records the residual
+ * source capacities the folds read; a lazily built batch (the default) needs no record, so there it is also accepted
+ * after a solve and admits the folds from then on.  With the option
+ * they fold as on a single lattice handle, before or after a solve: node ids are C-order over (batch, ...image); a listed
+ * pair across the seam between two images is no lattice pair (MGC_E_ARG, the handle unchanged); the dense n-link forms
+ * take the lattice's canonical axis (0 = the image's Z axis of 3-D images) and ignore the last plane of every image along
+ * axis 0; each fold's change of the add_tweights constants goes to the images it touched, so mgc_get_batch_energies
+ * stays per image and the images a fold does not touch keep their energies bit for bit.
  * Adding these three entry points left MGC_ABI_VERSION at 3 and mgc_stats unchanged. */
 int mgc_create_batch(int32_t ndim, const int64_t* image_shape, int64_t batch, int32_t device, mgc_graph** out);
 /* The terms of every image in one fused build.  The arrays of `terms` are over the logical (batch, ...image) shape

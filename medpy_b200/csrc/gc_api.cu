@@ -681,8 +681,8 @@ int mgc_set_option(mgc_graph* g, int32_t option, int64_t value)
     if (option == MGC_OPT_DEFER_WEIGHT_CHECK) { g->defer_check = value != 0; return MGC_OK; }
     if (option == MGC_OPT_KEEP_DEVICE_INPUTS) { g->keep_device_inputs = value != 0; return MGC_OK; }
     if (option == MGC_OPT_WARM) {
-        if (batch_refused(g)) return MGC_E_STATE;
         // the record is taken before the first push; a lazily built handle folds without it, so there it changes nothing now
+        // (on a batch handle the option also admits the folds at all, batch_warm)
         const bool on = value != 0;
         if (on != g->warm_opt && g->flow_started && !g->lazy_built)
             FAIL(MGC_E_STATE, "MGC_OPT_WARM is set before the first solve (the residual source capacities are recorded at "

@@ -6,6 +6,7 @@
 // solver, which only sees capacities and rmask bits, computes B independent minimum cuts without knowing about images.
 #include "gc_handle.cuh"
 
+#include <algorithm>
 #include <cmath>
 
 namespace {
@@ -72,15 +73,119 @@ __global__ void k_batch_norms(double* __restrict__ ktab, const double* __restric
     if (b < B && ktab[b] != ktab[b]) ktab[b] = mm[2 * b + which];
 }
 
+// The change a fold made to the add_tweights constant, per image: tconst[b] += the sum of dk[i] over the fold's entries i
+// < *count in image b.  The entries are in ascending voxel order (vox[i * vstride] is entry i's voxel), so each image's
+// entries form one run.  Two passes over fixed chunks of FOLD_CHUNK entries, so the same calls give the same bits and no
+// chain of dependent steps grows with the length of a run:
+//   k_batch_fold_chunks: one block per chunk sums every piece of a run inside the chunk with a segmented Hillis-Steele
+//     scan (eight fixed steps).  A run that starts and ends in the chunk goes straight into tconst[b]; the piece at the
+//     chunk's start of a run that began earlier is cont[c]; the piece at its end of a run that goes on is head[c], with
+//     span[c] = b (else -1);
+//   k_batch_fold_spans: one block per chunk with span[c] = b finds the end of b's run (a binary search over the entries)
+//     and adds head[c] + the cont[] of the chunks the run covers, summed by the block in a fixed tree.
+// Each image is written by one thread of one block.  The work is proportional to the entries, not to B.
+constexpr unsigned FOLD_CHUNK = 256;
+
+__device__ __forceinline__ int fold_image(const Lattice& L, const unsigned* __restrict__ vox, int vstride, unsigned i)
+{
+    return image_of(L, (int)div_stride(L, __ldg(vox + (size_t)i * (unsigned)vstride), 0));
+}
+
+__global__ void __launch_bounds__(FOLD_CHUNK) k_batch_fold_chunks(Lattice L, const unsigned* __restrict__ vox, int vstride,
+                                                                  const int* __restrict__ count,
+                                                                  const double* __restrict__ dk, double* __restrict__ tconst,
+                                                                  double* __restrict__ cont, double* __restrict__ head,
+                                                                  int* __restrict__ span)
+{
+    __shared__ double sv[FOLD_CHUNK];
+    __shared__ unsigned char sf[FOLD_CHUNK];
+    __shared__ int s_first;                    // the image of the chunk's first entry if its run began earlier, else -1
+    const unsigned n = (unsigned)*count;       // < 2^31: no index below overflows
+    const unsigned t = threadIdx.x;
+    for (unsigned c = blockIdx.x; c * FOLD_CHUNK < n; c += gridDim.x) {
+        const unsigned i = c * FOLD_CHUNK + t;
+        const bool in = i < n;
+        int b = -1;
+        double v = 0.0;
+        bool start = false;                    // the run of b starts at i
+        if (in) {
+            b = fold_image(L, vox, vstride, i);
+            start = i == 0 || fold_image(L, vox, vstride, i - 1) != b;
+            v = dk[i];
+        }
+        if (t == 0) { s_first = start ? -1 : b; span[c] = -1; }
+        bool f = t == 0 || start;              // a piece starts at t
+        sv[t] = v;
+        sf[t] = f;
+        __syncthreads();
+        for (unsigned d = 1; d < FOLD_CHUNK; d <<= 1) {
+            double pv = 0.0;
+            bool pf = true;
+            if (t >= d) { pv = sv[t - d]; pf = sf[t - d] != 0; }
+            __syncthreads();
+            if (!f) { v = __dadd_rn(pv, v); f = pf; }
+            sv[t] = v;
+            sf[t] = f;
+            __syncthreads();
+        }
+        if (in) {
+            const bool ends = i + 1 == n || fold_image(L, vox, vstride, i + 1) != b;     // the run of b ends at i
+            if (ends || t + 1 == FOLD_CHUNK) {                                          // i ends its piece
+                if (b == s_first) cont[c] = v;
+                else if (ends) tconst[b] = __dadd_rn(tconst[b], v);
+                else { head[c] = v; span[c] = b; }
+            }
+        }
+        __syncthreads();                       // s_first and the scan arrays are reused by the next chunk
+    }
+}
+
+__global__ void __launch_bounds__(FOLD_CHUNK) k_batch_fold_spans(Lattice L, const unsigned* __restrict__ vox, int vstride,
+                                                                 const int* __restrict__ count,
+                                                                 const double* __restrict__ cont,
+                                                                 const double* __restrict__ head,
+                                                                 const int* __restrict__ span, double* __restrict__ tconst)
+{
+    __shared__ double sh[FOLD_CHUNK];
+    __shared__ unsigned s_last;
+    const unsigned n = (unsigned)*count;
+    const unsigned t = threadIdx.x;
+    for (unsigned c = blockIdx.x; c * FOLD_CHUNK < n; c += gridDim.x) {
+        const int b = span[c];                 // block-uniform
+        if (b < 0) continue;
+        if (t == 0) {
+            // the first entry past b's run, in (c + 1) * FOLD_CHUNK .. n: the images are ascending
+            unsigned lo = (c + 1) * FOLD_CHUNK, hi = n;
+            while (lo < hi) {
+                const unsigned mid = lo + ((hi - lo) >> 1);
+                if (fold_image(L, vox, vstride, mid) <= b) lo = mid + 1; else hi = mid;
+            }
+            s_last = (lo - 1) / FOLD_CHUNK;    // the chunk of the run's last entry
+        }
+        __syncthreads();
+        double s = 0.0;
+        for (unsigned k = c + 1 + t; k <= s_last; k += FOLD_CHUNK) s = __dadd_rn(s, cont[k]);
+        sh[t] = s;
+        __syncthreads();
+        for (unsigned k = FOLD_CHUNK / 2; k > 0; k >>= 1) {
+            if (t < k) sh[t] = __dadd_rn(sh[t], sh[t + k]);
+            __syncthreads();
+        }
+        if (t == 0) tconst[b] = __dadd_rn(tconst[b], __dadd_rn(head[c], sh[0]));
+        __syncthreads();                       // s_last and sh are reused by the next chunk
+    }
+}
+
 double* ktab_of(mgc_graph* g) { return g->batch_buf; }
 double* tconst_of(mgc_graph* g) { return g->batch_buf + g->batch; }
 double* energy_of(mgc_graph* g) { return g->batch_buf + 2 * g->batch; }
 double* mm_of(mgc_graph* g) { return g->batch_buf + 3 * g->batch; }
 double* part_of(mgc_graph* g) { return g->batch_buf + 5 * g->batch; }
+}  // namespace
 
 // A (B, ...) input array as a C-contiguous array over the batch lattice (B * Z, Y, X): the array itself with the
-// lattice's strides when it is one, else a copy gathered into the build's staging slot (what stage_input does for a
-// strided input of a single image; the build then reads the slot in place).
+// lattice's strides when it is one, else a copy gathered into the staging slot (what stage_input does for a strided
+// input of a single image; the build, or the dense fold that stages the result, then reads the slot in place).
 int batch_view(mgc_graph* g, const mgc_array* a, int slot, mgc_array* out)
 {
     const size_t es = dtype_size(a->dtype);
@@ -144,7 +249,27 @@ int batch_view(mgc_graph* g, const mgc_array* a, int slot, mgc_array* out)
     out->mem = MGC_MEM_DEVICE;
     return MGC_OK;
 }
-}  // namespace
+
+// Chunks of the per-image constant sum for a fold of at most max_count entries (the size of `part`: 2 doubles each, and
+// of `span`: 1 int each)
+size_t batch_fold_chunks(int max_count) { return ((size_t)(max_count > 0 ? max_count : 0) + FOLD_CHUNK - 1) / FOLD_CHUNK; }
+
+// The per-image constant sum after a fold's kernels, on the fold's entries (at most max_count; their count is on the
+// device); part / span: scratch of batch_fold_chunks(max_count) chunks
+int batch_fold_const(mgc_graph* g, const unsigned* vox, int vstride, const int* count, int max_count, const double* dk,
+                     double* part, int* span)
+{
+    const size_t chunks = batch_fold_chunks(max_count);
+    if (!chunks) return MGC_OK;
+    const unsigned grid = (unsigned)std::min<size_t>(chunks, (size_t)g->n_ctas * 4u);
+    double* cont = part;
+    double* head = part + chunks;
+    k_batch_fold_chunks<<<grid, FOLD_CHUNK, 0, g->stream>>>(g->L, vox, vstride, count, dk, tconst_of(g), cont, head, span);
+    k_batch_fold_spans<<<grid, FOLD_CHUNK, 0, g->stream>>>(g->L, vox, vstride, count, cont, head, span, tconst_of(g));
+    g->st.kernel_launches += 2;
+    CK(cudaGetLastError());
+    return MGC_OK;
+}
 
 // The term-constant table of a batch build (BoundaryParams::ktab): the host values of mgc_build_voxel_batch, and for the
 // linear terms the normaliser M of every image whose entry is NaN, reduced on the device over that image alone

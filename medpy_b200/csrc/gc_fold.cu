@@ -43,19 +43,23 @@ int warm_prepare(mgc_graph* g)
 namespace {
 
 // f(A) with the residual access of a fold on this handle (gc_seeds.cuh): LazyResidual with the lazy build's instantiation,
-// or (eager: an MGC_OPT_WARM handle) EagerResidual<3> / <4>
+// or (eager: an MGC_OPT_WARM handle) EagerResidual<3> / <4>; batch handles (3-D lattices) take the BATCH variants
 template <typename F>
 void residual_dispatch(const mgc_graph* g, bool eager, F&& f)
 {
     if (eager) {
-        if (g->nd == 4) f(EagerResidual<4>{g->S, g->smask});
-        else            f(EagerResidual<3>{g->S, g->smask});
+        if (g->nd == 4)     f(EagerResidual<4>{g->S, g->smask});
+        else if (g->batch)  f(EagerResidual<3, true>{g->S, g->smask});
+        else                f(EagerResidual<3>{g->S, g->smask});
         return;
     }
     lazy_dispatch(g, [&](auto t) {
         using T = decltype(t);
         using E = typename T::E;
-        f(LazyResidual<E, T::FN, T::USE_MAX, T::SPACING>{g->L, g->S, (const E*)g->caps_img, g->caps_P});
+        // a batch replays each voxel's capacities with its image's constants and stores each entry's constant change;
+        // single handles keep the plain kernels
+        if (g->batch) f(LazyResidual<E, T::FN, T::USE_MAX, T::SPACING, true>{g->L, g->S, (const E*)g->caps_img, g->caps_P});
+        else          f(LazyResidual<E, T::FN, T::USE_MAX, T::SPACING, false>{g->L, g->S, (const E*)g->caps_img, g->caps_P});
     });
 }
 
@@ -156,7 +160,7 @@ static cudaError_t tails_sort(void* tmp, size_t* bytes, const unsigned* tails, u
 static int warm_check(mgc_graph* g, bool* eager)
 {
     *eager = false;
-    if (batch_refused(g)) return MGC_E_STATE;
+    if (g->batch && !batch_warm(g)) return batch_refused(g);
     if (!g->slab && g->lazy_built && g->state_init && g->nd == 3) return MGC_OK;
     if (warm_wanted(g)) { *eager = true; return MGC_OK; }
     FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
@@ -216,7 +220,8 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
         rc = caps_launch(g, WorkList{tiles, d_ctl + 2});
         if (rc) return rc;
     }
-    // 2. the fold, its change of the add_tweights constant summed in a fixed order into flow_const
+    // 2. the fold, its change of the add_tweights constant summed in a fixed order into flow_const (on a batch handle the
+    // fold also adds each image's share into that image's constant, batch_fold_const)
     unsigned grid = (unsigned)((ni + 255) / 256);
     if (grid > REDUCE_BLOCKS) grid = REDUCE_BLOCKS;
     { int rc = fold(grid, ni); if (rc) return rc; }
@@ -291,6 +296,9 @@ struct FoldBufs {
     unsigned* tails;
     double* dx;                   // item_flows: one double per item
     unsigned* stails;             // item_flows: the tails in ascending order (tails_sort)
+    double* dk;                   // batch handles: the change of the add_tweights constant per item (or per sorted tail),
+    double* dk_part;              // ... and the chunk sums and run images of its per-image sum (batch_fold_const)
+    int* dk_span;
     void* tmp;                    // cub scratch
     size_t tmp_bytes;
 };
@@ -326,8 +334,15 @@ static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold,
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
     const void* in[4] = {c.in[0], c.in[1], c.in[2], c.in[3]};
-    for (int k = 0; k < 2; ++k)
-        if (c.arrays[k]) { int rc0 = stage_input(g, c.arrays[k], k, &in[2 + k]); if (rc0) return rc0; }
+    for (int k = 0; k < 2; ++k) {
+        if (!c.arrays[k]) continue;
+        // a batch's dense arrays are over (B, ...image): first as an array over its (B * Z, Y, X) lattice
+        mgc_array view;
+        const mgc_array* a = c.arrays[k];
+        if (g->batch) { int rc0 = batch_view(g, a, k, &view); if (rc0) return rc0; a = &view; }
+        int rc0 = stage_input(g, a, k, &in[2 + k]);
+        if (rc0) return rc0;
+    }
     int rc = MGC_OK;
     if (c.count) {                              // else nothing to fold: the solved state, mask and energy stay as they are
         const auto host_t0 = std::chrono::steady_clock::now();
@@ -371,6 +386,10 @@ static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold,
             b.tails = m.take<unsigned>(ntails);
             b.dx = m.take<double>(c.item_flows ? (size_t)n : 0);
             b.stails = m.take<unsigned>(c.item_flows ? ntails : 0);
+            const size_t nd = g->batch ? std::max((size_t)n, ntails) : 0;
+            b.dk = nd ? m.take<double>(nd) : nullptr;
+            b.dk_part = nd ? m.take<double>(2 * batch_fold_chunks((int)nd)) : nullptr;
+            b.dk_span = nd ? m.take<int>(batch_fold_chunks((int)nd)) : nullptr;
             b.tmp = m.take<char>(tmp_bytes);
             b.tmp_bytes = tmp_bytes;
             return m.used;
@@ -423,6 +442,20 @@ static int fold_run(mgc_graph* g, const FoldCall& c, Group&& group, Fold&& fold,
     return rc;
 }
 
+// The t-link fold over a grouping's items, then on a batch handle the per-image sum of their constant changes (the
+// items are in ascending voxel order, TweightItem::v first)
+template <typename Calls>
+static int tlink_fold(mgc_graph* g, const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni,
+                      const Calls& calls)
+{
+    residual_dispatch(g, eager, [&](auto A) {
+        k_tlink_fold<<<grid, 256, 0, g->stream>>>(A, b.items, ni, calls, g->partials, b.dk);
+    });
+    if (!g->batch) return MGC_OK;
+    return batch_fold_const(g, reinterpret_cast<const unsigned*>(b.items), (int)(sizeof(TweightItem) / sizeof(unsigned)),
+                            b.ctl, ni, b.dk, b.dk_part, b.dk_span);
+}
+
 extern "C" {
 
 // mgc_add_seeds (cap = 65535) and mgc_remove_seeds (cap = -65535): add_tweights(v, cap, 0) for every fg id in list order,
@@ -452,9 +485,7 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
             return MGC_OK;
         },
         [&](const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni) {
-            residual_dispatch(g, eager, [&](auto A) {
-                k_tlink_fold<<<grid, 256, 0, g->stream>>>(A, b.items, ni, SeedCalls{b.skeys, cap}, g->partials);
-            });
+            return tlink_fold(g, b, eager, grid, ni, SeedCalls{b.skeys, cap});
         });
 }
 
@@ -501,9 +532,7 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
         },
         [&](const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni) {
             const ListCalls calls{dense ? nullptr : b.svals, (const double*)b.in[1], (const double*)b.in[2]};
-            residual_dispatch(g, eager, [&](auto A) {
-                k_tlink_fold<<<grid, 256, 0, g->stream>>>(A, b.items, ni, calls, g->partials);
-            });
+            return tlink_fold(g, b, eager, grid, ni, calls);
         });
 }
 
@@ -523,8 +552,13 @@ static int nweights_group(mgc_graph* g, const FoldCall& c, const NlinkBufs& b, u
     const double* d_cap = (const double*)b.in[2];
     const double* d_rev = (const double*)b.in[3];
     if (c.dense) {
-        const unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
-        const unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
+        // axis 0 spans the lattice, or one image of a batch (k_nlinks_dense_heads)
+        unsigned span = axis == 0 ? g->L.n : g->L.stride[axis - 1];
+        unsigned long long magic = axis == 0 ? 0ull : g->L.magic[axis - 1];
+        if (axis == 0 && g->L.zper) {
+            span = (unsigned)g->L.zper * g->L.stride[0];
+            magic = span <= 1 ? 0ull : (~0ull / span) + 1ull;
+        }
         k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap, d_rev,
                                                            b.head, b.ctl + 1);
         return MGC_OK;
@@ -608,9 +642,10 @@ static int nweights_remove_fold(mgc_graph* g, FoldCall& c, int axis)
             const unsigned long long* skeys = dense ? nullptr : b.skeys;
             residual_dispatch(g, eager, [&](auto A) {
                 k_nlinks_remove_voxels<<<grid, 256, 0, g->stream>>>(A, g->L, skeys, b.head, b.pos, n, axis, b.dx, b.stails,
-                                                                    ntails, g->partials);
+                                                                    ntails, g->partials, b.dk);
             });
-            return MGC_OK;
+            // a batch: the shortfalls the terminal links covered, per image (the sorted tails are in ascending order)
+            return g->batch ? batch_fold_const(g, b.stails, 1, ntails, nt, b.dk, b.dk_part, b.dk_span) : MGC_OK;
         },
         [&](const NlinkBufs& b, bool eager) {
             // after the first read-back: the item count is on the device in b.ctl[0]

@@ -197,7 +197,8 @@ struct mgc_graph {
     int64_t batch = 0;                 // images (0: not a batch handle)
     int batch_ndim = 0;                // dimensions of one image (1..3)
     int batch_chunks = 1;              // blocks per image of the per-image reductions
-    bool batch_built = false;          // the state comes from mgc_build_voxel_batch (cleared by mgc_reset)
+    bool batch_built = false;          // the state comes from mgc_build_voxel_batch (cleared by mgc_reset); with
+                                       // MGC_OPT_WARM the warm folds edit it and its per-image constants (batch_warm)
     double* batch_buf = nullptr;       // [B] term constants (BoundaryParams::ktab) | [B] add_tweights constants |
                                        // [B] energies | [2B] min / max read-outs | [B * batch_chunks] partials
     std::vector<double> batch_k_host;  // the term constants of the next build (NaN: M computed on the device)
@@ -246,6 +247,10 @@ int voxel_build(mgc_graph* g, const mgc_voxel_terms* t);
 // ---- gc_batch.cu ----------------------------------------------------------------------------------------
 int batch_constants(mgc_graph* g, int dtype, const void* d_img, BoundaryParams* P);
 int batch_tconst(mgc_graph* g, const BuildArgs& A);
+int batch_view(mgc_graph* g, const mgc_array* a, int slot, mgc_array* out);
+size_t batch_fold_chunks(int max_count);
+int batch_fold_const(mgc_graph* g, const unsigned* vox, int vstride, const int* count, int max_count, const double* dk,
+                     double* part, int* span);
 
 // ---- gc_fold.cu -----------------------------------------------------------------------------------------
 int warm_prepare(mgc_graph* g);
@@ -254,14 +259,20 @@ int warm_prepare(mgc_graph* g);
 void slab_comm_release(mgc_graph* g);
 
 // ---- inline helpers ---------------------------------------------------------------------------------------
-// The one refusal of every call a batch handle does not take: MGC_E_STATE with this message (else MGC_OK)
+// The one refusal of every call a batch handle does not take: MGC_E_STATE with this message (else MGC_OK).  The warm
+// folds take it too, unless the handle has MGC_OPT_WARM and a state from mgc_build_voxel_batch (batch_warm).
 inline int batch_refused(const mgc_graph* g)
 {
     if (!g->batch) return MGC_OK;
-    const_cast<mgc_graph*>(g)->err = "batch handles take their terms from mgc_build_voxel_batch only: the per-term calls, "
-                                     "warm edits, MGC_OPT_WARM and the z-slab calls are not available on them";
+    const_cast<mgc_graph*>(g)->err = "batch handles take their terms from mgc_build_voxel_batch only: the per-term calls "
+                                     "and the z-slab calls are not available on them, and the warm edits need "
+                                     "MGC_OPT_WARM set before mgc_build_voxel_batch";
     return MGC_E_STATE;
 }
+
+// a batch handle whose state the warm folds may edit: MGC_OPT_WARM was set, and the state comes from the batch build
+// (the per-image constants exist and stay valid until mgc_reset)
+inline bool batch_warm(const mgc_graph* g) { return g->batch && g->warm_opt && g->batch_built; }
 
 // NVTX range per phase (build / relabel / push / readout / exchange): visible in nsys / ncu timelines, a no-op without a
 // profiler attached (SURVEY.md §5.1)

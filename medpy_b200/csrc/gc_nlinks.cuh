@@ -45,7 +45,8 @@ struct NlinkItem {
 };
 
 // canonical axis of the pair (lo, lo + d): the axis a with d == stride[a] whose extent lo does not end; -1 if there is none
-// (strides of extent-1 axes repeat a larger one, but lo is on their last plane)
+// (strides of extent-1 axes repeat a larger one, but lo is on their last plane).  Axis 0 takes z_pairs' rule, so on a
+// batch lattice a pair across the seam between two images is no pair either.
 template <int ND>
 __device__ __forceinline__ int nlink_axis(const Lattice& L, unsigned lo, unsigned d)
 {
@@ -54,7 +55,7 @@ __device__ __forceinline__ int nlink_axis(const Lattice& L, unsigned lo, unsigne
     int a = -1;
 #pragma unroll
     for (int k = 0; k < ND; ++k)
-        if (d == L.stride[k] && c[k] + 1 < L.dim[k]) a = k;
+        if (d == L.stride[k] && (k == 0 ? (z_pairs(L, c[0]) & 2u) != 0u : c[k] + 1 < L.dim[k])) a = k;
     return a;
 }
 
@@ -89,6 +90,8 @@ __global__ void __launch_bounds__(256) k_nlinks_keys(Lattice L, const int64_t* _
 // (as mgc_add_nweights_dense ignores them).  The axis arrives as scalars, so no lattice array is indexed at run time:
 // span = stride[axis] * dim[axis] (the stride of the next slower axis, or n for axis 0), span_magic its ceil(2^64 / span)
 // (0: p < span for every p, or span == 1), last = span - stride[axis].  p lies on the last plane iff p mod span >= last.
+// On a batch lattice axis 0 spans one image (zper * stride[0]), so the last plane of every image is ignored: its entries
+// would name pairs across a seam (z_pairs).  Items, decrements and the pair check all come from these heads.
 __global__ void __launch_bounds__(256) k_nlinks_dense_heads(unsigned n, unsigned span, unsigned long long span_magic,
                                                             unsigned last, const double* __restrict__ fwd,
                                                             const double* __restrict__ bwd, int* __restrict__ head,

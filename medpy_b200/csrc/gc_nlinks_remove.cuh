@@ -53,8 +53,8 @@ __device__ __forceinline__ void nlink_decrements(const NlinkItem& it, const int*
 // fold edited was claimed by it.  That weight is recomputed from the image as residual_read does (build_weight, or
 // exp_caps6 for the exponential term without spacing); |a - b| and max(|a|, |b|) are symmetric, so it is the same double
 // from either end of the pair.
-template <typename E, int FN, int USE_MAX, int SPACING>
-__device__ __forceinline__ double remove_arc_residual(const LazyResidual<E, FN, USE_MAX, SPACING>& A, const Lattice& L,
+template <typename E, int FN, int USE_MAX, int SPACING, bool BATCH>
+__device__ __forceinline__ double remove_arc_residual(const LazyResidual<E, FN, USE_MAX, SPACING, BATCH>& A, const Lattice& L,
                                                       const Tiles& TL, const int* __restrict__ cmat, unsigned lo, int axis,
                                                       bool fwd)
 {
@@ -64,7 +64,7 @@ __device__ __forceinline__ double remove_arc_residual(const LazyResidual<E, FN, 
     decode<3>(L, v, c);
     const int t = ((c[0] / TILE) * TL.nt[1] + c[1] / TILE) * TL.nt[2] + c[2] / TILE;
     if (!cmat || cmat[t]) return fwd ? nlink_pick(A.S.cap, 2 * axis + 1, 6)[v] : nlink_pick(A.S.cap, 2 * axis, 6)[v];
-    const BoundaryParams& P = A.P;
+    const BoundaryParams P = BATCH ? params_at(A.P, L, c[0]) : A.P;      // a batch: the constants of the pair's image
     const bool use_max = USE_MAX >= 0 ? (USE_MAX != 0) : (P.use_max != 0);
     const bool spacing = SPACING >= 0 ? (SPACING != 0) : (P.inv_spacing_on != 0.0);
     const double a = build_val<E>(__ldg(A.img + lo), use_max);
@@ -80,8 +80,8 @@ __device__ __forceinline__ double remove_arc_residual(const LazyResidual<E, FN, 
     return build_weight<FN, E>(P, a, q, use_max, spacing, nlink_pick(P.spacing, axis, 3));
 }
 
-template <int ND>
-__device__ __forceinline__ double remove_arc_residual(const EagerResidual<ND>& A, const Lattice& L, const Tiles&, const int*,
+template <int ND, bool BATCH>
+__device__ __forceinline__ double remove_arc_residual(const EagerResidual<ND, BATCH>& A, const Lattice& L, const Tiles&, const int*,
                                                       unsigned lo, int axis, bool fwd)
 {
     return fwd ? nlink_pick(A.S.cap, 2 * axis + 1, 2 * ND)[lo]
@@ -160,12 +160,14 @@ __device__ __forceinline__ int remove_item_of(const unsigned long long* __restri
 // f = A.read(v) (f.e = e') moves the absorbed sink flow into f.dk as every fold does, then the un-pushed source residual
 // covers min(max(r, 0), s), and the rest is a raise of both terminal links by the same amount, which keeps the cut and
 // lowers the constant by it: dk += min(max(r, 0), s) - s, r -= s, e = 0.  keys == nullptr: the dense form, whose only
-// axis is `axis`.  The change of the add_tweights constant is summed into one partial per block for fold_items' sum.
+// axis is `axis`.  The change of the add_tweights constant is summed into one partial per block for fold_items' sum and
+// on a batch handle (Access::BATCH) stored per listed endpoint in tail_dk.
 template <typename Access>
 __global__ void __launch_bounds__(256)
 k_nlinks_remove_voxels(Access A, Lattice L, const unsigned long long* __restrict__ keys, const int* __restrict__ head,
                        const int* __restrict__ pos, int ncalls, int axis, const double* __restrict__ dx,
-                       const unsigned* __restrict__ tails, const int* __restrict__ ntails, double* __restrict__ partials)
+                       const unsigned* __restrict__ tails, const int* __restrict__ ntails, double* __restrict__ partials,
+                       double* __restrict__ tail_dk)
 {
     constexpr int ND = Access::ND;
     constexpr unsigned ARCS = (1u << (2 * ND)) - 1u;
@@ -190,6 +192,7 @@ k_nlinks_remove_voxels(Access A, Lattice L, const unsigned long long* __restrict
         S.rmask[v] = (uint8_t)((S.rmask[v] & ~ARCS) | nlink_arc_bits<ND>(S, v));
         const double e = __dadd_rn(S.excess[v], de);
         if (de != 0.0) S.excess[v] = e;
+        double dk = 0.0;
         if (e < 0) {
             auto f = A.read(v);                       // f.e = e, stored above
             const double s = -f.e;
@@ -199,7 +202,9 @@ k_nlinks_remove_voxels(Access A, Lattice L, const unsigned long long* __restrict
             f.e = 0.0;
             A.write(v, f);
             m = __dadd_rn(m, f.dk);
+            dk = f.dk;
         }
+        if constexpr (Access::BATCH) tail_dk[i] = dk;
     }
     block_sum_store(m, partials);
 }

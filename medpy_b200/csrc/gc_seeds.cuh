@@ -124,7 +124,9 @@ struct Residual {
     unsigned rm;      // rmask
 };
 
-template <typename E, int FN, int USE_MAX, int SPACING>
+// BATCH: a batch lattice, whose voxels take the term constants of their own image (params_at); false compiles the
+// single-image read with P itself.
+template <typename E, int FN, int USE_MAX, int SPACING, bool BATCH>
 __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<double>& S, const E* __restrict__ img,
                                                   const BoundaryParams& P, unsigned v)
 {
@@ -133,9 +135,11 @@ __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<
     Residual f;
     int c[3];
     decode<3>(L, v, c);
-    // capacities before any flow: the doubles k_caps_tiles computed from the same image copy
+    // capacities before any flow: the doubles k_caps_tiles computed from the same image copy, with the same term
+    // constants (a batch: those of v's image)
     const unsigned valid = z_pairs(L, c[0]) | (c[1] > 0 ? 4u : 0u) | (c[1] + 1 < L.dim[1] ? 8u : 0u) |
                            (c[2] > 0 ? 16u : 0u) | (c[2] + 1 < L.dim[2] ? 32u : 0u);
+    const BoundaryParams Pv = BATCH ? params_at(P, L, c[0]) : P;
     const double a = build_val<E>(__ldg(img + v), use_max);
     if (FN == 1 && SPACING == 0) {
         double t6[6];
@@ -144,7 +148,7 @@ __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<
             t6[k] = 0.0;
             if ((valid >> k) & 1u) {
                 const double b = build_val<E>(__ldg(img + (unsigned)((int)v + dir_offset(L, k))), use_max);
-                t6[k] = exp_term_arg(P, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
+                t6[k] = exp_term_arg(Pv, use_max ? fmax(a, b) : fabs(__dsub_rn(a, b)));
             }
         }
         exp_caps6(t6, false, valid, f.co);     // the general branch: the same doubles for ordinary arguments
@@ -152,7 +156,7 @@ __device__ __forceinline__ Residual residual_read(const Lattice& L, const State<
 #pragma unroll
         for (int k = 0; k < 6; ++k)
             f.co[k] = ((valid >> k) & 1u)
-                          ? build_weight<FN, E>(P, a, __ldg(img + (unsigned)((int)v + dir_offset(L, k))), use_max, spacing,
+                          ? build_weight<FN, E>(Pv, a, __ldg(img + (unsigned)((int)v + dir_offset(L, k))), use_max, spacing,
                                                 P.spacing[k >> 1])
                           : 0.0;
     }
@@ -390,20 +394,24 @@ __device__ __forceinline__ void eager_write(const State<double>& S, uint8_t* __r
 // residual source capacity is the access type's business: a lazily built handle recomputes the pushed source flow from
 // its image (residual_read), an eager or 4-D handle recorded r(v) itself at the first solve (eager_read).  The members
 // are the fold kernels' first parameters.
-template <typename E, int FN, int USE_MAX, int SPACING>
+// BATCH: a batch handle, whose fold kernels also store each entry's change of the add_tweights constant for the
+// per-image sum (batch_fold_const); false compiles the single-handle kernels without it.
+template <typename E, int FN, int USE_MAX, int SPACING, bool BATCH_>
 struct LazyResidual {
     static constexpr int ND = 3;
+    static constexpr bool BATCH = BATCH_;
     Lattice L;
     State<double> S;
     const E* img;
     BoundaryParams P;
-    __device__ __forceinline__ Residual read(unsigned v) const { return residual_read<E, FN, USE_MAX, SPACING>(L, S, img, P, v); }
+    __device__ __forceinline__ Residual read(unsigned v) const { return residual_read<E, FN, USE_MAX, SPACING, BATCH>(L, S, img, P, v); }
     __device__ __forceinline__ void write(unsigned v, const Residual& f) const { residual_write(S, v, f); }
 };
 
-template <int ND_>
+template <int ND_, bool BATCH_ = false>
 struct EagerResidual {
     static constexpr int ND = ND_;
+    static constexpr bool BATCH = BATCH_;
     State<double> S;
     uint8_t* smask;
     __device__ __forceinline__ EagerRead read(unsigned v) const { return eager_read<ND>(S, v); }
@@ -438,11 +446,13 @@ struct ListCalls {
 };
 
 // One thread per touched voxel: r(v) read, its calls applied in order with the reference's arithmetic, r' written back;
-// the change of the add_tweights constant summed into one partial per block.  residual_write and eager_write hold for
-// any finite r and r', so any weights may come.
+// the change of the add_tweights constant summed into one partial per block, and on a batch handle (Access::BATCH),
+// whose images keep their own constants, stored per item in item_dk.  residual_write and eager_write hold for any finite r and r',
+// so any weights may come.
 template <typename Access, typename Calls>
 __global__ void __launch_bounds__(256)
-k_tlink_fold(Access A, const TweightItem* __restrict__ items, int n, Calls C, double* __restrict__ partials)
+k_tlink_fold(Access A, const TweightItem* __restrict__ items, int n, Calls C, double* __restrict__ partials,
+             double* __restrict__ item_dk)
 {
     double m = 0.0;
     const int step = (int)(gridDim.x * blockDim.x);
@@ -456,6 +466,7 @@ k_tlink_fold(Access A, const TweightItem* __restrict__ items, int n, Calls C, do
         }
         A.write(it.v, f);
         m = __dadd_rn(m, f.dk);
+        if constexpr (Access::BATCH) item_dk[i] = f.dk;
     }
     block_sum_store(m, partials);
 }

@@ -11,6 +11,15 @@ def on_device(x):
     return hasattr(x, "__cuda_array_interface__")
 
 
+def one_space(message, *args):
+    """Whether the arguments of one warm call are on the device, for native folds that take their arrays all on the host
+    or all on the device: a mix raises ``ValueError(message)``; host scalars (and None) go with either."""
+    cuda = any(on_device(x) for x in args)
+    if cuda and any(not on_device(x) and numpy.ndim(x) for x in args):
+        raise ValueError(message)
+    return cuda
+
+
 def _array(x):
     """``x`` as a torch tensor if it is a CUDA array, else as a numpy array; and numpy's kind of its dtype: "b" bool,
     "i" / "u" integer, "f" float, "c" complex, ..."""

@@ -12,6 +12,7 @@ import numbers
 
 import numpy
 
+from . import _warm_args
 from .device import _KINDS, _as_u8
 from .energy_voxel import _device_image, _native_order
 
@@ -87,11 +88,21 @@ def _prob_arg(prob, alpha):
 
 
 class BatchGraph:
-    """The graph of a batch of images (``graph_from_voxels_batch``)."""
+    """The graph of a batch of images (``graph_from_voxels_batch``).
 
-    def __init__(self, native, batch):
+    Built with ``warm=True``, it takes the warm edits of ``GraphDouble`` (``add_seeds``, ``remove_seeds``,
+    ``add_tweights_warm``, ``add_nweights_warm``, ``remove_nweights_warm`` and their dense forms), before or after a
+    ``maxflow()``: the next ``maxflow()`` re-solves the batch from its residual state and returns the B energies of the
+    edited images.  Node ids are flat C-order indices over the ``(B, ...image)`` shape, so image b's voxel p is
+    ``b * N + p`` (N voxels per image); masks and dense arrays have the batch shape.  An n-link pair never joins two
+    images: a listed pair across two images is refused like any pair of non-neighbours.  Without ``warm=True`` every
+    warm edit raises ``RuntimeError``."""
+
+    def __init__(self, native, batch, shape=None, warm=False):
         self._native = native
         self.batch = batch
+        self.shape = tuple(shape) if shape is not None else None
+        self._warm = warm
 
     def maxflow(self):
         """Solve every image; returns a float64 array of the B energies."""
@@ -105,30 +116,97 @@ class BatchGraph:
     def stats(self):
         return self._native.stats()
 
-    # Warm edits are not available on a batch: each of these raises (the native handle refuses them).
+    # The warm edits take the arguments of GraphDouble's (see there for their meaning), over the batch shape.  Without
+    # warm=True the arguments go to the native handle as given, which refuses the call.
     def add_seeds(self, fg_ids=None, bg_ids=None):
-        self._native.add_seeds(fg_ids, bg_ids)
+        """``add_tweights(v, 65535, 0)`` for every foreground id, then ``add_tweights(v, 0, 65535)`` for every
+        background id; ``fg_ids`` / ``bg_ids``: a boolean mask of the batch shape, a 1-D integer id array, or None."""
+        self._seeds("add_seeds", fg_ids, bg_ids)
 
     def remove_seeds(self, fg_ids=None, bg_ids=None):
-        self._native.remove_seeds(fg_ids, bg_ids)
+        """The inverse of ``add_seeds``: ``add_tweights(v, -65535, 0)`` / ``add_tweights(v, 0, -65535)``."""
+        self._seeds("remove_seeds", fg_ids, bg_ids)
+
+    def _seeds(self, native, fg, bg):
+        if self._warm:
+            _warm_args.one_space("fg_ids and bg_ids must both be host or both be device arrays", fg, bg)
+            fg, bg = (None if x is None else _warm_args.node_ids(x, self.shape, self._n, what)
+                      for x, what in ((fg, "fg_ids"), (bg, "bg_ids")))
+        getattr(self._native, native)(fg, bg)
 
     def add_tweights_warm(self, ids, src, snk):
+        """``add_tweights(ids[k], src[k], snk[k])`` per entry in order; ``ids`` None is the dense form, one call per
+        voxel with ``src`` / ``snk`` of the batch shape (or one entry per voxel).  Scalars broadcast."""
+        if self._warm:
+            cuda = _warm_args.one_space("ids, src and snk must all be host or all be device arrays", ids, src, snk)
+            ids = None if ids is None else _warm_args.node_ids(ids, self.shape, self._n, "ids")
+            m, dense = (self._n, self.shape) if ids is None else (ids.shape[0], None)
+            src = _warm_args.weights(src, m, "src", dense, cuda)
+            snk = _warm_args.weights(snk, m, "snk", dense, cuda)
         self._native.add_tweights_warm(ids, src, snk)
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
+        """``sum_edge(i[k], j[k], cap[k], rev_cap[k])`` per entry in order, on pairs of neighbours inside one image."""
+        if self._warm:
+            i, j, cap, rev_cap, _ = self._nlink_args(i, j, cap, rev_cap)
         self._native.add_nweights_warm(i, j, cap, rev_cap)
 
     def remove_nweights_warm(self, i, j, cap, rev_cap):
+        """``sum_edge(i[k], j[k], -cap[k], -rev_cap[k])`` per entry in order (nonnegative decrements)."""
+        if self._warm:
+            i, j, cap, rev_cap, cuda = self._nlink_args(i, j, cap, rev_cap)
+            if not cuda:        # the native grouping checks device decrements in the same pass
+                _warm_args.check_amounts(((cap, "cap"), (rev_cap, "rev_cap")), _warm_args.DECREMENTS)
         self._native.remove_nweights_warm(i, j, cap, rev_cap)
 
     def add_nweights_dense_warm(self, axis, fwd, bwd):
+        """The dense form of ``add_nweights_warm``: ``fwd`` / ``bwd`` have the batch shape and entry p holds the
+        increments of p -> p + e_axis and back.  ``axis`` counts the axes of the batch shape: axis 0, the batch axis,
+        joins no voxels and raises ``ValueError``; axis a >= 1 is the images' axis a - 1, whose last plane in every image
+        is ignored."""
+        if self._warm:
+            axis, fwd, bwd, _ = self._dense_args(axis, fwd, bwd)
         self._native.add_nweights_dense_warm(axis, fwd, bwd)
 
     def remove_nweights_dense_warm(self, axis, fwd, bwd):
+        """The dense form of ``remove_nweights_warm``, in the layout of ``add_nweights_dense_warm``."""
+        if self._warm:
+            lattice_axis, fwd, bwd, cuda = self._dense_args(axis, fwd, bwd)
+            if not cuda:        # the entries that name a pair: all but the last plane of `axis` in every image
+                cut = tuple(slice(0, s - 1) if d == int(axis) else slice(None) for d, s in enumerate(self.shape))
+                _warm_args.check_amounts(((fwd[cut], "fwd"), (bwd[cut], "bwd")), _warm_args.DECREMENTS)
+            axis = lattice_axis
         self._native.remove_nweights_dense_warm(axis, fwd, bwd)
 
+    @property
+    def _n(self):
+        return math.prod(self.shape)
 
-def graph_from_voxels_batch(fg_markers, bg_markers, image, boundary, sigma=None, spacing=False, prob=None, alpha=None):
+    def _nlink_args(self, i, j, cap, rev_cap):
+        """The list-form n-link arguments as four contiguous 1-D arrays of one length, and whether they are on the
+        device."""
+        cuda = _warm_args.one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
+        ii, jj = _warm_args.pair_ids(i, self._n, "i"), _warm_args.pair_ids(j, self._n, "j")
+        return _warm_args.nlink_calls(ii, jj, cap, rev_cap, cuda) + (cuda,)
+
+    def _dense_args(self, axis, fwd, bwd):
+        """The dense n-link arguments: the lattice axis of batch axis ``axis`` (the images' axes are the last of the
+        lattice's three), and fwd / bwd as float64 arrays of the batch shape; and whether they are on the device."""
+        axis = int(axis)
+        if axis == 0:
+            raise ValueError("axis 0 is the batch axis: no n-link joins two images")
+        if not 0 < axis < len(self.shape):
+            raise ValueError("axis {} is out of range for a batch of shape {}".format(axis, self.shape))
+        cuda = _warm_args.one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
+        fwd, bwd = _warm_args.real(fwd, "fwd"), _warm_args.real(bwd, "bwd")
+        for a, what in ((fwd, "fwd"), (bwd, "bwd")):
+            if tuple(a.shape) != self.shape:
+                raise ValueError("{} of shape {} does not match the batch shape {}".format(what, tuple(a.shape), self.shape))
+        return 3 - len(self.shape) + axis, fwd, bwd, cuda
+
+
+def graph_from_voxels_batch(fg_markers, bg_markers, image, boundary, sigma=None, spacing=False, prob=None, alpha=None,
+                            warm=False):
     """Build the graphs of B independent images in one fused build.
 
     The leading axis of every array is the batch; numpy arrays and CUDA arrays (``__cuda_array_interface__``, e.g. torch
@@ -136,6 +214,8 @@ def graph_from_voxels_batch(fg_markers, bg_markers, image, boundary, sigma=None,
     boundary : one of the eight ``energy_voxel.boundary_*`` names without the prefix (required)
     sigma : a float for every image, or one per image
     spacing, prob, alpha : as in ``graph_from_device_arrays``; shared by the whole batch
+    warm : let the graph take warm edits (``BatchGraph.add_seeds`` ...) and re-solve from its residual state, so that a
+        correction to a few images does not rebuild the batch.  Off by default, where the warm edits raise.
     """
     if boundary not in _KINDS:
         raise ValueError(f"a batch needs one of the boundary terms {sorted(_KINDS)}, got {boundary!r}")
@@ -168,6 +248,8 @@ def graph_from_voxels_batch(fg_markers, bg_markers, image, boundary, sigma=None,
 
     from .. import _lib   # raises ImportError loudly when the extension is not built
     native = _lib.Graph.batch(list(image_shape), batch, -1)
+    if warm:        # before the build: an eagerly built batch records its residual source capacities at the first solve
+        native.set_option(_lib._mgc.OPT_WARM, 1)
     native.build_voxel_batch(prob, alpha, compute_f32, _KINDS[boundary], image, sigmas, sp, norms, _markers(fg_markers),
                              _markers(bg_markers))
-    return BatchGraph(native, batch)
+    return BatchGraph(native, batch, shape, warm)

@@ -500,10 +500,7 @@ class GraphDouble:
     def _one_space(message, *args):
         """Whether the arguments of one warm call are on the device.  The native folds take their arrays all on the host or
         all on the device: a mix raises ``ValueError(message)``; host scalars go with either."""
-        cuda = any(_warm_args.on_device(x) for x in args)
-        if cuda and any(not _warm_args.on_device(x) and numpy.ndim(x) for x in args):
-            raise ValueError(message)
-        return cuda
+        return _warm_args.one_space(message, *args)
 
     def add_tweights_warm(self, nodes, cap_source, cap_sink):
         """``add_tweights`` calls on a solved graph, re-solved warm by the next ``maxflow()``: soft strokes, a GrabCut-style
