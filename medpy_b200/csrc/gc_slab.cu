@@ -239,7 +239,20 @@ int mgc_slab_relabel_begin(mgc_graph* g)
     if (!g->state_init) FAIL(MGC_E_STATE, "call mgc_slab_begin first");
     CK(cudaSetDevice(g->device));
     g->st.global_relabels++;
-    return relabel_tiles_begin(g);
+    const int rc = relabel_tiles_begin(g);
+    if (rc) return rc;
+    // a neighbour may have pushed (with a stale ghost label) into a voxel this slab had labelled HINF, which can reach the
+    // sink now: every tile with excess goes back on the push lists, the only tiles the stop test counts
+    const int ntiles = g->nd == 4 ? g->TL4.ntiles : g->TL.ntiles;
+    unsigned grid = (unsigned)g->n_ctas * 4u;
+    if (grid > (unsigned)ntiles) grid = (unsigned)ntiles;
+    if (g->nd == 4)
+        k_slab_relist4<double><<<grid, T4_VOX, 0, g->stream>>>(g->L, g->TL4, g->S, g->pflag, pl(g, 0, g->pl_sel[0]), pl(g, 1, g->pl_sel[1]));
+    else
+        k_slab_relist<double><<<grid, TILE_VOX, 0, g->stream>>>(g->L, g->TL, g->S, g->pflag, pl(g, 0, g->pl_sel[0]), pl(g, 1, g->pl_sel[1]));
+    g->st.kernel_launches++;
+    CK(cudaGetLastError());
+    return MGC_OK;
 }
 
 int mgc_slab_relabel_relax(mgc_graph* g, int32_t* changed_out)

@@ -1,5 +1,5 @@
-// gc_slab_kernels.cuh -- the z-slab border message kernels, launched only by gc_slab.cu: k_slab_pack (from
-// gc_solver.cuh) and the tile-aware unpacks (from gc_tiles.cuh / gc_tiles4.cuh).
+// gc_slab_kernels.cuh -- the z-slab kernels, launched only by gc_slab.cu: the border messages (k_slab_pack and the
+// tile-aware unpacks) and the push-list relisting at the start of every distributed global relabel.
 #pragma once
 #include "gc_tiles.cuh"
 #include "gc_tiles4.cuh"
@@ -94,5 +94,33 @@ __global__ void k_slab_unpack_tiles4(Lattice L, Tiles4 TL, State<T> S, int z_gho
         S.rmask[vb] |= (uint8_t)(1u << k_border_to_ghost);
         const int color = ((z_border >> 2) + (c1 >> 2) + (c2 >> 3) + (c3 >> 2)) & 1;
         list_push(pflag, color ? pl1 : pl0, tb);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// push lists at the start of a distributed global relabel: every tile holding an owned voxel with excess goes on the list
+// its colour consumes next.  On one lattice a voxel the last relabel left at HINF never gets a finite label again, so its
+// tile may leave the lists.  On a slab it can: a neighbour pushes into it across the border with a stale ghost label,
+// and the reverse residual arc connects it to the sink at the next relabel.  The stop test counts only listed tiles.
+// ---------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(TILE_VOX) k_slab_relist(Lattice L, Tiles TL, State<T> S, int* __restrict__ pflag,
+                                                          WorkList pl0, WorkList pl1)
+{
+    for (int t = blockIdx.x; t < TL.ntiles; t += gridDim.x) {
+        const TileCtx c = tile_ctx(L, TL, t);
+        const int act = (c.own && S.excess[c.v] > 0) ? 1 : 0;
+        if (__syncthreads_or(act) && threadIdx.x == 0) list_push(pflag, tile_color(c) ? pl1 : pl0, t);
+    }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(T4_VOX) k_slab_relist4(Lattice L, Tiles4 TL, State<T> S, int* __restrict__ pflag,
+                                                         WorkList pl0, WorkList pl1)
+{
+    for (int t = blockIdx.x; t < TL.ntiles; t += gridDim.x) {
+        const Tile4Ctx c = tile4_ctx(L, TL, t);
+        const int act = (c.own && S.excess[c.v] > 0) ? 1 : 0;
+        if (__syncthreads_or(act) && threadIdx.x == 0) list_push(pflag, tile4_color(c) ? pl1 : pl0, t);
     }
 }

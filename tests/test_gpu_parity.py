@@ -14,7 +14,6 @@ import numpy
 import pytest
 
 from conftest import golden
-from test_gpu_push_window import _env
 
 pytestmark = pytest.mark.gpu
 
@@ -406,105 +405,8 @@ def test_device_resident_inputs_via_cuda_array_interface():
 
 
 # ------------------------------------------------------------------------------------------------------
-# z-slab path
+# z-slab path over NCCL (the N-slab runs on one GPU are in test_gpu_slabs.py)
 # ------------------------------------------------------------------------------------------------------
-def _two_slabs_one_gpu(vol, regional, split):
-    """Drive two slab handles that live on the SAME GPU through the mgc_slab_* protocol, moving the border messages
-    with plain device copies: exercises ghost planes, pack/unpack, the distributed relabel and the stop test
-    without needing two devices."""
-    import torch
-    from medpy_b200 import _lib
-    shape = vol["image"].shape
-    Z = shape[0]
-    bounds = [(0, split), (split, Z)]
-    hs = [_lib.Graph(list(shape), a, b, 0) for a, b in bounds]
-    P = hs[0].slab_plane_elems()
-    for (a, b), h in zip(bounds, hs):
-        lo = a - (1 if a > 0 else 0)
-        hi = b + (1 if b < Z else 0)
-        if regional:
-            h.add_regional_probability(numpy.ascontiguousarray(vol["prob"][lo:hi]), vol["alpha"], True)
-        h.add_boundary(1, numpy.ascontiguousarray(vol["image"][lo:hi]), vol["sigma"], None, float("nan"))
-        h.add_markers(numpy.ascontiguousarray(vol["fg"][lo:hi]), numpy.ascontiguousarray(vol["bg"][lo:hi]))
-        h.slab_begin()
-    mk = lambda dt: torch.zeros(P, dtype=dt, device="cuda")
-    # message buffers: rank 0's upper side <-> rank 1's lower side
-    s0h, s0f, s1h, s1f = mk(torch.int32), mk(torch.float64), mk(torch.int32), mk(torch.float64)
-    flag = torch.zeros(1, dtype=torch.int32, device="cuda")
-
-    def exchange():
-        flag.zero_()
-        torch.cuda.synchronize()
-        hs[0].slab_pack(0, 0, s0h.data_ptr(), s0f.data_ptr())
-        hs[1].slab_pack(s1h.data_ptr(), s1f.data_ptr(), 0, 0)
-        for h in hs:
-            h.synchronize()
-        hs[0].slab_unpack(0, 0, s1h.data_ptr(), s1f.data_ptr(), flag.data_ptr())
-        hs[1].slab_unpack(s0h.data_ptr(), s0f.data_ptr(), 0, 0, flag.data_ptr())
-        for h in hs:
-            h.synchronize()
-        return int(flag.item())
-
-    passes, rounds = 1, 0
-    while True:
-        for h in hs:
-            h.slab_relabel_begin()
-        while True:
-            for h in hs:
-                h.slab_relabel_relax(False)
-            if not exchange():
-                break
-        if sum(h.slab_count_active() for h in hs) == 0:
-            break
-        rounds += 1
-        assert rounds < 1000
-        for _ in range(passes):
-            for h in hs:
-                h.slab_push(1)
-            exchange()
-        passes = min(8, passes * 2)
-    energy = sum(h.slab_finish() for h in hs)
-    mask = numpy.concatenate([h.get_mask() for h in hs], axis=0)
-    return energy, mask
-
-
-# 4-D slabs (4 x 4 x 8 x 4 tiles with ghost planes): ragged, one-plane and even splits, and a split that leaves both
-# slabs at least 64 tiles (72 and 96), so that their relabels can run directional sweeps
-SLABS4 = [((20, 12, 16, 9), 7, True), ((17, 10, 8, 33), 1, False), ((16, 8, 8, 4), 8, True), ((24, 16, 16, 12), 11, False)]
-
-# tile-solver options that change how a slab is relabelled or how long a tile visit runs; create_impl reads them
-SLAB4_OPTIONS = {
-    "hard": dict(MEDPY_GC_SWEEP_FRAC=1000000),      # directional sweeps in front of every relabel
-    "sweep_off": dict(MEDPY_GC_SWEEP=0),
-    "iters1": dict(MEDPY_GC_ITERS=1),
-}
-
-
-def _two_slabs_vs_oracle(shape, split, regional):
-    from medpy_b200 import synthetic
-    from oracle import energy_terms as et
-    vol = synthetic.two_blob_volume(shape, seed=4)
-    energy, mask = _two_slabs_one_gpu(vol, regional, split)
-    prob = et.build_problem(vol["fg"], vol["bg"], regional=(vol["prob"], vol["alpha"]) if regional else None,
-                            boundary=("difference_exponential", vol["image"], vol["sigma"], False))
-    oflow, omask, _ = _oracle_solve(prob)
-    assert numpy.array_equal(mask, omask)
-    assert abs(energy - oflow) <= 1e-9 * abs(oflow)
-
-
-@pytest.mark.parametrize("shape,split,regional", [((40, 32, 32), 20, True), ((40, 32, 32), 13, False), ((37, 24, 40), 9, True)]
-                         + SLABS4)
-def test_two_slabs_on_one_gpu_vs_oracle(shape, split, regional):
-    _two_slabs_vs_oracle(shape, split, regional)
-
-
-@pytest.mark.parametrize("opt", list(SLAB4_OPTIONS))
-@pytest.mark.parametrize("shape,split,regional", SLABS4)
-def test_two_4d_slabs_on_one_gpu_under_solver_options(shape, split, regional, opt):
-    with _env(**SLAB4_OPTIONS[opt]):
-        _two_slabs_vs_oracle(shape, split, regional)
-
-
 @pytest.mark.parametrize("case", ["regional", "boundary"])
 def test_multi_gpu_nccl_slabs_vs_oracle(tmp_path, case):
     """All visible GPUs (>= 2) solve one 48x40x40 volume together over NCCL; result must equal the oracle's."""
