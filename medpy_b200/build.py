@@ -55,8 +55,9 @@ def _includes(path, seen=None):
 
 def build_lib(force=False, verbose=False):
     """One object per translation unit (rebuilt only when the unit or a header it includes changed), linked into one
-    shared library: the lattice C ABI (gc_api.cu, gc_build_api.cu, gc_solve.cu, gc_fold.cu, gc_slab.cu; gc_handle.cuh)
-    and gc_sparse_api.cu (sparse graphs + label images).  The units compile concurrently, one nvcc process each."""
+    shared library: the lattice C ABI (gc_api.cu, gc_build_api.cu, gc_solve.cu, gc_fold.cu, gc_slab.cu, gc_batch.cu;
+    gc_handle.cuh), gc_sparse_api.cu (sparse graphs) and gc_labels_api.cu (label images).  Every .cu file in csrc/ is a
+    unit; they compile concurrently, one nvcc process each."""
     units = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith(".cu")]
     objdir = os.path.join(LIBDIR, "obj")
     os.makedirs(objdir, exist_ok=True)

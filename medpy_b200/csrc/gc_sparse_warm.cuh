@@ -226,13 +226,6 @@ __global__ void __launch_bounds__(256) k_spw_sum_partials(const double* __restri
     if (threadIdx.x == 0) out[0] = sh[0];
 }
 
-// (key, call index) pairs of the calls; the stable sort groups them by key
-__global__ void __launch_bounds__(256) k_spw_iota(unsigned* __restrict__ a, long long m)
-{
-    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-    if (i < m) a[i] = (unsigned)i;
-}
-
 __device__ __forceinline__ bool spw_is_head(const unsigned* keys, long long i, long long m)
 {
     return i < m && keys[i] != 0xffffffffu && (i == 0 || keys[i - 1] != keys[i]);

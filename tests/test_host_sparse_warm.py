@@ -130,14 +130,15 @@ def emu(tmp_path_factory):
     lib = ctypes.CDLL(so)
     ip, dp = ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_double)
     lib.emu_warm_create.restype = ctypes.c_void_p
-    lib.emu_warm_create.argtypes = [ctypes.c_int, ctypes.c_longlong, ip, ip, dp, dp, dp, ctypes.c_double]
+    lib.emu_warm_create.argtypes = [ctypes.c_int]
     lib.emu_warm_destroy.argtypes = [ctypes.c_void_p]
     lib.emu_warm_solve.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_uint8), dp]
-    for f in (lib.emu_warm_tweights,):
-        f.argtypes = [ctypes.c_void_p, ctypes.c_longlong, ip, dp, dp]
+    lib.emu_warm_tweights.argtypes = [ctypes.c_void_p, ctypes.c_longlong, ip, dp, dp]
     for f in (lib.emu_warm_edges, lib.emu_warm_remove):
         f.argtypes = [ctypes.c_void_p, ctypes.c_longlong, ip, ip, dp, dp]
     lib.emu_warm_remove.restype = ctypes.c_int
+    lib.emu_warm_host.restype = ctypes.c_longlong
+    lib.emu_warm_host.argtypes = [ctypes.c_void_p, ip, ip, dp, dp, dp, dp]
     return lib
 
 
@@ -146,10 +147,20 @@ class _Emu:
 
     def __init__(self, lib, n, edges, tw, steps=4, sweeps=16):
         self.lib, self.n, self.steps, self.sweeps = lib, n, steps, sweeps
-        lo, hi, c_lh, c_hl = elt.merge_edges(*edges)
-        tr, const = elt.add_tweights_replay(n, tw)
-        self._keep = [numpy.ascontiguousarray(x) for x in (lo.astype(numpy.int32), hi.astype(numpy.int32), c_lh, c_hl, tr)]
-        self.h = lib.emu_warm_create(n, lo.size, *[self._p(x) for x in self._keep], const)
+        self.h = lib.emu_warm_create(n)
+        self.edges(*edges)
+        for op in tw:
+            self.tweights(*op)
+        # the C ABI's host state of the raw calls against the oracle's replay of them
+        np_ = lib.emu_warm_host(self.h, None, None, None, None, None, None)
+        lo, hi = numpy.zeros(np_, numpy.int32), numpy.zeros(np_, numpy.int32)
+        c_lh, c_hl, tr, const = numpy.zeros(np_), numpy.zeros(np_), numpy.zeros(n), numpy.zeros(1)
+        lib.emu_warm_host(self.h, *[self._p(x) for x in (lo, hi, c_lh, c_hl, tr, const)])
+        order = numpy.lexsort((hi, lo))
+        for got, want in zip((lo, hi, c_lh, c_hl), elt.merge_edges(*edges)):
+            assert numpy.array_equal(got[order], want)
+        want_tr, want_const = elt.add_tweights_replay(n, tw)
+        assert numpy.array_equal(tr, want_tr) and const[0] == want_const
 
     @staticmethod
     def _p(a):

@@ -1,6 +1,7 @@
-"""Logic check of the sparse push-relabel without a GPU: the per-node functions of medpy_b200/csrc/gc_sparse.cuh are
-compiled as host C++ (tests/emu/sparse_emu.cpp) and compared with the real reference BK (oracle/_ref) on random sparse
-graphs and on the golden region adjacency graphs.  The CUDA kernels wrap exactly these functions."""
+"""Logic check of the sparse push-relabel without a GPU: the C ABI's host state (medpy_b200/csrc/gc_sparse_host.hpp)
+and the per-node functions of medpy_b200/csrc/gc_sparse.cuh are compiled as host C++ (tests/emu/sparse_emu.cpp) and
+compared with the label-term oracle and the real reference BK (oracle/_ref) on random sparse graphs and on the golden
+region adjacency graphs.  gc_sparse_api.cu runs the same host code, and the CUDA kernels wrap exactly these functions."""
 import ctypes
 import os
 import subprocess
@@ -15,51 +16,41 @@ from oracle import energy_label_terms as elt  # noqa: E402
 from oracle import solvers  # noqa: E402
 
 
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
     so = str(tmp_path_factory.mktemp("emu") / "libsparse_emu.so")
     subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-x", "c++", "-o", so,
                            os.path.join(HERE, "emu", "sparse_emu.cpp")])
     lib = ctypes.CDLL(so)
-    lib.emu_sparse_solve.restype = ctypes.c_int
+    ip, dp, ll = ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_double), ctypes.c_longlong
+    lib.emu_sparse_calls.restype = ll
+    lib.emu_sparse_calls.argtypes = ([ctypes.c_int, ll, ip, ip, dp, dp, ll, ip, dp, dp, ctypes.c_int, ctypes.c_int, ip, ip]
+                                     + [dp] * 4 + [ctypes.POINTER(ctypes.c_uint8), dp])
     return lib
 
 
-def csr(n, lo, hi, c_lh, c_hl):
-    """Same layout as sparse_solve() in gc_sparse_api.cu: arcs in pair insertion order."""
-    row = numpy.zeros(n + 1, dtype=numpy.int32)
-    numpy.add.at(row, lo + 1, 1)
-    numpy.add.at(row, hi + 1, 1)
-    row = numpy.cumsum(row).astype(numpy.int32)
-    fill = row[:-1].copy()
-    m2 = 2 * lo.size
-    head = numpy.zeros(m2, numpy.int32)
-    sis = numpy.zeros(m2, numpy.int32)
-    cap = numpy.zeros(m2)
-    for p in range(lo.size):
-        a = fill[lo[p]]; fill[lo[p]] += 1
-        b = fill[hi[p]]; fill[hi[p]] += 1
-        head[a], head[b] = hi[p], lo[p]
-        sis[a], sis[b] = b, a
-        cap[a], cap[b] = c_lh[p], c_hl[p]
-    return row, head, sis, cap
+def _p(a):
+    return a.ctypes.data_as(ctypes.POINTER({numpy.int32: ctypes.c_int, numpy.uint8: ctypes.c_uint8}.get(a.dtype.type, ctypes.c_double)))
 
 
 def run_emu(lib, n, i, j, cap, rev, tw_ops, steps=4, sweeps=16):
-    lo, hi, c_lh, c_hl = elt.merge_edges(i, j, cap, rev)
-    tr, const = elt.add_tweights_replay(n, tw_ops)
-    row, head, sis, c = csr(n, lo.astype(numpy.int64), hi.astype(numpy.int64), c_lh, c_hl)
-    mask = numpy.zeros(n, numpy.uint8)
-    absorbed = ctypes.c_double(0)
-    rounds = ctypes.c_longlong(0)
-    ip = ctypes.POINTER(ctypes.c_int)
-    dp = ctypes.POINTER(ctypes.c_double)
-    rc = lib.emu_sparse_solve(n, int(c.size), row.ctypes.data_as(ip), head.ctypes.data_as(ip), sis.ctypes.data_as(ip),
-                              c.ctypes.data_as(dp), tr.ctypes.data_as(dp), steps, sweeps,
-                              mask.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), ctypes.byref(absorbed), ctypes.byref(rounds))
-    assert rc == 0
-    return const + absorbed.value, mask
+    """The raw calls through the C ABI's host state, whose merged pairs, tr and constant must equal the oracle's, and
+    the solve of the CSR it lays out."""
+    calls = [numpy.ascontiguousarray(a, dtype=t) for a, t in zip((i, j, cap, rev), (numpy.int32, numpy.int32, float, float))]
+    tws = [numpy.ascontiguousarray(numpy.concatenate([numpy.asarray(op[k]) for op in tw_ops]), dtype=t)
+           for k, t in enumerate((numpy.int32, float, float))]
+    m = calls[0].size
+    lo, hi, mask = numpy.zeros(m, numpy.int32), numpy.zeros(m, numpy.int32), numpy.zeros(n, numpy.uint8)
+    c_lh, c_hl, tr, const, energy = (numpy.zeros(s) for s in (m, m, n, 1, 1))
+    np_ = lib.emu_sparse_calls(n, m, *map(_p, calls), tws[0].size, *map(_p, tws), steps, sweeps,
+                               *map(_p, (lo, hi, c_lh, c_hl, tr, const, mask, energy)))
+    assert np_ >= 0
+    order = numpy.lexsort((hi[:np_], lo[:np_]))                  # insertion order -> the oracle's (lo, hi) order
+    for got, want in zip((lo, hi, c_lh, c_hl), elt.merge_edges(i, j, cap, rev)):
+        assert numpy.array_equal(got[:np_][order], want)
+    want_tr, want_const = elt.add_tweights_replay(n, tw_ops)
+    assert numpy.array_equal(tr, want_tr) and const[0] == want_const
+    return energy[0], mask
 
 
 def random_graph(rng, n, m, integer):
