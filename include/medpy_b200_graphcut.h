@@ -281,8 +281,8 @@ int mgc_maxflow(mgc_graph* g, double* energy);
  * fold recomputes capacities from the copies that build keeps.  Elsewhere reset() and a rebuild with the seeds is the way.
  * mgc_add_tweights_dense / mgc_add_markers and the other term entry points still refuse a solved graph.  Adding this
  * entry point left MGC_ABI_VERSION at 3: nothing that existed changed.
- * MGC_OPT_WARM = 1 (mgc_set_option) extends these folds to every other tile-solver handle of one GPU: 4-D lattices,
- * 1-D..3-D graphs built term by term, and the eager fused build (lazy capacities off).  Such a handle keeps no copy of its
+ * MGC_OPT_WARM = 1 (mgc_set_option) extends these folds to every other tile-solver handle: 4-D lattices, 1-D..3-D graphs
+ * built term by term, the eager fused build (lazy capacities off), and z-slab handles.  Such a handle keeps no copy of its
  * inputs, so its first solve records the residual source capacity of every voxel in place of the net t-link, before the
  * first push (a pass over tr and the capacities after the eager fused build; nothing extra on the per-term path).
  *   - Set it before the first solve: while no flow has started (a handle fresh from create / mgc_reset / a build).  Later
@@ -290,7 +290,16 @@ int mgc_maxflow(mgc_graph* g, double* energy);
  *   - It persists across mgc_reset, like MGC_OPT_DEFER_WEIGHT_CHECK, and changes neither results nor the first solve's
  *     mask and energy.
  *   - A fold on such a handle before its first solve initialises the solver state and takes the record first.
- *   - z-slab handles still return MGC_E_STATE with the option set.
+ *   - z-slab handles (mgc_create_slab): set the option before the first mgc_slab_begin / mgc_slab_solve; the first one
+ *     takes the record, and the next mgc_slab_solve (or the stepped sequence) re-solves from the state the folds left.
+ *     Node ids are the slab's local lattice ids (owned planes plus ghost planes, C order, as mgc_get_edge /
+ *     mgc_what_segment / mgc_get_trcap take them), and the dense forms take the arrays the slab's cold
+ *     mgc_add_tweights_dense / mgc_add_nweights_dense take, ghost planes included.  Each slab applies only what it owns:
+ *     a t-link call on a ghost voxel is skipped (the neighbour owns it), and an n-link call on (u, v) adds cap to
+ *     r(u->v) only if u is owned and rev_cap to r(v->u) only if v is owned, so an axis-0 pair across a border is applied
+ *     half on each slab with no communication, and a pair inside a ghost plane is skipped.  Range, neighbour, finiteness
+ *     and sign checks run over every entry, skipped ones included.  Each slab adds the constant change of its owned
+ *     voxels to its own share of the energy, so the all-reduced total is the energy of the edited global graph.
  * MGC_ABI_VERSION stays 3 and mgc_stats keeps its layout. */
 int mgc_add_seeds(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const int64_t* bg_ids, int64_t n_bg, int32_t mem);
 /* Seeds erased from a graph and solved warm: the inverse call of mgc_add_seeds, as the reference erases a seed
@@ -358,7 +367,9 @@ int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd
  * decrement, or bad counts and pointers; MGC_E_WEIGHT for a negative decrement or a pair whose decrement exceeds its
  * residual sum.  Every check finishes before anything is written, and the handle is left unchanged when one fails (an
  * MGC_OPT_WARM handle that was never solved may have run the init its first solve would run).  Same preconditions,
- * memory spaces, statistics and MGC_E_STATE message as mgc_add_nweights_warm; z-slab handles and sparse graphs refuse.
+ * memory spaces, statistics and MGC_E_STATE message as mgc_add_nweights_warm; sparse graphs refuse.  z-slab handles return
+ * MGC_E_STATE for every call, whatever the pairs: a decrement of a pair across a border needs the neighbour's residual, and
+ * a refusal on every slab alike would need a two-phase collective, so the answer does not depend on the partition.
  * Adding this entry point left MGC_ABI_VERSION at 3. */
 int mgc_remove_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
                              int64_t count, int32_t mem);

@@ -63,6 +63,34 @@ void residual_dispatch(const mgc_graph* g, bool eager, F&& f)
     });
 }
 
+// f(std::bool_constant<SLAB>{}, own): the grouping and n-link kernels of a z-slab handle (SLAB = true) take its owned
+// voxels and drop what lies in its ghost planes (SlabOwn, gc_seeds.cuh); every other handle keeps the kernels without
+// the test
+template <typename F>
+void slab_dispatch(const mgc_graph* g, F&& f)
+{
+    if (g->slab) f(std::true_type{}, SlabOwn{(unsigned)g->L.own0 * g->L.plane, (unsigned)g->L.own1 * g->L.plane, g->L.plane});
+    else         f(std::false_type{}, SlabOwn{});
+}
+
+// MEDPY_GC_DEBUG=1 on a z-slab handle: after a fold the ghost planes' excess -- the outbox of flow pushed towards the
+// neighbour, emptied by every exchange -- is still zero, so the next exchange sends nothing the fold made up
+int slab_outbox_check(mgc_graph* g)
+{
+    if (!g->slab || !g->debug_checks) return MGC_OK;
+    const size_t P = g->L.plane;
+    std::vector<double> box(P);
+    for (int side = 0; side < 2; ++side) {
+        if (!(side == 0 ? g->ghost_lo : g->ghost_hi)) continue;
+        const size_t ghost = side == 0 ? (size_t)(g->L.own0 - 1) * P : (size_t)g->L.own1 * P;
+        CK(cudaMemcpyAsync(box.data(), g->S.excess + ghost, P * sizeof(double), cudaMemcpyDeviceToHost, g->stream));
+        CK(cudaStreamSynchronize(g->stream));
+        for (double x : box)
+            if (x != 0.0) FAIL(MGC_E_CUDA, "debug check: a fold left flow in a ghost plane's excess (the z-slab's outbox)");
+    }
+    return MGC_OK;
+}
+
 }  // namespace
 
 // ---- folds into the residual state (mgc_add_seeds / mgc_remove_seeds / mgc_add_tweights_warm / mgc_add_nweights*_warm /
@@ -156,13 +184,17 @@ static cudaError_t tails_sort(void* tmp, size_t* bytes, const unsigned* tails, u
 }
 
 // preconditions of every fold into the residual state: the copies of the lazy fused build are what the fold reads, or
-// (MGC_OPT_WARM, *eager = true) the residual source capacities the first solve records in tr on any other tile-solver handle
+// (MGC_OPT_WARM, *eager = true) the residual source capacities the first solve records in tr on any other tile-solver
+// handle, z-slabs included
 static int warm_check(mgc_graph* g, bool* eager)
 {
     *eager = false;
     if (g->batch && !batch_warm(g)) return batch_refused(g);
     if (!g->slab && g->lazy_built && g->state_init && g->nd == 3) return MGC_OK;
     if (warm_wanted(g)) { *eager = true; return MGC_OK; }
+    if (g->slab)
+        FAIL(MGC_E_STATE, "a warm re-solve of a z-slab handle needs MGC_OPT_WARM set before its first solve; reset() it and "
+                          "rebuild the graph with the edits instead");
     FAIL(MGC_E_STATE, "a warm re-solve needs a lazily built 3-D handle (mgc_build_voxel_graph on a 1-D..3-D lattice with a "
                       "boundary term, tile solver, lazy capacities); on this handle reset() it and rebuild the graph with "
                       "the seeds instead");
@@ -228,7 +260,8 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     sum_partials(g, g->partials, grid, g->d_scalars);
     // 3. solver state for the next solve: fresh push lists over every materialised tile with excess (every tile of an
     // eager handle; TL.ntiles is the 4-D tile count on a 4-D handle); labels from a full relabel reset (sweep_mode = -1: a
-    // fold can remove a sink link, so the last solve's labels bound nothing)
+    // fold can remove a sink link, so the last solve's labels bound nothing).  On a z-slab only owned excess lists a tile:
+    // the ghost planes' excess is the outbox, and the fold wrote none of it.
     CK(cudaMemsetAsync(g->d_tcount, 0, 256, g->stream));
     CK(cudaMemsetAsync(g->pflag, 0, (size_t)g->TL.ntiles * sizeof(int), g->stream));
     g->pl_sel[0] = g->pl_sel[1] = 0;
@@ -256,7 +289,7 @@ static int fold_items(mgc_graph* g, int* d_ctl, int* tiles, const std::function<
     g->solved = false;
     g->host_mask_valid = false;
     g->st.seed_folds++;
-    return MGC_OK;
+    return slab_outbox_check(g);
 }
 
 // One fold call as its entry point describes it to fold_run: the argument checks, the inputs, and how the grouping keys
@@ -481,7 +514,9 @@ static int seeds_fold(mgc_graph* g, const int64_t* fg_ids, int64_t n_fg, const i
             k_seed_keys<<<kgrid, 256, 0, g->stream>>>((const int64_t*)b.in[0], (int)n_fg, (const int64_t*)b.in[1], (int)n_bg,
                                                       (int64_t)g->L.n, b.keys, b.ctl + 1);
             CK(sort());
-            k_seed_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, (int)(n_fg + n_bg), b.head);
+            slab_dispatch(g, [&](auto slab, SlabOwn own) {
+                k_seed_heads<decltype(slab)::value><<<kgrid, 256, 0, g->stream>>>(b.skeys, (int)(n_fg + n_bg), b.head, own);
+            });
             return MGC_OK;
         },
         [&](const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni) {
@@ -521,13 +556,19 @@ int mgc_add_tweights_warm(mgc_graph* g, const int64_t* ids, const double* src, c
             const double* d_src = (const double*)b.in[1];
             const double* d_snk = (const double*)b.in[2];
             if (dense) {
-                k_tweights_dense_heads<<<kgrid, 256, 0, g->stream>>>(d_src, d_snk, (int)count, b.head, b.ctl + 1);
+                slab_dispatch(g, [&](auto slab, SlabOwn own) {
+                    k_tweights_dense_heads<decltype(slab)::value><<<kgrid, 256, 0, g->stream>>>(d_src, d_snk, (int)count,
+                                                                                              b.head, b.ctl + 1, own);
+                });
                 return MGC_OK;
             }
             k_tweights_keys<<<kgrid, 256, 0, g->stream>>>((const int64_t*)b.in[0], d_src, d_snk, (int)count, (int64_t)g->L.n,
                                                           b.keys, b.vals, b.ctl + 1);
             CK(sort());
-            k_weighted_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_src, d_snk, (int)count, b.head);
+            slab_dispatch(g, [&](auto slab, SlabOwn own) {
+                k_weighted_heads<unsigned, decltype(slab)::value><<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_src, d_snk,
+                                                                                              (int)count, b.head, own);
+            });
             return MGC_OK;
         },
         [&](const FoldBufs<unsigned, TweightItem>& b, bool eager, unsigned grid, int ni) {
@@ -559,8 +600,11 @@ static int nweights_group(mgc_graph* g, const FoldCall& c, const NlinkBufs& b, u
             span = (unsigned)g->L.zper * g->L.stride[0];
             magic = span <= 1 ? 0ull : (~0ull / span) + 1ull;
         }
-        k_nlinks_dense_heads<<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic, span - g->L.stride[axis], d_cap, d_rev,
-                                                           b.head, b.ctl + 1);
+        slab_dispatch(g, [&](auto slab, SlabOwn own) {
+            k_nlinks_dense_heads<decltype(slab)::value><<<kgrid, 256, 0, g->stream>>>(g->L.n, span, magic,
+                                                                                    span - g->L.stride[axis], d_cap, d_rev,
+                                                                                    b.head, b.ctl + 1, own);
+        });
         return MGC_OK;
     }
     const int64_t* d_i = (const int64_t*)b.in[0];
@@ -568,7 +612,10 @@ static int nweights_group(mgc_graph* g, const FoldCall& c, const NlinkBufs& b, u
     if (g->nd == 4) k_nlinks_keys<4><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
     else            k_nlinks_keys<3><<<kgrid, 256, 0, g->stream>>>(g->L, d_i, d_j, d_cap, d_rev, n, b.keys, b.vals, b.ctl + 1);
     CK(sort());
-    k_weighted_heads<<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_cap, d_rev, n, b.head);
+    slab_dispatch(g, [&](auto slab, SlabOwn own) {
+        k_weighted_heads<unsigned long long, decltype(slab)::value><<<kgrid, 256, 0, g->stream>>>(b.skeys, b.svals, d_cap,
+                                                                                                d_rev, n, b.head, own);
+    });
     return MGC_OK;
 }
 
@@ -587,8 +634,11 @@ static int nweights_fold(mgc_graph* g, FoldCall& c, int axis)
             const double* d_cap = (const double*)b.in[2];
             const double* d_rev = (const double*)b.in[3];
             int* ntails = b.ctl + 3;
-            if (g->nd == 4) k_nlinks_fold<4><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.tbits, b.tails, ntails);
-            else            k_nlinks_fold<3><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.tbits, b.tails, ntails);
+            slab_dispatch(g, [&](auto slab, SlabOwn own) {
+                constexpr bool S = decltype(slab)::value;
+                if (g->nd == 4) k_nlinks_fold<4, S><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.tbits, b.tails, ntails, own);
+                else            k_nlinks_fold<3, S><<<grid, 256, 0, g->stream>>>(g->L, g->S, b.items, ni, order, ids, d_cap, d_rev, b.tbits, b.tails, ntails, own);
+            });
             g->st.kernel_launches++;
             residual_dispatch(g, eager, [&](auto A) {
                 k_nlinks_reclamp<<<grid, 256, 0, g->stream>>>(A, b.tails, ntails, g->partials);
@@ -709,9 +759,21 @@ int mgc_add_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd
     return nweights_fold(g, c, axis + g->shift);
 }
 
+// n-link decrements on a z-slab handle: refused whatever the pairs.  A decrement of a pair across a slab border needs the
+// residual of the arc the neighbour owns, and the pair check's verdict is known on the owning slab only, so refusing a bad
+// call on every slab alike would take a two-phase collective.  Refusing them all keeps the answer the same however the
+// volume is partitioned.
+static int slab_decrement_refused(mgc_graph* g)
+{
+    if (!g || !g->slab) return MGC_OK;
+    FAIL(MGC_E_STATE, "n-link decrements are not available on z-slab handles (a pair across a slab border needs the "
+                      "neighbour's residual); reset() the slabs and rebuild the graph without the weight instead");
+}
+
 int mgc_remove_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, const double* cap, const double* rev_cap,
                              int64_t count, int32_t mem)
 {
+    if (int rc = slab_decrement_refused(g)) return rc;
     FoldCall c{};
     nweights_list_call(c, "mgc:remove_nweights_warm", i, j, cap, rev_cap, count, mem);
     return nweights_remove_fold(g, c, 0);
@@ -719,6 +781,7 @@ int mgc_remove_nweights_warm(mgc_graph* g, const int64_t* i, const int64_t* j, c
 
 int mgc_remove_nweights_dense_warm(mgc_graph* g, int32_t axis, const mgc_array* fwd, const mgc_array* bwd)
 {
+    if (int rc = slab_decrement_refused(g)) return rc;
     FoldCall c{};
     int rc = nweights_dense_call(g, c, "mgc:remove_nweights_dense_warm", axis, fwd, bwd);
     if (rc) return rc;

@@ -98,9 +98,9 @@ struct mgc_graph {
     // mgc_add_tweights_warm may fold t-link calls into the residual state.  Unlike caps_lazy this stays true once every
     // tile is materialised (hard instances).
     bool lazy_built = false;
-    // MGC_OPT_WARM: the other tile-solver handles (eager fused build, per-term path, 4-D lattices) record their residual
-    // source capacities in tr at the first solve, which lets the same folds work on them (gc_seeds.cuh).  Kept across
-    // mgc_reset, like defer_check.
+    // MGC_OPT_WARM: the other tile-solver handles (eager fused build, per-term path, 4-D lattices, z-slabs) record their
+    // residual source capacities in tr at the first solve, which lets the same folds work on them (gc_seeds.cuh).  Kept
+    // across mgc_reset, like defer_check.
     bool warm_opt = false;
     bool warm_state = false;           // tr holds BK's residual source capacity: recorded since the last init
     int* cmat = nullptr;              // per tile: push state materialised since the last lazy build
@@ -289,8 +289,9 @@ inline WorkList rl(mgc_graph* g, int i) { return WorkList{g->rl_items[i], g->d_t
 inline WorkList pl(mgc_graph* g, int color, int buf) { return WorkList{g->pl_items[color][buf], g->d_tcount + 2 + color * 2 + buf}; }
 inline int* cursor(mgc_graph* g) { return g->d_tcount + 8; }
 
-// MGC_OPT_WARM applies: a tile-solver handle of one GPU whose state does not come from the lazy fused build
-inline bool warm_wanted(const mgc_graph* g) { return g->warm_opt && !g->slab && !g->lazy_built; }
+// MGC_OPT_WARM applies: a tile-solver handle whose state does not come from the lazy fused build (z-slabs included: they
+// build eagerly, and their folds apply only what the slab owns, DESIGN.md §4.6)
+inline bool warm_wanted(const mgc_graph* g) { return g->warm_opt && !g->lazy_built; }
 
 // term kernels are not synchronised one by one: their span on the stream is measured between the first term after a
 // reset and the last term before the solve, and read when the solve synchronises anyway

@@ -92,10 +92,13 @@ __global__ void __launch_bounds__(256) k_nlinks_keys(Lattice L, const int64_t* _
 // (0: p < span for every p, or span == 1), last = span - stride[axis].  p lies on the last plane iff p mod span >= last.
 // On a batch lattice axis 0 spans one image (zper * stride[0]), so the last plane of every image is ignored: its entries
 // would name pairs across a seam (z_pairs).  Items, decrements and the pair check all come from these heads.
+// SLAB: only an increment of an arc whose tail the slab owns counts (fwd: p owned, bwd: p + stride[axis] = p + span - last
+// owned), so a pair inside a ghost plane, or one whose owned direction is zero, is no item; every entry is checked.
+template <bool SLAB = false>
 __global__ void __launch_bounds__(256) k_nlinks_dense_heads(unsigned n, unsigned span, unsigned long long span_magic,
                                                             unsigned last, const double* __restrict__ fwd,
                                                             const double* __restrict__ bwd, int* __restrict__ head,
-                                                            int* __restrict__ err)
+                                                            int* __restrict__ err, SlabOwn own = {})
 {
     for (unsigned p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
         const unsigned q = span_magic ? (unsigned)__umul64hi((unsigned long long)p, span_magic) : 0u;
@@ -104,7 +107,8 @@ __global__ void __launch_bounds__(256) k_nlinks_dense_heads(unsigned n, unsigned
             const double f = fwd[p], b = bwd[p];
             if (!isfinite(f) || !isfinite(b)) atomicOr(err, FOLD_ERR_NONFINITE);
             else if (f < 0.0 || b < 0.0) atomicOr(err, FOLD_ERR_NEGATIVE);
-            h = (f != 0.0 || b != 0.0) ? 1 : 0;
+            if constexpr (SLAB) h = ((f != 0.0 && own.voxel(p)) || (b != 0.0 && own.voxel(p + span - last))) ? 1 : 0;
+            else h = (f != 0.0 || b != 0.0) ? 1 : 0;
         }
         head[p] = h;
     }
@@ -150,12 +154,14 @@ __device__ __forceinline__ void nlink_tail_once(unsigned v, unsigned* __restrict
 // sum_edge does.  ids != nullptr: the list form, where a call (i, j) with i > j names the pair from its upper end, so its
 // cap is the backward and its rev_cap the forward increment.  A zero increment is skipped (exact: r + 0 == r).  Nothing
 // else is written here: the residual bits and the source re-clamp of the tails wait for k_nlinks_reclamp, after every
-// arc of the call has its new capacity.
-template <int ND>
+// arc of the call has its new capacity.  SLAB: an arc whose tail lies in a ghost plane is the neighbour slab's; its
+// increments are dropped here, so no ghost voxel is written or listed for the re-clamp (whose source push would land in
+// the ghost's excess, the outbox, and reach the neighbour as flow that no source sent).
+template <int ND, bool SLAB = false>
 __global__ void __launch_bounds__(256)
 k_nlinks_fold(Lattice L, State<double> S, const NlinkItem* __restrict__ items, int n, const int* __restrict__ order,
               const int64_t* __restrict__ ids, const double* __restrict__ cap, const double* __restrict__ rev,
-              unsigned* __restrict__ tbits, unsigned* __restrict__ tails, int* __restrict__ ntails)
+              unsigned* __restrict__ tbits, unsigned* __restrict__ tails, int* __restrict__ ntails, SlabOwn own = {})
 {
     const int step = (int)(gridDim.x * blockDim.x);
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += step) {
@@ -172,6 +178,7 @@ k_nlinks_fold(Lattice L, State<double> S, const NlinkItem* __restrict__ items, i
             if (f != 0.0) { rf = __dadd_rn(rf, f); up_f = true; }
             if (b != 0.0) { rb = __dadd_rn(rb, b); up_b = true; }
         }
+        if constexpr (SLAB) { up_f = up_f && own.voxel(it.lo); up_b = up_b && own.voxel(hi); }
         if (up_f) { cf[it.lo] = rf; nlink_tail_once(it.lo, tbits, tails, ntails); }
         if (up_b) { cb[hi] = rb; nlink_tail_once(hi, tbits, tails, ntails); }
     }

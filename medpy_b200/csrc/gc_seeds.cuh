@@ -30,6 +30,24 @@
 #define FOLD_ERR_PAIR 4         // a pair of ids that are not lattice neighbours (or i == j)
 #define FOLD_ERR_NEGATIVE 8     // a negative n-link increment
 
+// The voxels a z-slab handle owns, for the folds on it (DESIGN.md §4.6): local ids [lo, hi), its owned planes; the ghost
+// planes lie outside.  A fold applies a t-link call to owned voxels only, and an n-link increment to the arcs whose tail
+// is owned; the neighbour slab applies the rest to its own copy.  plane = voxels per axis-0 plane, the stride of axis 0.
+// The grouping kernels take it behind a compile-time flag SLAB (false: every voxel is owned, the handle's kernels do not
+// test it), as the batch kernels take BATCH.
+struct SlabOwn {
+    unsigned lo, hi, plane;
+    __device__ __forceinline__ bool voxel(unsigned v) const { return v - lo < hi - lo; }
+    // a t-link key of the grouping: the voxel itself
+    __device__ __forceinline__ bool key(unsigned v) const { return voxel(v); }
+    // an n-link key lo << 2 | axis: the pair has an owned end (an axis-0 pair reaches one plane up)
+    __device__ __forceinline__ bool key(unsigned long long k) const
+    {
+        const unsigned v = (unsigned)(k >> 2);
+        return (k & 3ull) == 0ull ? v + plane - lo < hi - lo + plane : voxel(v);
+    }
+};
+
 // One voxel's calls: calls first .. first + count - 1 of the sorted grouping (the dense form: the single call `first`)
 struct TweightItem {
     unsigned v;
@@ -76,11 +94,17 @@ __device__ __forceinline__ void claim_tile_once(const Lattice& L, const Tiles& T
     if (tflag[t] == 0 && atomicExch(&tflag[t], 1) == 0) tiles[atomicAdd(&ctl[2], 1)] = t;
 }
 
-// 1 at the first sorted key of each voxel (a run of keys 2v, then 2v + 1)
-__global__ void __launch_bounds__(256) k_seed_heads(const unsigned* __restrict__ keys, int n, int* __restrict__ head)
+// 1 at the first sorted key of each voxel (a run of keys 2v, then 2v + 1); SLAB: of each owned voxel (a seed in a ghost
+// plane is the neighbour slab's)
+template <bool SLAB = false>
+__global__ void __launch_bounds__(256) k_seed_heads(const unsigned* __restrict__ keys, int n, int* __restrict__ head,
+                                                    SlabOwn own = {})
 {
-    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x))
-        head[i] = (i == 0 || (keys[i] >> 1) != (keys[i - 1] >> 1)) ? 1 : 0;
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
+        int h = (i == 0 || (keys[i] >> 1) != (keys[i - 1] >> 1)) ? 1 : 0;
+        if constexpr (SLAB) h = h && own.voxel(keys[i] >> 1);
+        head[i] = h;
+    }
 }
 
 // Residual terminal capacity r(v) in the state of a materialised voxel (BK's tr_cap after the flow so far):
@@ -238,15 +262,18 @@ __global__ void __launch_bounds__(256) k_tweights_keys(const int64_t* __restrict
 // add_tweights(v, 0, 0) is an exact no-op in BK's arithmetic (the minimum is 0 and s - t gives tr back in both branches), so
 // only voxels with a call of a nonzero weight become items, in both forms.
 // list form: 1 at the first sorted key of each voxel that has such a call (order = the sorted call indices).  The n-link
-// list form (gc_nlinks.cuh) groups its arcs the same way: a, b = cap, rev_cap there.
-template <typename K>
+// list form (gc_nlinks.cuh) groups its arcs the same way: a, b = cap, rev_cap there.  SLAB: only a key the slab owns
+// heads an item (SlabOwn::key: an owned voxel, or a pair with an owned end).
+template <typename K, bool SLAB = false>
 __global__ void __launch_bounds__(256) k_weighted_heads(const K* __restrict__ keys, const int* __restrict__ order,
                                                         const double* __restrict__ a, const double* __restrict__ b, int n,
-                                                        int* __restrict__ head)
+                                                        int* __restrict__ head, SlabOwn own = {})
 {
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
         int h = 0;
-        if (i == 0 || keys[i] != keys[i - 1]) {
+        bool first = i == 0 || keys[i] != keys[i - 1];
+        if constexpr (SLAB) first = first && own.key(keys[i]);
+        if (first) {
             const int e = lower_bound(keys, i, n, (K)(keys[i] + 1u));
             for (int j = i; j < e && !h; ++j) h = (a[order[j]] != 0.0 || b[order[j]] != 0.0) ? 1 : 0;
         }
@@ -254,14 +281,18 @@ __global__ void __launch_bounds__(256) k_weighted_heads(const K* __restrict__ ke
     }
 }
 
-// dense form: 1 where the call has a nonzero weight
+// dense form: 1 where the call has a nonzero weight (SLAB: and the voxel is owned; every entry is checked)
+template <bool SLAB = false>
 __global__ void __launch_bounds__(256) k_tweights_dense_heads(const double* __restrict__ src, const double* __restrict__ snk,
-                                                              int n, int* __restrict__ head, int* __restrict__ err)
+                                                              int n, int* __restrict__ head, int* __restrict__ err,
+                                                              SlabOwn own = {})
 {
     for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) {
         const double s = src[i], t = snk[i];
         if (!isfinite(s) || !isfinite(t)) atomicOr(err, FOLD_ERR_NONFINITE);
-        head[i] = (s != 0.0 || t != 0.0) ? 1 : 0;
+        int h = (s != 0.0 || t != 0.0) ? 1 : 0;
+        if constexpr (SLAB) h = h && own.voxel((unsigned)i);
+        head[i] = h;
     }
 }
 

@@ -166,7 +166,12 @@ int mgc_slab_begin(mgc_graph* g)
     CK(cudaSetDevice(g->device));
     { int rc0 = check_pending(g); if (rc0) return rc0; }
     resolve_term_span(g);
-    int rc = materialise_zeros(g);
+    // MGC_OPT_WARM: the first solve records the residual source capacities before any push (the init of the per-term
+    // builds, k_warm_convert after the fused build); a no-op once recorded, so a re-solve after a fold continues from
+    // the state the fold left
+    int rc = warm_prepare(g);
+    if (rc) return rc;
+    rc = materialise_zeros(g);
     if (rc) return rc;
     return g->state_init ? MGC_OK : init_tiles(g);
 }

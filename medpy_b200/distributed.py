@@ -29,6 +29,33 @@ def slab_bounds(extent, world, rank):
     return (rank * extent) // world, ((rank + 1) * extent) // world
 
 
+def _contiguous(a):
+    return numpy.ascontiguousarray(a) if isinstance(a, numpy.ndarray) else a.contiguous()
+
+
+def _all_finite(a):
+    """No NaN or infinite value in a numpy array or a tensor."""
+    if isinstance(a, numpy.ndarray):
+        return bool(numpy.isfinite(a).all())
+    import torch
+    return bool(torch.isfinite(a).all())
+
+
+def _neighbours(i, j, shape):
+    """Whether every pair (i[k], j[k]) of global ids (numpy arrays or tensors) is a pair of lattice neighbours."""
+    if isinstance(i, numpy.ndarray):
+        lo = numpy.minimum(i, j)
+    else:
+        import torch
+        lo = torch.minimum(i, j)
+    d = abs(i - j)
+    ok = d < 0
+    for a in range(len(shape)):
+        stride = math.prod(shape[a + 1:])
+        ok = ok | ((d == stride) & ((lo // stride) % shape[a] + 1 < shape[a]))
+    return bool(ok.all())
+
+
 def _native_factory(shape, z0, z1, device):
     from . import _lib
     return _lib.Graph(list(shape), int(z0), int(z1), int(device))
@@ -38,7 +65,11 @@ class SlabSolver:
     """One rank's share of a z-slab partitioned graph cut."""
 
     def __init__(self, shape, rank=None, world=None, device=None, handle_factory=None, group=None,
-                 passes0=1, passes_max=8):
+                 passes0=1, passes_max=8, warm=False):
+        """``warm=True`` sets MGC_OPT_WARM on the slab's handle before anything is built: the first solve records the
+        residual state that the warm edits (``add_seeds``, ``remove_seeds``, ``add_tweights_warm``, ``add_nweights_warm``,
+        ``add_nweights_dense_warm``) fold into, and the next ``solve()`` continues from it.  It persists across
+        ``reset()``."""
         import torch
         import torch.distributed as dist
         self.torch, self.dist = torch, dist
@@ -71,6 +102,10 @@ class SlabSolver:
         else:
             self.tdev = torch.device("cpu")
             self.handle = handle_factory(self.shape, self.z0, self.z1)
+        self.warm = bool(warm)
+        if self.warm:
+            from . import _lib
+            self.handle.set_option(_lib._mgc.OPT_WARM, 1)
         self.plane = int(self.handle.slab_plane_elems())
         # one message per direction: [labels int32 x P | pad to 8 B | flow float64 x P]
         self.h_bytes = (self.plane * 4 + 7) // 8 * 8
@@ -116,6 +151,115 @@ class SlabSolver:
         sp = [float(s) for s in spacing] if spacing else None
         self.handle.build_voxel_graph(prob_local, 0.0 if alpha is None else float(alpha), bool(compute_f32) and prob_local is not None,
                                       k, image_local, 0.0 if sigma is None else float(sigma), sp, float(norm), fg_local, bg_local)
+
+    # ---------------------------------------------------------------------------------------------- warm edits
+    # Every rank passes the SAME global arguments, as to graphcut_slab: flat global node ids (C order over the whole
+    # lattice) or boolean masks of the global shape, numpy arrays or CUDA tensors.  All checks run before any native call
+    # and give every rank the same verdict, so either every rank raises the same ValueError or every rank folds.  A rank
+    # applies what it owns (DESIGN.md §4.6): the t-link calls on its planes, and of an n-link call the arcs whose tail is
+    # on its planes; an axis-0 pair across a border is applied half on each side, with no communication.
+    def _local_ids(self, ids):
+        """Global ids -> the rank's local ids (its planes plus the ghost planes, C order)."""
+        return ids - (self.z0 - (1 if self.ghost_lo else 0)) * self.plane
+
+    def _owned(self, ids):
+        return (ids >= self.z0 * self.plane) & (ids < self.z1 * self.plane)
+
+    def _any_bad(self, bad):
+        """One all-reduce of a rank's verdict on its part of a dense argument: True if any rank found a bad entry."""
+        t = self.torch.tensor([1 if bad else 0], dtype=self.torch.int64, device=self.tdev)
+        if self.world > 1:
+            self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
+        return bool(int(t.item()))
+
+    def add_seeds(self, fg=None, bg=None):
+        """Foreground / background seeds folded into the solved slabs (``add_tweights(v, 65535, 0)`` per fg id, then
+        ``add_tweights(v, 0, 65535)`` per bg id); the next ``solve()`` re-solves warm.  ``fg`` / ``bg``: a boolean mask
+        of the global shape, a 1-D integer array of global ids, or None."""
+        self._fold_seeds(fg, bg, self.handle.add_seeds)
+
+    def remove_seeds(self, fg=None, bg=None):
+        """The inverse of ``add_seeds``: ``add_tweights(v, -65535, 0)`` / ``add_tweights(v, 0, -65535)``."""
+        self._fold_seeds(fg, bg, self.handle.remove_seeds)
+
+    def _fold_seeds(self, fg, bg, native):
+        from .graphcut import _warm_args
+        _warm_args.one_space("fg and bg must both be host or both be device arrays", fg, bg)
+        n = math.prod(self.shape)
+        ids = [None if x is None else _warm_args.node_ids(x, self.shape, n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
+        native(*(None if a is None else self._local_ids(a[self._owned(a)]) for a in ids))
+
+    def add_tweights_warm(self, ids, src, snk):
+        """``add_tweights(ids[k], src[k], snk[k])`` calls folded into the solved slabs, in order.  ``ids``: global ids or
+        a boolean mask of the global shape; None for the dense form, where ``src`` / ``snk`` have the global shape (each
+        rank reads its planes and its ghost planes).  Scalars broadcast; weights are finite reals of either sign."""
+        from .graphcut import _warm_args
+        cuda = _warm_args.one_space("ids, src and snk must all be host or all be device arrays", ids, src, snk)
+        n = math.prod(self.shape)
+        if ids is None:
+            s = _warm_args.weights(src, n, "src", self.shape, cuda)
+            t = _warm_args.weights(snk, n, "snk", self.shape, cuda)
+            s, t = (self._slice_flat(a) for a in (s, t))
+            if self._any_bad(not (_all_finite(s) and _all_finite(t))):
+                raise ValueError("src or snk holds NaN or infinite values")
+            self.handle.add_tweights_warm(None, s, t)
+            return
+        ids = _warm_args.node_ids(ids, self.shape, n, "ids")
+        m = ids.shape[0]
+        s = _warm_args.weights(src, m, "src", device=cuda)
+        t = _warm_args.weights(snk, m, "snk", device=cuda)
+        if not (_all_finite(s) and _all_finite(t)):
+            raise ValueError("src or snk holds NaN or infinite values")
+        keep = self._owned(ids)
+        self.handle.add_tweights_warm(self._local_ids(ids[keep]), s[keep], t[keep])
+
+    def add_nweights_warm(self, i, j, cap, rev_cap):
+        """``sum_edge(i[k], j[k], cap[k], rev_cap[k])`` calls folded into the solved slabs, in order: ``i`` / ``j`` global
+        ids of lattice neighbours, ``cap`` / ``rev_cap`` nonnegative finite increments (scalars broadcast).  There is no
+        decrement on slabs: take capacity off by rebuilding."""
+        from .graphcut import _warm_args
+        cuda = _warm_args.one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
+        n = math.prod(self.shape)
+        ii, jj = _warm_args.pair_ids(i, n, "i"), _warm_args.pair_ids(j, n, "j")
+        ii, jj, c, r = _warm_args.nlink_calls(ii, jj, cap, rev_cap, cuda)
+        if not _neighbours(ii, jj, self.shape):
+            raise ValueError("i and j hold a pair that is not lattice neighbours")
+        for w, what in ((c, "cap"), (r, "rev_cap")):
+            if not _all_finite(w):
+                raise ValueError("{} holds NaN or infinite values".format(what))
+            if bool((w < 0).any()):
+                raise ValueError("{} holds negative values: {}".format(what, _warm_args.ONLY_RAISES))
+        keep = self._owned(ii) | self._owned(jj)
+        self.handle.add_nweights_warm(self._local_ids(ii[keep]), self._local_ids(jj[keep]), c[keep], r[keep])
+
+    def add_nweights_dense_warm(self, axis, fwd, bwd):
+        """The dense form of ``add_nweights_warm`` in the layout of ``add_nweights_dense``: ``fwd`` / ``bwd`` have the
+        global shape and entry p holds the increments of p -> p + e_axis and back; the last plane of ``axis`` is
+        ignored.  Each rank reads its planes and its ghost planes, so an axis-0 pair across a border reaches both."""
+        from .graphcut import _warm_args
+        axis = int(axis)
+        if not 0 <= axis < len(self.shape):
+            raise ValueError("axis {} is out of range for a lattice of shape {}".format(axis, self.shape))
+        _warm_args.one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
+        fwd, bwd = _warm_args.real(fwd, "fwd"), _warm_args.real(bwd, "bwd")
+        for a, what in ((fwd, "fwd"), (bwd, "bwd")):
+            if tuple(a.shape) != self.shape:
+                raise ValueError("{} of shape {} does not match the lattice's shape {}".format(what, tuple(a.shape), self.shape))
+        f, b = self.local_slice(fwd), self.local_slice(bwd)
+        f, b = (_contiguous(a) for a in (f, b))
+        # the entries the native grouping reads: all but the local last plane of the axis, whose pairs are another
+        # rank's (or, on the last rank, the global last plane, which names no pair)
+        cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(f.shape))
+        bad = not (_all_finite(f[cut]) and _all_finite(b[cut])) or bool((f[cut] < 0).any()) or bool((b[cut] < 0).any())
+        if self._any_bad(bad):
+            raise ValueError("fwd or bwd holds negative, NaN or infinite values: " + _warm_args.ONLY_RAISES)
+        self.handle.add_nweights_dense_warm(axis, f, b)
+
+    def _slice_flat(self, a):
+        """The rank's planes plus ghost planes of a flat global array of one entry per voxel, C-contiguous."""
+        lo = (self.z0 - (1 if self.ghost_lo else 0)) * self.plane
+        hi = (self.z1 + (1 if self.ghost_hi else 0)) * self.plane
+        return _contiguous(a[lo:hi])
 
     # ---------------------------------------------------------------------------------------------- messages
     def _views(self, buf):
