@@ -500,6 +500,17 @@ int mgc_sparse_set_option(mgc_sparse* g, int32_t option, int64_t value);
  * / infinite values. */
 int mgc_sparse_remove_edges_warm(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t* j, const double* cap,
                                  const double* rev_cap);
+/* Energies of a graph made of independent parts (DESIGN.md §8, "A batch of label images").
+ * mgc_sparse_set_option(g, MGC_OPT_SEGMENT_ENERGIES, 1): before the first mgc_sparse_add_tweights and the first solve
+ * since create or reset, and not on a warm handle (MGC_E_STATE otherwise); it survives mgc_sparse_reset.  The handle
+ * then keeps every add_tweights call's contribution to the constant (12 B per call) and, after a solve, the flow each
+ * node's sink link absorbed (8 B per node on the device).
+ * mgc_sparse_get_segment_energies(g, B, node_off, out): node_off[0..B] ascending from 0 to n splits the nodes into B
+ * ranges; out[b] = the constant of the calls on nodes of range b, summed in call order, + the flow absorbed by those
+ * nodes, summed in a fixed order (solves first if needed).  When no arc joins two ranges, out[b] is the energy the range
+ * alone would have; mgc_sparse_maxflow keeps returning the total. */
+#define MGC_OPT_SEGMENT_ENERGIES 4
+int mgc_sparse_get_segment_energies(mgc_sparse* g, int64_t B, const int64_t* node_off, double* out);
 
 /* ---- label images: the region adjacency graph built on the device (row f3) ------------------------------------ */
 
@@ -542,6 +553,22 @@ int mgc_labels_region_flags(mgc_labels* l, const mgc_array* markers, uint8_t* fl
 /* out[p] = per_region[label[p] - 1]: maps the cut back onto the voxels (bin/medpy_graphcut_label.py:139-148).
  * per_region = host array of K bytes; out = C-contiguous uint8 over the shape in host or device memory. */
 int mgc_labels_apply(mgc_labels* l, const uint8_t* per_region, uint8_t* out, int32_t out_mem);
+/* A batch of `batch` label images of `ndim` axes each, cut as one disjoint union of their region graphs (DESIGN.md §8,
+ * "A batch of label images").  Image b has the extents shapes[b*ndim .. b*ndim+ndim-1]; the images may differ in shape.
+ * `labels` (MGC_I32) is the images' C-ordered voxels concatenated image after image, passed as one 1-D array of
+ * sum(voxels) elements.  Each image must hold exactly 1..K_b: MGC_E_LABELS otherwise, with last_error naming the image.
+ * Label l of image b is node node_off[b] + l - 1, node_off the exclusive prefix of the K_b.  Refused before any
+ * allocation (MGC_E_ARG): an image of 2^31 voxels or more, 2^31 voxels or more in all; then 2^31 regions or more in all
+ * (node ids are int32), and from mgc_labels_boundary 2^32 border pairs or more in all.
+ * On a batch handle every call above works on the concatenation: `values`, `markers` and `out` are 1-D arrays of
+ * sum(voxels) elements laid out like `labels`, per-region arrays have sum(K_b) entries in node order, and
+ * mgc_labels_region_count returns sum(K_b).  mgc_labels_boundary gives every image's own edge list (bit for bit what
+ * mgc_labels_create + mgc_labels_boundary on that image gives, its ids shifted by node_off[b]), image after image; a
+ * pair never crosses images.  The per-region sums are each image's own too. */
+int mgc_labels_create_batch(int32_t batch, int32_t ndim, const int64_t* shapes, const mgc_array* labels, int32_t device,
+                            mgc_labels** out);
+/* node_off[0 .. batch]: the first node id of every image and the total (a handle of one image: {0, K}). */
+int mgc_labels_batch_offsets(const mgc_labels* l, int64_t* node_off);
 
 #ifdef __cplusplus
 }

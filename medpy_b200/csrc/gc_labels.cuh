@@ -209,21 +209,16 @@ __device__ __forceinline__ double lab_weight_pyfloat(E a, E b)
     return lab_floor_min(__dmul_rn(r, r));
 }
 
-// MODE 0: adjacency only (weights unused), 1: boundary_stawiaski, 2: boundary_stawiaski_directed
-// key = (lo << 32) | hi with lo < hi the 0-based node ids; wf accumulates cap(lo -> hi), wr cap(hi -> lo)
+// The c records of border pair (p, q) from slot block_off[blockIdx.x] + ex on.  MODE 0: adjacency only (weights unused), 1: boundary_stawiaski,
+// 2: boundary_stawiaski_directed.  key = (lo << 32) | hi with lo < hi the 0-based node ids; wf accumulates cap(lo -> hi),
+// wr cap(hi -> lo)
 template <typename E, int MODE>
-__global__ void __launch_bounds__(LAB_BLOCK) k_lab_pair_emit(LabGeom G, const int* __restrict__ labels, const E* __restrict__ grad,
-                                                              double beta, int dark_to_light,
-                                                              const unsigned long long* __restrict__ block_off,
-                                                              unsigned long long* __restrict__ keys, double* __restrict__ wf,
-                                                              double* __restrict__ wr)
+__device__ __forceinline__ void lab_pair_write(const int* __restrict__ labels, const E* __restrict__ grad, double beta,
+                                               int dark_to_light, long long p, long long q, unsigned c,
+                                               const unsigned long long* __restrict__ block_off, unsigned ex,
+                                               unsigned long long* __restrict__ keys,
+                                               double* __restrict__ wf, double* __restrict__ wr)
 {
-    const long long idx = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x;
-    long long p = 0, q = 0;
-    const unsigned c = lab_pair_items(G, labels, idx, MODE == 2, &p, &q);
-    unsigned total;
-    const unsigned ex = lab_block_scan(c, &total);
-    if (!c) return;
     const int k1 = labels[p] - 1, k2 = labels[q] - 1;            // set_nweight(key1 - 1, key2 - 1, there, back)
     const bool fwd = k1 < k2;
     const unsigned long long lo = (unsigned long long)(fwd ? k1 : k2), hi = (unsigned long long)(fwd ? k2 : k1);
@@ -245,6 +240,166 @@ __global__ void __launch_bounds__(LAB_BLOCK) k_lab_pair_emit(LabGeom G, const in
             wr[pos + r] = fwd ? back : there;
         }
     }
+}
+
+template <typename E, int MODE>
+__global__ void __launch_bounds__(LAB_BLOCK) k_lab_pair_emit(LabGeom G, const int* __restrict__ labels, const E* __restrict__ grad,
+                                                              double beta, int dark_to_light,
+                                                              const unsigned long long* __restrict__ block_off,
+                                                              unsigned long long* __restrict__ keys, double* __restrict__ wf,
+                                                              double* __restrict__ wr)
+{
+    const long long idx = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x;
+    long long p = 0, q = 0;
+    const unsigned c = lab_pair_items(G, labels, idx, MODE == 2, &p, &q);
+    unsigned total;
+    const unsigned ex = lab_block_scan(c, &total);
+    if (!c) return;
+    lab_pair_write<E, MODE>(labels, grad, beta, dark_to_light, p, q, c, block_off, ex, keys, wf, wr);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// a batch of label images (mgc_labels_create_batch)
+// ---------------------------------------------------------------------------------------------------------------
+// The images' voxels are concatenated image after image, each image in its own C order, and the staged labels hold
+// label + node_off[b] (global node id + 1).  The kernels above that only read labels -- region items, flags, apply --
+// therefore run unchanged on the concatenation.  The border-pair item space is image-major, then axis-major, then C
+// order inside the image (image b owns items [nd * vox_off[b], nd * vox_off[b+1])); a pair never crosses images.
+struct LabBatch {
+    int B;                          // images
+    int nd;                         // axes of every image (1..4)
+    const long long* vox_off;       // [B+1] exclusive prefix of the images' voxel counts
+    const int* dim;                 // [4*B] extents per image, padded with 1
+};
+
+// The images that units [blockIdx.x * LAB_BLOCK, +LAB_BLOCK) of a block touch (`per` units per voxel: 1 for voxels, nd
+// for border-pair items), staged in shared memory: a block of 256 units touches at most 256 images, and every unit then
+// finds its image by a binary search here instead of in global memory.
+struct LabWindow {
+    int b0, count;                  // images b0 .. b0 + count - 1
+    long long vox[LAB_BLOCK + 1];   // their vox_off entries (count + 1)
+    int dim[LAB_BLOCK][4];
+};
+
+// largest i in [0, count) with off[i] <= x (off ascending, off[0] <= x)
+__device__ __forceinline__ int lab_batch_find(const long long* off, int count, long long x)
+{
+    int lo = 0, hi = count;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (off[mid] <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// every thread of the block calls it; units in [0, total)
+__device__ __forceinline__ void lab_batch_window(const LabBatch& L, int per, long long total, LabWindow& w)
+{
+    if (threadIdx.x == 0) {
+        const long long s = (long long)blockIdx.x * LAB_BLOCK;
+        const long long e = (s + LAB_BLOCK < total ? s + LAB_BLOCK : total) - 1;
+        const int b0 = lab_batch_find(L.vox_off, L.B, s / per);
+        w.b0 = b0;
+        w.count = lab_batch_find(L.vox_off, L.B, e / per) - b0 + 1;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i <= w.count; i += LAB_BLOCK) w.vox[i] = L.vox_off[w.b0 + i];
+    for (int i = threadIdx.x; i < w.count; i += LAB_BLOCK)
+        for (int d = 0; d < 4; ++d) w.dim[i][d] = L.dim[4 * (w.b0 + i) + d];
+    __syncthreads();
+}
+
+// lab_pair_items for item idx of the batch: the same rule inside the item's image, `dup_first` on each image's first
+// voxel; p and q come back as positions in the concatenation
+__device__ __forceinline__ unsigned lab_batch_pair_items(const LabBatch& L, const LabWindow& w, const int* __restrict__ labels,
+                                                         long long idx, long long total, int dup_first, long long* p_out,
+                                                         long long* q_out)
+{
+    if (idx >= total) return 0u;
+    const int i = lab_batch_find(w.vox, w.count, idx / L.nd);
+    const long long v0 = w.vox[i], n = w.vox[i + 1] - v0;
+    const long long li = idx - (long long)L.nd * v0;
+    const int d = (int)(li / n);
+    const long long p = li - (long long)d * n;
+    long long stride = 1;
+    for (int a = L.nd - 1; a > d; --a) stride *= w.dim[i][a];
+    const long long dd = w.dim[i][d];
+    if ((p / stride) % dd >= dd - 1) return 0u;
+    const long long q = p + stride;
+    if (labels[v0 + p] == labels[v0 + q]) return 0u;
+    *p_out = v0 + p;
+    *q_out = v0 + q;
+    return (dup_first && p == 0) ? 2u : 1u;
+}
+
+__global__ void __launch_bounds__(LAB_BLOCK) k_lab_batch_pair_count(LabBatch L, long long total, const int* __restrict__ labels,
+                                                                     int dup_first, unsigned* __restrict__ block_count)
+{
+    __shared__ LabWindow w;
+    lab_batch_window(L, L.nd, total, w);
+    const long long idx = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x;
+    long long p, q;
+    const unsigned c = lab_batch_pair_items(L, w, labels, idx, total, dup_first, &p, &q);
+    unsigned sum;
+    lab_block_scan(c, &sum);
+    if (threadIdx.x == 0) block_count[blockIdx.x] = sum;
+}
+
+// k_lab_pair_emit over the batch: keys are (global lo << 32) | global hi, so every key's records come from one image,
+// in that image's order
+template <typename E, int MODE>
+__global__ void __launch_bounds__(LAB_BLOCK) k_lab_batch_pair_emit(LabBatch L, long long total, const int* __restrict__ labels,
+                                                                    const E* __restrict__ grad, double beta, int dark_to_light,
+                                                                    const unsigned long long* __restrict__ block_off,
+                                                                    unsigned long long* __restrict__ keys,
+                                                                    double* __restrict__ wf, double* __restrict__ wr)
+{
+    __shared__ LabWindow w;
+    lab_batch_window(L, L.nd, total, w);
+    const long long idx = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x;
+    long long p = 0, q = 0;
+    const unsigned c = lab_batch_pair_items(L, w, labels, idx, total, MODE == 2, &p, &q);
+    unsigned sum;
+    const unsigned ex = lab_block_scan(c, &sum);
+    if (!c) return;
+    lab_pair_write<E, MODE>(labels, grad, beta, dark_to_light, p, q, c, block_off, ex, keys, wf, wr);
+}
+
+// __check_label_image per image, first pass: min and max label of every image (mm[2b], mm[2b+1]); one block reduces
+// its share of an image in shared memory before one atomic per image
+__global__ void __launch_bounds__(LAB_BLOCK) k_lab_batch_minmax(LabBatch L, const int* __restrict__ labels, long long n,
+                                                                int* __restrict__ mm)
+{
+    __shared__ LabWindow w;
+    __shared__ int lo[LAB_BLOCK], hi[LAB_BLOCK];
+    lab_batch_window(L, 1, n, w);
+    for (int i = threadIdx.x; i < w.count; i += LAB_BLOCK) { lo[i] = INT32_MAX; hi[i] = INT32_MIN; }
+    __syncthreads();
+    const long long p = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x;
+    if (p < n) {
+        const int i = lab_batch_find(w.vox, w.count, p), l = labels[p];
+        atomicMin(&lo[i], l);
+        atomicMax(&hi[i], l);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < w.count; i += LAB_BLOCK) {
+        atomicMin(&mm[2 * (w.b0 + i)], lo[i]);
+        atomicMax(&mm[2 * (w.b0 + i) + 1], hi[i]);
+    }
+}
+
+// second pass, once every image holds labels in 1..K_b: labels[p] += node_off[b] and present[global id] = 1
+__global__ void __launch_bounds__(LAB_BLOCK) k_lab_batch_offset(LabBatch L, int* __restrict__ labels, long long n,
+                                                                const long long* __restrict__ node_off,
+                                                                uint8_t* __restrict__ present)
+{
+    __shared__ LabWindow w;
+    lab_batch_window(L, 1, n, w);
+    const long long p = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x;
+    if (p >= n) return;
+    const int g = labels[p] + (int)node_off[w.b0 + lab_batch_find(w.vox, w.count, p)];
+    labels[p] = g;
+    present[g - 1] = 1;
 }
 
 __global__ void __launch_bounds__(LAB_BLOCK) k_lab_iota(unsigned* __restrict__ a, long long m)

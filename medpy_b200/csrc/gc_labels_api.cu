@@ -34,6 +34,14 @@ struct mgc_labels {
     std::vector<double> ew, er;
     int64_t kernel_launches = 0;
     std::string err;
+    // a batch (mgc_labels_create_batch): `batch` images of `bnd` axes each, concatenated; G is then the 1-D geometry of
+    // the concatenation, `labels` holds label + node_off[b] and k is the sum of the images' region counts
+    int32_t batch = 0;
+    int32_t bnd = 0;
+    std::vector<int64_t> vox_off, node_off;     // [batch + 1]
+    long long* d_vox_off = nullptr;             // device copies of vox_off and of the extents (4 per image)
+    int* d_dim = nullptr;
+    LabBatch geom() const { return LabBatch{batch, bnd, d_vox_off, d_dim}; }
 };
 
 namespace {
@@ -89,14 +97,15 @@ template <typename E, int MODE>
 int lab_boundary_run(mgc_labels* g, const E* grad, double directedness)
 {
     DevScope dev;
-    const long long items = (long long)g->G.nd * g->G.n;
+    const long long items = (long long)(g->batch ? g->bnd : g->G.nd) * g->G.n;
     const long long nb = (items + LAB_BLOCK - 1) / LAB_BLOCK;
     if (nb >= (long long)INT32_MAX) FAIL(MGC_E_ARG, "label image too large");
     unsigned* block_count;
     unsigned long long* block_off;
     CK(dev.alloc(&block_count, (size_t)nb));
     CK(dev.alloc(&block_off, (size_t)nb + 1));
-    k_lab_pair_count<<<(unsigned)nb, LAB_BLOCK>>>(g->G, g->labels, MODE == 2 ? 1 : 0, block_count);
+    if (g->batch) k_lab_batch_pair_count<<<(unsigned)nb, LAB_BLOCK>>>(g->geom(), items, g->labels, MODE == 2 ? 1 : 0, block_count);
+    else          k_lab_pair_count<<<(unsigned)nb, LAB_BLOCK>>>(g->G, g->labels, MODE == 2 ? 1 : 0, block_count);
     k_lab_scan_blocks<<<1, 1024>>>(block_count, nb, block_off);
     g->kernel_launches += 2;
     CK(cudaGetLastError());
@@ -113,8 +122,13 @@ int lab_boundary_run(mgc_labels* g, const E* grad, double directedness)
     CK(dev.alloc(&keys_sorted, (size_t)m));
     if (MODE >= 1) { CK(dev.alloc(&wf, (size_t)m)); CK(dev.alloc(&wf_s, (size_t)m)); }
     if (MODE == 2) { CK(dev.alloc(&wr, (size_t)m)); CK(dev.alloc(&wr_s, (size_t)m)); }
-    k_lab_pair_emit<E, MODE><<<(unsigned)nb, LAB_BLOCK>>>(g->G, g->labels, grad, directedness < 0 ? -directedness : directedness,
-                                                          directedness < 0 ? 1 : 0, block_off, keys, wf, wr);
+    const double beta = directedness < 0 ? -directedness : directedness;
+    const int dark_to_light = directedness < 0 ? 1 : 0;
+    if (g->batch)
+        k_lab_batch_pair_emit<E, MODE><<<(unsigned)nb, LAB_BLOCK>>>(g->geom(), items, g->labels, grad, beta, dark_to_light,
+                                                                    block_off, keys, wf, wr);
+    else
+        k_lab_pair_emit<E, MODE><<<(unsigned)nb, LAB_BLOCK>>>(g->G, g->labels, grad, beta, dark_to_light, block_off, keys, wf, wr);
     g->kernel_launches++;
     CK(cudaGetLastError());
     // stable sort by key: contributions of one region pair stay in the reference's order
@@ -282,10 +296,144 @@ int mgc_labels_create(int32_t ndim, const int64_t* shape, const mgc_array* label
     return MGC_OK;
 }
 
+int mgc_labels_create_batch(int32_t batch, int32_t ndim, const int64_t* shapes, const mgc_array* labels, int32_t device,
+                            mgc_labels** out)
+{
+    if (!out) return MGC_E_ARG;
+    *out = nullptr;
+    if (batch < 1 || !shapes) { g_lab_create_error = "a batch holds at least one label image"; return MGC_E_ARG; }
+    if (ndim < 1 || ndim > MGC_MAX_NDIM || !labels) { g_lab_create_error = "label images must have 1 to 4 dimensions"; return MGC_E_ARG; }
+    if (labels->dtype != MGC_I32) { g_lab_create_error = "label image must be int32"; return MGC_E_ARG; }
+    // the limits, before any allocation: each image within those of one image, the batch within what its int32 node
+    // ids, the region sums' sort and the int32 sort of the border pairs address
+    std::vector<int64_t> vox_off((size_t)batch + 1, 0);
+    std::vector<int> dims((size_t)batch * 4, 1);
+    for (int32_t b = 0; b < batch; ++b) {
+        long long n = 1;
+        for (int d = 0; d < ndim; ++d) {
+            const int64_t s = shapes[(size_t)b * ndim + d];
+            if (s < 1) { g_lab_create_error = "label image " + std::to_string(b) + ": empty label image"; return MGC_E_LABELS; }
+            if (s >= (int64_t)INT32_MAX) { g_lab_create_error = "label image " + std::to_string(b) + ": label image too large (2^31 voxels)"; return MGC_E_ARG; }
+            dims[(size_t)b * 4 + d] = (int)s;
+            n *= s;
+            if (n >= (long long)INT32_MAX) { g_lab_create_error = "label image " + std::to_string(b) + ": label image too large (2^31 voxels)"; return MGC_E_ARG; }
+        }
+        vox_off[(size_t)b + 1] = vox_off[(size_t)b] + n;
+        if (vox_off[(size_t)b + 1] >= (int64_t)INT32_MAX) { g_lab_create_error = "label batch too large (2^31 voxels in all)"; return MGC_E_ARG; }
+    }
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count < 1) {
+        cudaGetLastError();
+        g_lab_create_error = "no CUDA device available (this library has no CPU path)";
+        return MGC_E_CUDA;
+    }
+    if (device < 0) { if (cudaGetDevice(&device) != cudaSuccess) device = 0; }
+    if (device >= count) { g_lab_create_error = "invalid CUDA device ordinal"; return MGC_E_ARG; }
+    mgc_labels* g = new mgc_labels();
+    const long long n = (long long)vox_off[(size_t)batch];
+    g->device = device;
+    g->batch = batch;
+    g->bnd = ndim;
+    g->vox_off = vox_off;
+    g->G.nd = 1;                                    // the concatenation, as the region kernels and the staging see it
+    for (int d = 0; d < 4; ++d) { g->G.dim[d] = 1; g->G.stride[d] = 1; }
+    g->G.dim[0] = n;
+    g->G.n = n;
+    g->shape[0] = n;
+    auto fail = [&](int code) { g_lab_create_error = g->err; mgc_labels_destroy(g); return code; };
+    if (cudaSetDevice(device) != cudaSuccess) { g->err = "cudaSetDevice failed"; return fail(MGC_E_CUDA); }
+    if (cudaMalloc(&g->d_vox_off, vox_off.size() * sizeof(long long)) != cudaSuccess ||
+        cudaMalloc(&g->d_dim, dims.size() * sizeof(int)) != cudaSuccess) {
+        cudaGetLastError();
+        g->err = "device allocation failed";
+        return fail(MGC_E_NOMEM);
+    }
+    const LabBatch L = g->geom();
+    DevScope scope;
+    int* mm = nullptr;
+    long long* d_node_off = nullptr;
+    std::vector<int> got((size_t)batch * 2);
+    {
+        int rc = [&]() -> int {
+            CK(cudaMemcpy(g->d_vox_off, vox_off.data(), vox_off.size() * sizeof(long long), cudaMemcpyHostToDevice));
+            CK(cudaMemcpy(g->d_dim, dims.data(), dims.size() * sizeof(int), cudaMemcpyHostToDevice));
+            const int* p = nullptr;
+            RC(lab_stage<int>(g, labels, scope, &p));
+            // the offsets are added in place: keep a copy of our own
+            if (scope.ptrs.empty()) {
+                int* own = nullptr;
+                CK(scope.alloc(&own, (size_t)n));
+                CK(cudaMemcpy(own, p, (size_t)n * sizeof(int), cudaMemcpyDeviceToDevice));
+                p = own;
+            }
+            g->labels = (int*)p;
+            g->owns_labels = true;
+            scope.keep(p);
+            // __check_label_image per image: min == 1 and every id up to max present
+            for (int32_t b = 0; b < batch; ++b) { got[2 * (size_t)b] = INT32_MAX; got[2 * (size_t)b + 1] = INT32_MIN; }
+            CK(scope.alloc(&mm, got.size()));
+            CK(cudaMemcpy(mm, got.data(), got.size() * sizeof(int), cudaMemcpyHostToDevice));
+            k_lab_batch_minmax<<<(unsigned)((n + LAB_BLOCK - 1) / LAB_BLOCK), LAB_BLOCK>>>(L, g->labels, n, mm);
+            g->kernel_launches++;
+            CK(cudaGetLastError());
+            CK(cudaMemcpy(got.data(), mm, got.size() * sizeof(int), cudaMemcpyDeviceToHost));
+            return MGC_OK;
+        }();
+        if (rc) return fail(rc);
+    }
+    const char* msg = "The supplied label image does either not contain any regions or they are not labeled consecutively starting from 1.";
+    std::vector<int64_t> node_off((size_t)batch + 1, 0);
+    for (int32_t b = 0; b < batch; ++b) {
+        if (got[2 * (size_t)b] != 1 || got[2 * (size_t)b + 1] < 1) { g->err = "label image " + std::to_string(b) + ": " + msg; return fail(MGC_E_LABELS); }
+        node_off[(size_t)b + 1] = node_off[(size_t)b] + got[2 * (size_t)b + 1];
+        if (node_off[(size_t)b + 1] >= (int64_t)INT32_MAX) { g->err = "label batch has 2^31 regions or more (node ids are int32)"; return fail(MGC_E_ARG); }
+    }
+    const int64_t k = node_off[(size_t)batch];
+    int rc = [&]() -> int {
+        uint8_t* present = nullptr;
+        unsigned long long* cnt = nullptr;
+        CK(scope.alloc(&d_node_off, node_off.size()));
+        CK(scope.alloc(&present, (size_t)k));
+        CK(scope.alloc(&cnt, 1));
+        CK(cudaMemcpy(d_node_off, node_off.data(), node_off.size() * sizeof(long long), cudaMemcpyHostToDevice));
+        CK(cudaMemset(present, 0, (size_t)k));
+        CK(cudaMemset(cnt, 0, sizeof(unsigned long long)));
+        k_lab_batch_offset<<<(unsigned)((n + LAB_BLOCK - 1) / LAB_BLOCK), LAB_BLOCK>>>(L, g->labels, n, d_node_off, present);
+        k_lab_count_u8<<<grid_for(k), LAB_BLOCK>>>(present, k, cnt);
+        g->kernel_launches += 2;
+        CK(cudaGetLastError());
+        unsigned long long c = 0;
+        CK(cudaMemcpy(&c, cnt, sizeof(c), cudaMemcpyDeviceToHost));
+        if ((int64_t)c == k) return MGC_OK;
+        // some image misses an id: name the first one
+        std::vector<uint8_t> h((size_t)k);
+        CK(cudaMemcpy(h.data(), present, (size_t)k, cudaMemcpyDeviceToHost));
+        for (int32_t b = 0; b < batch; ++b)
+            for (int64_t r = node_off[(size_t)b]; r < node_off[(size_t)b + 1]; ++r)
+                if (!h[(size_t)r]) FAIL(MGC_E_LABELS, "label image " + std::to_string(b) + ": " + msg);
+        FAIL(MGC_E_LABELS, msg);
+    }();
+    if (rc) return fail(rc);
+    g->k = k;
+    g->node_off = node_off;
+    *out = g;
+    return MGC_OK;
+}
+
+int mgc_labels_batch_offsets(const mgc_labels* g, int64_t* node_off)
+{
+    if (!g || !node_off) return MGC_E_ARG;
+    if (!g->batch) { node_off[0] = 0; node_off[1] = g->k; return MGC_OK; }
+    std::memcpy(node_off, g->node_off.data(), g->node_off.size() * sizeof(int64_t));
+    return MGC_OK;
+}
+
 void mgc_labels_destroy(mgc_labels* g)
 {
     if (!g) return;
     if (g->owns_labels && g->labels) { cudaSetDevice(g->device); cudaFree(g->labels); }
+    if (g->d_vox_off) cudaFree(g->d_vox_off);
+    if (g->d_dim) cudaFree(g->d_dim);
     delete g;
 }
 

@@ -620,6 +620,16 @@ public:
         check_sparse(rc, g_);
     }
     void set_option(int32_t option, int64_t value) { check_sparse(mgc_sparse_set_option(g_, option, value), g_); }
+    py::array_t<double> segment_energies(py::array_t<int64_t, py::array::c_style | py::array::forcecast> node_off)
+    {
+        const py::ssize_t b = node_off.size() - 1;
+        if (b < 1) throw py::value_error("node offsets of at least one range expected");
+        py::array_t<double> out(b);
+        int rc;
+        { double* p = out.mutable_data(); const int64_t* o = node_off.data(); py::gil_scoped_release rel; rc = mgc_sparse_get_segment_energies(g_, (int64_t)b, o, p); }
+        check_sparse(rc, g_);
+        return out;
+    }
     void add_tweights(const py::object& nodes, py::array_t<double, py::array::c_style | py::array::forcecast> src,
                       py::array_t<double, py::array::c_style | py::array::forcecast> snk)
     {
@@ -691,6 +701,37 @@ public:
             if (rc == MGC_E_ARG) throw py::value_error(m);
             throw std::runtime_error(m);
         }
+    }
+    // a batch: `shapes` one extent list per image (one ndim), `labels` the images' C-ordered voxels concatenated (1-D)
+    static std::unique_ptr<PyLabels> batch(const std::vector<std::vector<int64_t>>& shapes, const py::object& labels, int device)
+    {
+        if (shapes.empty()) throw py::value_error("a batch holds at least one label image");
+        const size_t nd = shapes[0].size();
+        std::vector<int64_t> flat;
+        for (const auto& s : shapes) {
+            if (s.size() != nd) throw py::value_error("the images of a batch must have one number of dimensions");
+            flat.insert(flat.end(), s.begin(), s.end());
+        }
+        ArrayRef r = make_ref(labels, MGC_I32, "label_images");
+        if (r.shape.size() != 1) throw py::value_error("label_images: the concatenated images as one 1-D array expected");
+        std::unique_ptr<PyLabels> out(new PyLabels());
+        out->shape_ = r.shape;
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_labels_create_batch((int32_t)shapes.size(), (int32_t)nd, flat.data(), &r.a, device, &out->l_); }
+        if (rc != MGC_OK) {
+            std::string m = mgc_labels_last_error(nullptr);
+            if (rc == MGC_E_LABELS) { PyErr_SetString(PyExc_AttributeError, m.c_str()); throw py::error_already_set(); }
+            if (rc == MGC_E_ARG) throw py::value_error(m);
+            throw std::runtime_error(m);
+        }
+        out->batch_ = (int64_t)shapes.size();
+        return out;
+    }
+    py::array_t<int64_t> batch_offsets() const
+    {
+        py::array_t<int64_t> off((py::ssize_t)batch_ + 1);
+        check(mgc_labels_batch_offsets(l_, off.mutable_data()));
+        return off;
     }
     ~PyLabels() { if (l_) mgc_labels_destroy(l_); }
     PyLabels(const PyLabels&) = delete;
@@ -765,8 +806,10 @@ public:
     std::vector<int64_t> shape() const { return shape_; }
 
 private:
+    PyLabels() = default;
     mgc_labels* l_ = nullptr;
     std::vector<int64_t> shape_;
+    int64_t batch_ = 1;
 };
 
 }  // namespace
@@ -798,6 +841,7 @@ PYBIND11_MODULE(_mgc, m)
     m.attr("OPT_DEFER_WEIGHT_CHECK") = MGC_OPT_DEFER_WEIGHT_CHECK;
     m.attr("OPT_WARM") = MGC_OPT_WARM;
     m.attr("OPT_KEEP_DEVICE_INPUTS") = MGC_OPT_KEEP_DEVICE_INPUTS;
+    m.attr("OPT_SEGMENT_ENERGIES") = MGC_OPT_SEGMENT_ENERGIES;
     m.attr("LABELS_ADJACENCY") = MGC_LABELS_ADJACENCY;
     m.attr("LABELS_STAWIASKI") = MGC_LABELS_STAWIASKI;
     m.attr("LABELS_STAWIASKI_DIRECTED") = MGC_LABELS_STAWIASKI_DIRECTED;
@@ -808,6 +852,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("sum_edges", &PySparse::sum_edges)
         .def("remove_edges_warm", &PySparse::remove_edges_warm)
         .def("set_option", &PySparse::set_option)
+        .def("segment_energies", &PySparse::segment_energies)
         .def("add_tweights", &PySparse::add_tweights)
         .def("maxflow", &PySparse::maxflow)
         .def("get_mask", &PySparse::get_mask)
@@ -825,6 +870,8 @@ PYBIND11_MODULE(_mgc, m)
         .def("region_sums", &PyLabels::region_sums)
         .def("region_flags", &PyLabels::region_flags)
         .def("apply", &PyLabels::apply)
+        .def_static("batch", &PyLabels::batch, py::arg("shapes"), py::arg("label_images"), py::arg("device") = -1)
+        .def("batch_offsets", &PyLabels::batch_offsets)
         .def_property_readonly("shape", &PyLabels::shape);
     py::class_<PyGraph>(m, "Graph")
         .def(py::init<const std::vector<int64_t>&, int>(), py::arg("shape"), py::arg("device") = -1)

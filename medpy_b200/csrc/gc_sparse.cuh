@@ -201,4 +201,26 @@ __global__ void __launch_bounds__(256) k_sp_readout(SparseState G, uint8_t* __re
     }
     if (tid == 0) absorbed[0] = sh[0];
 }
+
+// absorbed[s] = flow absorbed by the nodes [off[s], off[s+1]), summed as k_sp_readout sums a whole graph's (256 chains
+// interleaved from the range's first node, then the same tree): one block per range, no atomics, the same bits every run
+__global__ void __launch_bounds__(256) k_sp_segment_absorbed(const double* __restrict__ sunk, const long long* __restrict__ off,
+                                                             long long segs, double* __restrict__ absorbed)
+{
+    __shared__ double sh[256];
+    const int tid = threadIdx.x;
+    for (long long s = blockIdx.x; s < segs; s += gridDim.x) {
+        const long long a = off[s], b = off[s + 1];
+        double acc = 0.0;
+        for (long long u = a + tid; u < b; u += 256) acc = __dadd_rn(acc, sunk[u]);
+        sh[tid] = acc;
+        __syncthreads();
+        for (int k = 128; k > 0; k >>= 1) {
+            if (tid < k) sh[tid] = __dadd_rn(sh[tid], sh[tid + k]);
+            __syncthreads();
+        }
+        if (tid == 0) absorbed[s] = sh[0];
+        __syncthreads();
+    }
+}
 #endif  // __CUDACC__

@@ -98,8 +98,13 @@ struct mgc_sparse {
     bool warm_bad = false;                             // that solve's graph held a NaN or infinite capacity: no folds
     double wconst = 0.0;                               // constant of the resident state (energy = wconst + absorbed)
     SparseDev dev;                                     // a cold solve's arrays for the call, a warm one's until reset
+    // MGC_OPT_SEGMENT_ENERGIES: host.log_const is set, and every solve leaves its per-node absorbed flow in `seg_sunk`
+    bool segments = false;
+    bool tweights_added = false;                       // add_tweights was called since create / reset
+    double* seg_sunk = nullptr;
     void release()
     {
+        if (seg_sunk) { cudaSetDevice(device); cudaFree(seg_sunk); seg_sunk = nullptr; }
         if (!resident) return;
         cudaSetDevice(device);
         dev.release();
@@ -221,7 +226,14 @@ int sparse_solve(mgc_sparse* g)
         return sparse_loop(g, ev, g->wconst);
     }
     const int rc = sparse_first_solve(g);
-    if (!g->resident) g->dev.release();             // a cold solve's arrays live for the call
+    if (!g->resident) {
+        if (g->segments && rc == MGC_OK) {          // the absorbed flow per node outlives the solve
+            if (g->seg_sunk) cudaFree(g->seg_sunk);
+            g->seg_sunk = g->dev.sunk;
+            g->dev.sunk = nullptr;
+        }
+        g->dev.release();                           // a cold solve's arrays live for the call
+    }
     return rc;
 }
 
@@ -482,6 +494,8 @@ int mgc_sparse_reset(mgc_sparse* g)
 {
     if (!g) return MGC_E_ARG;
     g->host = SparseHost(g->host.n);
+    g->host.log_const = g->segments;
+    g->tweights_added = false;
     g->solved = false;
     g->energy = 0.0;
     g->mask.clear();
@@ -496,7 +510,17 @@ int mgc_sparse_reset(mgc_sparse* g)
 int mgc_sparse_set_option(mgc_sparse* g, int32_t option, int64_t value)
 {
     if (!g) return MGC_E_ARG;
+    if (option == MGC_OPT_SEGMENT_ENERGIES) {
+        if (g->solved_once || g->resident || g->tweights_added)
+            FAIL(MGC_E_STATE, "MGC_OPT_SEGMENT_ENERGIES must be set before the first add_tweights and maxflow(): reset() the "
+                              "graph and rebuild it");
+        if (g->warm && value) FAIL(MGC_E_STATE, "segment energies are not kept on a warm graph");
+        g->segments = value != 0;
+        g->host.log_const = g->segments;
+        return MGC_OK;
+    }
     if (option != MGC_OPT_WARM) FAIL(MGC_E_ARG, "unknown option for a sparse graph");
+    if (value && g->segments) FAIL(MGC_E_STATE, "segment energies are not kept on a warm graph");
     if (g->solved_once || g->resident)
         FAIL(MGC_E_STATE, "MGC_OPT_WARM must be set before the first maxflow(): reset() the graph and rebuild it");
     g->warm = value != 0;
@@ -540,7 +564,7 @@ int mgc_sparse_add_tweights(mgc_sparse* g, int64_t count, const int32_t* nodes, 
         if (rc) return rc;
     }
     g->host.add_tweights(count, nodes, src, snk);
-    if (count) g->solved = false;
+    if (count) { g->solved = false; g->tweights_added = true; }
     return MGC_OK;
 }
 
@@ -599,6 +623,39 @@ int mgc_sparse_get_mask(mgc_sparse* g, uint8_t* out)
     if (!g || !out) return MGC_E_ARG;
     if (!g->solved) { int rc = sparse_solve(g); if (rc) return rc; }
     std::memcpy(out, g->mask.data(), (size_t)g->host.n);
+    return MGC_OK;
+}
+
+int mgc_sparse_get_segment_energies(mgc_sparse* g, int64_t B, const int64_t* node_off, double* out)
+{
+    if (!g) return MGC_E_ARG;
+    if (B < 1 || !node_off || !out) FAIL(MGC_E_ARG, "segment energies need B >= 1 ranges and their B + 1 offsets");
+    if (!g->segments) FAIL(MGC_E_STATE, "segment energies need MGC_OPT_SEGMENT_ENERGIES, set before the graph was built");
+    if (node_off[0] != 0 || node_off[B] != g->host.n) FAIL(MGC_E_ARG, "node offsets must run from 0 to the node count");
+    for (int64_t b = 0; b < B; ++b)
+        if (node_off[b + 1] < node_off[b]) FAIL(MGC_E_ARG, "node offsets must be ascending");
+    if (!g->solved) RC(sparse_solve(g));
+    CK(cudaSetDevice(g->device));
+    DevScope dev;
+    long long* d_off;
+    double* d_abs;
+    CK(dev.alloc(&d_off, (size_t)B + 1));
+    CK(dev.alloc(&d_abs, (size_t)B));
+    CK(cudaMemcpy(d_off, node_off, ((size_t)B + 1) * sizeof(long long), cudaMemcpyHostToDevice));
+    const long long cap = 32LL * cached_sm_count(g->device);
+    k_sp_segment_absorbed<<<(unsigned)(B < cap ? B : cap), 256>>>(g->seg_sunk, d_off, (long long)B, d_abs);
+    g->st.kernel_launches++;
+    CK(cudaGetLastError());
+    std::vector<double> absorbed((size_t)B);
+    CK(cudaMemcpy(absorbed.data(), d_abs, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost));
+    // the constants: each call's part added to its range's sum, in call order
+    std::vector<double> k((size_t)B, 0.0);
+    const SparseHost& h = g->host;
+    for (size_t c = 0; c < h.const_node.size(); ++c) {
+        const int64_t b = (int64_t)(std::upper_bound(node_off, node_off + B + 1, (int64_t)h.const_node[c]) - node_off) - 1;
+        k[(size_t)b] += h.const_part[c];
+    }
+    for (int64_t b = 0; b < B; ++b) out[b] = k[(size_t)b] + absorbed[(size_t)b];
     return MGC_OK;
 }
 

@@ -26,6 +26,9 @@ struct SparseHost {
     bool indexed = true;                               // pair_of covers every pair
     std::vector<int32_t> olo, ohi;                     // per pair: node-local offsets of its arcs lo->hi and hi->lo
     std::vector<int32_t> deg;                          // arcs per node; empty while no offsets are recorded
+    bool log_const = false;                            // keep every add_tweights call's node and constant (segment energies)
+    std::vector<int32_t> const_node;
+    std::vector<double> const_part;
 
     explicit SparseHost(int64_t nodes = 0) : n(nodes), tr((size_t)nodes, 0.0) {}
 
@@ -163,8 +166,10 @@ struct SparseHost {
             double s = src[k], t = snk[k];
             const double delta = tr[v];
             if (delta > 0) s += delta; else t -= delta;
-            flow_const += (s < t) ? s : t;
+            const double part = (s < t) ? s : t;
+            flow_const += part;
             tr[v] = s - t;
+            if (log_const) { const_node.push_back((int32_t)v); const_part.push_back(part); }
         }
     }
 

@@ -31,6 +31,43 @@ _DEVICE_DTYPES = (numpy.float32, numpy.float64, numpy.uint8, numpy.int16, numpy.
 _DBL_MIN = sys.float_info.min
 
 
+def device_labels(label_image):
+    """The host-side checks of a label image and its int32 form the kernels read (the ids' consecutiveness is checked
+    on the device)."""
+    if label_image.ndim < 1 or label_image.ndim > 4:
+        raise ValueError("label images with 1 to 4 dimensions are supported, got {}".format(label_image.ndim))
+    if label_image.size == 0:
+        raise AttributeError("The supplied label image does either not contain any regions or they are not labeled "
+                             "consecutively starting from 1.")
+    dev = label_image
+    if dev.dtype != numpy.int32:
+        # the kernels read int32; anything else is converted once (ids that do not fit cannot be consecutive)
+        lo, hi = dev.min(), dev.max()
+        if lo < 1 or hi > numpy.iinfo(numpy.int32).max or (dev.dtype.kind == "f" and not (dev == numpy.floor(dev)).all()):
+            raise AttributeError("The supplied label image does either not contain any regions or they are not labeled "
+                                 "consecutively starting from 1.")
+        dev = dev.astype(numpy.int32)
+    elif any(s <= 0 and n > 1 for s, n in zip(dev.strides, dev.shape)):
+        dev = numpy.ascontiguousarray(dev)
+    return dev
+
+
+def device_values(array, shape, what):
+    """``array`` as an image of ``shape`` in a dtype the kernels read: the rule of ``LabelContext.values``."""
+    a = numpy.asarray(array)
+    if a.shape != shape:
+        raise ValueError("{} of shape {} does not match the label image of shape {}".format(what, a.shape, shape))
+    if not a.dtype.isnative:                       # '>f4', '>i2' (FITS / NIfTI readers): the kernels read native values
+        a = a.astype(a.dtype.newbyteorder("="))
+    if a.dtype == numpy.bool_:
+        a = a.view(numpy.uint8)
+    if a.dtype.type not in _DEVICE_DTYPES:
+        a = a.astype(numpy.float64)
+    if any(s <= 0 and n > 1 for s, n in zip(a.strides, a.shape)):
+        a = numpy.ascontiguousarray(a)
+    return a
+
+
 class LabelContext:
     """A label image resident on the device (``mgc_labels``): created once by ``graph_from_labels`` and shared by the
     terms and the marker step, or created on the fly when a term is called on its own."""
@@ -38,21 +75,7 @@ class LabelContext:
     def __init__(self, label_image, device=-1):
         label_image = numpy.asarray(label_image)
         self.source = label_image
-        if label_image.ndim < 1 or label_image.ndim > 4:
-            raise ValueError("label images with 1 to 4 dimensions are supported, got {}".format(label_image.ndim))
-        if label_image.size == 0:
-            raise AttributeError("The supplied label image does either not contain any regions or they are not labeled "
-                                 "consecutively starting from 1.")
-        dev = label_image
-        if dev.dtype != numpy.int32:
-            # the kernels read int32; anything else is converted once (ids that do not fit cannot be consecutive)
-            lo, hi = dev.min(), dev.max()
-            if lo < 1 or hi > numpy.iinfo(numpy.int32).max or (dev.dtype.kind == "f" and not (dev == numpy.floor(dev)).all()):
-                raise AttributeError("The supplied label image does either not contain any regions or they are not labeled "
-                                     "consecutively starting from 1.")
-            dev = dev.astype(numpy.int32)
-        elif any(s <= 0 and n > 1 for s, n in zip(dev.strides, dev.shape)):
-            dev = numpy.ascontiguousarray(dev)
+        dev = device_labels(label_image)
         from .. import _lib  # raises ImportError loudly when the extension is not built
         self._mgc = _lib._mgc
         self.native = _lib._mgc.LabelImage(dev, device)     # AttributeError unless the ids are exactly 1..K
@@ -62,18 +85,7 @@ class LabelContext:
     def values(self, array, what):
         """An image over the label image's shape in a dtype the kernels read (others are widened to float64, which is
         what the reference's arithmetic does to them anyway)."""
-        a = numpy.asarray(array)
-        if a.shape != self.shape:
-            raise ValueError("{} of shape {} does not match the label image of shape {}".format(what, a.shape, self.shape))
-        if not a.dtype.isnative:                       # '>f4', '>i2' (FITS / NIfTI readers): the kernels read native values
-            a = a.astype(a.dtype.newbyteorder("="))
-        if a.dtype == numpy.bool_:
-            a = a.view(numpy.uint8)
-        if a.dtype.type not in _DEVICE_DTYPES:
-            a = a.astype(numpy.float64)
-        if any(s <= 0 and n > 1 for s, n in zip(a.strides, a.shape)):
-            a = numpy.ascontiguousarray(a)
-        return a
+        return device_values(array, self.shape, what)
 
     def region_flags(self, markers):
         m = numpy.asarray(markers, dtype=numpy.bool_)
