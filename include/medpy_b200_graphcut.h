@@ -502,13 +502,17 @@ int mgc_sparse_remove_edges_warm(mgc_sparse* g, int64_t count, const int32_t* i,
                                  const double* rev_cap);
 /* Energies of a graph made of independent parts (DESIGN.md §8, "A batch of label images").
  * mgc_sparse_set_option(g, MGC_OPT_SEGMENT_ENERGIES, 1): before the first mgc_sparse_add_tweights and the first solve
- * since create or reset, and not on a warm handle (MGC_E_STATE otherwise); it survives mgc_sparse_reset.  The handle
- * then keeps every add_tweights call's contribution to the constant (12 B per call) and, after a solve, the flow each
- * node's sink link absorbed (8 B per node on the device).
+ * since create or reset (MGC_E_STATE otherwise); it survives mgc_sparse_reset and may be combined with MGC_OPT_WARM.  The
+ * handle then keeps the contribution to the constant of every add_tweights call made before the first solve (12 B per
+ * call) and, after a solve, the flow each node's sink link absorbed (8 B per node on the device).  On a warm handle the
+ * folds after the first solve also add each node's change of the constant into a per-node account (8 B per node more,
+ * counted in device_bytes; cleared by mgc_sparse_reset).
  * mgc_sparse_get_segment_energies(g, B, node_off, out): node_off[0..B] ascending from 0 to n splits the nodes into B
- * ranges; out[b] = the constant of the calls on nodes of range b, summed in call order, + the flow absorbed by those
- * nodes, summed in a fixed order (solves first if needed).  When no arc joins two ranges, out[b] is the energy the range
- * alone would have; mgc_sparse_maxflow keeps returning the total. */
+ * ranges; out[b] = the constant of the logged calls on nodes of range b, summed in call order, + on a warm handle the
+ * range's accounts, + the flow absorbed by those nodes in the current (resident) state; both device sums run in a fixed
+ * order with no atomics, so two reads give the same bits (solves first if needed).  When no arc joins two ranges, out[b]
+ * is the energy the range alone would have, and a range whose nodes no fold touched keeps its value bit for bit across
+ * warm re-solves; mgc_sparse_maxflow keeps returning the total. */
 #define MGC_OPT_SEGMENT_ENERGIES 4
 int mgc_sparse_get_segment_energies(mgc_sparse* g, int64_t B, const int64_t* node_off, double* out);
 
@@ -550,6 +554,11 @@ int mgc_labels_region_sums(mgc_labels* l, const mgc_array* values, int32_t mode,
 /* flags[r] = 1 if any voxel of region r+1 is marked (numpy.unique(label_image[markers] - 1), generate.py:334-337);
  * `markers` MGC_U8 over the same shape, flags = host array of K bytes. */
 int mgc_labels_region_flags(mgc_labels* l, const mgc_array* markers, uint8_t* flags);
+/* The flags of mgc_labels_region_flags from a list of marked voxels instead of a full marker image: flags[label[ids[t]]
+ * - 1] = 1 for t < count, ids = host int64 voxel indices in [0, voxels) (C order; on a batch handle indices into the
+ * concatenation), flags = host array of K bytes.  MGC_E_ARG for an id out of range, before any device work.  A stroke on
+ * one image of a large batch then moves its own voxel ids instead of a marker image of the whole batch. */
+int mgc_labels_voxel_flags(mgc_labels* l, int64_t count, const int64_t* ids, uint8_t* flags);
 /* out[p] = per_region[label[p] - 1]: maps the cut back onto the voxels (bin/medpy_graphcut_label.py:139-148).
  * per_region = host array of K bytes; out = C-contiguous uint8 over the shape in host or device memory. */
 int mgc_labels_apply(mgc_labels* l, const uint8_t* per_region, uint8_t* out, int32_t out_mem);

@@ -501,6 +501,14 @@ __global__ void __launch_bounds__(LAB_BLOCK) k_lab_region_flags(const int* __res
         if (markers[p]) flags[labels[p] - 1] = 1;
 }
 
+// the same flags from a list of marked voxels: one thread per id, flags[label[id] - 1] = 1
+__global__ void __launch_bounds__(LAB_BLOCK) k_lab_voxel_flags(const int* __restrict__ labels, const long long* __restrict__ ids, long long m,
+                                                               uint8_t* __restrict__ flags)
+{
+    for (long long t = (long long)blockIdx.x * LAB_BLOCK + threadIdx.x; t < m; t += (long long)gridDim.x * LAB_BLOCK)
+        flags[labels[ids[t]] - 1] = 1;
+}
+
 // out[p] = per_region[label[p] - 1]: the relabel_map step of bin/medpy_graphcut_label.py:139-148
 __global__ void __launch_bounds__(LAB_BLOCK) k_lab_apply(const int* __restrict__ labels, const uint8_t* __restrict__ per_region, long long n,
                                                          uint8_t* __restrict__ out)

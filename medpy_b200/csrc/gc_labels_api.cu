@@ -516,6 +516,29 @@ int mgc_labels_region_flags(mgc_labels* g, const mgc_array* markers, uint8_t* fl
     return MGC_OK;
 }
 
+int mgc_labels_voxel_flags(mgc_labels* g, int64_t count, const int64_t* ids, uint8_t* flags)
+{
+    if (!g || !flags || count < 0 || (count > 0 && !ids)) return MGC_E_ARG;
+    for (int64_t t = 0; t < count; ++t)
+        if (ids[t] < 0 || ids[t] >= g->G.n)
+            FAIL(MGC_E_ARG, "voxel id " + std::to_string(ids[t]) + " out of range: valid ids are 0 to " + std::to_string(g->G.n - 1));
+    CK(cudaSetDevice(g->device));
+    DevScope dev;
+    long long* d_ids;
+    uint8_t* d_flags;
+    CK(dev.alloc(&d_ids, (size_t)count));
+    CK(dev.alloc(&d_flags, (size_t)g->k));
+    if (count) CK(cudaMemcpy(d_ids, ids, (size_t)count * sizeof(long long), cudaMemcpyHostToDevice));
+    CK(cudaMemset(d_flags, 0, (size_t)g->k));
+    if (count) {
+        k_lab_voxel_flags<<<grid_for(count), LAB_BLOCK>>>(g->labels, d_ids, (long long)count, d_flags);
+        g->kernel_launches++;
+    }
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(flags, d_flags, (size_t)g->k, cudaMemcpyDeviceToHost));
+    return MGC_OK;
+}
+
 int mgc_labels_apply(mgc_labels* g, const uint8_t* per_region, uint8_t* out, int32_t out_mem)
 {
     if (!g || !per_region || !out) return MGC_E_ARG;

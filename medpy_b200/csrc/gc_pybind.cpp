@@ -793,6 +793,15 @@ public:
         check(rc);
         return flags;
     }
+    // flags over all regions from int64 voxel ids (C order over the image, or over a batch's concatenation)
+    py::array_t<uint8_t> voxel_flags(py::array_t<int64_t, py::array::c_style | py::array::forcecast> ids)
+    {
+        py::array_t<uint8_t> flags((py::ssize_t)region_count());
+        int rc;
+        { uint8_t* p = flags.mutable_data(); const int64_t* q = ids.data(); const int64_t m = (int64_t)ids.size(); py::gil_scoped_release rel; rc = mgc_labels_voxel_flags(l_, m, q, p); }
+        check(rc);
+        return flags;
+    }
     py::array_t<uint8_t> apply(py::array_t<uint8_t, py::array::c_style | py::array::forcecast> per_region)
     {
         if (per_region.size() != region_count()) throw py::value_error("one value per region expected");
@@ -869,6 +878,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("boundary", &PyLabels::boundary, py::arg("kind"), py::arg("values") = py::none(), py::arg("directedness") = 0.0)
         .def("region_sums", &PyLabels::region_sums)
         .def("region_flags", &PyLabels::region_flags)
+        .def("voxel_flags", &PyLabels::voxel_flags)
         .def("apply", &PyLabels::apply)
         .def_static("batch", &PyLabels::batch, py::arg("shapes"), py::arg("label_images"), py::arg("device") = -1)
         .def("batch_offsets", &PyLabels::batch_offsets)

@@ -26,11 +26,13 @@ namespace {
 thread_local std::string g_sp_create_error;
 
 // The device arrays of a solve: the push-relabel state, the loop's flag words, active-node count, mask and absorbed
-// flow, and on a warm handle `sent` and the edge fold's tail flags.
+// flow, on a warm handle `sent` and the edge fold's tail flags, and on a warm handle with segment energies each node's
+// account of the constant changes its folds made.
 struct SparseDev {
     int n = 0, m2 = 0;
     int *row = nullptr, *head = nullptr, *sis = nullptr, *height = nullptr, *flags = nullptr;
     double *cap = nullptr, *tr = nullptr, *excess = nullptr, *sunk = nullptr, *sent = nullptr, *abs = nullptr;
+    double* acct = nullptr;
     uint8_t *mask = nullptr, *tail = nullptr;
     unsigned long long* count = nullptr;
 
@@ -39,7 +41,7 @@ struct SparseDev {
     {
         if (e == cudaSuccess) e = cudaMalloc(&p, (count ? count : 1) * sizeof(T));
     }
-    cudaError_t alloc(int nodes, int arcs, bool warm)
+    cudaError_t alloc(int nodes, int arcs, bool warm, bool segments)
     {
         n = nodes;
         m2 = arcs;
@@ -48,11 +50,12 @@ struct SparseDev {
         get(e, tr, (size_t)n); get(e, excess, (size_t)n); get(e, sunk, (size_t)n); get(e, height, (size_t)n);
         get(e, mask, (size_t)n); get(e, flags, 2); get(e, abs, 1); get(e, count, 1);
         if (warm) { get(e, sent, (size_t)n); get(e, tail, (size_t)n); }
+        if (warm && segments) get(e, acct, (size_t)n);
         return e;
     }
     void release()
     {
-        void* ps[] = {row, head, sis, height, flags, cap, tr, excess, sunk, sent, abs, mask, tail, count};
+        void* ps[] = {row, head, sis, height, flags, cap, tr, excess, sunk, sent, abs, acct, mask, tail, count};
         for (void* p : ps)
             if (p) cudaFree(p);
         *this = SparseDev{};
@@ -98,7 +101,9 @@ struct mgc_sparse {
     bool warm_bad = false;                             // that solve's graph held a NaN or infinite capacity: no folds
     double wconst = 0.0;                               // constant of the resident state (energy = wconst + absorbed)
     SparseDev dev;                                     // a cold solve's arrays for the call, a warm one's until reset
-    // MGC_OPT_SEGMENT_ENERGIES: host.log_const is set, and every solve leaves its per-node absorbed flow in `seg_sunk`
+    // MGC_OPT_SEGMENT_ENERGIES: host.log_const is set, and every cold solve leaves its per-node absorbed flow in
+    // `seg_sunk`.  On a warm handle the log stops at the first solve (the calls after it fold into the resident state),
+    // the folds add each node's change of the constant into dev.acct and the absorbed flow is the resident dev.sunk.
     bool segments = false;
     bool tweights_added = false;                       // add_tweights was called since create / reset
     double* seg_sunk = nullptr;
@@ -174,7 +179,7 @@ int sparse_loop(mgc_sparse* g, const Events& ev, double base)
     g->st.active_last = active;
     g->st.flow_const = g->host.flow_const;
     g->st.energy = g->energy;
-    g->st.device_bytes = (int64_t)((size_t)S.m2 * 16 + (size_t)n * (g->warm ? 41 : 33));
+    g->st.device_bytes = (int64_t)((size_t)S.m2 * 16 + (size_t)n * (g->warm ? (g->segments ? 49 : 41) : 33));
     return MGC_OK;
 }
 
@@ -190,7 +195,7 @@ int sparse_first_solve(mgc_sparse* g)
     std::vector<double> cap;
     h.csr(row, head, sis, cap);
     SparseDev& d = g->dev;
-    CK(d.alloc(n, m2, g->warm));
+    CK(d.alloc(n, m2, g->warm, g->segments));
     CK(cudaMemcpy(d.row, row.data(), ((size_t)n + 1) * sizeof(int), cudaMemcpyHostToDevice));
     if (m2) {
         CK(cudaMemcpy(d.head, head.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
@@ -199,6 +204,7 @@ int sparse_first_solve(mgc_sparse* g)
     }
     CK(cudaMemcpy(d.tr, h.tr.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
     if (g->warm) CK(cudaMemset(d.tail, 0, (size_t)n));
+    if (d.acct) CK(cudaMemset(d.acct, 0, (size_t)n * sizeof(double)));
     Events ev;
     CK(ev.begin());
     const unsigned blocks = grid_for(n);
@@ -209,6 +215,7 @@ int sparse_first_solve(mgc_sparse* g)
     // warm: the state stays resident whether the loop converges or not; so do the pairs' arc offsets
     g->resident = true;
     g->wconst = h.flow_const;
+    g->host.log_const = false;                      // the log holds the constants of the state solved here, no later ones
     bool bad = false;
     for (int v = 0; v < n && !bad; ++v) bad = !std::isfinite(h.tr[(size_t)v]);
     for (int a = 0; a < m2 && !bad; ++a) bad = !std::isfinite(cap[(size_t)a]);
@@ -330,7 +337,8 @@ int warm_fold_tweights(mgc_sparse* g, int64_t count, const int32_t* nodes, const
     RC(warm_upload(g, dev, src, (size_t)count, &d_src));
     RC(warm_upload(g, dev, snk, (size_t)count, &d_snk));
     CK(dev.alloc(&partials, (size_t)nb));
-    k_spw_tlink_fold<<<(unsigned)nb, 256>>>(g->dev.warm(), ks, order, count, d_src, d_snk, partials);
+    if (g->dev.acct) k_spw_tlink_fold_seg<<<(unsigned)nb, 256>>>(g->dev.warm(), ks, order, count, d_src, d_snk, partials, g->dev.acct);
+    else             k_spw_tlink_fold<<<(unsigned)nb, 256>>>(g->dev.warm(), ks, order, count, d_src, d_snk, partials);
     g->st.kernel_launches++;
     double dk = 0.0;
     RC(warm_constant(g, dev, partials, nb, &dk));
@@ -430,7 +438,8 @@ int warm_fold_decrements(mgc_sparse* g, const SparseCalls& c)
     RC(warm_sort(g, dev, end_key, 2 * m, 0xffffffffu, &end_ks, &end_order));
     const long long nb = (2 * m + 255) / 256;
     CK(dev.alloc(&partials, (size_t)nb));
-    k_spw_ends<<<(unsigned)nb, 256>>>(W, end_ks, end_order, 2 * m, end_dx, partials);
+    if (g->dev.acct) k_spw_ends_seg<<<(unsigned)nb, 256>>>(W, end_ks, end_order, 2 * m, end_dx, partials, g->dev.acct);
+    else             k_spw_ends<<<(unsigned)nb, 256>>>(W, end_ks, end_order, 2 * m, end_dx, partials);
     g->st.kernel_launches++;
     double dk = 0.0;
     RC(warm_constant(g, dev, partials, nb, &dk));
@@ -514,13 +523,11 @@ int mgc_sparse_set_option(mgc_sparse* g, int32_t option, int64_t value)
         if (g->solved_once || g->resident || g->tweights_added)
             FAIL(MGC_E_STATE, "MGC_OPT_SEGMENT_ENERGIES must be set before the first add_tweights and maxflow(): reset() the "
                               "graph and rebuild it");
-        if (g->warm && value) FAIL(MGC_E_STATE, "segment energies are not kept on a warm graph");
         g->segments = value != 0;
         g->host.log_const = g->segments;
         return MGC_OK;
     }
     if (option != MGC_OPT_WARM) FAIL(MGC_E_ARG, "unknown option for a sparse graph");
-    if (value && g->segments) FAIL(MGC_E_STATE, "segment energies are not kept on a warm graph");
     if (g->solved_once || g->resident)
         FAIL(MGC_E_STATE, "MGC_OPT_WARM must be set before the first maxflow(): reset() the graph and rebuild it");
     g->warm = value != 0;
@@ -640,14 +647,20 @@ int mgc_sparse_get_segment_energies(mgc_sparse* g, int64_t B, const int64_t* nod
     long long* d_off;
     double* d_abs;
     CK(dev.alloc(&d_off, (size_t)B + 1));
-    CK(dev.alloc(&d_abs, (size_t)B));
+    CK(dev.alloc(&d_abs, (size_t)B * (g->resident ? 2 : 1)));
     CK(cudaMemcpy(d_off, node_off, ((size_t)B + 1) * sizeof(long long), cudaMemcpyHostToDevice));
     const long long cap = 32LL * cached_sm_count(g->device);
-    k_sp_segment_absorbed<<<(unsigned)(B < cap ? B : cap), 256>>>(g->seg_sunk, d_off, (long long)B, d_abs);
+    const unsigned grid = (unsigned)(B < cap ? B : cap);
+    // a resident handle: its absorbed flow is the resident state's, and its folds' constant changes are the accounts
+    k_sp_segment_absorbed<<<grid, 256>>>(g->resident ? g->dev.sunk : g->seg_sunk, d_off, (long long)B, d_abs);
     g->st.kernel_launches++;
+    if (g->resident) {
+        k_sp_segment_absorbed<<<grid, 256>>>(g->dev.acct, d_off, (long long)B, d_abs + B);
+        g->st.kernel_launches++;
+    }
     CK(cudaGetLastError());
-    std::vector<double> absorbed((size_t)B);
-    CK(cudaMemcpy(absorbed.data(), d_abs, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost));
+    std::vector<double> absorbed((size_t)B * (g->resident ? 2 : 1));
+    CK(cudaMemcpy(absorbed.data(), d_abs, absorbed.size() * sizeof(double), cudaMemcpyDeviceToHost));
     // the constants: each call's part added to its range's sum, in call order
     std::vector<double> k((size_t)B, 0.0);
     const SparseHost& h = g->host;
@@ -655,6 +668,8 @@ int mgc_sparse_get_segment_energies(mgc_sparse* g, int64_t B, const int64_t* nod
         const int64_t b = (int64_t)(std::upper_bound(node_off, node_off + B + 1, (int64_t)h.const_node[c]) - node_off) - 1;
         k[(size_t)b] += h.const_part[c];
     }
+    if (g->resident)
+        for (int64_t b = 0; b < B; ++b) k[(size_t)b] += absorbed[(size_t)(B + b)];
     for (int64_t b = 0; b < B; ++b) out[b] = k[(size_t)b] + absorbed[(size_t)b];
     return MGC_OK;
 }

@@ -11,6 +11,9 @@
 //     residual out-capacity;
 //   * spw_pair_dec / spw_excess_change: n-link decrements, flow beyond the new capacity cancelled, a node left short
 //     covered by the Kohli-Torr step.
+// On a handle with segment energies the two folds that change the constant (t-links, decrement ends) also keep each
+// node's change in a per-node account (the `_seg` kernels), so the energy stays split by node ranges (DESIGN.md §8,
+// "A batch of label images", "Warm edits").
 // Like gc_sparse.cuh the bodies are plain inline functions, so tests/emu/sparse_warm_emu.cpp runs them on the host.
 #pragma once
 #include "gc_sparse.cuh"
@@ -238,15 +241,35 @@ __device__ __forceinline__ long long spw_run_end(const unsigned* keys, long long
     return k;
 }
 
-// one thread per node with calls (the first of its run of sorted keys)
+// one thread per node with calls (the first of its run of sorted keys).  SEG: a handle with segment energies, which also
+// adds each node's change of the constant into its own account acct[v] (one thread per node: no atomics), so the
+// constant stays split by node ranges; false compiles the single-graph kernel, which has no account.
+template <bool SEG>
+__device__ __forceinline__ void spw_tlink_fold(const SparseWarm& W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
+                                               long long m, const double* __restrict__ src, const double* __restrict__ snk,
+                                               double* __restrict__ partials, double* __restrict__ acct)
+{
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    double dk = 0.0;
+    if (spw_is_head(keys, i, m)) {
+        dk = spw_tlink_node(W, (int)keys[i], order, i, spw_run_end(keys, i, m) - i, src, snk);
+        if constexpr (SEG) acct[keys[i]] += dk;
+    }
+    spw_block_sum(dk, partials);
+}
+
 __global__ void __launch_bounds__(256) k_spw_tlink_fold(SparseWarm W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
                                                         long long m, const double* __restrict__ src, const double* __restrict__ snk,
                                                         double* __restrict__ partials)
 {
-    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
-    double dk = 0.0;
-    if (spw_is_head(keys, i, m)) dk = spw_tlink_node(W, (int)keys[i], order, i, spw_run_end(keys, i, m) - i, src, snk);
-    spw_block_sum(dk, partials);
+    spw_tlink_fold<false>(W, keys, order, m, src, snk, partials, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_spw_tlink_fold_seg(SparseWarm W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
+                                                            long long m, const double* __restrict__ src, const double* __restrict__ snk,
+                                                            double* __restrict__ partials, double* __restrict__ acct)
+{
+    spw_tlink_fold<true>(W, keys, order, m, src, snk, partials, acct);
 }
 
 // CSR re-assembly: new degree per node, the exclusive scan as int row offsets, old arcs, new pairs
@@ -362,9 +385,12 @@ __global__ void __launch_bounds__(256) k_spw_pair_dec(SparseWarm W, const unsign
     end_dx[2 * i + 1] = eh;
 }
 
-// each end once, in ascending node order; its changes summed in the order of the (stable) sorted entries
-__global__ void __launch_bounds__(256) k_spw_ends(SparseWarm W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
-                                                  long long m, const double* __restrict__ dx, double* __restrict__ partials)
+// each end once, in ascending node order; its changes summed in the order of the (stable) sorted entries.  SEG: as in
+// spw_tlink_fold, the end's change of the constant also goes into its account
+template <bool SEG>
+__device__ __forceinline__ void spw_ends(const SparseWarm& W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
+                                         long long m, const double* __restrict__ dx, double* __restrict__ partials,
+                                         double* __restrict__ acct)
 {
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
     double dk = 0.0;
@@ -373,7 +399,21 @@ __global__ void __launch_bounds__(256) k_spw_ends(SparseWarm W, const unsigned* 
         double de = 0.0;
         for (long long k = i; k < end; ++k) de += dx[order[k]];
         dk = spw_excess_change(W, (int)keys[i], de);
+        if constexpr (SEG) acct[keys[i]] += dk;
     }
     spw_block_sum(dk, partials);
+}
+
+__global__ void __launch_bounds__(256) k_spw_ends(SparseWarm W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
+                                                  long long m, const double* __restrict__ dx, double* __restrict__ partials)
+{
+    spw_ends<false>(W, keys, order, m, dx, partials, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_spw_ends_seg(SparseWarm W, const unsigned* __restrict__ keys, const unsigned* __restrict__ order,
+                                                      long long m, const double* __restrict__ dx, double* __restrict__ partials,
+                                                      double* __restrict__ acct)
+{
+    spw_ends<true>(W, keys, order, m, dx, partials, acct);
 }
 #endif  // __CUDACC__

@@ -7,13 +7,18 @@ region-sum pass per term that needs one, one sparse solve and one voxel gather. 
 ``node_offsets[b] + r - 1``.  No arc joins two images, so every image is cut as its own ``graph_from_labels`` call would
 cut it: the same edge weights (bit for bit), the same t-links, the same mask; its energy is split off the union's by the
 solver (``mgc_sparse_get_segment_energies``).
+
+A batch built with ``warm=True`` keeps the solved state: seeds, t-links and edges added or lowered on the regions of one
+or more images fold into it, and the next ``maxflow()`` continues from the flow already routed.  Each image keeps its
+own energy through the folds, and an image that no edit touched keeps its mask and energy bit for bit.
 """
 import numpy
 
-from . import energy_label
+from . import _warm_args, energy_label
 from .energy_label import _DBL_MIN, device_labels, device_values
 from .graph import GCGraph
 from .maxflow import _termtype
+from .sparse import warm_ids, warm_pairs, warm_weights
 
 __all__ = ["graph_from_labels_batch", "LabelBatchGraph"]
 
@@ -106,7 +111,7 @@ class _Term:
 
 
 def graph_from_labels_batch(label_images, fg_markers, bg_markers, regional_term=False, boundary_term=False,
-                            regional_term_args=False, boundary_term_args=False):
+                            regional_term_args=False, boundary_term_args=False, *, warm=False):
     """``graph_from_labels`` for B label images at once, cut as one graph.
 
     ``label_images``, ``fg_markers`` and ``bg_markers`` are lists of B arrays (the images may differ in shape, not in
@@ -120,6 +125,10 @@ def graph_from_labels_batch(label_images, fg_markers, bg_markers, regional_term=
     Each image raises what its own ``graph_from_labels`` call would raise, naming its index; when several images fail,
     the host-side checks (label images, term inputs, marker shapes) come first, image by image, then the label ids, then
     the markers' region sets.  Returns a ``LabelBatchGraph``.
+
+    ``warm=True`` keeps the solved state for the warm edits of ``LabelBatchGraph`` (``add_seeds``, ``remove_seeds``,
+    ``add_tweights_warm``, ``add_nweights_warm``, ``remove_nweights_warm``), as ``graph_from_labels(..., warm=True)``
+    does for one image.
     """
     stacked = not isinstance(label_images, (list, tuple))
     labels = _per_image(label_images, None, "label_images")
@@ -160,6 +169,8 @@ def graph_from_labels_batch(label_images, fg_markers, bg_markers, regional_term=
     native = mgc.LabelImage.batch([list(s) for s in shapes], _concat(dev))   # AttributeError naming the image
     off = numpy.asarray(native.batch_offsets(), dtype=numpy.int64)
     graph = mgc.SparseGraph(int(off[-1]))
+    if warm:
+        graph.set_option(mgc.OPT_WARM, 1)
     graph.set_option(mgc.OPT_SEGMENT_ENERGIES, 1)
     for t in terms:                                               # regional term, then boundary term
         t.apply(mgc, native, graph, off)
@@ -172,20 +183,33 @@ def graph_from_labels_batch(label_images, fg_markers, bg_markers, regional_term=
     for f, src, snk in ((flags[0], GCGraph.MAX, 0.0), (flags[1], 0.0, GCGraph.MAX)):
         ids = numpy.nonzero(f)[0].astype(numpy.int32)
         graph.add_tweights(ids, numpy.full(ids.size, float(src)), numpy.full(ids.size, float(snk)))
-    return LabelBatchGraph(native, graph, off, shapes, stacked)
+    return LabelBatchGraph(native, graph, off, shapes, stacked, warm)
 
 
 class LabelBatchGraph:
-    """The solved union of a batch's region graphs (what ``graph_from_labels_batch`` returns)."""
+    """The solved union of a batch's region graphs (what ``graph_from_labels_batch`` returns).
+
+    On a batch built with ``warm=True`` the warm methods take node ids over the union (region r of image b is node
+    ``node_offsets[b] + r - 1``) or a boolean mask over all ``node_offsets[-1]`` regions, with the arguments, checks and
+    errors of ``SparseGraphDouble``'s warm calls; ``region_flags`` turns strokes drawn on the images into such a mask.
+    A pair whose ends lie in two images raises ``ValueError``.  Every refusal comes before any native call, so the
+    batch is unchanged."""
 
     termtype = _termtype
 
-    def __init__(self, native_labels, graph, node_offsets, shapes, stacked):
+    def __init__(self, native_labels, graph, node_offsets, shapes, stacked, warm=False):
         self._labels = native_labels
         self._graph = graph
         self._off = node_offsets
         self._shapes = [tuple(s) for s in shapes]
         self._stacked = stacked
+        self._warm = bool(warm)
+        self._vox_off = numpy.concatenate([[0], numpy.cumsum([int(numpy.prod(s)) for s in self._shapes])]).astype(numpy.int64)
+
+    @property
+    def warm(self):
+        """Whether the batch keeps its solved state for warm edits (``graph_from_labels_batch(..., warm=True)``)."""
+        return self._warm
 
     @property
     def node_offsets(self):
@@ -218,3 +242,90 @@ class LabelBatchGraph:
         d = dict(self._graph.stats())
         d["images"] = len(self._shapes)
         return d
+
+    def region_flags(self, strokes):
+        """bool[node_offsets[-1]]: True for every region of the union that holds a marked voxel.  ``strokes`` has one
+        entry per image, ``None`` or a mask of that image's shape (a numpy array or a CUDA tensor), as a list or stacked
+        along a first axis.  Only the marked voxels of the given images go to the device, as ids."""
+        items = list(strokes)
+        if len(items) != len(self._shapes):
+            raise ValueError("strokes: {} entries for a batch of {} label images".format(len(items), len(self._shapes)))
+        ids = [numpy.zeros(0, numpy.int64)]
+        for b, m in enumerate(items):
+            if m is None:
+                continue
+            if _warm_args.on_device(m):
+                import torch
+                m = torch.as_tensor(m)
+                shape = tuple(m.shape)
+            else:
+                m = numpy.asarray(m, dtype=numpy.bool_)
+                shape = m.shape
+            if shape != self._shapes[b]:
+                raise IndexError("label image {}: boolean index did not match the label image: stroke shape {} vs "
+                                 "{}".format(b, shape, self._shapes[b]))
+            v = numpy.flatnonzero(m) if isinstance(m, numpy.ndarray) else m.reshape(-1).nonzero().reshape(-1).cpu().numpy()
+            ids.append(v.astype(numpy.int64) + self._vox_off[b])
+        return self._labels.voxel_flags(numpy.concatenate(ids)).view(numpy.bool_)
+
+    # ------------------------------------------------------------------ warm edits (batches built with warm=True)
+    def _require_warm(self, what):
+        if not self._warm:
+            raise RuntimeError("{} needs a label batch built with warm=True; rebuild it with "
+                               "graph_from_labels_batch(..., warm=True) instead".format(what))
+
+    def add_seeds(self, fg=None, bg=None):
+        """add_tweights(v, 65535, 0) per foreground id in order, then add_tweights(v, 0, 65535) per background id."""
+        self._require_warm("add_seeds")
+        self._seed_calls(fg, bg, 65535.0)
+
+    def remove_seeds(self, fg=None, bg=None):
+        """The inverse of add_seeds: add_tweights(v, -65535, 0) / add_tweights(v, 0, -65535)."""
+        self._require_warm("remove_seeds")
+        self._seed_calls(fg, bg, -65535.0)
+
+    def _seed_calls(self, fg, bg, cap):
+        n = int(self._off[-1])
+        ids = [None if x is None else warm_ids(x, n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
+        for v, src, snk in ((ids[0], cap, 0.0), (ids[1], 0.0, cap)):
+            if v is not None and v.size:
+                self._graph.add_tweights(v, numpy.full(v.size, src), numpy.full(v.size, snk))
+
+    def add_tweights_warm(self, nodes, cap_source, cap_sink):
+        """add_tweights(nodes[k], cap_source[k], cap_sink[k]) per entry in order; nodes None: one call per node."""
+        self._require_warm("add_tweights_warm")
+        n = int(self._off[-1])
+        ids = None if nodes is None else warm_ids(nodes, n, "nodes")
+        m = n if ids is None else ids.size
+        src, snk = warm_weights(cap_source, m, "cap_source"), warm_weights(cap_sink, m, "cap_sink")
+        if m:
+            self._graph.add_tweights(ids, src, snk)
+
+    def _pairs(self, i, j, cap, rev_cap, why):
+        """warm_pairs over the union; a pair across two images is refused (no arc may join them, or the energy split
+        would be meaningless)."""
+        ii, jj, c, r = warm_pairs(i, j, cap, rev_cap, int(self._off[-1]), why)
+        bi = numpy.searchsorted(self._off, ii, side="right") - 1
+        bj = numpy.searchsorted(self._off, jj, side="right") - 1
+        cross = numpy.flatnonzero(bi != bj)
+        if cross.size:
+            k = cross[0]
+            raise ValueError("the pair ({}, {}) joins label image {} and label image {}: an edge must stay inside one "
+                             "image".format(ii[k], jj[k], bi[k], bj[k]))
+        return ii, jj, c, r
+
+    def add_nweights_warm(self, i, j, cap, rev_cap):
+        """sum_edge(i[k], j[k], cap[k], rev_cap[k]) per entry in order, on any pairs inside one image (new ones
+        included)."""
+        self._require_warm("add_nweights_warm")
+        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, _warm_args.ONLY_RAISES)
+        if ii.size:
+            self._graph.sum_edges(ii, jj, c, r)
+
+    def remove_nweights_warm(self, i, j, cap, rev_cap):
+        """sum_edge(i[k], j[k], -cap[k], -rev_cap[k]) per entry in order on existing pairs.  A pair whose decrements
+        exceed what it holds (beyond a few hundred roundings) raises ValueError with the batch unchanged."""
+        self._require_warm("remove_nweights_warm")
+        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, _warm_args.DECREMENTS)
+        if ii.size:
+            self._graph.remove_edges_warm(ii, jj, c, r)

@@ -34,6 +34,36 @@ def _host(x):
 _LOWER = "a solved graph lowers capacities only through remove_nweights_warm"
 
 
+def warm_ids(x, n, what):
+    """Node ids of one warm-call argument on a graph of n nodes, as host int32: a boolean mask of shape (n,), a 1-D
+    integer id array or a single id."""
+    a = numpy.asarray(_host(x))
+    if a.ndim == 0 and a.dtype != numpy.bool_:
+        a = a.reshape(1)
+    return _warm_args.node_ids(a, (n,), n, what).astype(numpy.int32)
+
+
+def warm_weights(w, m, what):
+    """One weight argument of a warm call as m finite host float64 values."""
+    w = _warm_args.weights(_host(w), m, what)
+    _warm_args.check_finite(w, what)
+    return w
+
+
+def warm_pairs(i, j, cap, rev_cap, n, why):
+    """The sum_edge calls of an n-link edit on a graph of n nodes as host arrays.  Unlike on the lattice, a one-element
+    id array broadcasts to the length of the longest argument."""
+    ii, jj = warm_ids(i, n, "i"), warm_ids(j, n, "j")
+    cap, rev_cap = _host(cap), _host(rev_cap)
+    m = max(ii.size, jj.size, *(numpy.size(w) for w in (cap, rev_cap) if numpy.ndim(w)))
+    ii, jj = (numpy.repeat(x, m) if x.size == 1 else x for x in (ii, jj))
+    ii, jj, c, r = _warm_args.nlink_calls(ii, jj, cap, rev_cap)
+    _warm_args.check_amounts(((c, "cap"), (r, "rev_cap")), why)
+    if (ii == jj).any():
+        raise ValueError("invalid node ids in the edge arrays")
+    return ii, jj, c, r
+
+
 class SparseGraphDouble:
     """``GraphDouble(node_num_max, edge_num_max)`` for arbitrary node pairs."""
 
@@ -215,19 +245,6 @@ class SparseGraphDouble:
             raise RuntimeError("{} needs a sparse graph created with warm=True; reset() the graph and rebuild it "
                                "instead".format(what))
 
-    def _ids(self, x, what):
-        """Node ids of one warm-call argument as host int32: a boolean mask of shape (n,), a 1-D integer id array or a
-        single id."""
-        a = numpy.asarray(_host(x))
-        if a.ndim == 0 and a.dtype != numpy.bool_:
-            a = a.reshape(1)
-        return _warm_args.node_ids(a, (self._n,), self._n, what).astype(numpy.int32)
-
-    def _weights(self, w, m, what):
-        w = _warm_args.weights(_host(w), m, what)
-        _warm_args.check_finite(w, what)
-        return w
-
     def add_seeds(self, fg=None, bg=None):
         """add_tweights(v, 65535, 0) per foreground id in order, then add_tweights(v, 0, 65535) per background id."""
         self._require_warm("add_seeds")
@@ -239,7 +256,7 @@ class SparseGraphDouble:
         self._seed_calls(fg, bg, -65535.0)
 
     def _seed_calls(self, fg, bg, cap):
-        ids = [None if x is None else self._ids(x, what) for x, what in ((fg, "fg"), (bg, "bg"))]
+        ids = [None if x is None else warm_ids(x, self._n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
         for v, src, snk in ((ids[0], cap, 0.0), (ids[1], 0.0, cap)):
             if v is not None and v.size:
                 self.add_tweights_bulk(v, numpy.full(v.size, src), numpy.full(v.size, snk))
@@ -247,27 +264,14 @@ class SparseGraphDouble:
     def add_tweights_warm(self, nodes, cap_source, cap_sink):
         """add_tweights(nodes[k], cap_source[k], cap_sink[k]) per entry in order; nodes None: one call per node."""
         self._require_warm("add_tweights_warm")
-        ids = None if nodes is None else self._ids(nodes, "nodes")
+        ids = None if nodes is None else warm_ids(nodes, self._n, "nodes")
         m = self._n if ids is None else ids.size
-        self.add_tweights_bulk(ids, self._weights(cap_source, m, "cap_source"), self._weights(cap_sink, m, "cap_sink"))
-
-    def _pairs(self, i, j, cap, rev_cap, why):
-        """The sum_edge calls of an n-link edit as host arrays.  Unlike on the lattice, a one-element id array broadcasts
-        to the length of the longest argument."""
-        ii, jj = self._ids(i, "i"), self._ids(j, "j")
-        cap, rev_cap = _host(cap), _host(rev_cap)
-        m = max(ii.size, jj.size, *(numpy.size(w) for w in (cap, rev_cap) if numpy.ndim(w)))
-        ii, jj = (numpy.repeat(x, m) if x.size == 1 else x for x in (ii, jj))
-        ii, jj, c, r = _warm_args.nlink_calls(ii, jj, cap, rev_cap)
-        _warm_args.check_amounts(((c, "cap"), (r, "rev_cap")), why)
-        if (ii == jj).any():
-            raise ValueError("invalid node ids in the edge arrays")
-        return ii, jj, c, r
+        self.add_tweights_bulk(ids, warm_weights(cap_source, m, "cap_source"), warm_weights(cap_sink, m, "cap_sink"))
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
         """sum_edge(i[k], j[k], cap[k], rev_cap[k]) per entry in order, on any node pairs (new ones included)."""
         self._require_warm("add_nweights_warm")
-        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, _warm_args.ONLY_RAISES)
+        ii, jj, c, r = warm_pairs(i, j, cap, rev_cap, self._n, _warm_args.ONLY_RAISES)
         if ii.size:
             self.sum_edges_bulk(ii, jj, c, r)
 
@@ -276,7 +280,7 @@ class SparseGraphDouble:
         capacity.  What is staged is folded first, so the call order is kept.  A pair whose decrements exceed what it
         holds (beyond a few hundred roundings) raises ValueError with the graph unchanged."""
         self._require_warm("remove_nweights_warm")
-        ii, jj, c, r = self._pairs(i, j, cap, rev_cap, _warm_args.DECREMENTS)
+        ii, jj, c, r = warm_pairs(i, j, cap, rev_cap, self._n, _warm_args.DECREMENTS)
         self._flush()
         self._mask = None
         if ii.size:
