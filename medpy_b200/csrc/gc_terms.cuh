@@ -10,6 +10,7 @@
 #pragma once
 #include "gc_common.cuh"
 #include "gc_exprange.cuh"
+#include "gc_expneg.cuh"
 #include <cfloat>
 
 // ---------------------------------------------------------------------------------------------------
@@ -84,7 +85,13 @@ __global__ void __launch_bounds__(256) k_gather_fortran3(int Z, int Y, int X, co
 // ---------------------------------------------------------------------------------------------------
 // K0: global min / max (difference_linear: |max - min| in the input dtype, energy_voxel.py:174;
 //     maximum_linear: max |x| in the input dtype, energy_voxel.py:99)
+// A NaN anywhere makes min, max and max |x| NaN, as numpy's min / max do, whatever cell, thread or block it falls in: the
+// folds below keep a NaN once they have met one (x < NaN is false) and take the other operand when it is NaN.  For the
+// integer types x != x is false and the folds are the plain ones.
 // ---------------------------------------------------------------------------------------------------
+template <typename E> __device__ __forceinline__ E min_nan(E acc, E x) { return (x < acc || x != x) ? x : acc; }
+template <typename E> __device__ __forceinline__ E max_nan(E acc, E x) { return (x > acc || x != x) ? x : acc; }
+
 template <typename E>
 __global__ void k_minmax_partial(const E* __restrict__ img, unsigned n, E* __restrict__ pmin, E* __restrict__ pmax,
                                  E* __restrict__ pabs)
@@ -97,17 +104,17 @@ __global__ void k_minmax_partial(const E* __restrict__ img, unsigned n, E* __res
     for (; i < n; i += step) {
         E x = img[i];
         E a = Elem<E>::absv(x);
-        lo = x < lo ? x : lo;
-        hi = x > hi ? x : hi;
-        ab = a > ab ? a : ab;
+        lo = min_nan(lo, x);
+        hi = max_nan(hi, x);
+        ab = max_nan(ab, a);
     }
     smin[tid] = lo; smax[tid] = hi; sabs[tid] = ab;
     __syncthreads();
     for (unsigned s = 128; s > 0; s >>= 1) {
         if (tid < s) {
-            smin[tid] = smin[tid + s] < smin[tid] ? smin[tid + s] : smin[tid];
-            smax[tid] = smax[tid + s] > smax[tid] ? smax[tid + s] : smax[tid];
-            sabs[tid] = sabs[tid + s] > sabs[tid] ? sabs[tid + s] : sabs[tid];
+            smin[tid] = min_nan(smin[tid], smin[tid + s]);
+            smax[tid] = max_nan(smax[tid], smax[tid + s]);
+            sabs[tid] = max_nan(sabs[tid], sabs[tid + s]);
         }
         __syncthreads();
     }
@@ -121,9 +128,9 @@ __global__ void k_minmax_final(const E* pmin, const E* pmax, const E* pabs, unsi
     if (threadIdx.x || blockIdx.x) return;
     E lo = pmin[0], hi = pmax[0], ab = pabs[0];
     for (unsigned i = 1; i < nb; ++i) {
-        lo = pmin[i] < lo ? pmin[i] : lo;
-        hi = pmax[i] > hi ? pmax[i] : hi;
-        ab = pabs[i] > ab ? pabs[i] : ab;
+        lo = min_nan(lo, pmin[i]);
+        hi = max_nan(hi, pmax[i]);
+        ab = max_nan(ab, pabs[i]);
     }
     E diff = (E)(hi - lo);            // in the input dtype, like numpy (wraps for narrow ints)
     diff = Elem<E>::absv(diff);
@@ -172,51 +179,7 @@ __device__ __forceinline__ double range_inv_sigma2(const BoundaryParams& P, cons
     return exp_table_inv_max(P.ktab, image_of(L, z_lo), image_of(L, z_hi));
 }
 
-// exp(-t) for t >= 0 in ~25 instructions (CUDA's general exp() costs ~80 here, and K1 is bound by instruction issue):
-// n = rint(-t*log2 e), r = -t - n*ln2 (two-step, exact product with the hi part), e^r by a degree-13 Taylor polynomial in
-// Horner form (|r| <= 0.347: truncation 4e-18), result scaled by 2^n through the exponent field.  <= 1 ulp from the
-// correctly rounded value on [0, 708]; the (rare) subnormal range goes through ldexp; t > 745.2 gives 0 like exp does
-// (the caller turns 0 into DBL_MIN, energy_voxel.py:235), NaN propagates.
-__constant__ double EXPN_C[14] = {
-    1.0, 1.0, 0.5, 1.6666666666666666e-01, 4.1666666666666664e-02, 8.3333333333333332e-03, 1.3888888888888889e-03,
-    1.9841269841269841e-04, 2.4801587301587302e-05, 2.7557319223985893e-06, 2.7557319223985888e-07,
-    2.5052108385441720e-08, 2.0876756987868100e-09, 1.6059043836821613e-10};
-
-__device__ __forceinline__ double exp_neg(double t)
-{
-    // branch-free: the three independent evaluations a voxel needs (+z, +y, +x pair) can be interleaved by the scheduler,
-    // which hides the latency of the dependent DFMA chain.  Out-of-range arguments are computed on a clamped value and
-    // selected away at the end.
-    const double y = fmax(-t, -800.0);                       // NaN -> -800 here, restored by the last select
-    const double n = rint(__dmul_rn(y, 1.4426950408889634));
-    double r = __fma_rn(-n, 6.93147180369123816490e-01, y);
-    r = __fma_rn(-n, 1.90821492927058770002e-10, r);
-    double p = EXPN_C[13];
-#pragma unroll
-    for (int k = 12; k >= 0; --k) p = __fma_rn(p, r, EXPN_C[k]);
-    const int ni = (int)n;
-    const bool tiny = ni < -1020;                             // result (nearly) subnormal: scale in two exact/rounded-once steps
-    const unsigned adj = (unsigned)(tiny ? ni + 64 : ni);
-    double res = __hiloint2double((int)((unsigned)__double2hiint(p) + (adj << 20)), __double2loint(p));
-    res = __dmul_rn(res, tiny ? 5.42101086242752217004e-20 : 1.0);     // 2^-64: one rounding, like ldexp
-    res = (t <= 745.2) ? res : 0.0;
-    return (t != t) ? t : res;
-}
-
-// The same function for arguments known to lie in [0, 700] (no NaN): none of the range handling, bit-identical results
-// (y = -t needs no clamp, n >= -1010 keeps the scaled result normal, so the exponent-field add is exact and the result is
-// positive -- no DBL_MIN clamp either).  Callers establish the range for the whole warp with one vote.
-__device__ __forceinline__ double exp_neg_inrange(double t)
-{
-    const double y = -t;
-    const double n = rint(__dmul_rn(y, 1.4426950408889634));
-    double r = __fma_rn(-n, 6.93147180369123816490e-01, y);
-    r = __fma_rn(-n, 1.90821492927058770002e-10, r);
-    double p = EXPN_C[13];
-#pragma unroll
-    for (int k = 12; k >= 0; --k) p = __fma_rn(p, r, EXPN_C[k]);
-    return __hiloint2double(__double2hiint(p) + ((int)n << 20), __double2loint(p));
-}
+// exp_neg / exp_neg_inrange: gc_expneg.cuh
 
 // argument of the exponential term, exactly as g_weight<1> forms it (gc_exprange.cuh)
 __device__ __forceinline__ double exp_term_arg(const BoundaryParams& P, double x)

@@ -18,6 +18,8 @@ followed by ``/ spacing[axis]`` when a spacing is given (:657-658).  Reference q
 ``boundary_maximum_division`` evaluates the *difference* form (:347), the linear normaliser M is formed in the
 image's own dtype (:99, :174), and the two linear terms take a 2-tuple, the others a 3-tuple.
 """
+import math
+
 import numpy
 
 __all__ = [
@@ -75,6 +77,8 @@ def _boundary(graph, kind, image, sigma, spacing):
             norm = float(numpy.abs(image).max())
         elif kind == _DIFF_LINEAR:
             norm = float(abs(image.max() - image.min()))
+    if kind in (_DIFF_EXP, _MAX_EXP) and sigma is not None:
+        math.pow(sigma, 2)      # the reference's sigma^2 (energy_voxel.py:232, :296): OverflowError for |sigma| > ~1.3e154
     dev = _device_image(image)
     if kind in (_MAX_LINEAR, _MAX_EXP, _MAX_POW) and dev.dtype != image.dtype:
         dev = numpy.abs(image).astype(numpy.float64)  # numpy.abs in the input dtype first (energy_voxel.py:558)

@@ -150,13 +150,14 @@ def test_borrowed_copied_and_eager_builds_agree(case):
     for mode in ("copied", "eager"):
         for x, y in zip(res["borrowed"][0], res[mode][0]):
             assert numpy.array_equal(x, y)
-    # bit for bit where the solve itself repeats bit for bit (the cross-tile flow of a hard instance, e.g. the boundary
-    # term alone, may be summed in another order from run to run)
-    repeatable = all(float(x[0]).hex() == float(y[0]).hex() for x, y in zip(res["borrowed"][1], res["borrowed_again"][1]))
-    (_identical if repeatable else _close)(res["borrowed"][1], res["copied"][1])
+    # bit for bit where the solve itself repeats bit for bit.  The warm re-solves of a hard instance (the boundary term
+    # alone) move cross-tile flow in an order that varies from run to run, so their energies may differ in the last bit
+    # between any two runs, two of the same mode included: one pair of runs that happens to agree does not make a third
+    # agree, and there every mode is held to rounding instead.
+    same = _close if case == "boundary_only" else _identical
+    same(res["borrowed"][1], res["borrowed_again"][1])
+    same(res["borrowed"][1], res["copied"][1])
     _close(res["borrowed"][1], res["eager"][1])
-    if case != "boundary_only":
-        assert repeatable
 
 
 @pytest.mark.parametrize("how", ["host_chunked", "host_unchunked", "strided_device"])

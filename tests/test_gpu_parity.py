@@ -5,7 +5,8 @@ duality evaluated independently with the oracle's weights).
 
 Tolerances: integer / byte / index results bit-exact (masks, integer-capacity energies, t-links, the linear
 and division weights); float64 energies within 1e-9 relative (north star allows 1e-5); exp / pow weights
-within 4 ulp of numpy's libm.
+within 2e-13 relative of numpy's (the exponential's argument is formed with the reciprocal of sigma^2, which moves it by
+a few ulp; test_gpu_boundary_domain.py bounds every weight from the arithmetic instead, over the whole domain).
 """
 import ctypes
 import os
@@ -591,3 +592,58 @@ def test_gradient_magnitude_prewitt_equals_scipy(shape, dtype):
     assert numpy.array_equal(got, want), float(numpy.abs(got - want).max())
     # Fortran-ordered input (as medpy.io.load returns) gives the same logical result
     assert numpy.array_equal(gradient_magnitude_prewitt(numpy.asfortranarray(img)), want)
+
+
+def _prewitt_cases():
+    """(name, image): uint8, int32 and float64 in 3-D and 4-D; extents 1, 2 and 3 on every axis; NaN, +-inf, -0 and
+    subnormal cells; bool, uint16 and int64 (widened by the binding)."""
+    rng = numpy.random.default_rng(77)
+    cases = []
+    for dtype in (numpy.uint8, numpy.int32, numpy.float64):
+        for shape in ((7, 9, 11), (5, 4, 6, 3)):
+            if dtype == numpy.uint8:
+                img = rng.integers(0, 256, shape).astype(dtype)
+            elif dtype == numpy.int32:
+                img = rng.integers(-2 ** 31, 2 ** 31 - 1, shape, endpoint=True).astype(dtype)
+            else:
+                img = rng.normal(0.0, 1e3, shape)
+            cases.append(("%s_%dd" % (numpy.dtype(dtype).name, len(shape)), img))
+    for ext in (1, 2, 3):
+        for nd in (1, 2, 3, 4):
+            for ax in range(nd):
+                shape = [4] * nd
+                shape[ax] = ext
+                cases.append(("ext%d_axis%d_of_%dd" % (ext, ax, nd), (rng.normal(size=shape) * 50).astype(numpy.float32)))
+        cases.append(("ext%d_all_3d" % ext, (rng.normal(size=(ext, ext, ext)) * 50).astype(numpy.float32)))
+    for dtype in (numpy.float32, numpy.float64):
+        img = (rng.normal(size=(6, 7, 8)) * 50).astype(dtype)
+        tiny = numpy.finfo(dtype).smallest_subnormal
+        flat = img.reshape(-1)
+        flat[[3, 60, 61, 200, 250]] = numpy.array([numpy.nan, numpy.inf, -numpy.inf, -0.0, tiny], dtype=dtype)
+        flat[300:310] = numpy.array([tiny, -tiny, 3 * tiny, numpy.finfo(dtype).tiny, -0.0] * 2, dtype=dtype)
+        cases.append(("specials_" + numpy.dtype(dtype).name, img))
+        sub = (rng.normal(size=(5, 6, 7)) * 100 * tiny).astype(dtype)       # every cell subnormal
+        cases.append(("all_subnormal_" + numpy.dtype(dtype).name, sub))
+    cases.append(("bool", rng.random((6, 7, 9)) < 0.4))
+    cases.append(("uint16", rng.integers(0, 65536, (6, 7, 9)).astype(numpy.uint16)))
+    cases.append(("int64", rng.integers(-2 ** 40, 2 ** 40, (6, 7, 9)).astype(numpy.int64)))
+    cases.append(("int64_4d", rng.integers(-1000, 1000, (3, 4, 5, 2)).astype(numpy.int64)))
+    return cases
+
+
+_PREWITT = _prewitt_cases()
+
+
+@pytest.mark.parametrize("case", range(len(_PREWITT)), ids=[c[0] for c in _PREWITT])
+def test_gradient_magnitude_prewitt_domain(case):
+    """The Prewitt gradient magnitude against scipy bit for bit (NaN where scipy has NaN) over dtypes, dimensions,
+    extents 1 to 3 (where mode 'reflect' folds both neighbours onto the cell or onto each other) and special cells."""
+    import scipy.ndimage as ndi
+    from medpy_b200.gradient import gradient_magnitude_prewitt
+    _, img = _PREWITT[case]
+    want = numpy.zeros(img.shape, dtype=numpy.float32)
+    with numpy.errstate(all="ignore"):
+        ndi.generic_gradient_magnitude(img, ndi.prewitt, output=want)
+    got = gradient_magnitude_prewitt(img)
+    assert got.dtype == numpy.float32 and got.shape == img.shape
+    assert numpy.array_equal(got, want, equal_nan=True), numpy.flatnonzero(~((got == want) | (numpy.isnan(got) & numpy.isnan(want))))[:8]
