@@ -373,6 +373,7 @@ def graphcut_slab(fg_markers, bg_markers, image=None, boundary=None, sigma=None,
     is assembled on every rank (all_gather of the slabs), otherwise only the rank's own planes are returned."""
     import torch
     import torch.distributed as dist
+    from .graphcut.energy_voxel import _device_products
     shape = tuple(fg_markers.shape)
     s = SlabSolver(shape, group=group, handle_factory=handle_factory)
     if boundary is not None and boundary.endswith("linear") and (isinstance(norm, float) and math.isnan(norm)):
@@ -380,7 +381,7 @@ def graphcut_slab(fg_markers, bg_markers, image=None, boundary=None, sigma=None,
     s.build(s.local_slice(fg_markers), s.local_slice(bg_markers),
             image_local=s.local_slice(image) if boundary is not None else None, kind=boundary, sigma=sigma, spacing=spacing,
             prob_local=s.local_slice(prob) if prob is not None else None, alpha=alpha, norm=norm,
-            compute_f32=prob is not None and "float32" in str(prob.dtype))
+            compute_f32=prob is not None and _device_products(prob, alpha))
     s.solve()
     energy = s.energy()
     own = s.mask()

@@ -14,7 +14,7 @@ import numpy
 
 from . import _warm_args
 from .device import _KINDS, _as_u8
-from .energy_voxel import _device_image, _native_order
+from .energy_voxel import _device_image, _device_products, _exact_as_float64, _native_order, _regional_products
 
 # the lattice index of one handle is 32-bit: batch x voxels per image must stay below this
 INDEX_LIMIT = 1 << 31
@@ -70,21 +70,23 @@ def _host_image(image, boundary):
 def _prob_arg(prob, alpha):
     """The probability map as the fused build reads it, and whether its products are float32, decided as
     ``energy_voxel.regional_probability_map`` decides them for one image: the map in native byte order, float32 products
-    where numpy forms them in float32 (a float32 map times a Python float).  Integer maps give float64 products, which a
-    float64 copy gives exactly; other dtypes (float16) have products the build cannot form."""
+    where numpy forms them in float32 (a float32 map times a Python float), float64 products where numpy forms them in
+    float64 from a float64 map.  An integer or bool map whose products numpy forms exactly in float64 goes as a float64
+    copy.
+    Every other map has products the build cannot form, and is refused: float16 maps, a float32 map with a
+    ``numpy.float64`` alpha (numpy rounds ``1 - p`` in float32, then multiplies in float64), and integer maps where
+    ``1 - p`` wraps around in the map's dtype (an unsigned map holding 2 or more, a signed map within 1 of its minimum)."""
     if _is_cuda(prob):
-        kind = str(prob.dtype)
-        if "float32" not in kind and "float64" not in kind:
-            raise ValueError(f"a batch's probability map must be float32 or float64, got {prob.dtype}")
-        return prob, "float32" in kind
+        return prob, _device_products(prob, alpha, "a batch's")
     prob = _native_order(numpy.asarray(prob))
-    src_dtype = (prob[:0] * alpha).dtype
-    snk_dtype = ((1 - prob[:0]) * alpha).dtype
-    if prob.dtype == numpy.float32 or prob.dtype == numpy.float64:
-        return prob, bool(prob.dtype == numpy.float32 and src_dtype == numpy.float32 and snk_dtype == numpy.float32)
-    if src_dtype == numpy.float64 and snk_dtype == numpy.float64:
+    mode = _regional_products(prob.dtype, alpha)
+    if mode is not None:
+        return prob, mode == "f32"
+    if _exact_as_float64(prob, alpha):
         return prob.astype(numpy.float64), False
-    raise ValueError(f"a batch's probability map must give float32 or float64 products, got {prob.dtype}")
+    raise ValueError(f"the products of a {prob.dtype} probability map with a {type(alpha).__name__} alpha cannot be "
+                     f"formed exactly by a batch build: pass a float32 or float64 map (integer maps must keep 1 - p "
+                     f"within their dtype)")
 
 
 class BatchGraph:
@@ -241,10 +243,11 @@ def graph_from_voxels_batch(fg_markers, bg_markers, image, boundary, sigma=None,
     else:
         image, norms = _host_image(image, boundary)
 
-    alpha = 0.0 if alpha is None else float(alpha)
+    alpha = 0.0 if alpha is None else alpha
     compute_f32 = False
     if prob is not None:
-        prob, compute_f32 = _prob_arg(prob, alpha)
+        prob, compute_f32 = _prob_arg(prob, alpha)     # on alpha as given: its type decides the products' dtype
+    alpha = float(alpha)
 
     from .. import _lib   # raises ImportError loudly when the extension is not built
     native = _lib.Graph.batch(list(image_shape), batch, -1)

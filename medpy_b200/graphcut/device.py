@@ -5,6 +5,7 @@ reference's: regional term, boundary term, foreground markers, background marker
 """
 import math
 
+from .energy_voxel import _device_products
 from .maxflow import GraphDouble
 
 _KINDS = {
@@ -29,7 +30,9 @@ def graph_from_device_arrays(fg_markers, bg_markers, image=None, boundary=None, 
     """Build (or rebuild into ``graph``) the lattice graph from device arrays.
 
     boundary : one of the eight ``energy_voxel.boundary_*`` names without the prefix
-    prob/alpha : ``regional_probability_map`` arguments (float32 map * Python float -> float32 products)
+    prob/alpha : ``regional_probability_map`` arguments, with the products numpy forms for a host map of prob's dtype
+        (float32 map * Python float -> float32 products); a map and alpha whose products numpy forms in mixed or other
+        dtypes (a float32 map with a ``numpy.float64`` alpha, integer or float16 maps) raise ``ValueError``
     graph : an earlier result to reuse (its device memory is kept, all weights are reset)
     stream : cudaStream_t as int (e.g. ``torch.cuda.current_stream().cuda_stream``) to run on
 
@@ -40,6 +43,7 @@ def graph_from_device_arrays(fg_markers, bg_markers, image=None, boundary=None, 
     build raises ``RuntimeError``, and a rebuild takes the arrays as they are then.  (A contiguous array is read in place;
     a strided one is gathered into a buffer the graph owns.)
     """
+    compute_f32 = prob is not None and _device_products(prob, alpha)
     shape = tuple(int(s) for s in fg_markers.shape)
     n = 1
     for s in shape:
@@ -55,7 +59,6 @@ def graph_from_device_arrays(fg_markers, bg_markers, image=None, boundary=None, 
     # one native call: single-pass fused build on 1-D..3-D lattices (mgc_build_voxel_graph), the per-term kernels in
     # the reference's order otherwise.  A non-positive n-link weight is reported by maxflow() (ValueError).
     graph.defer_weight_check(True)
-    compute_f32 = prob is not None and "float32" in str(prob.dtype)
     kind = _KINDS[boundary] if boundary is not None else -1
     sp = [float(s) for s in spacing] if spacing else None
     nat.build_voxel_graph(prob, 0.0 if alpha is None else float(alpha), compute_f32, kind, image,

@@ -85,6 +85,50 @@ def _boundary(graph, kind, image, sigma, spacing):
     graph._add_boundary(kind, dev, 0.0 if sigma is None else float(sigma), _spacing_arg(spacing, image.ndim), norm)
 
 
+def _regional_products(dtype, alpha):
+    """How numpy forms the two products ``p * alpha`` and ``(1 - p) * alpha`` of a map of this dtype: ``"f32"`` (a
+    float32 map, both in float32, as a float32 map times a Python float), ``"f64"`` (a float64 map, both in float64), or
+    None for every other mix, whose products only numpy itself forms exactly (a float32 map times a ``numpy.float64``
+    rounds ``1 - p`` in float32 and multiplies in float64; integer maps form ``1 - p`` in their own dtype)."""
+    if dtype is None:
+        return None
+    z = numpy.zeros(0, dtype)
+    src, snk = (z * alpha).dtype, ((1 - z) * alpha).dtype      # numpy-2 weak scalars
+    if z.dtype == numpy.float32 and src == numpy.float32 and snk == numpy.float32:
+        return "f32"
+    if z.dtype == numpy.float64 and src == numpy.float64 and snk == numpy.float64:
+        return "f64"
+    return None
+
+
+def _device_products(prob, alpha, whose="the"):
+    """Whether the products of a device probability map (torch tensor, or any array with a numpy-like ``dtype``) are
+    float32, decided as ``_regional_products`` decides them for the host map of the same dtype; ``ValueError`` where
+    they are neither pure float32 nor pure float64, since a device map has no dense fallback."""
+    try:
+        dtype = numpy.dtype(str(prob.dtype).rsplit(".", 1)[-1])      # torch.float32 -> float32
+    except TypeError:
+        dtype = None
+    mode = _regional_products(dtype, 0.0 if alpha is None else alpha)
+    if mode is None:
+        raise ValueError(f"{whose} probability map must be float32 or float64 and give products of its own dtype with "
+                         f"alpha, got a {prob.dtype} map with a {type(alpha).__name__} alpha")
+    return mode == "f32"
+
+
+def _exact_as_float64(prob, alpha):
+    """True when an integer or bool map's products are the float64 products of its float64 copy: numpy forms both in
+    float64, ``1 - p`` does not wrap around in the map's dtype, and every p and 1 - p is an integer a double holds
+    exactly.  A bool map always qualifies when numpy's products are float64: ``1 - p`` is formed in int64 and is 0 or 1."""
+    if prob.dtype.kind not in "biu" or (prob[:0] * alpha).dtype != numpy.float64 or ((1 - prob[:0]) * alpha).dtype != numpy.float64:
+        return False
+    if prob.size == 0 or prob.dtype.kind == "b":
+        return True
+    lo, hi = int(prob.min()), int(prob.max())
+    info = numpy.iinfo(prob.dtype)
+    return 1 - hi >= info.min and 1 - lo <= info.max and -2 ** 53 < lo and hi <= 2 ** 53
+
+
 def regional_probability_map(graph, term_args):
     """Regional term based on a probability atlas (reference: energy_voxel.py:33-65).
 
@@ -93,13 +137,9 @@ def regional_probability_map(graph, term_args):
     ``graph.set_tweights_all`` semantics, i.e. ``add_tweights`` per voxel in node order."""
     (probability_map, alpha) = term_args
     probability_map = _native_order(numpy.asarray(probability_map))
-    # dtype numpy gives the two products (numpy-2 weak scalars: float32 map * Python float stays float32)
-    src_dtype = (probability_map[:0] * alpha).dtype
-    snk_dtype = ((1 - probability_map[:0]) * alpha).dtype
-    pure32 = probability_map.dtype == numpy.float32 and src_dtype == numpy.float32 and snk_dtype == numpy.float32
-    pure64 = probability_map.dtype == numpy.float64 and src_dtype == numpy.float64 and snk_dtype == numpy.float64
-    if pure32 or pure64:
-        graph._add_regional_probability(probability_map, float(alpha), bool(pure32))
+    mode = _regional_products(probability_map.dtype, alpha)
+    if mode is not None:
+        graph._add_regional_probability(probability_map, float(alpha), mode == "f32")
     else:
         # unusual dtype mixes: form the products with numpy exactly as the reference does, upload densely
         graph.set_tweights_dense((probability_map * alpha).astype(numpy.float64).ravel(),

@@ -149,10 +149,19 @@ def test_big_endian_probability_map_is_normalised(rec):
 
 
 def test_integer_probability_map_gives_float64_products(rec):
+    """An integer map goes as a float64 copy only where its float64 products are numpy's: 1 - p must not wrap around in
+    the map's dtype (uint8 at p >= 2, int16 at p <= -32767) and alpha must give float64 products."""
     image, fg, bg = _arrays()
     _build(arrays=(image, fg, bg), prob=numpy.ones(image.shape, numpy.int16), alpha=0.5)
     args = rec[0].build
     assert args[0].dtype == numpy.float64 and args[2] is False
+    rec.clear()
+    for dtype, value, alpha in ((numpy.uint8, 2, 0.5), (numpy.int16, -32767, 0.5), (numpy.int16, 1, numpy.float32(0.5))):
+        prob = numpy.ones(image.shape, dtype)
+        prob[1, 2, 3] = value
+        with pytest.raises(ValueError, match="probability map"):
+            _build(arrays=(image, fg, bg), prob=prob, alpha=alpha)
+    assert not rec
 
 
 def test_float16_probability_map_is_refused(rec):
