@@ -18,6 +18,8 @@ import os
 
 import numpy
 
+from .graphcut import _warm_args
+
 KINDS = {
     "difference_linear": 0, "difference_exponential": 1, "difference_division": 2, "difference_power": 3,
     "maximum_linear": 4, "maximum_exponential": 5, "maximum_division": 6, "maximum_power": 7,
@@ -31,29 +33,6 @@ def slab_bounds(extent, world, rank):
 
 def _contiguous(a):
     return numpy.ascontiguousarray(a) if isinstance(a, numpy.ndarray) else a.contiguous()
-
-
-def _all_finite(a):
-    """No NaN or infinite value in a numpy array or a tensor."""
-    if isinstance(a, numpy.ndarray):
-        return bool(numpy.isfinite(a).all())
-    import torch
-    return bool(torch.isfinite(a).all())
-
-
-def _neighbours(i, j, shape):
-    """Whether every pair (i[k], j[k]) of global ids (numpy arrays or tensors) is a pair of lattice neighbours."""
-    if isinstance(i, numpy.ndarray):
-        lo = numpy.minimum(i, j)
-    else:
-        import torch
-        lo = torch.minimum(i, j)
-    d = abs(i - j)
-    ok = d < 0
-    for a in range(len(shape)):
-        stride = math.prod(shape[a + 1:])
-        ok = ok | ((d == stride) & ((lo // stride) % shape[a] + 1 < shape[a]))
-    return bool(ok.all())
 
 
 def _native_factory(shape, z0, z1, device):
@@ -165,12 +144,19 @@ class SlabSolver:
     def _owned(self, ids):
         return (ids >= self.z0 * self.plane) & (ids < self.z1 * self.plane)
 
-    def _any_bad(self, bad):
-        """One all-reduce of a rank's verdict on its part of a dense argument: True if any rank found a bad entry."""
-        t = self.torch.tensor([1 if bad else 0], dtype=self.torch.int64, device=self.tdev)
+    def _check_every_rank(self, check, message):
+        """``check()`` on the rank's part of a dense argument, and one all-reduce of the verdicts: if it raised
+        ValueError on any rank, every rank raises ``ValueError(message)``."""
+        try:
+            check()
+            bad = 0
+        except ValueError:
+            bad = 1
+        t = self.torch.tensor([bad], dtype=self.torch.int64, device=self.tdev)
         if self.world > 1:
             self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX, group=self.group)
-        return bool(int(t.item()))
+        if int(t.item()):
+            raise ValueError(message)
 
     def add_seeds(self, fg=None, bg=None):
         """Foreground / background seeds folded into the solved slabs (``add_tweights(v, 65535, 0)`` per fg id, then
@@ -183,52 +169,33 @@ class SlabSolver:
         self._fold_seeds(fg, bg, self.handle.remove_seeds)
 
     def _fold_seeds(self, fg, bg, native):
-        from .graphcut import _warm_args
-        _warm_args.one_space("fg and bg must both be host or both be device arrays", fg, bg)
-        n = math.prod(self.shape)
-        ids = [None if x is None else _warm_args.node_ids(x, self.shape, n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
+        ids = _warm_args.seed_args(fg, bg, self.shape, math.prod(self.shape))
         native(*(None if a is None else self._local_ids(a[self._owned(a)]) for a in ids))
 
     def add_tweights_warm(self, ids, src, snk):
         """``add_tweights(ids[k], src[k], snk[k])`` calls folded into the solved slabs, in order.  ``ids``: global ids or
         a boolean mask of the global shape; None for the dense form, where ``src`` / ``snk`` have the global shape (each
         rank reads its planes and its ghost planes).  Scalars broadcast; weights are finite reals of either sign."""
-        from .graphcut import _warm_args
-        cuda = _warm_args.one_space("ids, src and snk must all be host or all be device arrays", ids, src, snk)
-        n = math.prod(self.shape)
-        if ids is None:
-            s = _warm_args.weights(src, n, "src", self.shape, cuda)
-            t = _warm_args.weights(snk, n, "snk", self.shape, cuda)
-            s, t = (self._slice_flat(a) for a in (s, t))
-            if self._any_bad(not (_all_finite(s) and _all_finite(t))):
-                raise ValueError("src or snk holds NaN or infinite values")
-            self.handle.add_tweights_warm(None, s, t)
+        ids, s, t = _warm_args.tlink_args(ids, src, snk, self.shape, math.prod(self.shape))
+        if ids is not None:
+            _warm_args.check_finite(s, "src")
+            _warm_args.check_finite(t, "snk")
+            keep = self._owned(ids)
+            self.handle.add_tweights_warm(self._local_ids(ids[keep]), s[keep], t[keep])
             return
-        ids = _warm_args.node_ids(ids, self.shape, n, "ids")
-        m = ids.shape[0]
-        s = _warm_args.weights(src, m, "src", device=cuda)
-        t = _warm_args.weights(snk, m, "snk", device=cuda)
-        if not (_all_finite(s) and _all_finite(t)):
-            raise ValueError("src or snk holds NaN or infinite values")
-        keep = self._owned(ids)
-        self.handle.add_tweights_warm(self._local_ids(ids[keep]), s[keep], t[keep])
+        s, t = (self._slice_flat(a) for a in (s, t))
+        self._check_every_rank(lambda: (_warm_args.check_finite(s, "src"), _warm_args.check_finite(t, "snk")),
+                               "src or snk holds NaN or infinite values")
+        self.handle.add_tweights_warm(None, s, t)
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
         """``sum_edge(i[k], j[k], cap[k], rev_cap[k])`` calls folded into the solved slabs, in order: ``i`` / ``j`` global
         ids of lattice neighbours, ``cap`` / ``rev_cap`` nonnegative finite increments (scalars broadcast).  There is no
         decrement on slabs: take capacity off by rebuilding."""
-        from .graphcut import _warm_args
-        cuda = _warm_args.one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
-        n = math.prod(self.shape)
-        ii, jj = _warm_args.pair_ids(i, n, "i"), _warm_args.pair_ids(j, n, "j")
-        ii, jj, c, r = _warm_args.nlink_calls(ii, jj, cap, rev_cap, cuda)
-        if not _neighbours(ii, jj, self.shape):
+        ii, jj, c, r, _ = _warm_args.nlink_args(i, j, cap, rev_cap, math.prod(self.shape))
+        if bool((_warm_args.lattice_axes(ii, jj, self.shape) < 0).any()):
             raise ValueError("i and j hold a pair that is not lattice neighbours")
-        for w, what in ((c, "cap"), (r, "rev_cap")):
-            if not _all_finite(w):
-                raise ValueError("{} holds NaN or infinite values".format(what))
-            if bool((w < 0).any()):
-                raise ValueError("{} holds negative values: {}".format(what, _warm_args.ONLY_RAISES))
+        _warm_args.check_amounts(((c, "cap"), (r, "rev_cap")), _warm_args.ONLY_RAISES)
         keep = self._owned(ii) | self._owned(jj)
         self.handle.add_nweights_warm(self._local_ids(ii[keep]), self._local_ids(jj[keep]), c[keep], r[keep])
 
@@ -236,23 +203,13 @@ class SlabSolver:
         """The dense form of ``add_nweights_warm`` in the layout of ``add_nweights_dense``: ``fwd`` / ``bwd`` have the
         global shape and entry p holds the increments of p -> p + e_axis and back; the last plane of ``axis`` is
         ignored.  Each rank reads its planes and its ghost planes, so an axis-0 pair across a border reaches both."""
-        from .graphcut import _warm_args
-        axis = int(axis)
-        if not 0 <= axis < len(self.shape):
-            raise ValueError("axis {} is out of range for a lattice of shape {}".format(axis, self.shape))
-        _warm_args.one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
-        fwd, bwd = _warm_args.real(fwd, "fwd"), _warm_args.real(bwd, "bwd")
-        for a, what in ((fwd, "fwd"), (bwd, "bwd")):
-            if tuple(a.shape) != self.shape:
-                raise ValueError("{} of shape {} does not match the lattice's shape {}".format(what, tuple(a.shape), self.shape))
-        f, b = self.local_slice(fwd), self.local_slice(bwd)
-        f, b = (_contiguous(a) for a in (f, b))
+        axis, fwd, bwd, _ = _warm_args.nlink_dense_args(axis, fwd, bwd, self.shape, "lattice")
+        f, b = (_contiguous(self.local_slice(a)) for a in (fwd, bwd))
         # the entries the native grouping reads: all but the local last plane of the axis, whose pairs are another
         # rank's (or, on the last rank, the global last plane, which names no pair)
-        cut = tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(f.shape))
-        bad = not (_all_finite(f[cut]) and _all_finite(b[cut])) or bool((f[cut] < 0).any()) or bool((b[cut] < 0).any())
-        if self._any_bad(bad):
-            raise ValueError("fwd or bwd holds negative, NaN or infinite values: " + _warm_args.ONLY_RAISES)
+        cut = _warm_args.pair_entries(f.shape, axis)
+        self._check_every_rank(lambda: _warm_args.check_amounts(((f[cut], "fwd"), (b[cut], "bwd")), _warm_args.ONLY_RAISES),
+                               "fwd or bwd holds negative, NaN or infinite values: " + _warm_args.ONLY_RAISES)
         self.handle.add_nweights_dense_warm(axis, f, b)
 
     def _slice_flat(self, a):

@@ -1,7 +1,16 @@
-"""Argument parsing of the warm edit calls, shared by the lattice graph (maxflow.py) and the general sparse graph
-(sparse.py).  A result stays in the memory space of its argument: a CUDA tensor gives a CUDA tensor, which the lattice's
-native folds read in place, anything else (numpy arrays, lists, scalars, CPU tensors) a numpy array.  Broadcasts go to
-the device when the caller asks for it; which memory spaces one call may mix is the caller's decision."""
+"""Argument parsing of the warm edit calls (``add_seeds``, ``remove_seeds``, ``add_tweights_warm``, the list and dense
+n-link edits), shared by every front-end that takes them.
+
+The lattice front-ends -- a lattice graph (maxflow.GraphDouble), a batch of images (batch.BatchGraph) and one rank's
+z-slab (distributed.SlabSolver) -- parse each kind of edit with one function here: ``seed_args``,
+``tlink_args``, ``nlink_args`` and ``nlink_dense_args``.  They keep only what is their own: staging before a solve,
+the batch axis, the slab's ownership.  The sparse-id front-ends (sparse.SparseGraphDouble,
+labels_batch.LabelBatchGraph) parse through the sparse-id functions of sparse.py, which build on ``node_ids``,
+``weights`` and ``nlink_calls`` here.
+
+A result stays in the memory space of its argument: a CUDA tensor gives a CUDA tensor, which the native folds read in
+place, anything else (numpy arrays, lists, scalars, CPU tensors) a numpy array.  The checks of parsed weights
+(``check_finite``, ``check_amounts``) take both; on a CUDA tensor each verdict is one read-back."""
 import math
 
 import numpy
@@ -119,9 +128,65 @@ def nlink_calls(i, j, cap, rev_cap, device=False):
             weights(cap, m, "cap", device=device), weights(rev_cap, m, "rev_cap", device=device))
 
 
+def seed_args(fg, bg, shape, n, names=("fg", "bg"), mixed=False):
+    """The node ids of an add_seeds / remove_seeds call (``node_ids``; None stays None).  fg and bg must share one
+    memory space unless ``mixed``: a graph that stages the seeds on the host takes either."""
+    if not mixed:
+        one_space("{} and {} must both be host or both be device arrays".format(*names), fg, bg)
+    return tuple(None if x is None else node_ids(x, shape, n, what) for x, what in zip((fg, bg), names))
+
+
+def tlink_args(ids, src, snk, shape, n, names=("ids", "src", "snk")):
+    """The calls of an add_tweights_warm edit: the node ids (``node_ids``; None for the dense form, one call per node in
+    C order) and the weights as C-contiguous float64 arrays of one entry per call.  Scalars broadcast; a dense form's
+    weights have ``shape`` or one entry per node.  All three arguments share one memory space."""
+    cuda = one_space("{}, {} and {} must all be host or all be device arrays".format(*names), ids, src, snk)
+    ids = None if ids is None else node_ids(ids, shape, n, names[0])
+    m, dense = (n, tuple(shape)) if ids is None else (ids.shape[0], None)
+    return ids, weights(src, m, names[1], dense, cuda), weights(snk, m, names[2], dense, cuda)
+
+
+def nlink_args(i, j, cap, rev_cap, n):
+    """The calls of a list-form n-link edit on a graph of n nodes as ``nlink_calls`` gives them, from id arguments that
+    ``pair_ids`` parses; and whether they are on the device.  All four arguments share one memory space."""
+    cuda = one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
+    return nlink_calls(pair_ids(i, n, "i"), pair_ids(j, n, "j"), cap, rev_cap, cuda) + (cuda,)
+
+
+def nlink_dense_args(axis, fwd, bwd, shape, what="graph"):
+    """The arguments of a dense n-link edit: the axis, checked against ``shape`` (that of a ``what``), and fwd / bwd as
+    float64 arrays of ``shape``, strides kept; and whether they are on the device.  Both arrays share one memory space."""
+    axis, shape = int(axis), tuple(shape)
+    if not 0 <= axis < len(shape):
+        raise ValueError("axis {} is out of range for a {} of shape {}".format(axis, what, shape))
+    cuda = one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
+    fwd, bwd = real(fwd, "fwd"), real(bwd, "bwd")
+    for a, name in ((fwd, "fwd"), (bwd, "bwd")):
+        if tuple(a.shape) != shape:
+            raise ValueError("{} of shape {} does not match the {} shape {}".format(name, tuple(a.shape), what, shape))
+    return axis, fwd, bwd, cuda
+
+
+def pair_entries(shape, axis):
+    """The entries of a dense n-link array of ``shape`` that name a pair: the last plane of ``axis`` names none."""
+    return tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(shape))
+
+
+def lattice_axes(i, j, shape):
+    """The axis that joins each pair (i[k], j[k]) of C-order node ids on a lattice of ``shape``, or -1 where the two are
+    not lattice neighbours; int64 numpy arrays or CUDA tensors, with no read-back."""
+    lo, d = (numpy.minimum(i, j) if isinstance(i, numpy.ndarray) else i.minimum(j)), abs(i - j)
+    axes = d * 0 - 1
+    for axis in range(len(shape)):
+        stride = math.prod(shape[axis + 1:])
+        # at most one axis joins a pair: of two axes with one stride the later has size 1, and a size-1 axis joins none
+        axes = axes + ((d == stride) & ((lo // stride) % shape[axis] < shape[axis] - 1)) * (axis + 1)
+    return axes
+
+
 def check_finite(w, what):
-    """Host weights: no NaN or infinite value."""
-    if not numpy.isfinite(w).all():
+    """Weights on the host or the device: no NaN or infinite value."""
+    if not bool((w.isfinite() if on_device(w) else numpy.isfinite(w)).all()):
         raise ValueError("{} holds NaN or infinite values".format(what))
 
 
@@ -131,9 +196,9 @@ DECREMENTS = "n-link decrements are nonnegative amounts"
 
 
 def check_amounts(named, why):
-    """Host n-link amounts ``[(weights, name), ...]``: finite and nonnegative, argument by argument; ``why`` ends the
-    message about a negative value."""
+    """N-link amounts ``[(weights, name), ...]`` on the host or the device: finite and nonnegative, argument by argument;
+    ``why`` ends the message about a negative value."""
     for w, what in named:
         check_finite(w, what)
-        if (numpy.asarray(w) < 0).any():
+        if bool(((w if on_device(w) else numpy.asarray(w)) < 0).any()):
             raise ValueError("{} holds negative values: {}".format(what, why))

@@ -131,32 +131,26 @@ class BatchGraph:
 
     def _seeds(self, native, fg, bg):
         if self._warm:
-            _warm_args.one_space("fg_ids and bg_ids must both be host or both be device arrays", fg, bg)
-            fg, bg = (None if x is None else _warm_args.node_ids(x, self.shape, self._n, what)
-                      for x, what in ((fg, "fg_ids"), (bg, "bg_ids")))
+            fg, bg = _warm_args.seed_args(fg, bg, self.shape, self._n, ("fg_ids", "bg_ids"))
         getattr(self._native, native)(fg, bg)
 
     def add_tweights_warm(self, ids, src, snk):
         """``add_tweights(ids[k], src[k], snk[k])`` per entry in order; ``ids`` None is the dense form, one call per
         voxel with ``src`` / ``snk`` of the batch shape (or one entry per voxel).  Scalars broadcast."""
         if self._warm:
-            cuda = _warm_args.one_space("ids, src and snk must all be host or all be device arrays", ids, src, snk)
-            ids = None if ids is None else _warm_args.node_ids(ids, self.shape, self._n, "ids")
-            m, dense = (self._n, self.shape) if ids is None else (ids.shape[0], None)
-            src = _warm_args.weights(src, m, "src", dense, cuda)
-            snk = _warm_args.weights(snk, m, "snk", dense, cuda)
+            ids, src, snk = _warm_args.tlink_args(ids, src, snk, self.shape, self._n)
         self._native.add_tweights_warm(ids, src, snk)
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
         """``sum_edge(i[k], j[k], cap[k], rev_cap[k])`` per entry in order, on pairs of neighbours inside one image."""
         if self._warm:
-            i, j, cap, rev_cap, _ = self._nlink_args(i, j, cap, rev_cap)
+            i, j, cap, rev_cap, _ = _warm_args.nlink_args(i, j, cap, rev_cap, self._n)
         self._native.add_nweights_warm(i, j, cap, rev_cap)
 
     def remove_nweights_warm(self, i, j, cap, rev_cap):
         """``sum_edge(i[k], j[k], -cap[k], -rev_cap[k])`` per entry in order (nonnegative decrements)."""
         if self._warm:
-            i, j, cap, rev_cap, cuda = self._nlink_args(i, j, cap, rev_cap)
+            i, j, cap, rev_cap, cuda = _warm_args.nlink_args(i, j, cap, rev_cap, self._n)
             if not cuda:        # the native grouping checks device decrements in the same pass
                 _warm_args.check_amounts(((cap, "cap"), (rev_cap, "rev_cap")), _warm_args.DECREMENTS)
         self._native.remove_nweights_warm(i, j, cap, rev_cap)
@@ -175,7 +169,7 @@ class BatchGraph:
         if self._warm:
             lattice_axis, fwd, bwd, cuda = self._dense_args(axis, fwd, bwd)
             if not cuda:        # the entries that name a pair: all but the last plane of `axis` in every image
-                cut = tuple(slice(0, s - 1) if d == int(axis) else slice(None) for d, s in enumerate(self.shape))
+                cut = _warm_args.pair_entries(self.shape, int(axis))
                 _warm_args.check_amounts(((fwd[cut], "fwd"), (bwd[cut], "bwd")), _warm_args.DECREMENTS)
             axis = lattice_axis
         self._native.remove_nweights_dense_warm(axis, fwd, bwd)
@@ -184,26 +178,12 @@ class BatchGraph:
     def _n(self):
         return math.prod(self.shape)
 
-    def _nlink_args(self, i, j, cap, rev_cap):
-        """The list-form n-link arguments as four contiguous 1-D arrays of one length, and whether they are on the
-        device."""
-        cuda = _warm_args.one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
-        ii, jj = _warm_args.pair_ids(i, self._n, "i"), _warm_args.pair_ids(j, self._n, "j")
-        return _warm_args.nlink_calls(ii, jj, cap, rev_cap, cuda) + (cuda,)
-
     def _dense_args(self, axis, fwd, bwd):
-        """The dense n-link arguments: the lattice axis of batch axis ``axis`` (the images' axes are the last of the
-        lattice's three), and fwd / bwd as float64 arrays of the batch shape; and whether they are on the device."""
-        axis = int(axis)
-        if axis == 0:
+        """The dense n-link arguments with the lattice axis of batch axis ``axis`` (the images' axes are the last of the
+        lattice's three)."""
+        if int(axis) == 0:
             raise ValueError("axis 0 is the batch axis: no n-link joins two images")
-        if not 0 < axis < len(self.shape):
-            raise ValueError("axis {} is out of range for a batch of shape {}".format(axis, self.shape))
-        cuda = _warm_args.one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
-        fwd, bwd = _warm_args.real(fwd, "fwd"), _warm_args.real(bwd, "bwd")
-        for a, what in ((fwd, "fwd"), (bwd, "bwd")):
-            if tuple(a.shape) != self.shape:
-                raise ValueError("{} of shape {} does not match the batch shape {}".format(what, tuple(a.shape), self.shape))
+        axis, fwd, bwd, cuda = _warm_args.nlink_dense_args(axis, fwd, bwd, self.shape, "batch")
         return 3 - len(self.shape) + axis, fwd, bwd, cuda
 
 

@@ -18,7 +18,7 @@ from . import _warm_args, energy_label
 from .energy_label import _DBL_MIN, device_labels, device_values
 from .graph import GCGraph
 from .maxflow import _termtype
-from .sparse import warm_ids, warm_pairs, warm_weights
+from .sparse import warm_pairs, warm_seeds, warm_tweights
 
 __all__ = ["graph_from_labels_batch", "LabelBatchGraph"]
 
@@ -277,28 +277,20 @@ class LabelBatchGraph:
     def add_seeds(self, fg=None, bg=None):
         """add_tweights(v, 65535, 0) per foreground id in order, then add_tweights(v, 0, 65535) per background id."""
         self._require_warm("add_seeds")
-        self._seed_calls(fg, bg, 65535.0)
+        for call in warm_seeds(fg, bg, 65535.0, int(self._off[-1])):
+            self._graph.add_tweights(*call)
 
     def remove_seeds(self, fg=None, bg=None):
         """The inverse of add_seeds: add_tweights(v, -65535, 0) / add_tweights(v, 0, -65535)."""
         self._require_warm("remove_seeds")
-        self._seed_calls(fg, bg, -65535.0)
-
-    def _seed_calls(self, fg, bg, cap):
-        n = int(self._off[-1])
-        ids = [None if x is None else warm_ids(x, n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
-        for v, src, snk in ((ids[0], cap, 0.0), (ids[1], 0.0, cap)):
-            if v is not None and v.size:
-                self._graph.add_tweights(v, numpy.full(v.size, src), numpy.full(v.size, snk))
+        for call in warm_seeds(fg, bg, -65535.0, int(self._off[-1])):
+            self._graph.add_tweights(*call)
 
     def add_tweights_warm(self, nodes, cap_source, cap_sink):
         """add_tweights(nodes[k], cap_source[k], cap_sink[k]) per entry in order; nodes None: one call per node."""
         self._require_warm("add_tweights_warm")
-        n = int(self._off[-1])
-        ids = None if nodes is None else warm_ids(nodes, n, "nodes")
-        m = n if ids is None else ids.size
-        src, snk = warm_weights(cap_source, m, "cap_source"), warm_weights(cap_sink, m, "cap_sink")
-        if m:
+        ids, src, snk = warm_tweights(nodes, cap_source, cap_sink, int(self._off[-1]))
+        if src.size:
             self._graph.add_tweights(ids, src, snk)
 
     def _pairs(self, i, j, cap, rev_cap, why):

@@ -476,8 +476,7 @@ class GraphDouble:
         self._fold_seeds(fg, bg, -65535.0, "remove_seeds", "without the seeds")
 
     def _fold_seeds(self, fg, bg, cap, native, rebuild):
-        ids = [None if x is None else _warm_args.node_ids(x, self._shape, self._n, what)
-               for x, what in ((fg, "fg"), (bg, "bg"))]
+        ids = _warm_args.seed_args(fg, bg, self._shape, self._n, mixed=True)
         self._warm_call(native, ids, lambda f, b: self._stage_seeds(f, b, cap), rebuild)
 
     def _stage_seeds(self, fg, bg, cap):
@@ -495,12 +494,6 @@ class GraphDouble:
             raise _cannot_fold(rebuild)
         self._dirty()
         getattr(self._nat(), native)(*args)
-
-    @staticmethod
-    def _one_space(message, *args):
-        """Whether the arguments of one warm call are on the device.  The native folds take their arrays all on the host or
-        all on the device: a mix raises ``ValueError(message)``; host scalars go with either."""
-        return _warm_args.one_space(message, *args)
 
     def add_tweights_warm(self, nodes, cap_source, cap_sink):
         """``add_tweights`` calls on a solved graph, re-solved warm by the next ``maxflow()``: soft strokes, a GrabCut-style
@@ -521,12 +514,8 @@ class GraphDouble:
         build the graph again with the calls."""
         if self._warm_sparse():
             return self._sp.add_tweights_warm(nodes, cap_source, cap_sink)
-        cuda = self._one_space("nodes, cap_source and cap_sink must all be host or all be device arrays",
-                               nodes, cap_source, cap_sink)
-        ids = None if nodes is None else _warm_args.node_ids(nodes, self._shape, self._n, "nodes")
-        m, dense = (self._n, self._shape) if ids is None else (ids.shape[0], None)
-        src = _warm_args.weights(cap_source, m, "cap_source", dense, cuda)
-        snk = _warm_args.weights(cap_sink, m, "cap_sink", dense, cuda)
+        ids, src, snk = _warm_args.tlink_args(nodes, cap_source, cap_sink, self._shape, self._n,
+                                              ("nodes", "cap_source", "cap_sink"))
         self._warm_call("add_tweights_warm", (ids, src, snk), self._stage_tweights_calls, "with the t-link calls")
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
@@ -544,15 +533,8 @@ class GraphDouble:
         ``RuntimeError``: ``reset()`` it and build the graph again with the calls."""
         if self._warm_sparse():
             return self._sp.add_nweights_warm(i, j, cap, rev_cap)
-        ii, jj, c, r, _ = self._nlink_args(i, j, cap, rev_cap)
+        ii, jj, c, r, _ = _warm_args.nlink_args(i, j, cap, rev_cap, self._n)
         self._warm_call("add_nweights_warm", (ii, jj, c, r), self._stage_nweights_calls, "with the n-link calls")
-
-    def _nlink_args(self, i, j, cap, rev_cap):
-        """The arguments of add_nweights_warm / remove_nweights_warm as four contiguous 1-D arrays of one length (int64 ids,
-        float64 weights), and whether they are on the device."""
-        cuda = self._one_space("i, j, cap and rev_cap must all be host or all be device arrays", i, j, cap, rev_cap)
-        ii, jj = _warm_args.pair_ids(i, self._n, "i"), _warm_args.pair_ids(j, self._n, "j")
-        return _warm_args.nlink_calls(ii, jj, cap, rev_cap, cuda) + (cuda,)
 
     def add_nweights_dense_warm(self, axis, fwd, bwd):
         """The dense form of ``add_nweights_warm``, in the layout of ``add_nweights_dense``: ``fwd`` / ``bwd`` have the
@@ -565,30 +547,13 @@ class GraphDouble:
         as ``add_nweights_warm`` fold it into the solved state (mgc_add_nweights_dense_warm)."""
         if self._warm_sparse():
             return self._sp.add_nweights_dense_warm(axis, fwd, bwd)
-        axis, fwd, bwd, _ = self._dense_args(axis, fwd, bwd)
+        axis, fwd, bwd, _ = _warm_args.nlink_dense_args(axis, fwd, bwd, self._shape)
         self._warm_call("add_nweights_dense_warm", (axis, fwd, bwd), self._stage_nweights_dense, "with the n-link calls")
-
-    def _dense_args(self, axis, fwd, bwd):
-        """The arguments of the dense n-link folds: the axis, checked, and fwd / bwd as float64 arrays of the lattice shape;
-        and whether they are on the device."""
-        axis = int(axis)
-        if not 0 <= axis < len(self._shape):
-            raise ValueError("axis {} is out of range for a graph of shape {}".format(axis, self._shape))
-        cuda = self._one_space("fwd and bwd must both be host or both be device arrays", fwd, bwd)
-        fwd, bwd = _warm_args.real(fwd, "fwd"), _warm_args.real(bwd, "bwd")
-        for a, what in ((fwd, "fwd"), (bwd, "bwd")):
-            if tuple(a.shape) != self._shape:
-                raise ValueError("{} of shape {} does not match the graph's shape {}".format(what, tuple(a.shape), self._shape))
-        return axis, fwd, bwd, cuda
-
-    def _pairs_of_axis(self, axis):
-        """The entries of a dense n-link array that name a pair: the last plane of ``axis`` names none."""
-        return tuple(slice(0, s - 1) if d == axis else slice(None) for d, s in enumerate(self._shape))
 
     def _stage_nweights_dense(self, axis, fwd, bwd):
         """add_nweights_dense_warm before the first solve: checked like the warm fold checks it, then staged exactly like
         ``add_nweights_dense``."""
-        cut = self._pairs_of_axis(axis)
+        cut = _warm_args.pair_entries(self._shape, axis)
         _warm_args.check_amounts(((fwd[cut], "fwd"), (bwd[cut], "bwd")), _warm_args.ONLY_RAISES)
         staged = [numpy.zeros(self._shape), numpy.zeros(self._shape)]
         staged[0][cut], staged[1][cut] = fwd[cut], bwd[cut]
@@ -614,7 +579,7 @@ class GraphDouble:
         ``RuntimeError``: ``reset()`` it and build the graph again without the weight."""
         if self._warm_sparse():
             return self._sp.remove_nweights_warm(i, j, cap, rev_cap)
-        ii, jj, c, r, cuda = self._nlink_args(i, j, cap, rev_cap)
+        ii, jj, c, r, cuda = _warm_args.nlink_args(i, j, cap, rev_cap, self._n)
         if not cuda:        # the native grouping checks device decrements in the same pass
             _warm_args.check_amounts(((c, "cap"), (r, "rev_cap")), _warm_args.DECREMENTS)
         self._fold_decrements("remove_nweights_warm", ii, jj, c, r)
@@ -625,9 +590,9 @@ class GraphDouble:
         the pairs with a nonzero entry are touched.  Same meaning, checks and errors as ``remove_nweights_warm``."""
         if self._warm_sparse():
             return self._sp.remove_nweights_dense_warm(axis, fwd, bwd)
-        axis, fwd, bwd, cuda = self._dense_args(axis, fwd, bwd)
+        axis, fwd, bwd, cuda = _warm_args.nlink_dense_args(axis, fwd, bwd, self._shape)
         if not cuda:
-            cut = self._pairs_of_axis(axis)
+            cut = _warm_args.pair_entries(self._shape, axis)
             _warm_args.check_amounts(((fwd[cut], "fwd"), (bwd[cut], "bwd")), _warm_args.DECREMENTS)
         self._fold_decrements("remove_nweights_dense_warm", axis, fwd, bwd)
 
@@ -670,11 +635,7 @@ class GraphDouble:
             for a, b, c, r in zip(i.tolist(), j.tolist(), cap.tolist(), rev.tolist()):
                 self._sp.sum_edge(a, b, c, r)
             return
-        lo, d = numpy.minimum(i, j), numpy.abs(i - j)
-        axes = numpy.full(i.shape, -1, numpy.int64)
-        for axis, st in enumerate(self._strides):
-            n_ax = self._shape[axis]
-            axes[(axes < 0) & (d == st) & ((lo // st) % n_ax < n_ax - 1)] = axis
+        axes = _warm_args.lattice_axes(i, j, self._shape)
         if (axes < 0).any():
             k = int(numpy.flatnonzero(axes < 0)[0])
             raise ValueError("node ids ({}, {}) are not lattice neighbours".format(int(i[k]), int(j[k])))
@@ -682,7 +643,7 @@ class GraphDouble:
             for a, b, c, r in zip(i.tolist(), j.tolist(), cap.tolist(), rev.tolist()):
                 self.sum_edge(a, b, c, r)
             return
-        up = i < j
+        lo, up = numpy.minimum(i, j), i < j
         f, b = numpy.where(up, cap, rev), numpy.where(up, rev, cap)
         for axis in numpy.unique(axes).tolist():
             sel = axes == axis

@@ -64,6 +64,22 @@ def warm_pairs(i, j, cap, rev_cap, n, why):
     return ii, jj, c, r
 
 
+def warm_seeds(fg, bg, cap, n):
+    """The add_tweights calls of add_seeds (``cap`` 65535) or remove_seeds (-65535) on a graph of n nodes, as
+    ``[(ids, src, snk), ...]`` host arrays: the foreground call, then the background call, each only where it has ids."""
+    ids = [None if x is None else warm_ids(x, n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
+    return [(v, numpy.full(v.size, src), numpy.full(v.size, snk))
+            for v, src, snk in ((ids[0], cap, 0.0), (ids[1], 0.0, cap)) if v is not None and v.size]
+
+
+def warm_tweights(nodes, cap_source, cap_sink, n):
+    """The add_tweights calls of add_tweights_warm on a graph of n nodes as host arrays: node ids (None: one call per
+    node) and finite weights of one entry per call."""
+    ids = None if nodes is None else warm_ids(nodes, n, "nodes")
+    m = n if ids is None else ids.size
+    return ids, warm_weights(cap_source, m, "cap_source"), warm_weights(cap_sink, m, "cap_sink")
+
+
 class SparseGraphDouble:
     """``GraphDouble(node_num_max, edge_num_max)`` for arbitrary node pairs."""
 
@@ -248,25 +264,19 @@ class SparseGraphDouble:
     def add_seeds(self, fg=None, bg=None):
         """add_tweights(v, 65535, 0) per foreground id in order, then add_tweights(v, 0, 65535) per background id."""
         self._require_warm("add_seeds")
-        self._seed_calls(fg, bg, 65535.0)
+        for call in warm_seeds(fg, bg, 65535.0, self._n):
+            self.add_tweights_bulk(*call)
 
     def remove_seeds(self, fg=None, bg=None):
         """The inverse of add_seeds: add_tweights(v, -65535, 0) / add_tweights(v, 0, -65535)."""
         self._require_warm("remove_seeds")
-        self._seed_calls(fg, bg, -65535.0)
-
-    def _seed_calls(self, fg, bg, cap):
-        ids = [None if x is None else warm_ids(x, self._n, what) for x, what in ((fg, "fg"), (bg, "bg"))]
-        for v, src, snk in ((ids[0], cap, 0.0), (ids[1], 0.0, cap)):
-            if v is not None and v.size:
-                self.add_tweights_bulk(v, numpy.full(v.size, src), numpy.full(v.size, snk))
+        for call in warm_seeds(fg, bg, -65535.0, self._n):
+            self.add_tweights_bulk(*call)
 
     def add_tweights_warm(self, nodes, cap_source, cap_sink):
         """add_tweights(nodes[k], cap_source[k], cap_sink[k]) per entry in order; nodes None: one call per node."""
         self._require_warm("add_tweights_warm")
-        ids = None if nodes is None else warm_ids(nodes, self._n, "nodes")
-        m = self._n if ids is None else ids.size
-        self.add_tweights_bulk(ids, warm_weights(cap_source, m, "cap_source"), warm_weights(cap_sink, m, "cap_sink"))
+        self.add_tweights_bulk(*warm_tweights(nodes, cap_source, cap_sink, self._n))
 
     def add_nweights_warm(self, i, j, cap, rev_cap):
         """sum_edge(i[k], j[k], cap[k], rev_cap[k]) per entry in order, on any node pairs (new ones included)."""
