@@ -579,6 +579,54 @@ int mgc_labels_create_batch(int32_t batch, int32_t ndim, const int64_t* shapes, 
 /* node_off[0 .. batch]: the first node id of every image and the total (a handle of one image: {0, K}). */
 int mgc_labels_batch_offsets(const mgc_labels* l, int64_t* node_off);
 
+/* ---- K-label segmentation by alpha-expansion (DESIGN.md §11) ------------------------------------------------------ */
+
+/* Labels 0..K-1 (2 <= K <= 255) over a lattice of shape[ndim] (1 <= ndim <= 4), minimising the Potts energy
+ *   E(l) = sum_p D_p(l_p) + sum_{lattice pairs} w_pq [l_p != l_q]
+ * by alpha-expansion (Boykov, Veksler & Zabih 2001): cycles of moves alpha = 0, 1, ..., K-1, each move one binary s-t cut
+ * of the lattice on the eager handle and mgc_maxflow, until a full cycle switches no voxel or max_cycles cycles ran.
+ *   D_p(k)  cost plane k at p widened to double; + 65535.0 (GCGraph.MAX) for every k != m-1 where the marker image holds
+ *           m > 0 (the soft-hard seed of graph_from_voxels: with K = 2, marker 1 = background, 2 = foreground, the
+ *           result is graph_from_voxels' cut)
+ *   w_pq    the float64 weight mgc_add_boundary puts on both arcs of the pair; 0 without a boundary term
+ * The move graph for alpha, its case table and the exactness argument are in DESIGN.md §11.  A voxel switches to alpha
+ * only where its move's minimal sink set puts it, so a move that switches nothing shows that no expansion on alpha lowers
+ * E.  Labels start from the init image, or argmin_k D_p(k) with ties to the lowest k.
+ * Arrays are mgc_array over the lattice shape (host or device, any positive strides), borrowed for the call.  Adding
+ * these entry points left MGC_ABI_VERSION at 3. */
+typedef struct mgc_expansion mgc_expansion;
+typedef struct mgc_expansion_stats {
+    int64_t moves;          /* moves cut by the last run                                               */
+    int64_t cycles;         /* cycles started (the last may be the one that switched nothing)          */
+    int64_t converged;      /* 1: the last cycle switched no voxel; 0: max_cycles stopped the run       */
+    double energy;          /* E of the final labels, fixed-order device sum (same labels, same bits)   */
+    double ms_build;        /* device ms of the move kernels, summed over the moves                     */
+    double ms_solve;        /* ... of mgc_maxflow (solve and read-out)                                  */
+    double ms_apply;        /* ... of the label updates                                                 */
+    double ms_total;        /* device ms of the whole run: initial labels to the energy                 */
+} mgc_expansion_stats;
+/* MGC_E_ARG for K outside 2..255 or a bad shape (as mgc_create). */
+int mgc_expansion_create(int32_t ndim, const int64_t* shape, int32_t labels, int32_t device, mgc_expansion** out);
+void mgc_expansion_destroy(mgc_expansion* e);
+const char* mgc_expansion_last_error(const mgc_expansion* e);   /* e may be NULL: last create() failure */
+/* Cost plane of one label: MGC_F32 or MGC_F64 (the same for every plane), finite and >= 0, else MGC_E_ARG. */
+int mgc_expansion_set_cost(mgc_expansion* e, int32_t label, const mgc_array* cost);
+/* The pair weights of one of the eight boundary terms, arguments as mgc_add_boundary (MGC_E_WEIGHT where it refuses);
+ * replaces the weights of an earlier call. */
+int mgc_expansion_set_boundary(mgc_expansion* e, int32_t kind, const mgc_array* image, double sigma, const double* spacing,
+                               double norm);
+/* MGC_U8 marker image, 0 = none, m = label m-1; MGC_E_ARG for a value above K. */
+int mgc_expansion_set_markers(mgc_expansion* e, const mgc_array* markers);
+/* MGC_U8 initial labels, each below K (MGC_E_ARG otherwise); mgc_expansion_run refuses (MGC_E_ARG) an init that gives a
+ * marked voxel another label than its marker. */
+int mgc_expansion_set_init(mgc_expansion* e, const mgc_array* init);
+/* MGC_E_STATE until every cost plane is set; max_cycles >= 1. */
+int mgc_expansion_run(mgc_expansion* e, int32_t max_cycles);
+/* After a run: the labels (uint8, C order, host or device), the statistics, and moves int64 switch counts, one per move. */
+int mgc_expansion_get_labels(mgc_expansion* e, uint8_t* out, int32_t mem);
+int mgc_expansion_get_stats(const mgc_expansion* e, mgc_expansion_stats* out);
+int mgc_expansion_get_switched(const mgc_expansion* e, int64_t* out);
+
 #ifdef __cplusplus
 }
 #endif

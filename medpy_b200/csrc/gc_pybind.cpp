@@ -821,6 +821,114 @@ private:
     int64_t batch_ = 1;
 };
 
+// K-label alpha-expansion over one lattice (mgc_expansion_*)
+class PyExpansion {
+public:
+    PyExpansion(const std::vector<int64_t>& shape, int labels, int device) : shape_(shape)
+    {
+        int rc = mgc_expansion_create((int32_t)shape.size(), shape.data(), labels, device, &e_);
+        if (rc != MGC_OK) { std::string m = mgc_expansion_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
+    }
+    ~PyExpansion() { if (e_) mgc_expansion_destroy(e_); }
+    PyExpansion(const PyExpansion&) = delete;
+    PyExpansion& operator=(const PyExpansion&) = delete;
+
+    void check(int rc) const
+    {
+        if (rc == MGC_OK) return;
+        std::string msg = mgc_expansion_last_error(e_);
+        if (msg.empty()) msg = "medpy_b200 expansion error " + std::to_string(rc);
+        if (rc == MGC_E_ARG || rc == MGC_E_WEIGHT) throw py::value_error(msg);
+        throw std::runtime_error(msg);
+    }
+    ArrayRef ref(const py::object& a, int want, const char* what) const
+    {
+        ArrayRef r = make_ref(a, want, what);
+        if (r.shape != shape_) throw py::value_error(std::string(what) + ": shape does not match the lattice");
+        return r;
+    }
+    void set_cost(int label, const py::object& cost)
+    {
+        ArrayRef r = ref(cost, -1, "costs");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_set_cost(e_, label, &r.a); }
+        check(rc);
+    }
+    // the GCGraph._add_boundary arguments a boundary term recorded
+    void set_boundary(int kind, const py::object& image, double sigma, const py::object& spacing, double norm)
+    {
+        ArrayRef r = ref(image, -1, "image");
+        std::vector<double> sp;
+        if (!spacing.is_none()) {
+            sp = spacing.cast<std::vector<double>>();
+            if (sp.size() < shape_.size()) throw py::value_error("spacing has fewer entries than the image has dimensions");
+        }
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_set_boundary(e_, kind, &r.a, sigma, sp.empty() ? nullptr : sp.data(), norm); }
+        check(rc);
+    }
+    void set_markers(const py::object& markers)
+    {
+        ArrayRef r = ref(markers, MGC_U8, "markers");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_set_markers(e_, &r.a); }
+        check(rc);
+    }
+    void set_init(const py::object& init)
+    {
+        ArrayRef r = ref(init, MGC_U8, "init");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_set_init(e_, &r.a); }
+        check(rc);
+    }
+    void run(int max_cycles)
+    {
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_run(e_, max_cycles); }
+        check(rc);
+    }
+    py::array_t<uint8_t> labels()
+    {
+        std::vector<py::ssize_t> shp(shape_.begin(), shape_.end());
+        py::array_t<uint8_t> out(shp);
+        int rc;
+        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_expansion_get_labels(e_, p, MGC_MEM_HOST); }
+        check(rc);
+        return out;
+    }
+    // into a contiguous uint8 device array of the lattice shape (e.g. a torch CUDA tensor)
+    void labels_into(const py::object& out)
+    {
+        ArrayRef r = ref(out, MGC_U8, "out");
+        if (r.a.mem != MGC_MEM_DEVICE) throw py::value_error("out: a device array expected");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_get_labels(e_, (uint8_t*)r.a.data, MGC_MEM_DEVICE); }
+        check(rc);
+    }
+    py::dict stats() const
+    {
+        mgc_expansion_stats s{};
+        check(mgc_expansion_get_stats(e_, &s));
+        std::vector<int64_t> sw((size_t)s.moves);
+        check(mgc_expansion_get_switched(e_, sw.data()));
+        py::dict d;
+        d["moves"] = s.moves;
+        d["cycles"] = s.cycles;
+        d["converged"] = s.converged != 0;
+        d["energy"] = s.energy;
+        d["switched"] = sw;
+        d["ms_build"] = s.ms_build;
+        d["ms_solve"] = s.ms_solve;
+        d["ms_apply"] = s.ms_apply;
+        d["ms_total"] = s.ms_total;
+        return d;
+    }
+
+private:
+    mgc_expansion* e_ = nullptr;
+    std::vector<int64_t> shape_;
+};
+
 }  // namespace
 
 py::array_t<float> gradient_magnitude_prewitt(const py::object& image, int device)
@@ -856,6 +964,16 @@ PYBIND11_MODULE(_mgc, m)
     m.attr("LABELS_STAWIASKI_DIRECTED") = MGC_LABELS_STAWIASKI_DIRECTED;
     m.attr("SUM_BINCOUNT") = MGC_SUM_BINCOUNT;
     m.attr("SUM_PAIRWISE") = MGC_SUM_PAIRWISE;
+    py::class_<PyExpansion>(m, "Expansion")
+        .def(py::init<const std::vector<int64_t>&, int, int>(), py::arg("shape"), py::arg("labels"), py::arg("device") = -1)
+        .def("set_cost", &PyExpansion::set_cost)
+        .def("set_boundary", &PyExpansion::set_boundary)
+        .def("set_markers", &PyExpansion::set_markers)
+        .def("set_init", &PyExpansion::set_init)
+        .def("run", &PyExpansion::run)
+        .def("labels", &PyExpansion::labels)
+        .def("labels_into", &PyExpansion::labels_into)
+        .def("stats", &PyExpansion::stats);
     py::class_<PySparse>(m, "SparseGraph")
         .def(py::init<int64_t, int>(), py::arg("n_nodes"), py::arg("device") = -1)
         .def("sum_edges", &PySparse::sum_edges)
