@@ -627,6 +627,39 @@ int mgc_expansion_get_labels(mgc_expansion* e, uint8_t* out, int32_t mem);
 int mgc_expansion_get_stats(const mgc_expansion* e, mgc_expansion_stats* out);
 int mgc_expansion_get_switched(const mgc_expansion* e, int64_t* out);
 
+/* Region labels 0..K-1 (2 <= K <= 255) over the R regions of a region adjacency graph (the nodes of graph_from_labels:
+ * region r of a label image is node r-1), minimising the Potts energy
+ *   E(l) = sum_r D_r(l_r) + sum_{region pairs r<s} w_rs [l_r != l_s]
+ * by alpha-expansion: cycles of moves alpha = 0, 1, ..., K-1, each move one binary s-t cut of the region graph by the
+ * sparse push-relabel, until a full cycle switches no region or max_cycles cycles ran.
+ *   D_r(k)  entry r of the cost row of label k widened to double (marker seeds, if any, are the caller's additions)
+ *   w_rs    the weight of the pair (r, s) given to mgc_region_expansion_set_pairs; 0 (no pair) otherwise
+ * The handle keeps the CSR of the pairs on the device; a move writes only its capacities and t-links there (the per-arc
+ * rules and the exactness argument are in DESIGN.md §11, "Region graphs") and a region switches to alpha only where the
+ * move's minimal sink set puts it.  Labels start from the init labels, or argmin_k D_r(k) with ties to the lowest k.
+ * Per-region arrays are 1-D mgc_array of R entries with unit stride (host or device), borrowed for the call.  The
+ * statistics are those of mgc_expansion_*, with regions in place of voxels.  Adding these entry points left
+ * MGC_ABI_VERSION at 3. */
+typedef struct mgc_region_expansion mgc_region_expansion;
+/* MGC_E_ARG for K outside 2..255 or R outside [1, 2^31-2]; device < 0: the current device. */
+int mgc_region_expansion_create(int64_t regions, int32_t labels, int32_t device, mgc_region_expansion** out);
+void mgc_region_expansion_destroy(mgc_region_expansion* e);
+const char* mgc_region_expansion_last_error(const mgc_region_expansion* e);   /* e may be NULL: last create() failure */
+/* Cost row of one label: R entries, MGC_F32 or MGC_F64 (the same for every row), finite and >= 0, else MGC_E_ARG. */
+int mgc_region_expansion_set_cost(mgc_region_expansion* e, int32_t label, const mgc_array* cost);
+/* The pairs: host arrays of `count` entries, 0 <= i[k] < j[k] < R, (i, j) strictly ascending, w finite and >= 0, else
+ * MGC_E_ARG.  A second call replaces the pairs. */
+int mgc_region_expansion_set_pairs(mgc_region_expansion* e, int64_t count, const int32_t* i, const int32_t* j,
+                                   const double* w);
+/* MGC_U8 initial region labels, each below K (MGC_E_ARG otherwise). */
+int mgc_region_expansion_set_init(mgc_region_expansion* e, const mgc_array* init);
+/* MGC_E_STATE until every cost row is set; max_cycles >= 1. */
+int mgc_region_expansion_run(mgc_region_expansion* e, int32_t max_cycles);
+/* After a run: the R region labels (uint8, host or device), the statistics, and moves int64 switch counts. */
+int mgc_region_expansion_get_labels(mgc_region_expansion* e, uint8_t* out, int32_t mem);
+int mgc_region_expansion_get_stats(const mgc_region_expansion* e, mgc_expansion_stats* out);
+int mgc_region_expansion_get_switched(const mgc_region_expansion* e, int64_t* out);
+
 #ifdef __cplusplus
 }
 #endif

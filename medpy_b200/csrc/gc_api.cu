@@ -214,6 +214,11 @@ void sum_partials(mgc_graph* g, const double* partials, unsigned n, double* out)
     k_sum_partials<<<1, 256, 0, g->stream>>>(partials, n, out);
 }
 
+void sum_partials_on(cudaStream_t s, const double* partials, unsigned n, double* out)
+{
+    k_sum_partials<<<1, 256, 0, s>>>(partials, n, out);
+}
+
 namespace {
 int finish_flow_const(mgc_graph* g)
 {

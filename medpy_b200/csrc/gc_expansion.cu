@@ -93,6 +93,31 @@ float elapsed(cudaEvent_t a, cudaEvent_t b)
 }
 }  // namespace
 
+// ---- gc_host.hpp: the element-wise kernels for the region expansion unit -------------------------------------------
+void exp_init_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dtype, const void* costs, const uint8_t* init,
+                     uint8_t* labels, int* bad)
+{
+    if (dtype == MGC_F32) k_exp_init<float><<<blocks, 256, 0, s>>>(n, K, (const float*)costs, nullptr, init, labels, bad);
+    else                  k_exp_init<double><<<blocks, 256, 0, s>>>(n, K, (const double*)costs, nullptr, init, labels, bad);
+}
+
+void exp_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* mask, uint8_t* labels, int alpha,
+                      unsigned long long* switched)
+{
+    k_exp_apply<<<blocks, 256, 0, s>>>(n, mask, labels, alpha, switched);
+}
+
+void exp_check_costs_launch(cudaStream_t s, unsigned blocks, unsigned n, int dtype, const void* cost, int* bad)
+{
+    if (dtype == MGC_F32) k_exp_check_costs<float><<<blocks, 256, 0, s>>>(n, (const float*)cost, bad);
+    else                  k_exp_check_costs<double><<<blocks, 256, 0, s>>>(n, (const double*)cost, bad);
+}
+
+void exp_check_u8_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* a, int limit, int* bad)
+{
+    k_exp_check_u8<<<blocks, 256, 0, s>>>(n, a, limit, bad);
+}
+
 extern "C" {
 
 int mgc_expansion_create(int32_t ndim, const int64_t* shape, int32_t labels, int32_t device, mgc_expansion** out)

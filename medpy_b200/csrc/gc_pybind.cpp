@@ -812,6 +812,16 @@ public:
         check(rc);
         return out;
     }
+    // the same gather into a contiguous uint8 device array of the image shape (e.g. a torch CUDA tensor)
+    void apply_into(py::array_t<uint8_t, py::array::c_style | py::array::forcecast> per_region, const py::object& out)
+    {
+        if (per_region.size() != region_count()) throw py::value_error("one value per region expected");
+        ArrayRef r = make_ref(out, MGC_U8, "out");
+        if (r.a.mem != MGC_MEM_DEVICE || r.shape != shape_) throw py::value_error("out: a device array of the image shape expected");
+        int rc;
+        { const uint8_t* q = per_region.data(); py::gil_scoped_release rel; rc = mgc_labels_apply(l_, q, (uint8_t*)r.a.data, MGC_MEM_DEVICE); }
+        check(rc);
+    }
     std::vector<int64_t> shape() const { return shape_; }
 
 private:
@@ -929,6 +939,99 @@ private:
     std::vector<int64_t> shape_;
 };
 
+// K-label alpha-expansion over a region adjacency graph (mgc_region_expansion_*)
+class PyRegionExpansion {
+public:
+    PyRegionExpansion(int64_t regions, int labels, int device) : n_(regions)
+    {
+        int rc = mgc_region_expansion_create(regions, labels, device, &e_);
+        if (rc != MGC_OK) { std::string m = mgc_region_expansion_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
+    }
+    ~PyRegionExpansion() { if (e_) mgc_region_expansion_destroy(e_); }
+    PyRegionExpansion(const PyRegionExpansion&) = delete;
+    PyRegionExpansion& operator=(const PyRegionExpansion&) = delete;
+
+    void check(int rc) const
+    {
+        if (rc == MGC_OK) return;
+        std::string msg = mgc_region_expansion_last_error(e_);
+        if (msg.empty()) msg = "medpy_b200 region expansion error " + std::to_string(rc);
+        if (rc == MGC_E_ARG) throw py::value_error(msg);
+        throw std::runtime_error(msg);
+    }
+    ArrayRef ref(const py::object& a, int want, const char* what) const
+    {
+        ArrayRef r = make_ref(a, want, what);
+        if (r.shape != std::vector<int64_t>{n_}) throw py::value_error(std::string(what) + ": one entry per region expected");
+        return r;
+    }
+    void set_cost(int label, const py::object& cost)
+    {
+        ArrayRef r = ref(cost, -1, "costs");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_region_expansion_set_cost(e_, label, &r.a); }
+        check(rc);
+    }
+    void set_pairs(py::array_t<int32_t, py::array::c_style | py::array::forcecast> i,
+                   py::array_t<int32_t, py::array::c_style | py::array::forcecast> j,
+                   py::array_t<double, py::array::c_style | py::array::forcecast> w)
+    {
+        if (i.size() != j.size() || i.size() != w.size()) throw py::value_error("i, j and w must have the same length");
+        int rc;
+        {
+            const int32_t *pi = i.data(), *pj = j.data();
+            const double* pw = w.data();
+            const int64_t m = (int64_t)i.size();
+            py::gil_scoped_release rel;
+            rc = mgc_region_expansion_set_pairs(e_, m, pi, pj, pw);
+        }
+        check(rc);
+    }
+    void set_init(const py::object& init)
+    {
+        ArrayRef r = ref(init, MGC_U8, "init");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_region_expansion_set_init(e_, &r.a); }
+        check(rc);
+    }
+    void run(int max_cycles)
+    {
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_region_expansion_run(e_, max_cycles); }
+        check(rc);
+    }
+    py::array_t<uint8_t> labels()
+    {
+        py::array_t<uint8_t> out((py::ssize_t)n_);
+        int rc;
+        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_region_expansion_get_labels(e_, p, MGC_MEM_HOST); }
+        check(rc);
+        return out;
+    }
+    py::dict stats() const
+    {
+        mgc_expansion_stats s{};
+        check(mgc_region_expansion_get_stats(e_, &s));
+        std::vector<int64_t> sw((size_t)s.moves);
+        check(mgc_region_expansion_get_switched(e_, sw.data()));
+        py::dict d;
+        d["moves"] = s.moves;
+        d["cycles"] = s.cycles;
+        d["converged"] = s.converged != 0;
+        d["energy"] = s.energy;
+        d["switched"] = sw;
+        d["ms_build"] = s.ms_build;
+        d["ms_solve"] = s.ms_solve;
+        d["ms_apply"] = s.ms_apply;
+        d["ms_total"] = s.ms_total;
+        return d;
+    }
+
+private:
+    mgc_region_expansion* e_ = nullptr;
+    int64_t n_ = 0;
+};
+
 }  // namespace
 
 py::array_t<float> gradient_magnitude_prewitt(const py::object& image, int device)
@@ -974,6 +1077,14 @@ PYBIND11_MODULE(_mgc, m)
         .def("labels", &PyExpansion::labels)
         .def("labels_into", &PyExpansion::labels_into)
         .def("stats", &PyExpansion::stats);
+    py::class_<PyRegionExpansion>(m, "RegionExpansion")
+        .def(py::init<int64_t, int, int>(), py::arg("regions"), py::arg("labels"), py::arg("device") = -1)
+        .def("set_cost", &PyRegionExpansion::set_cost)
+        .def("set_pairs", &PyRegionExpansion::set_pairs)
+        .def("set_init", &PyRegionExpansion::set_init)
+        .def("run", &PyRegionExpansion::run)
+        .def("labels", &PyRegionExpansion::labels)
+        .def("stats", &PyRegionExpansion::stats);
     py::class_<PySparse>(m, "SparseGraph")
         .def(py::init<int64_t, int>(), py::arg("n_nodes"), py::arg("device") = -1)
         .def("sum_edges", &PySparse::sum_edges)
@@ -998,6 +1109,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("region_flags", &PyLabels::region_flags)
         .def("voxel_flags", &PyLabels::voxel_flags)
         .def("apply", &PyLabels::apply)
+        .def("apply_into", &PyLabels::apply_into)
         .def_static("batch", &PyLabels::batch, py::arg("shapes"), py::arg("label_images"), py::arg("device") = -1)
         .def("batch_offsets", &PyLabels::batch_offsets)
         .def_property_readonly("shape", &PyLabels::shape);

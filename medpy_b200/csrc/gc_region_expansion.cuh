@@ -1,0 +1,69 @@
+// gc_region_expansion.cuh -- kernels of the region alpha-expansion unit (gc_region_expansion.cu, DESIGN.md §11 "Region
+// graphs"): a K-label Potts segmentation of a region adjacency graph, each move cut by the sparse push-relabel
+// (gc_sparse.cuh).  Launched by gc_region_expansion.cu only.
+//
+// The graph is the CSR of the region pairs (row, head; each row in ascending neighbour id) with the pair's weight w on
+// both of its arcs (wt).  The labelling energy E(l) = sum_r D_r(l_r) + sum_{pairs r<s} w_rs [l_r != l_s], D_r(k) =
+// costs[k * n + r] widened to double (markers are already in the costs).
+#pragma once
+#include "gc_terms.cuh"
+
+// One move for label `alpha` over the current labels: writes the sparse solver's state exactly as a fresh mgc_sparse
+// would hold it after sum_edge of every pair and add_tweights of every node -- every arc's capacity, tr, and the
+// add_tweights constant as one fixed-order partial per block (summed by k_sum_partials).  x_u = SINK means "u switches to
+// alpha".  Node u with a = l_u, arc u->v with b = l_v and weight w:
+//   snk_u += w       if a != alpha and (b == alpha or (b != a and u < v)), in the row's order
+//   cap(u->v) = w    if a != alpha and b != alpha and (a == b or u > v), else 0
+// src_u = D_u(alpha), snk_u starts at D_u(a); then add_tweights(u, src_u, snk_u) on tr = 0.
+template <typename C>
+__global__ void __launch_bounds__(256)
+k_rexp_move(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
+            const C* __restrict__ costs, const uint8_t* __restrict__ labels, int alpha, double* __restrict__ cap,
+            double* __restrict__ tr, double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = gridDim.x * blockDim.x;
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
+        const int a = labels[u];
+        const double src = (double)costs[(size_t)alpha * n + u];
+        double snk = (double)costs[(size_t)a * n + u];
+        const int end = row[u + 1];
+        for (int e = row[u]; e < end; ++e) {
+            double c = 0.0;
+            if (a != alpha) {
+                const int v = head[e];
+                const int b = labels[v];
+                const double w = wt[e];
+                if (b == alpha || (b != a && u < v)) snk = __dadd_rn(snk, w);
+                if (b != alpha && (a == b || u > v)) c = w;
+            }
+            cap[e] = c;
+        }
+        double t = 0.0;
+        m = __dadd_rn(m, add_tweights_dev(t, src, snk));
+        tr[u] = t;
+    }
+    block_sum_store(m, partials);
+}
+
+// E(l) per block in a fixed order (each node: D_u(l_u), then its pairs to higher ids in the row's order); k_sum_partials
+// adds the partials in a fixed order, so the same labels give the same bits
+template <typename C>
+__global__ void __launch_bounds__(256)
+k_rexp_energy(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
+              const C* __restrict__ costs, const uint8_t* __restrict__ labels, double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = gridDim.x * blockDim.x;
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
+        const int a = labels[u];
+        double e = (double)costs[(size_t)a * n + u];
+        const int end = row[u + 1];
+        for (int k = row[u]; k < end; ++k) {
+            const int v = head[k];
+            if (v > u && labels[v] != a) e = __dadd_rn(e, wt[k]);
+        }
+        m = __dadd_rn(m, e);
+    }
+    block_sum_store(m, partials);
+}

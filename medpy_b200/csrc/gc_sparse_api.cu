@@ -18,6 +18,7 @@
 #include "../../include/medpy_b200_graphcut.h"
 #include "gc_host.hpp"
 #include "gc_sort.cuh"
+#include "gc_sparse_held.hpp"
 #include "gc_sparse_host.hpp"
 #include "gc_sparse_warm.cuh"
 
@@ -107,13 +108,15 @@ struct mgc_sparse {
     bool segments = false;
     bool tweights_added = false;                       // add_tweights was called since create / reset
     double* seg_sunk = nullptr;
+    bool held = false;                                 // `dev` holds a topology of sparse_hold (gc_sparse_held.hpp)
     void release()
     {
         if (seg_sunk) { cudaSetDevice(device); cudaFree(seg_sunk); seg_sunk = nullptr; }
-        if (!resident) return;
+        if (!resident && !held) return;
         cudaSetDevice(device);
         dev.release();
         resident = false;
+        held = false;
     }
     ~mgc_sparse() { release(); }
 };
@@ -472,6 +475,46 @@ int warm_sum_edges(mgc_sparse* g, int64_t count, const int32_t* i, const int32_t
 }
 
 }  // namespace
+
+// ---- gc_sparse_held.hpp: a topology kept on the device, capacities written there by the caller ---------------------
+int sparse_hold(mgc_sparse* g, const std::vector<int>& row, const std::vector<int>& head, const std::vector<int>& sis,
+                SparseHeld* out)
+{
+    const int n = (int)g->host.n;
+    const int m2 = (int)head.size();
+    if ((int64_t)row.size() != (int64_t)n + 1 || sis.size() != head.size()) FAIL(MGC_E_ARG, "malformed CSR topology");
+    CK(cudaSetDevice(g->device));
+    g->release();
+    g->held = true;                                 // set first: a failed allocation is freed with the handle
+    SparseDev& d = g->dev;
+    CK(d.alloc(n, m2, false, false));
+    CK(cudaMemcpy(d.row, row.data(), ((size_t)n + 1) * sizeof(int), cudaMemcpyHostToDevice));
+    if (m2) {
+        CK(cudaMemcpy(d.head, head.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(d.sis, sis.data(), (size_t)m2 * sizeof(int), cudaMemcpyHostToDevice));
+    }
+    out->n = n;
+    out->m2 = m2;
+    out->row = d.row;
+    out->head = d.head;
+    out->cap = d.cap;
+    out->tr = d.tr;
+    return MGC_OK;
+}
+
+int sparse_solve_held(mgc_sparse* g, double base, double* energy, const uint8_t** mask)
+{
+    if (!g->held) FAIL(MGC_E_STATE, "no topology is held: call sparse_hold first");
+    CK(cudaSetDevice(g->device));
+    Events ev;
+    CK(ev.begin());
+    k_sp_init<<<grid_for(g->dev.n), 256>>>(g->dev.state());
+    g->st.kernel_launches++;
+    RC(sparse_loop(g, ev, base));
+    *energy = g->energy;
+    *mask = g->dev.mask;
+    return MGC_OK;
+}
 
 extern "C" {
 

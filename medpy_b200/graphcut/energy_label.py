@@ -115,7 +115,8 @@ def _refuse_size_one_axes(shape):
 
 def _add_edges(graph, i, j, w_there, w_back):
     from .graph import GCGraph
-    if isinstance(graph, GCGraph) and type(graph).set_nweight is GCGraph.set_nweight:
+    from .multilabel import _PairRecorder
+    if isinstance(graph, _PairRecorder) or (isinstance(graph, GCGraph) and type(graph).set_nweight is GCGraph.set_nweight):
         graph.set_nweights_bulk(i, j, w_there, w_back)
     else:   # someone else's graph object (e.g. the recording double of tests/graphcut_/energy_label.py:189-210)
         for a, b, x, y in zip(i.tolist(), j.tolist(), w_there.tolist(), w_back.tolist()):

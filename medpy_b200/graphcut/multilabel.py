@@ -1,4 +1,5 @@
-"""K-label segmentation of a voxel image by alpha-expansion (Boykov, Veksler & Zabih 2001; DESIGN.md §11).
+"""K-label segmentation of a voxel image, or of a label image's regions, by alpha-expansion (Boykov, Veksler & Zabih
+2001; DESIGN.md §11).
 
 MedPy's cut is binary: one structure against the rest.  ``expansion_from_voxels`` labels every voxel with one of K
 labels (organs, tumour sub-regions) by minimising the Potts energy whose terms ``graph_from_voxels`` already defines:
@@ -7,11 +8,17 @@ labels (organs, tumour sub-regions) by minimising the Potts energy whose terms `
 
 ``D_p(k)`` is the caller's cost of label k at p, ``w_pq`` the weight the boundary term puts on the pair.  Each move is one
 binary cut of the lattice on the GPU; the loop, the move graphs, the label updates and the energy never leave the device.
+``expansion_from_labels`` does the same over the region adjacency graph ``graph_from_labels`` builds, with the region
+sums of the caller's costs as the data term and the ``energy_label`` boundary term's weight as the pair term; each move is
+one cut of the region graph by the sparse push-relabel.
 """
 import numpy
 
 from .energy_voxel import _native_order
-from .generate import _takes_two_parameters
+from .generate import _takes_three_parameters, _takes_two_parameters
+from .graph import GCGraph
+
+_MAX = float(GCGraph.MAX)       # the soft-hard seed of a marker
 
 
 class _BoundaryRecorder:
@@ -27,8 +34,51 @@ class _BoundaryRecorder:
         self.call = (kind, image, sigma, spacing, norm)
 
 
+class _PairRecorder:
+    """What a boundary term of ``energy_label`` receives in place of a GCGraph: it keeps the term's one bulk edge call
+    (``energy_label._add_edges``), whose pairs and weights become the pair term of every move.  The Potts energy has one
+    weight per region pair, so the two directions must carry the same bits."""
+
+    def __init__(self, context):
+        self._label_context = context       # the terms reuse the staged label image
+        self.pairs = None
+
+    def set_nweights_bulk(self, i, j, w_there, w_back):
+        if self.pairs is not None:
+            raise ValueError("the boundary term added more than one set of pair weights")
+        w = numpy.ascontiguousarray(w_there, dtype=numpy.float64)
+        w_back = numpy.ascontiguousarray(w_back, dtype=numpy.float64)
+        if w.shape != w_back.shape or not numpy.array_equal(w.view(numpy.uint64), w_back.view(numpy.uint64)):
+            raise ValueError("the boundary term's weights differ between the two directions of a pair (w_ij != w_ji); "
+                             "the Potts energy takes one weight per region pair")
+        if w.size and not bool((numpy.isfinite(w) & (w >= 0)).all()):
+            raise ValueError("the boundary term's weights must be finite and >= 0")
+        self.pairs = (numpy.ascontiguousarray(i, dtype=numpy.int32), numpy.ascontiguousarray(j, dtype=numpy.int32), w)
+
+
 def _on_device(a):
     return hasattr(a, "__cuda_array_interface__")
+
+
+def _float_costs(a, what):
+    """``a`` as a float32 / float64 CUDA tensor or numpy array in native byte order."""
+    if _on_device(a):
+        if str(a.dtype) not in ("torch.float32", "torch.float64"):
+            raise ValueError("{} must be float32 or float64, got {}".format(what, a.dtype))
+        return a
+    a = _native_order(numpy.asarray(a))
+    if a.dtype not in (numpy.float32, numpy.float64):
+        raise ValueError("{} must be float32 or float64, got {}".format(what, a.dtype))
+    return a
+
+
+def _check_range(a, what):
+    if _on_device(a):
+        bad = a.numel() and not bool((a.isfinite() & (a >= 0)).all())
+    else:
+        bad = a.size and not bool((numpy.isfinite(a) & (a >= 0)).all())
+    if bad:
+        raise ValueError("{} must be finite and >= 0".format(what))
 
 
 def _label_image(a, shape, what, limit):
@@ -75,22 +125,12 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
     reaches the device.
     """
     device = -1
+    costs = _float_costs(costs, "costs")
+    if costs.ndim < 2 or costs.ndim > 5:
+        raise ValueError("costs must have shape (K, *image shape) with a 1- to 4-D image")
+    _check_range(costs, "costs")
     if _on_device(costs):
-        if str(costs.dtype) not in ("torch.float32", "torch.float64"):
-            raise ValueError("costs must be float32 or float64, got {}".format(costs.dtype))
-        if costs.dim() < 2 or costs.dim() > 5:
-            raise ValueError("costs must have shape (K, *image shape) with a 1- to 4-D image")
-        if costs.numel() and not bool((costs.isfinite() & (costs >= 0)).all()):
-            raise ValueError("costs must be finite and >= 0")
         device = costs.device.index
-    else:
-        costs = _native_order(numpy.asarray(costs))
-        if costs.dtype not in (numpy.float32, numpy.float64):
-            raise ValueError("costs must be float32 or float64, got {}".format(costs.dtype))
-        if costs.ndim < 2 or costs.ndim > 5:
-            raise ValueError("costs must have shape (K, *image shape) with a 1- to 4-D image")
-        if costs.size and not bool((numpy.isfinite(costs) & (costs >= 0)).all()):
-            raise ValueError("costs must be finite and >= 0")
     K = int(costs.shape[0])
     shape = tuple(int(s) for s in costs.shape[1:])
     if not 2 <= K <= 255:
@@ -145,3 +185,128 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
     if stats:
         return labels, st["energy"], st
     return labels, st["energy"]
+
+
+def _region_values(a, regions, what, limit):
+    """Integer region values of shape (regions,) in 0..limit, as a uint8 numpy array."""
+    if _on_device(a):
+        a = a.cpu()
+    a = numpy.asarray(a)
+    if a.shape != (regions,):
+        raise ValueError("{} must have one entry per region, shape ({},), got {}".format(what, regions, a.shape))
+    if a.dtype.kind not in "biu":
+        raise ValueError("{} must hold integers".format(what))
+    if a.size and (int(a.min()) < 0 or int(a.max()) > limit):
+        raise ValueError("{} must hold values in 0..{}".format(what, limit))
+    return numpy.ascontiguousarray(a, dtype=numpy.uint8)
+
+
+def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary_term_args=False, markers=None, init=None,
+                          max_cycles=20, stats=False, *, region_costs=None):
+    """Segment the regions of a label image into K labels by alpha-expansion (DESIGN.md §11, "Region graphs").
+
+    Minimises E(l) = sum_r D_r(l_r) + sum_{region pairs r<s} w_rs [l_r != l_s] over region labels 0..K-1
+    (2 <= K <= 255) of a 1- to 4-D label image whose ids are exactly 1..R (``AttributeError`` otherwise, as
+    ``graph_from_labels``); region r is node r-1.
+
+    label_image        the regions, e.g. supervoxels.
+    costs              (K, *label_image.shape) float32 or float64, a numpy array or a CUDA tensor, finite and >= 0:
+                       D_r(k) is the sum of ``costs[k]`` over the voxels of region r+1 (numpy.bincount's float64 sum).
+    region_costs       (K, R) float32 or float64, finite and >= 0: D_r(k) directly.  Give exactly one of the two.
+    boundary_term      an ``energy_label`` boundary term with its ``boundary_term_args``, as ``graph_from_labels`` takes
+                       them (a three-parameter callable); w_rs is the weight it puts on the pair, which must be the same
+                       in both directions.  False: no pair term.
+    markers            integer voxel image, 0 = free, m > 0 = label m-1: for every marker value in a region, every other
+                       label costs 65535 (GCGraph.MAX) more there, so a region holding two marker values pays it for
+                       every label.  With K = 2, region_costs (src, snk) of graph_from_labels' t-links and markers
+                       1 = background, 2 = foreground, the result is graph_from_labels' cut.
+    init               initial region labels, shape (R,), 0..K-1; a marked region must start at one of its markers'
+                       labels.  Default argmin_k D_r(k), ties to the lowest k.
+    max_cycles         cycles of the moves 0, 1, ..., K-1 at most; the loop stops earlier after a cycle that switches no
+                       region.
+    stats              also return a dict: moves, cycles, converged, switched (regions per move), energy and device ms.
+
+    Returns ``(labels, region_labels, energy)`` (``+ (stats,)`` with ``stats=True``): ``labels`` the uint8 voxel image
+    ``region_labels[label_image - 1]`` (a CUDA tensor when the costs are one, numpy otherwise), ``region_labels`` uint8
+    of shape (R,), ``energy`` the Potts energy of those labels.
+    """
+    if (costs is None) == (region_costs is None):
+        raise ValueError("give exactly one of costs and region_costs")
+    label_image = numpy.asarray(label_image)
+    shape = label_image.shape
+    what = "costs" if region_costs is None else "region_costs"
+    data = _float_costs(costs if region_costs is None else region_costs, what)
+    if region_costs is None and (data.ndim != label_image.ndim + 1 or tuple(data.shape[1:]) != shape):
+        raise ValueError("costs must have shape (K, *label_image.shape) = (K, {}), got {}".format(
+            ", ".join(str(s) for s in shape), tuple(data.shape)))
+    if region_costs is not None and data.ndim != 2:
+        raise ValueError("region_costs must have shape (K, R), got {}".format(tuple(data.shape)))
+    _check_range(data, what)
+    K = int(data.shape[0])
+    if not 2 <= K <= 255:
+        raise ValueError("the number of labels K = {}.shape[0] must be 2..255, got {}".format(what, K))
+    if isinstance(max_cycles, bool) or not isinstance(max_cycles, (int, numpy.integer)) or max_cycles < 1:
+        raise ValueError("max_cycles must be an integer >= 1")
+    if boundary_term and not _takes_three_parameters(boundary_term):
+        raise AttributeError("boundary_term has to be a callable object which takes three parameters.")
+    if markers is not None:
+        markers = _label_image(markers, shape, "markers", K)
+        if _on_device(markers):
+            markers = markers.cpu().numpy()
+
+    from .energy_label import LabelContext
+    on_dev = _on_device(data)
+    device = data.device.index if on_dev else -1
+    if on_dev:
+        import torch
+        torch.cuda.current_stream(device).synchronize()
+    ctx = LabelContext(label_image, device)          # stages the image; AttributeError unless the ids are 1..R
+    R = ctx.regions
+    if region_costs is not None and int(data.shape[1]) != R:
+        raise ValueError("region_costs must have shape (K, R) = ({}, {}), got {}".format(K, R, tuple(data.shape)))
+    if init is not None:
+        init = _region_values(init, R, "init", K - 1)
+
+    if region_costs is None:
+        D = numpy.empty((K, R))
+        for k in range(K):
+            D[k] = ctx.native.region_sums(data[k], ctx._mgc.SUM_BINCOUNT)[0]
+    else:
+        D = numpy.array(data.cpu().numpy() if on_dev else data, dtype=numpy.float64)
+    if markers is not None:
+        marked = numpy.zeros(R, bool)
+        agrees = numpy.zeros(R, bool)
+        for m in numpy.unique(markers):                 # ascending: the additions' order
+            if m == 0:
+                continue
+            inside = ctx.native.region_flags(numpy.ascontiguousarray(markers == m).view(numpy.uint8)).astype(bool)
+            D[numpy.ix_(numpy.arange(K) != m - 1, inside)] += _MAX
+            marked |= inside
+            if init is not None:
+                agrees |= inside & (init == m - 1)
+        if init is not None and bool((marked & ~agrees).any()):
+            raise ValueError("init gives a marked region a label none of its markers gives it")
+
+    rec = _PairRecorder(ctx)
+    if boundary_term:
+        boundary_term(rec, label_image, boundary_term_args)
+
+    nat = ctx._mgc.RegionExpansion(R, K, device)
+    for k in range(K):
+        nat.set_cost(k, D[k])
+    if rec.pairs is not None:
+        nat.set_pairs(*rec.pairs)
+    if init is not None:
+        nat.set_init(init)
+    nat.run(int(max_cycles))
+    st = nat.stats()
+    region_labels = nat.labels()
+    if on_dev:
+        import torch
+        labels = torch.empty(shape, dtype=torch.uint8, device=data.device)
+        ctx.native.apply_into(region_labels, labels)
+    else:
+        labels = ctx.apply(region_labels)
+    if stats:
+        return labels, region_labels, st["energy"], st
+    return labels, region_labels, st["energy"]
