@@ -627,6 +627,58 @@ int mgc_expansion_get_labels(mgc_expansion* e, uint8_t* out, int32_t mem);
 int mgc_expansion_get_stats(const mgc_expansion* e, mgc_expansion_stats* out);
 int mgc_expansion_get_switched(const mgc_expansion* e, int64_t* out);
 
+/* The same segmentation for B images of one shape image_shape[ndim] (1 <= ndim <= 3, B * voxels per image < 2^31), all
+ * cut together: the images are stacked along axis 0 of one batch lattice (as mgc_create_batch stacks them), and every
+ * move alpha is one move kernel, one mgc_maxflow and one label update over the whole batch.  Each image's move graphs are
+ * bit for bit those mgc_expansion_* builds for it alone, and where the tile solver returns the minimal minimum cut of
+ * every move (BK's), the image gets exactly the single run's labels, per-move switch counts, moves, cycles and converged
+ * flag, and its energy up to the order of the sums.  The tile solver's floating-point residuals can, on some graphs,
+ * leave an ulp on a saturated arc and so move voxels off the minimal cut; which graphs depends on the tile colour parity
+ * of the image's position in the lattice, so on such a graph the batch and the single run can differ (DESIGN.md §11,
+ * "Batches").  An image whose cycle switched no voxel is frozen from then on (its move
+ * graphs are empty and its labels stay): its own run would have stopped there, and its labels are a fixed point of every
+ * later move.  The batch loop stops after a cycle in which no image switched a voxel, or after max_cycles cycles.
+ * Arrays are mgc_array of shape (B, *image_shape) (host or device, any positive strides), borrowed for the call; D_p(k),
+ * markers and init have the meaning of mgc_expansion_*, image by image.  Adding these entry points left MGC_ABI_VERSION
+ * at 3. */
+typedef struct mgc_expansion_batch mgc_expansion_batch;
+/* MGC_E_ARG for K outside 2..255, a batch < 1 or a bad shape (as mgc_create_batch). */
+int mgc_expansion_batch_create(int32_t ndim, const int64_t* image_shape, int64_t batch, int32_t labels, int32_t device,
+                               mgc_expansion_batch** out);
+void mgc_expansion_batch_destroy(mgc_expansion_batch* e);
+const char* mgc_expansion_batch_last_error(const mgc_expansion_batch* e);   /* e may be NULL: last create() failure */
+/* Cost of one label for every image, (B, *image): MGC_F32 or MGC_F64 (the same for every label), finite and >= 0, else
+ * MGC_E_ARG.  costs[:, k] of a (B, K, *image) device array goes in as it is (gathered on the device). */
+int mgc_expansion_batch_set_cost(mgc_expansion_batch* e, int32_t label, const mgc_array* cost);
+/* The pair weights of one of the eight boundary terms on the (B, *image) image, with one sigma and one linear normaliser
+ * per image (NaN: reduced on the device over that image), as mgc_build_voxel_batch takes them; spacing has ndim entries
+ * or is NULL.  The weights of image b are bit for bit those mgc_expansion_set_boundary gives that image alone (what
+ * mgc_add_boundary writes on a fresh handle), 0 across the seams; MGC_E_WEIGHT where the build refuses.  Without this
+ * call every weight is 0.  Replaces the weights of an earlier call. */
+int mgc_expansion_batch_set_boundary(mgc_expansion_batch* e, int32_t kind, const mgc_array* image, const double* sigmas,
+                                     const double* spacing, const double* norms);
+/* MGC_U8 (B, *image) marker images, 0 = none, m = label m-1; MGC_E_ARG for a value above K. */
+int mgc_expansion_batch_set_markers(mgc_expansion_batch* e, const mgc_array* markers);
+/* MGC_U8 (B, *image) initial labels, each below K (MGC_E_ARG otherwise); mgc_expansion_batch_run refuses (MGC_E_ARG) an
+ * init that gives a marked voxel another label than its marker. */
+int mgc_expansion_batch_set_init(mgc_expansion_batch* e, const mgc_array* init);
+/* MGC_E_STATE until every cost plane is set; max_cycles >= 1 (per image, as mgc_expansion_run). */
+int mgc_expansion_batch_run(mgc_expansion_batch* e, int32_t max_cycles);
+/* After a run: the (B, *image) labels (uint8, C order, host or device). */
+int mgc_expansion_batch_get_labels(mgc_expansion_batch* e, uint8_t* out, int32_t mem);
+/* The batch loop: moves and cycles it ran, converged = 1 when every image converged, energy = the sum of the B image
+ * energies in image order, and the device ms of its phases. */
+int mgc_expansion_batch_get_stats(const mgc_expansion_batch* e, mgc_expansion_stats* out);
+/* out[B]: per image its moves (K x cycles), cycles (the first cycle that switched none of its voxels, or max_cycles),
+ * converged and energy (fixed-order device sum: same labels, same bits); the ms fields are 0. */
+int mgc_expansion_batch_get_image_stats(const mgc_expansion_batch* e, mgc_expansion_stats* out);
+/* out[moves x B], row-major: the voxels of image b the move switched (0 once b is frozen); image b's own switch counts
+ * are the first moves_b rows of column b. */
+int mgc_expansion_batch_get_switched(const mgc_expansion_batch* e, int64_t* out);
+/* The pair weights along image axis `axis` (0..ndim-1) as a (B, *image) float64 array, host or device: entry p holds the
+ * weight of the pair (p, p + e_axis), 0 on the last plane of the axis in every image. */
+int mgc_expansion_batch_get_weights(mgc_expansion_batch* e, int32_t axis, double* out, int32_t mem);
+
 /* Region labels 0..K-1 (2 <= K <= 255) over the R regions of a region adjacency graph (the nodes of graph_from_labels:
  * region r of a label image is node r-1), minimising the Potts energy
  *   E(l) = sum_r D_r(l_r) + sum_{region pairs r<s} w_rs [l_r != l_s]

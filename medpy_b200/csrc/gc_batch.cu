@@ -297,6 +297,13 @@ int batch_constants(mgc_graph* g, int dtype, const void* d_img, BoundaryParams* 
     return MGC_OK;
 }
 
+// out[b] = the fixed-order sum of partials[b * n .. (b + 1) * n), for every image b (k_batch_sum)
+void batch_sum(mgc_graph* g, const double* partials, unsigned n, double* out)
+{
+    k_batch_sum<<<(unsigned)g->batch, 256, 0, g->stream>>>(partials, n, nullptr, out);
+    g->st.kernel_launches++;
+}
+
 // the per-image add_tweights constants of the build whose t-link inputs A holds
 int batch_tconst(mgc_graph* g, const BuildArgs& A)
 {

@@ -93,12 +93,19 @@ float elapsed(cudaEvent_t a, cudaEvent_t b)
 }
 }  // namespace
 
-// ---- gc_host.hpp: the element-wise kernels for the region expansion unit -------------------------------------------
+// ---- gc_host.hpp: the element-wise kernels for the region and batch expansion units -------------------------------------------
 void exp_init_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dtype, const void* costs, const uint8_t* init,
                      uint8_t* labels, int* bad)
 {
     if (dtype == MGC_F32) k_exp_init<float><<<blocks, 256, 0, s>>>(n, K, (const float*)costs, nullptr, init, labels, bad);
     else                  k_exp_init<double><<<blocks, 256, 0, s>>>(n, K, (const double*)costs, nullptr, init, labels, bad);
+}
+
+void exp_init_marked_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dtype, const void* costs,
+                            const uint8_t* markers, const uint8_t* init, uint8_t* labels, int* bad)
+{
+    if (dtype == MGC_F32) k_exp_init<float><<<blocks, 256, 0, s>>>(n, K, (const float*)costs, markers, init, labels, bad);
+    else                  k_exp_init<double><<<blocks, 256, 0, s>>>(n, K, (const double*)costs, markers, init, labels, bad);
 }
 
 void exp_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* mask, uint8_t* labels, int alpha,

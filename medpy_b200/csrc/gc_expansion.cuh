@@ -6,19 +6,7 @@
 //   w_pq    the float64 weight graph_from_voxels puts on both arcs of the pair: k_boundary's own output, kept per axis in
 //           w[d][p] for the pair (p, p + e_d) (0 on the last plane of d)
 #pragma once
-#include "gc_terms.cuh"
-
-struct ExpWeights {
-    const double* w[4];      // canonical axes
-};
-
-template <typename C>
-__device__ __forceinline__ double exp_cost(const C* __restrict__ costs, unsigned n, unsigned v, int k, int mark)
-{
-    double d = (double)costs[(size_t)k * n + v];
-    if (mark && mark - 1 != k) d = __dadd_rn(d, 65535.0);
-    return d;
-}
+#include "gc_expansion_cost.cuh"
 
 // One move for label `alpha` over the current labels: writes the eager handle's state exactly as mgc_add_tweights_dense +
 // mgc_add_nweights_dense leave it on a fresh handle -- every capacity plane entry (0 where no arc), tr, and the

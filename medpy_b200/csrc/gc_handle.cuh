@@ -247,6 +247,7 @@ int voxel_build(mgc_graph* g, const mgc_voxel_terms* t);
 // ---- gc_batch.cu ----------------------------------------------------------------------------------------
 int batch_constants(mgc_graph* g, int dtype, const void* d_img, BoundaryParams* P);
 int batch_tconst(mgc_graph* g, const BuildArgs& A);
+void batch_sum(mgc_graph* g, const double* partials, unsigned n, double* out);
 int batch_view(mgc_graph* g, const mgc_array* a, int slot, mgc_array* out);
 size_t batch_fold_chunks(int max_count);
 int batch_fold_const(mgc_graph* g, const unsigned* vox, int vstride, const int* count, int max_count, const double* dk,

@@ -112,3 +112,6 @@ void exp_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t
                       unsigned long long* switched);
 void exp_check_costs_launch(cudaStream_t s, unsigned blocks, unsigned n, int dtype, const void* cost, int* bad);
 void exp_check_u8_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* a, int limit, int* bad);
+// k_exp_init with a marker image (nullptr: none), for the batch expansion unit
+void exp_init_marked_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dtype, const void* costs,
+                            const uint8_t* markers, const uint8_t* init, uint8_t* labels, int* bad);

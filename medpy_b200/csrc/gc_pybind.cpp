@@ -939,6 +939,161 @@ private:
     std::vector<int64_t> shape_;
 };
 
+// K-label alpha-expansion of a batch of images of one shape, every move one cut of the whole batch (mgc_expansion_batch_*)
+class PyExpansionBatch {
+public:
+    PyExpansionBatch(const std::vector<int64_t>& image_shape, int64_t batch, int labels, int device) : shape_(image_shape)
+    {
+        int rc = mgc_expansion_batch_create((int32_t)image_shape.size(), image_shape.data(), batch, labels, device, &e_);
+        if (rc != MGC_OK) { std::string m = mgc_expansion_batch_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
+        shape_.insert(shape_.begin(), batch);
+    }
+    ~PyExpansionBatch() { if (e_) mgc_expansion_batch_destroy(e_); }
+    PyExpansionBatch(const PyExpansionBatch&) = delete;
+    PyExpansionBatch& operator=(const PyExpansionBatch&) = delete;
+
+    void check(int rc) const
+    {
+        if (rc == MGC_OK) return;
+        std::string msg = mgc_expansion_batch_last_error(e_);
+        if (msg.empty()) msg = "medpy_b200 batch expansion error " + std::to_string(rc);
+        if (rc == MGC_E_ARG || rc == MGC_E_WEIGHT) throw py::value_error(msg);
+        throw std::runtime_error(msg);
+    }
+    ArrayRef ref(const py::object& a, int want, const char* what) const
+    {
+        ArrayRef r = make_ref(a, want, what);
+        if (r.shape != shape_) throw py::value_error(std::string(what) + ": shape does not match (batch, *image)");
+        return r;
+    }
+    // (batch, *image), any positive strides
+    void set_cost(int label, const py::object& cost)
+    {
+        ArrayRef r = ref(cost, -1, "costs");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_batch_set_cost(e_, label, &r.a); }
+        check(rc);
+    }
+    // one sigma and one normaliser per image (NaN: reduced on the device), as build_voxel_batch takes them
+    void set_boundary(int kind, const py::object& image, const std::vector<double>& sigmas, const py::object& spacing,
+                      const std::vector<double>& norms)
+    {
+        if ((int64_t)sigmas.size() != shape_[0] || (int64_t)norms.size() != shape_[0])
+            throw py::value_error("sigmas and norms need one entry per image");
+        ArrayRef r = ref(image, -1, "image");
+        std::vector<double> sp;
+        if (!spacing.is_none()) {
+            sp = spacing.cast<std::vector<double>>();
+            if (sp.size() + 1 < shape_.size()) throw py::value_error("spacing has fewer entries than the images have dimensions");
+        }
+        int rc;
+        {
+            py::gil_scoped_release rel;
+            rc = mgc_expansion_batch_set_boundary(e_, kind, &r.a, sigmas.data(), sp.empty() ? nullptr : sp.data(), norms.data());
+        }
+        check(rc);
+    }
+    void set_markers(const py::object& markers)
+    {
+        ArrayRef r = ref(markers, MGC_U8, "markers");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_batch_set_markers(e_, &r.a); }
+        check(rc);
+    }
+    void set_init(const py::object& init)
+    {
+        ArrayRef r = ref(init, MGC_U8, "init");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_batch_set_init(e_, &r.a); }
+        check(rc);
+    }
+    void run(int max_cycles)
+    {
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_batch_run(e_, max_cycles); }
+        check(rc);
+    }
+    py::array_t<uint8_t> labels()
+    {
+        std::vector<py::ssize_t> shp(shape_.begin(), shape_.end());
+        py::array_t<uint8_t> out(shp);
+        int rc;
+        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_expansion_batch_get_labels(e_, p, MGC_MEM_HOST); }
+        check(rc);
+        return out;
+    }
+    // into a contiguous uint8 device array of shape (batch, *image) (e.g. a torch CUDA tensor)
+    void labels_into(const py::object& out)
+    {
+        ArrayRef r = ref(out, MGC_U8, "out");
+        if (r.a.mem != MGC_MEM_DEVICE) throw py::value_error("out: a device array expected");
+        int rc;
+        { py::gil_scoped_release rel; rc = mgc_expansion_batch_get_labels(e_, (uint8_t*)r.a.data, MGC_MEM_DEVICE); }
+        check(rc);
+    }
+    // the batch loop: moves, cycles, converged (every image), energy (the sum over the images) and device ms
+    py::dict stats() const
+    {
+        mgc_expansion_stats s{};
+        check(mgc_expansion_batch_get_stats(e_, &s));
+        py::dict d;
+        d["moves"] = s.moves;
+        d["cycles"] = s.cycles;
+        d["converged"] = s.converged != 0;
+        d["energy"] = s.energy;
+        d["ms_build"] = s.ms_build;
+        d["ms_solve"] = s.ms_solve;
+        d["ms_apply"] = s.ms_apply;
+        d["ms_total"] = s.ms_total;
+        return d;
+    }
+    // per image: arrays of moves, cycles, converged and energy
+    py::dict image_stats() const
+    {
+        const size_t B = (size_t)shape_[0];
+        std::vector<mgc_expansion_stats> s(B);
+        check(mgc_expansion_batch_get_image_stats(e_, s.data()));
+        py::array_t<int64_t> moves((py::ssize_t)B), cycles((py::ssize_t)B);
+        py::array_t<bool> conv((py::ssize_t)B);
+        py::array_t<double> energy((py::ssize_t)B);
+        for (size_t b = 0; b < B; ++b) {
+            moves.mutable_data()[b] = s[b].moves;
+            cycles.mutable_data()[b] = s[b].cycles;
+            conv.mutable_data()[b] = s[b].converged != 0;
+            energy.mutable_data()[b] = s[b].energy;
+        }
+        py::dict d;
+        d["moves"] = moves;
+        d["cycles"] = cycles;
+        d["converged"] = conv;
+        d["energy"] = energy;
+        return d;
+    }
+    // (moves, batch) int64: the voxels of every image each move switched
+    py::array_t<int64_t> switched() const
+    {
+        mgc_expansion_stats s{};
+        check(mgc_expansion_batch_get_stats(e_, &s));
+        py::array_t<int64_t> out({(py::ssize_t)s.moves, (py::ssize_t)shape_[0]});
+        check(mgc_expansion_batch_get_switched(e_, out.mutable_data()));
+        return out;
+    }
+    // the pair weights along image axis `axis`, shape (batch, *image)
+    py::array_t<double> weights(int axis)
+    {
+        std::vector<py::ssize_t> shp(shape_.begin(), shape_.end());
+        py::array_t<double> out(shp);
+        int rc;
+        { double* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_expansion_batch_get_weights(e_, axis, p, MGC_MEM_HOST); }
+        check(rc);
+        return out;
+    }
+
+private:
+    mgc_expansion_batch* e_ = nullptr;
+    std::vector<int64_t> shape_;
+};
+
 // K-label alpha-expansion over a region adjacency graph (mgc_region_expansion_*)
 class PyRegionExpansion {
 public:
@@ -1077,6 +1232,20 @@ PYBIND11_MODULE(_mgc, m)
         .def("labels", &PyExpansion::labels)
         .def("labels_into", &PyExpansion::labels_into)
         .def("stats", &PyExpansion::stats);
+    py::class_<PyExpansionBatch>(m, "ExpansionBatch")
+        .def(py::init<const std::vector<int64_t>&, int64_t, int, int>(), py::arg("image_shape"), py::arg("batch"),
+             py::arg("labels"), py::arg("device") = -1)
+        .def("set_cost", &PyExpansionBatch::set_cost)
+        .def("set_boundary", &PyExpansionBatch::set_boundary)
+        .def("set_markers", &PyExpansionBatch::set_markers)
+        .def("set_init", &PyExpansionBatch::set_init)
+        .def("run", &PyExpansionBatch::run)
+        .def("labels", &PyExpansionBatch::labels)
+        .def("labels_into", &PyExpansionBatch::labels_into)
+        .def("stats", &PyExpansionBatch::stats)
+        .def("image_stats", &PyExpansionBatch::image_stats)
+        .def("switched", &PyExpansionBatch::switched)
+        .def("weights", &PyExpansionBatch::weights);
     py::class_<PyRegionExpansion>(m, "RegionExpansion")
         .def(py::init<int64_t, int, int>(), py::arg("regions"), py::arg("labels"), py::arg("device") = -1)
         .def("set_cost", &PyRegionExpansion::set_cost)

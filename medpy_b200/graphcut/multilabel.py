@@ -10,8 +10,11 @@ labels (organs, tumour sub-regions) by minimising the Potts energy whose terms `
 binary cut of the lattice on the GPU; the loop, the move graphs, the label updates and the energy never leave the device.
 ``expansion_from_labels`` does the same over the region adjacency graph ``graph_from_labels`` builds, with the region
 sums of the caller's costs as the data term and the ``energy_label`` boundary term's weight as the pair term; each move is
-one cut of the region graph by the sparse push-relabel.
+one cut of the region graph by the sparse push-relabel.  ``expansion_from_voxels_batch`` segments B images of one shape
+together, every move one cut of the whole batch lattice, each image exactly as ``expansion_from_voxels`` segments it alone.
 """
+import math
+
 import numpy
 
 from .energy_voxel import _native_order
@@ -185,6 +188,125 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
     if stats:
         return labels, st["energy"], st
     return labels, st["energy"]
+
+
+def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, spacing=False, markers=None, init=None,
+                                max_cycles=20, stats=False):
+    """Segment B images of one shape into K labels by alpha-expansion, all in one loop (DESIGN.md §11, "Batches").
+
+    Image b is segmented as ``expansion_from_voxels`` segments it alone: the same energy, bit for bit the same move
+    graphs, the same stopping rule and ``max_cycles``.  Where the lattice solver returns each move's minimal minimum cut
+    (as BK does), the labels, per-move switch counts, moves, cycles and converged flag are the single call's, and the
+    energy is its energy up to the order of the sums.  The solver's floating-point residuals can move voxels off that
+    cut on some graphs, depending on the image's tile position, so there the two calls can differ (DESIGN.md §11,
+    "Batches").  Every move alpha is one cut of the whole batch; an image whose cycle switched nothing is frozen from
+    then on, and the loop stops when every image is frozen or ``max_cycles`` cycles ran.
+
+    costs              (B, K, *image) float32 or float64, a numpy array or a CUDA tensor, finite and >= 0; ``costs[b, k]``
+                       is the cost of label k in image b.  2 <= K <= 255, images 1- to 3-D, B x voxels per image < 2^31.
+    image, boundary    the (B, *image) image (numpy or CUDA) and one of the eight ``energy_voxel`` boundary terms by name
+                       without the ``boundary_`` prefix (``"difference_exponential"`` ...), as ``graph_from_voxels_batch``
+                       takes them.  None: no pair term.
+    sigma              the term's sigma: one float for every image, or one per image.
+    spacing            voxel spacing of the images (one entry per image axis), or False.
+    markers, init      (B, *image) integer images with the meaning ``expansion_from_voxels`` gives them per image.
+    max_cycles         cycles of the moves 0, 1, ..., K-1 at most, per image.
+    stats              also return a dict: the batch loop's ``batch_moves``, ``batch_cycles``, ``batch_converged``, per-image
+                       lists ``moves``, ``cycles``, ``converged``, ``switched`` (voxels per move) and ``energy``, and the
+                       device ms (``ms_build``, ``ms_solve``, ``ms_apply`` summed over the moves, ``ms_total``).
+
+    Returns ``(labels, energies)`` (``+ (stats,)`` with ``stats=True``): uint8 labels of shape (B, *image), a numpy array
+    or, for CUDA costs, a CUDA tensor; ``energies`` a float64 numpy array of the B Potts energies.  Raises ``ValueError``
+    for malformed arguments before anything reaches the device.
+    """
+    from .batch import INDEX_LIMIT, _host_image, _is_cuda, _sigmas
+    from .device import _KINDS
+    costs = _float_costs(costs, "costs")
+    if costs.ndim < 3 or costs.ndim > 5:
+        raise ValueError("costs must have shape (B, K, *image shape) with a 1- to 3-D image")
+    _check_range(costs, "costs")
+    B, K = int(costs.shape[0]), int(costs.shape[1])
+    shape = tuple(int(s) for s in costs.shape[2:])
+    if not 2 <= K <= 255:
+        raise ValueError("the number of labels K = costs.shape[1] must be 2..255, got {}".format(K))
+    if B < 1 or min(shape) < 1:
+        raise ValueError("the batch and its images must not be empty")
+    if B * math.prod(shape) >= INDEX_LIMIT:
+        raise ValueError("{} images of {} voxels reach the 2^31 voxel index limit of one batch".format(B, math.prod(shape)))
+    if isinstance(max_cycles, bool) or not isinstance(max_cycles, (int, numpy.integer)) or max_cycles < 1:
+        raise ValueError("max_cycles must be an integer >= 1")
+    bshape = (B,) + shape
+    if (image is None) != (boundary is None):
+        raise ValueError("give both image and boundary for a pair term, or neither")
+    if boundary is not None:
+        if boundary not in _KINDS:
+            raise ValueError("boundary must be one of {}, got {!r}".format(sorted(_KINDS), boundary))
+        if tuple(int(s) for s in image.shape) != bshape:
+            raise ValueError("image has shape {}, the costs need {}".format(tuple(image.shape), bshape))
+        sigmas = _sigmas(sigma, B)
+        sp = None
+        if spacing:
+            sp = [float(s) for s in spacing]
+            if len(sp) < len(shape):
+                raise ValueError("spacing has fewer entries than the images have dimensions")
+        if _is_cuda(image):
+            norms = [math.nan] * B
+        else:
+            image, norms = _host_image(image, boundary)
+
+    if markers is not None:
+        markers = _label_image(markers, bshape, "markers", K)
+    if init is not None:
+        init = _label_image(init, bshape, "init", K - 1)
+        if markers is not None:
+            if _on_device(markers) and _on_device(init):
+                m, i = markers.long(), init.long()
+            else:       # one side on the host: compare there
+                m, i = (numpy.asarray(a.cpu() if _on_device(a) else a, dtype=numpy.int64) for a in (markers, init))
+            if bool(((m > 0) & (i != m - 1)).any()):
+                raise ValueError("init gives a marked voxel another label than its marker")
+
+    from .. import _lib  # raises ImportError loudly when the extension is not built
+    on_dev = _on_device(costs)
+    device = costs.device.index if on_dev else -1
+    if on_dev or _on_device(markers) or _on_device(init) or (boundary is not None and _on_device(image)):
+        import torch
+        torch.cuda.current_stream(device if device >= 0 else None).synchronize()
+    nat = _lib._mgc.ExpansionBatch(list(shape), B, K, device)
+    for k in range(K):
+        # a host plane goes contiguous (a strided host array would upload its whole span); a CUDA plane is gathered there
+        nat.set_cost(k, costs[:, k] if on_dev else numpy.ascontiguousarray(costs[:, k]))
+    if boundary is not None:
+        nat.set_boundary(_KINDS[boundary], image, sigmas, sp, norms)
+    if markers is not None:
+        nat.set_markers(markers)
+    if init is not None:
+        nat.set_init(init)
+    nat.run(int(max_cycles))
+    per = nat.image_stats()
+    energies = numpy.asarray(per["energy"], dtype=numpy.float64)
+    if on_dev:
+        import torch
+        labels = torch.empty(bshape, dtype=torch.uint8, device=costs.device)
+        nat.labels_into(labels)
+    else:
+        labels = nat.labels()
+    if not stats:
+        return labels, energies
+    return labels, energies, _batch_stats(nat.stats(), per, nat.switched())
+
+
+def _batch_stats(total, per, switched):
+    """The stats dict of ``expansion_from_voxels_batch`` from the native batch totals, the per-image statistics and the
+    (moves, B) switch matrix: image b's switch counts are the first ``moves[b]`` rows of column b."""
+    switched = numpy.asarray(switched, dtype=numpy.int64)
+    moves = [int(m) for m in per["moves"]]
+    return dict(batch_moves=int(total["moves"]), batch_cycles=int(total["cycles"]), batch_converged=bool(total["converged"]),
+                moves=moves, cycles=[int(c) for c in per["cycles"]], converged=[bool(c) for c in per["converged"]],
+                switched=[switched[:m, b].tolist() for b, m in enumerate(moves)],
+                energy=[float(e) for e in per["energy"]],
+                ms_build=total["ms_build"], ms_solve=total["ms_solve"], ms_apply=total["ms_apply"],
+                ms_total=total["ms_total"])
 
 
 def _region_values(a, regions, what, limit):
