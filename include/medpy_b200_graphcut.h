@@ -593,7 +593,11 @@ int mgc_labels_batch_offsets(const mgc_labels* l, int64_t* node_off);
  * only where its move's minimal sink set puts it, so a move that switches nothing shows that no expansion on alpha lowers
  * E.  Labels start from the init image, or argmin_k D_p(k) with ties to the lowest k.
  * Arrays are mgc_array over the lattice shape (host or device, any positive strides), borrowed for the call.  Adding
- * these entry points left MGC_ABI_VERSION at 3. */
+ * these entry points left MGC_ABI_VERSION at 3.
+ * A refused input leaves nothing behind, here and in mgc_expansion_batch_* and mgc_region_expansion_*: set_cost,
+ * set_markers and set_init unset that input (the label's costs, the markers, the init) and the last run's results before
+ * they read it, and set it only once it passed its checks.  So after a refused cost plane the run returns MGC_E_STATE
+ * until the label's costs are set again, and after refused markers or init it runs without them. */
 typedef struct mgc_expansion mgc_expansion;
 typedef struct mgc_expansion_stats {
     int64_t moves;          /* moves cut by the last run                                               */

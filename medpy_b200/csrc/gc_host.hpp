@@ -103,15 +103,3 @@ void lab_scan_blocks(const unsigned* cnt, long long nb, unsigned long long* out)
 
 // k_sum_partials, compiled into gc_api.cu only, on stream `s`: *out += the fixed-order sum of partials[0..n)
 void sum_partials_on(cudaStream_t s, const double* partials, unsigned n, double* out);
-
-// the element-wise kernels of gc_expansion.cuh the region expansion unit launches too, compiled into gc_expansion.cu
-// only; `dtype` (MGC_F32 / MGC_F64) selects the cost type, and k_exp_init runs without markers
-void exp_init_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dtype, const void* costs, const uint8_t* init,
-                     uint8_t* labels, int* bad);
-void exp_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* mask, uint8_t* labels, int alpha,
-                      unsigned long long* switched);
-void exp_check_costs_launch(cudaStream_t s, unsigned blocks, unsigned n, int dtype, const void* cost, int* bad);
-void exp_check_u8_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* a, int limit, int* bad);
-// k_exp_init with a marker image (nullptr: none), for the batch expansion unit
-void exp_init_marked_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dtype, const void* costs,
-                            const uint8_t* markers, const uint8_t* init, uint8_t* labels, int* bad);

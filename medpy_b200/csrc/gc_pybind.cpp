@@ -831,22 +831,55 @@ private:
     int64_t batch_ = 1;
 };
 
-// K-label alpha-expansion over one lattice (mgc_expansion_*)
-class PyExpansion {
+// The C ABI of one expansion unit, by handle type: the calls every expansion class makes
+template <typename H> struct ExpansionAbi;
+template <> struct ExpansionAbi<mgc_expansion> {
+    static constexpr auto destroy = mgc_expansion_destroy;
+    static constexpr auto last_error = mgc_expansion_last_error;
+    static constexpr auto set_cost = mgc_expansion_set_cost;
+    static constexpr auto set_markers = mgc_expansion_set_markers;
+    static constexpr auto set_init = mgc_expansion_set_init;
+    static constexpr auto run = mgc_expansion_run;
+    static constexpr auto get_labels = mgc_expansion_get_labels;
+    static constexpr auto get_stats = mgc_expansion_get_stats;
+    static constexpr auto get_switched = mgc_expansion_get_switched;
+};
+template <> struct ExpansionAbi<mgc_expansion_batch> {
+    static constexpr auto destroy = mgc_expansion_batch_destroy;
+    static constexpr auto last_error = mgc_expansion_batch_last_error;
+    static constexpr auto set_cost = mgc_expansion_batch_set_cost;
+    static constexpr auto set_markers = mgc_expansion_batch_set_markers;
+    static constexpr auto set_init = mgc_expansion_batch_set_init;
+    static constexpr auto run = mgc_expansion_batch_run;
+    static constexpr auto get_labels = mgc_expansion_batch_get_labels;
+    static constexpr auto get_stats = mgc_expansion_batch_get_stats;
+    static constexpr auto get_switched = mgc_expansion_batch_get_switched;
+};
+template <> struct ExpansionAbi<mgc_region_expansion> {     // no markers: they are in the caller's costs
+    static constexpr auto destroy = mgc_region_expansion_destroy;
+    static constexpr auto last_error = mgc_region_expansion_last_error;
+    static constexpr auto set_cost = mgc_region_expansion_set_cost;
+    static constexpr auto set_init = mgc_region_expansion_set_init;
+    static constexpr auto run = mgc_region_expansion_run;
+    static constexpr auto get_labels = mgc_region_expansion_get_labels;
+    static constexpr auto get_stats = mgc_region_expansion_get_stats;
+    static constexpr auto get_switched = mgc_region_expansion_get_switched;
+};
+
+// What the three K-label alpha-expansion classes share: every array has the handle's shape (`shape_`), and a refused
+// call raises ValueError for MGC_E_ARG / MGC_E_WEIGHT, RuntimeError otherwise
+template <typename H>
+class PyExpansionBase {
 public:
-    PyExpansion(const std::vector<int64_t>& shape, int labels, int device) : shape_(shape)
-    {
-        int rc = mgc_expansion_create((int32_t)shape.size(), shape.data(), labels, device, &e_);
-        if (rc != MGC_OK) { std::string m = mgc_expansion_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
-    }
-    ~PyExpansion() { if (e_) mgc_expansion_destroy(e_); }
-    PyExpansion(const PyExpansion&) = delete;
-    PyExpansion& operator=(const PyExpansion&) = delete;
+    using Abi = ExpansionAbi<H>;
+    ~PyExpansionBase() { if (e_) Abi::destroy(e_); }
+    PyExpansionBase(const PyExpansionBase&) = delete;
+    PyExpansionBase& operator=(const PyExpansionBase&) = delete;
 
     void check(int rc) const
     {
         if (rc == MGC_OK) return;
-        std::string msg = mgc_expansion_last_error(e_);
+        std::string msg = Abi::last_error(e_);
         if (msg.empty()) msg = "medpy_b200 expansion error " + std::to_string(rc);
         if (rc == MGC_E_ARG || rc == MGC_E_WEIGHT) throw py::value_error(msg);
         throw std::runtime_error(msg);
@@ -854,15 +887,100 @@ public:
     ArrayRef ref(const py::object& a, int want, const char* what) const
     {
         ArrayRef r = make_ref(a, want, what);
-        if (r.shape != shape_) throw py::value_error(std::string(what) + ": shape does not match the lattice");
+        if (r.shape != shape_) throw py::value_error(std::string(what) + ": " + mismatch_);
         return r;
     }
     void set_cost(int label, const py::object& cost)
     {
         ArrayRef r = ref(cost, -1, "costs");
         int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_set_cost(e_, label, &r.a); }
+        { py::gil_scoped_release rel; rc = Abi::set_cost(e_, label, &r.a); }
         check(rc);
+    }
+    void set_markers(const py::object& markers)
+    {
+        ArrayRef r = ref(markers, MGC_U8, "markers");
+        int rc;
+        { py::gil_scoped_release rel; rc = Abi::set_markers(e_, &r.a); }
+        check(rc);
+    }
+    void set_init(const py::object& init)
+    {
+        ArrayRef r = ref(init, MGC_U8, "init");
+        int rc;
+        { py::gil_scoped_release rel; rc = Abi::set_init(e_, &r.a); }
+        check(rc);
+    }
+    void run(int max_cycles)
+    {
+        int rc;
+        { py::gil_scoped_release rel; rc = Abi::run(e_, max_cycles); }
+        check(rc);
+    }
+    py::array_t<uint8_t> labels()
+    {
+        std::vector<py::ssize_t> shp(shape_.begin(), shape_.end());
+        py::array_t<uint8_t> out(shp);
+        int rc;
+        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = Abi::get_labels(e_, p, MGC_MEM_HOST); }
+        check(rc);
+        return out;
+    }
+    // into a contiguous uint8 device array of the handle's shape (e.g. a torch CUDA tensor)
+    void labels_into(const py::object& out)
+    {
+        ArrayRef r = ref(out, MGC_U8, "out");
+        if (r.a.mem != MGC_MEM_DEVICE) throw py::value_error("out: a device array expected");
+        int rc;
+        { py::gil_scoped_release rel; rc = Abi::get_labels(e_, (uint8_t*)r.a.data, MGC_MEM_DEVICE); }
+        check(rc);
+    }
+    // moves, cycles, converged, energy, switched (one count per move) and device ms
+    py::dict stats() const { return stats_dict(true); }
+
+protected:
+    PyExpansionBase(std::vector<int64_t> shape, const char* mismatch) : shape_(std::move(shape)), mismatch_(mismatch) {}
+    // after the unit's create(): raise its refusal
+    void created(int rc) const
+    {
+        if (rc == MGC_OK) return;
+        std::string m = Abi::last_error(nullptr);
+        if (rc == MGC_E_ARG) throw py::value_error(m);
+        throw std::runtime_error(m);
+    }
+    py::dict stats_dict(bool with_switched) const
+    {
+        mgc_expansion_stats s{};
+        check(Abi::get_stats(e_, &s));
+        py::dict d;
+        d["moves"] = s.moves;
+        d["cycles"] = s.cycles;
+        d["converged"] = s.converged != 0;
+        d["energy"] = s.energy;
+        if (with_switched) {
+            std::vector<int64_t> sw((size_t)s.moves);
+            check(Abi::get_switched(e_, sw.data()));
+            d["switched"] = sw;
+        }
+        d["ms_build"] = s.ms_build;
+        d["ms_solve"] = s.ms_solve;
+        d["ms_apply"] = s.ms_apply;
+        d["ms_total"] = s.ms_total;
+        return d;
+    }
+
+    H* e_ = nullptr;
+    std::vector<int64_t> shape_;
+    const char* mismatch_;
+};
+
+// K-label alpha-expansion over one lattice (mgc_expansion_*)
+class PyExpansion : public PyExpansionBase<mgc_expansion> {
+public:
+    PyExpansion(const std::vector<int64_t>& shape, int labels, int device)
+        : PyExpansionBase(shape, "shape does not match the lattice")
+    {
+        created(mgc_expansion_create((int32_t)shape.size(), shape.data(), labels, device, &e_));
     }
     // the GCGraph._add_boundary arguments a boundary term recorded
     void set_boundary(int kind, const py::object& image, double sigma, const py::object& spacing, double norm)
@@ -877,102 +995,17 @@ public:
         { py::gil_scoped_release rel; rc = mgc_expansion_set_boundary(e_, kind, &r.a, sigma, sp.empty() ? nullptr : sp.data(), norm); }
         check(rc);
     }
-    void set_markers(const py::object& markers)
-    {
-        ArrayRef r = ref(markers, MGC_U8, "markers");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_set_markers(e_, &r.a); }
-        check(rc);
-    }
-    void set_init(const py::object& init)
-    {
-        ArrayRef r = ref(init, MGC_U8, "init");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_set_init(e_, &r.a); }
-        check(rc);
-    }
-    void run(int max_cycles)
-    {
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_run(e_, max_cycles); }
-        check(rc);
-    }
-    py::array_t<uint8_t> labels()
-    {
-        std::vector<py::ssize_t> shp(shape_.begin(), shape_.end());
-        py::array_t<uint8_t> out(shp);
-        int rc;
-        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_expansion_get_labels(e_, p, MGC_MEM_HOST); }
-        check(rc);
-        return out;
-    }
-    // into a contiguous uint8 device array of the lattice shape (e.g. a torch CUDA tensor)
-    void labels_into(const py::object& out)
-    {
-        ArrayRef r = ref(out, MGC_U8, "out");
-        if (r.a.mem != MGC_MEM_DEVICE) throw py::value_error("out: a device array expected");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_get_labels(e_, (uint8_t*)r.a.data, MGC_MEM_DEVICE); }
-        check(rc);
-    }
-    py::dict stats() const
-    {
-        mgc_expansion_stats s{};
-        check(mgc_expansion_get_stats(e_, &s));
-        std::vector<int64_t> sw((size_t)s.moves);
-        check(mgc_expansion_get_switched(e_, sw.data()));
-        py::dict d;
-        d["moves"] = s.moves;
-        d["cycles"] = s.cycles;
-        d["converged"] = s.converged != 0;
-        d["energy"] = s.energy;
-        d["switched"] = sw;
-        d["ms_build"] = s.ms_build;
-        d["ms_solve"] = s.ms_solve;
-        d["ms_apply"] = s.ms_apply;
-        d["ms_total"] = s.ms_total;
-        return d;
-    }
-
-private:
-    mgc_expansion* e_ = nullptr;
-    std::vector<int64_t> shape_;
 };
 
-// K-label alpha-expansion of a batch of images of one shape, every move one cut of the whole batch (mgc_expansion_batch_*)
-class PyExpansionBatch {
+// K-label alpha-expansion of a batch of images of one shape, every move one cut of the whole batch
+// (mgc_expansion_batch_*); arrays are (batch, *image) with any positive strides
+class PyExpansionBatch : public PyExpansionBase<mgc_expansion_batch> {
 public:
-    PyExpansionBatch(const std::vector<int64_t>& image_shape, int64_t batch, int labels, int device) : shape_(image_shape)
+    PyExpansionBatch(const std::vector<int64_t>& image_shape, int64_t batch, int labels, int device)
+        : PyExpansionBase(image_shape, "shape does not match (batch, *image)")
     {
-        int rc = mgc_expansion_batch_create((int32_t)image_shape.size(), image_shape.data(), batch, labels, device, &e_);
-        if (rc != MGC_OK) { std::string m = mgc_expansion_batch_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
+        created(mgc_expansion_batch_create((int32_t)image_shape.size(), image_shape.data(), batch, labels, device, &e_));
         shape_.insert(shape_.begin(), batch);
-    }
-    ~PyExpansionBatch() { if (e_) mgc_expansion_batch_destroy(e_); }
-    PyExpansionBatch(const PyExpansionBatch&) = delete;
-    PyExpansionBatch& operator=(const PyExpansionBatch&) = delete;
-
-    void check(int rc) const
-    {
-        if (rc == MGC_OK) return;
-        std::string msg = mgc_expansion_batch_last_error(e_);
-        if (msg.empty()) msg = "medpy_b200 batch expansion error " + std::to_string(rc);
-        if (rc == MGC_E_ARG || rc == MGC_E_WEIGHT) throw py::value_error(msg);
-        throw std::runtime_error(msg);
-    }
-    ArrayRef ref(const py::object& a, int want, const char* what) const
-    {
-        ArrayRef r = make_ref(a, want, what);
-        if (r.shape != shape_) throw py::value_error(std::string(what) + ": shape does not match (batch, *image)");
-        return r;
-    }
-    // (batch, *image), any positive strides
-    void set_cost(int label, const py::object& cost)
-    {
-        ArrayRef r = ref(cost, -1, "costs");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_batch_set_cost(e_, label, &r.a); }
-        check(rc);
     }
     // one sigma and one normaliser per image (NaN: reduced on the device), as build_voxel_batch takes them
     void set_boundary(int kind, const py::object& image, const std::vector<double>& sigmas, const py::object& spacing,
@@ -993,60 +1026,8 @@ public:
         }
         check(rc);
     }
-    void set_markers(const py::object& markers)
-    {
-        ArrayRef r = ref(markers, MGC_U8, "markers");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_batch_set_markers(e_, &r.a); }
-        check(rc);
-    }
-    void set_init(const py::object& init)
-    {
-        ArrayRef r = ref(init, MGC_U8, "init");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_batch_set_init(e_, &r.a); }
-        check(rc);
-    }
-    void run(int max_cycles)
-    {
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_batch_run(e_, max_cycles); }
-        check(rc);
-    }
-    py::array_t<uint8_t> labels()
-    {
-        std::vector<py::ssize_t> shp(shape_.begin(), shape_.end());
-        py::array_t<uint8_t> out(shp);
-        int rc;
-        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_expansion_batch_get_labels(e_, p, MGC_MEM_HOST); }
-        check(rc);
-        return out;
-    }
-    // into a contiguous uint8 device array of shape (batch, *image) (e.g. a torch CUDA tensor)
-    void labels_into(const py::object& out)
-    {
-        ArrayRef r = ref(out, MGC_U8, "out");
-        if (r.a.mem != MGC_MEM_DEVICE) throw py::value_error("out: a device array expected");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_expansion_batch_get_labels(e_, (uint8_t*)r.a.data, MGC_MEM_DEVICE); }
-        check(rc);
-    }
     // the batch loop: moves, cycles, converged (every image), energy (the sum over the images) and device ms
-    py::dict stats() const
-    {
-        mgc_expansion_stats s{};
-        check(mgc_expansion_batch_get_stats(e_, &s));
-        py::dict d;
-        d["moves"] = s.moves;
-        d["cycles"] = s.cycles;
-        d["converged"] = s.converged != 0;
-        d["energy"] = s.energy;
-        d["ms_build"] = s.ms_build;
-        d["ms_solve"] = s.ms_solve;
-        d["ms_apply"] = s.ms_apply;
-        d["ms_total"] = s.ms_total;
-        return d;
-    }
+    py::dict stats() const { return stats_dict(false); }
     // per image: arrays of moves, cycles, converged and energy
     py::dict image_stats() const
     {
@@ -1088,44 +1069,14 @@ public:
         check(rc);
         return out;
     }
-
-private:
-    mgc_expansion_batch* e_ = nullptr;
-    std::vector<int64_t> shape_;
 };
 
-// K-label alpha-expansion over a region adjacency graph (mgc_region_expansion_*)
-class PyRegionExpansion {
+// K-label alpha-expansion over a region adjacency graph (mgc_region_expansion_*); per-region arrays are (regions,)
+class PyRegionExpansion : public PyExpansionBase<mgc_region_expansion> {
 public:
-    PyRegionExpansion(int64_t regions, int labels, int device) : n_(regions)
+    PyRegionExpansion(int64_t regions, int labels, int device) : PyExpansionBase({regions}, "one entry per region expected")
     {
-        int rc = mgc_region_expansion_create(regions, labels, device, &e_);
-        if (rc != MGC_OK) { std::string m = mgc_region_expansion_last_error(nullptr); if (rc == MGC_E_ARG) throw py::value_error(m); throw std::runtime_error(m); }
-    }
-    ~PyRegionExpansion() { if (e_) mgc_region_expansion_destroy(e_); }
-    PyRegionExpansion(const PyRegionExpansion&) = delete;
-    PyRegionExpansion& operator=(const PyRegionExpansion&) = delete;
-
-    void check(int rc) const
-    {
-        if (rc == MGC_OK) return;
-        std::string msg = mgc_region_expansion_last_error(e_);
-        if (msg.empty()) msg = "medpy_b200 region expansion error " + std::to_string(rc);
-        if (rc == MGC_E_ARG) throw py::value_error(msg);
-        throw std::runtime_error(msg);
-    }
-    ArrayRef ref(const py::object& a, int want, const char* what) const
-    {
-        ArrayRef r = make_ref(a, want, what);
-        if (r.shape != std::vector<int64_t>{n_}) throw py::value_error(std::string(what) + ": one entry per region expected");
-        return r;
-    }
-    void set_cost(int label, const py::object& cost)
-    {
-        ArrayRef r = ref(cost, -1, "costs");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_region_expansion_set_cost(e_, label, &r.a); }
-        check(rc);
+        created(mgc_region_expansion_create(regions, labels, device, &e_));
     }
     void set_pairs(py::array_t<int32_t, py::array::c_style | py::array::forcecast> i,
                    py::array_t<int32_t, py::array::c_style | py::array::forcecast> j,
@@ -1142,49 +1093,6 @@ public:
         }
         check(rc);
     }
-    void set_init(const py::object& init)
-    {
-        ArrayRef r = ref(init, MGC_U8, "init");
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_region_expansion_set_init(e_, &r.a); }
-        check(rc);
-    }
-    void run(int max_cycles)
-    {
-        int rc;
-        { py::gil_scoped_release rel; rc = mgc_region_expansion_run(e_, max_cycles); }
-        check(rc);
-    }
-    py::array_t<uint8_t> labels()
-    {
-        py::array_t<uint8_t> out((py::ssize_t)n_);
-        int rc;
-        { uint8_t* p = out.mutable_data(); py::gil_scoped_release rel; rc = mgc_region_expansion_get_labels(e_, p, MGC_MEM_HOST); }
-        check(rc);
-        return out;
-    }
-    py::dict stats() const
-    {
-        mgc_expansion_stats s{};
-        check(mgc_region_expansion_get_stats(e_, &s));
-        std::vector<int64_t> sw((size_t)s.moves);
-        check(mgc_region_expansion_get_switched(e_, sw.data()));
-        py::dict d;
-        d["moves"] = s.moves;
-        d["cycles"] = s.cycles;
-        d["converged"] = s.converged != 0;
-        d["energy"] = s.energy;
-        d["switched"] = sw;
-        d["ms_build"] = s.ms_build;
-        d["ms_solve"] = s.ms_solve;
-        d["ms_apply"] = s.ms_apply;
-        d["ms_total"] = s.ms_total;
-        return d;
-    }
-
-private:
-    mgc_region_expansion* e_ = nullptr;
-    int64_t n_ = 0;
 };
 
 }  // namespace

@@ -105,6 +105,26 @@ def _label_image(a, shape, what, limit):
     return numpy.ascontiguousarray(a, dtype=numpy.uint8)
 
 
+def _check_labels_and_cycles(K, where, max_cycles):
+    """K (the labels, from the costs' axis `where`) in 2..255 and max_cycles an integer >= 1."""
+    if not 2 <= K <= 255:
+        raise ValueError("the number of labels K = {} must be 2..255, got {}".format(where, K))
+    if isinstance(max_cycles, bool) or not isinstance(max_cycles, (int, numpy.integer)) or max_cycles < 1:
+        raise ValueError("max_cycles must be an integer >= 1")
+
+
+def _check_init_markers(markers, init):
+    """Refuse an init that gives a marked voxel another label than its marker (either may be None)."""
+    if markers is None or init is None:
+        return
+    if _on_device(markers) and _on_device(init):
+        m, i = markers.long(), init.long()
+    else:       # one side on the host: compare there
+        m, i = (numpy.asarray(a.cpu() if _on_device(a) else a, dtype=numpy.int64) for a in (markers, init))
+    if bool(((m > 0) & (i != m - 1)).any()):
+        raise ValueError("init gives a marked voxel another label than its marker")
+
+
 def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, markers=None, init=None, max_cycles=20,
                           stats=False):
     """Segment a voxel image into K labels by alpha-expansion.
@@ -136,12 +156,9 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
         device = costs.device.index
     K = int(costs.shape[0])
     shape = tuple(int(s) for s in costs.shape[1:])
-    if not 2 <= K <= 255:
-        raise ValueError("the number of labels K = costs.shape[0] must be 2..255, got {}".format(K))
+    _check_labels_and_cycles(K, "costs.shape[0]", max_cycles)
     if min(shape) < 1:
         raise ValueError("the image must not be empty")
-    if isinstance(max_cycles, bool) or not isinstance(max_cycles, (int, numpy.integer)) or max_cycles < 1:
-        raise ValueError("max_cycles must be an integer >= 1")
 
     rec = _BoundaryRecorder()
     if boundary_term:
@@ -155,13 +172,7 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
         markers = _label_image(markers, shape, "markers", K)
     if init is not None:
         init = _label_image(init, shape, "init", K - 1)
-        if markers is not None:
-            if _on_device(markers) and _on_device(init):
-                m, i = markers.long(), init.long()
-            else:       # one side on the host: compare there
-                m, i = (numpy.asarray(a.cpu() if _on_device(a) else a, dtype=numpy.int64) for a in (markers, init))
-            if bool(((m > 0) & (i != m - 1)).any()):
-                raise ValueError("init gives a marked voxel another label than its marker")
+    _check_init_markers(markers, init)
 
     from .. import _lib  # raises ImportError loudly when the extension is not built
     on_dev = _on_device(costs)
@@ -227,14 +238,11 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
     _check_range(costs, "costs")
     B, K = int(costs.shape[0]), int(costs.shape[1])
     shape = tuple(int(s) for s in costs.shape[2:])
-    if not 2 <= K <= 255:
-        raise ValueError("the number of labels K = costs.shape[1] must be 2..255, got {}".format(K))
+    _check_labels_and_cycles(K, "costs.shape[1]", max_cycles)
     if B < 1 or min(shape) < 1:
         raise ValueError("the batch and its images must not be empty")
     if B * math.prod(shape) >= INDEX_LIMIT:
         raise ValueError("{} images of {} voxels reach the 2^31 voxel index limit of one batch".format(B, math.prod(shape)))
-    if isinstance(max_cycles, bool) or not isinstance(max_cycles, (int, numpy.integer)) or max_cycles < 1:
-        raise ValueError("max_cycles must be an integer >= 1")
     bshape = (B,) + shape
     if (image is None) != (boundary is None):
         raise ValueError("give both image and boundary for a pair term, or neither")
@@ -258,13 +266,7 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
         markers = _label_image(markers, bshape, "markers", K)
     if init is not None:
         init = _label_image(init, bshape, "init", K - 1)
-        if markers is not None:
-            if _on_device(markers) and _on_device(init):
-                m, i = markers.long(), init.long()
-            else:       # one side on the host: compare there
-                m, i = (numpy.asarray(a.cpu() if _on_device(a) else a, dtype=numpy.int64) for a in (markers, init))
-            if bool(((m > 0) & (i != m - 1)).any()):
-                raise ValueError("init gives a marked voxel another label than its marker")
+    _check_init_markers(markers, init)
 
     from .. import _lib  # raises ImportError loudly when the extension is not built
     on_dev = _on_device(costs)
@@ -365,10 +367,7 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
         raise ValueError("region_costs must have shape (K, R), got {}".format(tuple(data.shape)))
     _check_range(data, what)
     K = int(data.shape[0])
-    if not 2 <= K <= 255:
-        raise ValueError("the number of labels K = {}.shape[0] must be 2..255, got {}".format(what, K))
-    if isinstance(max_cycles, bool) or not isinstance(max_cycles, (int, numpy.integer)) or max_cycles < 1:
-        raise ValueError("max_cycles must be an integer >= 1")
+    _check_labels_and_cycles(K, what + ".shape[0]", max_cycles)
     if boundary_term and not _takes_three_parameters(boundary_term):
         raise AttributeError("boundary_term has to be a callable object which takes three parameters.")
     if markers is not None:
