@@ -624,6 +624,15 @@ int mgc_expansion_set_markers(mgc_expansion* e, const mgc_array* markers);
 /* MGC_U8 initial labels, each below K (MGC_E_ARG otherwise); mgc_expansion_run refuses (MGC_E_ARG) an init that gives a
  * marked voxel another label than its marker. */
 int mgc_expansion_set_init(mgc_expansion* e, const mgc_array* init);
+/* A metric label distance: the pair term becomes w_pq V(l_p, l_q) in place of w_pq [l_p != l_q].  dist holds K x K host
+ * doubles, row-major, borrowed for the call; every entry finite and >= 0, V[a][a] == 0, V[a][b] == V[b][a], and
+ * V[a][c] <= V[a][b] + V[b][c] in float64 (zero off the diagonal is allowed).  A matrix that breaks a rule is refused
+ * (MGC_E_ARG, the message names the rule and the first (a, b) or (a, b, c)) and leaves the handle on Potts, as NULL does.
+ * Semi-metrics such as truncated quadratic break the triangle inequality: alpha-expansion cannot cut them exactly.  The
+ * move graph with a distance is in DESIGN.md §11, "Label distances"; V = 1 - I gives the Potts move graphs bit for bit.
+ * Adding it, mgc_expansion_batch_set_label_distance and mgc_region_expansion_set_label_distance left MGC_ABI_VERSION
+ * at 3. */
+int mgc_expansion_set_label_distance(mgc_expansion* e, const double* dist);
 /* MGC_E_STATE until every cost plane is set; max_cycles >= 1. */
 int mgc_expansion_run(mgc_expansion* e, int32_t max_cycles);
 /* After a run: the labels (uint8, C order, host or device), the statistics, and moves int64 switch counts, one per move. */
@@ -666,6 +675,8 @@ int mgc_expansion_batch_set_markers(mgc_expansion_batch* e, const mgc_array* mar
 /* MGC_U8 (B, *image) initial labels, each below K (MGC_E_ARG otherwise); mgc_expansion_batch_run refuses (MGC_E_ARG) an
  * init that gives a marked voxel another label than its marker. */
 int mgc_expansion_batch_set_init(mgc_expansion_batch* e, const mgc_array* init);
+/* The label distance of every image, as mgc_expansion_set_label_distance (NULL: Potts). */
+int mgc_expansion_batch_set_label_distance(mgc_expansion_batch* e, const double* dist);
 /* MGC_E_STATE until every cost plane is set; max_cycles >= 1 (per image, as mgc_expansion_run). */
 int mgc_expansion_batch_run(mgc_expansion_batch* e, int32_t max_cycles);
 /* After a run: the (B, *image) labels (uint8, C order, host or device). */
@@ -709,6 +720,8 @@ int mgc_region_expansion_set_pairs(mgc_region_expansion* e, int64_t count, const
                                    const double* w);
 /* MGC_U8 initial region labels, each below K (MGC_E_ARG otherwise). */
 int mgc_region_expansion_set_init(mgc_region_expansion* e, const mgc_array* init);
+/* The label distance, as mgc_expansion_set_label_distance (NULL: Potts): the pair term becomes w_rs V(l_r, l_s). */
+int mgc_region_expansion_set_label_distance(mgc_region_expansion* e, const double* dist);
 /* MGC_E_STATE until every cost row is set; max_cycles >= 1. */
 int mgc_region_expansion_run(mgc_region_expansion* e, int32_t max_cycles);
 /* After a run: the R region labels (uint8, host or device), the statistics, and moves int64 switch counts. */

@@ -33,8 +33,13 @@ void move_launch(mgc_expansion* e, int alpha)
     mgc_graph* g = e->g;
     ExpWeights W{};
     for (int d = 0; d < ND; ++d) W.w[d] = e->w + (size_t)d * g->L.n;
-    k_exp_move<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, (const C*)e->costs, e->have_markers ? e->markers : nullptr,
-                                                         e->labels, W, alpha, g->partials);
+    const C* costs = (const C*)e->costs;
+    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
+    if (e->have_dist)
+        k_exp_move_m<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, W, e->dist, e->K, alpha,
+                                                               g->partials);
+    else
+        k_exp_move<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, W, alpha, g->partials);
 }
 
 template <typename C, int ND>
@@ -43,8 +48,12 @@ void energy_launch(mgc_expansion* e)
     mgc_graph* g = e->g;
     ExpWeights W{};
     for (int d = 0; d < ND; ++d) W.w[d] = e->w + (size_t)d * g->L.n;
-    k_exp_energy<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, (const C*)e->costs, e->have_markers ? e->markers : nullptr,
-                                                           e->labels, W, g->partials);
+    const C* costs = (const C*)e->costs;
+    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
+    if (e->have_dist)
+        k_exp_energy_m<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, costs, mk, e->labels, W, e->dist, e->K, g->partials);
+    else
+        k_exp_energy<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, costs, mk, e->labels, W, g->partials);
 }
 
 template <int ND>
@@ -176,6 +185,7 @@ int mgc_expansion_set_boundary(mgc_expansion* e, int32_t kind, const mgc_array* 
 
 int mgc_expansion_set_markers(mgc_expansion* e, const mgc_array* markers) { return e ? e->set_markers(markers) : MGC_E_ARG; }
 int mgc_expansion_set_init(mgc_expansion* e, const mgc_array* init) { return e ? e->set_init(init) : MGC_E_ARG; }
+int mgc_expansion_set_label_distance(mgc_expansion* e, const double* dist) { return e ? e->set_label_distance(dist) : MGC_E_ARG; }
 int mgc_expansion_run(mgc_expansion* e, int32_t max_cycles) { return e ? e->run(max_cycles) : MGC_E_ARG; }
 int mgc_expansion_get_labels(mgc_expansion* e, uint8_t* out, int32_t mem) { return e ? e->get_labels(out, mem) : MGC_E_ARG; }
 int mgc_expansion_get_stats(const mgc_expansion* e, mgc_expansion_stats* out) { return e ? e->get_stats(out) : MGC_E_ARG; }

@@ -5,8 +5,12 @@
 //   D_p(k)  cost plane k at p widened to double, + GCGraph.MAX (65535) when p is marked with a label other than k
 //   w_pq    the float64 weight graph_from_voxels puts on both arcs of the pair: k_boundary's own output, kept per axis in
 //           w[d][p] for the pair (p, p + e_d) (0 on the last plane of d)
+//
+// With a label distance V (DESIGN.md §11, "Label distances") the pair term is w_pq V(l_p, l_q): k_exp_move_m and
+// k_exp_energy_m.
 #pragma once
 #include "gc_expansion_cost.cuh"
+#include "gc_expansion_metric.cuh"
 
 // One move for label `alpha` over the current labels: writes the eager handle's state exactly as mgc_add_tweights_dense +
 // mgc_add_nweights_dense leave it on a fresh handle -- every capacity plane entry (0 where no arc), tr, and the
@@ -54,6 +58,75 @@ k_exp_move(Lattice L, State<double> S, const C* __restrict__ costs, const uint8_
         double tr = 0.0;
         m = __dadd_rn(m, add_tweights_dev(tr, src, snk));
         S.tr[v] = tr;
+    }
+    block_sum_store(m, partials);
+}
+
+// k_exp_move with the pair term w_pq V(l_p, l_q) of a metric label distance (DESIGN.md §11, "Label distances"): each pair
+// adds what exp_metric_pair says, in k_exp_move's order and to its planes.  A voxel labelled alpha has no arcs and no
+// pair contributions, as there.
+template <typename C, int ND>
+__global__ void __launch_bounds__(256)
+k_exp_move_m(Lattice L, State<double> S, const C* __restrict__ costs, const uint8_t* __restrict__ markers,
+             const uint8_t* __restrict__ labels, ExpWeights W, const double* __restrict__ V, int K, int alpha,
+             double* __restrict__ partials)
+{
+    double m = 0.0;
+    const unsigned step = gridDim.x * blockDim.x;
+    for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < L.n; v += step) {
+        int c[ND];
+        decode<ND>(L, v, c);
+        const int lp = labels[v];
+        const int mk = markers ? markers[v] : 0;
+        const double src = exp_cost(costs, L.n, v, alpha, mk);
+        double snk = exp_cost(costs, L.n, v, lp, mk);
+#pragma unroll
+        for (int d = 0; d < ND; ++d) {
+            double lo_c = 0.0, up_c = 0.0, fwd = 0.0, bwd = 0.0;
+            if (c[d] + 1 < L.dim[d] && lp != alpha) {            // p is the lower end of (p, p + e_d)
+                const ExpPair r = exp_metric_pair(W.w[d][v], V, K, lp, labels[v + L.stride[d]], alpha);
+                lo_c = r.lo;
+                fwd = r.fwd;
+            }
+            if (c[d] > 0 && lp != alpha) {                       // p is the upper end of (p - e_d, p)
+                const unsigned o = v - L.stride[d];
+                const ExpPair r = exp_metric_pair(W.w[d][o], V, K, labels[o], lp, alpha);
+                up_c = r.up;
+                bwd = r.bwd;
+            }
+            snk = __dadd_rn(snk, lo_c);
+            snk = __dadd_rn(snk, up_c);
+            S.cap[2 * d + 1][v] = fwd;
+            S.cap[2 * d][v] = bwd;
+        }
+        double tr = 0.0;
+        m = __dadd_rn(m, add_tweights_dev(tr, src, snk));
+        S.tr[v] = tr;
+    }
+    block_sum_store(m, partials);
+}
+
+// k_exp_energy with w_pq V(l_p, l_q) in place of w_pq for a lower-end pair whose labels differ
+template <typename C, int ND>
+__global__ void __launch_bounds__(256)
+k_exp_energy_m(Lattice L, const C* __restrict__ costs, const uint8_t* __restrict__ markers, const uint8_t* __restrict__ labels,
+               ExpWeights W, const double* __restrict__ V, int K, double* __restrict__ partials)
+{
+    double m = 0.0;
+    const unsigned step = gridDim.x * blockDim.x;
+    for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < L.n; v += step) {
+        int c[ND];
+        decode<ND>(L, v, c);
+        const int lp = labels[v];
+        double e = exp_cost(costs, L.n, v, lp, markers ? markers[v] : 0);
+#pragma unroll
+        for (int d = 0; d < ND; ++d) {
+            if (c[d] + 1 < L.dim[d]) {
+                const int lq = labels[v + L.stride[d]];
+                if (lq != lp) e = __dadd_rn(e, exp_dist(W.w[d][v], V, K, lp, lq));
+            }
+        }
+        m = __dadd_rn(m, e);
     }
     block_sum_store(m, partials);
 }

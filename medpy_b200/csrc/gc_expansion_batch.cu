@@ -64,14 +64,41 @@ namespace {
 thread_local std::string g_bexp_create_error;
 }  // namespace
 
+namespace {
+template <typename C>
+void bexp_move_launch(mgc_expansion_batch* e, int alpha)
+{
+    mgc_graph* g = e->g;
+    const C* costs = (const C*)e->costs;
+    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
+    if (e->have_dist)
+        k_bexp_move_m<C><<<e->blocks, 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, e->weights(), e->dist, e->K,
+                                                           e->d_active, alpha, g->partials);
+    else
+        k_bexp_move<C><<<e->blocks, 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, e->weights(), e->d_active, alpha,
+                                                         g->partials);
+}
+
+template <typename C>
+void bexp_energy_launch(mgc_expansion_batch* e)
+{
+    mgc_graph* g = e->g;
+    const unsigned chunks = (unsigned)g->batch_chunks;
+    const C* costs = (const C*)e->costs;
+    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
+    if (e->have_dist)
+        k_bexp_energy_m<C><<<(unsigned)e->B * chunks, 256, 0, g->stream>>>(g->L, costs, mk, e->labels, e->weights(), e->dist,
+                                                                           e->K, chunks, e->d_part);
+    else
+        k_bexp_energy<C><<<(unsigned)e->B * chunks, 256, 0, g->stream>>>(g->L, costs, mk, e->labels, e->weights(), chunks,
+                                                                         e->d_part);
+}
+}  // namespace
+
 int mgc_expansion_batch::build(int alpha)
 {
-    if (cost_dtype == MGC_F32)
-        k_bexp_move<float><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const float*)costs, have_markers ? markers : nullptr,
-                                                          labels, weights(), d_active, alpha, g->partials);
-    else
-        k_bexp_move<double><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const double*)costs, have_markers ? markers : nullptr,
-                                                           labels, weights(), d_active, alpha, g->partials);
+    if (cost_dtype == MGC_F32) bexp_move_launch<float>(this, alpha);
+    else                       bexp_move_launch<double>(this, alpha);
     CK(cudaGetLastError());
     sum_partials(g, g->partials, blocks, g->d_scalars);     // the add_tweights constant of the active images
     g->caps_fresh = false;
@@ -83,16 +110,10 @@ int mgc_expansion_batch::build(int alpha)
 
 int mgc_expansion_batch::energy()
 {
-    const unsigned chunks = (unsigned)g->batch_chunks;
-    const uint8_t* mk = have_markers ? markers : nullptr;
-    if (cost_dtype == MGC_F32)
-        k_bexp_energy<float><<<(unsigned)B * chunks, 256, 0, g->stream>>>(g->L, (const float*)costs, mk, labels, weights(),
-                                                                         chunks, d_part);
-    else
-        k_bexp_energy<double><<<(unsigned)B * chunks, 256, 0, g->stream>>>(g->L, (const double*)costs, mk, labels, weights(),
-                                                                          chunks, d_part);
+    if (cost_dtype == MGC_F32) bexp_energy_launch<float>(this);
+    else                       bexp_energy_launch<double>(this);
     CK(cudaGetLastError());
-    batch_sum(g, d_part, chunks, d_energy);
+    batch_sum(g, d_part, (unsigned)g->batch_chunks, d_energy);
     return MGC_OK;
 }
 
@@ -172,6 +193,11 @@ int mgc_expansion_batch_set_boundary(mgc_expansion_batch* e, int32_t kind, const
 
 int mgc_expansion_batch_set_markers(mgc_expansion_batch* e, const mgc_array* markers) { return e ? e->set_markers(markers) : MGC_E_ARG; }
 int mgc_expansion_batch_set_init(mgc_expansion_batch* e, const mgc_array* init) { return e ? e->set_init(init) : MGC_E_ARG; }
+int mgc_expansion_batch_set_label_distance(mgc_expansion_batch* e, const double* dist)
+{
+    return e ? e->set_label_distance(dist) : MGC_E_ARG;
+}
+
 int mgc_expansion_batch_run(mgc_expansion_batch* e, int32_t max_cycles) { return e ? e->run(max_cycles) : MGC_E_ARG; }
 int mgc_expansion_batch_get_labels(mgc_expansion_batch* e, uint8_t* out, int32_t mem) { return e ? e->get_labels(out, mem) : MGC_E_ARG; }
 int mgc_expansion_batch_get_stats(const mgc_expansion_batch* e, mgc_expansion_stats* out) { return e ? e->get_stats(out) : MGC_E_ARG; }

@@ -3,6 +3,7 @@
 #include "gc_expansion_loop.hpp"
 
 #include <algorithm>
+#include <cmath>
 
 namespace {
 float elapsed(cudaEvent_t a, cudaEvent_t b)
@@ -17,6 +18,39 @@ int expansion_check_labels(int K, std::string& err)
     if (K >= 2 && K <= 255) return MGC_OK;
     err = "the number of labels must be 2..255";
     return MGC_E_ARG;
+}
+
+int expansion_check_distance(const double* V, int K, std::string& err)
+{
+    const auto at = [&](int a, int b) { return V[(size_t)a * K + b]; };
+    const auto pair = [](int a, int b) { return "V[" + std::to_string(a) + "][" + std::to_string(b) + "]"; };
+    for (int a = 0; a < K; ++a)
+        for (int b = 0; b < K; ++b)
+            if (!std::isfinite(at(a, b)) || !(at(a, b) >= 0.0)) {
+                err = "label_distance must be finite and >= 0, " + pair(a, b) + " is not";
+                return MGC_E_ARG;
+            }
+    for (int a = 0; a < K; ++a)
+        if (at(a, a) != 0.0) {
+            err = "label_distance must have a zero diagonal, " + pair(a, a) + " is not 0";
+            return MGC_E_ARG;
+        }
+    for (int a = 0; a < K; ++a)
+        for (int b = a + 1; b < K; ++b)
+            if (at(a, b) != at(b, a)) {
+                err = "label_distance must be symmetric, " + pair(a, b) + " != " + pair(b, a);
+                return MGC_E_ARG;
+            }
+    for (int a = 0; a < K; ++a)
+        for (int b = 0; b < K; ++b)
+            for (int c = 0; c < K; ++c)
+                if (at(a, c) > at(a, b) + at(b, c)) {
+                    err = "label_distance must satisfy the triangle inequality V[a][c] <= V[a][b] + V[b][c], (a, b, c) = (" +
+                          std::to_string(a) + ", " + std::to_string(b) + ", " + std::to_string(c) +
+                          ") breaks it; a semi-metric such as truncated quadratic needs alpha-beta swap moves";
+                    return MGC_E_ARG;
+                }
+    return MGC_OK;
 }
 
 // In the members below `g` is the handle itself: the CK and FAIL macros of gc_host.hpp report into g->err.
@@ -108,6 +142,22 @@ int Expansion::set_u8(const mgc_array* a, uint8_t** dst, bool* have, int limit, 
 int Expansion::set_markers(const mgc_array* a) { return set_u8(a, &markers, &have_markers, K, "markers"); }
 
 int Expansion::set_init(const mgc_array* a) { return set_u8(a, &init, &have_init, K - 1, "init"); }
+
+int Expansion::set_label_distance(const double* host_V)
+{
+    Expansion* const g = this;
+    have_dist = false;
+    ran = false;
+    if (!host_V) return MGC_OK;
+    RC(expansion_check_distance(host_V, K, err));
+    CK(cudaSetDevice(device));
+    const size_t bytes = (size_t)K * K * sizeof(double);
+    if (!dist) RC(alloc(bytes, (void**)&dist));
+    CK(cudaMemcpyAsync(dist, host_V, bytes, cudaMemcpyHostToDevice, stream));
+    CK(cudaStreamSynchronize(stream));      // the caller's matrix is borrowed for the call only
+    have_dist = true;
+    return MGC_OK;
+}
 
 int Expansion::run(int max_cycles)
 {

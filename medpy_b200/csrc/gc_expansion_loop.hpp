@@ -5,8 +5,8 @@
 // loop with B = 1.  The loop is gc_expansion_loop.cu; the element-wise kernels it launches are compiled into
 // gc_expansion.cu only, behind the launchers at the end of this file.
 //
-// A refused input leaves nothing behind: set_cost, set_markers and set_init clear the input's flag and `ran` before they
-// stage it, and set the flag only once the input passed its check, so run never sees a refused input.
+// A refused input leaves nothing behind: set_cost, set_markers, set_init and set_label_distance clear the input's flag and
+// `ran` before they stage it, and set the flag only once the input passed its check, so run never sees a refused input.
 #pragma once
 #include "gc_host.hpp"
 
@@ -47,6 +47,8 @@ struct Expansion {
     int set_cost(int label, const mgc_array* cost);
     int set_markers(const mgc_array* markers);
     int set_init(const mgc_array* init);
+    // the K x K host matrix of a metric label distance (checked here, uploaded to `dist`), nullptr: back to Potts
+    int set_label_distance(const double* host_V);
     int run(int max_cycles);
     int get_labels(uint8_t* out, int mem);
     int get_stats(mgc_expansion_stats* out) const;
@@ -67,6 +69,8 @@ struct Expansion {
     uint8_t* markers = nullptr;         // 0 none, m > 0: label m - 1
     uint8_t* init = nullptr;
     bool have_markers = false, have_init = false;
+    double* dist = nullptr;             // K x K label distance, row-major; a unit's build and energy hooks take the metric
+    bool have_dist = false;             // kernels while it is set, the Potts ones otherwise
     unsigned long long* d_switched = nullptr;   // [B] elements the current move switched per image
     double* d_energy = nullptr;                 // [B]
     int* d_bad = nullptr;
@@ -83,6 +87,10 @@ private:
 
 // the create() check of every unit: MGC_E_ARG with the message in `err` unless 2 <= K <= 255
 int expansion_check_labels(int K, std::string& err);
+// MGC_E_ARG with the message in `err` unless the K x K row-major V is a metric: finite entries >= 0, a zero diagonal,
+// symmetric, and V[a][c] <= V[a][b] + V[b][c] in float64 (DESIGN.md §11, "Label distances"); the message names the rule
+// and the first (a, b) or (a, b, c) that breaks it
+int expansion_check_distance(const double* V, int K, std::string& err);
 
 // the element-wise kernels of gc_expansion.cuh the loop launches, compiled into gc_expansion.cu only; `dtype` (MGC_F32 /
 // MGC_F64) selects the cost type, and markers / init may be nullptr

@@ -839,6 +839,7 @@ template <> struct ExpansionAbi<mgc_expansion> {
     static constexpr auto set_cost = mgc_expansion_set_cost;
     static constexpr auto set_markers = mgc_expansion_set_markers;
     static constexpr auto set_init = mgc_expansion_set_init;
+    static constexpr auto set_label_distance = mgc_expansion_set_label_distance;
     static constexpr auto run = mgc_expansion_run;
     static constexpr auto get_labels = mgc_expansion_get_labels;
     static constexpr auto get_stats = mgc_expansion_get_stats;
@@ -850,6 +851,7 @@ template <> struct ExpansionAbi<mgc_expansion_batch> {
     static constexpr auto set_cost = mgc_expansion_batch_set_cost;
     static constexpr auto set_markers = mgc_expansion_batch_set_markers;
     static constexpr auto set_init = mgc_expansion_batch_set_init;
+    static constexpr auto set_label_distance = mgc_expansion_batch_set_label_distance;
     static constexpr auto run = mgc_expansion_batch_run;
     static constexpr auto get_labels = mgc_expansion_batch_get_labels;
     static constexpr auto get_stats = mgc_expansion_batch_get_stats;
@@ -860,6 +862,7 @@ template <> struct ExpansionAbi<mgc_region_expansion> {     // no markers: they 
     static constexpr auto last_error = mgc_region_expansion_last_error;
     static constexpr auto set_cost = mgc_region_expansion_set_cost;
     static constexpr auto set_init = mgc_region_expansion_set_init;
+    static constexpr auto set_label_distance = mgc_region_expansion_set_label_distance;
     static constexpr auto run = mgc_region_expansion_run;
     static constexpr auto get_labels = mgc_region_expansion_get_labels;
     static constexpr auto get_stats = mgc_region_expansion_get_stats;
@@ -911,6 +914,22 @@ public:
         { py::gil_scoped_release rel; rc = Abi::set_init(e_, &r.a); }
         check(rc);
     }
+    // a (K, K) float64 label distance, or None for Potts
+    void set_label_distance(const py::object& dist)
+    {
+        py::array_t<double, py::array::c_style | py::array::forcecast> v;
+        const double* p = nullptr;
+        if (!dist.is_none()) {
+            v = py::array_t<double, py::array::c_style | py::array::forcecast>::ensure(dist);
+            if (!v || v.ndim() != 2 || v.shape(0) != labels_ || v.shape(1) != labels_)
+                throw py::value_error("label_distance must be a (K, K) = (" + std::to_string(labels_) + ", " +
+                                      std::to_string(labels_) + ") matrix");
+            p = v.data();
+        }
+        int rc;
+        { py::gil_scoped_release rel; rc = Abi::set_label_distance(e_, p); }
+        check(rc);
+    }
     void run(int max_cycles)
     {
         int rc;
@@ -939,7 +958,10 @@ public:
     py::dict stats() const { return stats_dict(true); }
 
 protected:
-    PyExpansionBase(std::vector<int64_t> shape, const char* mismatch) : shape_(std::move(shape)), mismatch_(mismatch) {}
+    PyExpansionBase(std::vector<int64_t> shape, int labels, const char* mismatch)
+        : shape_(std::move(shape)), labels_(labels), mismatch_(mismatch)
+    {
+    }
     // after the unit's create(): raise its refusal
     void created(int rc) const
     {
@@ -971,6 +993,7 @@ protected:
 
     H* e_ = nullptr;
     std::vector<int64_t> shape_;
+    int labels_;
     const char* mismatch_;
 };
 
@@ -978,7 +1001,7 @@ protected:
 class PyExpansion : public PyExpansionBase<mgc_expansion> {
 public:
     PyExpansion(const std::vector<int64_t>& shape, int labels, int device)
-        : PyExpansionBase(shape, "shape does not match the lattice")
+        : PyExpansionBase(shape, labels, "shape does not match the lattice")
     {
         created(mgc_expansion_create((int32_t)shape.size(), shape.data(), labels, device, &e_));
     }
@@ -1002,7 +1025,7 @@ public:
 class PyExpansionBatch : public PyExpansionBase<mgc_expansion_batch> {
 public:
     PyExpansionBatch(const std::vector<int64_t>& image_shape, int64_t batch, int labels, int device)
-        : PyExpansionBase(image_shape, "shape does not match (batch, *image)")
+        : PyExpansionBase(image_shape, labels, "shape does not match (batch, *image)")
     {
         created(mgc_expansion_batch_create((int32_t)image_shape.size(), image_shape.data(), batch, labels, device, &e_));
         shape_.insert(shape_.begin(), batch);
@@ -1074,7 +1097,7 @@ public:
 // K-label alpha-expansion over a region adjacency graph (mgc_region_expansion_*); per-region arrays are (regions,)
 class PyRegionExpansion : public PyExpansionBase<mgc_region_expansion> {
 public:
-    PyRegionExpansion(int64_t regions, int labels, int device) : PyExpansionBase({regions}, "one entry per region expected")
+    PyRegionExpansion(int64_t regions, int labels, int device) : PyExpansionBase({regions}, labels, "one entry per region expected")
     {
         created(mgc_region_expansion_create(regions, labels, device, &e_));
     }
@@ -1136,6 +1159,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("set_boundary", &PyExpansion::set_boundary)
         .def("set_markers", &PyExpansion::set_markers)
         .def("set_init", &PyExpansion::set_init)
+        .def("set_label_distance", &PyExpansion::set_label_distance)
         .def("run", &PyExpansion::run)
         .def("labels", &PyExpansion::labels)
         .def("labels_into", &PyExpansion::labels_into)
@@ -1147,6 +1171,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("set_boundary", &PyExpansionBatch::set_boundary)
         .def("set_markers", &PyExpansionBatch::set_markers)
         .def("set_init", &PyExpansionBatch::set_init)
+        .def("set_label_distance", &PyExpansionBatch::set_label_distance)
         .def("run", &PyExpansionBatch::run)
         .def("labels", &PyExpansionBatch::labels)
         .def("labels_into", &PyExpansionBatch::labels_into)
@@ -1159,6 +1184,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("set_cost", &PyRegionExpansion::set_cost)
         .def("set_pairs", &PyRegionExpansion::set_pairs)
         .def("set_init", &PyRegionExpansion::set_init)
+        .def("set_label_distance", &PyRegionExpansion::set_label_distance)
         .def("run", &PyRegionExpansion::run)
         .def("labels", &PyRegionExpansion::labels)
         .def("stats", &PyRegionExpansion::stats);

@@ -97,12 +97,20 @@ int mgc_region_expansion::stage(const mgc_array* a, size_t es, const char* what,
 int mgc_region_expansion::build(int alpha)
 {
     mgc_region_expansion* const g = this;
-    if (cost_dtype == MGC_F32)
+    if (have_dist) {
+        if (cost_dtype == MGC_F32)
+            k_rexp_move_m<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, dist, K, alpha, H.cap,
+                                                  H.tr, partials);
+        else
+            k_rexp_move_m<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, dist, K, alpha, H.cap,
+                                                   H.tr, partials);
+    } else if (cost_dtype == MGC_F32) {
         k_rexp_move<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, alpha, H.cap, H.tr,
                                             partials);
-    else
+    } else {
         k_rexp_move<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, alpha, H.cap, H.tr,
                                              partials);
+    }
     CK(cudaGetLastError());
     CK(cudaMemsetAsync(d_base, 0, sizeof(double), 0));
     sum_partials_on(0, partials, blocks, d_base);       // the add_tweights constant
@@ -123,10 +131,16 @@ int mgc_region_expansion::energy()
 {
     mgc_region_expansion* const g = this;
     CK(cudaMemsetAsync(d_energy, 0, sizeof(double), 0));
-    if (cost_dtype == MGC_F32)
+    if (have_dist) {
+        if (cost_dtype == MGC_F32)
+            k_rexp_energy_m<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, dist, K, partials);
+        else
+            k_rexp_energy_m<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, dist, K, partials);
+    } else if (cost_dtype == MGC_F32) {
         k_rexp_energy<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, partials);
-    else
+    } else {
         k_rexp_energy<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, partials);
+    }
     CK(cudaGetLastError());
     sum_partials_on(0, partials, blocks, d_energy);
     return MGC_OK;
@@ -188,6 +202,11 @@ int mgc_region_expansion_set_pairs(mgc_region_expansion* g, int64_t count, const
 }
 
 int mgc_region_expansion_set_init(mgc_region_expansion* g, const mgc_array* init) { return g ? g->set_init(init) : MGC_E_ARG; }
+int mgc_region_expansion_set_label_distance(mgc_region_expansion* g, const double* dist)
+{
+    return g ? g->set_label_distance(dist) : MGC_E_ARG;
+}
+
 int mgc_region_expansion_run(mgc_region_expansion* g, int32_t max_cycles) { return g ? g->run(max_cycles) : MGC_E_ARG; }
 int mgc_region_expansion_get_labels(mgc_region_expansion* g, uint8_t* out, int32_t mem) { return g ? g->get_labels(out, mem) : MGC_E_ARG; }
 int mgc_region_expansion_get_stats(const mgc_region_expansion* g, mgc_expansion_stats* out) { return g ? g->get_stats(out) : MGC_E_ARG; }

@@ -5,7 +5,11 @@
 // The graph is the CSR of the region pairs (row, head; each row in ascending neighbour id) with the pair's weight w on
 // both of its arcs (wt).  The labelling energy E(l) = sum_r D_r(l_r) + sum_{pairs r<s} w_rs [l_r != l_s], D_r(k) =
 // costs[k * n + r] widened to double (markers are already in the costs).
+//
+// With a label distance V (DESIGN.md §11, "Label distances") the pair term is w_rs V(l_r, l_s): k_rexp_move_m and
+// k_rexp_energy_m.
 #pragma once
+#include "gc_expansion_metric.cuh"
 #include "gc_terms.cuh"
 
 // One move for label `alpha` over the current labels: writes the sparse solver's state exactly as a fresh mgc_sparse
@@ -42,6 +46,74 @@ k_rexp_move(int n, const int* __restrict__ row, const int* __restrict__ head, co
         double t = 0.0;
         m = __dadd_rn(m, add_tweights_dev(t, src, snk));
         tr[u] = t;
+    }
+    block_sum_store(m, partials);
+}
+
+// k_rexp_move with the pair term w_rs V(l_r, l_s) of a metric label distance (exp_metric_pair, DESIGN.md §11, "Label
+// distances").  Node u with a = l_u != alpha, arc u->v with b = l_v and weight w, in the row's order: u < v takes (lo, fwd)
+// of the pair (u, v) as (snk_u term, cap(u->v)); u > v takes (up, bwd) of the pair (v, u).  A node labelled alpha has no
+// arcs and no pair contributions, as in k_rexp_move.
+template <typename C>
+__global__ void __launch_bounds__(256)
+k_rexp_move_m(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
+              const C* __restrict__ costs, const uint8_t* __restrict__ labels, const double* __restrict__ V, int K, int alpha,
+              double* __restrict__ cap, double* __restrict__ tr, double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = gridDim.x * blockDim.x;
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
+        const int a = labels[u];
+        const double src = (double)costs[(size_t)alpha * n + u];
+        double snk = (double)costs[(size_t)a * n + u];
+        const int end = row[u + 1];
+        for (int e = row[u]; e < end; ++e) {
+            double c = 0.0;
+            if (a != alpha) {
+                const int v = head[e];
+                const int b = labels[v];
+                double t;
+                if (u < v) {
+                    const ExpPair r = exp_metric_pair(wt[e], V, K, a, b, alpha);
+                    t = r.lo;
+                    c = r.fwd;
+                } else {
+                    const ExpPair r = exp_metric_pair(wt[e], V, K, b, a, alpha);
+                    t = r.up;
+                    c = r.bwd;
+                }
+                snk = __dadd_rn(snk, t);
+            }
+            cap[e] = c;
+        }
+        double t = 0.0;
+        m = __dadd_rn(m, add_tweights_dev(t, src, snk));
+        tr[u] = t;
+    }
+    block_sum_store(m, partials);
+}
+
+// k_rexp_energy with w_rs V(l_r, l_s) in place of w_rs for a pair whose labels differ
+template <typename C>
+__global__ void __launch_bounds__(256)
+k_rexp_energy_m(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
+                const C* __restrict__ costs, const uint8_t* __restrict__ labels, const double* __restrict__ V, int K,
+                double* __restrict__ partials)
+{
+    double m = 0.0;
+    const int step = gridDim.x * blockDim.x;
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
+        const int a = labels[u];
+        double e = (double)costs[(size_t)a * n + u];
+        const int end = row[u + 1];
+        for (int k = row[u]; k < end; ++k) {
+            const int v = head[k];
+            if (v > u) {
+                const int b = labels[v];
+                if (b != a) e = __dadd_rn(e, exp_dist(wt[k], V, K, a, b));
+            }
+        }
+        m = __dadd_rn(m, e);
     }
     block_sum_store(m, partials);
 }

@@ -125,8 +125,41 @@ def _check_init_markers(markers, init):
         raise ValueError("init gives a marked voxel another label than its marker")
 
 
+def _label_distance(V, K):
+    """A label distance as a C-contiguous float64 (K, K) numpy array, refused (ValueError) unless it is a metric: finite
+    entries >= 0, a zero diagonal, symmetric, and V[a][c] <= V[a][b] + V[b][c] in float64 for every a, b, c.  The
+    message names the rule and the first (a, b) or (a, b, c), in C order, that breaks it: the native check's words.  A
+    CUDA tensor is copied to the host (K^2 numbers)."""
+    if _on_device(V):
+        V = V.detach().cpu().numpy()
+    V = numpy.asarray(V)
+    if V.dtype.kind not in "iuf":
+        raise ValueError("label_distance must hold real numbers, got {}".format(V.dtype))
+    V = numpy.ascontiguousarray(V, dtype=numpy.float64)
+    if V.shape != (K, K):
+        raise ValueError("label_distance must be a (K, K) = ({}, {}) matrix, got shape {}".format(K, K, V.shape))
+    bad = numpy.argwhere(~(numpy.isfinite(V) & (V >= 0)))
+    if bad.size:
+        raise ValueError("label_distance must be finite and >= 0, V[{}][{}] is not".format(*bad[0]))
+    bad = numpy.flatnonzero(numpy.diagonal(V) != 0)
+    if bad.size:
+        raise ValueError("label_distance must have a zero diagonal, V[{0}][{0}] is not 0".format(bad[0]))
+    bad = numpy.argwhere(V != V.T)
+    if bad.size:
+        a, b = bad[0]
+        raise ValueError("label_distance must be symmetric, V[{0}][{1}] != V[{1}][{0}]".format(a, b))
+    for a in range(K):
+        bad = numpy.argwhere(V[a][None, :] > V[a][:, None] + V)        # [b, c]: V[a][c] > V[a][b] + V[b][c]
+        if bad.size:
+            b, c = bad[0]
+            raise ValueError("label_distance must satisfy the triangle inequality V[a][c] <= V[a][b] + V[b][c], "
+                             "(a, b, c) = ({}, {}, {}) breaks it; a semi-metric such as truncated quadratic needs "
+                             "alpha-beta swap moves".format(a, b, c))
+    return V
+
+
 def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, markers=None, init=None, max_cycles=20,
-                          stats=False):
+                          stats=False, *, label_distance=None):
     """Segment a voxel image into K labels by alpha-expansion.
 
     costs              (K, *shape) float32 or float64, a numpy array or a CUDA tensor; ``costs[k]`` is the cost of label k
@@ -141,9 +174,15 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
     max_cycles         cycles of the moves 0, 1, ..., K-1 at most; the loop stops earlier after a cycle that switches no
                        voxel.
     stats              also return a dict: moves, cycles, converged, switched (voxels per move), energy and device ms.
+    label_distance     (K, K) metric label distance V (numpy array, nested sequence or CUDA tensor; keyword only): the
+                       pair term becomes w_pq V(l_p, l_q), so a change between distant labels costs more than one between
+                       neighbours, e.g. ``numpy.minimum(abs(i - j), 2)`` for ordered labels.  Finite, >= 0, zero on the
+                       diagonal, symmetric and satisfying the triangle inequality (DESIGN.md §11, "Label distances").
+                       None: Potts.
 
     Returns ``(labels, energy)`` (``(labels, energy, stats)`` with ``stats=True``): uint8 labels of the image shape, a
-    numpy array or, for CUDA costs, a CUDA tensor; ``energy`` the Potts energy of those labels.  Raises ``ValueError`` for
+    numpy array or, for CUDA costs, a CUDA tensor; ``energy`` the energy of those labels (Potts, or with the label
+    distance).  Raises ``ValueError`` for
     malformed arguments and ``AttributeError`` for a boundary term that is not a two-parameter callable, before anything
     reaches the device.
     """
@@ -173,6 +212,8 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
     if init is not None:
         init = _label_image(init, shape, "init", K - 1)
     _check_init_markers(markers, init)
+    if label_distance is not None:
+        label_distance = _label_distance(label_distance, K)
 
     from .. import _lib  # raises ImportError loudly when the extension is not built
     on_dev = _on_device(costs)
@@ -188,6 +229,8 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
         nat.set_markers(markers)
     if init is not None:
         nat.set_init(init)
+    if label_distance is not None:
+        nat.set_label_distance(label_distance)
     nat.run(int(max_cycles))
     st = nat.stats()
     if on_dev:
@@ -202,7 +245,7 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
 
 
 def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, spacing=False, markers=None, init=None,
-                                max_cycles=20, stats=False):
+                                max_cycles=20, stats=False, *, label_distance=None):
     """Segment B images of one shape into K labels by alpha-expansion, all in one loop (DESIGN.md §11, "Batches").
 
     Image b is segmented as ``expansion_from_voxels`` segments it alone: the same energy, bit for bit the same move
@@ -225,9 +268,11 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
     stats              also return a dict: the batch loop's ``batch_moves``, ``batch_cycles``, ``batch_converged``, per-image
                        lists ``moves``, ``cycles``, ``converged``, ``switched`` (voxels per move) and ``energy``, and the
                        device ms (``ms_build``, ``ms_solve``, ``ms_apply`` summed over the moves, ``ms_total``).
+    label_distance     (K, K) metric label distance of every image, as ``expansion_from_voxels`` takes it; None: Potts.
 
     Returns ``(labels, energies)`` (``+ (stats,)`` with ``stats=True``): uint8 labels of shape (B, *image), a numpy array
-    or, for CUDA costs, a CUDA tensor; ``energies`` a float64 numpy array of the B Potts energies.  Raises ``ValueError``
+    or, for CUDA costs, a CUDA tensor; ``energies`` a float64 numpy array of the B energies (Potts, or with the label
+    distance).  Raises ``ValueError``
     for malformed arguments before anything reaches the device.
     """
     from .batch import INDEX_LIMIT, _host_image, _is_cuda, _sigmas
@@ -267,6 +312,8 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
     if init is not None:
         init = _label_image(init, bshape, "init", K - 1)
     _check_init_markers(markers, init)
+    if label_distance is not None:
+        label_distance = _label_distance(label_distance, K)
 
     from .. import _lib  # raises ImportError loudly when the extension is not built
     on_dev = _on_device(costs)
@@ -284,6 +331,8 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
         nat.set_markers(markers)
     if init is not None:
         nat.set_init(init)
+    if label_distance is not None:
+        nat.set_label_distance(label_distance)
     nat.run(int(max_cycles))
     per = nat.image_stats()
     energies = numpy.asarray(per["energy"], dtype=numpy.float64)
@@ -326,7 +375,7 @@ def _region_values(a, regions, what, limit):
 
 
 def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary_term_args=False, markers=None, init=None,
-                          max_cycles=20, stats=False, *, region_costs=None):
+                          max_cycles=20, stats=False, *, region_costs=None, label_distance=None):
     """Segment the regions of a label image into K labels by alpha-expansion (DESIGN.md §11, "Region graphs").
 
     Minimises E(l) = sum_r D_r(l_r) + sum_{region pairs r<s} w_rs [l_r != l_s] over region labels 0..K-1
@@ -349,10 +398,12 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
     max_cycles         cycles of the moves 0, 1, ..., K-1 at most; the loop stops earlier after a cycle that switches no
                        region.
     stats              also return a dict: moves, cycles, converged, switched (regions per move), energy and device ms.
+    label_distance     (K, K) metric label distance, as ``expansion_from_voxels`` takes it: the pair term becomes
+                       w_rs V(l_r, l_s).  None: Potts.
 
     Returns ``(labels, region_labels, energy)`` (``+ (stats,)`` with ``stats=True``): ``labels`` the uint8 voxel image
     ``region_labels[label_image - 1]`` (a CUDA tensor when the costs are one, numpy otherwise), ``region_labels`` uint8
-    of shape (R,), ``energy`` the Potts energy of those labels.
+    of shape (R,), ``energy`` the energy of those labels (Potts, or with the label distance).
     """
     if (costs is None) == (region_costs is None):
         raise ValueError("give exactly one of costs and region_costs")
@@ -368,6 +419,8 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
     _check_range(data, what)
     K = int(data.shape[0])
     _check_labels_and_cycles(K, what + ".shape[0]", max_cycles)
+    if label_distance is not None:
+        label_distance = _label_distance(label_distance, K)
     if boundary_term and not _takes_three_parameters(boundary_term):
         raise AttributeError("boundary_term has to be a callable object which takes three parameters.")
     if markers is not None:
@@ -419,6 +472,8 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
         nat.set_pairs(*rec.pairs)
     if init is not None:
         nat.set_init(init)
+    if label_distance is not None:
+        nat.set_label_distance(label_distance)
     nat.run(int(max_cycles))
     st = nat.stats()
     region_labels = nat.labels()
