@@ -22,58 +22,32 @@ struct mgc_expansion : Expansion {
     int build(int alpha) override;
     int solve(const uint8_t** mask) override;
     int energy() override;
+
+    ExpWeights weights() const
+    {
+        ExpWeights W{};
+        for (int d = 0; d < g->nd; ++d) W.w[d] = w + (size_t)d * n;
+        return W;
+    }
 };
 
 namespace {
 thread_local std::string g_exp_create_error;
-
-template <typename C, int ND>
-void move_launch(mgc_expansion* e, int alpha)
-{
-    mgc_graph* g = e->g;
-    ExpWeights W{};
-    for (int d = 0; d < ND; ++d) W.w[d] = e->w + (size_t)d * g->L.n;
-    const C* costs = (const C*)e->costs;
-    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
-    if (e->have_dist)
-        k_exp_move_m<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, W, e->dist, e->K, alpha,
-                                                               g->partials);
-    else
-        k_exp_move<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, W, alpha, g->partials);
-}
-
-template <typename C, int ND>
-void energy_launch(mgc_expansion* e)
-{
-    mgc_graph* g = e->g;
-    ExpWeights W{};
-    for (int d = 0; d < ND; ++d) W.w[d] = e->w + (size_t)d * g->L.n;
-    const C* costs = (const C*)e->costs;
-    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
-    if (e->have_dist)
-        k_exp_energy_m<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, costs, mk, e->labels, W, e->dist, e->K, g->partials);
-    else
-        k_exp_energy<C, ND><<<rblocks(g), 256, 0, g->stream>>>(g->L, costs, mk, e->labels, W, g->partials);
-}
-
-template <int ND>
-void by_dtype(mgc_expansion* e, int alpha)
-{
-    if (e->cost_dtype == MGC_F32) { if (alpha >= 0) move_launch<float, ND>(e, alpha); else energy_launch<float, ND>(e); }
-    else                          { if (alpha >= 0) move_launch<double, ND>(e, alpha); else energy_launch<double, ND>(e); }
-}
-
-// alpha >= 0: the move kernel for alpha; -1: the energy kernel
-void dispatch(mgc_expansion* e, int alpha)
-{
-    if (e->g->nd == 3) by_dtype<3>(e, alpha);
-    else               by_dtype<4>(e, alpha);
-}
 }  // namespace
 
 int mgc_expansion::build(int alpha)
 {
-    dispatch(this, alpha);
+    const uint8_t* mk = have_markers ? markers : nullptr;
+    with_pair_rule(*this, [&](auto c, auto pair) {
+        using C = decltype(c);
+        using P = decltype(pair);
+        if (g->nd == 3)
+            k_exp_move<P, C, 3><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), alpha,
+                                                              g->partials, pair);
+        else
+            k_exp_move<P, C, 4><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), alpha,
+                                                              g->partials, pair);
+    });
     CK(cudaGetLastError());
     sum_partials(g, g->partials, blocks, g->d_scalars);     // the add_tweights constant, as finish_flow_const forms it
     g->caps_fresh = false;
@@ -94,7 +68,15 @@ int mgc_expansion::solve(const uint8_t** mask)
 int mgc_expansion::energy()
 {
     CK(cudaMemsetAsync(d_energy, 0, sizeof(double), g->stream));
-    dispatch(this, -1);
+    const uint8_t* mk = have_markers ? markers : nullptr;
+    with_pair_rule(*this, [&](auto c, auto pair) {
+        using C = decltype(c);
+        using P = decltype(pair);
+        if (g->nd == 3)
+            k_exp_energy<P, C, 3><<<blocks, 256, 0, g->stream>>>(g->L, (const C*)costs, mk, labels, weights(), g->partials, pair);
+        else
+            k_exp_energy<P, C, 4><<<blocks, 256, 0, g->stream>>>(g->L, (const C*)costs, mk, labels, weights(), g->partials, pair);
+    });
     CK(cudaGetLastError());
     sum_partials(g, g->partials, blocks, d_energy);
     return MGC_OK;

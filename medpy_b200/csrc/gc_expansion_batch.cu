@@ -64,41 +64,14 @@ namespace {
 thread_local std::string g_bexp_create_error;
 }  // namespace
 
-namespace {
-template <typename C>
-void bexp_move_launch(mgc_expansion_batch* e, int alpha)
-{
-    mgc_graph* g = e->g;
-    const C* costs = (const C*)e->costs;
-    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
-    if (e->have_dist)
-        k_bexp_move_m<C><<<e->blocks, 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, e->weights(), e->dist, e->K,
-                                                           e->d_active, alpha, g->partials);
-    else
-        k_bexp_move<C><<<e->blocks, 256, 0, g->stream>>>(g->L, g->S, costs, mk, e->labels, e->weights(), e->d_active, alpha,
-                                                         g->partials);
-}
-
-template <typename C>
-void bexp_energy_launch(mgc_expansion_batch* e)
-{
-    mgc_graph* g = e->g;
-    const unsigned chunks = (unsigned)g->batch_chunks;
-    const C* costs = (const C*)e->costs;
-    const uint8_t* mk = e->have_markers ? e->markers : nullptr;
-    if (e->have_dist)
-        k_bexp_energy_m<C><<<(unsigned)e->B * chunks, 256, 0, g->stream>>>(g->L, costs, mk, e->labels, e->weights(), e->dist,
-                                                                           e->K, chunks, e->d_part);
-    else
-        k_bexp_energy<C><<<(unsigned)e->B * chunks, 256, 0, g->stream>>>(g->L, costs, mk, e->labels, e->weights(), chunks,
-                                                                         e->d_part);
-}
-}  // namespace
-
 int mgc_expansion_batch::build(int alpha)
 {
-    if (cost_dtype == MGC_F32) bexp_move_launch<float>(this, alpha);
-    else                       bexp_move_launch<double>(this, alpha);
+    const uint8_t* mk = have_markers ? markers : nullptr;
+    with_pair_rule(*this, [&](auto c, auto pair) {
+        using C = decltype(c);
+        k_bexp_move<<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), d_active, alpha,
+                                                  g->partials, pair);
+    });
     CK(cudaGetLastError());
     sum_partials(g, g->partials, blocks, g->d_scalars);     // the add_tweights constant of the active images
     g->caps_fresh = false;
@@ -110,8 +83,13 @@ int mgc_expansion_batch::build(int alpha)
 
 int mgc_expansion_batch::energy()
 {
-    if (cost_dtype == MGC_F32) bexp_energy_launch<float>(this);
-    else                       bexp_energy_launch<double>(this);
+    const unsigned chunks = (unsigned)g->batch_chunks;
+    const uint8_t* mk = have_markers ? markers : nullptr;
+    with_pair_rule(*this, [&](auto c, auto pair) {
+        using C = decltype(c);
+        k_bexp_energy<<<(unsigned)B * chunks, 256, 0, g->stream>>>(g->L, (const C*)costs, mk, labels, weights(), chunks,
+                                                                  d_part, pair);
+    });
     CK(cudaGetLastError());
     batch_sum(g, d_part, (unsigned)g->batch_chunks, d_energy);
     return MGC_OK;

@@ -7,16 +7,15 @@
 // and tr 0, no constant) and its labels stay as they are.
 #pragma once
 #include "gc_expansion_cost.cuh"
-#include "gc_expansion_metric.cuh"
 
-// k_exp_move's case table and summation order over the batch lattice, for the images whose flag is set; the axis-0 pairs
-// are those inside the image (none across a seam, as z_pairs), so a voxel's t-link has the bits of the single image's run.  The pair
-// weights W.w[d] are 0 across the seams and on the last plane of every axis.
-template <typename C>
+// k_exp_move over the batch lattice, for the images whose flag is set: the same exp_move_voxel, with the axis-0 pairs
+// those inside the image (none across a seam, as z_pairs), so a voxel's t-link has the bits of the single image's run.
+// The pair weights W.w[d] are 0 across the seams and on the last plane of every axis.
+template <typename P, typename C>
 __global__ void __launch_bounds__(256)
 k_bexp_move(Lattice L, State<double> S, const C* __restrict__ costs, const uint8_t* __restrict__ markers,
             const uint8_t* __restrict__ labels, ExpWeights W, const uint8_t* __restrict__ active, int alpha,
-            double* __restrict__ partials)
+            double* __restrict__ partials, P pair)
 {
     double m = 0.0;
     const unsigned step = gridDim.x * blockDim.x;
@@ -27,116 +26,12 @@ k_bexp_move(Lattice L, State<double> S, const C* __restrict__ costs, const uint8
         double tr = 0.0;
         if (active[img]) {
             c[0] -= img * L.zper;                   // the plane within the image: its axis-0 pairs stop at the seams
-            const int lp = labels[v];
-            const int mk = markers ? markers[v] : 0;
-            const double src = exp_cost(costs, L.n, v, alpha, mk);
-            double snk = exp_cost(costs, L.n, v, lp, mk);
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                double lo_c = 0.0, up_c = 0.0, fwd = 0.0, bwd = 0.0;
-                if (c[d] + 1 < (d == 0 ? L.zper : L.dim[d]) && lp != alpha) {   // p is the lower end of (p, p + e_d)
-                    const double w = W.w[d][v];
-                    if (labels[v + L.stride[d]] == lp) fwd = w;
-                    else lo_c = w;
-                }
-                if (c[d] > 0 && lp != alpha) {                                    // p is the upper end of (p - e_d, p)
-                    const unsigned o = v - L.stride[d];
-                    const double w = W.w[d][o];
-                    if (labels[o] == alpha) up_c = w;
-                    else bwd = w;
-                }
-                snk = __dadd_rn(snk, lo_c);
-                snk = __dadd_rn(snk, up_c);
-                S.cap[2 * d + 1][v] = fwd;
-                S.cap[2 * d][v] = bwd;
-            }
-            m = __dadd_rn(m, add_tweights_dev(tr, src, snk));
+            m = __dadd_rn(m, exp_move_voxel<3>(L, S, costs, markers, labels, W, pair, alpha, v, c, L.zper, tr));
         } else {                                    // frozen: the empty graph
 #pragma unroll
             for (int k = 0; k < 6; ++k) S.cap[k][v] = 0.0;
         }
         S.tr[v] = tr;
-    }
-    block_sum_store(m, partials);
-}
-
-// k_bexp_move with the pair term w_pq V(l_p, l_q) of a metric label distance (exp_metric_pair, DESIGN.md §11, "Label
-// distances"): the same frozen-image empty graph, the same seams and order, so a voxel's t-link has the bits of the single
-// image's k_exp_move_m
-template <typename C>
-__global__ void __launch_bounds__(256)
-k_bexp_move_m(Lattice L, State<double> S, const C* __restrict__ costs, const uint8_t* __restrict__ markers,
-              const uint8_t* __restrict__ labels, ExpWeights W, const double* __restrict__ V, int K,
-              const uint8_t* __restrict__ active, int alpha, double* __restrict__ partials)
-{
-    double m = 0.0;
-    const unsigned step = gridDim.x * blockDim.x;
-    for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < L.n; v += step) {
-        int c[3];
-        decode<3>(L, v, c);
-        const int img = image_of(L, c[0]);
-        double tr = 0.0;
-        if (active[img]) {
-            c[0] -= img * L.zper;                   // the plane within the image: its axis-0 pairs stop at the seams
-            const int lp = labels[v];
-            const int mk = markers ? markers[v] : 0;
-            const double src = exp_cost(costs, L.n, v, alpha, mk);
-            double snk = exp_cost(costs, L.n, v, lp, mk);
-#pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                double lo_c = 0.0, up_c = 0.0, fwd = 0.0, bwd = 0.0;
-                if (c[d] + 1 < (d == 0 ? L.zper : L.dim[d]) && lp != alpha) {   // p is the lower end of (p, p + e_d)
-                    const ExpPair r = exp_metric_pair(W.w[d][v], V, K, lp, labels[v + L.stride[d]], alpha);
-                    lo_c = r.lo;
-                    fwd = r.fwd;
-                }
-                if (c[d] > 0 && lp != alpha) {                                    // p is the upper end of (p - e_d, p)
-                    const unsigned o = v - L.stride[d];
-                    const ExpPair r = exp_metric_pair(W.w[d][o], V, K, labels[o], lp, alpha);
-                    up_c = r.up;
-                    bwd = r.bwd;
-                }
-                snk = __dadd_rn(snk, lo_c);
-                snk = __dadd_rn(snk, up_c);
-                S.cap[2 * d + 1][v] = fwd;
-                S.cap[2 * d][v] = bwd;
-            }
-            m = __dadd_rn(m, add_tweights_dev(tr, src, snk));
-        } else {                                    // frozen: the empty graph
-#pragma unroll
-            for (int k = 0; k < 6; ++k) S.cap[k][v] = 0.0;
-        }
-        S.tr[v] = tr;
-    }
-    block_sum_store(m, partials);
-}
-
-// k_bexp_energy with w_pq V(l_p, l_q) in place of w_pq for a lower-end pair whose labels differ
-template <typename C>
-__global__ void __launch_bounds__(256)
-k_bexp_energy_m(Lattice L, const C* __restrict__ costs, const uint8_t* __restrict__ markers, const uint8_t* __restrict__ labels,
-                ExpWeights W, const double* __restrict__ V, int K, unsigned chunks, double* __restrict__ partials)
-{
-    const unsigned per = (unsigned)L.zper * L.plane, base = (blockIdx.x / chunks) * per, ch = blockIdx.x % chunks;
-    double m = 0.0;
-    for (unsigned i = ch * blockDim.x + threadIdx.x; i < per; i += chunks * blockDim.x) {
-        const unsigned v = base + i;
-        int c[3];
-        decode<3>(L, v, c);
-        const int lp = labels[v];
-        double e = exp_cost(costs, L.n, v, lp, markers ? markers[v] : 0);
-        if (z_pairs(L, c[0]) & 2u) {
-            const int lq = labels[v + L.stride[0]];
-            if (lq != lp) e = __dadd_rn(e, exp_dist(W.w[0][v], V, K, lp, lq));
-        }
-#pragma unroll
-        for (int d = 1; d < 3; ++d) {
-            if (c[d] + 1 < L.dim[d]) {
-                const int lq = labels[v + L.stride[d]];
-                if (lq != lp) e = __dadd_rn(e, exp_dist(W.w[d][v], V, K, lp, lq));
-            }
-        }
-        m = __dadd_rn(m, e);
     }
     block_sum_store(m, partials);
 }
@@ -188,13 +83,13 @@ k_bexp_apply(Lattice L, const uint8_t* __restrict__ mask, uint8_t* __restrict__ 
     if (lane == 0 && cnt) atomicAdd(switched + cur, (unsigned long long)cnt);
 }
 
-// E(l) of every image in a fixed order: block b * chunks + c sums the voxels c * 256 + t of image b, stepping by
-// chunks * 256 (each voxel: D_p(l_p), then its lower-end pairs in axis order, none across a seam), into
-// partials[b * chunks + c]; batch_sum then adds each image's partials in a fixed tree.  The same labels give the same bits.
-template <typename C>
+// E(l) of every image in a fixed order: block b * chunks + c sums exp_energy_voxel (its axis-0 pairs none across a seam)
+// over the voxels c * 256 + t of image b, stepping by chunks * 256, into partials[b * chunks + c]; batch_sum then adds
+// each image's partials in a fixed tree.  The same labels give the same bits.
+template <typename P, typename C>
 __global__ void __launch_bounds__(256)
 k_bexp_energy(Lattice L, const C* __restrict__ costs, const uint8_t* __restrict__ markers, const uint8_t* __restrict__ labels,
-              ExpWeights W, unsigned chunks, double* __restrict__ partials)
+              ExpWeights W, unsigned chunks, double* __restrict__ partials, P pair)
 {
     const unsigned per = (unsigned)L.zper * L.plane, base = (blockIdx.x / chunks) * per, ch = blockIdx.x % chunks;
     double m = 0.0;
@@ -202,13 +97,7 @@ k_bexp_energy(Lattice L, const C* __restrict__ costs, const uint8_t* __restrict_
         const unsigned v = base + i;
         int c[3];
         decode<3>(L, v, c);
-        const int lp = labels[v];
-        double e = exp_cost(costs, L.n, v, lp, markers ? markers[v] : 0);
-        if ((z_pairs(L, c[0]) & 2u) && labels[v + L.stride[0]] != lp) e = __dadd_rn(e, W.w[0][v]);
-#pragma unroll
-        for (int d = 1; d < 3; ++d)
-            if (c[d] + 1 < L.dim[d] && labels[v + L.stride[d]] != lp) e = __dadd_rn(e, W.w[d][v]);
-        m = __dadd_rn(m, e);
+        m = __dadd_rn(m, exp_energy_voxel<3>(L, costs, markers, labels, W, pair, v, c));
     }
     block_sum_store(m, partials);
 }

@@ -69,8 +69,8 @@ struct Expansion {
     uint8_t* markers = nullptr;         // 0 none, m > 0: label m - 1
     uint8_t* init = nullptr;
     bool have_markers = false, have_init = false;
-    double* dist = nullptr;             // K x K label distance, row-major; a unit's build and energy hooks take the metric
-    bool have_dist = false;             // kernels while it is set, the Potts ones otherwise
+    double* dist = nullptr;             // K x K label distance, row-major; a unit's build and energy hooks launch the
+    bool have_dist = false;             // MetricPair kernels while it is set, the PottsPair ones otherwise (with_pair_rule)
     unsigned long long* d_switched = nullptr;   // [B] elements the current move switched per image
     double* d_energy = nullptr;                 // [B]
     int* d_bad = nullptr;

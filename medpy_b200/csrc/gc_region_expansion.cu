@@ -97,20 +97,10 @@ int mgc_region_expansion::stage(const mgc_array* a, size_t es, const char* what,
 int mgc_region_expansion::build(int alpha)
 {
     mgc_region_expansion* const g = this;
-    if (have_dist) {
-        if (cost_dtype == MGC_F32)
-            k_rexp_move_m<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, dist, K, alpha, H.cap,
-                                                  H.tr, partials);
-        else
-            k_rexp_move_m<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, dist, K, alpha, H.cap,
-                                                   H.tr, partials);
-    } else if (cost_dtype == MGC_F32) {
-        k_rexp_move<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, alpha, H.cap, H.tr,
-                                            partials);
-    } else {
-        k_rexp_move<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, alpha, H.cap, H.tr,
-                                             partials);
-    }
+    with_pair_rule(*this, [&](auto c, auto pair) {
+        using C = decltype(c);
+        k_rexp_move<<<blocks, 256>>>(H.n, H.row, H.head, wt, (const C*)costs, labels, alpha, H.cap, H.tr, partials, pair);
+    });
     CK(cudaGetLastError());
     CK(cudaMemsetAsync(d_base, 0, sizeof(double), 0));
     sum_partials_on(0, partials, blocks, d_base);       // the add_tweights constant
@@ -131,16 +121,10 @@ int mgc_region_expansion::energy()
 {
     mgc_region_expansion* const g = this;
     CK(cudaMemsetAsync(d_energy, 0, sizeof(double), 0));
-    if (have_dist) {
-        if (cost_dtype == MGC_F32)
-            k_rexp_energy_m<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, dist, K, partials);
-        else
-            k_rexp_energy_m<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, dist, K, partials);
-    } else if (cost_dtype == MGC_F32) {
-        k_rexp_energy<float><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const float*)costs, labels, partials);
-    } else {
-        k_rexp_energy<double><<<blocks, 256>>>(H.n, H.row, H.head, wt, (const double*)costs, labels, partials);
-    }
+    with_pair_rule(*this, [&](auto c, auto pair) {
+        using C = decltype(c);
+        k_rexp_energy<<<blocks, 256>>>(H.n, H.row, H.head, wt, (const C*)costs, labels, partials, pair);
+    });
     CK(cudaGetLastError());
     sum_partials_on(0, partials, blocks, d_energy);
     return MGC_OK;

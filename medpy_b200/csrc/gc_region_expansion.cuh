@@ -1,29 +1,28 @@
 // gc_region_expansion.cuh -- kernels of the region alpha-expansion unit (gc_region_expansion.cu, DESIGN.md §11 "Region
-// graphs"): a K-label Potts segmentation of a region adjacency graph, each move cut by the sparse push-relabel
-// (gc_sparse.cuh).  Launched by gc_region_expansion.cu only.
+// graphs"): a K-label segmentation of a region adjacency graph, each move cut by the sparse push-relabel (gc_sparse.cuh).
+// Launched by gc_region_expansion.cu only.
 //
 // The graph is the CSR of the region pairs (row, head; each row in ascending neighbour id) with the pair's weight w on
-// both of its arcs (wt).  The labelling energy E(l) = sum_r D_r(l_r) + sum_{pairs r<s} w_rs [l_r != l_s], D_r(k) =
-// costs[k * n + r] widened to double (markers are already in the costs).
-//
-// With a label distance V (DESIGN.md §11, "Label distances") the pair term is w_rs V(l_r, l_s): k_rexp_move_m and
-// k_rexp_energy_m.
+// both of its arcs (wt).  The labelling energy E(l) = sum_r D_r(l_r) + sum_{pairs r<s} w_rs V(l_r, l_s), D_r(k) =
+// costs[k * n + r] widened to double (markers are already in the costs), V Potts or a metric label distance: the pair
+// rule P (gc_expansion_pair.cuh) the kernels are instantiated with.
 #pragma once
-#include "gc_expansion_metric.cuh"
+#include "gc_expansion_pair.cuh"
 #include "gc_terms.cuh"
 
 // One move for label `alpha` over the current labels: writes the sparse solver's state exactly as a fresh mgc_sparse
 // would hold it after sum_edge of every pair and add_tweights of every node -- every arc's capacity, tr, and the
 // add_tweights constant as one fixed-order partial per block (summed by k_sum_partials).  x_u = SINK means "u switches to
-// alpha".  Node u with a = l_u, arc u->v with b = l_v and weight w:
-//   snk_u += w       if a != alpha and (b == alpha or (b != a and u < v)), in the row's order
-//   cap(u->v) = w    if a != alpha and b != alpha and (a == b or u > v), else 0
-// src_u = D_u(alpha), snk_u starts at D_u(a); then add_tweights(u, src_u, snk_u) on tr = 0.
-template <typename C>
+// alpha".  Node u with a = l_u != alpha, arc u->v with b = l_v and weight w, in the row's order: u < v takes P's lower end
+// of the pair (u, v), u > v its upper end of the pair (v, u), as (snk_u term, cap(u->v)); every such term is added, +0.0
+// included, which can only turn a zero tr's sign (DESIGN.md §11, "Region graphs").  A node labelled alpha has no arcs and
+// no pair contributions.  src_u = D_u(alpha), snk_u starts at D_u(a); then add_tweights(u, src_u, snk_u) on
+// tr = 0.
+template <typename P, typename C>
 __global__ void __launch_bounds__(256)
 k_rexp_move(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
             const C* __restrict__ costs, const uint8_t* __restrict__ labels, int alpha, double* __restrict__ cap,
-            double* __restrict__ tr, double* __restrict__ partials)
+            double* __restrict__ tr, double* __restrict__ partials, P pair)
 {
     double m = 0.0;
     const int step = gridDim.x * blockDim.x;
@@ -37,51 +36,9 @@ k_rexp_move(int n, const int* __restrict__ row, const int* __restrict__ head, co
             if (a != alpha) {
                 const int v = head[e];
                 const int b = labels[v];
-                const double w = wt[e];
-                if (b == alpha || (b != a && u < v)) snk = __dadd_rn(snk, w);
-                if (b != alpha && (a == b || u > v)) c = w;
-            }
-            cap[e] = c;
-        }
-        double t = 0.0;
-        m = __dadd_rn(m, add_tweights_dev(t, src, snk));
-        tr[u] = t;
-    }
-    block_sum_store(m, partials);
-}
-
-// k_rexp_move with the pair term w_rs V(l_r, l_s) of a metric label distance (exp_metric_pair, DESIGN.md §11, "Label
-// distances").  Node u with a = l_u != alpha, arc u->v with b = l_v and weight w, in the row's order: u < v takes (lo, fwd)
-// of the pair (u, v) as (snk_u term, cap(u->v)); u > v takes (up, bwd) of the pair (v, u).  A node labelled alpha has no
-// arcs and no pair contributions, as in k_rexp_move.
-template <typename C>
-__global__ void __launch_bounds__(256)
-k_rexp_move_m(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
-              const C* __restrict__ costs, const uint8_t* __restrict__ labels, const double* __restrict__ V, int K, int alpha,
-              double* __restrict__ cap, double* __restrict__ tr, double* __restrict__ partials)
-{
-    double m = 0.0;
-    const int step = gridDim.x * blockDim.x;
-    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
-        const int a = labels[u];
-        const double src = (double)costs[(size_t)alpha * n + u];
-        double snk = (double)costs[(size_t)a * n + u];
-        const int end = row[u + 1];
-        for (int e = row[u]; e < end; ++e) {
-            double c = 0.0;
-            if (a != alpha) {
-                const int v = head[e];
-                const int b = labels[v];
-                double t;
-                if (u < v) {
-                    const ExpPair r = exp_metric_pair(wt[e], V, K, a, b, alpha);
-                    t = r.lo;
-                    c = r.fwd;
-                } else {
-                    const ExpPair r = exp_metric_pair(wt[e], V, K, b, a, alpha);
-                    t = r.up;
-                    c = r.bwd;
-                }
+                double t = 0.0;
+                if (u < v) pair.lower(wt[e], a, b, alpha, t, c);
+                else       pair.upper(wt[e], b, a, alpha, t, c);
                 snk = __dadd_rn(snk, t);
             }
             cap[e] = c;
@@ -93,12 +50,12 @@ k_rexp_move_m(int n, const int* __restrict__ row, const int* __restrict__ head, 
     block_sum_store(m, partials);
 }
 
-// k_rexp_energy with w_rs V(l_r, l_s) in place of w_rs for a pair whose labels differ
-template <typename C>
+// E(l) per block in a fixed order (each node: D_u(l_u), then its pairs to higher ids in the row's order); k_sum_partials
+// adds the partials in a fixed order, so the same labels give the same bits
+template <typename P, typename C>
 __global__ void __launch_bounds__(256)
-k_rexp_energy_m(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
-                const C* __restrict__ costs, const uint8_t* __restrict__ labels, const double* __restrict__ V, int K,
-                double* __restrict__ partials)
+k_rexp_energy(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
+              const C* __restrict__ costs, const uint8_t* __restrict__ labels, double* __restrict__ partials, P pair)
 {
     double m = 0.0;
     const int step = gridDim.x * blockDim.x;
@@ -110,30 +67,8 @@ k_rexp_energy_m(int n, const int* __restrict__ row, const int* __restrict__ head
             const int v = head[k];
             if (v > u) {
                 const int b = labels[v];
-                if (b != a) e = __dadd_rn(e, exp_dist(wt[k], V, K, a, b));
+                if (b != a) e = __dadd_rn(e, pair.energy(wt[k], a, b));
             }
-        }
-        m = __dadd_rn(m, e);
-    }
-    block_sum_store(m, partials);
-}
-
-// E(l) per block in a fixed order (each node: D_u(l_u), then its pairs to higher ids in the row's order); k_sum_partials
-// adds the partials in a fixed order, so the same labels give the same bits
-template <typename C>
-__global__ void __launch_bounds__(256)
-k_rexp_energy(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
-              const C* __restrict__ costs, const uint8_t* __restrict__ labels, double* __restrict__ partials)
-{
-    double m = 0.0;
-    const int step = gridDim.x * blockDim.x;
-    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
-        const int a = labels[u];
-        double e = (double)costs[(size_t)a * n + u];
-        const int end = row[u + 1];
-        for (int k = row[u]; k < end; ++k) {
-            const int v = head[k];
-            if (v > u && labels[v] != a) e = __dadd_rn(e, wt[k]);
         }
         m = __dadd_rn(m, e);
     }

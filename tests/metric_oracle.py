@@ -2,7 +2,7 @@
 
 CPU restatement of the alpha-expansion with a metric label distance V (DESIGN.md §11, "Label distances"): the pair term
 w_pq V(l_p, l_q) in place of Potts' w_pq [l_p != l_q], for the voxel, region and batch units.  ``pair_terms`` is the one
-case table (the numpy mirror of ``exp_metric_pair`` in gc_expansion_metric.cuh); the voxel and region move problems lay
+case table (the numpy mirror of ``exp_metric_pair`` in gc_expansion_pair.cuh); the voxel and region move problems lay
 it out as oracle/expansion.py and oracle/region_expansion.py lay out theirs, in the same summation order, and are cut by
 the same BK restatements.  Everything else (data costs, pair weights, initial labels, the pairs' arc order) is those
 oracles' own code.  Every entry point takes ``V=None``, which runs the Potts oracle unchanged.
