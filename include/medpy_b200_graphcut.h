@@ -624,14 +624,27 @@ int mgc_expansion_set_markers(mgc_expansion* e, const mgc_array* markers);
 /* MGC_U8 initial labels, each below K (MGC_E_ARG otherwise); mgc_expansion_run refuses (MGC_E_ARG) an init that gives a
  * marked voxel another label than its marker. */
 int mgc_expansion_set_init(mgc_expansion* e, const mgc_array* init);
-/* A metric label distance: the pair term becomes w_pq V(l_p, l_q) in place of w_pq [l_p != l_q].  dist holds K x K host
- * doubles, row-major, borrowed for the call; every entry finite and >= 0, V[a][a] == 0, V[a][b] == V[b][a], and
- * V[a][c] <= V[a][b] + V[b][c] in float64 (zero off the diagonal is allowed).  A matrix that breaks a rule is refused
- * (MGC_E_ARG, the message names the rule and the first (a, b) or (a, b, c)) and leaves the handle on Potts, as NULL does.
- * Semi-metrics such as truncated quadratic break the triangle inequality: alpha-expansion cannot cut them exactly.  The
- * move graph with a distance is in DESIGN.md §11, "Label distances"; V = 1 - I gives the Potts move graphs bit for bit.
- * Adding it, mgc_expansion_batch_set_label_distance and mgc_region_expansion_set_label_distance left MGC_ABI_VERSION
- * at 3. */
+/* The move kind of mgc_expansion_run (and of the batch and region units' set_moves):
+ *   MGC_MOVES_EXPANSION  (the default) cycles of alpha-expansions alpha = 0, 1, ..., K-1; the label distance must be a
+ *                        metric
+ *   MGC_MOVES_SWAP       cycles of alpha-beta swaps (0, 1), (0, 2), ..., (K-2, K-1), K(K-1)/2 moves per cycle; each
+ *                        move is one binary cut in which only the voxels labelled alpha or beta take part, and the label
+ *                        distance may be any semi-metric (the triangle rule is not needed), e.g. truncated quadratic
+ *                        min((i - j)^2, T).  The move graph and the stop argument are in DESIGN.md §11, "Swap moves".
+ * Any other kind is refused (MGC_E_ARG) and leaves the handle as it was.  set_moves clears the last run's results and
+ * drops a label distance the handle holds, leaving it on Potts: call it before set_label_distance.  Adding it,
+ * mgc_expansion_batch_set_moves and mgc_region_expansion_set_moves left MGC_ABI_VERSION at 3. */
+#define MGC_MOVES_EXPANSION 0
+#define MGC_MOVES_SWAP 1
+int mgc_expansion_set_moves(mgc_expansion* e, int32_t kind);
+/* A label distance: the pair term becomes w_pq V(l_p, l_q) in place of w_pq [l_p != l_q].  dist holds K x K host
+ * doubles, row-major, borrowed for the call; every entry finite and >= 0, V[a][a] == 0, V[a][b] == V[b][a], and, under
+ * expansion moves, V[a][c] <= V[a][b] + V[b][c] in float64 (zero off the diagonal is allowed).  A matrix that breaks a
+ * rule is refused (MGC_E_ARG, the message names the rule and the first (a, b) or (a, b, c)) and leaves the handle on
+ * Potts, as NULL does.  Semi-metrics such as truncated quadratic break the triangle inequality: alpha-expansion cannot
+ * cut them exactly, so they need MGC_MOVES_SWAP, set before this call.  The move graphs with a distance are in DESIGN.md
+ * §11, "Label distances" and "Swap moves"; V = 1 - I gives the Potts move graphs bit for bit.  Adding it,
+ * mgc_expansion_batch_set_label_distance and mgc_region_expansion_set_label_distance left MGC_ABI_VERSION at 3. */
 int mgc_expansion_set_label_distance(mgc_expansion* e, const double* dist);
 /* MGC_E_STATE until every cost plane is set; max_cycles >= 1. */
 int mgc_expansion_run(mgc_expansion* e, int32_t max_cycles);
@@ -675,6 +688,8 @@ int mgc_expansion_batch_set_markers(mgc_expansion_batch* e, const mgc_array* mar
 /* MGC_U8 (B, *image) initial labels, each below K (MGC_E_ARG otherwise); mgc_expansion_batch_run refuses (MGC_E_ARG) an
  * init that gives a marked voxel another label than its marker. */
 int mgc_expansion_batch_set_init(mgc_expansion_batch* e, const mgc_array* init);
+/* The move kind of every image, as mgc_expansion_set_moves: a swap cycle gives each image K(K-1)/2 moves. */
+int mgc_expansion_batch_set_moves(mgc_expansion_batch* e, int32_t kind);
 /* The label distance of every image, as mgc_expansion_set_label_distance (NULL: Potts). */
 int mgc_expansion_batch_set_label_distance(mgc_expansion_batch* e, const double* dist);
 /* MGC_E_STATE until every cost plane is set; max_cycles >= 1 (per image, as mgc_expansion_run). */
@@ -684,7 +699,7 @@ int mgc_expansion_batch_get_labels(mgc_expansion_batch* e, uint8_t* out, int32_t
 /* The batch loop: moves and cycles it ran, converged = 1 when every image converged, energy = the sum of the B image
  * energies in image order, and the device ms of its phases. */
 int mgc_expansion_batch_get_stats(const mgc_expansion_batch* e, mgc_expansion_stats* out);
-/* out[B]: per image its moves (K x cycles), cycles (the first cycle that switched none of its voxels, or max_cycles),
+/* out[B]: per image its moves (K x cycles, or K(K-1)/2 x cycles under swap moves), cycles (the first cycle that switched none of its voxels, or max_cycles),
  * converged and energy (fixed-order device sum: same labels, same bits); the ms fields are 0. */
 int mgc_expansion_batch_get_image_stats(const mgc_expansion_batch* e, mgc_expansion_stats* out);
 /* out[moves x B], row-major: the voxels of image b the move switched (0 once b is frozen); image b's own switch counts
@@ -720,6 +735,8 @@ int mgc_region_expansion_set_pairs(mgc_region_expansion* e, int64_t count, const
                                    const double* w);
 /* MGC_U8 initial region labels, each below K (MGC_E_ARG otherwise). */
 int mgc_region_expansion_set_init(mgc_region_expansion* e, const mgc_array* init);
+/* The move kind, as mgc_expansion_set_moves. */
+int mgc_region_expansion_set_moves(mgc_region_expansion* e, int32_t kind);
 /* The label distance, as mgc_expansion_set_label_distance (NULL: Potts): the pair term becomes w_rs V(l_r, l_s). */
 int mgc_region_expansion_set_label_distance(mgc_region_expansion* e, const double* dist);
 /* MGC_E_STATE until every cost row is set; max_cycles >= 1. */

@@ -1,5 +1,5 @@
-// gc_expansion.cu -- C ABI of the alpha-expansion segmentation (mgc_expansion_*, include/medpy_b200_graphcut.h; DESIGN.md
-// §11).  A handle owns one eager lattice handle (mgc_graph) and cuts every move on it: the move kernel writes the state
+// gc_expansion.cu -- C ABI of the K-label segmentation by alpha-expansion or alpha-beta swap moves (mgc_expansion_*,
+// include/medpy_b200_graphcut.h; DESIGN.md §11).  A handle owns one eager lattice handle (mgc_graph) and cuts every move on it: the move kernel writes the state
 // mgc_add_tweights_dense + mgc_add_nweights_dense would leave on a fresh handle, and mgc_maxflow solves it unchanged.
 // The loop is gc_expansion_loop.cu's, with B = 1; this unit also compiles the element-wise kernels it launches.
 #include "gc_handle.cuh"
@@ -19,7 +19,7 @@ struct mgc_expansion : Expansion {
     int stage(const mgc_array* a, size_t, const char*, const void** out) override { return stage_input(g, a, 0, out); }
     void release() override { slots_release(g, 1u); }
     int reset() override { return mgc_reset(g); }
-    int build(int alpha) override;
+    int build(const ExpMove& m) override;
     int solve(const uint8_t** mask) override;
     int energy() override;
 
@@ -35,13 +35,21 @@ namespace {
 thread_local std::string g_exp_create_error;
 }  // namespace
 
-int mgc_expansion::build(int alpha)
+int mgc_expansion::build(const ExpMove& m)
 {
     const uint8_t* mk = have_markers ? markers : nullptr;
+    const int alpha = m.alpha, beta = m.beta;
     with_pair_rule(*this, [&](auto c, auto pair) {
         using C = decltype(c);
         using P = decltype(pair);
-        if (g->nd == 3)
+        if (beta >= 0) {
+            if (g->nd == 3)
+                k_swap_move<P, C, 3><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(),
+                                                                   alpha, beta, g->partials, pair);
+            else
+                k_swap_move<P, C, 4><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(),
+                                                                   alpha, beta, g->partials, pair);
+        } else if (g->nd == 3)
             k_exp_move<P, C, 3><<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), alpha,
                                                               g->partials, pair);
         else
@@ -94,6 +102,12 @@ void exp_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t
                       unsigned long long* switched)
 {
     k_exp_apply<<<blocks, 256, 0, s>>>(n, mask, labels, alpha, switched);
+}
+
+void swap_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* mask, uint8_t* labels, int alpha, int beta,
+                       unsigned long long* switched)
+{
+    k_swap_apply<<<blocks, 256, 0, s>>>(n, mask, labels, alpha, beta, switched);
 }
 
 void exp_check_costs_launch(cudaStream_t s, unsigned blocks, unsigned n, int dtype, const void* cost, int* bad)
@@ -167,6 +181,7 @@ int mgc_expansion_set_boundary(mgc_expansion* e, int32_t kind, const mgc_array* 
 
 int mgc_expansion_set_markers(mgc_expansion* e, const mgc_array* markers) { return e ? e->set_markers(markers) : MGC_E_ARG; }
 int mgc_expansion_set_init(mgc_expansion* e, const mgc_array* init) { return e ? e->set_init(init) : MGC_E_ARG; }
+int mgc_expansion_set_moves(mgc_expansion* e, int32_t kind) { return e ? e->set_moves(kind) : MGC_E_ARG; }
 int mgc_expansion_set_label_distance(mgc_expansion* e, const double* dist) { return e ? e->set_label_distance(dist) : MGC_E_ARG; }
 int mgc_expansion_run(mgc_expansion* e, int32_t max_cycles) { return e ? e->run(max_cycles) : MGC_E_ARG; }
 int mgc_expansion_get_labels(mgc_expansion* e, uint8_t* out, int32_t mem) { return e ? e->get_labels(out, mem) : MGC_E_ARG; }

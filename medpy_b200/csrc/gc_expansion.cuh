@@ -1,5 +1,6 @@
 // gc_expansion.cuh -- kernels of the alpha-expansion unit (gc_expansion.cu, DESIGN.md §11): a K-label segmentation cut
-// as a sequence of binary moves on the eager lattice handle.  Launched by gc_expansion.cu only.
+// as a sequence of binary moves (alpha-expansions or alpha-beta swaps) on the eager lattice handle.  Launched by
+// gc_expansion.cu only.
 //
 // The labelling energy E(l) = sum_p D_p(l_p) + sum_pairs w_pq V(l_p, l_q):
 //   D_p(k)  cost plane k at p widened to double, + GCGraph.MAX (65535) when p is marked with a label other than k
@@ -38,6 +39,43 @@ k_exp_apply(unsigned n, const uint8_t* __restrict__ mask, uint8_t* __restrict__ 
     const unsigned step = gridDim.x * blockDim.x;
     for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += step) {
         if (!mask[v] && labels[v] != alpha) { labels[v] = (uint8_t)alpha; ++cnt; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_down_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(switched, (unsigned long long)cnt);
+}
+
+// One swap move of (alpha, beta): swap_move_voxel at every voxel, the constant as k_exp_move forms it
+template <typename P, typename C, int ND>
+__global__ void __launch_bounds__(256)
+k_swap_move(Lattice L, State<double> S, const C* __restrict__ costs, const uint8_t* __restrict__ markers,
+            const uint8_t* __restrict__ labels, ExpWeights W, int alpha, int beta, double* __restrict__ partials, P pair)
+{
+    double m = 0.0;
+    const unsigned step = gridDim.x * blockDim.x;
+    for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < L.n; v += step) {
+        int c[ND];
+        decode<ND>(L, v, c);
+        double tr = 0.0;
+        m = __dadd_rn(m, swap_move_voxel<ND>(L, S, costs, markers, labels, W, pair, alpha, beta, v, c, L.dim[0], tr));
+        S.tr[v] = tr;
+    }
+    block_sum_store(m, partials);
+}
+
+// labels of alpha or beta <- beta where the cut put the element on the SINK side (mask 0), alpha elsewhere; *switched +=
+// the elements that changed
+__global__ void __launch_bounds__(256)
+k_swap_apply(unsigned n, const uint8_t* __restrict__ mask, uint8_t* __restrict__ labels, int alpha, int beta,
+             unsigned long long* __restrict__ switched)
+{
+    unsigned cnt = 0;
+    const unsigned step = gridDim.x * blockDim.x;
+    for (unsigned v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += step) {
+        const int l = labels[v];
+        if (l != alpha && l != beta) continue;
+        const int to = mask[v] ? alpha : beta;
+        if (l != to) { labels[v] = (uint8_t)to; ++cnt; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) cnt += __shfl_down_sync(0xffffffffu, cnt, o);

@@ -33,7 +33,7 @@ struct mgc_expansion_batch : Expansion {
     }
     void release() override { slots_release(g, 1u); }
     int reset() override { return mgc_reset(g); }
-    int build(int alpha) override;
+    int build(const ExpMove& m) override;
     int solve(const uint8_t** mask) override
     {
         double flow = 0.0;
@@ -41,9 +41,10 @@ struct mgc_expansion_batch : Expansion {
         *mask = g->mask_dev;
         return MGC_OK;
     }
-    void apply(const uint8_t* mask, int alpha) override
+    void apply(const uint8_t* mask, const ExpMove& m) override
     {
-        k_bexp_apply<<<blocks, 256, 0, g->stream>>>(g->L, mask, labels, d_active, alpha, d_switched);
+        if (m.beta < 0) k_bexp_apply<<<blocks, 256, 0, g->stream>>>(g->L, mask, labels, d_active, m.alpha, d_switched);
+        else k_bswap_apply<<<blocks, 256, 0, g->stream>>>(g->L, mask, labels, d_active, m.alpha, m.beta, d_switched);
     }
     int freeze(const std::vector<uint8_t>& active) override
     {
@@ -64,13 +65,17 @@ namespace {
 thread_local std::string g_bexp_create_error;
 }  // namespace
 
-int mgc_expansion_batch::build(int alpha)
+int mgc_expansion_batch::build(const ExpMove& m)
 {
     const uint8_t* mk = have_markers ? markers : nullptr;
     with_pair_rule(*this, [&](auto c, auto pair) {
         using C = decltype(c);
-        k_bexp_move<<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), d_active, alpha,
-                                                  g->partials, pair);
+        if (m.beta >= 0)
+            k_bswap_move<<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), d_active,
+                                                       m.alpha, m.beta, g->partials, pair);
+        else
+            k_bexp_move<<<blocks, 256, 0, g->stream>>>(g->L, g->S, (const C*)costs, mk, labels, weights(), d_active,
+                                                      m.alpha, g->partials, pair);
     });
     CK(cudaGetLastError());
     sum_partials(g, g->partials, blocks, g->d_scalars);     // the add_tweights constant of the active images
@@ -171,6 +176,7 @@ int mgc_expansion_batch_set_boundary(mgc_expansion_batch* e, int32_t kind, const
 
 int mgc_expansion_batch_set_markers(mgc_expansion_batch* e, const mgc_array* markers) { return e ? e->set_markers(markers) : MGC_E_ARG; }
 int mgc_expansion_batch_set_init(mgc_expansion_batch* e, const mgc_array* init) { return e ? e->set_init(init) : MGC_E_ARG; }
+int mgc_expansion_batch_set_moves(mgc_expansion_batch* e, int32_t kind) { return e ? e->set_moves(kind) : MGC_E_ARG; }
 int mgc_expansion_batch_set_label_distance(mgc_expansion_batch* e, const double* dist)
 {
     return e ? e->set_label_distance(dist) : MGC_E_ARG;

@@ -51,6 +51,55 @@ __device__ __forceinline__ double exp_move_voxel(const Lattice& L, const State<d
     return add_tweights_dev(tr, src, snk);
 }
 
+// The swap move of (alpha, beta), alpha < beta, at voxel v over the current labels (DESIGN.md §11, "Swap moves"): every
+// capacity plane entry of v and its tr, as exp_move_voxel leaves them; returns v's add_tweights constant.  Only voxels
+// labelled alpha or beta take part; x_p = SINK means "p takes beta", SOURCE "p takes alpha".  A participant has
+// src_p = D_p(beta) and snk_p = D_p(alpha), plus for each neighbour q labelled c: P's swap_fixed(w, c) when q is no
+// participant (ts to src_p, tk to snk_p, no arc), else the arc p -> q = P's swap_arc(w).  The sums run in the order axis
+// 0..nd-1, within an axis the pair where p is the lower end first; then add_tweights(p, src_p, snk_p) on tr = 0.  Any
+// other voxel reads nothing but its label: no arcs, tr = 0 and no constant.
+template <int ND, typename P, typename C>
+__device__ __forceinline__ double swap_move_voxel(const Lattice& L, const State<double>& S, const C* __restrict__ costs,
+                                                  const uint8_t* __restrict__ markers, const uint8_t* __restrict__ labels,
+                                                  const ExpWeights& W, const P& pair, int alpha, int beta, unsigned v,
+                                                  const int (&c)[ND], int zext, double& tr)
+{
+    const int lp = labels[v];
+    if (lp != alpha && lp != beta) {
+#pragma unroll
+        for (int d = 0; d < ND; ++d) {
+            S.cap[2 * d + 1][v] = 0.0;
+            S.cap[2 * d][v] = 0.0;
+        }
+        return 0.0;
+    }
+    const int mk = markers ? markers[v] : 0;
+    double src = exp_cost(costs, L.n, v, beta, mk);
+    double snk = exp_cost(costs, L.n, v, alpha, mk);
+#pragma unroll
+    for (int d = 0; d < ND; ++d) {
+        double lo_s = 0.0, lo_k = 0.0, up_s = 0.0, up_k = 0.0, fwd = 0.0, bwd = 0.0;
+        if (c[d] + 1 < (d == 0 ? zext : L.dim[d])) {                      // p is the lower end of (p, p + e_d)
+            const int lq = labels[v + L.stride[d]];
+            if (lq == alpha || lq == beta) fwd = pair.swap_arc(W.w[d][v], alpha, beta);
+            else                           pair.swap_fixed(W.w[d][v], lq, alpha, beta, lo_s, lo_k);
+        }
+        if (c[d] > 0) {                                                     // p is the upper end of (p - e_d, p)
+            const unsigned o = v - L.stride[d];
+            const int lq = labels[o];
+            if (lq == alpha || lq == beta) bwd = pair.swap_arc(W.w[d][o], alpha, beta);
+            else                           pair.swap_fixed(W.w[d][o], lq, alpha, beta, up_s, up_k);
+        }
+        src = __dadd_rn(src, lo_s);
+        src = __dadd_rn(src, up_s);
+        snk = __dadd_rn(snk, lo_k);
+        snk = __dadd_rn(snk, up_k);
+        S.cap[2 * d + 1][v] = fwd;
+        S.cap[2 * d][v] = bwd;
+    }
+    return add_tweights_dev(tr, src, snk);
+}
+
 // v's share of E(l): D_p(l_p), then its lower-end pairs in axis order.  c holds v's lattice coordinates; the axis-0 pairs
 // are z_pairs', so none crosses a seam of a batch.
 template <int ND, typename P, typename C>

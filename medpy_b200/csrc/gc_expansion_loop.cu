@@ -20,7 +20,7 @@ int expansion_check_labels(int K, std::string& err)
     return MGC_E_ARG;
 }
 
-int expansion_check_distance(const double* V, int K, std::string& err)
+int expansion_check_distance(const double* V, int K, std::string& err, bool semi_metric)
 {
     const auto at = [&](int a, int b) { return V[(size_t)a * K + b]; };
     const auto pair = [](int a, int b) { return "V[" + std::to_string(a) + "][" + std::to_string(b) + "]"; };
@@ -41,6 +41,7 @@ int expansion_check_distance(const double* V, int K, std::string& err)
                 err = "label_distance must be symmetric, " + pair(a, b) + " != " + pair(b, a);
                 return MGC_E_ARG;
             }
+    if (semi_metric) return MGC_OK;
     for (int a = 0; a < K; ++a)
         for (int b = 0; b < K; ++b)
             for (int c = 0; c < K; ++c)
@@ -60,9 +61,10 @@ Expansion::~Expansion()
     for (auto& e : ev) if (e) cudaEventDestroy(e);
 }
 
-void Expansion::apply(const uint8_t* mask, int alpha)
+void Expansion::apply(const uint8_t* mask, const ExpMove& m)
 {
-    exp_apply_launch(stream, blocks, n, mask, labels, alpha, d_switched);
+    if (m.beta < 0) exp_apply_launch(stream, blocks, n, mask, labels, m.alpha, d_switched);
+    else            swap_apply_launch(stream, blocks, n, mask, labels, m.alpha, m.beta, d_switched);
 }
 
 int Expansion::setup()
@@ -143,13 +145,24 @@ int Expansion::set_markers(const mgc_array* a) { return set_u8(a, &markers, &hav
 
 int Expansion::set_init(const mgc_array* a) { return set_u8(a, &init, &have_init, K - 1, "init"); }
 
+int Expansion::set_moves(int kind)
+{
+    Expansion* const g = this;
+    if (kind != MGC_MOVES_EXPANSION && kind != MGC_MOVES_SWAP)
+        FAIL(MGC_E_ARG, "moves must be MGC_MOVES_EXPANSION (0) or MGC_MOVES_SWAP (1)");
+    moves = kind;
+    have_dist = false;
+    ran = false;
+    return MGC_OK;
+}
+
 int Expansion::set_label_distance(const double* host_V)
 {
     Expansion* const g = this;
     have_dist = false;
     ran = false;
     if (!host_V) return MGC_OK;
-    RC(expansion_check_distance(host_V, K, err));
+    RC(expansion_check_distance(host_V, K, err, moves == MGC_MOVES_SWAP));
     CK(cudaSetDevice(device));
     const size_t bytes = (size_t)K * K * sizeof(double);
     if (!dist) RC(alloc(bytes, (void**)&dist));
@@ -181,6 +194,12 @@ int Expansion::run(int max_cycles)
         RC(read_bad(&bad));
         if (bad) FAIL(MGC_E_ARG, "init gives a marked voxel another label than its marker");
     }
+    // the moves of one cycle: alpha = 0..K-1, or the pairs alpha < beta in lexicographic order
+    std::vector<ExpMove> cycle_moves;
+    for (int a = 0; a < K; ++a) {
+        if (moves == MGC_MOVES_EXPANSION) cycle_moves.push_back({a, -1});
+        else for (int b = a + 1; b < K; ++b) cycle_moves.push_back({a, b});
+    }
     std::vector<uint8_t> active((size_t)B, 1);
     std::vector<unsigned long long> sw((size_t)B);
     std::vector<int64_t> changed((size_t)B);
@@ -188,16 +207,16 @@ int Expansion::run(int max_cycles)
     int live = B;
     for (int cycle = 0; cycle < max_cycles && live; ++cycle) {
         std::fill(changed.begin(), changed.end(), 0);
-        for (int alpha = 0; alpha < K; ++alpha) {
+        for (const ExpMove& m : cycle_moves) {
             RC(reset());
             CK(cudaEventRecord(ev[0], stream));
-            RC(build(alpha));
+            RC(build(m));
             CK(cudaEventRecord(ev[1], stream));
             const uint8_t* mask = nullptr;
             RC(solve(&mask));
             CK(cudaEventRecord(ev[2], stream));
             CK(cudaMemsetAsync(d_switched, 0, (size_t)B * sizeof(unsigned long long), stream));
-            apply(mask, alpha);
+            apply(mask, m);
             CK(cudaGetLastError());
             CK(cudaEventRecord(ev[3], stream));
             CK(cudaMemcpyAsync(sw.data(), d_switched, (size_t)B * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
@@ -219,7 +238,7 @@ int Expansion::run(int max_cycles)
             if (!active[(size_t)b]) continue;
             mgc_expansion_stats& s = per[(size_t)b];
             s.cycles++;
-            s.moves += K;
+            s.moves += (int64_t)cycle_moves.size();
             if (!changed[(size_t)b]) { s.converged = 1; active[(size_t)b] = 0; --live; froze = true; }
         }
         if (froze && live) RC(freeze(active));

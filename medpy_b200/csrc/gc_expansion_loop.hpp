@@ -1,6 +1,6 @@
-// gc_expansion_loop.hpp -- the alpha-expansion loop the three expansion units share (DESIGN.md §11): the cost planes,
-// markers and initial labels with their checks, the cycles of moves alpha = 0, 1, ..., K-1 over B images with freezing,
-// the statistics and the energy read-back.  A unit's handle derives from Expansion and supplies the hooks: where its
+// gc_expansion_loop.hpp -- the K-label move loop the three expansion units share (DESIGN.md §11): the cost planes,
+// markers and initial labels with their checks, the cycles of moves over B images with freezing (alpha-expansions
+// alpha = 0, 1, ..., K-1, or alpha-beta swaps (0, 1), (0, 2), ..., (K-2, K-1)), the statistics and the energy read-back.  A unit's handle derives from Expansion and supplies the hooks: where its
 // buffers come from, how an input is staged, and how a move is built, cut and applied.  The single-image units run the
 // loop with B = 1.  The loop is gc_expansion_loop.cu; the element-wise kernels it launches are compiled into
 // gc_expansion.cu only, behind the launchers at the end of this file.
@@ -13,6 +13,11 @@
 #include <cstdint>
 #include <string>
 #include <vector>
+
+// One move of the loop: the alpha-expansion of `alpha` (beta < 0), or the alpha-beta swap of (alpha, beta), alpha < beta
+struct ExpMove {
+    int alpha, beta;
+};
 
 struct Expansion {
     Expansion(std::string& err, const char* abi, int device, cudaStream_t stream, unsigned n, unsigned blocks, int K, int B)
@@ -30,12 +35,12 @@ struct Expansion {
     virtual void release() {}
     // before a move's first event (outside its timing)
     virtual int reset() { return MGC_OK; }
-    // the move graph of `alpha` over the current labels, between the build and solve events
-    virtual int build(int alpha) = 0;
-    // its cut, between the solve and apply events: *mask = 0 where a voxel switches to alpha
+    // the graph of move `m` over the current labels, between the build and solve events
+    virtual int build(const ExpMove& m) = 0;
+    // its cut, between the solve and apply events: *mask = 0 (SINK) where a voxel takes alpha (expansion) or beta (swap)
     virtual int solve(const uint8_t** mask) = 0;
-    // labels <- alpha where the mask says so, d_switched[b] += the switches of image b (k_exp_apply unless overridden)
-    virtual void apply(const uint8_t* mask, int alpha);
+    // the labels the mask gives, d_switched[b] += the switches of image b (k_exp_apply / k_swap_apply unless overridden)
+    virtual void apply(const uint8_t* mask, const ExpMove& m);
     // the images still in the loop, uploaded before the first cycle and after a cycle that froze some but not all
     // images; only a unit whose move kernel freezes images needs them
     virtual int freeze(const std::vector<uint8_t>& active) { (void)active; return MGC_OK; }
@@ -47,7 +52,10 @@ struct Expansion {
     int set_cost(int label, const mgc_array* cost);
     int set_markers(const mgc_array* markers);
     int set_init(const mgc_array* init);
-    // the K x K host matrix of a metric label distance (checked here, uploaded to `dist`), nullptr: back to Potts
+    // MGC_MOVES_EXPANSION or MGC_MOVES_SWAP; clears `ran` and the label distance (back to Potts)
+    int set_moves(int kind);
+    // the K x K host matrix of a label distance (checked here, uploaded to `dist`): a metric for expansion moves, a
+    // semi-metric for swap moves; nullptr: back to Potts
     int set_label_distance(const double* host_V);
     int run(int max_cycles);
     int get_labels(uint8_t* out, int mem);
@@ -69,6 +77,7 @@ struct Expansion {
     uint8_t* markers = nullptr;         // 0 none, m > 0: label m - 1
     uint8_t* init = nullptr;
     bool have_markers = false, have_init = false;
+    int moves = MGC_MOVES_EXPANSION;    // the move kind of run; a unit's build and apply hooks launch its kernels
     double* dist = nullptr;             // K x K label distance, row-major; a unit's build and energy hooks launch the
     bool have_dist = false;             // MetricPair kernels while it is set, the PottsPair ones otherwise (with_pair_rule)
     unsigned long long* d_switched = nullptr;   // [B] elements the current move switched per image
@@ -89,8 +98,8 @@ private:
 int expansion_check_labels(int K, std::string& err);
 // MGC_E_ARG with the message in `err` unless the K x K row-major V is a metric: finite entries >= 0, a zero diagonal,
 // symmetric, and V[a][c] <= V[a][b] + V[b][c] in float64 (DESIGN.md §11, "Label distances"); the message names the rule
-// and the first (a, b) or (a, b, c) that breaks it
-int expansion_check_distance(const double* V, int K, std::string& err);
+// and the first (a, b) or (a, b, c) that breaks it.  semi_metric skips the triangle rule only (swap moves).
+int expansion_check_distance(const double* V, int K, std::string& err, bool semi_metric = false);
 
 // the element-wise kernels of gc_expansion.cuh the loop launches, compiled into gc_expansion.cu only; `dtype` (MGC_F32 /
 // MGC_F64) selects the cost type, and markers / init may be nullptr
@@ -98,5 +107,7 @@ void exp_init_launch(cudaStream_t s, unsigned blocks, unsigned n, int K, int dty
                      const uint8_t* init, uint8_t* labels, int* bad);
 void exp_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* mask, uint8_t* labels, int alpha,
                       unsigned long long* switched);
+void swap_apply_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* mask, uint8_t* labels, int alpha, int beta,
+                       unsigned long long* switched);
 void exp_check_costs_launch(cudaStream_t s, unsigned blocks, unsigned n, int dtype, const void* cost, int* bad);
 void exp_check_u8_launch(cudaStream_t s, unsigned blocks, unsigned n, const uint8_t* a, int limit, int* bad);

@@ -1,8 +1,8 @@
-// gc_expansion_pair.cuh -- the pair rules of the alpha-expansion kernels (DESIGN.md §11): how one pair enters the move
-// graph of alpha and the energy, under Potts (PottsPair) or a metric label distance V (MetricPair, "Label distances").
-// The move and energy kernels of the voxel, batch and region units are templates over the rule, so each rule is an
-// instantiation of its own: the Potts one loads no V and multiplies nothing.  with_pair_rule picks the cost type and the
-// rule of a handle at launch.
+// gc_expansion_pair.cuh -- the pair rules of the K-label move kernels (DESIGN.md §11): how one pair enters the move
+// graph of an alpha-expansion or an alpha-beta swap and the energy, under Potts (PottsPair) or a label distance V
+// (MetricPair, "Label distances").  The move and energy kernels of the voxel, batch and region units are templates over
+// the rule, so each rule is an instantiation of its own: the Potts one loads no V and multiplies nothing.
+// with_pair_rule picks the cost type and the rule of a handle at launch.
 #pragma once
 #include "gc_expansion_loop.hpp"
 
@@ -12,6 +12,10 @@
 //   upper(w, a, b, alpha, t, arc)   seen from q (b != alpha): t = t_up to q's sink link, arc = bwd on arc q -> p
 //   energy(w, a, b)                 the pair's energy when a != b
 // The caller zeroes t and arc; a rule writes what the pair adds.
+// For the swap move of (alpha, beta) (DESIGN.md §11, "Swap moves"), seen from a participant p (labelled alpha or beta):
+//   swap_fixed(w, c, alpha, beta, ts, tk)   neighbour labelled c, not a participant: ts = e(beta, c) to p's src (paid
+//                                           at SINK = beta), tk = e(alpha, c) to p's snk (paid at SOURCE = alpha)
+//   swap_arc(w, alpha, beta)                neighbour a participant: the arc p -> q, e(alpha, beta) = e(beta, alpha)
 
 // Potts, V = 1 - I: the table of DESIGN.md §11, "One move", with no V load and no multiply
 struct PottsPair {
@@ -26,6 +30,12 @@ struct PottsPair {
         else arc = w;
     }
     __device__ __forceinline__ double energy(double w, int, int) const { return w; }
+    __device__ __forceinline__ void swap_fixed(double w, int, int, int, double& ts, double& tk) const
+    {
+        ts = w;
+        tk = w;
+    }
+    __device__ __forceinline__ double swap_arc(double w, int, int) const { return w; }
 };
 
 // What one pair (p, q), p its lower end, adds to the move graph of `alpha` under the metric V: `lo` to p's sink link, `up`
@@ -69,7 +79,8 @@ __device__ __forceinline__ ExpPair exp_metric_pair(double w, const double* __res
     return r;
 }
 
-// A metric V (K x K, row-major, on the device): each end takes its half of exp_metric_pair
+// A label distance V (K x K, row-major, on the device).  Expansion moves take a metric, each end its half of
+// exp_metric_pair; swap moves take any semi-metric (>= 0, symmetric, zero diagonal) and read V directly.
 struct MetricPair {
     const double* V;
     int K;
@@ -87,6 +98,12 @@ struct MetricPair {
         arc = r.bwd;
     }
     __device__ __forceinline__ double energy(double w, int a, int b) const { return exp_dist(w, V, K, a, b); }
+    __device__ __forceinline__ void swap_fixed(double w, int c, int alpha, int beta, double& ts, double& tk) const
+    {
+        ts = exp_dist(w, V, K, beta, c);
+        tk = exp_dist(w, V, K, alpha, c);
+    }
+    __device__ __forceinline__ double swap_arc(double w, int alpha, int beta) const { return exp_dist(w, V, K, alpha, beta); }
 };
 
 // f(C{}, rule) with C the cost type of e's planes (float for MGC_F32, else double) and rule MetricPair over e.dist while a

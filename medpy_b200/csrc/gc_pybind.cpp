@@ -839,6 +839,7 @@ template <> struct ExpansionAbi<mgc_expansion> {
     static constexpr auto set_cost = mgc_expansion_set_cost;
     static constexpr auto set_markers = mgc_expansion_set_markers;
     static constexpr auto set_init = mgc_expansion_set_init;
+    static constexpr auto set_moves = mgc_expansion_set_moves;
     static constexpr auto set_label_distance = mgc_expansion_set_label_distance;
     static constexpr auto run = mgc_expansion_run;
     static constexpr auto get_labels = mgc_expansion_get_labels;
@@ -851,6 +852,7 @@ template <> struct ExpansionAbi<mgc_expansion_batch> {
     static constexpr auto set_cost = mgc_expansion_batch_set_cost;
     static constexpr auto set_markers = mgc_expansion_batch_set_markers;
     static constexpr auto set_init = mgc_expansion_batch_set_init;
+    static constexpr auto set_moves = mgc_expansion_batch_set_moves;
     static constexpr auto set_label_distance = mgc_expansion_batch_set_label_distance;
     static constexpr auto run = mgc_expansion_batch_run;
     static constexpr auto get_labels = mgc_expansion_batch_get_labels;
@@ -862,6 +864,7 @@ template <> struct ExpansionAbi<mgc_region_expansion> {     // no markers: they 
     static constexpr auto last_error = mgc_region_expansion_last_error;
     static constexpr auto set_cost = mgc_region_expansion_set_cost;
     static constexpr auto set_init = mgc_region_expansion_set_init;
+    static constexpr auto set_moves = mgc_region_expansion_set_moves;
     static constexpr auto set_label_distance = mgc_region_expansion_set_label_distance;
     static constexpr auto run = mgc_region_expansion_run;
     static constexpr auto get_labels = mgc_region_expansion_get_labels;
@@ -912,6 +915,13 @@ public:
         ArrayRef r = ref(init, MGC_U8, "init");
         int rc;
         { py::gil_scoped_release rel; rc = Abi::set_init(e_, &r.a); }
+        check(rc);
+    }
+    // MGC_MOVES_EXPANSION (0) or MGC_MOVES_SWAP (1); drops the label distance
+    void set_moves(int kind)
+    {
+        int rc;
+        { py::gil_scoped_release rel; rc = Abi::set_moves(e_, kind); }
         check(rc);
     }
     // a (K, K) float64 label distance, or None for Potts
@@ -1148,6 +1158,8 @@ PYBIND11_MODULE(_mgc, m)
     m.attr("OPT_WARM") = MGC_OPT_WARM;
     m.attr("OPT_KEEP_DEVICE_INPUTS") = MGC_OPT_KEEP_DEVICE_INPUTS;
     m.attr("OPT_SEGMENT_ENERGIES") = MGC_OPT_SEGMENT_ENERGIES;
+    m.attr("MOVES_EXPANSION") = MGC_MOVES_EXPANSION;
+    m.attr("MOVES_SWAP") = MGC_MOVES_SWAP;
     m.attr("LABELS_ADJACENCY") = MGC_LABELS_ADJACENCY;
     m.attr("LABELS_STAWIASKI") = MGC_LABELS_STAWIASKI;
     m.attr("LABELS_STAWIASKI_DIRECTED") = MGC_LABELS_STAWIASKI_DIRECTED;
@@ -1159,6 +1171,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("set_boundary", &PyExpansion::set_boundary)
         .def("set_markers", &PyExpansion::set_markers)
         .def("set_init", &PyExpansion::set_init)
+        .def("set_moves", &PyExpansion::set_moves)
         .def("set_label_distance", &PyExpansion::set_label_distance)
         .def("run", &PyExpansion::run)
         .def("labels", &PyExpansion::labels)
@@ -1171,6 +1184,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("set_boundary", &PyExpansionBatch::set_boundary)
         .def("set_markers", &PyExpansionBatch::set_markers)
         .def("set_init", &PyExpansionBatch::set_init)
+        .def("set_moves", &PyExpansionBatch::set_moves)
         .def("set_label_distance", &PyExpansionBatch::set_label_distance)
         .def("run", &PyExpansionBatch::run)
         .def("labels", &PyExpansionBatch::labels)
@@ -1184,6 +1198,7 @@ PYBIND11_MODULE(_mgc, m)
         .def("set_cost", &PyRegionExpansion::set_cost)
         .def("set_pairs", &PyRegionExpansion::set_pairs)
         .def("set_init", &PyRegionExpansion::set_init)
+        .def("set_moves", &PyRegionExpansion::set_moves)
         .def("set_label_distance", &PyRegionExpansion::set_label_distance)
         .def("run", &PyRegionExpansion::run)
         .def("labels", &PyRegionExpansion::labels)

@@ -46,7 +46,7 @@ struct mgc_region_expansion : Expansion {
     int alloc(size_t bytes, void** out) override;
     // a 1-D array of n entries with unit stride, as every per-region argument is passed: read where it is
     int stage(const mgc_array* a, size_t es, const char* what, const void** out) override;
-    int build(int alpha) override;
+    int build(const ExpMove& m) override;
     int solve(const uint8_t** mask) override;
     int energy() override;
 };
@@ -94,12 +94,17 @@ int mgc_region_expansion::stage(const mgc_array* a, size_t es, const char* what,
     return MGC_OK;
 }
 
-int mgc_region_expansion::build(int alpha)
+int mgc_region_expansion::build(const ExpMove& m)
 {
     mgc_region_expansion* const g = this;
     with_pair_rule(*this, [&](auto c, auto pair) {
         using C = decltype(c);
-        k_rexp_move<<<blocks, 256>>>(H.n, H.row, H.head, wt, (const C*)costs, labels, alpha, H.cap, H.tr, partials, pair);
+        if (m.beta >= 0)
+            k_rswap_move<<<blocks, 256>>>(H.n, H.row, H.head, wt, (const C*)costs, labels, m.alpha, m.beta, H.cap, H.tr,
+                                          partials, pair);
+        else
+            k_rexp_move<<<blocks, 256>>>(H.n, H.row, H.head, wt, (const C*)costs, labels, m.alpha, H.cap, H.tr, partials,
+                                         pair);
     });
     CK(cudaGetLastError());
     CK(cudaMemsetAsync(d_base, 0, sizeof(double), 0));
@@ -186,6 +191,7 @@ int mgc_region_expansion_set_pairs(mgc_region_expansion* g, int64_t count, const
 }
 
 int mgc_region_expansion_set_init(mgc_region_expansion* g, const mgc_array* init) { return g ? g->set_init(init) : MGC_E_ARG; }
+int mgc_region_expansion_set_moves(mgc_region_expansion* g, int32_t kind) { return g ? g->set_moves(kind) : MGC_E_ARG; }
 int mgc_region_expansion_set_label_distance(mgc_region_expansion* g, const double* dist)
 {
     return g ? g->set_label_distance(dist) : MGC_E_ARG;

@@ -50,6 +50,45 @@ k_rexp_move(int n, const int* __restrict__ row, const int* __restrict__ head, co
     block_sum_store(m, partials);
 }
 
+// One swap move of (alpha, beta) over the current labels (DESIGN.md §11, "Swap moves"), written as k_rexp_move writes a
+// move.  Only nodes labelled alpha or beta take part; x_u = SINK means "u takes beta".  A participant u has src_u =
+// D_u(beta), snk_u = D_u(alpha); for each arc u -> v in the row's order, v labelled b: P's swap_fixed(w, b) to src_u and
+// snk_u when v is no participant (no arc), else cap(u -> v) = P's swap_arc(w); then add_tweights(u, src_u, snk_u) on tr
+// = 0.  Any other node has no arcs, tr = 0 and no constant.
+template <typename P, typename C>
+__global__ void __launch_bounds__(256)
+k_rswap_move(int n, const int* __restrict__ row, const int* __restrict__ head, const double* __restrict__ wt,
+             const C* __restrict__ costs, const uint8_t* __restrict__ labels, int alpha, int beta, double* __restrict__ cap,
+             double* __restrict__ tr, double* __restrict__ partials, P pair)
+{
+    double m = 0.0;
+    const int step = gridDim.x * blockDim.x;
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < n; u += step) {
+        const int a = labels[u];
+        const int end = row[u + 1];
+        if (a != alpha && a != beta) {
+            for (int e = row[u]; e < end; ++e) cap[e] = 0.0;
+            tr[u] = 0.0;
+            continue;
+        }
+        double src = (double)costs[(size_t)beta * n + u];
+        double snk = (double)costs[(size_t)alpha * n + u];
+        for (int e = row[u]; e < end; ++e) {
+            const int b = labels[head[e]];
+            double c = 0.0, ts = 0.0, tk = 0.0;
+            if (b == alpha || b == beta) c = pair.swap_arc(wt[e], alpha, beta);
+            else                         pair.swap_fixed(wt[e], b, alpha, beta, ts, tk);
+            src = __dadd_rn(src, ts);
+            snk = __dadd_rn(snk, tk);
+            cap[e] = c;
+        }
+        double t = 0.0;
+        m = __dadd_rn(m, add_tweights_dev(t, src, snk));
+        tr[u] = t;
+    }
+    block_sum_store(m, partials);
+}
+
 // E(l) per block in a fixed order (each node: D_u(l_u), then its pairs to higher ids in the row's order); k_sum_partials
 // adds the partials in a fixed order, so the same labels give the same bits
 template <typename P, typename C>

@@ -125,11 +125,19 @@ def _check_init_markers(markers, init):
         raise ValueError("init gives a marked voxel another label than its marker")
 
 
-def _label_distance(V, K):
+def _check_moves(moves):
+    """The move kind, "expansion" or "swap"; True for swap moves."""
+    if not isinstance(moves, str) or moves not in ("expansion", "swap"):
+        raise ValueError("moves must be \"expansion\" or \"swap\", got {!r}".format(moves))
+    return moves == "swap"
+
+
+def _label_distance(V, K, swap=False):
     """A label distance as a C-contiguous float64 (K, K) numpy array, refused (ValueError) unless it is a metric: finite
-    entries >= 0, a zero diagonal, symmetric, and V[a][c] <= V[a][b] + V[b][c] in float64 for every a, b, c.  The
-    message names the rule and the first (a, b) or (a, b, c), in C order, that breaks it: the native check's words.  A
-    CUDA tensor is copied to the host (K^2 numbers)."""
+    entries >= 0, a zero diagonal, symmetric, and V[a][c] <= V[a][b] + V[b][c] in float64 for every a, b, c.  With
+    ``swap`` the triangle rule is skipped: swap moves take any semi-metric.  The message names the rule and the first
+    (a, b) or (a, b, c), in C order, that breaks it: the native check's words.  A CUDA tensor is copied to the host (K^2
+    numbers)."""
     if _on_device(V):
         V = V.detach().cpu().numpy()
     V = numpy.asarray(V)
@@ -148,6 +156,8 @@ def _label_distance(V, K):
     if bad.size:
         a, b = bad[0]
         raise ValueError("label_distance must be symmetric, V[{0}][{1}] != V[{1}][{0}]".format(a, b))
+    if swap:
+        return V
     for a in range(K):
         bad = numpy.argwhere(V[a][None, :] > V[a][:, None] + V)        # [b, c]: V[a][c] > V[a][b] + V[b][c]
         if bad.size:
@@ -159,7 +169,7 @@ def _label_distance(V, K):
 
 
 def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, markers=None, init=None, max_cycles=20,
-                          stats=False, *, label_distance=None):
+                          stats=False, *, label_distance=None, moves="expansion"):
     """Segment a voxel image into K labels by alpha-expansion.
 
     costs              (K, *shape) float32 or float64, a numpy array or a CUDA tensor; ``costs[k]`` is the cost of label k
@@ -171,14 +181,18 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
                        (GCGraph.MAX) more there, MedPy's soft-hard seed.  With K = 2 and markers 1 = background,
                        2 = foreground, the result is graph_from_voxels' cut.
     init               initial labels (0..K-1, agreeing with the markers); default argmin_k costs[k], ties to the lowest k.
-    max_cycles         cycles of the moves 0, 1, ..., K-1 at most; the loop stops earlier after a cycle that switches no
-                       voxel.
+    max_cycles         cycles at most, of the moves 0, 1, ..., K-1 (expansion) or of the K(K-1)/2 pairs (swap); the loop
+                       stops earlier after a cycle that switches no voxel.
     stats              also return a dict: moves, cycles, converged, switched (voxels per move), energy and device ms.
-    label_distance     (K, K) metric label distance V (numpy array, nested sequence or CUDA tensor; keyword only): the
-                       pair term becomes w_pq V(l_p, l_q), so a change between distant labels costs more than one between
+    label_distance     (K, K) label distance V (numpy array, nested sequence or CUDA tensor; keyword only): the pair term
+                       becomes w_pq V(l_p, l_q), so a change between distant labels costs more than one between
                        neighbours, e.g. ``numpy.minimum(abs(i - j), 2)`` for ordered labels.  Finite, >= 0, zero on the
-                       diagonal, symmetric and satisfying the triangle inequality (DESIGN.md §11, "Label distances").
-                       None: Potts.
+                       diagonal and symmetric; under expansion moves it must also satisfy the triangle inequality
+                       (DESIGN.md §11, "Label distances"), under swap moves it need not (truncated quadratic
+                       ``numpy.minimum((i - j) ** 2, 4)``).  None: Potts.
+    moves              (keyword only) "expansion": cycles of alpha-expansions alpha = 0, 1, ..., K-1; "swap": cycles of
+                       alpha-beta swaps (0, 1), (0, 2), ..., (K-2, K-1), each a cut over the voxels labelled alpha or beta
+                       only, exact for any semi-metric label distance (DESIGN.md §11, "Swap moves").
 
     Returns ``(labels, energy)`` (``(labels, energy, stats)`` with ``stats=True``): uint8 labels of the image shape, a
     numpy array or, for CUDA costs, a CUDA tensor; ``energy`` the energy of those labels (Potts, or with the label
@@ -187,6 +201,7 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
     reaches the device.
     """
     device = -1
+    swap = _check_moves(moves)
     costs = _float_costs(costs, "costs")
     if costs.ndim < 2 or costs.ndim > 5:
         raise ValueError("costs must have shape (K, *image shape) with a 1- to 4-D image")
@@ -213,7 +228,7 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
         init = _label_image(init, shape, "init", K - 1)
     _check_init_markers(markers, init)
     if label_distance is not None:
-        label_distance = _label_distance(label_distance, K)
+        label_distance = _label_distance(label_distance, K, swap)
 
     from .. import _lib  # raises ImportError loudly when the extension is not built
     on_dev = _on_device(costs)
@@ -229,6 +244,8 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
         nat.set_markers(markers)
     if init is not None:
         nat.set_init(init)
+    if swap:
+        nat.set_moves(_lib._mgc.MOVES_SWAP)
     if label_distance is not None:
         nat.set_label_distance(label_distance)
     nat.run(int(max_cycles))
@@ -245,7 +262,7 @@ def expansion_from_voxels(costs, boundary_term=False, boundary_term_args=False, 
 
 
 def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, spacing=False, markers=None, init=None,
-                                max_cycles=20, stats=False, *, label_distance=None):
+                                max_cycles=20, stats=False, *, label_distance=None, moves="expansion"):
     """Segment B images of one shape into K labels by alpha-expansion, all in one loop (DESIGN.md §11, "Batches").
 
     Image b is segmented as ``expansion_from_voxels`` segments it alone: the same energy, bit for bit the same move
@@ -264,11 +281,13 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
     sigma              the term's sigma: one float for every image, or one per image.
     spacing            voxel spacing of the images (one entry per image axis), or False.
     markers, init      (B, *image) integer images with the meaning ``expansion_from_voxels`` gives them per image.
-    max_cycles         cycles of the moves 0, 1, ..., K-1 at most, per image.
+    max_cycles         cycles at most per image, of the moves 0, 1, ..., K-1 (expansion) or of the K(K-1)/2 pairs (swap).
     stats              also return a dict: the batch loop's ``batch_moves``, ``batch_cycles``, ``batch_converged``, per-image
                        lists ``moves``, ``cycles``, ``converged``, ``switched`` (voxels per move) and ``energy``, and the
                        device ms (``ms_build``, ``ms_solve``, ``ms_apply`` summed over the moves, ``ms_total``).
-    label_distance     (K, K) metric label distance of every image, as ``expansion_from_voxels`` takes it; None: Potts.
+    label_distance     (K, K) label distance of every image, as ``expansion_from_voxels`` takes it; None: Potts.
+    moves              "expansion" or "swap", as ``expansion_from_voxels`` takes it; a swap cycle is K(K-1)/2 moves of
+                       every image.
 
     Returns ``(labels, energies)`` (``+ (stats,)`` with ``stats=True``): uint8 labels of shape (B, *image), a numpy array
     or, for CUDA costs, a CUDA tensor; ``energies`` a float64 numpy array of the B energies (Potts, or with the label
@@ -277,6 +296,7 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
     """
     from .batch import INDEX_LIMIT, _host_image, _is_cuda, _sigmas
     from .device import _KINDS
+    swap = _check_moves(moves)
     costs = _float_costs(costs, "costs")
     if costs.ndim < 3 or costs.ndim > 5:
         raise ValueError("costs must have shape (B, K, *image shape) with a 1- to 3-D image")
@@ -313,7 +333,7 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
         init = _label_image(init, bshape, "init", K - 1)
     _check_init_markers(markers, init)
     if label_distance is not None:
-        label_distance = _label_distance(label_distance, K)
+        label_distance = _label_distance(label_distance, K, swap)
 
     from .. import _lib  # raises ImportError loudly when the extension is not built
     on_dev = _on_device(costs)
@@ -331,6 +351,8 @@ def expansion_from_voxels_batch(costs, image=None, boundary=None, sigma=None, sp
         nat.set_markers(markers)
     if init is not None:
         nat.set_init(init)
+    if swap:
+        nat.set_moves(_lib._mgc.MOVES_SWAP)
     if label_distance is not None:
         nat.set_label_distance(label_distance)
     nat.run(int(max_cycles))
@@ -375,7 +397,7 @@ def _region_values(a, regions, what, limit):
 
 
 def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary_term_args=False, markers=None, init=None,
-                          max_cycles=20, stats=False, *, region_costs=None, label_distance=None):
+                          max_cycles=20, stats=False, *, region_costs=None, label_distance=None, moves="expansion"):
     """Segment the regions of a label image into K labels by alpha-expansion (DESIGN.md §11, "Region graphs").
 
     Minimises E(l) = sum_r D_r(l_r) + sum_{region pairs r<s} w_rs [l_r != l_s] over region labels 0..K-1
@@ -395,16 +417,18 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
                        1 = background, 2 = foreground, the result is graph_from_labels' cut.
     init               initial region labels, shape (R,), 0..K-1; a marked region must start at one of its markers'
                        labels.  Default argmin_k D_r(k), ties to the lowest k.
-    max_cycles         cycles of the moves 0, 1, ..., K-1 at most; the loop stops earlier after a cycle that switches no
-                       region.
+    max_cycles         cycles at most, of the moves 0, 1, ..., K-1 (expansion) or of the K(K-1)/2 pairs (swap); the loop
+                       stops earlier after a cycle that switches no region.
     stats              also return a dict: moves, cycles, converged, switched (regions per move), energy and device ms.
-    label_distance     (K, K) metric label distance, as ``expansion_from_voxels`` takes it: the pair term becomes
+    label_distance     (K, K) label distance, as ``expansion_from_voxels`` takes it: the pair term becomes
                        w_rs V(l_r, l_s).  None: Potts.
+    moves              "expansion" or "swap", as ``expansion_from_voxels`` takes it.
 
     Returns ``(labels, region_labels, energy)`` (``+ (stats,)`` with ``stats=True``): ``labels`` the uint8 voxel image
     ``region_labels[label_image - 1]`` (a CUDA tensor when the costs are one, numpy otherwise), ``region_labels`` uint8
     of shape (R,), ``energy`` the energy of those labels (Potts, or with the label distance).
     """
+    swap = _check_moves(moves)
     if (costs is None) == (region_costs is None):
         raise ValueError("give exactly one of costs and region_costs")
     label_image = numpy.asarray(label_image)
@@ -420,7 +444,7 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
     K = int(data.shape[0])
     _check_labels_and_cycles(K, what + ".shape[0]", max_cycles)
     if label_distance is not None:
-        label_distance = _label_distance(label_distance, K)
+        label_distance = _label_distance(label_distance, K, swap)
     if boundary_term and not _takes_three_parameters(boundary_term):
         raise AttributeError("boundary_term has to be a callable object which takes three parameters.")
     if markers is not None:
@@ -472,6 +496,8 @@ def expansion_from_labels(label_image, costs=None, boundary_term=False, boundary
         nat.set_pairs(*rec.pairs)
     if init is not None:
         nat.set_init(init)
+    if swap:
+        nat.set_moves(ctx._mgc.MOVES_SWAP)
     if label_distance is not None:
         nat.set_label_distance(label_distance)
     nat.run(int(max_cycles))
